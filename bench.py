@@ -57,7 +57,8 @@ def parse_args():
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--workload", default=WORKLOAD)
     ap.add_argument("--no-cpu-baseline", action="store_true")
-    ap.add_argument("--repeats", type=int, default=10, help="extra timed regions of --steps steps each (median / p10 / p90)")
+    ap.add_argument("--repeats", type=int, default=0,
+                    help="extra timed regions of --steps steps each (median / p10 / p90); 0 = the headline times exactly --steps steps")
     ap.add_argument("--exchange-streams", type=int, default=1, choices=[1, 2],
                     help="N > 1: 2 = the all-gather of the compact exchange on a second NCCL communicator, concurrent with the all-reduce")
     ap.add_argument("--exchange", default="auto", choices=["auto", "multimem", "nccl"],
@@ -65,13 +66,16 @@ def parse_args():
                          "nccl = ncclAllReduce + ncclAllGather, auto = multimem where the group has multicast support, else nccl")
     ap.add_argument("--exchange-blocks", type=int, default=0, help="CTAs of the multimem exchange kernel (0 = two per SM)")
     ap.add_argument("--overlap-expansion-nccl", action="store_true",
-                    help="NCCL exchange: gather first and expand the SH columns beside the all-reduce (measured slower at 2 ranks)")
+                    help="NCCL exchange: gather first and expand the SH columns beside the all-reduce")
     ap.add_argument("--overlap-expansion", action="store_true",
                     help="multimem exchange: expand the SH columns on a second stream while the all-reduce is on the wire instead of "
-                         "one expansion pass behind it (measured slower at 8 GPUs: 1.809 vs 1.797 ms per step)")
+                         "one expansion pass behind it")
     ap.add_argument("--serial-expansion", action="store_true", help="(default behaviour; kept so that older call scripts still parse)")
     ap.add_argument("--dense-exchange", action="store_true",
                     help="N > 1: one all-reduce of the dense gradients instead of the compact exchange (comparison)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed (rank 0) as DIR/<name>.npy: image, "
+                         "depth, pixel count and a fixed seeded sample of the per-Gaussian gradient rows")
     return ap.parse_args()
 
 
@@ -80,8 +84,8 @@ def measured_peaks():
     if os.path.exists(path):
         with open(path) as f:
             d = json.load(f)
-        return float(d.get("hbm_gbs", 6650.0)), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+        return float(d.get("hbm_gbs", 3350.0)), "measured (MEASURED_PEAKS.json)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3)"
 
 
 # --------------------------------------------------------------------------- clocks
@@ -203,8 +207,8 @@ def run_reference(args):
     print(json.dumps(line), flush=True)
 
 
-# --------------------------------------------------------------------------- B200 arm
-SM_CLOCK_HZ, NUM_SMS = 1.965e9, 148
+# --------------------------------------------------------------------------- GPU arm (H100 SXM: 132 SMs, 1.98 GHz max boost clock)
+SM_CLOCK_HZ, NUM_SMS = 1.98e9, 132
 ISSUE_PEAK = NUM_SMS * 4 * SM_CLOCK_HZ          # warp instructions / s (one per SMSP per cycle)
 FP32_LANE_PEAK = NUM_SMS * 128 * SM_CLOCK_HZ    # FP32 lane operations / s (an FMA counts once)
 MUFU_LANE_PEAK = NUM_SMS * 16 * SM_CLOCK_HZ     # MUFU (ex2 / rcp) lane operations / s
@@ -237,8 +241,8 @@ def run_b200(args):
     Input = GPCR.GaussianPointCloudRasterisationInput
     exchange, exchange_kind = None, "dense all-reduce"
     if world > 1 and not args.dense_exchange:
-        # measured (profiles/r02_bench_n*_{multimem,nccl}.json): at 2 ranks the NCCL collectives win (1.69 vs 1.73 ms per step: two
-        # barriers + two launches outweigh 60 MB of wire time), from 4 ranks on the hand-written NVLS kernel does (8 ranks: 1.90 vs 2.00)
+        # auto: the NCCL collectives at 2 ranks (the NVLS kernel's two barriers + two launches weigh more in a small group), the
+        # hand-written NVLS kernel from 4 ranks on; the multi-GPU paths have not been timed on H100s yet (--exchange picks one)
         if args.exchange == "multimem" or (args.exchange == "auto" and world >= 4):
             try:
                 exchange = MulticastViewParallelExchange(num_blocks=args.exchange_blocks, overlap_expansion=args.overlap_expansion and not args.serial_expansion)
@@ -262,8 +266,8 @@ def run_b200(args):
     def timed(fn, k, rewarm=2):
         """k calls of fn between barrier + synchronize on both sides, CUDA events on the launching stream, MAX over ranks.
         `rewarm` untimed calls run immediately before the region: rank 0 has just started the clock sampler / printed, the
-        other ranks have been spinning in a barrier -- the first timed step must not pay for that (observed at 8 GPUs:
-        a first region of 2.7 ms per step against a median of 1.9 ms without it)."""
+        other ranks have been spinning in a barrier -- the first timed step must not pay for that (without it the first region
+        a first region well above the median without it)."""
         for _ in range(rewarm):
             fn()
         barrier()
@@ -312,9 +316,10 @@ def run_b200(args):
             sc = self.scene
             sc.point_cloud.grad = None
             sc.point_cloud_features.grad = None
-            image, _, _ = self.op(self.dev_input)
+            image, depth, count = self.op(self.dev_input)
             image.backward(self.grad_image)  # N > 1: the gradient exchange over NVLink happens inside this backward
             self.finish_step()
+            self.last_outputs = (image.detach(), depth, count)
 
         def mpix(self, ms_per_step):
             return world * self.H * self.W / (ms_per_step * 1e-3) / 1e6
@@ -334,6 +339,8 @@ def run_b200(args):
     regions = [timed(wl.step, steps) / steps for _ in range(1 + max(args.repeats, 0))]
     first_region_ms = regions[0]
     ms_per_step = statistics.median(regions)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, wl)
     value = wl.mpix(ms_per_step)
     frame = op.last_frame
     M, Kk = frame.num_points_in_camera, frame.num_keys
@@ -409,7 +416,7 @@ def run_b200(args):
         exchange_check["fwd_bwd_without_exchange_ms_per_rank"] = [round(float(x), 4) for x in every]
 
     # ---- e2e: per-step inputs in pinned HOST memory (target image, pose, intrinsics), loss scalar back
-    target_host = torch.rand((H, W, 3), dtype=torch.float32).pin_memory()
+    target_host = torch.rand((H, W, 3), generator=torch.Generator().manual_seed(4321), dtype=torch.float32).pin_memory()
     q_host = scene.q_pointcloud_camera.detach().cpu().pin_memory()
     t_host = scene.t_pointcloud_camera.detach().cpu().pin_memory()
     K_host = scene.camera_info.camera_intrinsics.detach().cpu().pin_memory()
@@ -605,8 +612,8 @@ def run_b200(args):
                 "inner_loop_sass_instructions_per_visit": instr_per_visit,
                 "inner_loop_issue_slot_fraction": round(visits * instr_per_visit / s_ / ISSUE_PEAK, 3),
                 "mufu_fraction_of_peak": round(evals * mufu_per_eval / s_ / MUFU_LANE_PEAK, 3),
-                "what": f"{kind}: counted on the device by the kernel's COUNT instantiation; issue peak = 148 SMs x 4 schedulers x "
-                        f"1.965 GHz, MUFU peak = 16 lanes / SM / clk"}
+                "what": f"{kind}: counted on the device by the kernel's COUNT instantiation; issue peak = {NUM_SMS} SMs x 4 schedulers x "
+                        f"{SM_CLOCK_HZ / 1e9:.2f} GHz, MUFU peak = 16 lanes / SM / clk"}
     compute = {
         "blend_forward": compute_side("forward blend", work["forward_warp_splat_visits"], work["forward_contributing_evaluations"],
                                       stage_ms["blend_forward"], FWD_INSTR_PER_VISIT, 1),
@@ -623,22 +630,15 @@ def run_b200(args):
                                              "4x4_two_splats_per_warp_iteration_lower_bound": round(work["staged_patch_pairs_4x4"] / 2 / max(p84, 1), 3)},
         "what": "counted on the device at staging time: a two-pixels-per-thread warp (8x8 or 16x4 patch) visits a splat if either of its "
                 "two 8x4 halves can be reached and then pays ~4 shared + 2 x 25 per-pixel instructions instead of 29 per 8x4 visit"}
-    ncu = None
-    npath = os.path.join(ROOT, "profiles", "r02_ncu_step_full.json")
-    if args.workload == "C3" and os.path.exists(npath):  # committed ncu --set full capture of both blend kernels (not live)
-        with open(npath) as f:
-            ncu = json.load(f)
-    traffic = (ncu or {}).get(dominant, {}).get("dram_bytes_per_launch")
     roofline = {
         "kernel": dominant,
         "bound": "issue (FP32/ALU instruction slots): the blend kernels reuse each 48-B record across up to 256 pixels, "
                  "so neither hbm nor tensor bounds them; the hbm figures below are the mandated algorithmic-bytes roofline, "
                  "`compute` is the one that explains the time",
         "achieved": round(dom_gbs, 2), "peak": peak, "unit": "GB/s",
-        "frac": round(dom_gbs / peak, 5), "traffic": traffic, "peak_source": peak_src,
+        "frac": round(dom_gbs / peak, 5), "peak_source": peak_src,
         "launch_ms": round(stage_ms[dominant], 4),
         "compute": compute,
-        "ncu_committed_capture": ncu,
         "per_stage": per_stage,
     }
 
@@ -678,7 +678,7 @@ def run_b200(args):
                    "frame": f"M={M} in frustum, K={Kk} (tile,splat) pairs sorted and blended (of {K_ref} in the reference's "
                             f"3-sigma squares; the rest cannot reach alpha>=1/255)",
                    "parallelism": parallelism,
-                   "l2": "inputs larger than L2 (scene 236 MB + 200 MB workspace per frame vs 126 MB L2)",
+                   "l2": "inputs larger than L2 (scene 236 MB + 200 MB workspace per frame vs 50 MB L2)",
                    "backward_impl": op.backward_impl},
         "spread": dict(percentiles(regions), first_region_ms_per_step=round(first_region_ms, 4),
                        what=f"{len(regions)} timed regions of {steps} steps each; `value` / `ms_per_step` are the median region"),
@@ -714,6 +714,31 @@ def main():
         run_reference(args)
     else:
         run_b200(args)
+
+
+DUMP_GRAD_ROWS = 65536  # fixed seeded sample of the per-Gaussian gradient rows (the dense (N, 59) gradients exceed 64 MB at C3)
+DUMP_MAX_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, wl):
+    """What the last timed step handed its caller: the forward's image / depth / per-pixel point count and the backward's
+    gradients (a fixed seeded sample of N rows), as float32 .npy files under `out_dir`."""
+    import numpy as np
+    import torch
+    image, depth, count = wl.last_outputs
+    rows = np.sort(np.random.default_rng(0).choice(wl.N, size=min(wl.N, DUMP_GRAD_ROWS), replace=False))
+    idx = torch.from_numpy(rows).to(image.device)
+    arrays = {
+        "image": image, "depth": depth, "pixel_valid_point_count": count,
+        "grad_pointcloud_rows": wl.scene.point_cloud.grad[idx], "grad_pointcloud_features_rows": wl.scene.point_cloud_features.grad[idx],
+    }
+    arrays = {k: v.detach().float().cpu().numpy() for k, v in arrays.items()}
+    arrays["sampled_rows"] = rows.astype(np.float64)
+    total = sum(a.nbytes for a in arrays.values())
+    assert total <= DUMP_MAX_BYTES, f"--dump-outputs: {total} bytes > {DUMP_MAX_BYTES}"
+    os.makedirs(out_dir, exist_ok=True)
+    for k, a in arrays.items():
+        np.save(os.path.join(out_dir, f"{k}.npy"), a)
 
 
 if __name__ == "__main__":

@@ -1,5 +1,5 @@
 /*
- * gsb200.h -- C ABI of libgsb200.so: the B200-native (sm_100a) replacement for the rasteriser
+ * gsb200.h -- C ABI of libgsb200.so: the H100-native (sm_90a) replacement for the rasteriser
  * hot path of wanmeihuali/taichi_3d_gaussian_splatting.
  *
  * This header is the drop-in boundary.  Every entry point names the reference interface it
@@ -53,8 +53,8 @@ enum {
                                             pass is bit-identical to the first (normalising twice is not). */
 #define GSB_FLAG_BACKWARD_TRANSPOSED 16u /* backward only: loop A accumulates per splat in registers after a shared-memory
                                             transposition (csrc/blend_bwd_transposed.cu; what the Python operator passes by
-                                            default: 769 us at C3 on a B200) instead of a warp butterfly per (warp, splat)
-                                            (csrc/blend_bwd.cu, 997 us; flag clear) */
+                                            default) instead of a warp butterfly per (warp, splat)
+                                            (csrc/blend_bwd.cu; flag clear) */
 #define GSB_FLAG_NO_HOOK_STATS 32u       /* backward only, opt-in: skip the statistics only a
                                             backward hook reads (|d/duv| magnitude, affected-pixel count, magnitude image) --
                                             the reference's need_extra_info = False, GPCR:521, 690-704.  accum[:, 9:11] and

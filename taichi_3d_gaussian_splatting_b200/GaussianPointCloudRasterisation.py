@@ -6,7 +6,7 @@ of the reference: ``GaussianPointCloudRasterisation(config, backward_valid_point
 ``(image (H,W,3) f32, depth (H,W) f32, pixel_valid_point_count (H,W) i32)`` and whose autograd
 backward produces dense ``(N,3)`` / ``(N,56)`` gradients, scales them with the fixed factors,
 and calls the ``BackwardValidPointHookInput`` side channel -- but every kernel is hand-written
-sm_100a CUDA behind the C ABI of ``libgsb200.so`` (``include/gsb200.h``).  PyTorch is used only
+sm_90a CUDA behind the C ABI of ``libgsb200.so`` (``include/gsb200.h``).  PyTorch is used only
 for device memory, streams and autograd plumbing.  There is no CPU fallback.
 
 Contract details kept from the reference (SURVEY.md §8(b), §9):
@@ -46,7 +46,7 @@ def _require(t: torch.Tensor, name: str, dtype: torch.dtype, shape_tail=None) ->
     if not isinstance(t, torch.Tensor):
         raise TypeError(f"{name} must be a torch.Tensor")
     if not t.is_cuda:
-        raise RuntimeError(f"{name} must live on a CUDA device: the B200 rasteriser has no CPU path")
+        raise RuntimeError(f"{name} must live on a CUDA device: the rasteriser has no CPU path")
     if t.dtype != dtype:
         raise TypeError(f"{name} must be {dtype}, got {t.dtype}")
     if shape_tail is not None and tuple(t.shape[1:]) != tuple(shape_tail):
@@ -235,8 +235,8 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
         every tile of the reference's 3-sigma square instead of only the tiles the splat can actually reach with
         alpha >= 1/255 (same outputs, ~1.5x more keys; used by tests that compare the sorted list itself).
         ``backward_impl``: ``"transposed"`` (default; ``csrc/blend_bwd_transposed.cu``: splat-per-lane accumulation after a
-        shared-memory transposition, 769 us at C3 on a B200) or ``"butterfly"`` (``csrc/blend_bwd.cu``: warp butterfly per
-        (warp, splat), 997 us; kept as the second implementation the parity tests cross-check).  Constructor argument only:
+        shared-memory transposition) or ``"butterfly"`` (``csrc/blend_bwd.cu``: warp butterfly per (warp, splat), slower;
+        kept as the second implementation the parity tests cross-check).  Constructor argument only:
         no environment variable can switch the kernel of a production run.  With no backward hook installed the transposed
         kernel does not compute the statistics only a hook reads (the reference's ``need_extra_info = False``, GPCR:521).
         ``skip_unused_hook_statistics``: the same switch for the butterfly kernel (opt-in; ``None`` reads

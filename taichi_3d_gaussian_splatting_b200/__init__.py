@@ -1,4 +1,4 @@
-"""taichi_3d_gaussian_splatting_b200 -- B200-native (sm_100a) differentiable 3D Gaussian splatting
+"""taichi_3d_gaussian_splatting_b200 -- H100-native (sm_90a) differentiable 3D Gaussian splatting
 rasteriser, a drop-in for the hot path of wanmeihuali/taichi_3d_gaussian_splatting
 (``GaussianPointCloudRasterisation``).  Host code is Python/PyTorch (memory, streams, autograd,
 ``torch.distributed``); every kernel is hand-written CUDA behind the C ABI in ``include/gsb200.h``.

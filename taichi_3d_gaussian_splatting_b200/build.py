@@ -1,4 +1,4 @@
-"""Build ``libgsb200.so`` in-tree with nvcc for sm_100a (no JIT cache: the .so travels with the repo).
+"""Build ``libgsb200.so`` in-tree with nvcc for sm_90a (H100; no JIT cache: the .so is built in the tree).
 
     python -m taichi_3d_gaussian_splatting_b200.build [--force] [--verbose]
 
@@ -18,7 +18,7 @@ EXTRA_DEFINES = os.environ.get("GSB200_DEFINES", "").split()  # e.g. "-DGSB_SORT
 OBJ_DIR = os.path.join(HERE, "build" + ("_" + os.environ["GSB200_LIB_NAME"] if "GSB200_LIB_NAME" in os.environ else ""))
 STAMP = os.path.join(OBJ_DIR, "sources.sha1")
 
-ARCH_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC",
           "--expt-relaxed-constexpr"]
 SOURCES = {

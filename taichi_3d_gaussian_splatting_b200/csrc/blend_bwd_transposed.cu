@@ -1,6 +1,5 @@
-// blend_bwd_transposed.cu -- loop A of the backward (GPCR:531-705); the DEFAULT implementation since round 2 (0.72 ms at
-// BASELINE config 3 on a B200 against 1.00 ms for the round-1 butterfly kernel of blend_bwd.cu, which stays selectable:
-// backward_impl="butterfly").  Verified on the CPU under tests/simt (the kernel body compiled as host C++ and run by a
+// blend_bwd_transposed.cu -- loop A of the backward (GPCR:531-705); the DEFAULT implementation (the butterfly kernel of
+// blend_bwd.cu stays selectable: backward_impl="butterfly").  Verified on the CPU under tests/simt (the kernel body compiled as host C++ and run by a
 // lock-step SIMT emulator against the butterfly kernel and the oracle) and on the GPU by every backward parity test.
 //
 // blend_bwd.cu reduces the 11 per-splat partials of every (warp, splat) visit across the 32 pixels of the warp with a
@@ -29,8 +28,7 @@ struct TbShared {  // dynamic shared memory image, 73 KB -> 3 CTAs per SM
     float4 rec[2 * 3 * GSB_TILE_PIXELS];  // [buf][plane][splat] as in blend_bwd.cu
     float4 g[8][32];                      // dL/dimage of the warp's pixels
     float xg[8][32 * TB_ROW];             // G  per (pixel, splat of the chunk); reused for the finished rows
-    float xa[8][32 * TB_ROW];             // alpha * T   (interleaving the two as float2 -- one 64-bit store / load instead of
-                                          //   two 32-bit ones -- was measured SLOWER on a B200: 724 vs 718 us, profiles/r02_call20.log)
+    float xa[8][32 * TB_ROW];             // alpha * T
     int off[2][GSB_TILE_PIXELS];          // in-camera offset of the staged splats
     float4 chunk[8][3][TB_CHUNK];         // per warp: records of the current chunk's splats [plane][slot]; the unused
                                           //   radius word of plane 2 carries the splat's position in the tile's sorted list
@@ -49,7 +47,7 @@ __device__ __forceinline__ unsigned char *tb_dynamic_smem() { return gsb_tb_dyna
 #endif
 
 #ifndef GSB_TB_P1_UNROLL
-#define GSB_TB_P1_UNROLL 4  // phase-1 splats per loop trip (measured: 1 -> 746, 2 -> 734, 4 -> 725 us at C3)
+#define GSB_TB_P1_UNROLL 4  // phase-1 splats per loop trip
 #endif
 constexpr int TB_P1_UNROLL = GSB_TB_P1_UNROLL;
 #ifndef GSB_TB_MIN_BLOCKS

@@ -60,7 +60,7 @@ __device__ __forceinline__ void count_if_blended(float wgt, int idx, int &cnt, i
 #define GSB_FWD_MIN_BLOCKS 4
 #endif
 #ifndef GSB_FWD_UNROLL
-#define GSB_FWD_UNROLL 8  // measured at C3: unroll 2 / 4 / 8 at 5 CTAs per SM 384 / 381 / 380 us, unroll 8 at 4 CTAs per SM (64 registers) 374 us
+#define GSB_FWD_UNROLL 8  // tuning knob (GSB200_DEFINES="-DGSB_FWD_UNROLL=4")
 #endif
 constexpr int FW_UNROLL = GSB_FWD_UNROLL;
 constexpr int FW_CHUNK = 32;  // splats per private chunk of a warp

@@ -1,4 +1,4 @@
-// common.cuh -- shared declarations of libgsb200 (sm_100a only).
+// common.cuh -- shared declarations of libgsb200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -133,7 +133,7 @@ __device__ __forceinline__ float4 lds128(unsigned int saddr) {
     return v;
 }
 // Shared-space address of a __shared__ object, made opaque so that the compiler keeps it in a register
-// instead of re-deriving it (S2R SR_CgaCtaId + LEA chain on sm_100) inside the inner loops.
+// instead of re-deriving it (S2R SR_CgaCtaId + LEA chain) inside the inner loops.
 __device__ __forceinline__ unsigned int smem_u32(const void *p) {
     unsigned int a = (unsigned int)__cvta_generic_to_shared(p);
     asm volatile("" : "+r"(a));
@@ -305,7 +305,7 @@ static inline int num_sms() {
         int dev = 0;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-        if (n <= 0) n = 148;
+        if (n <= 0) n = 132;
     }
     return n;
 }

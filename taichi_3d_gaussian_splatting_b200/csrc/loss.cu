@@ -7,7 +7,7 @@
 namespace gsb {
 
 constexpr int L1_THREADS = 256;
-constexpr int L1_MAX_BLOCKS = 1184;  // 148 SMs x 8
+constexpr int L1_MAX_BLOCKS = 1056;  // 132 SMs x 8
 
 struct L1Params {
     const float *pred;

@@ -9,11 +9,10 @@
 // This translation unit is compiled with -fmad=false: every float op is a plain IEEE op in the same
 // order as the CPU oracle, and exp() is evaluated in double and rounded once, so all discrete per-point
 // decisions (frustum test, tile bbox, depth key) are bit-reproducible.  On paper the stage is HBM-bound (~240 B read,
-// ~70 B + 8..12 B/key written per in-frustum point); measured on a B200 it is bound by instruction issue and latency:
-// 8.0e7 warp instructions per C3 frame (unfused IEEE arithmetic, seven exp() in double per point) at 32 resident warps per SM.
-// Tried in round 2 and rejected (commit ae2158f, profiles/r02_call7.log): staging each warp's 32 contiguous feature rows
-// (7 KB) with one TMA bulk copy -- the extra 28 KB of shared memory per CTA cut the occupancy from 8 to 5 CTAs per SM and the
-// bulk copy put the whole row fetch in front of the scan's aggregate publish: 166 us instead of 139 us at C3.
+// ~70 B + 8..12 B/key written per in-frustum point); in practice it is bound by instruction issue and latency (unfused
+// IEEE arithmetic, seven exp() in double per point).  Staging each warp's 32 contiguous feature rows (7 KB) with one TMA
+// bulk copy was rejected: the extra 28 KB of shared memory per CTA cut the occupancy from 8 to 5 CTAs per SM and the bulk
+// copy put the whole row fetch in front of the scan's aggregate publish.
 #include "common.cuh"
 
 namespace gsb {
@@ -208,8 +207,8 @@ preprocess_kernel(const PreParams p) {
     // Every global load of a point that depends on nothing but its index is issued HERE, in one go: the invalid mask, the
     // object id, the position and the first 32 bytes of the feature row (q | s, logit).  The kernel is bound by the latency
     // of a CTA's dependency chain (DESIGN section 3): mask -> object id -> pose -> position -> frustum test -> feature row
-    // were four dependent round trips, now they are one plus the (L1-resident) pose: 140.4 -> 136.2 us at C3
-    // (profiles/r02_call23.log).  Rows outside the frustum or unused fetch 32 bytes they do not need (they are allocated:
+    // were four dependent round trips, now they are one plus the (L1-resident) pose.  Rows outside the frustum or unused
+    // fetch 32 bytes they do not need (they are allocated:
     // (N,56)); the arithmetic is untouched.
     signed char h_inv = 1;
     int h_ob = 0;

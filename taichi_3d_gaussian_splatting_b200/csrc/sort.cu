@@ -25,9 +25,8 @@ constexpr int RBITS = 8;                     // digit width
 constexpr int RADIX = 1 << RBITS;            // = SORT_BLOCK_THREADS: thread t owns digit t
 static_assert(RADIX == SORT_BLOCK_THREADS, "one digit per thread");
 
-// Digit width for a key of `bits` live bits.  Measured on B200 in round 1 (C3, 30-bit keys, K = 4.0e6): three 10-bit
-// passes cost 244 us against 199 us for four 8-bit passes (1024-bin ranking + 4 KB of look-back state per CTA outweigh
-// the saved pass), so 8 bits are always used.
+// Digit width for a key of `bits` live bits.  10-bit digits would save a pass at C3 but need 1024-bin ranking and 4 KB
+// of look-back state per CTA, so 8 bits are always used.
 int sort_radix_bits(int bits) {
     (void)bits;
     return RBITS;
@@ -116,8 +115,8 @@ sort_histogram_kernel(const KeyT *__restrict__ keys, const long long *__restrict
     DigitSel<KeyT> sel[8];
 #pragma unroll
     for (int p = 0; p < 8; ++p) sel[p] = make_digit_sel<KeyT>(p, depth_bits, live);
-    // 16 bytes per load and HIST_U loads in flight per thread: with one 4-byte load per trip (round 1) the sweep was bound by
-    // the load latency (8 KB in flight per SM), not by the shared-memory atomics
+    // 16 bytes per load and HIST_U loads in flight per thread: with one 4-byte load per trip the sweep is bound by the load
+    // latency (8 KB in flight per SM), not by the shared-memory atomics
     constexpr int VEC = 16 / (int)sizeof(KeyT), HIST_U = 2;
     const long long stride = (long long)gridDim.x * SORT_BLOCK_THREADS;
     const long long nvec = n / VEC;  // the key buffers are 16-byte aligned (workspace: 256; gsb200_sort_pairs checks keys_in)
@@ -281,9 +280,8 @@ onesweep_pass_kernel(const PassParams<KeyT> P) {
     unsigned short ranks[SORT_ITEMS_PER_THREAD];
     const unsigned int lt_mask = (1u << lane) - 1u;
     unsigned short *const my_cnt = s.warp_cnt[warp];
-    // (Measured without effect, profiles/r02_call22.log: the twelve MATCH.ANY of a thread written as a loop of their own in
-    //  front of the counter chain -- 40 % of a pass's stall samples sit on the instruction behind each MATCH, but ptxas
-    //  re-interleaves the two loops with one MATCH ahead whatever fence is put between them: 128.3 vs 128.3 us.)
+    // (Writing the twelve MATCH.ANY of a thread as a loop of their own in front of the counter chain changes nothing:
+    //  ptxas re-interleaves the two loops with one MATCH ahead whatever fence is put between them.)
 #pragma unroll
     for (int j = 0; j < SORT_ITEMS_PER_THREAD; ++j) {
         const int idx = wbase + j * 32 + lane;

@@ -81,8 +81,8 @@ class ViewParallelExchange:
         """``gather_group``: optionally a SECOND process group over the same ranks (``dist.new_group()``): the all-gather
         then runs on its communicator concurrently with the all-reduce (two NCCL kernels in flight hide each other's
         latency) instead of behind it.  ``overlap_expansion``: gather first and expand the SH columns (they need only the
-        gathered blocks) on a second stream while the all-reduce of the summed columns is on the wire -- measured SLOWER with
-        the NCCL collectives at 2 ranks (1.698 vs 1.676 ms per step, profiles/r02_call18_2gpu.log), hence off by default."""
+        gathered blocks) on a second stream while the all-reduce of the summed columns is on the wire (opt-in, off by
+        default)."""
         if not dist.is_available() or not dist.is_initialized():
             raise RuntimeError("ViewParallelExchange needs an initialised torch.distributed process group")
         self.group = group
@@ -133,7 +133,7 @@ class ViewParallelExchange:
         Default: the collectives, then one expansion pass.  With ``overlap_expansion=True`` (CUDA tensors, one communicator) the
         blocks are gathered FIRST and the 48 SH columns -- 4/5 of the expansion's traffic, HBM-bound -- are expanded on a second
         stream while the all-reduce of the summed columns is on the wire; only the small part 2 (xyz, q, s, logit) waits for the
-        sums.  The two parts write disjoint pieces of the dense gradients.  (Opt-in: measured slower at 2 ranks.)"""
+        sums.  The two parts write disjoint pieces of the dense gradients.  (Opt-in.)"""
         if not (self._overlap and grad_sum.is_cuda) or self.gather_group is not None:
             self.run(grad_sum, blocks)
             return expand(0)
@@ -160,10 +160,8 @@ class MulticastViewParallelExchange(ViewParallelExchange):
 
     def __init__(self, group=None, barrier_timeout_ms: int = 20000, num_blocks: int = 0, overlap_expansion: bool = False):
         """``num_blocks``: CTAs of the exchange kernel (0 = two per SM).  ``overlap_expansion``: expand the SH columns (they
-        need only the gathered blocks) on a second stream while the all-reduce of the summed columns is on the wire.  Measured
-        at 8 GPUs (profiles/r02_call19_8gpu.log): 1.809 ms per step against 1.797 ms with the one-pass expansion behind the
-        second barrier (1.804 with one exchange CTA per SM) -- the expansion's 128-register CTAs and its 290 MB of HBM traffic
-        slow the wire-bound kernel down by more than the 45 us they hide -- so it is off by default."""
+        need only the gathered blocks) on a second stream while the all-reduce of the summed columns is on the wire.  Off by
+        default: the expansion's 128-register CTAs and its HBM traffic compete with the wire-bound exchange kernel."""
         super().__init__(group, overlap_expansion=overlap_expansion)
         self._num_blocks = int(num_blocks)
         self._overlap = bool(overlap_expansion)
@@ -238,7 +236,7 @@ class MulticastViewParallelExchange(ViewParallelExchange):
         every rank's block is in place after the FIRST barrier (the pushes were launched before it), so the 48 SH columns
         -- 4/5 of the expansion's traffic, HBM-bound -- are expanded on a second stream while the all-reduce of the summed
         columns is still bound by the NVLink wire; only the small part 2 (xyz, q, s, logit) follows the second barrier.
-        (Opt-in: measured slower at 8 GPUs, see ``__init__``.)"""
+        (Opt-in, see ``__init__``.)"""
         if not self._overlap:
             return super().run_and_expand(grad_sum, blocks, expand)
         e = self._check(grad_sum, blocks)

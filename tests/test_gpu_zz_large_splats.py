@@ -1,6 +1,5 @@
 """Large splats (17..96 tiles each) through the CUDA operator vs the oracle -- the more-than-64-tiles branch of the
-cooperative reach filter and ~1000-entry tile lists.  Kept in its own module, after the other GPU parity modules: it was
-written after the round's GPU minutes were spent, so its first B200 run is the round-end run (DESIGN.md section 6)."""
+cooperative reach filter and ~1000-entry tile lists.  Kept in its own module, after the other GPU parity modules."""
 import numpy as np
 import pytest
 import torch
