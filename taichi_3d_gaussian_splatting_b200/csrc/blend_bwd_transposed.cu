@@ -4,40 +4,66 @@
 //
 // blend_bwd.cu reduces the 11 per-splat partials of every (warp, splat) visit across the 32 pixels of the warp with a
 // 13-shuffle butterfly: ~52 of the ~117 SASS instructions of a visit.  Here a warp copies the splats of its culled list,
-// 16 at a time, into a private chunk buffer (a partial chunk at the end of a staging batch is carried over and topped up
-// from the next batch, so only the last chunk of a tile can be short) and works on a chunk in two phases:
+// TB_CHUNK at a time, into a private chunk buffer (a partial chunk at the end of a staging batch is carried over and topped
+// up from the next batch, so only the last chunk of a tile can be short) and works on a chunk in two phases:
 //   phase 1 (lane = pixel, as before): the sequential part of GPCR:609-657 -- alpha, the transmittance recursion and
 //     the colour recursion -- which leaves two numbers per (pixel, splat): G = dL/dalpha * alpha and alpha*T.  They go
-//     to a 32 x 16 exchange buffer in shared memory (row stride 17: conflict-free both ways);
-//   phase 2 (lane = splat; lanes 0..15 take pixels 0..15 of the patch, lanes 16..31 the same splats for pixels 16..31):
-//     every lane re-derives d and conic*d for its splat, accumulates the 11 partials over its 16 pixels in registers,
-//     the two halves are added with one shuffle per value, and the 16 finished rows leave through shared memory as
-//     8 RED.ADD.F32 instructions of two contiguous rows each (same 2 sectors per (warp, splat) as the butterfly kernel).
-// Per 32 (pixel, splat) pairs that is ~36 (phase 1) + ~36 (chunk fill, phase 2, epilogue) SASS instructions.
+//     as one float2 to a 32 x TB_CHUNK exchange buffer in shared memory (bank arithmetic at TbShared);
+//   phase 2 (lane = splat; 32/TB_CHUNK lanes share a splat, each takes TB_CHUNK/8 rows of the 8 x 4 patch): along a row
+//     conic*d is linear in the pixel's column offset k, so a lane sums only G, k G and k^2 G per row and rebuilds the five
+//     geometric partials from these moments after the row; the colour partials are summed per pixel.  The lanes of a
+//     splat are added with log2(32/TB_CHUNK) shuffles per value, and the TB_CHUNK finished rows leave through shared
+//     memory as 16-byte vector REDs, 3 per row (same 2 sectors per (warp, splat) as the butterfly kernel).
 // STATS = false (GSB_FLAG_NO_HOOK_STATS, the reference's need_extra_info = False, GPCR:521, 690-704) drops the |d/duv|
 // magnitude, the affected-pixel count and the per-pixel magnitude image.
 #include "blend_bwd.cuh"
 
 namespace gsb {
 
-constexpr int TB_CHUNK = 16;          // splats per chunk
-constexpr int TB_ROW = TB_CHUNK + 1;  // row stride (floats) of the (pixel, splat) exchange buffers
-constexpr int TB_TR_ROW = 13;         // row stride of the finished rows (12 accumulator words, odd stride)
+// Splats per chunk: 16 (a phase-2 lane owns two rows of the patch; 71 KB, 80 registers -> 3 CTAs per SM) or 8 (one row;
+// 52 KB, 64 registers -> 4 CTAs per SM).  On an H100 at C3 the 4th CTA does not pay for the second shuffle level and
+// the halved amortisation of the chunk's epilogue: 16 is the faster (DESIGN section 3).
+#ifndef GSB_TB_CHUNK
+#define GSB_TB_CHUNK 16
+#endif
+#ifndef GSB_TB_MIN_BLOCKS  // tuning knob (GSB200_DEFINES="-DGSB_TB_CHUNK=8 -DGSB_TB_MIN_BLOCKS=4")
+#if GSB_TB_CHUNK == 8
+#define GSB_TB_MIN_BLOCKS 4
+#else
+#define GSB_TB_MIN_BLOCKS 3
+#endif
+#endif
+constexpr int TB_CHUNK = GSB_TB_CHUNK;
+static_assert(TB_CHUNK == 8 || TB_CHUNK == 16, "a phase-2 lane takes whole rows of the 8 x 4 patch");
+constexpr int TB_ROWS = TB_CHUNK / 8;  // patch rows per phase-2 lane
+constexpr int TB_ROW = TB_CHUNK + 1;   // row stride (float2) of the (pixel, splat) exchange buffer: odd, see below
 
-struct TbShared {  // dynamic shared memory image, 73 KB -> 3 CTAs per SM
-    float4 rec[2 * 3 * GSB_TILE_PIXELS];  // [buf][plane][splat] as in blend_bwd.cu
-    float4 g[8][32];                      // dL/dimage of the warp's pixels
-    float xg[8][32 * TB_ROW];             // G  per (pixel, splat of the chunk); reused for the finished rows
-    float xa[8][32 * TB_ROW];             // alpha * T
-    int off[2][GSB_TILE_PIXELS];          // in-camera offset of the staged splats
-    float4 chunk[8][3][TB_CHUNK];         // per warp: records of the current chunk's splats [plane][slot]; the unused
-                                          //   radius word of plane 2 carries the splat's position in the tile's sorted list
-    int chunk_off[8][TB_CHUNK];           //   their accumulator row (set to -1 after phase 2 if nothing is to be added)
+// Exchange buffer bank arithmetic.  A 64-bit shared access is served per half-warp (16 lanes x 8 B = the 32 banks), so
+// both patterns take their minimum of 2 wavefronts when the 16 float2 indices of a half-warp are distinct mod 16:
+//   phase 1 (lane = pixel p, splat i fixed):  p * TB_ROW + i, TB_ROW odd -> distinct for 16 consecutive p;
+//   phase 2 (pixel pp = 8 row + k, k fixed):  TB_CHUNK = 16: one pixel, 16 consecutive splats; TB_CHUNK = 8: splats
+//     0..7 of pixels pp and pp + 8, 8 * 9 = 72 = 8 mod 16 apart -> two disjoint runs of 8.
+struct TbWarp {  // a warp's private buffers: one base register addresses them all
+    float4 g[32];                       // dL/dimage of the warp's pixels
+    float4 chunk[3][TB_CHUNK];          // records of the current chunk's splats [plane][slot]; the radius word of plane 2
+                                        //   carries the splat's position in the tile's sorted list
+    float2 x[32 * TB_ROW];              // (G, alpha * T) per (pixel, splat of the chunk); reused for the finished rows
+    int chunk_off[TB_CHUNK];            // accumulator rows of the chunk's splats (-1 after phase 2 if nothing is to be added)
+    unsigned char list[GSB_TILE_PIXELS];  // elements of the current batch to visit, back to front
+};
+struct TbShared {  // dynamic shared memory image: 52 KB (TB_CHUNK = 8) or 71 KB (16)
+    float4 rec[2 * 3 * GSB_TILE_PIXELS];  // [buf][plane][splat] as in blend_bwd.cu; the radius word of plane 2 (unused by
+                                          //   the backward) carries the splat's in-camera offset
+    TbWarp w[8];
     unsigned int bits[2][8][8];           // [buf][consumer warp patch][loader warp]
-    unsigned char list[8][GSB_TILE_PIXELS];  // per warp: elements of the current batch to visit, back to front
+    float2 origin;                        // the tile's corner in pixels: re-read where needed rather than held in two registers
     int max_last;
 };
-static_assert(32 * TB_ROW >= TB_CHUNK * TB_TR_ROW, "finished rows must fit into the exchange buffer");
+static_assert(2 * 32 * TB_ROW >= TB_CHUNK * GSB_ACCUM_FLOATS && GSB_ACCUM_FLOATS == 12,
+              "the finished rows (3 float4 each) must fit into the exchange buffer");
+// the H100 has 228 KB of shared memory per SM and reserves 1 KB of it per resident CTA
+static_assert(GSB_TB_MIN_BLOCKS * (sizeof(TbShared) + 1024) <= 228 * 1024,
+              "the shared-memory image does not allow GSB_TB_MIN_BLOCKS CTAs per SM");
 
 #ifdef GSB_HOST_EMU
 static inline unsigned char *tb_dynamic_smem() { return simt_emu::dynamic_smem(); }
@@ -50,9 +76,18 @@ __device__ __forceinline__ unsigned char *tb_dynamic_smem() { return gsb_tb_dyna
 #define GSB_TB_P1_UNROLL 4  // phase-1 splats per loop trip
 #endif
 constexpr int TB_P1_UNROLL = GSB_TB_P1_UNROLL;
-#ifndef GSB_TB_MIN_BLOCKS
-#define GSB_TB_MIN_BLOCKS 3  // 73 KB of shared memory per CTA allow 3; tuning knob (GSB200_DEFINES="-DGSB_TB_MIN_BLOCKS=2")
+static_assert(TB_CHUNK % TB_P1_UNROLL == 0, "a full chunk is a whole number of phase-1 groups");
+// one 16-byte RED.ADD of four f32 (sm_90: atomicAdd on a float4 in global memory); the emulator adds word by word
+__device__ __forceinline__ void red_add_f32x4(float *addr, const float4 v) {
+#ifdef GSB_HOST_EMU
+    atomicAdd(addr, v.x);
+    atomicAdd(addr + 1, v.y);
+    atomicAdd(addr + 2, v.z);
+    atomicAdd(addr + 3, v.w);
+#else
+    atomicAdd(reinterpret_cast<float4 *>(addr), v);
 #endif
+}
 // P if (idx < last && P >= 1/255) else 0 -- the two tests folded into one predicate (ISETP, FSETP.AND, FSEL instead of
 // the two selects the compiler makes of the && expression)
 __device__ __forceinline__ float keep_if_contributing(float P, int idx, int last) {
@@ -84,7 +119,6 @@ blend_backward_transposed_kernel(const BlendBwdParams p) {
     const int pu = tu * GSB_TILE_WIDTH + (warp & 1) * 8 + (lane & 7);
     const int pv = tv * GSB_TILE_HEIGHT + (warp >> 1) * 4 + (lane >> 3);
     const float px = (float)pu + 0.5f, py = (float)pv + 0.5f;
-    const float tile_x0 = (float)(tu * GSB_TILE_WIDTH), tile_y0 = (float)(tv * GSB_TILE_HEIGHT);
     const size_t pix = (size_t)pv * p.W + pu;
     const int start = p.tile_start[tile];
 
@@ -94,32 +128,29 @@ blend_backward_transposed_kernel(const BlendBwdParams p) {
     const float g0 = p.grad_image[3 * pix], g1 = p.grad_image[3 * pix + 1], g2 = p.grad_image[3 * pix + 2];
     float mag0 = 0.0f, mag1 = 0.0f;
     unsigned int n_visits = 0, n_pairs = 0;  // COUNT only
-    S.g[warp][lane] = make_float4(g0, g1, g2, 0.0f);
+    TbWarp &Wp = S.w[warp];
+    Wp.g[lane] = make_float4(g0, g1, g2, 0.0f);
 
-    // phase-2 role of this lane: splat `ci` of the chunk, pixels 16*half .. 16*half+15 of the patch (= rows 2*half, 2*half+1)
-    const int ci = lane & (TB_CHUNK - 1), half = lane >> 4;
-    const float pxb = tile_x0 + (float)((warp & 1) * 8) + 0.5f;
-    const float pyb = tile_y0 + (float)((warp >> 1) * 4 + 2 * half) + 0.5f;
-    float *const xg = S.xg[warp], *const xa = S.xa[warp];
-    // flush role of this lane: word fl_word of the even (lanes 0..11) or odd (lanes 12..23) row of a row pair
-    const int fl_row = lane >= GSB_ACCUM_FLOATS ? 1 : 0;
-    const int fl_word = lane - GSB_ACCUM_FLOATS * fl_row;
-    const bool fl_ok = lane < 2 * GSB_ACCUM_FLOATS && fl_word < NV;
-    const int *const fl_off = S.chunk_off[warp] + fl_row;
-    const float *const fl_val = xg + fl_row * TB_TR_ROW + (fl_ok ? fl_word : 0);
-    unsigned char *const list = S.list[warp];
+    // phase-2 role of this lane: splat `ci` of the chunk, rows row0 .. row0 + TB_ROWS - 1 of the patch
+    const int ci = lane % TB_CHUNK, row0 = (lane / TB_CHUNK) * TB_ROWS;
+    float2 *const x = Wp.x;
+    float4 *const fin = reinterpret_cast<float4 *>(x);  // the finished rows: 3 float4 per splat of the chunk
+    unsigned char *const list = Wp.list;
 
     int warp_last = last;
 #pragma unroll
     for (int d = 16; d > 0; d >>= 1) warp_last = max(warp_last, __shfl_xor_sync(0xffffffffu, warp_last, d));
-    if (tid == 0) S.max_last = start;
+    if (tid == 0) {
+        S.max_last = start;
+        S.origin = make_float2((float)(tu * GSB_TILE_WIDTH), (float)(tv * GSB_TILE_HEIGHT));
+    }
     __syncthreads();
     if (lane == 0) atomicMax(&S.max_last, warp_last);
     __syncthreads();
     const int end = min(p.tile_end[tile], S.max_last);
 
-    float4 *const ck0 = S.chunk[warp][0], *const ck1 = S.chunk[warp][1], *const ck2 = S.chunk[warp][2];
-    int *const ck_off = S.chunk_off[warp];
+    float4 *const ck0 = Wp.chunk[0], *const ck1 = Wp.chunk[1], *const ck2 = Wp.chunk[2];
+    int *const ck_off = Wp.chunk_off;
     int have = 0;  // splats waiting in the chunk buffer (warp-uniform)
 
     // One barrier per staging batch (double-buffered, see blend_fwd.cu).  After the last batch one more trip through the
@@ -148,9 +179,10 @@ blend_backward_transposed_kernel(const BlendBwdParams p) {
                         s_r0[tid] = f0;
                         s_r1[tid] = f1;
                     }
-                    s_r2[tid] = __ldg(rec + 2);
-                    S.off[buf][tid] = o;
-                    mask = splat_patch_mask(r0.x, r0.y, r0.z, r0.w, r1.x, r1.y * r1.z, tile_x0, tile_y0);
+                    float4 r2 = __ldg(rec + 2);
+                    r2.w = __int_as_float(o);  // in-camera offset instead of the radius (unused here)
+                    s_r2[tid] = r2;
+                    mask = splat_patch_mask(r0.x, r0.y, r0.z, r0.w, r1.x, r1.y * r1.z, S.origin.x, S.origin.y);
                 }
 #pragma unroll
                 for (int w = 0; w < 8; ++w) {
@@ -188,9 +220,9 @@ blend_backward_transposed_kernel(const BlendBwdParams p) {
                     ck0[slot] = s_r0[j];
                     ck1[slot] = s_r1[j];
                     float4 r2 = s_r2[j];
-                    r2.w = __int_as_float(block_end - 1 - j);  // sorted index instead of the radius (unused here)
+                    ck_off[slot] = __float_as_int(r2.w);
+                    r2.w = __int_as_float(block_end - 1 - j);  // sorted index instead of the in-camera offset
                     ck2[slot] = r2;
-                    ck_off[slot] = S.off[buf][j];
                 }
                 have += take;
                 pos += take;
@@ -205,8 +237,7 @@ blend_backward_transposed_kernel(const BlendBwdParams p) {
                     GSB_EMU_COUNT(EC_TB_CHUNKS, 1);
                 }
                 // ---- phase 1: lane = pixel; sequential over the chunk's splats (back to front)
-#pragma unroll TB_P1_UNROLL
-                for (int i = 0; i < n; ++i) {
+                const auto p1 = [&](const int i) -> float2 {
                     const float4 r0 = ck0[i];  // u v a b                   (fast path: u v A B, conic scaled by -log2(e)/2)
                     const float4 r1 = ck1[i];  // c rescale opacity depth   (fast path: C rescale*opacity 1-opacity depth)
                     const float4 r2 = ck2[i];  // r g b | sorted index
@@ -258,12 +289,27 @@ blend_backward_transposed_kernel(const BlendBwdParams p) {
                         }
                     }
                     if (COUNT) n_pairs += aT > 0.0f ? 1u : 0u;
-                    xg[lane * TB_ROW + i] = G;
-                    xa[lane * TB_ROW + i] = aT;
+                    return make_float2(G, aT);
+                };
+                if (n == TB_CHUNK) {
+                    // Groups of TB_P1_UNROLL splats, their exchange stores after the group: the compiler cannot tell the
+                    // exchange buffer from the chunk buffer, so a store between two splats would keep the next splat's
+                    // loads and alpha (independent of the recursion) from being scheduled under the previous one.
+#pragma unroll 1
+                    for (int i0 = 0; i0 < TB_CHUNK; i0 += TB_P1_UNROLL) {
+                        float2 ex[TB_P1_UNROLL];
+#pragma unroll
+                        for (int u = 0; u < TB_P1_UNROLL; ++u) ex[u] = p1(i0 + u);
+#pragma unroll
+                        for (int u = 0; u < TB_P1_UNROLL; ++u) x[lane * TB_ROW + i0 + u] = ex[u];
+                    }
+                } else {  // the short last chunk of a tile
+#pragma unroll 1
+                    for (int i = 0; i < n; ++i) x[lane * TB_ROW + i] = p1(i);
                 }
                 __syncwarp();
 
-                // ---- phase 2: lane = splat ci of the chunk, over 16 pixels
+                // ---- phase 2: lane = splat ci of the chunk, over the TB_CHUNK pixels of its rows
                 const bool active = ci < n;
                 float4 s0 = ck0[active ? ci : 0];
                 float4 s1 = ck1[active ? ci : 0];
@@ -272,64 +318,85 @@ blend_backward_transposed_kernel(const BlendBwdParams p) {
                     s0.w *= -1.0f / GSB_L2E;
                     s1.x *= -2.0f / GSB_L2E;
                 }
-                // conic * d at the first pixel of each of this lane's two rows; along a row d0 grows by exactly 1 per pixel, so
-                // q0 += a, q1 += b (two FADD instead of two FMUL + two FFMA per pixel)
-                const float dx0 = pxb - s0.x;
+                const float ca = s0.z, cb = s0.w, cc = s1.x;  // conic (a, b, c)
+                // this lane's rows: pixel centres pxc + kc, kc = k - 3.5 for the pixels k = 0..7 of a row (half-integers:
+                // kc and kc^2 are exact)
+                const float2 org = S.origin;
+                const float pxc = org.x + (float)((warp & 1) * 8) + 4.0f;
+                const float pyb = org.y + (float)((warp >> 1) * 4 + row0) + 0.5f;
+                const float dxc = pxc - s0.x;  // d0 at the centre of the row
                 float acc[11];
 #pragma unroll
                 for (int k = 0; k < 11; ++k) acc[k] = 0.0f;
                 unsigned int nz = 0u;
 #pragma unroll
-                for (int row = 0; row < 2; ++row) {
+                for (int row = 0; row < TB_ROWS; ++row) {
+                    // along the row d0 = dxc + kc, so conic * d = (q0r + a kc, q1r + b kc): the moments m0 = sum G,
+                    // m1 = sum kc G, m2 = sum kc^2 G of the row (one FADD and two FFMA per pixel) give all five geometric sums
                     const float d1 = (pyb + (float)row) - s0.y;
-                    float q0 = s0.z * dx0 + s0.w * d1;
-                    float q1 = s0.w * dx0 + s1.x * d1;
+                    const float q0r = fmaf(ca, dxc, cb * d1);
+                    const float q1r = fmaf(cb, dxc, cc * d1);
+                    float m0 = 0.0f, m1 = 0.0f, m2 = 0.0f;
 #pragma unroll
                     for (int k = 0; k < 8; ++k) {
-                        const int pp = 8 * row + k + 16 * half;  // the pixel = phase-1 lane
-                        const float G = xg[pp * TB_ROW + ci], aT = xa[pp * TB_ROW + ci];
-                        const float4 gp = S.g[warp][pp];
-                        const float vs0 = G * q0, vs1 = G * q1;
-                        acc[0] += vs0;
-                        acc[1] += vs1;
-                        acc[2] = fmaf(vs0, q0, acc[2]);  // the 1/2 of UT:345 is applied once per point in the epilogue kernel
-                        acc[3] = fmaf(vs0, q1, acc[3]);
-                        acc[4] = fmaf(vs1, q1, acc[4]);
-                        acc[5] = fmaf(aT, gp.x, acc[5]);
-                        acc[6] = fmaf(aT, gp.y, acc[6]);
-                        acc[7] = fmaf(aT, gp.z, acc[7]);
-                        acc[8] += G;
+                        const float kc = (float)k - 3.5f;
+                        const int pp = 8 * (row0 + row) + k;  // the pixel = phase-1 lane
+                        const float2 ga = x[pp * TB_ROW + ci];  // (G, alpha * T)
+                        const float4 gp = Wp.g[pp];
+                        m0 += ga.x;
+                        m1 = fmaf(kc, ga.x, m1);
+                        m2 = fmaf(kc * kc, ga.x, m2);
+                        acc[5] = fmaf(ga.y, gp.x, acc[5]);
+                        acc[6] = fmaf(ga.y, gp.y, acc[6]);
+                        acc[7] = fmaf(ga.y, gp.z, acc[7]);
                         if (STATS) {
-                            const float m2 = vs0 * vs0 + vs1 * vs1;
-                            acc[9] += EXACT_EXP ? sqrtf(m2) : sqrt_approx(m2);
-                            acc[10] += aT > 0.0f ? 1.0f : 0.0f;  // alpha >= 1/255 and T > 0: alpha*T > 0 exactly for the contributing pixels
+                            const float vs0 = ga.x * fmaf(ca, kc, q0r), vs1 = ga.x * fmaf(cb, kc, q1r);
+                            const float mm = vs0 * vs0 + vs1 * vs1;
+                            acc[9] += EXACT_EXP ? sqrtf(mm) : sqrt_approx(mm);
+                            acc[10] += ga.y > 0.0f ? 1.0f : 0.0f;  // alpha >= 1/255 and T > 0: alpha*T > 0 exactly for the contributing pixels
                         }
-                        nz |= __float_as_uint(aT);
-                        q0 += s0.z;
-                        q1 += s0.w;
+                        nz |= __float_as_uint(ga.y);
                     }
+                    // t = sum G q, u = sum kc G q; sum G q0 q0 = q0r t0 + a u0, sum G q0 q1 = q1r t0 + b u0, sum G q1 q1 = q1r t1 + b u1
+                    const float t0 = fmaf(ca, m1, q0r * m0), t1 = fmaf(cb, m1, q1r * m0);
+                    const float u0 = fmaf(ca, m2, q0r * m1), u1 = fmaf(cb, m2, q1r * m1);
+                    acc[0] += t0;
+                    acc[1] += t1;
+                    acc[2] += fmaf(ca, u0, q0r * t0);  // the 1/2 of UT:345 is applied once per point in the epilogue kernel
+                    acc[3] += fmaf(cb, u0, q1r * t0);
+                    acc[4] += fmaf(cb, u1, q1r * t1);
+                    acc[8] += m0;
                 }
-                // rows 0..1 + rows 2..3 of the patch
+                // the lanes of the splat: rows 0..3 of the patch
 #pragma unroll
-                for (int k = 0; k < NV; ++k) acc[k] += __shfl_xor_sync(0xffffffffu, acc[k], 16);
-                nz |= __shfl_xor_sync(0xffffffffu, nz, 16);
+                for (int d = TB_CHUNK; d < 32; d *= 2) {
+#pragma unroll
+                    for (int k = 0; k < NV; ++k) acc[k] += __shfl_xor_sync(0xffffffffu, acc[k], d);
+                    nz |= __shfl_xor_sync(0xffffffffu, nz, d);
+                }
                 acc[8] *= EXACT_EXP ? (1.0f - s1.z) : s1.z;  // d alpha / d logit = alpha (1 - opacity)
-                __syncwarp();  // every lane has consumed its xg / xa entries: xg now takes the finished rows
+                __syncwarp();  // every lane has consumed its exchange entries: the buffer now takes the finished rows
                 if (lane < TB_CHUNK) {
                     if (!(active && nz != 0u)) ck_off[ci] = -1;
                     else GSB_EMU_COUNT(EC_TB_ROWS, 1);
-#pragma unroll
-                    for (int k = 0; k < NV; ++k) xg[ci * TB_TR_ROW + k] = acc[k];
+                    // the whole 12-word row (words NV..11 are zero): 48 B apart, so the 8 lanes of a quarter-warp cover
+                    // the 32 banks once per float4
+                    fin[3 * ci] = make_float4(acc[0], acc[1], acc[2], acc[3]);
+                    fin[3 * ci + 1] = make_float4(acc[4], acc[5], acc[6], acc[7]);
+                    fin[3 * ci + 2] = make_float4(acc[8], STATS ? acc[9] : 0.0f, STATS ? acc[10] : 0.0f, 0.0f);
                 }
                 __syncwarp();
-                // two rows per step: lanes 0..11 the words of row 2s, lanes 12..23 those of row 2s+1 (no index division)
+                // float4 e of the chunk's finished rows goes to word 4 (e % 3) of row e / 3: the same 2 sectors per row
+                // as 12 scalar REDs, in 3 vector REDs
 #pragma unroll
-                for (int step = 0; step < TB_CHUNK / 2; ++step) {
-                    const int o = fl_off[2 * step];
-                    const float v = fl_val[2 * step * TB_TR_ROW];
-                    if (fl_ok && o >= 0) atomicAdd(p.accum + (size_t)o * GSB_ACCUM_FLOATS + fl_word, v);
+                for (int e0 = 0; e0 < 3 * TB_CHUNK; e0 += 32) {
+                    const int e = e0 + lane, row = e / 3;
+                    if (e < 3 * TB_CHUNK) {
+                        const int o = ck_off[row];
+                        if (o >= 0) red_add_f32x4(p.accum + (size_t)o * GSB_ACCUM_FLOATS + 4 * (e - 3 * row), fin[e]);
+                    }
                 }
-                __syncwarp();  // the next chunk overwrites the chunk buffer and xg
+                __syncwarp();  // the next chunk overwrites the chunk buffer and the exchange buffer
             }
         } while (pos < count);
         if (!real) break;
