@@ -68,7 +68,7 @@ enum {
  * gsb200_workspace_layout(); the Python shim uses it to expose saved-for-backward tensors as views. */
 typedef struct GsbWorkspaceLayout {
     int64_t total_bytes;
-    int64_t zero_bytes;        /* [0, zero_bytes) is memset to 0 at the start of every forward */
+    int64_t zero_bytes;        /* [0, zero_bytes): per-frame state, cleared on the device by every forward's own kernels */
     int64_t counters;          /* int64[8]: [0]=M in-frustum points, [1]=K (tile,splat) pairs emitted/needed,
                                   [2]=overflow (K > key_capacity), [4]=largest depth key int32(depth * scale) of the frame
                                   (low 32 bits): the sort only runs the passes its live bits need */
@@ -286,7 +286,8 @@ int gsb200_stage_blend(const GsbForwardArgs *args);        /* K6 */
 
 /* Diagnostic variants of forward/backward: identical launches with a CUDA event recorded on the
  * launching stream between stages; block until done and return device milliseconds per stage in
- * stage_ms_out[8] (host): forward = {workspace memset, preprocess, sort, tile ranges, blend};
+ * stage_ms_out[8] (host): forward = {empty (no workspace memset: the pose kernel clears the per-frame state), preprocess,
+ * sort, tile ranges, blend};
  * backward = {grad/accumulator memsets, blend backward, per-point chain rule}.  (The reference's
  * counterpart is the Taichi kernel profiler, GaussianPointTrainer.py:217-219.) */
 int gsb200_forward_timed(const GsbForwardArgs *args, float *stage_ms_out);

@@ -83,7 +83,7 @@ int sort_radix_bits(int bits);
 int sort_pairs_device(const void *keys_in, const int *vals_in, void *keys_out, int *vals_out,
                       const long long *n_dev, int64_t n_capacity, int key_bytes, int depth_bits, int end_bit,
                       const int *max_depth_key /*device or NULL*/, unsigned int *hist /*8*256, zeroed*/,
-                      unsigned int *state /*zeroed*/, unsigned int *tickets /*9, zeroed*/, void *tmp_keys,
+                      unsigned int *state /*cleared by the sort*/, unsigned int *tickets /*9, zeroed*/, void *tmp_keys,
                       int *tmp_vals, cudaStream_t stream);
 
 #ifndef GSB_SORT_ITEMS
@@ -242,6 +242,7 @@ __device__ __forceinline__ void bulk_copy_g2s(void *dst_smem, const void *src_gm
 // every lane of the warp calls the wait (warp-uniform condition at both call sites): under the emulator it is a warp
 // rendezvous, so the lane that issued the (immediate) copy has done so before any lane reads the destination
 __device__ __forceinline__ void mbar_wait(unsigned long long *, unsigned int) { simt_emu::warp_exchange(0u); }
+__device__ __forceinline__ void fence_proxy_async_smem() {}
 #else
 // ---- mbarrier / bulk-copy helpers (TMA 1-D bulk copy, global -> shared)
 __device__ __forceinline__ unsigned int smem_addr(const void *p) {
@@ -277,6 +278,8 @@ __device__ __forceinline__ void mbar_wait(unsigned long long *bar, unsigned int 
         "r"(parity)
         : "memory");
 }
+// orders this CTA's earlier generic-proxy accesses to shared memory before a following bulk copy into the same bytes
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 #endif
 
 #endif

@@ -57,9 +57,17 @@ __device__ __forceinline__ void quat_mul(const float *a, const float *b, float *
 // ------------------------------------------------------------------ pose kernel
 // inverse_SE3_qt_torch (UT:426-432, called at GPCR:845) + transform_matrix_from_quaternion_and_translation
 // (GP3D:51-62) + camera centre of taichi_inverse_SE3 (UT:495-510), once per object instead of per point.
+// It is the frame's first kernel, so it also zeroes the two 16-byte-aligned ranges [clear0, clear0 + clear0_vec) and
+// [clear1, clear1 + clear1_vec) of per-frame state (counters, tickets, the compaction scan's look-back state, the digit
+// histograms, the tile ranges) that the later kernels count into or spin on, so the forward needs no driver memset.  The
+// sort's look-back state is cleared by the histogram kernel, which knows the frame's key count.
 __global__ void pose_kernel(const float *__restrict__ q_pc, const float *__restrict__ t_pc, int n_obj,
-                            PoseBlock *__restrict__ poses) {
-    int o = blockIdx.x * blockDim.x + threadIdx.x;
+                            PoseBlock *__restrict__ poses, uint4 *__restrict__ clear0 = nullptr, int clear0_vec = 0,
+                            uint4 *__restrict__ clear1 = nullptr, int clear1_vec = 0) {
+    const int o = blockIdx.x * blockDim.x + threadIdx.x;
+    const int stride = gridDim.x * blockDim.x;
+    for (int k = o; k < clear0_vec; k += stride) clear0[k] = make_uint4(0u, 0u, 0u, 0u);
+    for (int k = o; k < clear1_vec; k += stride) clear1[k] = make_uint4(0u, 0u, 0u, 0u);
     if (o >= n_obj) return;
     float qi[4] = {-q_pc[4 * o], -q_pc[4 * o + 1], -q_pc[4 * o + 2], q_pc[4 * o + 3]};
     float t[3] = {t_pc[3 * o], t_pc[3 * o + 1], t_pc[3 * o + 2]};
@@ -147,7 +155,7 @@ __device__ __forceinline__ void bounding_box(float u, float v, float radii, int 
 }
 
 #ifndef GSB_PRE_MIN_BLOCKS
-#define GSB_PRE_MIN_BLOCKS 8
+#define GSB_PRE_MIN_BLOCKS 5
 #endif
 // Per-warp staging area of the cooperative reach filter / key emission (32 splats of the warp).
 struct WarpStage {
@@ -542,10 +550,17 @@ preprocess_kernel(const PreParams p) {
 #ifndef GSB_HOST_EMU  // tests/simt compiles the kernels above as host C++ under the SIMT emulator
 int launch_preprocess(const GsbForwardArgs &a, const Workspace &ws, cudaStream_t stream) {
     const GsbWorkspaceLayout &L = ws.layout;
-    if (a.num_objects > 0) {
+    {
+        // per-frame state to zero: [counters, sort_state) and [tile_start, zero_bytes) -- every offset is 256-B aligned
+        const int clear0_vec = (int)((L.sort_state - L.counters) / 16), clear1_vec = (int)((L.zero_bytes - L.tile_start) / 16);
         const int threads = 64;
-        pose_kernel<<<(a.num_objects + threads - 1) / threads, threads, 0, stream>>>(
-            a.q_pointcloud_camera, a.t_pointcloud_camera, a.num_objects, ws.poses);
+        const int pose_blocks = (a.num_objects + threads - 1) / threads;
+        int clear_blocks = (clear0_vec + clear1_vec + 4 * threads - 1) / (4 * threads);  // four 16-B stores per thread
+        if (clear_blocks > 4 * num_sms()) clear_blocks = 4 * num_sms();
+        const int blocks = pose_blocks > clear_blocks ? pose_blocks : clear_blocks;
+        pose_kernel<<<blocks > 0 ? blocks : 1, threads, 0, stream>>>(
+            a.q_pointcloud_camera, a.t_pointcloud_camera, a.num_objects, ws.poses,
+            reinterpret_cast<uint4 *>(ws.counters), clear0_vec, reinterpret_cast<uint4 *>(ws.tile_start), clear1_vec);
         GSB_CUDA_CHECK(cudaGetLastError());
     }
     if (a.num_points <= 0) return GSB_OK;

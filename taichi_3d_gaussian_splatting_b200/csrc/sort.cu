@@ -4,7 +4,7 @@
 // One-sweep organisation: one histogram kernel builds the digit histograms of every pass (and their exclusive
 // prefixes); each pass is a single kernel in which a CTA (a) pulls its 3072-key tile into shared memory with one
 // TMA bulk copy (cp.async.bulk + mbarrier -> SASS UBLKCP), (b) ranks the keys stably with
-// warp-level match_any, (c) obtains the global digit offsets by a per-digit decoupled look-back
+// per-bit warp ballots, (c) obtains the global digit offsets by a per-digit decoupled look-back
 // over the preceding CTAs, and (d) scatters keys and payloads from a block-sorted shared-memory
 // staging area so that global stores go out in runs.  Keys are only as wide as the live bits:
 // ceil(log2 T) tile bits + the bits of int(far*scale); 32-bit keys whenever that is <= 32 bits.
@@ -37,6 +37,20 @@ __device__ __forceinline__ unsigned int ld_u32_volatile(const unsigned int *p) {
 }
 __device__ __forceinline__ void st_u32_volatile(unsigned int *p, unsigned int v) {
     *reinterpret_cast<volatile unsigned int *>(p) = v;
+}
+
+// The lanes of the warp whose v (< 2^(RBITS+1)) equals this lane's: what __match_any_sync(0xffffffff, v) returns, built from
+// one ballot per bit.  MATCH.ANY costs more the more distinct values the warp holds: with it the ranking loop of the later
+// passes, whose keys are no longer grouped by splat, took about three times as long as in the first pass.
+__device__ __forceinline__ unsigned int match_digit(int v) {
+    unsigned int peers = 0xffffffffu;
+#pragma unroll
+    for (int b = 0; b <= RBITS; ++b) {
+        const bool bit = (v >> b) & 1;
+        const unsigned int set = __ballot_sync(0xffffffffu, bit);
+        peers &= bit ? set : ~set;
+    }
+    return peers;
 }
 
 // ------------------------------------------------------------------ live-bit compaction
@@ -97,11 +111,14 @@ __device__ __forceinline__ DigitSel<KeyT> make_digit_sel(int pass, int depth_bit
 // One sweep over the keys builds the digit histograms of every active pass in shared memory; the block that finishes
 // last turns each histogram into its exclusive prefix in place, so a pass kernel reads the global base of digit d
 // directly (hist[pass * 256 + d]) instead of scanning the 256 bins again in each of its CTAs.
+// With `state` set it also zeroes the look-back state the passes will use -- of the active passes only, and of the CTAs that
+// have keys -- a few MB per frame where a memset sized for the key capacity would clear every pass of every CTA.
 template <typename KeyT>
 __global__ void __launch_bounds__(SORT_BLOCK_THREADS)
 sort_histogram_kernel(const KeyT *__restrict__ keys, const long long *__restrict__ n_dev, long long capacity,
                       int depth_bits, int end_bit, const int *__restrict__ max_depth_key,
-                      unsigned int *__restrict__ hist, unsigned int *__restrict__ done_ctr) {
+                      unsigned int *__restrict__ hist, unsigned int *__restrict__ done_ctr,
+                      unsigned int *__restrict__ state = nullptr, long long state_pass_words = 0) {
     __shared__ unsigned int s_hist[8 * RADIX];
     __shared__ unsigned int s_scan[SORT_BLOCK_THREADS / 32];
     __shared__ unsigned int s_last;
@@ -112,6 +129,14 @@ sort_histogram_kernel(const KeyT *__restrict__ keys, const long long *__restrict
     __syncthreads();
     long long n = *n_dev;
     if (n > capacity) n = capacity;
+    if (state) {  // [pass][blk][RADIX]: RADIX words (64 uint4) per CTA, state_pass_words per pass
+        const long long per_pass = (n + SORT_TILE - 1) / SORT_TILE * (RADIX / 4);
+        for (long long k = (long long)blockIdx.x * SORT_BLOCK_THREADS + tid; k < passes * per_pass;
+             k += (long long)gridDim.x * SORT_BLOCK_THREADS) {
+            const long long p = k / per_pass;
+            reinterpret_cast<uint4 *>(state + p * state_pass_words)[k - p * per_pass] = make_uint4(0u, 0u, 0u, 0u);
+        }
+    }
     DigitSel<KeyT> sel[8];
 #pragma unroll
     for (int p = 0; p < 8; ++p) sel[p] = make_digit_sel<KeyT>(p, depth_bits, live);
@@ -231,12 +256,6 @@ onesweep_pass_kernel(const PassParams<KeyT> P) {
     if (P.pass >= npass) return;  // surplus launch: the compacted key has fewer digits
     long long n = *P.n_dev;
     if (n > P.capacity) n = P.capacity;
-    if (tid == 0) s.ticket = atomicAdd(P.tickets + P.pass, 1u);
-    __syncthreads();
-    const unsigned int blk = s.ticket;
-    const long long tile_base = (long long)blk * SORT_TILE;
-    if (tile_base >= n) return;  // the grid is sized for the key CAPACITY: most CTAs of a typical frame leave here
-    const int count = (int)min((long long)SORT_TILE, n - tile_base);
     const DigitSel<KeyT> sel = make_digit_sel<KeyT>(P.pass, P.depth_bits, live);
     const bool to_b = ((npass - 1 - P.pass) & 1) == 0;
     const KeyT *const keys_in = P.pass == 0 ? P.keys_a : (to_b ? P.keys_c : P.keys_b);
@@ -245,141 +264,156 @@ onesweep_pass_kernel(const PassParams<KeyT> P) {
     int *const vals_out = to_b ? P.vals_b : P.vals_c;
     const unsigned int *const hist = P.hist + P.pass * RADIX;
     unsigned int *const state = P.state + (size_t)P.pass * P.blocks * RADIX;
-
     if (tid == 0) mbar_init(&s.mbar, 1);
-    {
-        unsigned int *z = reinterpret_cast<unsigned int *>(&s.warp_cnt[0][0]);
-#pragma unroll
-        for (int i = 0; i < (SORT_BLOCK_THREADS / 32) * RADIX / 2 / SORT_BLOCK_THREADS; ++i) z[i * SORT_BLOCK_THREADS + tid] = 0;
-    }
-    __syncthreads();
+    unsigned int phase = 0;  // parity of the mbarrier phase the next bulk copy completes
 
-    // (a) key tile -> shared memory with one TMA bulk copy (16-byte granules); the < 16-byte tail of a
-    //     partial last tile is fetched with ordinary loads.
-    const unsigned int bulk_bytes = ((unsigned int)count * (unsigned int)sizeof(KeyT)) & ~15u;
-    const int bulk_elems = (int)(bulk_bytes / sizeof(KeyT));
-    if (tid == 0 && bulk_bytes) {
-        mbar_arrive_expect_tx(&s.mbar, bulk_bytes);
-        bulk_copy_g2s(s.keys, keys_in + tile_base, bulk_bytes, &s.mbar);
-    }
-    if (bulk_elems + tid < count) s.keys[bulk_elems + tid] = keys_in[tile_base + bulk_elems + tid];
-    // payloads straight to registers, warp-striped (coalesced)
-    int vals[SORT_ITEMS_PER_THREAD];
-    const int wbase = warp * (32 * SORT_ITEMS_PER_THREAD);
-    {
-        const int *vp = vals_in + tile_base + wbase + lane;
+    // The grid is as large as the GPU holds at once, not one CTA per key tile: a CTA sorts tile after tile in ticket order
+    // until the frame's keys run out, so no CTA launches just to find that the frame has fewer keys than the capacity.
+    // Look-back only waits on smaller tickets, which CTAs that are already running hold.
+    for (;;) {
+        if (tid == 0) s.ticket = atomicAdd(P.tickets + P.pass, 1u);
+        {
+            unsigned int *z = reinterpret_cast<unsigned int *>(&s.warp_cnt[0][0]);
 #pragma unroll
-        for (int j = 0; j < SORT_ITEMS_PER_THREAD; ++j)
-            vals[j] = wbase + j * 32 + lane < count ? __ldg(vp + j * 32) : 0;
-    }
-    if (bulk_bytes) mbar_wait(&s.mbar, 0);
-    __syncthreads();  // tail keys written by other threads
-
-    // (b) stable ranking: per-warp digit counters, match_any groups equal digits in lane order
-    KeyT keys[SORT_ITEMS_PER_THREAD];
-    unsigned short ranks[SORT_ITEMS_PER_THREAD];
-    const unsigned int lt_mask = (1u << lane) - 1u;
-    unsigned short *const my_cnt = s.warp_cnt[warp];
-    // (Writing the twelve MATCH.ANY of a thread as a loop of their own in front of the counter chain changes nothing:
-    //  ptxas re-interleaves the two loops with one MATCH ahead whatever fence is put between them.)
-#pragma unroll
-    for (int j = 0; j < SORT_ITEMS_PER_THREAD; ++j) {
-        const int idx = wbase + j * 32 + lane;
-        const bool valid = idx < count;
-        keys[j] = s.keys[idx];
-        const int d = valid ? digit_of(keys[j], sel) : RADIX;
-        const unsigned int peers = __match_any_sync(0xffffffffu, d);
-        unsigned int prev = 0;
-        if (valid) prev = my_cnt[d];
-        ranks[j] = (unsigned short)(prev + __popc(peers & lt_mask));
-        __syncwarp();
-        if (valid && (peers & lt_mask) == 0) my_cnt[d] = (unsigned short)(prev + __popc(peers));
-        __syncwarp();
-    }
-    __syncthreads();
-
-    // per-digit totals (thread t owns digit t), warp-exclusive bases; publish the aggregate at once
-    unsigned int cnt = 0;
-#pragma unroll
-    for (int w = 0; w < SORT_BLOCK_THREADS / 32; ++w) {
-        const unsigned int x = s.warp_cnt[w][tid];
-        s.warp_cnt[w][tid] = (unsigned short)cnt;
-        cnt += x;
-    }
-    unsigned int *const my_state = state + (size_t)blk * RADIX + tid;
-    st_u32_volatile(my_state, (blk == 0 ? SS_INCLUSIVE : SS_AGGREGATE) | cnt);
-    {   // block-exclusive digit starts
-        unsigned int incl = cnt;
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) {
-            const unsigned int o = __shfl_up_sync(0xffffffffu, incl, d);
-            if (lane >= d) incl += o;
+            for (int i = 0; i < (SORT_BLOCK_THREADS / 32) * RADIX / 2 / SORT_BLOCK_THREADS; ++i) z[i * SORT_BLOCK_THREADS + tid] = 0;
         }
-        if (lane == 31) s.scan_tmp[warp] = incl;
         __syncthreads();
-        unsigned int wprefix = 0;
-#pragma unroll
-        for (int w = 0; w < SORT_BLOCK_THREADS / 32; ++w)
-            if (w < warp) wprefix += s.scan_tmp[w];
-        s.digit_start[tid] = wprefix + incl - cnt;
-    }
-    const unsigned int dglobal = hist[tid];  // exclusive prefix over the digits of the whole array (histogram kernel)
-    __syncthreads();  // digit_start and the warp bases are visible
+        const unsigned int blk = s.ticket;
+        const long long tile_base = (long long)blk * SORT_TILE;
+        if (tile_base >= n) return;
+        const int count = (int)min((long long)SORT_TILE, n - tile_base);
 
-    // block-sorted staging in shared memory (the TMA buffer is dead: all keys are in registers).  This needs
-    // only block-local offsets, so it runs BEFORE the look-back and gives the predecessors time to publish.
-#pragma unroll
-    for (int j = 0; j < SORT_ITEMS_PER_THREAD; ++j) {
-        const int idx = wbase + j * 32 + lane;
-        if (idx < count) {
-            const int d = digit_of(keys[j], sel);
-            const unsigned int pos = s.digit_start[d] + my_cnt[d] + ranks[j];
-            s.keys[pos] = keys[j];
-            s.vals[pos] = vals[j];
+        // (a) key tile -> shared memory with one TMA bulk copy (16-byte granules); the < 16-byte tail of a
+        //     partial last tile is fetched with ordinary loads.
+        const unsigned int bulk_bytes = ((unsigned int)count * (unsigned int)sizeof(KeyT)) & ~15u;
+        const int bulk_elems = (int)(bulk_bytes / sizeof(KeyT));
+        if (tid == 0 && bulk_bytes) {
+            fence_proxy_async_smem();  // the previous tile's reads of s.keys (ordered by the barrier above) come first
+            mbar_arrive_expect_tx(&s.mbar, bulk_bytes);
+            bulk_copy_g2s(s.keys, keys_in + tile_base, bulk_bytes, &s.mbar);
         }
-    }
+        if (bulk_elems + tid < count) s.keys[bulk_elems + tid] = keys_in[tile_base + bulk_elems + tid];
+        // payloads straight to registers, warp-striped (coalesced)
+        int vals[SORT_ITEMS_PER_THREAD];
+        const int wbase = warp * (32 * SORT_ITEMS_PER_THREAD);
+        {
+            const int *vp = vals_in + tile_base + wbase + lane;
+#pragma unroll
+            for (int j = 0; j < SORT_ITEMS_PER_THREAD; ++j)
+                vals[j] = wbase + j * 32 + lane < count ? __ldg(vp + j * 32) : 0;
+        }
+        if (bulk_bytes) {
+            mbar_wait(&s.mbar, phase);
+            phase ^= 1u;
+        }
+        __syncthreads();  // tail keys written by other threads
 
-    // (c) decoupled look-back over the preceding CTAs for this thread's digit, LOOKBACK predecessors in flight per round
-    unsigned int excl = 0;
-    if (blk != 0) {
-        int look = (int)blk - 1;
-        const unsigned int *const col = state + tid;
-        bool done = false;
-        while (!done) {
-            unsigned int w[LOOKBACK];
+        // (b) stable ranking: per-warp digit counters, match_digit groups equal digits in lane order
+        KeyT keys[SORT_ITEMS_PER_THREAD];
+        unsigned short ranks[SORT_ITEMS_PER_THREAD];
+        const unsigned int lt_mask = (1u << lane) - 1u;
+        unsigned short *const my_cnt = s.warp_cnt[warp];
 #pragma unroll
-            for (int r = 0; r < LOOKBACK; ++r)
-                w[r] = (look - r >= 0) ? ld_u32_volatile(col + (size_t)(look - r) * RADIX) : SS_INCLUSIVE;
+        for (int j = 0; j < SORT_ITEMS_PER_THREAD; ++j) {
+            const int idx = wbase + j * 32 + lane;
+            const bool valid = idx < count;
+            keys[j] = s.keys[idx];
+            const int d = valid ? digit_of(keys[j], sel) : RADIX;
+            const unsigned int peers = match_digit(d);
+            unsigned int prev = 0;
+            if (valid) prev = my_cnt[d];
+            ranks[j] = (unsigned short)(prev + __popc(peers & lt_mask));
+            __syncwarp();
+            if (valid && (peers & lt_mask) == 0) my_cnt[d] = (unsigned short)(prev + __popc(peers));
+            __syncwarp();
+        }
+        __syncthreads();
+
+        // per-digit totals (thread t owns digit t), warp-exclusive bases; publish the aggregate at once
+        unsigned int cnt = 0;
 #pragma unroll
-            for (int r = 0; r < LOOKBACK; ++r) {
-                if (done) continue;
-                while ((w[r] >> 30) == 0) w[r] = ld_u32_volatile(col + (size_t)(look - r) * RADIX);
-                excl += w[r] & SS_VALUE_MASK;
-                done = (w[r] >> 30) == 2;
+        for (int w = 0; w < SORT_BLOCK_THREADS / 32; ++w) {
+            const unsigned int x = s.warp_cnt[w][tid];
+            s.warp_cnt[w][tid] = (unsigned short)cnt;
+            cnt += x;
+        }
+        unsigned int *const my_state = state + (size_t)blk * RADIX + tid;
+        st_u32_volatile(my_state, (blk == 0 ? SS_INCLUSIVE : SS_AGGREGATE) | cnt);
+        {   // block-exclusive digit starts
+            unsigned int incl = cnt;
+#pragma unroll
+            for (int d = 1; d < 32; d <<= 1) {
+                const unsigned int o = __shfl_up_sync(0xffffffffu, incl, d);
+                if (lane >= d) incl += o;
             }
-            look -= LOOKBACK;
-        }
-        st_u32_volatile(my_state, SS_INCLUSIVE | (excl + cnt));
-    }
-    s.global_base[tid] = dglobal + excl - s.digit_start[tid];
-    __syncthreads();
-
-    // (d) scatter: consecutive local positions of one digit go to consecutive global addresses
+            if (lane == 31) s.scan_tmp[warp] = incl;
+            __syncthreads();
+            unsigned int wprefix = 0;
 #pragma unroll
-    for (int j = 0; j < SORT_ITEMS_PER_THREAD; ++j) {
-        const int pidx = j * SORT_BLOCK_THREADS + tid;
-        if (pidx < count) {
-            const KeyT k = s.keys[pidx];
-            const unsigned int dst = s.global_base[digit_of(k, sel)] + (unsigned int)pidx;
-            keys_out[dst] = k;
-            vals_out[dst] = s.vals[pidx];
+            for (int w = 0; w < SORT_BLOCK_THREADS / 32; ++w)
+                if (w < warp) wprefix += s.scan_tmp[w];
+            s.digit_start[tid] = wprefix + incl - cnt;
         }
+        const unsigned int dglobal = hist[tid];  // exclusive prefix over the digits of the whole array (histogram kernel)
+        __syncthreads();  // digit_start and the warp bases are visible
+
+        // block-sorted staging in shared memory (the TMA buffer is dead: all keys are in registers).  This needs
+        // only block-local offsets, so it runs BEFORE the look-back and gives the predecessors time to publish.
+#pragma unroll
+        for (int j = 0; j < SORT_ITEMS_PER_THREAD; ++j) {
+            const int idx = wbase + j * 32 + lane;
+            if (idx < count) {
+                const int d = digit_of(keys[j], sel);
+                const unsigned int pos = s.digit_start[d] + my_cnt[d] + ranks[j];
+                s.keys[pos] = keys[j];
+                s.vals[pos] = vals[j];
+            }
+        }
+
+        // (c) decoupled look-back over the preceding CTAs for this thread's digit, LOOKBACK predecessors in flight per round
+        unsigned int excl = 0;
+        if (blk != 0) {
+            int look = (int)blk - 1;
+            const unsigned int *const col = state + tid;
+            bool done = false;
+            while (!done) {
+                unsigned int w[LOOKBACK];
+#pragma unroll
+                for (int r = 0; r < LOOKBACK; ++r)
+                    w[r] = (look - r >= 0) ? ld_u32_volatile(col + (size_t)(look - r) * RADIX) : SS_INCLUSIVE;
+#pragma unroll
+                for (int r = 0; r < LOOKBACK; ++r) {
+                    if (done) continue;
+                    while ((w[r] >> 30) == 0) w[r] = ld_u32_volatile(col + (size_t)(look - r) * RADIX);
+                    excl += w[r] & SS_VALUE_MASK;
+                    done = (w[r] >> 30) == 2;
+                }
+                look -= LOOKBACK;
+            }
+            st_u32_volatile(my_state, SS_INCLUSIVE | (excl + cnt));
+        }
+        s.global_base[tid] = dglobal + excl - s.digit_start[tid];
+        __syncthreads();
+
+        // (d) scatter: consecutive local positions of one digit go to consecutive global addresses
+#pragma unroll
+        for (int j = 0; j < SORT_ITEMS_PER_THREAD; ++j) {
+            const int pidx = j * SORT_BLOCK_THREADS + tid;
+            if (pidx < count) {
+                const KeyT k = s.keys[pidx];
+                const unsigned int dst = s.global_base[digit_of(k, sel)] + (unsigned int)pidx;
+                keys_out[dst] = k;
+                vals_out[dst] = s.vals[pidx];
+            }
+        }
+        __syncthreads();  // shared memory is free for the next tile
     }
 }
 
 #ifndef GSB_HOST_EMU
 // in (never written) / out / tmp are three distinct buffers of `capacity` keys; `tickets` has one word per pass plus one
-// (index 8) for the histogram kernel's completion count; `max_depth_key` may be NULL (no compaction).
+// (index 8) for the histogram kernel's completion count; `max_depth_key` may be NULL (no compaction).  `hist` and `tickets`
+// must be zero; `state` need not be: the histogram kernel clears what the passes use.
 template <typename KeyT>
 static int sort_pairs_typed(const KeyT *keys_in, const int *vals_in, KeyT *keys_out, int *vals_out,
                             const long long *n_dev, int64_t capacity, int depth_bits, int end_bit,
@@ -389,18 +423,23 @@ static int sort_pairs_typed(const KeyT *keys_in, const int *vals_in, KeyT *keys_
     const int blocks = (int)((capacity + SORT_TILE - 1) / SORT_TILE);
     if (blocks == 0 || passes == 0) return GSB_OK;
     const size_t smem = sizeof(PassSmem<KeyT>);
-    static bool attr_set = false;
-    if (!attr_set) {
+    static int resident = 0;  // pass CTAs the whole GPU holds at once
+    if (!resident) {
         GSB_CUDA_CHECK(cudaFuncSetAttribute(onesweep_pass_kernel<KeyT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                             (int)smem));
-        attr_set = true;
+        int per_sm = 0;
+        GSB_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, onesweep_pass_kernel<KeyT>,
+                                                                     SORT_BLOCK_THREADS, smem));
+        resident = (per_sm > 0 ? per_sm : 1) * num_sms();
     }
+    const int pass_blocks = blocks < resident ? blocks : resident;
 #ifndef GSB_HIST_BLOCKS_PER_SM
 #define GSB_HIST_BLOCKS_PER_SM 4
 #endif
     int hist_blocks = blocks < GSB_HIST_BLOCKS_PER_SM * num_sms() ? blocks : GSB_HIST_BLOCKS_PER_SM * num_sms();
     sort_histogram_kernel<KeyT><<<hist_blocks, SORT_BLOCK_THREADS, 0, stream>>>(keys_in, n_dev, capacity, depth_bits, end_bit,
-                                                                                  max_depth_key, hist, tickets + 8);
+                                                                                  max_depth_key, hist, tickets + 8, state,
+                                                                                  (long long)blocks * RADIX);
     GSB_CUDA_CHECK(cudaGetLastError());
     PassParams<KeyT> P;
     P.keys_a = keys_in;
@@ -420,7 +459,7 @@ static int sort_pairs_typed(const KeyT *keys_in, const int *vals_in, KeyT *keys_
     P.tickets = tickets;
     for (int p = 0; p < passes; ++p) {
         P.pass = p;
-        onesweep_pass_kernel<KeyT><<<blocks, SORT_BLOCK_THREADS, smem, stream>>>(P);
+        onesweep_pass_kernel<KeyT><<<pass_blocks, SORT_BLOCK_THREADS, smem, stream>>>(P);
         GSB_CUDA_CHECK(cudaGetLastError());
     }
     return GSB_OK;
