@@ -231,6 +231,16 @@ int gsb200_forward(const GsbForwardArgs *args);
  * GPCR:1167-1182, factor scaling GPCR:1105-1125). */
 int gsb200_backward(const GsbBackwardArgs *args);
 
+/* gsb200_backward for a loss on the image AND the depth map (an extension: the reference's depth output is not
+ * differentiable).  With D = sum w z / S (S = sum w = pixel_accumulated_alpha) the depth gradient flows through alpha into
+ * uv, conic and opacity like a fourth colour channel with "colour" z - D, and directly into xyz along the camera's viewing
+ * axis.  Both pointers NULL: exactly gsb200_backward.  Exactly one NULL: GSB_EINVAL.  Depth without
+ * GSB_FLAG_BACKWARD_TRANSPOSED (the butterfly kernel does not implement it): GSB_EUNSUPPORTED.  These checks come before any
+ * CUDA call.  The accumulator rows carry dL/dz in their last word. */
+int gsb200_backward_with_depth(const GsbBackwardArgs *args,
+                               const float *grad_rasterized_depth, /* (H,W) f32, device */
+                               const float *rasterized_depth);     /* (H,W) f32: this frame's forward output */
+
 int gsb200_expand_view_gradients(const GsbExpandArgs *args);
 
 /* The two collectives of the compact exchange as ONE hand-written kernel over NVSwitch multicast memory (NVLS; csrc/exchange.cu):

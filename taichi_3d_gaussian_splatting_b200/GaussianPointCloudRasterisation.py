@@ -227,6 +227,7 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
         backward_impl: Optional[str] = None,
         skip_unused_hook_statistics: Optional[bool] = None,
         gradient_exchange=None,
+        differentiable_depth: bool = False,
     ):
         """``exact_exp``: blend kernels use ``expf`` instead of ``ex2.approx`` (parity debugging).
         ``force_key64``: sort the reference's 64-bit ``tile << 32 | depth`` keys even when the live
@@ -245,8 +246,19 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
         then returns the gradients SUMMED over the ranks' views -- the per-point kernel writes compact rows, the ranks
         exchange 14 instead of 59 floats per Gaussian and ``gsb200_expand_view_gradients`` rebuilds the dense sum.  A
         backward hook still sees this rank's own view (``grad_pointfeatures_in_camera`` is ``None`` in this mode: the
-        per-view dense feature gradients are never formed)."""
+        per-view dense feature gradients are never formed).
+        ``differentiable_depth``: make the returned depth map differentiable (an extension: the reference's depth output is
+        not, and by default neither is ours).  A loss on depth then trains xyz, q, s and the opacity through the blend
+        weights, and xyz also through each splat's camera-space depth (``gsb200_backward_with_depth``); a loss on depth
+        alone works too.  The hook sees the sum of both losses' shares in ``grad_point_in_camera``, ``grad_viewspace``
+        and the magnitudes, exactly as it sees the image loss's share.  Needs the transposed backward and the auxiliary
+        outputs: ``ValueError`` with ``backward_impl="butterfly"`` or ``config.rgb_only``."""
         super().__init__()
+        if differentiable_depth and backward_impl == "butterfly":
+            raise ValueError("differentiable_depth needs backward_impl='transposed': the butterfly kernel has no depth gradient")
+        if differentiable_depth and config.rgb_only:
+            raise ValueError("differentiable_depth needs the depth map: config.rgb_only=True renders none")
+        self.differentiable_depth = bool(differentiable_depth)
         self.config = config
         self.backward_valid_point_hook = backward_valid_point_hook
         self._flags = (_lib.GSB_FLAG_EXACT_EXP if exact_exp else 0) | (_lib.GSB_FLAG_FORCE_KEY64 if force_key64 else 0) | \
@@ -277,11 +289,15 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                 image, depth, acc_alpha, last_effective, valid_count = outs
                 ctx.save_for_backward(pointcloud, pointcloud_features, point_object_id,
                                       t_pointcloud_camera, saved["camera_intrinsics"], acc_alpha,
-                                      last_effective, frame.ws)
+                                      last_effective, frame.ws, *((depth,) if outer.differentiable_depth else ()))
                 ctx.frame = frame
                 ctx.num_objects = q_pointcloud_camera.shape[0]
                 ctx.color_max_sh_band = color_max_sh_band
-                ctx.mark_non_differentiable(depth, valid_count)
+                if outer.differentiable_depth:
+                    ctx.mark_non_differentiable(valid_count)
+                    ctx.set_materialize_grads(False)  # None tells an unused depth (or image) from a zero gradient
+                else:
+                    ctx.mark_non_differentiable(depth, valid_count)
                 return image, depth, valid_count
 
             @staticmethod
@@ -293,7 +309,12 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                         # this mode (GPCR:478-484), so its backward is undefined; refuse instead
                         raise RuntimeError("rgb_only=True is an inference-only mode: backward needs the "
                                            "auxiliary per-pixel outputs")
-                    grad_pointcloud, grad_pointcloud_features = outer._run_backward(ctx, grad_rasterized_image)
+                    if grad_rasterized_image is None:  # differentiable_depth: a loss on the depth map alone
+                        frame = ctx.frame
+                        grad_rasterized_image = torch.zeros((frame.height, frame.width, 3), dtype=torch.float32,
+                                                            device=frame.ws.device)
+                    grad_pointcloud, grad_pointcloud_features = outer._run_backward(ctx, grad_rasterized_image,
+                                                                                    grad_rasterized_depth)
                 return grad_pointcloud, grad_pointcloud_features, None, None, None, None, None, None
 
         self._module_function = _module_function
@@ -394,11 +415,14 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
         return (image, depth, acc_alpha, last_effective, valid_count), frame, {"camera_intrinsics": K}
 
     # ------------------------------------------------------------------ backward plumbing
-    def _run_backward(self, ctx, grad_rasterized_image):
+    def _run_backward(self, ctx, grad_rasterized_image, grad_rasterized_depth=None):
         cfg = self.config
         lib = _lib.load()
+        saved = ctx.saved_tensors
         (pointcloud, pointcloud_features, point_object_id, t_pointcloud_camera, K, acc_alpha,
-         last_effective, ws) = ctx.saved_tensors
+         last_effective, ws) = saved[:8]
+        # differentiable_depth: the depth gradient (None when the loss does not use depth) and the forward's depth map
+        depth = saved[8] if self.differentiable_depth and grad_rasterized_depth is not None else None
         frame: Frame = ctx.frame
         device = pointcloud.device
         N = pointcloud.shape[0]
@@ -447,7 +471,14 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                 grad_pointcloud_features=_ptr(grad_pointcloud_features),
                 magnitude_grad_viewspace_on_image=_ptr(magnitude_on_image), stream=stream.cuda_stream,
                 grad_sum_compact=_ptr(grad_sum), grad_color_compact=_ptr(blocks[exchange.rank]) if compact else None)
-            _lib.check(lib.gsb200_backward(ctypes.byref(args)), "gsb200_backward")
+            if depth is None:
+                _lib.check(lib.gsb200_backward(ctypes.byref(args)), "gsb200_backward")
+            else:
+                grad_depth = grad_rasterized_depth.contiguous()
+                if grad_depth.dtype != torch.float32:
+                    grad_depth = grad_depth.float()
+                _lib.check(lib.gsb200_backward_with_depth(ctypes.byref(args), _ptr(grad_depth), _ptr(depth)),
+                           "gsb200_backward_with_depth")
             own_view_grad_xyz = None
             if compact:
                 exchange.rows_written(grad_sum, blocks)

@@ -249,7 +249,9 @@ int gsb200_forward(const GsbForwardArgs *a) {
     return launch_blend_forward(*a, ws, st);
 }
 
-static int backward_impl(const GsbBackwardArgs *a, bool skip_on_overflow) {
+// grad_depth / depth: both NULL (the image gradient alone), or both set (gsb200_backward_with_depth, checked there)
+static int backward_impl(const GsbBackwardArgs *a, bool skip_on_overflow, const float *grad_depth = nullptr,
+                         const float *depth = nullptr) {
     if (!a) {
         set_error("backward: args is null");
         return GSB_EINVAL;
@@ -296,11 +298,24 @@ static int backward_impl(const GsbBackwardArgs *a, bool skip_on_overflow) {
     cudaStream_t st = static_cast<cudaStream_t>(a->stream);
     if (a->accum_rows > 0)
         GSB_CUDA_CHECK(cudaMemsetAsync(a->accum, 0, (size_t)a->accum_rows * GSB_ACCUM_FLOATS * 4, st));
-    if ((rc = launch_blend_backward(*a, ws, st)) != GSB_OK) return rc;
-    return launch_backward_points(*a, ws, st, skip_on_overflow ? ws.counters + CNT_OVERFLOW : nullptr);
+    if ((rc = launch_blend_backward(*a, ws, st, grad_depth, depth)) != GSB_OK) return rc;
+    return launch_backward_points(*a, ws, st, skip_on_overflow ? ws.counters + CNT_OVERFLOW : nullptr, grad_depth != nullptr);
 }
 
 int gsb200_backward(const GsbBackwardArgs *a) { return backward_impl(a, false); }
+
+int gsb200_backward_with_depth(const GsbBackwardArgs *a, const float *grad_rasterized_depth, const float *rasterized_depth) {
+    if ((grad_rasterized_depth == nullptr) != (rasterized_depth == nullptr)) {
+        set_error("backward_with_depth: grad_rasterized_depth and rasterized_depth must be both NULL or both set");
+        return GSB_EINVAL;
+    }
+    if (grad_rasterized_depth != nullptr && a != nullptr && !(a->flags & GSB_FLAG_BACKWARD_TRANSPOSED)) {
+        set_error("backward_with_depth: the depth gradient needs the transposed backward kernel "
+                  "(GSB_FLAG_BACKWARD_TRANSPOSED); the butterfly kernel does not implement it");
+        return GSB_EUNSUPPORTED;
+    }
+    return backward_impl(a, false, grad_rasterized_depth, rasterized_depth);
+}
 
 int gsb200_image_loss(const float *rasterized_image, const float *ground_truth_image, int32_t camera_height,
                       int32_t camera_width, float lambda_value, float upstream_grad, float *loss_out3,

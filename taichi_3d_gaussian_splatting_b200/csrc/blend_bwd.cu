@@ -276,10 +276,13 @@ static BlendBwdParams make_blend_bwd_params(const GsbBackwardArgs &a, const Work
     p.accum = a.accum;
     p.mag_image = a.magnitude_grad_viewspace_on_image;
     p.work_counters = nullptr;
+    p.grad_depth = nullptr;
+    p.depth = nullptr;
     return p;
 }
 
-int launch_blend_backward(const GsbBackwardArgs &a, const Workspace &ws, cudaStream_t stream) {
+int launch_blend_backward(const GsbBackwardArgs &a, const Workspace &ws, cudaStream_t stream, const float *grad_depth,
+                          const float *depth) {
     BlendBwdParams p;
     p.H = a.camera_height;
     p.W = a.camera_width;
@@ -294,11 +297,13 @@ int launch_blend_backward(const GsbBackwardArgs &a, const Workspace &ws, cudaStr
     p.accum = a.accum;
     p.mag_image = a.magnitude_grad_viewspace_on_image;
     p.work_counters = nullptr;
+    p.grad_depth = grad_depth;
+    p.depth = depth;
     const int tiles = p.tiles_x * (a.camera_height / GSB_TILE_HEIGHT);
     if (tiles <= 0) return GSB_OK;
     if (a.flags & GSB_FLAG_BACKWARD_TRANSPOSED)  // experimental, see blend_bwd_transposed.cu
         return launch_blend_backward_transposed(p, tiles, (a.flags & GSB_FLAG_EXACT_EXP) != 0,
-                                                (a.flags & GSB_FLAG_NO_HOOK_STATS) == 0, stream);
+                                                (a.flags & GSB_FLAG_NO_HOOK_STATS) == 0, stream, grad_depth != nullptr);
     const bool exact = (a.flags & GSB_FLAG_EXACT_EXP) != 0;
     if (a.flags & GSB_FLAG_NO_HOOK_STATS) {  // opt-in
         if (exact) blend_backward_kernel<true, false><<<tiles, GSB_TILE_PIXELS, 0, stream>>>(p);
@@ -375,7 +380,10 @@ constexpr int PT_ROW_COMPACT = 20;  // COMPACT: 16 staged floats per row, same b
 // applied -- and the 3 colour-argument gradients that must stay per view: the 48 SH gradients of a view are their outer product
 // with the view's SH basis, which gsb200_expand_view_gradients rebuilds AFTER the exchange (14 instead of 59 floats per row
 // cross NVLink, and this kernel writes 60 instead of 236 bytes per row).
-template <bool COMPACT>
+// DEPTH = true (gsb200_backward_with_depth): word 11 of the accumulator row is dL/dz of the point's camera-space depth
+// (blend_bwd_transposed.cu), and z = W[2,:] xyz + t adds it to dL/dxyz along the third row of W -- before gx feeds the
+// dense gradient, the controller epilogue or the compact row.
+template <bool COMPACT, bool DEPTH = false>
 __global__ void __launch_bounds__(GSB_POINTS_THREADS, 6)  // 6 x 33 KB of staging per SM
 backward_points_kernel(const PointsBwdParams p) {
     // One thread per scene row: rows outside the frustum get their zeros here (no separate memset of the
@@ -426,6 +434,7 @@ backward_points_kernel(const PointsBwdParams p) {
             const float d0 = dj[0] * Wm[c] + dj[1] * Wm[3 + c] + dj[2] * Wm[6 + c];
             const float d1 = dj[3] * Wm[c] + dj[4] * Wm[3 + c] + dj[5] * Wm[6 + c];
             gx[c] = a0.x * d0 + a0.y * d1;
+            if (DEPTH) gx[c] += a2.w * Wm[6 + c];
         }
         // Sigma' = U Sigma U^T, U = J W with J from fx, fy only (GP3D:65-87, 237-331)
         const float fx = Kc[0], fy = Kc[4];
@@ -659,7 +668,8 @@ expand_view_gradients_kernel(const ExpandParams p) {
 #ifndef GSB_HOST_EMU
 static int first_cleared_of_band(int band) { return band <= 0 ? 1 : band == 1 ? 4 : band == 2 ? 9 : 16; }
 
-int launch_backward_points(const GsbBackwardArgs &a, const Workspace &ws, cudaStream_t stream, const long long *skip_flag) {
+int launch_backward_points(const GsbBackwardArgs &a, const Workspace &ws, cudaStream_t stream, const long long *skip_flag,
+                           bool depth_grad) {
     if (a.num_points <= 0) return GSB_OK;
     PointsBwdParams p;
     p.ctl_num_in_camera = a.ctl_accumulated_num_in_camera;
@@ -694,8 +704,15 @@ int launch_backward_points(const GsbBackwardArgs &a, const Workspace &ws, cudaSt
     const long long cap = 16LL * num_sms();
     if (blocks > cap) blocks = cap;
     if (blocks <= 0) return GSB_OK;
-    if (a.flags & GSB_FLAG_COMPACT_GRADS) backward_points_kernel<true><<<(int)blocks, GSB_POINTS_THREADS, 0, stream>>>(p);
-    else backward_points_kernel<false><<<(int)blocks, GSB_POINTS_THREADS, 0, stream>>>(p);
+    const bool compact = (a.flags & GSB_FLAG_COMPACT_GRADS) != 0;
+    if (depth_grad) {
+        if (compact) backward_points_kernel<true, true><<<(int)blocks, GSB_POINTS_THREADS, 0, stream>>>(p);
+        else backward_points_kernel<false, true><<<(int)blocks, GSB_POINTS_THREADS, 0, stream>>>(p);
+    } else if (compact) {
+        backward_points_kernel<true><<<(int)blocks, GSB_POINTS_THREADS, 0, stream>>>(p);
+    } else {
+        backward_points_kernel<false><<<(int)blocks, GSB_POINTS_THREADS, 0, stream>>>(p);
+    }
     GSB_CUDA_CHECK(cudaGetLastError());
     return GSB_OK;
 }

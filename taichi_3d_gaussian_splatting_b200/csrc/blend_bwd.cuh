@@ -17,6 +17,8 @@ struct BlendBwdParams {
     float *accum;      // rows of 12 floats
     float *mag_image;  // (H,W,2)
     unsigned long long *work_counters;  // COUNT instantiation only: [0] (warp, splat) visits, [1] contributing (pixel, splat) pairs
+    const float *grad_depth;  // DEPTH instantiation only: (H,W) dL/d depth and the forward's depth output; NULL otherwise
+    const float *depth;
 };
 
 #ifdef GSB_HOST_EMU  // tests/simt: the kernels compiled as host C++ under a lock-step SIMT emulator
@@ -42,7 +44,7 @@ __device__ __forceinline__ float sqrt_approx(float x) {  // MUFU.RSQ based, ~1 u
 #endif
 
 int launch_blend_backward_transposed(const BlendBwdParams &p, int tiles, bool exact_exp, bool stats,
-                                     cudaStream_t stream);
+                                     cudaStream_t stream, bool depth = false);
 int launch_blend_backward_count(const BlendBwdParams &p, int tiles, cudaStream_t stream);
 
 }  // namespace gsb

@@ -16,6 +16,13 @@
 //     memory as 16-byte vector REDs, 3 per row (same 2 sectors per (warp, splat) as the butterfly kernel).
 // STATS = false (GSB_FLAG_NO_HOOK_STATS, the reference's need_extra_info = False, GPCR:521, 690-704) drops the |d/duv|
 // magnitude, the affected-pixel count and the per-pixel magnitude image.
+// DEPTH = true (gsb200_backward_with_depth; the reference never differentiates its depth output) adds the gradient of the
+// depth map D = sum w z / S (S = sum w = the accumulated alpha).  With g^ = dL/dD / S per pixel:
+//   through alpha: D behaves like a colour channel whose "colour" is z - D, weighted by g^ -- phase 1 folds it into the
+//     colour recursion (fast path: cg += g^ z - g^ D; exact path: a fourth accumulator w3 = sum (z - D) alpha T);
+//   direct:        dD/dz_i = alpha_i T_i / S -- phase 2 sums alpha T g^ per splat into the spare word 11 of the
+//     accumulator row (g^ rides in the unused .w of the warp's dL/dimage copy), which backward_points_kernel<_, true>
+//     turns into dL/dxyz along the camera's viewing axis.
 #include "blend_bwd.cuh"
 
 namespace gsb {
@@ -107,9 +114,10 @@ __device__ __forceinline__ float keep_if_contributing(float P, int idx, int last
 #endif
 }
 
-template <bool EXACT_EXP, bool STATS, bool COUNT = false>
+template <bool EXACT_EXP, bool STATS, bool COUNT = false, bool DEPTH = false>
 __global__ void __launch_bounds__(GSB_TILE_PIXELS, GSB_TB_MIN_BLOCKS)
 blend_backward_transposed_kernel(const BlendBwdParams p) {
+    static_assert(!(COUNT && DEPTH), "the work-counter diagnostic runs the default arithmetic only");
     TbShared &S = *reinterpret_cast<TbShared *>(tb_dynamic_smem());
     constexpr int NV = STATS ? 11 : 9;
 
@@ -128,8 +136,17 @@ blend_backward_transposed_kernel(const BlendBwdParams p) {
     const float g0 = p.grad_image[3 * pix], g1 = p.grad_image[3 * pix + 1], g2 = p.grad_image[3 * pix + 2];
     float mag0 = 0.0f, mag1 = 0.0f;
     unsigned int n_visits = 0, n_pairs = 0;  // COUNT only
+    // DEPTH only: gd = dL/dD / S (0 where nothing is blended: S = 0 exactly, and then no pair contributes either); hd = gd D
+    // on the fast path, D on the exact one.  S >= 1/255 wherever a splat is blended, so the forward's 1e-6 clamp of S
+    // never applies to a pixel with something to differentiate.
+    float gd = 0.0f, hd = 0.0f, w3 = 0.0f;
+    if (DEPTH) {
+        const float Sa = p.acc_alpha[pix];
+        gd = Sa > 0.0f ? p.grad_depth[pix] / Sa : 0.0f;
+        hd = EXACT_EXP ? p.depth[pix] : gd * p.depth[pix];
+    }
     TbWarp &Wp = S.w[warp];
-    Wp.g[lane] = make_float4(g0, g1, g2, 0.0f);
+    Wp.g[lane] = make_float4(g0, g1, g2, gd);
 
     // phase-2 role of this lane: splat `ci` of the chunk, rows row0 .. row0 + TB_ROWS - 1 of the patch
     const int ci = lane % TB_CHUNK, row0 = (lane / TB_CHUNK) * TB_ROWS;
@@ -254,9 +271,14 @@ blend_backward_transposed_kernel(const BlendBwdParams p) {
                         const float inv = 1.0f / (1.0f - alpha);
                         const float Tn = T * inv;
                         aT = contributes ? alpha * Tn : 0.0f;
-                        const float a_grad = contributes ? (r2.x * Tn - w0 * inv) * g0 + (r2.y * Tn - w1 * inv) * g1 +
-                                                               (r2.z * Tn - w2 * inv) * g2
-                                                         : 0.0f;
+                        float a_grad = contributes ? (r2.x * Tn - w0 * inv) * g0 + (r2.y * Tn - w1 * inv) * g1 +
+                                                         (r2.z * Tn - w2 * inv) * g2
+                                                   : 0.0f;
+                        if (DEPTH) {  // the depth map's "colour" z - D
+                            const float e = r1.w - hd;
+                            a_grad += contributes ? (e * Tn - w3 * inv) * gd : 0.0f;
+                            w3 = fmaf(e, aT, w3);
+                        }
                         T = contributes ? Tn : T;
                         w0 = fmaf(r2.x, aT, w0);
                         w1 = fmaf(r2.y, aT, w1);
@@ -277,7 +299,8 @@ blend_backward_transposed_kernel(const BlendBwdParams p) {
                         const float inv = rcp_approx(1.0f - alpha);
                         T *= inv;                 // T_i = T_{i+1} / (1 - alpha), GPCR:640
                         aT = alpha * T;
-                        const float cg = fmaf(r2.z, g2, fmaf(r2.y, g1, r2.x * g0));
+                        float cg = fmaf(r2.z, g2, fmaf(r2.y, g1, r2.x * g0));
+                        if (DEPTH) cg = fmaf(gd, r1.w, cg) - hd;  // + gd (z - D): the depth map as a fourth channel
                         const float a_grad = fmaf(cg, T, -(w0 * inv));
                         w0 = fmaf(cg, aT, w0);
                         G = a_grad * P;
@@ -325,9 +348,9 @@ blend_backward_transposed_kernel(const BlendBwdParams p) {
                 const float pxc = org.x + (float)((warp & 1) * 8) + 4.0f;
                 const float pyb = org.y + (float)((warp >> 1) * 4 + row0) + 0.5f;
                 const float dxc = pxc - s0.x;  // d0 at the centre of the row
-                float acc[11];
+                float acc[12];  // the accumulator row; word 11 only with DEPTH
 #pragma unroll
-                for (int k = 0; k < 11; ++k) acc[k] = 0.0f;
+                for (int k = 0; k < 12; ++k) acc[k] = 0.0f;
                 unsigned int nz = 0u;
 #pragma unroll
                 for (int row = 0; row < TB_ROWS; ++row) {
@@ -349,6 +372,7 @@ blend_backward_transposed_kernel(const BlendBwdParams p) {
                         acc[5] = fmaf(ga.y, gp.x, acc[5]);
                         acc[6] = fmaf(ga.y, gp.y, acc[6]);
                         acc[7] = fmaf(ga.y, gp.z, acc[7]);
+                        if (DEPTH) acc[11] = fmaf(ga.y, gp.w, acc[11]);  // sum alpha T gd: dL/dz of the splat
                         if (STATS) {
                             const float vs0 = ga.x * fmaf(ca, kc, q0r), vs1 = ga.x * fmaf(cb, kc, q1r);
                             const float mm = vs0 * vs0 + vs1 * vs1;
@@ -372,6 +396,7 @@ blend_backward_transposed_kernel(const BlendBwdParams p) {
                 for (int d = TB_CHUNK; d < 32; d *= 2) {
 #pragma unroll
                     for (int k = 0; k < NV; ++k) acc[k] += __shfl_xor_sync(0xffffffffu, acc[k], d);
+                    if (DEPTH) acc[11] += __shfl_xor_sync(0xffffffffu, acc[11], d);
                     nz |= __shfl_xor_sync(0xffffffffu, nz, d);
                 }
                 acc[8] *= EXACT_EXP ? (1.0f - s1.z) : s1.z;  // d alpha / d logit = alpha (1 - opacity)
@@ -379,11 +404,12 @@ blend_backward_transposed_kernel(const BlendBwdParams p) {
                 if (lane < TB_CHUNK) {
                     if (!(active && nz != 0u)) ck_off[ci] = -1;
                     else GSB_EMU_COUNT(EC_TB_ROWS, 1);
-                    // the whole 12-word row (words NV..11 are zero): 48 B apart, so the 8 lanes of a quarter-warp cover
-                    // the 32 banks once per float4
+                    // the whole 12-word row (words NV..10 are zero, and 11 without DEPTH): 48 B apart, so the 8 lanes of a
+                    // quarter-warp cover the 32 banks once per float4
                     fin[3 * ci] = make_float4(acc[0], acc[1], acc[2], acc[3]);
                     fin[3 * ci + 1] = make_float4(acc[4], acc[5], acc[6], acc[7]);
-                    fin[3 * ci + 2] = make_float4(acc[8], STATS ? acc[9] : 0.0f, STATS ? acc[10] : 0.0f, 0.0f);
+                    fin[3 * ci + 2] = make_float4(acc[8], STATS ? acc[9] : 0.0f, STATS ? acc[10] : 0.0f,
+                                                  DEPTH ? acc[11] : 0.0f);
                 }
                 __syncwarp();
                 // float4 e of the chunk's finished rows goes to word 4 (e % 3) of row e / 3: the same 2 sectors per row
@@ -419,21 +445,27 @@ blend_backward_transposed_kernel(const BlendBwdParams p) {
 }
 
 #ifndef GSB_HOST_EMU
-template <bool EXACT_EXP, bool STATS>
+template <bool EXACT_EXP, bool STATS, bool DEPTH = false>
 static int launch_tb(const BlendBwdParams &p, int tiles, cudaStream_t stream) {
     static bool configured = false;  // one device per process (one process per GPU)
     if (!configured) {
-        GSB_CUDA_CHECK(cudaFuncSetAttribute(blend_backward_transposed_kernel<EXACT_EXP, STATS>,
+        GSB_CUDA_CHECK(cudaFuncSetAttribute(blend_backward_transposed_kernel<EXACT_EXP, STATS, false, DEPTH>,
                                             cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TbShared)));
         configured = true;
     }
-    blend_backward_transposed_kernel<EXACT_EXP, STATS><<<tiles, GSB_TILE_PIXELS, sizeof(TbShared), stream>>>(p);
+    blend_backward_transposed_kernel<EXACT_EXP, STATS, false, DEPTH><<<tiles, GSB_TILE_PIXELS, sizeof(TbShared), stream>>>(p);
     GSB_CUDA_CHECK(cudaGetLastError());
     return GSB_OK;
 }
 
+// depth = true: p.grad_depth and p.depth must be set (the DEPTH instantiations)
 int launch_blend_backward_transposed(const BlendBwdParams &p, int tiles, bool exact_exp, bool stats,
-                                     cudaStream_t stream) {
+                                     cudaStream_t stream, bool depth) {
+    if (depth) {
+        if (exact_exp)
+            return stats ? launch_tb<true, true, true>(p, tiles, stream) : launch_tb<true, false, true>(p, tiles, stream);
+        return stats ? launch_tb<false, true, true>(p, tiles, stream) : launch_tb<false, false, true>(p, tiles, stream);
+    }
     if (exact_exp) return stats ? launch_tb<true, true>(p, tiles, stream) : launch_tb<true, false>(p, tiles, stream);
     return stats ? launch_tb<false, true>(p, tiles, stream) : launch_tb<false, false>(p, tiles, stream);
 }
