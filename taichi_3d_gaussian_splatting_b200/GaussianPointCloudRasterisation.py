@@ -576,8 +576,6 @@ def find_tile_start_and_end(point_in_camera_sort_key: torch.Tensor, tile_points_
     _require(tile_points_start, "tile_points_start", torch.int32)
     _require(tile_points_end, "tile_points_end", torch.int32)
     fn = lib.gsb200_find_tile_start_and_end
-    fn.argtypes = [_lib.c_vp, _lib.c_i64, _lib.c_vp, _lib.c_vp, _lib.c_i32, _lib.c_vp]
-    fn.restype = ctypes.c_int
     with torch.cuda.device(point_in_camera_sort_key.device):
         stream = torch.cuda.current_stream(point_in_camera_sort_key.device)
         keys = point_in_camera_sort_key.contiguous()

@@ -159,6 +159,20 @@ def load() -> ctypes.CDLL:
     lib.gsb200_train_step.restype = ctypes.c_int
     lib.gsb200_device_selftest.argtypes = [c_vp]
     lib.gsb200_device_selftest.restype = ctypes.c_int
+    # Every export gets its signature here: without argtypes ctypes passes a Python int as a 32-bit C int, which silently
+    # truncates device pointers and 64-bit sizes.
+    lib.gsb200_find_tile_start_and_end.argtypes = [c_vp, c_i64, c_vp, c_vp, c_i32, c_vp]
+    lib.gsb200_find_tile_start_and_end.restype = ctypes.c_int
+    lib.gsb200_forward_timed.argtypes = [ctypes.POINTER(GsbForwardArgs), ctypes.POINTER(c_f32)]
+    lib.gsb200_forward_timed.restype = ctypes.c_int
+    lib.gsb200_backward_timed.argtypes = [ctypes.POINTER(GsbBackwardArgs), ctypes.POINTER(c_f32)]
+    lib.gsb200_backward_timed.restype = ctypes.c_int
+    lib.gsb200_version.argtypes = []
+    lib.gsb200_last_error.argtypes = []
+    lib.gsb200_abi_sizes.argtypes = [ctypes.POINTER(c_i64)]
+    lib.gsb200_abi_sizes.restype = None
+    lib.gsb200_abi_sizes_ext.argtypes = [ctypes.POINTER(c_i64), c_i32]
+    lib.gsb200_abi_sizes_ext.restype = None
     sizes = (c_i64 * 3)()
     lib.gsb200_abi_sizes(sizes)
     mine = (ctypes.sizeof(GsbWorkspaceLayout), ctypes.sizeof(GsbForwardArgs), ctypes.sizeof(GsbBackwardArgs))
