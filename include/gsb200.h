@@ -236,10 +236,22 @@ int gsb200_backward(const GsbBackwardArgs *args);
  * uv, conic and opacity like a fourth colour channel with "colour" z - D, and directly into xyz along the camera's viewing
  * axis.  Both pointers NULL: exactly gsb200_backward.  Exactly one NULL: GSB_EINVAL.  Depth without
  * GSB_FLAG_BACKWARD_TRANSPOSED (the butterfly kernel does not implement it): GSB_EUNSUPPORTED.  These checks come before any
- * CUDA call.  The accumulator rows carry dL/dz in their last word. */
+ * CUDA call.  The accumulator rows carry dL/dz in their last word.  Same as gsb200_backward_aux(args, grad, depth, NULL). */
 int gsb200_backward_with_depth(const GsbBackwardArgs *args,
                                const float *grad_rasterized_depth, /* (H,W) f32, device */
                                const float *rasterized_depth);     /* (H,W) f32: this frame's forward output */
+
+/* gsb200_backward for a loss on the image and any of the other per-pixel float outputs (an extension: the reference
+ * differentiates the image alone).  The depth pair follows gsb200_backward_with_depth.  grad_pixel_accumulated_alpha is
+ * dL/dS for S = pixel_accumulated_alpha = 1 - prod (1 - alpha): S is the blend of a colour channel whose colour is 1
+ * (dS/dalpha_i = T_final / (1 - alpha_i)), so its gradient flows through alpha into uv, conic and opacity; NULL means no
+ * alpha term.  All three NULL: exactly gsb200_backward.  Depth pair with exactly one NULL: GSB_EINVAL.  Any term without
+ * GSB_FLAG_BACKWARD_TRANSPOSED (the butterfly kernel implements neither): GSB_EUNSUPPORTED.  These checks come before any
+ * CUDA call. */
+int gsb200_backward_aux(const GsbBackwardArgs *args,
+                        const float *grad_rasterized_depth,         /* (H,W) f32, device, or NULL */
+                        const float *rasterized_depth,              /* (H,W) f32: this frame's forward output, or NULL */
+                        const float *grad_pixel_accumulated_alpha); /* (H,W) f32, device, or NULL */
 
 int gsb200_expand_view_gradients(const GsbExpandArgs *args);
 

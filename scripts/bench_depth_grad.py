@@ -1,14 +1,19 @@
-"""Cost of the depth-map gradient (``differentiable_depth=True``) at a bench configuration (default C3).
+"""Cost of the depth-map and accumulated-alpha gradients (``differentiable_depth=True``, ``differentiable_alpha=True``) at a
+bench configuration (default C3).
 
-One forward of the scene in depth mode, then the backward is timed repeatedly (``torch.autograd.grad`` with
-``retain_graph``: no gradient accumulation kernels) in two variants that alternate within the process:
+One forward of the scene, then the backward is timed repeatedly (``torch.autograd.grad`` with ``retain_graph``: no
+gradient accumulation kernels) in variants that alternate within the process.  ``--mode depth`` (the default):
   image: dL/dimage only -> gsb200_backward, the default kernels;
   depth: dL/dimage and dL/ddepth -> gsb200_backward_with_depth, the DEPTH instantiations.
-Each of --regions regions runs --steps timed steps of both variants (CUDA events around each backward call; the order of
-the two flips every region), after --warmup untimed ones.  A torch.profiler pass then reports the device time per kernel.
-Prints the card name and power limit read in the same run, medians and p90 in ms, as one JSON object.
+``--mode alpha``:
+  image, depth: as above;
+  alpha: dL/dimage and dL/dalpha -> gsb200_backward_aux, the ALPHA instantiations;
+  depth+alpha: dL/dimage, dL/ddepth and dL/dalpha -> gsb200_backward_aux, the DEPTH + ALPHA instantiations.
+Each of --regions regions runs --steps timed steps of every variant (CUDA events around each backward call; the order of
+the variants reverses every region), after --warmup untimed ones.  A torch.profiler pass then reports the device time per
+kernel.  Prints the card name and power limit read in the same run, medians and p90 in ms, as one JSON object.
 
-    python scripts/bench_depth_grad.py [C3] [--regions 5] [--steps 20] [--warmup 3]
+    python scripts/bench_depth_grad.py [C3] [--mode depth|alpha] [--regions 5] [--steps 20] [--warmup 3]
 """
 import argparse
 import json
@@ -38,6 +43,7 @@ def card():
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("config", nargs="?", default="C3")
+    ap.add_argument("--mode", choices=("depth", "alpha"), default="depth")
     ap.add_argument("--regions", type=int, default=5)
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=3)
@@ -46,8 +52,9 @@ def main():
     scene = make_scene(**cfg).to("cuda")
     scene.point_cloud.requires_grad_(True)
     scene.point_cloud_features.requires_grad_(True)
-    op = GPCR(GPCR.GaussianPointCloudRasterisationConfig(), differentiable_depth=True)
-    image, depth, _ = op(GPCR.GaussianPointCloudRasterisationInput(
+    alpha_mode = args.mode == "alpha"
+    op = GPCR(GPCR.GaussianPointCloudRasterisationConfig(), differentiable_depth=True, differentiable_alpha=alpha_mode)
+    image, depth, *rest = op(GPCR.GaussianPointCloudRasterisationInput(
         point_cloud=scene.point_cloud, point_cloud_features=scene.point_cloud_features,
         point_object_id=scene.point_object_id, point_invalid_mask=scene.point_invalid_mask,
         camera_info=scene.camera_info, q_pointcloud_camera=scene.q_pointcloud_camera,
@@ -60,6 +67,12 @@ def main():
         "image": lambda: torch.autograd.grad([image], inputs, [g_img], retain_graph=True),
         "depth": lambda: torch.autograd.grad([image, depth], inputs, [g_img, g_dep], retain_graph=True),
     }
+    if alpha_mode:
+        alpha = rest[1]
+        g_alp = torch.randn(alpha.shape, generator=gen).cuda()
+        variants["alpha"] = lambda: torch.autograd.grad([image, alpha], inputs, [g_img, g_alp], retain_graph=True)
+        variants["depth+alpha"] = lambda: torch.autograd.grad([image, depth, alpha], inputs, [g_img, g_dep, g_alp],
+                                                              retain_graph=True)
     times = {k: [] for k in variants}
     start, stop = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     for region in range(args.regions):
@@ -88,14 +101,15 @@ def main():
                 per[e.key.split("(")[0][:120]] = round(t / 1e3 / args.steps, 4)  # ms per step
         kernels[k] = per
     name, power = card()
-    res = {"config": args.config, "card": name, "power_limit": power, "regions": args.regions, "steps": args.steps,
-           "M": op.last_frame.num_points_in_camera, "K": op.last_frame.num_keys}
+    res = {"config": args.config, "mode": args.mode, "card": name, "power_limit": power, "regions": args.regions,
+           "steps": args.steps, "M": op.last_frame.num_points_in_camera, "K": op.last_frame.num_keys}
     for k, v in times.items():
         a = np.asarray(v)
         res[k] = {"median_ms": round(float(np.median(a)), 4), "p90_ms": round(float(np.percentile(a, 90)), 4),
                   "region_medians_ms": [round(float(np.median(a[i * args.steps:(i + 1) * args.steps])), 4)
                                         for i in range(args.regions)]}
-    res["depth_over_image"] = round(res["depth"]["median_ms"] / res["image"]["median_ms"], 4)
+    for k in list(variants)[1:]:
+        res[f"{k}_over_image"] = round(res[k]["median_ms"] / res["image"]["median_ms"], 4)
     res["kernels_ms_per_step"] = kernels
     print(json.dumps(res))
 

@@ -42,6 +42,14 @@ def _ptr(t: Optional[torch.Tensor]) -> Optional[int]:
     return None if t is None else t.data_ptr()
 
 
+def _f32(t: Optional[torch.Tensor]) -> Optional[torch.Tensor]:
+    """An incoming gradient as the contiguous float32 tensor the kernels read (None stays None)."""
+    if t is None:
+        return None
+    t = t.contiguous()
+    return t if t.dtype == torch.float32 else t.float()
+
+
 def _require(t: torch.Tensor, name: str, dtype: torch.dtype, shape_tail=None) -> torch.Tensor:
     if not isinstance(t, torch.Tensor):
         raise TypeError(f"{name} must be a torch.Tensor")
@@ -228,6 +236,7 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
         skip_unused_hook_statistics: Optional[bool] = None,
         gradient_exchange=None,
         differentiable_depth: bool = False,
+        differentiable_alpha: bool = False,
     ):
         """``exact_exp``: blend kernels use ``expf`` instead of ``ex2.approx`` (parity debugging).
         ``force_key64``: sort the reference's 64-bit ``tile << 32 | depth`` keys even when the live
@@ -252,13 +261,22 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
         weights, and xyz also through each splat's camera-space depth (``gsb200_backward_with_depth``); a loss on depth
         alone works too.  The hook sees the sum of both losses' shares in ``grad_point_in_camera``, ``grad_viewspace``
         and the magnitudes, exactly as it sees the image loss's share.  Needs the transposed backward and the auxiliary
-        outputs: ``ValueError`` with ``backward_impl="butterfly"`` or ``config.rgb_only``."""
+        outputs: ``ValueError`` with ``backward_impl="butterfly"`` or ``config.rgb_only``.
+        ``differentiable_alpha``: ``forward`` also returns the per-pixel accumulated alpha S = 1 - prod (1 - alpha), (H, W)
+        float32, as a fourth output, differentiable (``gsb200_backward_aux``): a mask loss on S, or an image composited
+        on a background as ``image + (1 - S)[..., None] * bg``, trains xyz, q, s and the opacity through the blend weights;
+        a loss on S alone works too.  Combines with ``differentiable_depth``.  The hook sees the alpha loss's share as it
+        sees the image loss's share.  Same requirements as ``differentiable_depth``: ``ValueError`` with
+        ``backward_impl="butterfly"`` or ``config.rgb_only``."""
         super().__init__()
-        if differentiable_depth and backward_impl == "butterfly":
-            raise ValueError("differentiable_depth needs backward_impl='transposed': the butterfly kernel has no depth gradient")
-        if differentiable_depth and config.rgb_only:
-            raise ValueError("differentiable_depth needs the depth map: config.rgb_only=True renders none")
+        for name, on in (("differentiable_depth", differentiable_depth), ("differentiable_alpha", differentiable_alpha)):
+            if on and backward_impl == "butterfly":
+                raise ValueError(f"{name} needs backward_impl='transposed': the butterfly kernel implements only the "
+                                 "image gradient")
+            if on and config.rgb_only:
+                raise ValueError(f"{name} needs the auxiliary outputs: config.rgb_only=True renders none")
         self.differentiable_depth = bool(differentiable_depth)
+        self.differentiable_alpha = bool(differentiable_alpha)
         self.config = config
         self.backward_valid_point_hook = backward_valid_point_hook
         self._flags = (_lib.GSB_FLAG_EXACT_EXP if exact_exp else 0) | (_lib.GSB_FLAG_FORCE_KEY64 if force_key64 else 0) | \
@@ -295,13 +313,17 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                 ctx.color_max_sh_band = color_max_sh_band
                 if outer.differentiable_depth:
                     ctx.mark_non_differentiable(valid_count)
-                    ctx.set_materialize_grads(False)  # None tells an unused depth (or image) from a zero gradient
                 else:
                     ctx.mark_non_differentiable(depth, valid_count)
+                if outer.differentiable_depth or outer.differentiable_alpha:
+                    ctx.set_materialize_grads(False)  # None tells an unused output from a zero gradient
+                if outer.differentiable_alpha:
+                    return image, depth, valid_count, acc_alpha
                 return image, depth, valid_count
 
             @staticmethod
-            def backward(ctx, grad_rasterized_image, grad_rasterized_depth, grad_pixel_valid_point_count):
+            def backward(ctx, grad_rasterized_image, grad_rasterized_depth, grad_pixel_valid_point_count,
+                         grad_pixel_accumulated_alpha=None):
                 grad_pointcloud = grad_pointcloud_features = None
                 if ctx.needs_input_grad[0] or ctx.needs_input_grad[1]:  # GPCR:1028
                     if outer.config.rgb_only:
@@ -309,12 +331,13 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                         # this mode (GPCR:478-484), so its backward is undefined; refuse instead
                         raise RuntimeError("rgb_only=True is an inference-only mode: backward needs the "
                                            "auxiliary per-pixel outputs")
-                    if grad_rasterized_image is None:  # differentiable_depth: a loss on the depth map alone
+                    if grad_rasterized_image is None:  # a loss on the depth map or the accumulated alpha alone
                         frame = ctx.frame
                         grad_rasterized_image = torch.zeros((frame.height, frame.width, 3), dtype=torch.float32,
                                                             device=frame.ws.device)
                     grad_pointcloud, grad_pointcloud_features = outer._run_backward(ctx, grad_rasterized_image,
-                                                                                    grad_rasterized_depth)
+                                                                                    grad_rasterized_depth,
+                                                                                    grad_pixel_accumulated_alpha)
                 return grad_pointcloud, grad_pointcloud_features, None, None, None, None, None, None
 
         self._module_function = _module_function
@@ -415,7 +438,7 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
         return (image, depth, acc_alpha, last_effective, valid_count), frame, {"camera_intrinsics": K}
 
     # ------------------------------------------------------------------ backward plumbing
-    def _run_backward(self, ctx, grad_rasterized_image, grad_rasterized_depth=None):
+    def _run_backward(self, ctx, grad_rasterized_image, grad_rasterized_depth=None, grad_pixel_accumulated_alpha=None):
         cfg = self.config
         lib = _lib.load()
         saved = ctx.saved_tensors
@@ -471,14 +494,17 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                 grad_pointcloud_features=_ptr(grad_pointcloud_features),
                 magnitude_grad_viewspace_on_image=_ptr(magnitude_on_image), stream=stream.cuda_stream,
                 grad_sum_compact=_ptr(grad_sum), grad_color_compact=_ptr(blocks[exchange.rank]) if compact else None)
-            if depth is None:
-                _lib.check(lib.gsb200_backward(ctypes.byref(args)), "gsb200_backward")
-            else:
-                grad_depth = grad_rasterized_depth.contiguous()
-                if grad_depth.dtype != torch.float32:
-                    grad_depth = grad_depth.float()
+            grad_depth = _f32(grad_rasterized_depth) if depth is not None else None
+            # differentiable_alpha: None when the loss does not use the accumulated alpha
+            grad_alpha = _f32(grad_pixel_accumulated_alpha) if self.differentiable_alpha else None
+            if grad_alpha is not None:
+                _lib.check(lib.gsb200_backward_aux(ctypes.byref(args), _ptr(grad_depth), _ptr(depth), _ptr(grad_alpha)),
+                           "gsb200_backward_aux")
+            elif depth is not None:
                 _lib.check(lib.gsb200_backward_with_depth(ctypes.byref(args), _ptr(grad_depth), _ptr(depth)),
                            "gsb200_backward_with_depth")
+            else:
+                _lib.check(lib.gsb200_backward(ctypes.byref(args)), "gsb200_backward")
             own_view_grad_xyz = None
             if compact:
                 exchange.rows_written(grad_sum, blocks)

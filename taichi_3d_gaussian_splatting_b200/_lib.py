@@ -101,6 +101,7 @@ EXPORTS = (
     "gsb200_image_loss_temp_bytes", "gsb200_image_loss", "gsb200_adam_step", "gsb200_controller_update",
     "gsb200_forward_blend_work", "gsb200_backward_blend_work", "gsb200_device_selftest", "gsb200_expand_view_gradients",
     "gsb200_train_step", "gsb200_abi_sizes_ext", "gsb200_exchange_multimem", "gsb200_backward_with_depth",
+    "gsb200_backward_aux",
 )
 
 _lib = None
@@ -128,6 +129,8 @@ def load() -> ctypes.CDLL:
     lib.gsb200_backward.restype = ctypes.c_int
     lib.gsb200_backward_with_depth.argtypes = [ctypes.POINTER(GsbBackwardArgs), c_vp, c_vp]
     lib.gsb200_backward_with_depth.restype = ctypes.c_int
+    lib.gsb200_backward_aux.argtypes = [ctypes.POINTER(GsbBackwardArgs), c_vp, c_vp, c_vp]
+    lib.gsb200_backward_aux.restype = ctypes.c_int
     lib.gsb200_sort_temp_bytes.argtypes = [c_i64, c_i32]
     lib.gsb200_sort_temp_bytes.restype = c_i64
     lib.gsb200_sort_pairs.argtypes = [c_vp, c_vp, c_vp, c_vp, c_i64, c_i32, c_i32, c_vp, c_i64, c_vp]

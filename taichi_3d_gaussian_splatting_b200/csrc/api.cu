@@ -249,9 +249,10 @@ int gsb200_forward(const GsbForwardArgs *a) {
     return launch_blend_forward(*a, ws, st);
 }
 
-// grad_depth / depth: both NULL (the image gradient alone), or both set (gsb200_backward_with_depth, checked there)
+// grad_depth / depth: both NULL (no depth term), or both set; grad_alpha: NULL (no alpha term) or set.  The auxiliary terms
+// are checked in gsb200_backward_aux.
 static int backward_impl(const GsbBackwardArgs *a, bool skip_on_overflow, const float *grad_depth = nullptr,
-                         const float *depth = nullptr) {
+                         const float *depth = nullptr, const float *grad_alpha = nullptr) {
     if (!a) {
         set_error("backward: args is null");
         return GSB_EINVAL;
@@ -298,23 +299,29 @@ static int backward_impl(const GsbBackwardArgs *a, bool skip_on_overflow, const 
     cudaStream_t st = static_cast<cudaStream_t>(a->stream);
     if (a->accum_rows > 0)
         GSB_CUDA_CHECK(cudaMemsetAsync(a->accum, 0, (size_t)a->accum_rows * GSB_ACCUM_FLOATS * 4, st));
-    if ((rc = launch_blend_backward(*a, ws, st, grad_depth, depth)) != GSB_OK) return rc;
+    if ((rc = launch_blend_backward(*a, ws, st, grad_depth, depth, grad_alpha)) != GSB_OK) return rc;
     return launch_backward_points(*a, ws, st, skip_on_overflow ? ws.counters + CNT_OVERFLOW : nullptr, grad_depth != nullptr);
 }
 
 int gsb200_backward(const GsbBackwardArgs *a) { return backward_impl(a, false); }
 
-int gsb200_backward_with_depth(const GsbBackwardArgs *a, const float *grad_rasterized_depth, const float *rasterized_depth) {
+int gsb200_backward_aux(const GsbBackwardArgs *a, const float *grad_rasterized_depth, const float *rasterized_depth,
+                        const float *grad_pixel_accumulated_alpha) {
     if ((grad_rasterized_depth == nullptr) != (rasterized_depth == nullptr)) {
-        set_error("backward_with_depth: grad_rasterized_depth and rasterized_depth must be both NULL or both set");
+        set_error("backward_aux: grad_rasterized_depth and rasterized_depth must be both NULL or both set");
         return GSB_EINVAL;
     }
-    if (grad_rasterized_depth != nullptr && a != nullptr && !(a->flags & GSB_FLAG_BACKWARD_TRANSPOSED)) {
-        set_error("backward_with_depth: the depth gradient needs the transposed backward kernel "
-                  "(GSB_FLAG_BACKWARD_TRANSPOSED); the butterfly kernel does not implement it");
+    const bool aux = grad_rasterized_depth != nullptr || grad_pixel_accumulated_alpha != nullptr;
+    if (aux && a != nullptr && !(a->flags & GSB_FLAG_BACKWARD_TRANSPOSED)) {
+        set_error("backward_aux: the depth and alpha gradients need the transposed backward kernel "
+                  "(GSB_FLAG_BACKWARD_TRANSPOSED); the butterfly kernel does not implement them");
         return GSB_EUNSUPPORTED;
     }
-    return backward_impl(a, false, grad_rasterized_depth, rasterized_depth);
+    return backward_impl(a, false, grad_rasterized_depth, rasterized_depth, grad_pixel_accumulated_alpha);
+}
+
+int gsb200_backward_with_depth(const GsbBackwardArgs *a, const float *grad_rasterized_depth, const float *rasterized_depth) {
+    return gsb200_backward_aux(a, grad_rasterized_depth, rasterized_depth, nullptr);
 }
 
 int gsb200_image_loss(const float *rasterized_image, const float *ground_truth_image, int32_t camera_height,

@@ -278,11 +278,12 @@ static BlendBwdParams make_blend_bwd_params(const GsbBackwardArgs &a, const Work
     p.work_counters = nullptr;
     p.grad_depth = nullptr;
     p.depth = nullptr;
+    p.grad_alpha = nullptr;
     return p;
 }
 
 int launch_blend_backward(const GsbBackwardArgs &a, const Workspace &ws, cudaStream_t stream, const float *grad_depth,
-                          const float *depth) {
+                          const float *depth, const float *grad_alpha) {
     BlendBwdParams p;
     p.H = a.camera_height;
     p.W = a.camera_width;
@@ -299,11 +300,13 @@ int launch_blend_backward(const GsbBackwardArgs &a, const Workspace &ws, cudaStr
     p.work_counters = nullptr;
     p.grad_depth = grad_depth;
     p.depth = depth;
+    p.grad_alpha = grad_alpha;
     const int tiles = p.tiles_x * (a.camera_height / GSB_TILE_HEIGHT);
     if (tiles <= 0) return GSB_OK;
     if (a.flags & GSB_FLAG_BACKWARD_TRANSPOSED)  // experimental, see blend_bwd_transposed.cu
         return launch_blend_backward_transposed(p, tiles, (a.flags & GSB_FLAG_EXACT_EXP) != 0,
-                                                (a.flags & GSB_FLAG_NO_HOOK_STATS) == 0, stream, grad_depth != nullptr);
+                                                (a.flags & GSB_FLAG_NO_HOOK_STATS) == 0, stream, grad_depth != nullptr,
+                                                grad_alpha != nullptr);
     const bool exact = (a.flags & GSB_FLAG_EXACT_EXP) != 0;
     if (a.flags & GSB_FLAG_NO_HOOK_STATS) {  // opt-in
         if (exact) blend_backward_kernel<true, false><<<tiles, GSB_TILE_PIXELS, 0, stream>>>(p);

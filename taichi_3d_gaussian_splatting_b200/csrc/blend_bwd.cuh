@@ -19,6 +19,7 @@ struct BlendBwdParams {
     unsigned long long *work_counters;  // COUNT instantiation only: [0] (warp, splat) visits, [1] contributing (pixel, splat) pairs
     const float *grad_depth;  // DEPTH instantiation only: (H,W) dL/d depth and the forward's depth output; NULL otherwise
     const float *depth;
+    const float *grad_alpha;  // ALPHA instantiation only: (H,W) dL/d pixel_accumulated_alpha; NULL otherwise
 };
 
 #ifdef GSB_HOST_EMU  // tests/simt: the kernels compiled as host C++ under a lock-step SIMT emulator
@@ -44,7 +45,7 @@ __device__ __forceinline__ float sqrt_approx(float x) {  // MUFU.RSQ based, ~1 u
 #endif
 
 int launch_blend_backward_transposed(const BlendBwdParams &p, int tiles, bool exact_exp, bool stats,
-                                     cudaStream_t stream, bool depth = false);
+                                     cudaStream_t stream, bool depth = false, bool alpha = false);
 int launch_blend_backward_count(const BlendBwdParams &p, int tiles, cudaStream_t stream);
 
 }  // namespace gsb

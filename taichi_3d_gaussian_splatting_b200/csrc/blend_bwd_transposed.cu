@@ -23,6 +23,12 @@
 //   direct:        dD/dz_i = alpha_i T_i / S -- phase 2 sums alpha T g^ per splat into the spare word 11 of the
 //     accumulator row (g^ rides in the unused .w of the warp's dL/dimage copy), which backward_points_kernel<_, true>
 //     turns into dL/dxyz along the camera's viewing axis.
+// ALPHA = true (gsb200_backward_aux with an alpha gradient) adds the gradient of the accumulated alpha S = 1 - prod (1 - alpha).
+// S is the blend of a colour channel whose colour is 1, so dS/dalpha_i = T_i - sum_{j behind i} w_j / (1 - alpha_i)
+// = T_final / (1 - alpha_i), and with g_S = dL/dS per pixel (a register of phase 1; no direct term, nothing in phase 2):
+//   fast path:  the one-scalar recursion's cg = sum g c_i becomes sum g c_i + g_S (the FMA chain starts at g_S, or at
+//     g_S - g^ D with DEPTH);
+//   exact path: a_grad += g_S T_final / (1 - alpha) for a contributing pair.
 #include "blend_bwd.cuh"
 
 namespace gsb {
@@ -114,10 +120,10 @@ __device__ __forceinline__ float keep_if_contributing(float P, int idx, int last
 #endif
 }
 
-template <bool EXACT_EXP, bool STATS, bool COUNT = false, bool DEPTH = false>
+template <bool EXACT_EXP, bool STATS, bool COUNT = false, bool DEPTH = false, bool ALPHA = false>
 __global__ void __launch_bounds__(GSB_TILE_PIXELS, GSB_TB_MIN_BLOCKS)
 blend_backward_transposed_kernel(const BlendBwdParams p) {
-    static_assert(!(COUNT && DEPTH), "the work-counter diagnostic runs the default arithmetic only");
+    static_assert(!(COUNT && (DEPTH || ALPHA)), "the work-counter diagnostic runs the default arithmetic only");
     TbShared &S = *reinterpret_cast<TbShared *>(tb_dynamic_smem());
     constexpr int NV = STATS ? 11 : 9;
 
@@ -144,6 +150,12 @@ blend_backward_transposed_kernel(const BlendBwdParams p) {
         const float Sa = p.acc_alpha[pix];
         gd = Sa > 0.0f ? p.grad_depth[pix] / Sa : 0.0f;
         hd = EXACT_EXP ? p.depth[pix] : gd * p.depth[pix];
+    }
+    // ALPHA only: ga = g_S (- hd with DEPTH) starts the fast path's colour chain; g_S T_final on the exact path
+    float ga = 0.0f;
+    if (ALPHA) {
+        const float gs = p.grad_alpha[pix];
+        ga = EXACT_EXP ? gs * T : DEPTH ? gs - hd : gs;
     }
     TbWarp &Wp = S.w[warp];
     Wp.g[lane] = make_float4(g0, g1, g2, gd);
@@ -279,6 +291,7 @@ blend_backward_transposed_kernel(const BlendBwdParams p) {
                             a_grad += contributes ? (e * Tn - w3 * inv) * gd : 0.0f;
                             w3 = fmaf(e, aT, w3);
                         }
+                        if (ALPHA) a_grad += contributes ? ga * inv : 0.0f;  // g_S T_final / (1 - alpha)
                         T = contributes ? Tn : T;
                         w0 = fmaf(r2.x, aT, w0);
                         w1 = fmaf(r2.y, aT, w1);
@@ -299,8 +312,10 @@ blend_backward_transposed_kernel(const BlendBwdParams p) {
                         const float inv = rcp_approx(1.0f - alpha);
                         T *= inv;                 // T_i = T_{i+1} / (1 - alpha), GPCR:640
                         aT = alpha * T;
-                        float cg = fmaf(r2.z, g2, fmaf(r2.y, g1, r2.x * g0));
-                        if (DEPTH) cg = fmaf(gd, r1.w, cg) - hd;  // + gd (z - D): the depth map as a fourth channel
+                        // + g_S with ALPHA: the accumulated alpha as a channel of colour 1
+                        float cg = fmaf(r2.z, g2, fmaf(r2.y, g1, ALPHA ? fmaf(r2.x, g0, ga) : r2.x * g0));
+                        // + gd (z - D): the depth map as a fourth channel (with ALPHA, ga already holds the - hd)
+                        if (DEPTH) cg = ALPHA ? fmaf(gd, r1.w, cg) : fmaf(gd, r1.w, cg) - hd;
                         const float a_grad = fmaf(cg, T, -(w0 * inv));
                         w0 = fmaf(cg, aT, w0);
                         G = a_grad * P;
@@ -445,29 +460,35 @@ blend_backward_transposed_kernel(const BlendBwdParams p) {
 }
 
 #ifndef GSB_HOST_EMU
-template <bool EXACT_EXP, bool STATS, bool DEPTH = false>
+template <bool EXACT_EXP, bool STATS, bool DEPTH = false, bool ALPHA = false>
 static int launch_tb(const BlendBwdParams &p, int tiles, cudaStream_t stream) {
     static bool configured = false;  // one device per process (one process per GPU)
     if (!configured) {
-        GSB_CUDA_CHECK(cudaFuncSetAttribute(blend_backward_transposed_kernel<EXACT_EXP, STATS, false, DEPTH>,
+        GSB_CUDA_CHECK(cudaFuncSetAttribute(blend_backward_transposed_kernel<EXACT_EXP, STATS, false, DEPTH, ALPHA>,
                                             cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TbShared)));
         configured = true;
     }
-    blend_backward_transposed_kernel<EXACT_EXP, STATS, false, DEPTH><<<tiles, GSB_TILE_PIXELS, sizeof(TbShared), stream>>>(p);
+    blend_backward_transposed_kernel<EXACT_EXP, STATS, false, DEPTH, ALPHA>
+        <<<tiles, GSB_TILE_PIXELS, sizeof(TbShared), stream>>>(p);
     GSB_CUDA_CHECK(cudaGetLastError());
     return GSB_OK;
 }
 
-// depth = true: p.grad_depth and p.depth must be set (the DEPTH instantiations)
+template <bool DEPTH, bool ALPHA>
+static int launch_tb_terms(const BlendBwdParams &p, int tiles, bool exact_exp, bool stats, cudaStream_t stream) {
+    if (exact_exp)
+        return stats ? launch_tb<true, true, DEPTH, ALPHA>(p, tiles, stream) : launch_tb<true, false, DEPTH, ALPHA>(p, tiles, stream);
+    return stats ? launch_tb<false, true, DEPTH, ALPHA>(p, tiles, stream) : launch_tb<false, false, DEPTH, ALPHA>(p, tiles, stream);
+}
+
+// depth = true: p.grad_depth and p.depth must be set (the DEPTH instantiations); alpha = true: p.grad_alpha (ALPHA)
 int launch_blend_backward_transposed(const BlendBwdParams &p, int tiles, bool exact_exp, bool stats,
-                                     cudaStream_t stream, bool depth) {
-    if (depth) {
-        if (exact_exp)
-            return stats ? launch_tb<true, true, true>(p, tiles, stream) : launch_tb<true, false, true>(p, tiles, stream);
-        return stats ? launch_tb<false, true, true>(p, tiles, stream) : launch_tb<false, false, true>(p, tiles, stream);
-    }
-    if (exact_exp) return stats ? launch_tb<true, true>(p, tiles, stream) : launch_tb<true, false>(p, tiles, stream);
-    return stats ? launch_tb<false, true>(p, tiles, stream) : launch_tb<false, false>(p, tiles, stream);
+                                     cudaStream_t stream, bool depth, bool alpha) {
+    if (alpha)
+        return depth ? launch_tb_terms<true, true>(p, tiles, exact_exp, stats, stream)
+                     : launch_tb_terms<false, true>(p, tiles, exact_exp, stats, stream);
+    return depth ? launch_tb_terms<true, false>(p, tiles, exact_exp, stats, stream)
+                 : launch_tb_terms<false, false>(p, tiles, exact_exp, stats, stream);
 }
 
 // Diagnostic: loop A with GPU-side work counters (default arithmetic, no hook statistics): counters[0] = (warp, splat)
