@@ -204,7 +204,8 @@ const char *gsb200_last_error(void);
 /* sizeof(GsbWorkspaceLayout), sizeof(GsbForwardArgs), sizeof(GsbBackwardArgs) as compiled: lets a
  * foreign-language binding verify its struct mirrors. */
 void gsb200_abi_sizes(int64_t *out3);
-/* ... and of the first n of {GsbWorkspaceLayout, GsbForwardArgs, GsbBackwardArgs, GsbExpandArgs, GsbTrainStepArgs} */
+/* ... and of the first n of {GsbWorkspaceLayout, GsbForwardArgs, GsbBackwardArgs, GsbExpandArgs, GsbTrainStepArgs,
+ * GsbSupervisionArgs} */
 void gsb200_abi_sizes_ext(int64_t *out, int32_t n);
 
 /* Workspace sizing.  far_plane*depth_to_sort_key_scale fixes the depth-key width; (H/16)*(W/16)
@@ -299,6 +300,35 @@ typedef struct GsbTrainStepArgs {
     int32_t step;                    /* 1-based Adam step count */
 } GsbTrainStepArgs;
 int gsb200_train_step(const GsbTrainStepArgs *args);
+
+/* Depth, mask and background terms of the fused train step (an extension: the reference trains on the image alone).  For a
+ * view with I the rasterised image, S = pixel_accumulated_alpha, D = the rendered depth:
+ *   background (if set):  the image loss runs on I' = I + (1 - S) bg; with a mask target the ground truth is composited
+ *                         too, gt' = gt m + (1 - m) bg (without one it is taken to be on bg already);
+ *   mask term:            mask_weight * mean |S - m|;
+ *   depth term:           depth_weight * sum_valid |D - d*| / max(n_valid, 1), a pixel valid when d* is finite and > 0
+ *                         (0 or NaN = no measurement); d* in point-cloud units along the optical axis, like D.
+ * total = image loss + mask term + depth term.  The gradients w.r.t. S and D are written to the caller's buffers and fed to
+ * the backward (gsb200_backward_aux). */
+typedef struct GsbSupervisionArgs {
+    const float *depth_target;    /* (H,W) f32 or NULL */
+    const float *mask_target;     /* (H,W) f32 in [0,1] or NULL */
+    const float *background;      /* device float[3] or NULL (black: no compositing) */
+    float depth_weight, mask_weight; /* >= 0, finite; 0 = term off */
+    float *grad_depth;            /* (H,W) out: dL/dD (depth term) */
+    float *grad_pixel_accumulated_alpha; /* (H,W) out: dL/dS (mask term or background) */
+    float *loss_out3;             /* device: {total, mask term, depth term} */
+    void *temp;                   /* gsb200_supervision_temp_bytes(H, W), 16-byte aligned, first 16 bytes zero before first use */
+    int64_t temp_bytes;
+} GsbSupervisionArgs;
+int64_t gsb200_supervision_temp_bytes(int32_t camera_height, int32_t camera_width);
+/* gsb200_train_step with the supervision terms: forward -> pre-pass (composite, sums) -> image loss on (I', gt') ->
+ * post-pass (dL/dS, dL/dD, losses) -> backward with the depth and alpha gradients (skipped on overflow like the rest) ->
+ * both Adam steps.  NULL supervision, or every term off: exactly gsb200_train_step.  GSB_EINVAL, before any CUDA call, for a
+ * negative or non-finite weight, a weight > 0 without its target or gradient output, a background without the alpha
+ * gradient output, or a temp that is too small or not 16-byte aligned; GSB_EUNSUPPORTED without
+ * GSB_FLAG_BACKWARD_TRANSPOSED.  Deterministic: fixed grids and summation orders. */
+int gsb200_train_step_aux(const GsbTrainStepArgs *args, const GsbSupervisionArgs *supervision);
 
 /* Individual stages (same workspace), for tests and profiling. */
 int gsb200_stage_preprocess(const GsbForwardArgs *args);   /* K1+P1+K2+K3+P2+K4 fused */

@@ -84,6 +84,13 @@ class GsbTrainStepArgs(ctypes.Structure):
     ]
 
 
+class GsbSupervisionArgs(ctypes.Structure):
+    _fields_ = [
+        ("depth_target", c_vp), ("mask_target", c_vp), ("background", c_vp), ("depth_weight", c_f32), ("mask_weight", c_f32),
+        ("grad_depth", c_vp), ("grad_pixel_accumulated_alpha", c_vp), ("loss_out3", c_vp), ("temp", c_vp), ("temp_bytes", c_i64),
+    ]
+
+
 class GsbExpandArgs(ctypes.Structure):
     _fields_ = [
         ("num_points", c_i64), ("num_views", c_i32), ("num_objects", c_i32), ("grad_sum", c_vp),
@@ -101,7 +108,7 @@ EXPORTS = (
     "gsb200_image_loss_temp_bytes", "gsb200_image_loss", "gsb200_adam_step", "gsb200_controller_update",
     "gsb200_forward_blend_work", "gsb200_backward_blend_work", "gsb200_device_selftest", "gsb200_expand_view_gradients",
     "gsb200_train_step", "gsb200_abi_sizes_ext", "gsb200_exchange_multimem", "gsb200_backward_with_depth",
-    "gsb200_backward_aux",
+    "gsb200_backward_aux", "gsb200_supervision_temp_bytes", "gsb200_train_step_aux",
 )
 
 _lib = None
@@ -160,6 +167,10 @@ def load() -> ctypes.CDLL:
     lib.gsb200_exchange_multimem.restype = ctypes.c_int
     lib.gsb200_train_step.argtypes = [ctypes.POINTER(GsbTrainStepArgs)]
     lib.gsb200_train_step.restype = ctypes.c_int
+    lib.gsb200_train_step_aux.argtypes = [ctypes.POINTER(GsbTrainStepArgs), ctypes.POINTER(GsbSupervisionArgs)]
+    lib.gsb200_train_step_aux.restype = ctypes.c_int
+    lib.gsb200_supervision_temp_bytes.argtypes = [c_i32, c_i32]
+    lib.gsb200_supervision_temp_bytes.restype = c_i64
     lib.gsb200_device_selftest.argtypes = [c_vp]
     lib.gsb200_device_selftest.restype = ctypes.c_int
     # Every export gets its signature here: without argtypes ctypes passes a Python int as a 32-bit C int, which silently
@@ -187,6 +198,11 @@ def load() -> ctypes.CDLL:
     mine5 = mine + (ctypes.sizeof(GsbExpandArgs), ctypes.sizeof(GsbTrainStepArgs))
     if tuple(sizes5) != mine5:
         raise RuntimeError(f"libgsb200.so ABI mismatch: C struct sizes {tuple(sizes5)} != ctypes mirrors {mine5}")
+    sizes6 = (c_i64 * 6)()
+    lib.gsb200_abi_sizes_ext(sizes6, 6)
+    if sizes6[5] != ctypes.sizeof(GsbSupervisionArgs):
+        raise RuntimeError(f"libgsb200.so ABI mismatch: sizeof(GsbSupervisionArgs) {sizes6[5]} != ctypes mirror "
+                           f"{ctypes.sizeof(GsbSupervisionArgs)}")
     _lib = lib
     return lib
 

@@ -30,6 +30,7 @@ SOURCES = {
     "blend_bwd_transposed.cu": [],
     "loss.cu": [],
     "image_loss.cu": [],
+    "supervision_loss.cu": [],
     "adam.cu": [],
     "controller.cu": [],
     "exchange.cu": [],

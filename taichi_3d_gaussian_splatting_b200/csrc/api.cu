@@ -192,9 +192,9 @@ void gsb200_abi_sizes(int64_t *out3) {
 }
 
 void gsb200_abi_sizes_ext(int64_t *out, int32_t n) {
-    const int64_t all[5] = {(int64_t)sizeof(GsbWorkspaceLayout), (int64_t)sizeof(GsbForwardArgs), (int64_t)sizeof(GsbBackwardArgs),
-                            (int64_t)sizeof(GsbExpandArgs), (int64_t)sizeof(GsbTrainStepArgs)};
-    for (int i = 0; i < n && i < 5; ++i) out[i] = all[i];
+    const int64_t all[6] = {(int64_t)sizeof(GsbWorkspaceLayout), (int64_t)sizeof(GsbForwardArgs), (int64_t)sizeof(GsbBackwardArgs),
+                            (int64_t)sizeof(GsbExpandArgs), (int64_t)sizeof(GsbTrainStepArgs), (int64_t)sizeof(GsbSupervisionArgs)};
+    for (int i = 0; i < n && i < 6; ++i) out[i] = all[i];
 }
 
 int gsb200_workspace_layout(int64_t num_points, int32_t num_objects, int64_t key_capacity,
@@ -328,7 +328,11 @@ int gsb200_image_loss(const float *rasterized_image, const float *ground_truth_i
                       int32_t camera_width, float lambda_value, float upstream_grad, float *loss_out3,
                       float *grad_rasterized_image, void *temp, int64_t temp_bytes, void *stream);
 
-int gsb200_train_step(const GsbTrainStepArgs *t) {
+static bool weight_ok(float w) { return w >= 0.0f && w <= 3.402823466e38f; }  // false for NaN, inf and negatives
+
+int gsb200_train_step(const GsbTrainStepArgs *t) { return gsb200_train_step_aux(t, nullptr); }
+
+int gsb200_train_step_aux(const GsbTrainStepArgs *t, const GsbSupervisionArgs *s) {
     if (!t || !t->ground_truth_image || !t->loss_out3 || !t->loss_temp || !t->feature_exp_avg || !t->feature_exp_avg_sq ||
         !t->position_exp_avg || !t->position_exp_avg_sq || t->step < 1) {
         set_error("train_step: null pointer argument or step < 1");
@@ -343,16 +347,67 @@ int gsb200_train_step(const GsbTrainStepArgs *t) {
         set_error("train_step: forward / backward blocks do not describe one frame (or rgb_only / compact gradients set)");
         return GSB_EINVAL;
     }
+    bool depth_on = false, alpha_on = false;
+    if (s) {
+        if (!weight_ok(s->depth_weight) || !weight_ok(s->mask_weight)) {
+            set_error("train_step_aux: the depth and mask weights must be finite and >= 0 (got %g, %g)", (double)s->depth_weight,
+                      (double)s->mask_weight);
+            return GSB_EINVAL;
+        }
+        depth_on = s->depth_weight > 0.0f;
+        const bool mask_on = s->mask_weight > 0.0f;
+        if (depth_on && (!s->depth_target || !s->grad_depth)) {
+            set_error("train_step_aux: a depth weight > 0 needs depth_target and grad_depth");
+            return GSB_EINVAL;
+        }
+        if (mask_on && !s->mask_target) {
+            set_error("train_step_aux: a mask weight > 0 needs mask_target");
+            return GSB_EINVAL;
+        }
+        alpha_on = mask_on || s->background != nullptr;
+        if (alpha_on && !s->grad_pixel_accumulated_alpha) {
+            set_error("train_step_aux: the mask term and the background need grad_pixel_accumulated_alpha");
+            return GSB_EINVAL;
+        }
+        if (depth_on || alpha_on) {
+            if (!s->loss_out3 || !s->temp || reinterpret_cast<uintptr_t>(s->temp) % 16 ||
+                s->temp_bytes < gsb200_supervision_temp_bytes(f.camera_height, f.camera_width)) {
+                set_error("train_step_aux: loss_out3 missing, or temp null, not 16-byte aligned or smaller than "
+                          "gsb200_supervision_temp_bytes(H, W) (temp_bytes=%lld)", (long long)s->temp_bytes);
+                return GSB_EINVAL;
+            }
+            if (!(b.flags & GSB_FLAG_BACKWARD_TRANSPOSED)) {
+                set_error("train_step_aux: the depth and alpha gradients need the transposed backward kernel "
+                          "(GSB_FLAG_BACKWARD_TRANSPOSED)");
+                return GSB_EUNSUPPORTED;
+            }
+            if (!f.rasterized_depth || !f.pixel_accumulated_alpha) {
+                set_error("train_step_aux: the supervision terms need the forward's depth and accumulated alpha outputs");
+                return GSB_EINVAL;
+            }
+        }
+    }
+    const bool supervised = depth_on || alpha_on;
+    const int H = f.camera_height, W = f.camera_width;
+    cudaStream_t st = static_cast<cudaStream_t>(f.stream);
     int rc = gsb200_forward(&f);
     if (rc != GSB_OK) return rc;
-    rc = gsb200_image_loss(f.rasterized_image, t->ground_truth_image, f.camera_height, f.camera_width, t->lambda_value, 1.0f,
-                           t->loss_out3, const_cast<float *>(b.grad_rasterized_image), t->loss_temp, t->loss_temp_bytes, f.stream);
+    const float *loss_image = f.rasterized_image, *loss_gt = t->ground_truth_image;
+    if (supervised && (rc = launch_supervision_pre(*s, f.rasterized_image, t->ground_truth_image, f.pixel_accumulated_alpha,
+                                                   f.rasterized_depth, H, W, st, &loss_image, &loss_gt)) != GSB_OK)
+        return rc;
+    rc = gsb200_image_loss(loss_image, loss_gt, H, W, t->lambda_value, 1.0f, t->loss_out3,
+                           const_cast<float *>(b.grad_rasterized_image), t->loss_temp, t->loss_temp_bytes, f.stream);
     if (rc != GSB_OK) return rc;
-    if ((rc = backward_impl(&b, true)) != GSB_OK) return rc;
+    if (supervised && (rc = launch_supervision_post(*s, f.rasterized_image, t->ground_truth_image, f.pixel_accumulated_alpha,
+                                                    f.rasterized_depth, H, W, b.grad_rasterized_image, t->loss_out3, st)) != GSB_OK)
+        return rc;
+    if ((rc = backward_impl(&b, true, depth_on ? s->grad_depth : nullptr, depth_on ? f.rasterized_depth : nullptr,
+                            alpha_on ? s->grad_pixel_accumulated_alpha : nullptr)) != GSB_OK)
+        return rc;
     Workspace ws;
     if ((rc = resolve_fwd(&f, &ws)) != GSB_OK) return rc;
     const long long *skip = ws.counters + CNT_OVERFLOW;
-    cudaStream_t st = static_cast<cudaStream_t>(f.stream);
     rc = launch_adam_step(f.pointcloud_features, b.grad_pointcloud_features, t->feature_exp_avg, t->feature_exp_avg_sq,
                           (long long)f.num_points * GSB_FEATURE_DIM, t->feature_learning_rate, t->beta1, t->beta2, t->eps, t->step,
                           skip, st);

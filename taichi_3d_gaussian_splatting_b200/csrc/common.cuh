@@ -79,6 +79,13 @@ int launch_backward_points(const GsbBackwardArgs &a, const Workspace &ws, cudaSt
 int launch_adam_step(float *param, const float *grad, float *exp_avg, float *exp_avg_sq, long long n, double lr, double beta1,
                      double beta2, double eps, int step, const long long *skip_flag, cudaStream_t stream);
 int launch_expand_view_gradients(const GsbExpandArgs &a, cudaStream_t stream);
+// supervision_loss.cu: the pre-pass returns the image and ground truth the image loss must read (composited or the inputs)
+int launch_supervision_pre(const GsbSupervisionArgs &s, const float *image, const float *gt, const float *alpha,
+                           const float *depth, int H, int W, cudaStream_t stream, const float **loss_image,
+                           const float **loss_gt);
+int launch_supervision_post(const GsbSupervisionArgs &s, const float *image, const float *gt, const float *alpha,
+                            const float *depth, int H, int W, const float *grad_image, const float *image_loss,
+                            cudaStream_t stream);
 int launch_blend_forward_count(const GsbForwardArgs &a, const Workspace &ws, unsigned long long *counters_dev,
                                cudaStream_t stream);
 int launch_blend_backward_work(const GsbBackwardArgs &a, const Workspace &ws, unsigned long long *counters_dev,

@@ -10,6 +10,10 @@ waits for them once per frame; here nothing waits).  The accumulator buffer ther
 pairs than the key capacity turns itself into a no-op ON THE DEVICE (overflow counter checked by the accumulator update and
 both Adam kernels); the host reads the counters of iteration i while it prepares iteration i+1, grows the capacity and counts
 the skipped iteration in ``num_skipped_steps``.  CUDA only; there is no CPU path.
+
+Optional supervision terms (``depth_weight``, ``mask_weight``, ``run(..., targets=, background=)``): a masked-L1 depth loss,
+an L1 mask loss on the accumulated alpha and training on a background colour, in the same one call
+(``gsb200_train_step_aux``; ``loss.supervision_loss`` states the loss in torch).
 """
 import ctypes
 import warnings
@@ -20,14 +24,23 @@ import torch
 
 from . import _lib
 from .GaussianPointCloudRasterisation import Frame, GaussianPointCloudRasterisation, _ptr
+from .loss import SupervisionTargets
+
+__all__ = ["FusedTrainStep", "SupervisionTargets"]
 
 
 class FusedTrainStep:
     def __init__(self, scene, rasterisation_config, lambda_value: float = 0.2, controller=None, betas=(0.9, 0.999),
-                 eps: float = 1e-8, key_capacity: Optional[int] = None):
+                 eps: float = 1e-8, key_capacity: Optional[int] = None, depth_weight: float = 0.0,
+                 mask_weight: float = 0.0):
         """``scene``: object with ``point_cloud`` (N,3), ``point_cloud_features`` (N,56), ``point_invalid_mask``,
         ``point_object_id`` (CUDA, contiguous; updated in place).  ``controller``: a ``GaussianPointAdaptiveController`` whose
-        six accumulators are updated by the backward epilogue (or ``None``)."""
+        six accumulators are updated by the backward epilogue (or ``None``).  ``depth_weight`` / ``mask_weight``: weights of
+        the depth and mask terms (``loss.supervision_loss``); they need the matching target in ``run(targets=...)``."""
+        for name, w in (("depth_weight", depth_weight), ("mask_weight", mask_weight)):
+            if not (w >= 0.0 and w < float("inf")):
+                raise ValueError(f"{name} must be finite and >= 0, got {w}")
+        self.depth_weight, self.mask_weight = float(depth_weight), float(mask_weight)
         self.scene = scene
         self.config = rasterisation_config
         self.lambda_value = float(lambda_value)
@@ -51,7 +64,8 @@ class FusedTrainStep:
         self._flat = z(off + 56 * N)
         self.grad_pointcloud = self._flat[:3 * N].view(N, 3)
         self.grad_pointcloud_features = self._flat[off:off + 56 * N].view(N, 56)
-        self.loss = z(3)  # {loss, L1, 1 - SSIM} of the latest iteration (device)
+        self.loss = z(3)  # {loss, L1, 1 - SSIM} of the latest iteration (device); with supervision terms: of the image loss
+        self.supervision_loss = z(3)  # {total, mask term, depth term} of the latest supervised iteration (device)
         self._res = {}
         self._pinned = [torch.zeros(4, dtype=torch.int64).pin_memory() for _ in range(2)]
         self._events = [torch.cuda.Event() for _ in range(2)]
@@ -69,11 +83,14 @@ class FusedTrainStep:
             layout = _lib.workspace_layout(self.N, n_obj, self.key_capacity, H, W, cfg.far_plane, cfg.depth_to_sort_key_scale, 0)
             e = lambda shape, dt=torch.float32: torch.empty(shape, dtype=dt, device=dev)  # noqa: E731
             temp_bytes = int(self._lib.gsb200_image_loss_temp_bytes(H, W))
+            sup_bytes = int(self._lib.gsb200_supervision_temp_bytes(H, W))
             b = SimpleNamespace(layout=layout, ws=e((layout.total_bytes,), torch.uint8), image=e((H, W, 3)), depth=e((H, W)),
                                 acc_alpha=e((H, W)), last_effective=e((H, W), torch.int32), count=e((H, W), torch.int32),
                                 grad_image=e((H, W, 3)), mag_image=e((H, W, 2)),
                                 loss_temp=torch.zeros((temp_bytes + 15) // 16 * 16, dtype=torch.uint8, device=dev),
-                                temp_bytes=temp_bytes)
+                                temp_bytes=temp_bytes, grad_depth=e((H, W)), grad_alpha=e((H, W)),
+                                sup_temp=torch.zeros((sup_bytes + 15) // 16 * 16, dtype=torch.uint8, device=dev),
+                                sup_bytes=sup_bytes)
             self._res[key] = b
         return b
 
@@ -93,11 +110,28 @@ class FusedTrainStep:
 
     # ------------------------------------------------------------------ one iteration
     def run(self, image_gt: torch.Tensor, q_pointcloud_camera: torch.Tensor, t_pointcloud_camera: torch.Tensor, camera_info,
-            color_max_sh_band: int, feature_learning_rate: float, position_learning_rate: float) -> None:
+            color_max_sh_band: int, feature_learning_rate: float, position_learning_rate: float,
+            targets: Optional[SupervisionTargets] = None, background: Optional[torch.Tensor] = None) -> None:
+        """``targets``: the view's depth and / or mask target ((H, W) float32 CUDA tensors); ``background``: a (3,) float32
+        CUDA tensor the image is composited on (read on the device when the step runs, so it may be refilled per iteration).
+        Without supervision terms this is ``gsb200_train_step``; with them ``gsb200_train_step_aux``."""
         sc, cfg = self.scene, self.config
         H, W = int(camera_info.camera_height), int(camera_info.camera_width)
         if image_gt.shape != (3, H, W) or not image_gt.is_contiguous() or image_gt.dtype != torch.float32:
             raise ValueError(f"image_gt must be a contiguous float32 (3, {H}, {W}) tensor")
+        targets = targets or SupervisionTargets()
+        depth_t = targets.depth if self.depth_weight > 0 else None
+        mask_t = targets.mask if (self.mask_weight > 0 or background is not None) else None
+        if self.depth_weight > 0 and depth_t is None:
+            raise ValueError("depth_weight > 0 needs targets.depth")
+        if self.mask_weight > 0 and mask_t is None:
+            raise ValueError("mask_weight > 0 needs targets.mask")
+        for name, x, shape in (("targets.depth", depth_t, (H, W)), ("targets.mask", mask_t, (H, W)),
+                               ("background", background, (3,))):
+            if x is not None and (tuple(x.shape) != shape or not x.is_contiguous() or x.dtype != torch.float32
+                                  or x.device != image_gt.device):
+                raise ValueError(f"{name} must be a contiguous float32 {shape} tensor on {image_gt.device}")
+        supervised = depth_t is not None or self.mask_weight > 0 or background is not None
         self._check_previous()
         q, t = q_pointcloud_camera.contiguous(), t_pointcloud_camera.contiguous()
         K = camera_info.camera_intrinsics.contiguous()
@@ -146,9 +180,19 @@ class FusedTrainStep:
                 position_exp_avg=_ptr(self.position_exp_avg), position_exp_avg_sq=_ptr(self.position_exp_avg_sq),
                 feature_learning_rate=float(feature_learning_rate), position_learning_rate=float(position_learning_rate),
                 beta1=float(self.betas[0]), beta2=float(self.betas[1]), eps=self.eps, step=self.step_count)
-            _lib.check(self._lib.gsb200_train_step(ctypes.byref(args)), "gsb200_train_step")
+            if supervised:
+                sup = _lib.GsbSupervisionArgs(
+                    depth_target=_ptr(depth_t) if depth_t is not None else None,
+                    mask_target=_ptr(mask_t) if mask_t is not None else None,
+                    background=_ptr(background) if background is not None else None, depth_weight=self.depth_weight,
+                    mask_weight=self.mask_weight, grad_depth=_ptr(b.grad_depth), grad_pixel_accumulated_alpha=_ptr(b.grad_alpha),
+                    loss_out3=_ptr(self.supervision_loss), temp=_ptr(b.sup_temp), temp_bytes=b.sup_bytes)
+                _lib.check(self._lib.gsb200_train_step_aux(ctypes.byref(args), ctypes.byref(sup)), "gsb200_train_step_aux")
+            else:
+                _lib.check(self._lib.gsb200_train_step(ctypes.byref(args)), "gsb200_train_step")
         self._pending[slot] = True
-        self._last = SimpleNamespace(buffers=b, H=H, W=W, slot=slot, keep=(q, t, K, image_gt))
+        self._last = SimpleNamespace(buffers=b, H=H, W=W, slot=slot, supervised=supervised,
+                                     keep=(q, t, K, image_gt, depth_t, mask_t, background))
 
     # ------------------------------------------------------------------ the latest frame, on demand (these calls wait)
     @property

@@ -11,6 +11,11 @@ a JSON list of records with ``image_path``, ``T_pointcloud_camera`` (4x4, camera
 * frames with a side above ``MAX_RESOLUTION_TRAIN`` are resized (shorter side 1024, longer side capped at 1600,
   antialiased), cropped again and their fx, fy, cx, cy scaled (:41-66).
 Records are parsed with ``json`` (no pandas needed); relative image paths are resolved against the JSON file.
+With ``with_targets=True`` (an extension) items get a fifth element, ``loss.SupervisionTargets``, from the optional record
+keys ``depth_path`` (``.npy`` float32 (H, W) at the resolution of the image on disk, point-cloud units along the optical
+axis, 0 or NaN = no measurement) and ``mask_path`` (any image: its last channel / 255, so the alpha of an RGBA file or a
+grey mask), cropped and autoscaled with the image: the mask with the image's antialiased resize, the depth with nearest
+neighbour so that a sparse map stays sparse.
 Pinned against the reference class itself: ``tests/golden/make_dataset_golden.py`` imports it (Taichi stubbed) and
 stores its outputs for a small generated dataset; ``tests/test_dataset_cpu.py`` compares.
 """
@@ -24,6 +29,7 @@ import torch.utils.data
 
 from .Camera import CameraInfo
 from .GaussianPointCloudRasterisation import TILE_HEIGHT, TILE_WIDTH
+from .loss import SupervisionTargets
 from .utils import SE3_to_quaternion_and_translation_torch
 
 MAX_RESOLUTION_TRAIN = 1600
@@ -47,8 +53,9 @@ def _load_image(path: str) -> torch.Tensor:
 
 
 class ImagePoseDataset(torch.utils.data.Dataset):
-    def __init__(self, dataset_json_path: str):
+    def __init__(self, dataset_json_path: str, with_targets: bool = False):
         super().__init__()
+        self.with_targets = bool(with_targets)
         with open(dataset_json_path) as f:
             self.records: List[dict] = json.load(f)
         self.root = os.path.dirname(os.path.abspath(dataset_json_path))
@@ -76,11 +83,47 @@ class ImagePoseDataset(torch.utils.data.Dataset):
         return resized, CameraInfo(camera_intrinsics=K, camera_height=resized.shape[1], camera_width=resized.shape[2],
                                    camera_id=camera_info.camera_id)
 
-    def __getitem__(self, idx: int):
-        rec = self.records[idx]
-        path = rec["image_path"]
+    def _path(self, path: str) -> str:
         if not os.path.isabs(path) and not os.path.exists(path):
             path = os.path.join(self.root, path)
+        return path
+
+    def _load_targets(self, rec: dict, height: int, width: int) -> Tuple[torch.Tensor, torch.Tensor]:
+        """(depth, mask), each (H, W) float32 at the resolution of the image on disk, or None."""
+        depth = mask = None
+        if rec.get("depth_path"):
+            depth = torch.from_numpy(np.ascontiguousarray(np.load(self._path(rec["depth_path"])), dtype=np.float32))
+            if tuple(depth.shape) != (height, width):
+                raise ValueError(f"{rec['depth_path']}: depth map is {tuple(depth.shape)}, the image is {(height, width)}")
+        if rec.get("mask_path"):
+            m = _load_image(self._path(rec["mask_path"]))
+            mask = m[-1].contiguous()
+            if tuple(mask.shape) != (height, width):
+                raise ValueError(f"{rec['mask_path']}: mask is {tuple(mask.shape)}, the image is {(height, width)}")
+        return depth, mask
+
+    def _crop_and_scale_targets(self, depth, mask, info: CameraInfo) -> SupervisionTargets:
+        """The targets cropped to the tile multiple and, if the image was autoscaled, resized to its size."""
+        out = []
+        for x, nearest in ((depth, True), (mask, False)):
+            if x is not None:
+                x = _crop_to_tiles(x[None])[0]
+                if max(x.shape[0], x.shape[1]) > MAX_RESOLUTION_TRAIN:
+                    import torchvision.transforms.functional as TF
+                    mode = TF.InterpolationMode.NEAREST if nearest else TF.InterpolationMode.BILINEAR
+                    x = TF.resize(x[None], size=1024, max_size=MAX_RESOLUTION_TRAIN, interpolation=mode,
+                                  antialias=not nearest)
+                    x = _crop_to_tiles(x)[0]
+                if tuple(x.shape) != (info.camera_height, info.camera_width):
+                    raise ValueError(f"target size {tuple(x.shape)} does not match the image's "
+                                     f"{(info.camera_height, info.camera_width)}")
+                x = x.contiguous()
+            out.append(x)
+        return SupervisionTargets(depth=out[0], mask=out[1])
+
+    def __getitem__(self, idx: int):
+        rec = self.records[idx]
+        path = self._path(rec["image_path"])
         image = _load_image(path)
         T = torch.tensor(rec["T_pointcloud_camera"], dtype=torch.float32).reshape(4, 4)
         q, t = SE3_to_quaternion_and_translation_torch(T.unsqueeze(0))
@@ -88,8 +131,12 @@ class ImagePoseDataset(torch.utils.data.Dataset):
         # the image on disk decides the size, not the recorded (COLMAP) one
         K[0, :] = K[0, :] * image.shape[2] / rec["camera_width"]
         K[1, :] = K[1, :] * image.shape[1] / rec["camera_height"]
+        if self.with_targets:
+            depth, mask = self._load_targets(rec, image.shape[1], image.shape[2])
         image = _crop_to_tiles(image)
         info = CameraInfo(camera_intrinsics=K, camera_height=image.shape[1], camera_width=image.shape[2],
                           camera_id=rec["camera_id"])
         image, info = self._autoscale_image_and_camera_info(image, info)
+        if self.with_targets:
+            return image, q, t, info, self._crop_and_scale_targets(depth, mask, info)
         return image, q, t, info

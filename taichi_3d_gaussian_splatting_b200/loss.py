@@ -9,6 +9,7 @@ sigma = 1.5 applied separably with VALID padding, K1 = 0.01, K2 = 0.03, ``data_r
 the loss, so its parity is unpinned (SURVEY §8(f)-3).
 """
 from dataclasses import dataclass
+from typing import Callable, Optional
 
 import torch
 import torch.nn as nn
@@ -159,6 +160,68 @@ def fused_image_loss(rasterized_image: torch.Tensor, ground_truth_image: torch.T
     """Differentiable form of :func:`fused_image_loss_with_grad`: ``(L, L1, 1 - SSIM)`` as 0-dim tensors, ``L`` carrying
     the gradient to ``rasterized_image`` (one extra scaling kernel in backward)."""
     return _FusedImageLoss.apply(rasterized_image, ground_truth_image, lambda_value)
+
+
+@dataclass
+class SupervisionTargets:
+    """Optional per-view targets besides the image: ``depth`` (H, W) float32 in point-cloud units along the optical axis
+    (0 or NaN = no measurement, e.g. sparse LiDAR) and ``mask`` (H, W) float32 in [0, 1] (1 = object)."""
+    depth: Optional[torch.Tensor] = None
+    mask: Optional[torch.Tensor] = None
+
+
+def _torch_image_loss(rasterized_image, ground_truth_image, lambda_value):
+    """clamp + (1 - lambda) L1 + lambda (1 - SSIM) of the (H, W, 3) image against the (3, H, W) ground truth."""
+    pred = torch.clamp(rasterized_image, min=0, max=1).permute(2, 0, 1)[None]
+    gt = ground_truth_image[None]
+    l1 = torch.abs(pred - gt).mean()
+    ld_ssim = 1 - ssim(pred, gt, data_range=1, size_average=True)
+    return (1 - lambda_value) * l1 + lambda_value * ld_ssim, l1, ld_ssim
+
+
+def supervision_loss(image: torch.Tensor, depth: Optional[torch.Tensor], alpha: Optional[torch.Tensor],
+                     ground_truth_image: torch.Tensor, targets: Optional[SupervisionTargets] = None,
+                     background: Optional[torch.Tensor] = None, lambda_value: float = 0.2, depth_weight: float = 0.0,
+                     mask_weight: float = 0.0, image_loss: Optional[Callable] = None):
+    """The training loss with the optional depth, mask and background terms, for one view (the fused train step,
+    ``gsb200_train_step_aux`` / ``csrc/supervision_loss.cu``, computes the same):
+
+    * background ``bg`` (3,) given: the image loss runs on ``I' = image + (1 - alpha)[..., None] * bg``; with a mask the
+      ground truth is composited as well, ``gt' = gt * m + (1 - m) * bg``; without one it is taken to be on ``bg``;
+    * mask term ``mask_weight * mean |alpha - m|``;
+    * depth term ``depth_weight * sum_valid |depth - d*| / max(n_valid, 1)``, valid where ``d*`` is finite and > 0.
+
+    ``image`` (H, W, 3) unclamped as the rasteriser returns it, ``depth`` / ``alpha`` (H, W) (only needed by the terms that
+    use them), ``ground_truth_image`` (3, H, W).  ``image_loss(I', gt') -> (L, L1, 1 - SSIM)`` defaults to clamp +
+    ``(1 - lambda) L1 + lambda (1 - SSIM)`` in torch.  Returns ``(total, L1, 1 - SSIM, mask term, depth term)``; a term
+    that is off is a zero tensor."""
+    targets = targets or SupervisionTargets()
+    mask = targets.mask
+    gt = ground_truth_image
+    if background is not None:
+        bg = background.to(image.dtype)
+        image = image + (1 - alpha)[..., None] * bg
+        if mask is not None:
+            gt = gt * mask[None] + (1 - mask)[None] * bg[:, None, None]
+    if image_loss is None:
+        loss, l1, ld_ssim = _torch_image_loss(image, gt, lambda_value)
+    else:
+        loss, l1, ld_ssim = image_loss(image, gt)
+    zero = torch.zeros((), dtype=image.dtype, device=image.device)
+    mask_term = depth_term = zero
+    if mask_weight > 0:
+        if mask is None:
+            raise ValueError("mask_weight > 0 needs a mask target")
+        mask_term = mask_weight * torch.abs(alpha - mask).mean()
+    if depth_weight > 0:
+        if targets.depth is None:
+            raise ValueError("depth_weight > 0 needs a depth target")
+        d = targets.depth
+        valid = torch.isfinite(d) & (d > 0)
+        safe = torch.where(valid, d, torch.zeros_like(d))  # no NaN reaches the gradient of the unused branch
+        err = torch.where(valid, torch.abs(depth - safe), torch.zeros_like(d))
+        depth_term = depth_weight * err.sum() / valid.sum().clamp_min(1)
+    return loss + mask_term + depth_term, l1, ld_ssim, mask_term, depth_term
 
 
 class LossFunction(nn.Module):

@@ -7,6 +7,10 @@ optimisers (features / positions, :126-129), exponential decay of the position L
 4 -> 2 -> 1 with the crop-to-16 rule (:98-116, 139-148), SH band schedule ``it // interval`` (:164),
 clamp + HWC->CHW + ``LossFunction`` (:168-175), controller ``refinement`` after the optimiser step (:194).
 TensorBoard logging, the parquet/JSON dataset and validation image dumps are out of scope.
+Optional supervision (an extension; ``TrainConfig.depth_loss_weight`` / ``mask_loss_weight`` / ``background``, per-view
+``SupervisionTargets`` as a fifth view element): a masked-L1 depth loss, an L1 mask loss on the accumulated alpha and
+training on a white or random background, with the same loss (``loss.supervision_loss``) in the autograd loop and in the
+fused step.
 The rasteriser is injected (default: the CUDA operator) so that tests can run the identical loop with the
 CPU oracle behind the same interface and compare PSNR trajectories.
 """
@@ -20,9 +24,11 @@ import torch.nn.functional as F
 from .Camera import CameraInfo
 from .densification import GaussianPointAdaptiveController
 from .GaussianPointCloudRasterisation import GaussianPointCloudRasterisation
-from .loss import LossFunction
+from .loss import LossFunction, SupervisionTargets, supervision_loss
 
 View = Tuple[torch.Tensor, torch.Tensor, torch.Tensor, CameraInfo]  # image (3,H,W) in [0,1], q (1,4), t (1,3), camera
+# ... optionally followed by a SupervisionTargets (depth and / or mask at the image's resolution)
+BACKGROUNDS = ("black", "white", "random")
 
 
 def psnr(pred: torch.Tensor, target: torch.Tensor) -> float:
@@ -44,6 +50,21 @@ def downsample_image_and_camera_info(image: torch.Tensor, camera_info: CameraInf
     K[0, 2] /= downsample_factor
     K[1, 2] /= downsample_factor
     return image, CameraInfo(camera_intrinsics=K, camera_height=h, camera_width=w, camera_id=camera_info.camera_id)
+
+
+def downsample_targets(targets: SupervisionTargets, camera_info: CameraInfo, downsample_factor: int) -> SupervisionTargets:
+    """The targets of a view at the schedule's resolution: the mask with the image's antialiased resize, the depth with
+    nearest neighbour (a sparse map stays sparse, no depth is blended across an edge); both cropped like the image."""
+    h = camera_info.camera_height // downsample_factor
+    w = camera_info.camera_width // downsample_factor
+    hc, wc = h - h % 16, w - w % 16
+    mask = depth = None
+    if targets.mask is not None:
+        mask = F.interpolate(targets.mask[None, None], size=(h, w), mode="bilinear", antialias=True,
+                             align_corners=False)[0, 0, :hc, :wc].contiguous()
+    if targets.depth is not None:
+        depth = F.interpolate(targets.depth[None, None], size=(h, w), mode="nearest")[0, 0, :hc, :wc].contiguous()
+    return SupervisionTargets(depth=depth, mask=mask)
 
 
 @dataclass
@@ -73,11 +94,18 @@ class GaussianPointCloudTrainer:
             default_factory=GaussianPointAdaptiveController.GaussianPointAdaptiveControllerConfig)
         loss_function_config: LossFunction.LossFunctionConfig = field(
             default_factory=LossFunction.LossFunctionConfig)
+        # optional supervision (loss.supervision_loss): weights of the masked-L1 depth term and of the L1 mask term on the
+        # accumulated alpha, and the background the image is composited on ("black" = none, "white", or "random": one
+        # colour per iteration, which needs a mask on every view)
+        depth_loss_weight: float = 0.
+        mask_loss_weight: float = 0.
+        background: str = "black"
 
     def __init__(self, config: "GaussianPointCloudTrainer.TrainConfig", scene: Scene, train_views: List[View],
                  rasterisation_factory: Optional[Callable] = None, generator: Optional[torch.Generator] = None,
                  fused_image_loss: bool = False, fused_adam: bool = False, fused_controller_update: bool = False,
-                 fused_step: bool = False, shuffle_generator: Optional[torch.Generator] = None):
+                 fused_step: bool = False, shuffle_generator: Optional[torch.Generator] = None,
+                 background_generator: Optional[torch.Generator] = None):
         """``fused_image_loss``: clamp + L1 + D-SSIM and their gradient in two CUDA kernels (``gsb200_image_loss``)
         instead of ~60 autograd kernels per step; same loss values (CUDA only).  ``fused_adam``: the two Adam updates as
         one kernel each (``optim.FusedAdam`` / ``gsb200_adam_step``) instead of torch's foreach path (CUDA only).
@@ -86,8 +114,32 @@ class GaussianPointCloudTrainer:
         ``fused_step``: the WHOLE iteration as one library call (``gsb200_train_step``: forward, image loss, backward with the
         controller accumulators fused into its epilogue, both Adam updates; no autograd, no host wait; CUDA only).
         ``shuffle_generator``: a CPU ``torch.Generator``; the views are then visited in a fresh random permutation per
-        epoch like the reference's shuffling DataLoader (GaussianPointTrainer.py:120-124) instead of in fixed order."""
+        epoch like the reference's shuffling DataLoader (GaussianPointTrainer.py:120-124) instead of in fixed order.
+        ``background_generator``: a generator on the scene's device; with ``background="random"`` it draws the colour of
+        each iteration on the device (no host wait; the autograd loop and the fused step draw the same colours)."""
+        if config.background not in BACKGROUNDS:
+            raise ValueError(f"background must be one of {BACKGROUNDS}, got {config.background!r}")
+        for name in ("depth_loss_weight", "mask_loss_weight"):
+            w = getattr(config, name)
+            if not (w >= 0.0 and w < float("inf")):
+                raise ValueError(f"{name} must be finite and >= 0, got {w}")
+        targets = [v[4] if len(v) > 4 and v[4] is not None else SupervisionTargets() for v in train_views]
+        if config.depth_loss_weight > 0 and any(tg.depth is None for tg in targets):
+            raise ValueError("depth_loss_weight > 0 needs a depth target on every view")
+        if config.mask_loss_weight > 0 and any(tg.mask is None for tg in targets):
+            raise ValueError("mask_loss_weight > 0 needs a mask on every view")
+        if config.background == "random" and any(tg.mask is None for tg in targets):
+            raise ValueError('background="random" needs a mask on every view (the ground truth is composited by it)')
         self.config = config
+        self._need_depth = config.depth_loss_weight > 0
+        self._need_alpha = config.mask_loss_weight > 0 or config.background != "black"
+        self.supervised = self._need_depth or self._need_alpha
+        self._background_generator = background_generator
+        self._background = None
+        if config.background == "white":
+            self._background = torch.ones(3, dtype=torch.float32, device=scene.point_cloud.device)
+        elif config.background == "random":
+            self._background = torch.empty(3, dtype=torch.float32, device=scene.point_cloud.device)
         self.fused_step = fused_step
         if fused_step and config.loss_function_config.enable_regularization:
             raise ValueError("fused_step does not implement the optional scale regulariser (LossFunction.py:33-37)")
@@ -102,8 +154,11 @@ class GaussianPointCloudTrainer:
                 point_invalid_mask=scene.point_invalid_mask, point_object_id=scene.point_object_id),
             generator=generator, fused_update=fused_controller_update)
         factory = rasterisation_factory or GaussianPointCloudRasterisation
+        # the differentiable outputs only when a term needs them: injected factories without them keep working
+        extra = dict(**({"differentiable_depth": True} if self._need_depth else {}),
+                     **({"differentiable_alpha": True} if self._need_alpha else {}))
         self.rasterisation = factory(config=config.rasterisation_config,
-                                     backward_valid_point_hook=self.adaptive_controller.update)
+                                     backward_valid_point_hook=self.adaptive_controller.update, **extra)
         self.loss_function = LossFunction(config=config.loss_function_config)
         self.history: List[dict] = []
         self._downsampled = {}
@@ -117,13 +172,43 @@ class GaussianPointCloudTrainer:
             point_object_id=s.point_object_id, point_invalid_mask=s.point_invalid_mask,
             camera_info=camera_info, q_pointcloud_camera=q, t_pointcloud_camera=t, color_max_sh_band=band)
 
+    def _view(self, view_index: int, downsample_factor: int):
+        """(image, q, t, camera, targets) of a view at the schedule's resolution; resized once per (view, factor)."""
+        view = self.train_views[view_index]
+        image_gt, q, t, camera_info = view[:4]
+        targets = view[4] if len(view) > 4 and view[4] is not None else SupervisionTargets()
+        if downsample_factor > 1:
+            # the reference resizes the full-resolution frame in every iteration (GaussianPointTrainer.py:146-148); the
+            # result depends only on (view, factor), so it is computed once per pair (same tensors, ~10 launches less)
+            key = (view_index, downsample_factor)
+            if key not in self._downsampled:
+                image_ds, camera_ds = downsample_image_and_camera_info(image_gt, camera_info, downsample_factor)
+                self._downsampled[key] = (image_ds, camera_ds, downsample_targets(targets, camera_info, downsample_factor)
+                                          if self.supervised else targets)
+            image_gt, camera_info, targets = self._downsampled[key]
+        return image_gt, q, t, camera_info, targets
+
+    def _next_background(self) -> Optional[torch.Tensor]:
+        """The background of this iteration: None (black), white, or a fresh colour drawn on the device."""
+        if self.config.background == "random":
+            torch.rand(3, generator=self._background_generator, out=self._background)
+        return self._background
+
+    def _supervised_history(self, entry: dict, mask_term, depth_term) -> dict:
+        if self.config.mask_loss_weight > 0:
+            entry["mask_loss"] = float(mask_term)
+        if self.config.depth_loss_weight > 0:
+            entry["depth_loss"] = float(depth_term)
+        return entry
+
     def _train_fused(self, log_interval: int = 0):
         """The loop of ``train`` with the whole iteration enqueued by ONE library call (``fused_step.FusedTrainStep``):
         no autograd graph, no host wait, the controller's accumulators updated inside the backward kernel."""
         from .fused_step import FusedTrainStep
         cfg = self.config
         step = FusedTrainStep(self.scene, cfg.rasterisation_config, cfg.loss_function_config.lambda_value,
-                              controller=self.adaptive_controller)
+                              controller=self.adaptive_controller, depth_weight=cfg.depth_loss_weight,
+                              mask_weight=cfg.mask_loss_weight)
         self.fused_train_step = step
         position_lr = cfg.position_learning_rate
         downsample_factor = cfg.initial_downsample_factor
@@ -131,23 +216,27 @@ class GaussianPointCloudTrainer:
             if iteration % cfg.half_downsample_factor_interval == 0 and iteration > 0 and downsample_factor > 1:
                 downsample_factor //= 2
             view_index = self._next_view_index(iteration)
-            image_gt, q, t, camera_info = self.train_views[view_index]
-            if downsample_factor > 1:
-                key = (view_index, downsample_factor)
-                if key not in self._downsampled:
-                    self._downsampled[key] = downsample_image_and_camera_info(image_gt, camera_info, downsample_factor)
-                image_gt, camera_info = self._downsampled[key]
+            image_gt, q, t, camera_info, targets = self._view(view_index, downsample_factor)
             band = iteration // cfg.increase_color_max_sh_band_interval
-            step.run(image_gt, q, t, camera_info, band, cfg.feature_learning_rate, position_lr)
+            if self.supervised:
+                step.run(image_gt, q, t, camera_info, band, cfg.feature_learning_rate, position_lr, targets=targets,
+                         background=self._next_background())
+            else:
+                step.run(image_gt, q, t, camera_info, band, cfg.feature_learning_rate, position_lr)
             if iteration % cfg.position_learning_rate_decay_interval == 0:  # ExponentialLR.step() after the optimiser step
                 position_lr *= cfg.position_learning_rate_decay_rate
             self.adaptive_controller.after_fused_update(step.hook_input)
             self.adaptive_controller.refinement()
             if log_interval and iteration % log_interval == 0:
                 losses = step.loss.tolist()
-                self.history.append(dict(iteration=iteration, loss=losses[0], l1=losses[1],
-                                         psnr=psnr(step.image.detach().clamp(0, 1).permute(2, 0, 1), image_gt),
-                                         num_valid_points=int((self.scene.point_invalid_mask == 0).sum())))
+                entry = dict(iteration=iteration, loss=losses[0], l1=losses[1],
+                             psnr=psnr(step.image.detach().clamp(0, 1).permute(2, 0, 1), image_gt),
+                             num_valid_points=int((self.scene.point_invalid_mask == 0).sum()))
+                if self.supervised:
+                    total, mask_term, depth_term = step.supervision_loss.tolist()
+                    entry["loss"] = total
+                    self._supervised_history(entry, mask_term, depth_term)
+                self.history.append(entry)
         return self.history
 
     def _next_view_index(self, iteration: int) -> int:
@@ -180,22 +269,19 @@ class GaussianPointCloudTrainer:
             optimizer.zero_grad()
             position_optimizer.zero_grad()
             view_index = self._next_view_index(iteration)
-            image_gt, q, t, camera_info = self.train_views[view_index]
-            if downsample_factor > 1:
-                # the reference resizes the full-resolution frame in every iteration (GaussianPointTrainer.py:146-148); the
-                # result depends only on (view, factor), so it is computed once per pair (same tensors, ~10 launches less)
-                key = (view_index, downsample_factor)
-                if key not in self._downsampled:
-                    self._downsampled[key] = downsample_image_and_camera_info(image_gt, camera_info, downsample_factor)
-                image_gt, camera_info = self._downsampled[key]
+            image_gt, q, t, camera_info, targets = self._view(view_index, downsample_factor)
             band = iteration // cfg.increase_color_max_sh_band_interval
-            image_pred, _, _ = self.rasterisation(self._input(q, t, camera_info, band))
-            if self.fused_image_loss:
+            if self.supervised:
+                loss, l1_loss, mask_term, depth_term, image_pred = self._supervised_loss(q, t, camera_info, band, image_gt,
+                                                                                         targets)
+            elif self.fused_image_loss:
+                image_pred, _, _ = self.rasterisation(self._input(q, t, camera_info, band))
                 loss, l1_loss, ssim_loss = self.loss_function.forward_rasterized(
                     image_pred, image_gt, point_invalid_mask=self.scene.point_invalid_mask,
                     pointcloud_features=self.scene.point_cloud_features)
                 image_pred = image_pred.detach().clamp(0, 1).permute(2, 0, 1) if log_interval else image_pred
             else:
+                image_pred, _, _ = self.rasterisation(self._input(q, t, camera_info, band))
                 image_pred = torch.clamp(image_pred, min=0, max=1).permute(2, 0, 1)
                 loss, l1_loss, ssim_loss = self.loss_function(
                     image_pred, image_gt, point_invalid_mask=self.scene.point_invalid_mask,
@@ -207,17 +293,49 @@ class GaussianPointCloudTrainer:
                 scheduler.step()
             self.adaptive_controller.refinement()
             if log_interval and iteration % log_interval == 0:
-                self.history.append(dict(iteration=iteration, loss=float(loss.detach()), l1=float(l1_loss.detach()),
-                                         psnr=psnr(image_pred.detach(), image_gt),
-                                         num_valid_points=int((self.scene.point_invalid_mask == 0).sum())))
+                entry = dict(iteration=iteration, loss=float(loss.detach()), l1=float(l1_loss.detach()),
+                             psnr=psnr(image_pred.detach(), image_gt),
+                             num_valid_points=int((self.scene.point_invalid_mask == 0).sum()))
+                if self.supervised:
+                    self._supervised_history(entry, mask_term.detach(), depth_term.detach())
+                self.history.append(entry)
         return self.history
+
+    def _supervised_loss(self, q, t, camera_info, band, image_gt, targets):
+        """Forward with the differentiable outputs the terms need, then ``loss.supervision_loss`` with this trainer's image
+        loss (the torch one, or the fused kernels with ``fused_image_loss``; the scale regulariser if enabled).  Returns
+        (total, L1, mask term, depth term, the raw image as (3, H, W) for the PSNR log)."""
+        cfg = self.config
+        outs = self.rasterisation(self._input(q, t, camera_info, band))
+        image_pred, depth = outs[0], outs[1]
+        alpha = outs[3] if self._need_alpha else None
+        regulariser = dict(point_invalid_mask=self.scene.point_invalid_mask, pointcloud_features=self.scene.point_cloud_features)
+        if self.fused_image_loss:
+            image_loss = lambda pred, gt: self.loss_function.forward_rasterized(pred, gt, **regulariser)  # noqa: E731
+        else:
+            image_loss = lambda pred, gt: self.loss_function(  # noqa: E731
+                torch.clamp(pred, min=0, max=1).permute(2, 0, 1), gt, **regulariser)
+        total, l1, _, mask_term, depth_term = supervision_loss(
+            image_pred, depth, alpha, image_gt, targets, self._next_background(), cfg.loss_function_config.lambda_value,
+            cfg.depth_loss_weight, cfg.mask_loss_weight, image_loss=image_loss)
+        return total, l1, mask_term, depth_term, image_pred.detach().clamp(0, 1).permute(2, 0, 1)
 
     @torch.no_grad()
     def validation(self, views: Optional[List[View]] = None) -> float:
         """Mean PSNR over the views at full resolution (GaussianPointTrainer.py:334-415 without the logging)."""
         views = views if views is not None else self.train_views
         total = 0.0
-        for image_gt, q, t, camera_info in views:
-            image_pred, _, _ = self.rasterisation(self._input(q, t, camera_info, 3))
+        for view in views:
+            image_gt, q, t, camera_info = view[:4]
+            outs = self.rasterisation(self._input(q, t, camera_info, 3))
+            image_pred = outs[0]
+            if self.config.background != "black":
+                # white: the prediction on white and the ground truth composited by its mask; random: both on black
+                bg = 1.0 if self.config.background == "white" else 0.0
+                if bg:
+                    image_pred = image_pred + (1 - outs[3])[..., None] * bg
+                mask = view[4].mask if len(view) > 4 and view[4] is not None else None
+                if mask is not None:
+                    image_gt = image_gt * mask[None] + (1 - mask)[None] * bg
             total += psnr(image_pred.permute(2, 0, 1), image_gt)
         return total / max(len(views), 1)
