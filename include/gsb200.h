@@ -205,7 +205,7 @@ const char *gsb200_last_error(void);
  * foreign-language binding verify its struct mirrors. */
 void gsb200_abi_sizes(int64_t *out3);
 /* ... and of the first n of {GsbWorkspaceLayout, GsbForwardArgs, GsbBackwardArgs, GsbExpandArgs, GsbTrainStepArgs,
- * GsbSupervisionArgs} */
+ * GsbSupervisionArgs, GsbExtraFeatureArgs} */
 void gsb200_abi_sizes_ext(int64_t *out, int32_t n);
 
 /* Workspace sizing.  far_plane*depth_to_sort_key_scale fixes the depth-key width; (H/16)*(W/16)
@@ -253,6 +253,40 @@ int gsb200_backward_aux(const GsbBackwardArgs *args,
                         const float *grad_rasterized_depth,         /* (H,W) f32, device, or NULL */
                         const float *rasterized_depth,              /* (H,W) f32: this frame's forward output, or NULL */
                         const float *grad_pixel_accumulated_alpha); /* (H,W) f32, device, or NULL */
+
+/* Per-Gaussian feature vectors rendered and differentiated alongside the image (an extension: the reference blends the SH
+ * colour alone).  C values per Gaussian, chosen by the caller (semantic logits, instance encodings, distilled features),
+ * are blended with exactly the image's weights w_i = alpha_i T_i -- the 1/255 cut, the 0.99 clamp and the 1e-4 stop
+ * included -- into F_p = sum_i w_i f_i: no normalisation, no background, no activation.  Rows of invalid or out-of-frustum
+ * points never contribute.  All pointers are device memory, rows contiguous. */
+typedef struct GsbExtraFeatureArgs {
+    int32_t channels;              /* C, 1..16 */
+    const float *features;         /* (N,C) f32, indexed by scene row like pointcloud */
+    float *rasterized;             /* (H,W,C) f32: forward output */
+    const float *grad_rasterized;  /* (H,W,C) f32: backward input dL/dF */
+    float *grad_features;          /* (N,C) f32: backward output dL/df, fully written (zero for rows outside the frustum);
+                                      16-byte aligned */
+} GsbExtraFeatureArgs;
+
+/* gsb200_forward that also blends the feature vectors of `ext` into ext->rasterized (features / rasterized must be set;
+ * grad_* are not read).  NULL ext: exactly gsb200_forward (which is this call with NULL).  GSB_EINVAL, before any CUDA call,
+ * for channels outside 1..16, a NULL features / rasterized pointer or rgb_only.  Every other output of the frame is
+ * bit-identical to gsb200_forward's on the default arithmetic. */
+int gsb200_forward_ext(const GsbForwardArgs *args, const GsbExtraFeatureArgs *ext);
+
+/* gsb200_backward_aux that also back-propagates the feature map's gradient ext->grad_rasterized: dL/df_i = sum_p w_{p,i}
+ * dL/dF_p into ext->grad_features (zeroed by the call, no gradient factor), and the feature loss's share of dL/dalpha into
+ * uv, conic and opacity -- and from there into the hook statistics and the controller accumulators -- exactly as the image
+ * loss's share.  In the backward each feature channel is one more colour channel of the blend.  NULL ext: exactly
+ * gsb200_backward_aux (which is this call with NULL).  With ext, before any CUDA call: GSB_EINVAL for channels outside 1..16
+ * or a NULL features / grad_rasterized / grad_features pointer; GSB_EUNSUPPORTED without GSB_FLAG_BACKWARD_TRANSPOSED
+ * (the butterfly kernel does not implement it) or with GSB_FLAG_COMPACT_GRADS (the view-parallel exchange does not carry
+ * the feature rows).  ext->features must be the rows the forward of this frame blended. */
+int gsb200_backward_ext(const GsbBackwardArgs *args,
+                        const float *grad_rasterized_depth,          /* as gsb200_backward_aux */
+                        const float *rasterized_depth,
+                        const float *grad_pixel_accumulated_alpha,
+                        const GsbExtraFeatureArgs *ext);             /* or NULL */
 
 int gsb200_expand_view_gradients(const GsbExpandArgs *args);
 

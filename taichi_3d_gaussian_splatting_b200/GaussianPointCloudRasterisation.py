@@ -300,32 +300,38 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
 
             @staticmethod
             def forward(ctx, pointcloud, pointcloud_features, point_invalid_mask, point_object_id,
-                        q_pointcloud_camera, t_pointcloud_camera, camera_info, color_max_sh_band):
+                        q_pointcloud_camera, t_pointcloud_camera, camera_info, color_max_sh_band, extra_features=None):
                 outs, frame, saved = outer._run_forward(
                     pointcloud, pointcloud_features, point_invalid_mask, point_object_id,
-                    q_pointcloud_camera, t_pointcloud_camera, camera_info)
-                image, depth, acc_alpha, last_effective, valid_count = outs
+                    q_pointcloud_camera, t_pointcloud_camera, camera_info, extra_features)
+                image, depth, acc_alpha, last_effective, valid_count = outs[:5]
                 ctx.save_for_backward(pointcloud, pointcloud_features, point_object_id,
                                       t_pointcloud_camera, saved["camera_intrinsics"], acc_alpha,
-                                      last_effective, frame.ws, *((depth,) if outer.differentiable_depth else ()))
+                                      last_effective, frame.ws, *((depth,) if outer.differentiable_depth else ()),
+                                      *((extra_features,) if extra_features is not None else ()))
                 ctx.frame = frame
                 ctx.num_objects = q_pointcloud_camera.shape[0]
                 ctx.color_max_sh_band = color_max_sh_band
+                ctx.has_extra_features = extra_features is not None
                 if outer.differentiable_depth:
                     ctx.mark_non_differentiable(valid_count)
                 else:
                     ctx.mark_non_differentiable(depth, valid_count)
-                if outer.differentiable_depth or outer.differentiable_alpha:
+                if outer.differentiable_depth or outer.differentiable_alpha or extra_features is not None:
                     ctx.set_materialize_grads(False)  # None tells an unused output from a zero gradient
-                if outer.differentiable_alpha:
-                    return image, depth, valid_count, acc_alpha
-                return image, depth, valid_count
+                result = (image, depth, valid_count) + ((acc_alpha,) if outer.differentiable_alpha else ())
+                if extra_features is not None:
+                    result = result + (outs[5],)
+                return result
 
             @staticmethod
-            def backward(ctx, grad_rasterized_image, grad_rasterized_depth, grad_pixel_valid_point_count,
-                         grad_pixel_accumulated_alpha=None):
-                grad_pointcloud = grad_pointcloud_features = None
-                if ctx.needs_input_grad[0] or ctx.needs_input_grad[1]:  # GPCR:1028
+            def backward(ctx, grad_rasterized_image, grad_rasterized_depth, grad_pixel_valid_point_count, *grad_extra):
+                # grad_extra: dL/d pixel_accumulated_alpha (differentiable_alpha), then dL/d the feature map (extra features)
+                grad_pixel_accumulated_alpha = grad_extra[0] if outer.differentiable_alpha else None
+                grad_feature_map = grad_extra[-1] if ctx.has_extra_features else None
+                grad_pointcloud = grad_pointcloud_features = grad_extra_features = None
+                # GPCR:1028; with extra features the backward also runs for them alone (frozen geometry)
+                if ctx.needs_input_grad[0] or ctx.needs_input_grad[1] or (ctx.has_extra_features and ctx.needs_input_grad[8]):
                     if outer.config.rgb_only:
                         # the reference leaves accumulated alpha / last-effective offsets uninitialised in
                         # this mode (GPCR:478-484), so its backward is undefined; refuse instead
@@ -335,9 +341,12 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                         frame = ctx.frame
                         grad_rasterized_image = torch.zeros((frame.height, frame.width, 3), dtype=torch.float32,
                                                             device=frame.ws.device)
-                    grad_pointcloud, grad_pointcloud_features = outer._run_backward(ctx, grad_rasterized_image,
-                                                                                    grad_rasterized_depth,
-                                                                                    grad_pixel_accumulated_alpha)
+                    grad_pointcloud, grad_pointcloud_features, grad_extra_features = outer._run_backward(
+                        ctx, grad_rasterized_image, grad_rasterized_depth, grad_pixel_accumulated_alpha, grad_feature_map)
+                if ctx.has_extra_features:  # frozen geometry: None for the scene tensors that do not need a gradient
+                    return (grad_pointcloud if ctx.needs_input_grad[0] else None,
+                            grad_pointcloud_features if ctx.needs_input_grad[1] else None, None, None, None, None, None, None,
+                            grad_extra_features if ctx.needs_input_grad[8] else None)
                 return grad_pointcloud, grad_pointcloud_features, None, None, None, None, None, None
 
         self._module_function = _module_function
@@ -357,8 +366,31 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
             self._layout_cache[key] = cached
         return cached
 
+    def _check_extra_features(self, extra_features, pointcloud):
+        """The ``point_extra_features`` argument of ``forward``: (N, C) float32, contiguous, on the scene's device, 1 <= C <= 16,
+        and an operator that can differentiate it."""
+        if self.backward_impl == "butterfly":
+            raise ValueError("point_extra_features needs backward_impl='transposed': the butterfly kernel implements only the "
+                             "image gradient")
+        if self.config.rgb_only:
+            raise ValueError("point_extra_features needs the full forward: config.rgb_only=True renders only the image")
+        if self.gradient_exchange is not None:
+            raise ValueError("point_extra_features is not supported with a gradient_exchange (view-parallel training)")
+        if not isinstance(extra_features, torch.Tensor):
+            raise ValueError("point_extra_features must be a torch.Tensor")
+        N = pointcloud.shape[0]
+        if extra_features.dim() != 2 or extra_features.shape[0] != N or not 1 <= extra_features.shape[1] <= 16:
+            raise ValueError(f"point_extra_features must be (N, C) with N = {N} and 1 <= C <= 16, got "
+                             f"{tuple(extra_features.shape)}")
+        if extra_features.dtype != torch.float32:
+            raise ValueError(f"point_extra_features must be float32, got {extra_features.dtype}")
+        if extra_features.device != pointcloud.device:
+            raise ValueError(f"point_extra_features must be on {pointcloud.device}, got {extra_features.device}")
+        if not extra_features.is_contiguous():
+            raise ValueError("point_extra_features must be contiguous")
+
     def _run_forward(self, pointcloud, pointcloud_features, point_invalid_mask, point_object_id,
-                     q_pointcloud_camera, t_pointcloud_camera, camera_info):
+                     q_pointcloud_camera, t_pointcloud_camera, camera_info, extra_features=None):
         cfg = self.config
         lib = _lib.load()
         _require(pointcloud, "point_cloud", torch.float32, (3,))
@@ -396,6 +428,11 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                 acc_alpha = torch.empty((H, W), dtype=torch.float32, device=device)
                 last_effective = torch.empty((H, W), dtype=torch.int32, device=device)
                 valid_count = torch.empty((H, W), dtype=torch.int32, device=device)
+            feature_map = ext = None
+            if extra_features is not None:
+                C = extra_features.shape[1]
+                feature_map = torch.empty((H, W, C), dtype=torch.float32, device=device)
+                ext = _lib.GsbExtraFeatureArgs(channels=C, features=_ptr(extra_features), rasterized=_ptr(feature_map))
             readback = _PinnedCounters.acquire(device)
             pinned, event = readback
             retry_flag = 0
@@ -419,7 +456,10 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                         host_counters=pinned.data_ptr(), host_counters_event=event.cuda_event)
                     # The whole frame is enqueued by this one call; the library copies {M, K, overflow} to pinned
                     # host memory right after the per-point stage and records `event` behind that copy.
-                    _lib.check(lib.gsb200_forward(ctypes.byref(args)), "gsb200_forward")
+                    if ext is None:
+                        _lib.check(lib.gsb200_forward(ctypes.byref(args)), "gsb200_forward")
+                    else:  # the re-run after an overflow renders the feature map as well
+                        _lib.check(lib.gsb200_forward_ext(ctypes.byref(args), ctypes.byref(ext)), "gsb200_forward_ext")
                     frame = Frame(ws, layout, N, key_capacity, H, W, self._flags)
                     # ONE host wait per frame (the reference syncs twice, GPCR:864 and GPCR:916-931), and it ends
                     # when the first kernel is done: sort + blend are still in flight when we return.
@@ -435,10 +475,14 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
             finally:  # also when the library call raises: the pooled pair goes back
                 _PinnedCounters.release(device, readback)
         self.last_frame = frame
-        return (image, depth, acc_alpha, last_effective, valid_count), frame, {"camera_intrinsics": K}
+        outs = (image, depth, acc_alpha, last_effective, valid_count) + ((feature_map,) if feature_map is not None else ())
+        return outs, frame, {"camera_intrinsics": K}
 
     # ------------------------------------------------------------------ backward plumbing
-    def _run_backward(self, ctx, grad_rasterized_image, grad_rasterized_depth=None, grad_pixel_accumulated_alpha=None):
+    def _run_backward(self, ctx, grad_rasterized_image, grad_rasterized_depth=None, grad_pixel_accumulated_alpha=None,
+                      grad_feature_map=None):
+        """Returns dL/dxyz, dL/dfeatures and, for a call with extra features, dL/d of them ((N, C); zeros when the feature map
+        was not used)."""
         cfg = self.config
         lib = _lib.load()
         saved = ctx.saved_tensors
@@ -446,6 +490,7 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
          last_effective, ws) = saved[:8]
         # differentiable_depth: the depth gradient (None when the loss does not use depth) and the forward's depth map
         depth = saved[8] if self.differentiable_depth and grad_rasterized_depth is not None else None
+        extra_features = saved[-1] if ctx.has_extra_features else None
         frame: Frame = ctx.frame
         device = pointcloud.device
         N = pointcloud.shape[0]
@@ -497,7 +542,18 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
             grad_depth = _f32(grad_rasterized_depth) if depth is not None else None
             # differentiable_alpha: None when the loss does not use the accumulated alpha
             grad_alpha = _f32(grad_pixel_accumulated_alpha) if self.differentiable_alpha else None
-            if grad_alpha is not None:
+            grad_extra_features = None
+            if extra_features is not None:  # dL/df: written by the call, or zero when the feature map was not used
+                C = extra_features.shape[1]
+                grad_extra_features = torch.zeros((N, C), dtype=torch.float32, device=device) if grad_feature_map is None \
+                    else torch.empty((N, C), dtype=torch.float32, device=device)
+            if extra_features is not None and grad_feature_map is not None:
+                grad_map = _f32(grad_feature_map)
+                ext = _lib.GsbExtraFeatureArgs(channels=extra_features.shape[1], features=_ptr(extra_features),
+                                               grad_rasterized=_ptr(grad_map), grad_features=_ptr(grad_extra_features))
+                _lib.check(lib.gsb200_backward_ext(ctypes.byref(args), _ptr(grad_depth), _ptr(depth), _ptr(grad_alpha),
+                                                   ctypes.byref(ext)), "gsb200_backward_ext")
+            elif grad_alpha is not None:
                 _lib.check(lib.gsb200_backward_aux(ctypes.byref(args), _ptr(grad_depth), _ptr(depth), _ptr(grad_alpha)),
                            "gsb200_backward_aux")
             elif depth is not None:
@@ -543,7 +599,7 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                     point_uv_in_camera=frame.point_uv.contiguous(),
                     point_depth=frame.point_in_camera[:, 2],
                 ))
-        return grad_pointcloud, grad_pointcloud_features
+        return grad_pointcloud, grad_pointcloud_features, grad_extra_features
 
     def backward_flags(self, frame_flags: int) -> int:
         """Flags of the backward call for a frame rendered with ``frame_flags`` (adds the experimental kernel selection)."""
@@ -554,10 +610,27 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
         return frame_flags
 
     # ------------------------------------------------------------------ public forward (GPCR:1184-1204)
-    def forward(self, input_data: "GaussianPointCloudRasterisation.GaussianPointCloudRasterisationInput"):
+    def forward(self, input_data: "GaussianPointCloudRasterisation.GaussianPointCloudRasterisationInput",
+                point_extra_features: Optional[torch.Tensor] = None):
+        """Returns (image, depth, pixel_valid_point_count), then pixel_accumulated_alpha with ``differentiable_alpha``.
+        ``point_extra_features`` (an extension): an (N, C) float32 tensor of per-Gaussian values (1 <= C <= 16; semantic
+        logits, instance encodings, distilled features, ...), contiguous, on the scene's device.  The output tuple then
+        ends with their blend ``F_p = sum_i alpha_i T_i f_i``, (H, W, C) float32, with exactly the image's weights: no
+        normalisation, no background, no activation.  It is differentiable in the features (dL/dF rows of points outside
+        the frustum are zero, no gradient factor) and, through the weights, in xyz, q, s and the opacity, as the image is;
+        the backward runs for the features alone too.  Combines with ``differentiable_depth`` and ``differentiable_alpha``.
+        ``ValueError`` with ``backward_impl="butterfly"``, ``config.rgb_only``, a ``gradient_exchange``, or a tensor of the
+        wrong shape, dtype, device or layout.  The densification controller does not know these rows: a caller who clones,
+        splits or removes Gaussians must keep ``point_extra_features`` in step."""
         camera_info = input_data.camera_info
         assert camera_info.camera_width % TILE_WIDTH == 0
         assert camera_info.camera_height % TILE_HEIGHT == 0
+        if point_extra_features is not None:
+            self._check_extra_features(point_extra_features, input_data.point_cloud)
+            return self._module_function.apply(
+                input_data.point_cloud, input_data.point_cloud_features, input_data.point_invalid_mask,
+                input_data.point_object_id, input_data.q_pointcloud_camera, input_data.t_pointcloud_camera, camera_info,
+                input_data.color_max_sh_band, point_extra_features)
         return self._module_function.apply(
             input_data.point_cloud,
             input_data.point_cloud_features,

@@ -91,6 +91,12 @@ class GsbSupervisionArgs(ctypes.Structure):
     ]
 
 
+class GsbExtraFeatureArgs(ctypes.Structure):
+    _fields_ = [
+        ("channels", c_i32), ("features", c_vp), ("rasterized", c_vp), ("grad_rasterized", c_vp), ("grad_features", c_vp),
+    ]
+
+
 class GsbExpandArgs(ctypes.Structure):
     _fields_ = [
         ("num_points", c_i64), ("num_views", c_i32), ("num_objects", c_i32), ("grad_sum", c_vp),
@@ -108,7 +114,8 @@ EXPORTS = (
     "gsb200_image_loss_temp_bytes", "gsb200_image_loss", "gsb200_adam_step", "gsb200_controller_update",
     "gsb200_forward_blend_work", "gsb200_backward_blend_work", "gsb200_device_selftest", "gsb200_expand_view_gradients",
     "gsb200_train_step", "gsb200_abi_sizes_ext", "gsb200_exchange_multimem", "gsb200_backward_with_depth",
-    "gsb200_backward_aux", "gsb200_supervision_temp_bytes", "gsb200_train_step_aux",
+    "gsb200_backward_aux", "gsb200_supervision_temp_bytes", "gsb200_train_step_aux", "gsb200_forward_ext",
+    "gsb200_backward_ext",
 )
 
 _lib = None
@@ -138,6 +145,10 @@ def load() -> ctypes.CDLL:
     lib.gsb200_backward_with_depth.restype = ctypes.c_int
     lib.gsb200_backward_aux.argtypes = [ctypes.POINTER(GsbBackwardArgs), c_vp, c_vp, c_vp]
     lib.gsb200_backward_aux.restype = ctypes.c_int
+    lib.gsb200_forward_ext.argtypes = [ctypes.POINTER(GsbForwardArgs), ctypes.POINTER(GsbExtraFeatureArgs)]
+    lib.gsb200_forward_ext.restype = ctypes.c_int
+    lib.gsb200_backward_ext.argtypes = [ctypes.POINTER(GsbBackwardArgs), c_vp, c_vp, c_vp, ctypes.POINTER(GsbExtraFeatureArgs)]
+    lib.gsb200_backward_ext.restype = ctypes.c_int
     lib.gsb200_sort_temp_bytes.argtypes = [c_i64, c_i32]
     lib.gsb200_sort_temp_bytes.restype = c_i64
     lib.gsb200_sort_pairs.argtypes = [c_vp, c_vp, c_vp, c_vp, c_i64, c_i32, c_i32, c_vp, c_i64, c_vp]
@@ -203,6 +214,11 @@ def load() -> ctypes.CDLL:
     if sizes6[5] != ctypes.sizeof(GsbSupervisionArgs):
         raise RuntimeError(f"libgsb200.so ABI mismatch: sizeof(GsbSupervisionArgs) {sizes6[5]} != ctypes mirror "
                            f"{ctypes.sizeof(GsbSupervisionArgs)}")
+    sizes7 = (c_i64 * 7)()
+    lib.gsb200_abi_sizes_ext(sizes7, 7)
+    if sizes7[6] != ctypes.sizeof(GsbExtraFeatureArgs):
+        raise RuntimeError(f"libgsb200.so ABI mismatch: sizeof(GsbExtraFeatureArgs) {sizes7[6]} != ctypes mirror "
+                           f"{ctypes.sizeof(GsbExtraFeatureArgs)}")
     _lib = lib
     return lib
 

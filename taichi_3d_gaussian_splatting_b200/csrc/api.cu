@@ -192,9 +192,10 @@ void gsb200_abi_sizes(int64_t *out3) {
 }
 
 void gsb200_abi_sizes_ext(int64_t *out, int32_t n) {
-    const int64_t all[6] = {(int64_t)sizeof(GsbWorkspaceLayout), (int64_t)sizeof(GsbForwardArgs), (int64_t)sizeof(GsbBackwardArgs),
-                            (int64_t)sizeof(GsbExpandArgs), (int64_t)sizeof(GsbTrainStepArgs), (int64_t)sizeof(GsbSupervisionArgs)};
-    for (int i = 0; i < n && i < 6; ++i) out[i] = all[i];
+    const int64_t all[7] = {(int64_t)sizeof(GsbWorkspaceLayout), (int64_t)sizeof(GsbForwardArgs), (int64_t)sizeof(GsbBackwardArgs),
+                            (int64_t)sizeof(GsbExpandArgs), (int64_t)sizeof(GsbTrainStepArgs), (int64_t)sizeof(GsbSupervisionArgs),
+                            (int64_t)sizeof(GsbExtraFeatureArgs)};
+    for (int i = 0; i < n && i < 7; ++i) out[i] = all[i];
 }
 
 int gsb200_workspace_layout(int64_t num_points, int32_t num_objects, int64_t key_capacity,
@@ -233,7 +234,23 @@ int gsb200_stage_blend(const GsbForwardArgs *a) {
     return launch_blend_forward(*a, ws, static_cast<cudaStream_t>(a->stream));
 }
 
-int gsb200_forward(const GsbForwardArgs *a) {
+int gsb200_forward(const GsbForwardArgs *a) { return gsb200_forward_ext(a, nullptr); }
+
+int gsb200_forward_ext(const GsbForwardArgs *a, const GsbExtraFeatureArgs *ext) {
+    if (ext) {
+        if (ext->channels < 1 || ext->channels > 16) {
+            set_error("forward_ext: channels must be in 1..16 (got %d)", ext->channels);
+            return GSB_EINVAL;
+        }
+        if (!ext->features || !ext->rasterized) {
+            set_error("forward_ext: null features / rasterized pointer");
+            return GSB_EINVAL;
+        }
+        if (a && a->rgb_only) {
+            set_error("forward_ext: the feature map needs the full forward (rgb_only is set)");
+            return GSB_EINVAL;
+        }
+    }
     Workspace ws;
     int rc = resolve_fwd(a, &ws);
     if (rc != GSB_OK) return rc;
@@ -246,13 +263,14 @@ int gsb200_forward(const GsbForwardArgs *a) {
     if ((rc = launch_sort(ws, a->key_capacity, st)) != GSB_OK) return rc;
     const int T = (a->camera_height / GSB_TILE_HEIGHT) * (a->camera_width / GSB_TILE_WIDTH);
     if ((rc = launch_tile_ranges(ws, a->key_capacity, T, st)) != GSB_OK) return rc;
-    return launch_blend_forward(*a, ws, st);
+    return launch_blend_forward(*a, ws, st, ext);
 }
 
-// grad_depth / depth: both NULL (no depth term), or both set; grad_alpha: NULL (no alpha term) or set.  The auxiliary terms
-// are checked in gsb200_backward_aux.
+// grad_depth / depth: both NULL (no depth term), or both set; grad_alpha: NULL (no alpha term) or set; ext: NULL (no feature
+// term) or set.  The auxiliary terms are checked in gsb200_backward_ext.
 static int backward_impl(const GsbBackwardArgs *a, bool skip_on_overflow, const float *grad_depth = nullptr,
-                         const float *depth = nullptr, const float *grad_alpha = nullptr) {
+                         const float *depth = nullptr, const float *grad_alpha = nullptr,
+                         const GsbExtraFeatureArgs *ext = nullptr) {
     if (!a) {
         set_error("backward: args is null");
         return GSB_EINVAL;
@@ -291,6 +309,10 @@ static int backward_impl(const GsbBackwardArgs *a, bool skip_on_overflow, const 
         set_error("backward: accum is null");
         return GSB_EINVAL;
     }
+    if (ext && reinterpret_cast<uintptr_t>(ext->grad_features) % 16 != 0) {
+        set_error("backward_ext: grad_features must be 16-byte aligned");
+        return GSB_EINVAL;
+    }
     Workspace ws;
     int rc = resolve_workspace(a->workspace, a->workspace_bytes, a->num_points, a->num_objects,
                                a->key_capacity, a->camera_height, a->camera_width, a->far_plane,
@@ -299,7 +321,9 @@ static int backward_impl(const GsbBackwardArgs *a, bool skip_on_overflow, const 
     cudaStream_t st = static_cast<cudaStream_t>(a->stream);
     if (a->accum_rows > 0)
         GSB_CUDA_CHECK(cudaMemsetAsync(a->accum, 0, (size_t)a->accum_rows * GSB_ACCUM_FLOATS * 4, st));
-    if ((rc = launch_blend_backward(*a, ws, st, grad_depth, depth, grad_alpha)) != GSB_OK) return rc;
+    if (ext && a->num_points > 0)  // the blend adds into the rows it reaches; every other row stays zero
+        GSB_CUDA_CHECK(cudaMemsetAsync(ext->grad_features, 0, (size_t)a->num_points * ext->channels * 4, st));
+    if ((rc = launch_blend_backward(*a, ws, st, grad_depth, depth, grad_alpha, ext)) != GSB_OK) return rc;
     return launch_backward_points(*a, ws, st, skip_on_overflow ? ws.counters + CNT_OVERFLOW : nullptr, grad_depth != nullptr);
 }
 
@@ -307,17 +331,37 @@ int gsb200_backward(const GsbBackwardArgs *a) { return backward_impl(a, false); 
 
 int gsb200_backward_aux(const GsbBackwardArgs *a, const float *grad_rasterized_depth, const float *rasterized_depth,
                         const float *grad_pixel_accumulated_alpha) {
+    return gsb200_backward_ext(a, grad_rasterized_depth, rasterized_depth, grad_pixel_accumulated_alpha, nullptr);
+}
+
+int gsb200_backward_ext(const GsbBackwardArgs *a, const float *grad_rasterized_depth, const float *rasterized_depth,
+                        const float *grad_pixel_accumulated_alpha, const GsbExtraFeatureArgs *ext) {
     if ((grad_rasterized_depth == nullptr) != (rasterized_depth == nullptr)) {
         set_error("backward_aux: grad_rasterized_depth and rasterized_depth must be both NULL or both set");
         return GSB_EINVAL;
     }
-    const bool aux = grad_rasterized_depth != nullptr || grad_pixel_accumulated_alpha != nullptr;
+    if (ext) {
+        if (ext->channels < 1 || ext->channels > 16) {
+            set_error("backward_ext: channels must be in 1..16 (got %d)", ext->channels);
+            return GSB_EINVAL;
+        }
+        if (!ext->features || !ext->grad_rasterized || !ext->grad_features) {
+            set_error("backward_ext: null features / grad_rasterized / grad_features pointer");
+            return GSB_EINVAL;
+        }
+        if (a != nullptr && (a->flags & GSB_FLAG_COMPACT_GRADS)) {
+            set_error("backward_ext: the feature gradient is not carried by the compact rows of the view-parallel exchange "
+                      "(GSB_FLAG_COMPACT_GRADS)");
+            return GSB_EUNSUPPORTED;
+        }
+    }
+    const bool aux = grad_rasterized_depth != nullptr || grad_pixel_accumulated_alpha != nullptr || ext != nullptr;
     if (aux && a != nullptr && !(a->flags & GSB_FLAG_BACKWARD_TRANSPOSED)) {
-        set_error("backward_aux: the depth and alpha gradients need the transposed backward kernel "
+        set_error("backward_aux: the depth, alpha and feature gradients need the transposed backward kernel "
                   "(GSB_FLAG_BACKWARD_TRANSPOSED); the butterfly kernel does not implement them");
         return GSB_EUNSUPPORTED;
     }
-    return backward_impl(a, false, grad_rasterized_depth, rasterized_depth, grad_pixel_accumulated_alpha);
+    return backward_impl(a, false, grad_rasterized_depth, rasterized_depth, grad_pixel_accumulated_alpha, ext);
 }
 
 int gsb200_backward_with_depth(const GsbBackwardArgs *a, const float *grad_rasterized_depth, const float *rasterized_depth) {

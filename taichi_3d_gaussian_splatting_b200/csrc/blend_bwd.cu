@@ -283,7 +283,7 @@ static BlendBwdParams make_blend_bwd_params(const GsbBackwardArgs &a, const Work
 }
 
 int launch_blend_backward(const GsbBackwardArgs &a, const Workspace &ws, cudaStream_t stream, const float *grad_depth,
-                          const float *depth, const float *grad_alpha) {
+                          const float *depth, const float *grad_alpha, const GsbExtraFeatureArgs *ext) {
     BlendBwdParams p;
     p.H = a.camera_height;
     p.W = a.camera_width;
@@ -301,12 +301,14 @@ int launch_blend_backward(const GsbBackwardArgs &a, const Workspace &ws, cudaStr
     p.grad_depth = grad_depth;
     p.depth = depth;
     p.grad_alpha = grad_alpha;
+    const BlendFeatureParams feat{ext ? ext->channels : 0, ws.point_id, ext ? ext->features : nullptr,
+                                  ext ? ext->grad_rasterized : nullptr, ext ? ext->grad_features : nullptr};
     const int tiles = p.tiles_x * (a.camera_height / GSB_TILE_HEIGHT);
     if (tiles <= 0) return GSB_OK;
     if (a.flags & GSB_FLAG_BACKWARD_TRANSPOSED)  // experimental, see blend_bwd_transposed.cu
         return launch_blend_backward_transposed(p, tiles, (a.flags & GSB_FLAG_EXACT_EXP) != 0,
                                                 (a.flags & GSB_FLAG_NO_HOOK_STATS) == 0, stream, grad_depth != nullptr,
-                                                grad_alpha != nullptr);
+                                                grad_alpha != nullptr, ext ? &feat : nullptr);
     const bool exact = (a.flags & GSB_FLAG_EXACT_EXP) != 0;
     if (a.flags & GSB_FLAG_NO_HOOK_STATS) {  // opt-in
         if (exact) blend_backward_kernel<true, false><<<tiles, GSB_TILE_PIXELS, 0, stream>>>(p);

@@ -21,6 +21,24 @@ struct BlendBwdParams {
     const float *depth;
     const float *grad_alpha;  // ALPHA instantiation only: (H,W) dL/d pixel_accumulated_alpha; NULL otherwise
 };
+// gsb200_backward_ext: C = channels, the (N,C) feature rows the forward blended (gathered by scene row
+// point_id[in-camera offset]), the (H,W,C) feature-map gradient and the zeroed (N,C) rows dL/df
+struct BlendFeatureParams {
+    int channels;
+    const int *point_id;
+    const float *features;
+    const float *grad_feature_map;
+    float *grad_features;
+};
+// The parameter block of the feature instantiations (CF > 0) of the transposed kernel.  The other kernels keep
+// BlendBwdParams as it is: a larger parameter block changes their register allocation.
+struct BlendBwdFeatParams : BlendBwdParams {
+    BlendFeatureParams feat;
+};
+__device__ __forceinline__ BlendFeatureParams feature_params(const BlendBwdParams &) {
+    return BlendFeatureParams{0, nullptr, nullptr, nullptr, nullptr};
+}
+__device__ __forceinline__ BlendFeatureParams feature_params(const BlendBwdFeatParams &p) { return p.feat; }
 
 #ifdef GSB_HOST_EMU  // tests/simt: the kernels compiled as host C++ under a lock-step SIMT emulator
 __device__ __forceinline__ float ex2_approx_b(float x) { return exp2f(x); }
@@ -45,7 +63,8 @@ __device__ __forceinline__ float sqrt_approx(float x) {  // MUFU.RSQ based, ~1 u
 #endif
 
 int launch_blend_backward_transposed(const BlendBwdParams &p, int tiles, bool exact_exp, bool stats,
-                                     cudaStream_t stream, bool depth = false, bool alpha = false);
+                                     cudaStream_t stream, bool depth = false, bool alpha = false,
+                                     const BlendFeatureParams *feat = nullptr);
 int launch_blend_backward_count(const BlendBwdParams &p, int tiles, cudaStream_t stream);
 
 }  // namespace gsb

@@ -29,6 +29,17 @@
 //   fast path:  the one-scalar recursion's cg = sum g c_i becomes sum g c_i + g_S (the FMA chain starts at g_S, or at
 //     g_S - g^ D with DEPTH);
 //   exact path: a_grad += g_S T_final / (1 - alpha) for a contributing pair.
+// CF = 4, 8 or 16 (gsb200_backward_ext) adds the gradient of C <= CF per-Gaussian feature channels F_p = sum_i w_i f_i
+// (w_i = alpha_i T_i, the image's weights).  Each channel is one more colour channel of the blend; with g_{p,c} = dL/dF_{p,c}:
+//   phase 1: s = sum_c g_{p,c} f_{i,c} per visit (the pixel's g in registers, the chunk's feature rows in shared memory)
+//     fast path:  cg += s, so the one-scalar recursion carries it to the splats in front and G picks it up;
+//     exact path: a fifth accumulator wF = sum_{j behind} s_j alpha_j T_j, a_grad += s T_i - wF / (1 - alpha);
+//   phase 2: dL/df_{i,c} = sum_p (alpha T)_{p,i} g_{p,c} from the exchange buffer and the warp's g staged in shared memory,
+//     one shuffle level, then RED.ADD (F32x4 where C % 4 == 0) into the (N,C) rows.
+// The feature buffers are appended to the dynamic shared-memory image (TbFeat) and the kernel is compiled for 2 CTAs per
+// SM (DESIGN section 3); the existing buffers, the accumulator rows and the workspace are unchanged.
+#include <type_traits>
+
 #include "blend_bwd.cuh"
 
 namespace gsb {
@@ -78,6 +89,23 @@ static_assert(2 * 32 * TB_ROW >= TB_CHUNK * GSB_ACCUM_FLOATS && GSB_ACCUM_FLOATS
 static_assert(GSB_TB_MIN_BLOCKS * (sizeof(TbShared) + 1024) <= 228 * 1024,
               "the shared-memory image does not allow GSB_TB_MIN_BLOCKS CTAs per SM");
 
+template <int CF>
+struct TbFeat {  // CF > 0: appended to the dynamic shared-memory image after TbShared
+    int row[2][GSB_TILE_PIXELS];  // [buf][element]: scene rows of the staged splats
+    struct Warp {
+        float4 g[32][CF / 4];         // dL/dF of the warp's pixels (zero past C)
+        float4 f[TB_CHUNK][CF / 4];   // feature rows of the current chunk's splats (zero past C)
+        int row[TB_CHUNK];            // their scene rows
+    } w[8];
+};
+constexpr int TB_FEAT_MIN_BLOCKS = 2;
+constexpr int tb_min_blocks(int cf) { return cf == 0 ? GSB_TB_MIN_BLOCKS : TB_FEAT_MIN_BLOCKS; }
+template <int CF>
+constexpr size_t tb_smem_bytes() { return sizeof(TbShared) + (CF > 0 ? sizeof(TbFeat<(CF > 0 ? CF : 4)>) : 0); }
+static_assert(sizeof(TbShared) % 16 == 0, "TbFeat starts 16-byte aligned");
+static_assert(TB_FEAT_MIN_BLOCKS * (tb_smem_bytes<16>() + 1024) <= 228 * 1024,
+              "the feature instantiations' shared-memory image does not allow TB_FEAT_MIN_BLOCKS CTAs per SM");
+
 #ifdef GSB_HOST_EMU
 static inline unsigned char *tb_dynamic_smem() { return simt_emu::dynamic_smem(); }
 #else
@@ -120,12 +148,20 @@ __device__ __forceinline__ float keep_if_contributing(float P, int idx, int last
 #endif
 }
 
-template <bool EXACT_EXP, bool STATS, bool COUNT = false, bool DEPTH = false, bool ALPHA = false>
-__global__ void __launch_bounds__(GSB_TILE_PIXELS, GSB_TB_MIN_BLOCKS)
-blend_backward_transposed_kernel(const BlendBwdParams p) {
-    static_assert(!(COUNT && (DEPTH || ALPHA)), "the work-counter diagnostic runs the default arithmetic only");
+template <int CF>
+using TbParams = typename std::conditional<CF == 0, BlendBwdParams, BlendBwdFeatParams>::type;
+
+template <bool EXACT_EXP, bool STATS, bool COUNT = false, bool DEPTH = false, bool ALPHA = false, int CF = 0>
+__global__ void __launch_bounds__(GSB_TILE_PIXELS, tb_min_blocks(CF))
+blend_backward_transposed_kernel(const TbParams<CF> p) {
+    static_assert(!(COUNT && (DEPTH || ALPHA || CF)), "the work-counter diagnostic runs the default arithmetic only");
+    static_assert(CF % 4 == 0 && CF <= 16, "features: whole float4 groups");
     TbShared &S = *reinterpret_cast<TbShared *>(tb_dynamic_smem());
     constexpr int NV = STATS ? 11 : 9;
+    constexpr int CFW = CF > 0 ? CF : 4;
+    // phase-1 splats per loop trip: at CF = 16 the group's hoisted feature rows would not fit the 128 registers of 2 CTAs per SM
+    constexpr int P1U = CF >= 16 ? 2 : TB_P1_UNROLL;
+    TbFeat<CFW> &SF = *reinterpret_cast<TbFeat<CFW> *>(tb_dynamic_smem() + sizeof(TbShared));  // CF > 0 only
 
     const int tile = blockIdx.x;
     const int tu = tile % p.tiles_x, tv = tile / p.tiles_x;
@@ -159,6 +195,20 @@ blend_backward_transposed_kernel(const BlendBwdParams p) {
     }
     TbWarp &Wp = S.w[warp];
     Wp.g[lane] = make_float4(g0, g1, g2, gd);
+    // CF > 0: this pixel's dL/dF (registers for phase 1, the warp's shared copy for phase 2); wF the exact path's accumulator
+    float gf[CFW];
+    float wF;
+    typename TbFeat<CFW>::Warp &WF = SF.w[warp];
+    const BlendFeatureParams fp = feature_params(p);
+    const int C = CF > 0 ? fp.channels : 0;
+    if constexpr (CF > 0) {
+        wF = 0.0f;
+        const float *src = fp.grad_feature_map + pix * C;
+#pragma unroll
+        for (int c = 0; c < CF; ++c) gf[c] = c < C ? src[c] : 0.0f;
+#pragma unroll
+        for (int c = 0; c < CF; c += 4) WF.g[lane][c / 4] = make_float4(gf[c], gf[c + 1], gf[c + 2], gf[c + 3]);
+    }
 
     // phase-2 role of this lane: splat `ci` of the chunk, rows row0 .. row0 + TB_ROWS - 1 of the patch
     const int ci = lane % TB_CHUNK, row0 = (lane / TB_CHUNK) * TB_ROWS;
@@ -211,6 +261,7 @@ blend_backward_transposed_kernel(const BlendBwdParams p) {
                     float4 r2 = __ldg(rec + 2);
                     r2.w = __int_as_float(o);  // in-camera offset instead of the radius (unused here)
                     s_r2[tid] = r2;
+                    if constexpr (CF > 0) SF.row[buf][tid] = __ldg(&fp.point_id[o]);
                     mask = splat_patch_mask(r0.x, r0.y, r0.z, r0.w, r1.x, r1.y * r1.z, S.origin.x, S.origin.y);
                 }
 #pragma unroll
@@ -252,6 +303,16 @@ blend_backward_transposed_kernel(const BlendBwdParams p) {
                     ck_off[slot] = __float_as_int(r2.w);
                     r2.w = __int_as_float(block_end - 1 - j);  // sorted index instead of the in-camera offset
                     ck2[slot] = r2;
+                    if constexpr (CF > 0) {  // the splat's feature row, zero-padded to CF
+                        const int row = SF.row[buf][j];
+                        WF.row[slot] = row;
+                        const float *src = fp.features + (size_t)row * C;
+#pragma unroll
+                        for (int c = 0; c < CF; c += 4)
+                            WF.f[slot][c / 4] = make_float4(c < C ? __ldg(src + c) : 0.0f, c + 1 < C ? __ldg(src + c + 1) : 0.0f,
+                                                            c + 2 < C ? __ldg(src + c + 2) : 0.0f,
+                                                            c + 3 < C ? __ldg(src + c + 3) : 0.0f);
+                    }
                 }
                 have += take;
                 pos += take;
@@ -272,6 +333,17 @@ blend_backward_transposed_kernel(const BlendBwdParams p) {
                     const float4 r2 = ck2[i];  // r g b | sorted index
                     const int idx = __float_as_int(r2.w);
                     const float d0 = px - r0.x, d1 = py - r0.y;
+                    float sf = 0.0f;  // CF > 0: s = sum_c g_c f_c, the feature channels' share of the colour-gradient product
+                    if constexpr (CF > 0) {
+#pragma unroll
+                        for (int c = 0; c < CF; c += 4) {
+                            const float4 f = WF.f[i][c / 4];
+                            sf = fmaf(gf[c], f.x, sf);
+                            sf = fmaf(gf[c + 1], f.y, sf);
+                            sf = fmaf(gf[c + 2], f.z, sf);
+                            sf = fmaf(gf[c + 3], f.w, sf);
+                        }
+                    }
                     float G, aT;
                     if (EXACT_EXP) {
                         const float q0 = r0.z * d0 + r0.w * d1;
@@ -292,6 +364,10 @@ blend_backward_transposed_kernel(const BlendBwdParams p) {
                             w3 = fmaf(e, aT, w3);
                         }
                         if (ALPHA) a_grad += contributes ? ga * inv : 0.0f;  // g_S T_final / (1 - alpha)
+                        if constexpr (CF > 0) {  // the feature channels, summed: "colour" times gradient s
+                            a_grad += contributes ? sf * Tn - wF * inv : 0.0f;
+                            wF = fmaf(sf, aT, wF);
+                        }
                         T = contributes ? Tn : T;
                         w0 = fmaf(r2.x, aT, w0);
                         w1 = fmaf(r2.y, aT, w1);
@@ -316,6 +392,7 @@ blend_backward_transposed_kernel(const BlendBwdParams p) {
                         float cg = fmaf(r2.z, g2, fmaf(r2.y, g1, ALPHA ? fmaf(r2.x, g0, ga) : r2.x * g0));
                         // + gd (z - D): the depth map as a fourth channel (with ALPHA, ga already holds the - hd)
                         if (DEPTH) cg = ALPHA ? fmaf(gd, r1.w, cg) : fmaf(gd, r1.w, cg) - hd;
+                        if constexpr (CF > 0) cg += sf;  // + sum_c g_c f_c: the feature channels
                         const float a_grad = fmaf(cg, T, -(w0 * inv));
                         w0 = fmaf(cg, aT, w0);
                         G = a_grad * P;
@@ -334,12 +411,12 @@ blend_backward_transposed_kernel(const BlendBwdParams p) {
                     // exchange buffer from the chunk buffer, so a store between two splats would keep the next splat's
                     // loads and alpha (independent of the recursion) from being scheduled under the previous one.
 #pragma unroll 1
-                    for (int i0 = 0; i0 < TB_CHUNK; i0 += TB_P1_UNROLL) {
-                        float2 ex[TB_P1_UNROLL];
+                    for (int i0 = 0; i0 < TB_CHUNK; i0 += P1U) {
+                        float2 ex[P1U];
 #pragma unroll
-                        for (int u = 0; u < TB_P1_UNROLL; ++u) ex[u] = p1(i0 + u);
+                        for (int u = 0; u < P1U; ++u) ex[u] = p1(i0 + u);
 #pragma unroll
-                        for (int u = 0; u < TB_P1_UNROLL; ++u) x[lane * TB_ROW + i0 + u] = ex[u];
+                        for (int u = 0; u < P1U; ++u) x[lane * TB_ROW + i0 + u] = ex[u];
                     }
                 } else {  // the short last chunk of a tile
 #pragma unroll 1
@@ -366,6 +443,11 @@ blend_backward_transposed_kernel(const BlendBwdParams p) {
                 float acc[12];  // the accumulator row; word 11 only with DEPTH
 #pragma unroll
                 for (int k = 0; k < 12; ++k) acc[k] = 0.0f;
+                float af[CFW];  // CF > 0: sum alpha T g_c over this lane's pixels = dL/df_c of the splat
+                if constexpr (CF > 0) {
+#pragma unroll
+                    for (int c = 0; c < CF; ++c) af[c] = 0.0f;
+                }
                 unsigned int nz = 0u;
 #pragma unroll
                 for (int row = 0; row < TB_ROWS; ++row) {
@@ -406,13 +488,53 @@ blend_backward_transposed_kernel(const BlendBwdParams p) {
                     acc[4] += fmaf(cb, u1, q1r * t1);
                     acc[8] += m0;
                 }
+                if constexpr (CF > 0) {  // a loop of its own (alpha T re-read): the CF sums would not fit beside the moments' registers
+#pragma unroll 1
+                    for (int row = 0; row < TB_ROWS; ++row) {
+#pragma unroll 4
+                        for (int k = 0; k < 8; ++k) {
+                            const int pp = 8 * (row0 + row) + k;
+                            const float aT = x[pp * TB_ROW + ci].y;
+#pragma unroll
+                            for (int c = 0; c < CF; c += 4) {
+                                const float4 gc = WF.g[pp][c / 4];
+                                af[c] = fmaf(aT, gc.x, af[c]);
+                                af[c + 1] = fmaf(aT, gc.y, af[c + 1]);
+                                af[c + 2] = fmaf(aT, gc.z, af[c + 2]);
+                                af[c + 3] = fmaf(aT, gc.w, af[c + 3]);
+                            }
+                        }
+                    }
+                }
                 // the lanes of the splat: rows 0..3 of the patch
 #pragma unroll
                 for (int d = TB_CHUNK; d < 32; d *= 2) {
 #pragma unroll
                     for (int k = 0; k < NV; ++k) acc[k] += __shfl_xor_sync(0xffffffffu, acc[k], d);
                     if (DEPTH) acc[11] += __shfl_xor_sync(0xffffffffu, acc[11], d);
+                    if constexpr (CF > 0) {
+#pragma unroll
+                        for (int c = 0; c < CF; ++c) af[c] += __shfl_xor_sync(0xffffffffu, af[c], d);
+                    }
                     nz |= __shfl_xor_sync(0xffffffffu, nz, d);
+                }
+                if constexpr (CF > 0) if (active && nz != 0u) {
+                    // the 32 / TB_CHUNK lanes of the splat hold the same sums: lane part h adds the float4 groups q with
+                    // q % parts == h (one 16-byte RED per group when the rows are 16-byte aligned, C % 4 == 0)
+                    constexpr int parts = 32 / TB_CHUNK;
+                    const int h = lane / TB_CHUNK;
+                    float *dst = fp.grad_features + (size_t)WF.row[ci] * C;
+#pragma unroll
+                    for (int c = 0; c < CF; c += 4) {
+                        if ((c / 4) % parts != h || c >= C) continue;
+                        if (C % 4 == 0) {
+                            red_add_f32x4(dst + c, make_float4(af[c], af[c + 1], af[c + 2], af[c + 3]));
+                        } else {
+#pragma unroll
+                            for (int k = 0; k < 4; ++k)
+                                if (c + k < C) atomicAdd(dst + c + k, af[c + k]);
+                        }
+                    }
                 }
                 acc[8] *= EXACT_EXP ? (1.0f - s1.z) : s1.z;  // d alpha / d logit = alpha (1 - opacity)
                 __syncwarp();  // every lane has consumed its exchange entries: the buffer now takes the finished rows
@@ -460,30 +582,52 @@ blend_backward_transposed_kernel(const BlendBwdParams p) {
 }
 
 #ifndef GSB_HOST_EMU
-template <bool EXACT_EXP, bool STATS, bool DEPTH = false, bool ALPHA = false>
-static int launch_tb(const BlendBwdParams &p, int tiles, cudaStream_t stream) {
+template <bool EXACT_EXP, bool STATS, bool DEPTH = false, bool ALPHA = false, int CF = 0>
+static int launch_tb(const TbParams<CF> &p, int tiles, cudaStream_t stream) {
     static bool configured = false;  // one device per process (one process per GPU)
     if (!configured) {
-        GSB_CUDA_CHECK(cudaFuncSetAttribute(blend_backward_transposed_kernel<EXACT_EXP, STATS, false, DEPTH, ALPHA>,
-                                            cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TbShared)));
+        GSB_CUDA_CHECK(cudaFuncSetAttribute(blend_backward_transposed_kernel<EXACT_EXP, STATS, false, DEPTH, ALPHA, CF>,
+                                            cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tb_smem_bytes<CF>()));
         configured = true;
     }
-    blend_backward_transposed_kernel<EXACT_EXP, STATS, false, DEPTH, ALPHA>
-        <<<tiles, GSB_TILE_PIXELS, sizeof(TbShared), stream>>>(p);
+    blend_backward_transposed_kernel<EXACT_EXP, STATS, false, DEPTH, ALPHA, CF>
+        <<<tiles, GSB_TILE_PIXELS, tb_smem_bytes<CF>(), stream>>>(p);
     GSB_CUDA_CHECK(cudaGetLastError());
     return GSB_OK;
 }
 
-template <bool DEPTH, bool ALPHA>
-static int launch_tb_terms(const BlendBwdParams &p, int tiles, bool exact_exp, bool stats, cudaStream_t stream) {
+template <bool DEPTH, bool ALPHA, int CF = 0>
+static int launch_tb_terms(const TbParams<CF> &p, int tiles, bool exact_exp, bool stats, cudaStream_t stream) {
     if (exact_exp)
-        return stats ? launch_tb<true, true, DEPTH, ALPHA>(p, tiles, stream) : launch_tb<true, false, DEPTH, ALPHA>(p, tiles, stream);
-    return stats ? launch_tb<false, true, DEPTH, ALPHA>(p, tiles, stream) : launch_tb<false, false, DEPTH, ALPHA>(p, tiles, stream);
+        return stats ? launch_tb<true, true, DEPTH, ALPHA, CF>(p, tiles, stream)
+                     : launch_tb<true, false, DEPTH, ALPHA, CF>(p, tiles, stream);
+    return stats ? launch_tb<false, true, DEPTH, ALPHA, CF>(p, tiles, stream)
+                 : launch_tb<false, false, DEPTH, ALPHA, CF>(p, tiles, stream);
 }
 
-// depth = true: p.grad_depth and p.depth must be set (the DEPTH instantiations); alpha = true: p.grad_alpha (ALPHA)
+template <int CF>
+static int launch_tb_features(const BlendBwdFeatParams &p, int tiles, bool exact_exp, bool stats, cudaStream_t stream, bool depth,
+                              bool alpha) {
+    if (alpha)
+        return depth ? launch_tb_terms<true, true, CF>(p, tiles, exact_exp, stats, stream)
+                     : launch_tb_terms<false, true, CF>(p, tiles, exact_exp, stats, stream);
+    return depth ? launch_tb_terms<true, false, CF>(p, tiles, exact_exp, stats, stream)
+                 : launch_tb_terms<false, false, CF>(p, tiles, exact_exp, stats, stream);
+}
+
+// depth = true: p.grad_depth and p.depth must be set (the DEPTH instantiations); alpha = true: p.grad_alpha (ALPHA);
+// feat: the feature channels, C in 1..16 (the CF instantiation of width 4, 8 or 16), or NULL
 int launch_blend_backward_transposed(const BlendBwdParams &p, int tiles, bool exact_exp, bool stats,
-                                     cudaStream_t stream, bool depth, bool alpha) {
+                                     cudaStream_t stream, bool depth, bool alpha, const BlendFeatureParams *feat) {
+    if (feat) {
+        BlendBwdFeatParams fp;
+        static_cast<BlendBwdParams &>(fp) = p;
+        fp.feat = *feat;
+        const int C = feat->channels;
+        return C <= 4 ? launch_tb_features<4>(fp, tiles, exact_exp, stats, stream, depth, alpha)
+             : C <= 8 ? launch_tb_features<8>(fp, tiles, exact_exp, stats, stream, depth, alpha)
+                      : launch_tb_features<16>(fp, tiles, exact_exp, stats, stream, depth, alpha);
+    }
     if (alpha)
         return depth ? launch_tb_terms<true, true>(p, tiles, exact_exp, stats, stream)
                      : launch_tb_terms<false, true>(p, tiles, exact_exp, stats, stream);

@@ -12,6 +12,8 @@
 // branches never skipped much).  The CTA leaves the list as soon as every pixel has saturated
 // (__syncthreads_and) -- the reference walks the whole list (GPCR:387-394).  Compute-bound (FP32 issue +
 // MUFU.EX2), not HBM-bound: 48 B per (tile, splat) are reused by up to 256 pixels.
+#include <type_traits>
+
 #include "common.cuh"
 
 namespace gsb {
@@ -33,6 +35,36 @@ struct BlendFwdParams {
                                         //   pairs, [3] the same with 8x8 patches (two pixels per thread, vertical pairs),
                                         //   [4] with 16x4 patches (horizontal pairs), [5] with 4x4 sub-patches
 };
+// The parameter block of the feature instantiations (CF > 0, gsb200_forward_ext): C = channels per-Gaussian feature values,
+// blended with the image's weights into out_features (H,W,C); rows are gathered by scene row point_id[in-camera offset].
+// The other instantiations keep BlendFwdParams as it is: a larger parameter block changes their register allocation.
+struct BlendFwdFeatParams : BlendFwdParams {
+    int channels;
+    const int *point_id;
+    const float *features;   // (N,C)
+    float *out_features;     // (H,W,C)
+};
+template <int CF>
+using FwParams = typename std::conditional<CF == 0, BlendFwdParams, BlendFwdFeatParams>::type;
+struct FwFeatureArgs {
+    int channels;
+    const int *point_id;
+    const float *features;
+    float *out_features;
+};
+__device__ __forceinline__ FwFeatureArgs feature_args(const BlendFwdParams &) { return FwFeatureArgs{0, nullptr, nullptr, nullptr}; }
+__device__ __forceinline__ FwFeatureArgs feature_args(const BlendFwdFeatParams &p) {
+    return FwFeatureArgs{p.channels, p.point_id, p.features, p.out_features};
+}
+
+// The staged feature rows of the CF > 0 instantiations, [buf][element][CF] (dynamic shared memory: with the 39 KB of the
+// static arrays a CF = 16 stage would pass the 48 KB static limit)
+#ifdef GSB_HOST_EMU
+static inline float *fw_feature_smem() { return reinterpret_cast<float *>(simt_emu::dynamic_smem()); }
+#else
+extern __shared__ __align__(16) float gsb_fw_dynamic_smem[];
+__device__ __forceinline__ float *fw_feature_smem() { return gsb_fw_dynamic_smem; }
+#endif
 
 __device__ __forceinline__ float ex2_approx(float x) { return ex2_mufu(x); }
 
@@ -64,10 +96,22 @@ __device__ __forceinline__ void count_if_blended(float wgt, int idx, int &cnt, i
 #endif
 constexpr int FW_UNROLL = GSB_FWD_UNROLL;
 constexpr int FW_CHUNK = 32;  // splats per private chunk of a warp
+// the staged feature row of element j of staging buffer buf (the same address in every lane of a warp: a broadcast)
+template <int CF>
+__device__ __forceinline__ const float4 *fw_feature_row(int buf, int j) {
+    return reinterpret_cast<const float4 *>(fw_feature_smem() + (buf * GSB_TILE_PIXELS + j) * CF);
+}
+// CTAs per SM the feature instantiations are compiled for: the CF accumulators need the registers (DESIGN section 3)
+constexpr int fw_min_blocks(int cf, bool exact_exp) { return cf == 0 ? GSB_FWD_MIN_BLOCKS : (cf <= 8 && !exact_exp) ? 3 : 2; }
+// dynamic shared memory of a feature instantiation: two staging buffers of CF floats per splat
+constexpr int fw_feature_smem_bytes(int cf) { return 2 * GSB_TILE_PIXELS * cf * (int)sizeof(float); }
 
-template <bool RGB_ONLY, bool EXACT_EXP, bool COUNT = false>
-__global__ void __launch_bounds__(GSB_TILE_PIXELS, GSB_FWD_MIN_BLOCKS)
-blend_forward_kernel(const BlendFwdParams p) {
+// CF (4, 8 or 16; 0 = no features): compile-time width of the per-Gaussian feature vector (gsb200_forward_ext).  The
+// runtime C <= CF is padded with zeros in shared memory and registers; nothing past C is read or written in global memory.
+template <bool RGB_ONLY, bool EXACT_EXP, bool COUNT = false, int CF = 0>
+__global__ void __launch_bounds__(GSB_TILE_PIXELS, fw_min_blocks(CF, EXACT_EXP))
+blend_forward_kernel(const FwParams<CF> p) {
+    static_assert(CF == 0 || (CF % 4 == 0 && !RGB_ONLY && !COUNT), "features: whole float4 groups, full outputs only");
     // double-buffered staging area: [buf][plane][splat]; planes: u v a b | c rescale opacity depth | r g b radius
     __shared__ float4 s_rec[2 * 3 * GSB_TILE_PIXELS];
     __shared__ unsigned int s_bits[2][8][8];        // [buf][consumer warp patch][loader warp] -> splats that can reach it
@@ -94,6 +138,11 @@ blend_forward_kernel(const BlendFwdParams p) {
     float4 *const ck0 = s_chunk[warp][0], *const ck1 = s_chunk[warp][1], *const ck2 = s_chunk[warp][2];
     unsigned char *const list = s_list[warp];
     const unsigned int lt_mask = (1u << lane) - 1u;
+    constexpr int CFW = CF > 0 ? CF : 4;
+    const FwFeatureArgs fa = feature_args(p);
+    float F[CFW];  // CF > 0: the feature sums of this pixel
+#pragma unroll
+    for (int c = 0; c < CFW; ++c) F[c] = 0.0f;
 
     // One barrier per batch: batch k is staged into buffer k&1 while slower warps may still be copying chunks of
     // batch k-1 out of the other buffer; passing barrier k implies everybody is done with batch k-1.
@@ -117,6 +166,15 @@ blend_forward_kernel(const BlendFwdParams p) {
                 s_r1[tid] = f1;
             }
             s_r2[tid] = __ldg(rec + 2);
+            if constexpr (CF > 0) {  // the splat's feature row, by scene row, zero-padded to CF
+                const int C = fa.channels;
+                const float *src = fa.features + (size_t)__ldg(&fa.point_id[o]) * C;
+                float4 *dst = reinterpret_cast<float4 *>(fw_feature_smem() + (buf * GSB_TILE_PIXELS + tid) * CF);
+#pragma unroll
+                for (int c = 0; c < CF; c += 4)
+                    dst[c / 4] = make_float4(c < C ? __ldg(src + c) : 0.0f, c + 1 < C ? __ldg(src + c + 1) : 0.0f,
+                                             c + 2 < C ? __ldg(src + c + 2) : 0.0f, c + 3 < C ? __ldg(src + c + 3) : 0.0f);
+            }
             mask = splat_patch_mask(r0.x, r0.y, r0.z, r0.w, r1.x, r1.y * r1.z, tile_x0, tile_y0);
             if (COUNT) {  // patch w sits at column (w & 1), row (w >> 1)
                 n_p84 += __popc(mask);
@@ -186,6 +244,17 @@ blend_forward_kernel(const BlendFwdParams p) {
                                 Wt += alpha * T;
                                 cnt += 1;
                             }
+                            if constexpr (CF > 0) {  // the colour's expression
+                                const float4 *fi = fw_feature_row<CF>(buf, __float_as_int(r2.w) - 1 - base);
+#pragma unroll
+                                for (int c = 0; c < CF; c += 4) {
+                                    const float4 f = fi[c / 4];
+                                    F[c] += f.x * alpha * T;
+                                    F[c + 1] += f.y * alpha * T;
+                                    F[c + 2] += f.z * alpha * T;
+                                    F[c + 3] += f.w * alpha * T;
+                                }
+                            }
                             T = nT;
                             Tlive = nT;
                         } else {
@@ -213,6 +282,17 @@ blend_forward_kernel(const BlendFwdParams p) {
                         Wt += wgt;
                         count_if_blended(wgt, __float_as_int(r2.w), cnt, last);
                     }
+                    if constexpr (CF > 0) {  // the colour's weight
+                        const float4 *fi = fw_feature_row<CF>(buf, __float_as_int(r2.w) - 1 - base);
+#pragma unroll
+                        for (int c = 0; c < CF; c += 4) {
+                            const float4 f = fi[c / 4];
+                            F[c] = fmaf(f.x, wgt, F[c]);
+                            F[c + 1] = fmaf(f.y, wgt, F[c + 1]);
+                            F[c + 2] = fmaf(f.z, wgt, F[c + 2]);
+                            F[c + 3] = fmaf(f.w, wgt, F[c + 3]);
+                        }
+                    }
                     T = ok ? nT : -fabsf(T);
                 }
             }
@@ -229,6 +309,12 @@ blend_forward_kernel(const BlendFwdParams p) {
         p.acc_alpha[pix] = 1.0f - (EXACT_EXP ? Tlive : fabsf(T));
         p.last_effective[pix] = last;
         p.valid_count[pix] = cnt;
+    }
+    if constexpr (CF > 0) {
+        const int C = fa.channels;
+#pragma unroll
+        for (int c = 0; c < CF; ++c)
+            if (c < C) fa.out_features[pix * C + c] = F[c];
     }
     if (COUNT) {
 #pragma unroll
@@ -252,7 +338,25 @@ blend_forward_kernel(const BlendFwdParams p) {
 }
 
 #ifndef GSB_HOST_EMU
-int launch_blend_forward(const GsbForwardArgs &a, const Workspace &ws, cudaStream_t stream) {
+template <bool EXACT_EXP, int CF>
+static int launch_fwd_features(const BlendFwdFeatParams &p, int tiles, cudaStream_t stream) {
+    static bool configured = false;  // one device per process (one process per GPU)
+    if (!configured) {
+        GSB_CUDA_CHECK(cudaFuncSetAttribute(blend_forward_kernel<false, EXACT_EXP, false, CF>,
+                                            cudaFuncAttributeMaxDynamicSharedMemorySize, fw_feature_smem_bytes(CF)));
+        configured = true;
+    }
+    blend_forward_kernel<false, EXACT_EXP, false, CF><<<tiles, GSB_TILE_PIXELS, fw_feature_smem_bytes(CF), stream>>>(p);
+    GSB_CUDA_CHECK(cudaGetLastError());
+    return GSB_OK;
+}
+
+template <int CF>
+static int launch_fwd_features(const BlendFwdFeatParams &p, int tiles, bool exact, cudaStream_t stream) {
+    return exact ? launch_fwd_features<true, CF>(p, tiles, stream) : launch_fwd_features<false, CF>(p, tiles, stream);
+}
+
+int launch_blend_forward(const GsbForwardArgs &a, const Workspace &ws, cudaStream_t stream, const GsbExtraFeatureArgs *ext) {
     BlendFwdParams p;
     p.H = a.camera_height;
     p.W = a.camera_width;
@@ -270,6 +374,18 @@ int launch_blend_forward(const GsbForwardArgs &a, const Workspace &ws, cudaStrea
     const int tiles = p.tiles_x * (a.camera_height / GSB_TILE_HEIGHT);
     if (tiles <= 0) return GSB_OK;
     const bool exact = (a.flags & GSB_FLAG_EXACT_EXP) != 0;
+    if (ext) {  // checked by gsb200_forward_ext: 1 <= C <= 16, not rgb_only
+        BlendFwdFeatParams fp;
+        static_cast<BlendFwdParams &>(fp) = p;
+        fp.channels = ext->channels;
+        fp.point_id = ws.point_id;
+        fp.features = ext->features;
+        fp.out_features = ext->rasterized;
+        const int C = ext->channels;
+        return C <= 4 ? launch_fwd_features<4>(fp, tiles, exact, stream)
+             : C <= 8 ? launch_fwd_features<8>(fp, tiles, exact, stream)
+                      : launch_fwd_features<16>(fp, tiles, exact, stream);
+    }
     if (a.rgb_only) {
         if (exact) blend_forward_kernel<true, true><<<tiles, GSB_TILE_PIXELS, 0, stream>>>(p);
         else blend_forward_kernel<true, false><<<tiles, GSB_TILE_PIXELS, 0, stream>>>(p);

@@ -67,13 +67,16 @@ int launch_sort(const Workspace &ws, int64_t key_capacity, cudaStream_t stream);
 int launch_tile_ranges(const Workspace &ws, int64_t key_capacity, int num_tiles, cudaStream_t stream);
 int launch_tile_ranges_raw(const long long *keys_i64, int64_t n, int *tile_start, int *tile_end,
                            int num_tiles, cudaStream_t stream);
-int launch_blend_forward(const GsbForwardArgs &a, const Workspace &ws, cudaStream_t stream);
+// ext: the per-Gaussian feature vectors to blend alongside the image (gsb200_forward_ext, checked there), or NULL
+int launch_blend_forward(const GsbForwardArgs &a, const Workspace &ws, cudaStream_t stream,
+                         const GsbExtraFeatureArgs *ext = nullptr);
 // grad_depth / depth: the (H,W) depth gradient and the forward's depth output (gsb200_backward_aux; transposed
 // kernel only), or both NULL.  grad_alpha: the (H,W) gradient of the accumulated alpha (transposed kernel only), or NULL.
+// ext: the feature-map gradient and the (N,C) output rows, zeroed by the caller (transposed kernel only), or NULL.
 // depth_grad: the accumulator rows carry dL/dz in word 11.
 int launch_blend_backward(const GsbBackwardArgs &a, const Workspace &ws, cudaStream_t stream,
                           const float *grad_depth = nullptr, const float *depth = nullptr,
-                          const float *grad_alpha = nullptr);
+                          const float *grad_alpha = nullptr, const GsbExtraFeatureArgs *ext = nullptr);
 int launch_backward_points(const GsbBackwardArgs &a, const Workspace &ws, cudaStream_t stream,
                            const long long *skip_flag = nullptr, bool depth_grad = false);
 int launch_adam_step(float *param, const float *grad, float *exp_avg, float *exp_avg_sq, long long n, double lr, double beta1,
