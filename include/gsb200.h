@@ -205,7 +205,7 @@ const char *gsb200_last_error(void);
  * foreign-language binding verify its struct mirrors. */
 void gsb200_abi_sizes(int64_t *out3);
 /* ... and of the first n of {GsbWorkspaceLayout, GsbForwardArgs, GsbBackwardArgs, GsbExpandArgs, GsbTrainStepArgs,
- * GsbSupervisionArgs, GsbExtraFeatureArgs} */
+ * GsbSupervisionArgs, GsbExtraFeatureArgs, GsbFeatureTrainArgs} */
 void gsb200_abi_sizes_ext(int64_t *out, int32_t n);
 
 /* Workspace sizing.  far_plane*depth_to_sort_key_scale fixes the depth-key width; (H/16)*(W/16)
@@ -363,6 +363,40 @@ int64_t gsb200_supervision_temp_bytes(int32_t camera_height, int32_t camera_widt
  * gradient output, or a temp that is too small or not 16-byte aligned; GSB_EUNSUPPORTED without
  * GSB_FLAG_BACKWARD_TRANSPOSED.  Deterministic: fixed grids and summation orders. */
 int gsb200_train_step_aux(const GsbTrainStepArgs *args, const GsbSupervisionArgs *supervision);
+
+/* Feature term of the fused train step (an extension): a loss on the per-Gaussian feature map F = features.rasterized
+ * (H,W,C) that gsb200_forward_ext renders, back-propagated by gsb200_backward_ext, and an Adam step on the (N,C) features.
+ *   GSB_FEATURE_LOSS_CROSS_ENTROPY (semantic labels, C >= 2): labels (H,W) int32, a pixel labelled when 0 <= label < C;
+ *     weight * sum_labelled CE(softmax(F_p), label_p) / max(n_labelled, 1), with a max-subtracted log-sum-exp;
+ *   GSB_FEATURE_LOSS_L2 (distilled feature maps): target (H,W,C) f32, a pixel supervised when all C values are finite (NaN =
+ *     no target); weight * sum_supervised sum_c (F_pc - T_pc)^2 / max(n_supervised * C, 1).
+ * An unsupervised pixel gets a zero gradient; a frame without one supervised pixel has term 0. */
+#define GSB_FEATURE_LOSS_CROSS_ENTROPY 1
+#define GSB_FEATURE_LOSS_L2 2
+typedef struct GsbFeatureTrainArgs {
+    GsbExtraFeatureArgs features; /* features (N,C): updated in place by Adam; rasterized (H,W,C): the forward's feature map;
+                                     grad_rasterized (H,W,C): written by the loss (dL/dF); grad_features (N,C): dL/df */
+    int32_t loss_kind;            /* GSB_FEATURE_LOSS_* */
+    float weight;                 /* > 0, finite */
+    const int32_t *labels;        /* (H,W) cross entropy (not read for l2) */
+    const float *target;          /* (H,W,C) l2 (not read for cross entropy) */
+    float *loss_out2;             /* device: {feature term, n_supervised} */
+    void *temp;                   /* gsb200_feature_loss_temp_bytes(H, W), 16-byte aligned, first 16 bytes zero before first use */
+    int64_t temp_bytes;
+    float *exp_avg, *exp_avg_sq;  /* (N,C) Adam state of the features, zero before the first step, 16-byte aligned */
+    double learning_rate;         /* Adam of the features; betas, eps and step are the train step's */
+} GsbFeatureTrainArgs;
+int64_t gsb200_feature_loss_temp_bytes(int32_t camera_height, int32_t camera_width);
+/* gsb200_train_step_aux with the feature term: gsb200_forward_ext -> the supervision pre-pass, image loss and post-pass
+ * (unchanged) -> feature loss (pass 1: sums, pass 2: dL/dF and loss_out2) -> gsb200_backward_ext with the depth, alpha and
+ * feature gradients -> Adam on the 56 columns, on xyz and on the features, all three skipped on the device after a
+ * key-capacity overflow.  NULL features: exactly gsb200_train_step_aux (which is this call with NULL).  Before any CUDA call:
+ * GSB_EINVAL for channels outside 1..16, an unknown kind, cross entropy with C < 2, a weight that is not finite or not > 0,
+ * a NULL target, map, gradient, moment or output pointer, a temp that is too small or not 16-byte aligned, or features,
+ * grad_features or moments that are not 16-byte aligned; GSB_EUNSUPPORTED without GSB_FLAG_BACKWARD_TRANSPOSED or with
+ * GSB_FLAG_COMPACT_GRADS.  Deterministic: fixed grids and summation orders. */
+int gsb200_train_step_ext(const GsbTrainStepArgs *args, const GsbSupervisionArgs *supervision,
+                          const GsbFeatureTrainArgs *features);
 
 /* Individual stages (same workspace), for tests and profiling. */
 int gsb200_stage_preprocess(const GsbForwardArgs *args);   /* K1+P1+K2+K3+P2+K4 fused */

@@ -97,6 +97,18 @@ class GsbExtraFeatureArgs(ctypes.Structure):
     ]
 
 
+class GsbFeatureTrainArgs(ctypes.Structure):
+    _fields_ = [
+        ("features", GsbExtraFeatureArgs), ("loss_kind", c_i32), ("weight", c_f32), ("labels", c_vp), ("target", c_vp),
+        ("loss_out2", c_vp), ("temp", c_vp), ("temp_bytes", c_i64), ("exp_avg", c_vp), ("exp_avg_sq", c_vp),
+        ("learning_rate", ctypes.c_double),
+    ]
+
+
+GSB_FEATURE_LOSS_CROSS_ENTROPY = 1
+GSB_FEATURE_LOSS_L2 = 2
+
+
 class GsbExpandArgs(ctypes.Structure):
     _fields_ = [
         ("num_points", c_i64), ("num_views", c_i32), ("num_objects", c_i32), ("grad_sum", c_vp),
@@ -115,7 +127,7 @@ EXPORTS = (
     "gsb200_forward_blend_work", "gsb200_backward_blend_work", "gsb200_device_selftest", "gsb200_expand_view_gradients",
     "gsb200_train_step", "gsb200_abi_sizes_ext", "gsb200_exchange_multimem", "gsb200_backward_with_depth",
     "gsb200_backward_aux", "gsb200_supervision_temp_bytes", "gsb200_train_step_aux", "gsb200_forward_ext",
-    "gsb200_backward_ext",
+    "gsb200_backward_ext", "gsb200_feature_loss_temp_bytes", "gsb200_train_step_ext",
 )
 
 _lib = None
@@ -180,6 +192,11 @@ def load() -> ctypes.CDLL:
     lib.gsb200_train_step.restype = ctypes.c_int
     lib.gsb200_train_step_aux.argtypes = [ctypes.POINTER(GsbTrainStepArgs), ctypes.POINTER(GsbSupervisionArgs)]
     lib.gsb200_train_step_aux.restype = ctypes.c_int
+    lib.gsb200_train_step_ext.argtypes = [ctypes.POINTER(GsbTrainStepArgs), ctypes.POINTER(GsbSupervisionArgs),
+                                          ctypes.POINTER(GsbFeatureTrainArgs)]
+    lib.gsb200_train_step_ext.restype = ctypes.c_int
+    lib.gsb200_feature_loss_temp_bytes.argtypes = [c_i32, c_i32]
+    lib.gsb200_feature_loss_temp_bytes.restype = c_i64
     lib.gsb200_supervision_temp_bytes.argtypes = [c_i32, c_i32]
     lib.gsb200_supervision_temp_bytes.restype = c_i64
     lib.gsb200_device_selftest.argtypes = [c_vp]
@@ -219,6 +236,11 @@ def load() -> ctypes.CDLL:
     if sizes7[6] != ctypes.sizeof(GsbExtraFeatureArgs):
         raise RuntimeError(f"libgsb200.so ABI mismatch: sizeof(GsbExtraFeatureArgs) {sizes7[6]} != ctypes mirror "
                            f"{ctypes.sizeof(GsbExtraFeatureArgs)}")
+    sizes8 = (c_i64 * 8)()
+    lib.gsb200_abi_sizes_ext(sizes8, 8)
+    if sizes8[7] != ctypes.sizeof(GsbFeatureTrainArgs):
+        raise RuntimeError(f"libgsb200.so ABI mismatch: sizeof(GsbFeatureTrainArgs) {sizes8[7]} != ctypes mirror "
+                           f"{ctypes.sizeof(GsbFeatureTrainArgs)}")
     _lib = lib
     return lib
 

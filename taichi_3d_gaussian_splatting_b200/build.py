@@ -31,6 +31,7 @@ SOURCES = {
     "loss.cu": [],
     "image_loss.cu": [],
     "supervision_loss.cu": [],
+    "feature_loss.cu": [],
     "adam.cu": [],
     "controller.cu": [],
     "exchange.cu": [],

@@ -192,10 +192,10 @@ void gsb200_abi_sizes(int64_t *out3) {
 }
 
 void gsb200_abi_sizes_ext(int64_t *out, int32_t n) {
-    const int64_t all[7] = {(int64_t)sizeof(GsbWorkspaceLayout), (int64_t)sizeof(GsbForwardArgs), (int64_t)sizeof(GsbBackwardArgs),
+    const int64_t all[8] = {(int64_t)sizeof(GsbWorkspaceLayout), (int64_t)sizeof(GsbForwardArgs), (int64_t)sizeof(GsbBackwardArgs),
                             (int64_t)sizeof(GsbExpandArgs), (int64_t)sizeof(GsbTrainStepArgs), (int64_t)sizeof(GsbSupervisionArgs),
-                            (int64_t)sizeof(GsbExtraFeatureArgs)};
-    for (int i = 0; i < n && i < 7; ++i) out[i] = all[i];
+                            (int64_t)sizeof(GsbExtraFeatureArgs), (int64_t)sizeof(GsbFeatureTrainArgs)};
+    for (int i = 0; i < n && i < 8; ++i) out[i] = all[i];
 }
 
 int gsb200_workspace_layout(int64_t num_points, int32_t num_objects, int64_t key_capacity,
@@ -376,7 +376,58 @@ static bool weight_ok(float w) { return w >= 0.0f && w <= 3.402823466e38f; }  //
 
 int gsb200_train_step(const GsbTrainStepArgs *t) { return gsb200_train_step_aux(t, nullptr); }
 
-int gsb200_train_step_aux(const GsbTrainStepArgs *t, const GsbSupervisionArgs *s) {
+int gsb200_train_step_aux(const GsbTrainStepArgs *t, const GsbSupervisionArgs *s) { return gsb200_train_step_ext(t, s, nullptr); }
+
+static bool aligned16(const void *p) { return reinterpret_cast<uintptr_t>(p) % 16 == 0; }
+
+// The feature term's own rules (gsb200_train_step_ext); the frame's were checked before.
+static int check_feature_train_args(const GsbFeatureTrainArgs &x, const GsbBackwardArgs &b, int H, int W) {
+    const GsbExtraFeatureArgs &e = x.features;
+    if (e.channels < 1 || e.channels > 16) {
+        set_error("train_step_ext: channels must be in 1..16 (got %d)", e.channels);
+        return GSB_EINVAL;
+    }
+    if (x.loss_kind != GSB_FEATURE_LOSS_CROSS_ENTROPY && x.loss_kind != GSB_FEATURE_LOSS_L2) {
+        set_error("train_step_ext: unknown feature loss kind %d", x.loss_kind);
+        return GSB_EINVAL;
+    }
+    const bool ce = x.loss_kind == GSB_FEATURE_LOSS_CROSS_ENTROPY;
+    if (ce && e.channels < 2) {
+        set_error("train_step_ext: the cross-entropy feature loss needs C >= 2 channels (got %d)", e.channels);
+        return GSB_EINVAL;
+    }
+    if (!(x.weight > 0.0f && x.weight <= 3.402823466e38f)) {
+        set_error("train_step_ext: the feature loss weight must be finite and > 0 (got %g)", (double)x.weight);
+        return GSB_EINVAL;
+    }
+    if ((ce ? (const void *)x.labels : (const void *)x.target) == nullptr) {
+        set_error("train_step_ext: the %s feature loss needs its target (%s)", ce ? "cross-entropy" : "l2",
+                  ce ? "labels" : "target");
+        return GSB_EINVAL;
+    }
+    if (!e.features || !e.rasterized || !e.grad_rasterized || !e.grad_features || !x.exp_avg || !x.exp_avg_sq ||
+        !x.loss_out2) {
+        set_error("train_step_ext: null features / rasterized / grad_rasterized / grad_features / exp_avg / exp_avg_sq / "
+                  "loss_out2 pointer");
+        return GSB_EINVAL;
+    }
+    if (!x.temp || !aligned16(x.temp) || x.temp_bytes < gsb200_feature_loss_temp_bytes(H, W)) {
+        set_error("train_step_ext: feature temp null, not 16-byte aligned or smaller than gsb200_feature_loss_temp_bytes(H, W) "
+                  "(temp_bytes=%lld)", (long long)x.temp_bytes);
+        return GSB_EINVAL;
+    }
+    if (!aligned16(e.features) || !aligned16(e.grad_features) || !aligned16(x.exp_avg) || !aligned16(x.exp_avg_sq)) {
+        set_error("train_step_ext: features, grad_features, exp_avg and exp_avg_sq must be 16-byte aligned");
+        return GSB_EINVAL;
+    }
+    if (!(b.flags & GSB_FLAG_BACKWARD_TRANSPOSED)) {
+        set_error("train_step_ext: the feature gradient needs the transposed backward kernel (GSB_FLAG_BACKWARD_TRANSPOSED)");
+        return GSB_EUNSUPPORTED;
+    }
+    return GSB_OK;
+}
+
+int gsb200_train_step_ext(const GsbTrainStepArgs *t, const GsbSupervisionArgs *s, const GsbFeatureTrainArgs *x) {
     if (!t || !t->ground_truth_image || !t->loss_out3 || !t->loss_temp || !t->feature_exp_avg || !t->feature_exp_avg_sq ||
         !t->position_exp_avg || !t->position_exp_avg_sq || t->step < 1) {
         set_error("train_step: null pointer argument or step < 1");
@@ -384,6 +435,11 @@ int gsb200_train_step_aux(const GsbTrainStepArgs *t, const GsbSupervisionArgs *s
     }
     const GsbForwardArgs &f = t->forward;
     const GsbBackwardArgs &b = t->backward;
+    if (x && (b.flags & GSB_FLAG_COMPACT_GRADS)) {
+        set_error("train_step_ext: the feature gradient is not carried by the compact rows of the view-parallel exchange "
+                  "(GSB_FLAG_COMPACT_GRADS)");
+        return GSB_EUNSUPPORTED;
+    }
     if (f.rgb_only || f.num_points != b.num_points || f.workspace != b.workspace || f.camera_height != b.camera_height ||
         f.camera_width != b.camera_width || f.stream != b.stream || b.accum_rows < f.num_points ||
         (b.flags & GSB_FLAG_COMPACT_GRADS) || !b.grad_rasterized_image || !b.grad_pointcloud || !b.grad_pointcloud_features ||
@@ -433,9 +489,11 @@ int gsb200_train_step_aux(const GsbTrainStepArgs *t, const GsbSupervisionArgs *s
     }
     const bool supervised = depth_on || alpha_on;
     const int H = f.camera_height, W = f.camera_width;
+    int rc;
+    if (x && (rc = check_feature_train_args(*x, b, H, W)) != GSB_OK) return rc;
+    const GsbExtraFeatureArgs *ext = x ? &x->features : nullptr;
     cudaStream_t st = static_cast<cudaStream_t>(f.stream);
-    int rc = gsb200_forward(&f);
-    if (rc != GSB_OK) return rc;
+    if ((rc = gsb200_forward_ext(&f, ext)) != GSB_OK) return rc;
     const float *loss_image = f.rasterized_image, *loss_gt = t->ground_truth_image;
     if (supervised && (rc = launch_supervision_pre(*s, f.rasterized_image, t->ground_truth_image, f.pixel_accumulated_alpha,
                                                    f.rasterized_depth, H, W, st, &loss_image, &loss_gt)) != GSB_OK)
@@ -446,8 +504,9 @@ int gsb200_train_step_aux(const GsbTrainStepArgs *t, const GsbSupervisionArgs *s
     if (supervised && (rc = launch_supervision_post(*s, f.rasterized_image, t->ground_truth_image, f.pixel_accumulated_alpha,
                                                     f.rasterized_depth, H, W, b.grad_rasterized_image, t->loss_out3, st)) != GSB_OK)
         return rc;
+    if (x && (rc = launch_feature_loss(*x, H, W, st)) != GSB_OK) return rc;
     if ((rc = backward_impl(&b, true, depth_on ? s->grad_depth : nullptr, depth_on ? f.rasterized_depth : nullptr,
-                            alpha_on ? s->grad_pixel_accumulated_alpha : nullptr)) != GSB_OK)
+                            alpha_on ? s->grad_pixel_accumulated_alpha : nullptr, ext)) != GSB_OK)
         return rc;
     Workspace ws;
     if ((rc = resolve_fwd(&f, &ws)) != GSB_OK) return rc;
@@ -456,8 +515,11 @@ int gsb200_train_step_aux(const GsbTrainStepArgs *t, const GsbSupervisionArgs *s
                           (long long)f.num_points * GSB_FEATURE_DIM, t->feature_learning_rate, t->beta1, t->beta2, t->eps, t->step,
                           skip, st);
     if (rc != GSB_OK) return rc;
-    return launch_adam_step(const_cast<float *>(f.pointcloud), b.grad_pointcloud, t->position_exp_avg, t->position_exp_avg_sq,
-                            (long long)f.num_points * 3, t->position_learning_rate, t->beta1, t->beta2, t->eps, t->step, skip, st);
+    rc = launch_adam_step(const_cast<float *>(f.pointcloud), b.grad_pointcloud, t->position_exp_avg, t->position_exp_avg_sq,
+                          (long long)f.num_points * 3, t->position_learning_rate, t->beta1, t->beta2, t->eps, t->step, skip, st);
+    if (rc != GSB_OK || !x) return rc;
+    return launch_adam_step(const_cast<float *>(ext->features), ext->grad_features, x->exp_avg, x->exp_avg_sq,
+                            (long long)f.num_points * ext->channels, x->learning_rate, t->beta1, t->beta2, t->eps, t->step, skip, st);
 }
 
 int gsb200_expand_view_gradients(const GsbExpandArgs *a) {

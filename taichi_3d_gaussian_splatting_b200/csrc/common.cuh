@@ -89,6 +89,8 @@ int launch_supervision_pre(const GsbSupervisionArgs &s, const float *image, cons
 int launch_supervision_post(const GsbSupervisionArgs &s, const float *image, const float *gt, const float *alpha,
                             const float *depth, int H, int W, const float *grad_image, const float *image_loss,
                             cudaStream_t stream);
+// feature_loss.cu: both passes of the feature term (arguments checked by gsb200_train_step_ext)
+int launch_feature_loss(const GsbFeatureTrainArgs &x, int H, int W, cudaStream_t stream);
 int launch_blend_forward_count(const GsbForwardArgs &a, const Workspace &ws, unsigned long long *counters_dev,
                                cudaStream_t stream);
 int launch_blend_backward_work(const GsbBackwardArgs &a, const Workspace &ws, unsigned long long *counters_dev,

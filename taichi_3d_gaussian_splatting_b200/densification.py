@@ -78,6 +78,8 @@ class GaussianPointAdaptiveController:
         pointcloud_features: torch.Tensor  # [num_points, 56]
         point_invalid_mask: torch.Tensor  # [num_points] int8
         point_object_id: torch.Tensor  # [num_points] int32
+        # [num_points, C] or None: per-Gaussian feature vectors (an extension); a clone or split copies its source's row
+        point_extra_features: Optional[torch.Tensor] = None
 
     @dataclass
     class GaussianPointAdaptiveControllerDensifyPointInfo:
@@ -268,6 +270,8 @@ class GaussianPointAdaptiveController:
             xyz[slots] = info.densify_point_position_before_optimization[:filled]
             feat[slots] = feat[src]
             mp.point_object_id[slots] = mp.point_object_id[src]
+            if mp.point_extra_features is not None:
+                mp.point_extra_features[slots] = mp.point_extra_features[src]
             feat[slots, 4:7] -= shrink
             feat[src, 4:7] -= shrink
             split = (shrink > 1e-6).reshape(-1)

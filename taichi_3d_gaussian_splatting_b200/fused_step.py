@@ -14,6 +14,10 @@ the skipped iteration in ``num_skipped_steps``.  CUDA only; there is no CPU path
 Optional supervision terms (``depth_weight``, ``mask_weight``, ``run(..., targets=, background=)``): a masked-L1 depth loss,
 an L1 mask loss on the accumulated alpha and training on a background colour, in the same one call
 (``gsb200_train_step_aux``; ``loss.supervision_loss`` states the loss in torch).
+
+Optional feature term (``extra_features``, ``feature_loss``, ``run(..., targets=SupervisionTargets(labels=... | features=...))``):
+per-Gaussian feature vectors F (N, C) rendered alongside the image, a cross-entropy or l2 loss on the rendered (H, W, C) map
+and an Adam step on F, in the same one call (``gsb200_train_step_ext``; ``loss.feature_loss`` states the loss in torch).
 """
 import ctypes
 import warnings
@@ -24,7 +28,7 @@ import torch
 
 from . import _lib
 from .GaussianPointCloudRasterisation import Frame, GaussianPointCloudRasterisation, _ptr
-from .loss import SupervisionTargets
+from .loss import FEATURE_LOSSES, SupervisionTargets
 
 __all__ = ["FusedTrainStep", "SupervisionTargets"]
 
@@ -32,15 +36,26 @@ __all__ = ["FusedTrainStep", "SupervisionTargets"]
 class FusedTrainStep:
     def __init__(self, scene, rasterisation_config, lambda_value: float = 0.2, controller=None, betas=(0.9, 0.999),
                  eps: float = 1e-8, key_capacity: Optional[int] = None, depth_weight: float = 0.0,
-                 mask_weight: float = 0.0):
+                 mask_weight: float = 0.0, extra_features: Optional[torch.Tensor] = None, feature_loss: Optional[str] = None,
+                 feature_weight: float = 1.0, extra_feature_learning_rate: float = 1e-2):
         """``scene``: object with ``point_cloud`` (N,3), ``point_cloud_features`` (N,56), ``point_invalid_mask``,
         ``point_object_id`` (CUDA, contiguous; updated in place).  ``controller``: a ``GaussianPointAdaptiveController`` whose
         six accumulators are updated by the backward epilogue (or ``None``).  ``depth_weight`` / ``mask_weight``: weights of
-        the depth and mask terms (``loss.supervision_loss``); they need the matching target in ``run(targets=...)``."""
+        the depth and mask terms (``loss.supervision_loss``); they need the matching target in ``run(targets=...)``.
+        ``extra_features``: (N, C) float32 per-Gaussian feature vectors (CUDA, contiguous, 1 <= C <= 16; updated in place by
+        their own Adam at ``extra_feature_learning_rate``), trained with ``feature_loss`` ("cross_entropy": needs
+        ``targets.labels`` and C >= 2; "l2": needs ``targets.features``) weighted by ``feature_weight``
+        (``loss.feature_loss``)."""
         for name, w in (("depth_weight", depth_weight), ("mask_weight", mask_weight)):
             if not (w >= 0.0 and w < float("inf")):
                 raise ValueError(f"{name} must be finite and >= 0, got {w}")
         self.depth_weight, self.mask_weight = float(depth_weight), float(mask_weight)
+        self.extra_features = extra_features
+        self.feature_loss_kind = feature_loss
+        self.feature_weight = float(feature_weight)
+        self.extra_feature_learning_rate = float(extra_feature_learning_rate)
+        if (extra_features is None) != (feature_loss is None):
+            raise ValueError("extra_features and feature_loss must be given together")
         self.scene = scene
         self.config = rasterisation_config
         self.lambda_value = float(lambda_value)
@@ -66,6 +81,17 @@ class FusedTrainStep:
         self.grad_pointcloud_features = self._flat[off:off + 56 * N].view(N, 56)
         self.loss = z(3)  # {loss, L1, 1 - SSIM} of the latest iteration (device); with supervision terms: of the image loss
         self.supervision_loss = z(3)  # {total, mask term, depth term} of the latest supervised iteration (device)
+        self.feature_loss = z(2)  # {feature term, n_supervised} of the latest iteration with features (device)
+        if extra_features is not None:
+            self.C = self._check_extra_features(extra_features)
+            if feature_loss not in FEATURE_LOSSES:
+                raise ValueError(f"feature_loss must be one of {FEATURE_LOSSES}, got {feature_loss!r}")
+            if feature_loss == "cross_entropy" and self.C < 2:
+                raise ValueError(f'feature_loss "cross_entropy" needs C >= 2 channels, got {self.C}')
+            if not (self.feature_weight > 0.0 and self.feature_weight < float("inf")):
+                raise ValueError(f"feature_weight must be finite and > 0, got {feature_weight}")
+            self.extra_feature_exp_avg, self.extra_feature_exp_avg_sq = z(N, self.C), z(N, self.C)
+            self.grad_extra_features = z(N, self.C)
         self._res = {}
         self._pinned = [torch.zeros(4, dtype=torch.int64).pin_memory() for _ in range(2)]
         self._events = [torch.cuda.Event() for _ in range(2)]
@@ -73,6 +99,14 @@ class FusedTrainStep:
             e.record()
         self._pending = [False, False]
         self._last = None
+
+    def _check_extra_features(self, F) -> int:
+        if not isinstance(F, torch.Tensor) or F.dim() != 2 or F.shape[0] != self.N or not 1 <= F.shape[1] <= 16:
+            raise ValueError(f"extra_features must be an (N, C) tensor with N = {self.N} and 1 <= C <= 16, got "
+                             f"{tuple(F.shape) if isinstance(F, torch.Tensor) else type(F).__name__}")
+        if F.dtype != torch.float32 or F.device != self.device or not F.is_contiguous() or F.data_ptr() % 16:
+            raise ValueError(f"extra_features must be a contiguous, 16-byte aligned float32 tensor on {self.device}")
+        return int(F.shape[1])
 
     # ------------------------------------------------------------------ per-resolution buffers
     def _buffers(self, H, W, n_obj):
@@ -91,6 +125,11 @@ class FusedTrainStep:
                                 temp_bytes=temp_bytes, grad_depth=e((H, W)), grad_alpha=e((H, W)),
                                 sup_temp=torch.zeros((sup_bytes + 15) // 16 * 16, dtype=torch.uint8, device=dev),
                                 sup_bytes=sup_bytes)
+            if self.extra_features is not None:
+                feat_bytes = int(self._lib.gsb200_feature_loss_temp_bytes(H, W))
+                b.feature_map, b.grad_feature_map = e((H, W, self.C)), e((H, W, self.C))
+                b.feat_temp = torch.zeros((feat_bytes + 15) // 16 * 16, dtype=torch.uint8, device=dev)
+                b.feat_bytes = feat_bytes
             self._res[key] = b
         return b
 
@@ -112,9 +151,11 @@ class FusedTrainStep:
     def run(self, image_gt: torch.Tensor, q_pointcloud_camera: torch.Tensor, t_pointcloud_camera: torch.Tensor, camera_info,
             color_max_sh_band: int, feature_learning_rate: float, position_learning_rate: float,
             targets: Optional[SupervisionTargets] = None, background: Optional[torch.Tensor] = None) -> None:
-        """``targets``: the view's depth and / or mask target ((H, W) float32 CUDA tensors); ``background``: a (3,) float32
-        CUDA tensor the image is composited on (read on the device when the step runs, so it may be refilled per iteration).
-        Without supervision terms this is ``gsb200_train_step``; with them ``gsb200_train_step_aux``."""
+        """``targets``: the view's depth and / or mask target ((H, W) float32 CUDA tensors) and, with ``extra_features``, its
+        ``labels`` ((H, W) int32) or ``features`` ((H, W, C) float32); ``background``: a (3,) float32 CUDA tensor the image is
+        composited on (read on the device when the step runs, so it may be refilled per iteration).  Without supervision
+        terms or features this is ``gsb200_train_step``; with supervision terms ``gsb200_train_step_aux``; with features
+        ``gsb200_train_step_ext``."""
         sc, cfg = self.scene, self.config
         H, W = int(camera_info.camera_height), int(camera_info.camera_width)
         if image_gt.shape != (3, H, W) or not image_gt.is_contiguous() or image_gt.dtype != torch.float32:
@@ -132,6 +173,15 @@ class FusedTrainStep:
                                   or x.device != image_gt.device):
                 raise ValueError(f"{name} must be a contiguous float32 {shape} tensor on {image_gt.device}")
         supervised = depth_t is not None or self.mask_weight > 0 or background is not None
+        feat_t = None
+        if self.extra_features is not None:
+            ce = self.feature_loss_kind == "cross_entropy"
+            name, feat_t = ("targets.labels", targets.labels) if ce else ("targets.features", targets.features)
+            shape, dtype = ((H, W), torch.int32) if ce else ((H, W, self.C), torch.float32)
+            if feat_t is None or tuple(feat_t.shape) != shape or not feat_t.is_contiguous() or feat_t.dtype != dtype \
+                    or feat_t.device != image_gt.device:
+                raise ValueError(f'feature_loss "{self.feature_loss_kind}" needs {name}: a contiguous {dtype} {shape} '
+                                 f"tensor on {image_gt.device}")
         self._check_previous()
         q, t = q_pointcloud_camera.contiguous(), t_pointcloud_camera.contiguous()
         K = camera_info.camera_intrinsics.contiguous()
@@ -187,18 +237,37 @@ class FusedTrainStep:
                     background=_ptr(background) if background is not None else None, depth_weight=self.depth_weight,
                     mask_weight=self.mask_weight, grad_depth=_ptr(b.grad_depth), grad_pixel_accumulated_alpha=_ptr(b.grad_alpha),
                     loss_out3=_ptr(self.supervision_loss), temp=_ptr(b.sup_temp), temp_bytes=b.sup_bytes)
+            if feat_t is not None:
+                ext = _lib.GsbExtraFeatureArgs(channels=self.C, features=_ptr(self.extra_features), rasterized=_ptr(b.feature_map),
+                                               grad_rasterized=_ptr(b.grad_feature_map),
+                                               grad_features=_ptr(self.grad_extra_features))
+                ce = self.feature_loss_kind == "cross_entropy"
+                fx = _lib.GsbFeatureTrainArgs(
+                    features=ext, loss_kind=_lib.GSB_FEATURE_LOSS_CROSS_ENTROPY if ce else _lib.GSB_FEATURE_LOSS_L2,
+                    weight=self.feature_weight, labels=_ptr(feat_t) if ce else None, target=None if ce else _ptr(feat_t),
+                    loss_out2=_ptr(self.feature_loss), temp=_ptr(b.feat_temp), temp_bytes=b.feat_bytes,
+                    exp_avg=_ptr(self.extra_feature_exp_avg), exp_avg_sq=_ptr(self.extra_feature_exp_avg_sq),
+                    learning_rate=self.extra_feature_learning_rate)
+                _lib.check(self._lib.gsb200_train_step_ext(ctypes.byref(args), ctypes.byref(sup) if supervised else None,
+                                                           ctypes.byref(fx)), "gsb200_train_step_ext")
+            elif supervised:
                 _lib.check(self._lib.gsb200_train_step_aux(ctypes.byref(args), ctypes.byref(sup)), "gsb200_train_step_aux")
             else:
                 _lib.check(self._lib.gsb200_train_step(ctypes.byref(args)), "gsb200_train_step")
         self._pending[slot] = True
         self._last = SimpleNamespace(buffers=b, H=H, W=W, slot=slot, supervised=supervised,
-                                     keep=(q, t, K, image_gt, depth_t, mask_t, background))
+                                     keep=(q, t, K, image_gt, depth_t, mask_t, background, feat_t))
 
     # ------------------------------------------------------------------ the latest frame, on demand (these calls wait)
     @property
     def image(self) -> torch.Tensor:
         """(H,W,3) rasterised image of the latest iteration (before the clamp)."""
         return self._last.buffers.image
+
+    @property
+    def feature_map(self) -> torch.Tensor:
+        """(H,W,C) rendered feature map of the latest iteration (with ``extra_features``)."""
+        return self._last.buffers.feature_map
 
     def hook_input(self) -> "GaussianPointCloudRasterisation.BackwardValidPointHookInput":
         """The latest iteration's ``BackwardValidPointHookInput`` (GPCR:806-817): built only when the controller looks for

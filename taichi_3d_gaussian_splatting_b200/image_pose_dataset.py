@@ -15,13 +15,16 @@ With ``with_targets=True`` (an extension) items get a fifth element, ``loss.Supe
 keys ``depth_path`` (``.npy`` float32 (H, W) at the resolution of the image on disk, point-cloud units along the optical
 axis, 0 or NaN = no measurement) and ``mask_path`` (any image: its last channel / 255, so the alpha of an RGBA file or a
 grey mask), cropped and autoscaled with the image: the mask with the image's antialiased resize, the depth with nearest
-neighbour so that a sparse map stays sparse.
+neighbour so that a sparse map stays sparse.  Two more optional keys carry targets for per-Gaussian feature training:
+``labels_path`` (``.npy`` integer (H, W) class ids, read as int32; outside [0, C) = no label) and ``features_path``
+(``.npy`` float32 (H, W, C); NaN = no target), both at the resolution of the image on disk and cropped and autoscaled with
+the image by nearest neighbour.
 Pinned against the reference class itself: ``tests/golden/make_dataset_golden.py`` imports it (Taichi stubbed) and
 stores its outputs for a small generated dataset; ``tests/test_dataset_cpu.py`` compares.
 """
 import json
 import os
-from typing import List, Tuple
+from typing import List, Optional, Tuple
 
 import numpy as np
 import torch
@@ -88,8 +91,20 @@ class ImagePoseDataset(torch.utils.data.Dataset):
             path = os.path.join(self.root, path)
         return path
 
-    def _load_targets(self, rec: dict, height: int, width: int) -> Tuple[torch.Tensor, torch.Tensor]:
-        """(depth, mask), each (H, W) float32 at the resolution of the image on disk, or None."""
+    def _load_npy(self, rec: dict, key: str, dtype, height: int, width: int, what: str) -> Optional[torch.Tensor]:
+        if not rec.get(key):
+            return None
+        arr = np.load(self._path(rec[key]))
+        if dtype == np.int32 and not np.issubdtype(arr.dtype, np.integer):
+            raise ValueError(f"{rec[key]}: {what} must be integer, got {arr.dtype}")
+        x = torch.from_numpy(np.ascontiguousarray(arr, dtype=dtype))
+        if tuple(x.shape[:2]) != (height, width) or x.dim() != (2 if dtype == np.int32 else 3):
+            raise ValueError(f"{rec[key]}: {what} is {tuple(x.shape)}, the image is {(height, width)}")
+        return x
+
+    def _load_targets(self, rec: dict, height: int, width: int) -> Tuple[torch.Tensor, ...]:
+        """(depth, mask, labels, features) at the resolution of the image on disk, or None each: depth and mask (H, W)
+        float32, labels (H, W) int32, features (H, W, C) float32."""
         depth = mask = None
         if rec.get("depth_path"):
             depth = torch.from_numpy(np.ascontiguousarray(np.load(self._path(rec["depth_path"])), dtype=np.float32))
@@ -100,9 +115,31 @@ class ImagePoseDataset(torch.utils.data.Dataset):
             mask = m[-1].contiguous()
             if tuple(mask.shape) != (height, width):
                 raise ValueError(f"{rec['mask_path']}: mask is {tuple(mask.shape)}, the image is {(height, width)}")
-        return depth, mask
+        labels = self._load_npy(rec, "labels_path", np.int32, height, width, "label map")
+        features = self._load_npy(rec, "features_path", np.float32, height, width, "feature map")
+        return depth, mask, labels, features
 
-    def _crop_and_scale_targets(self, depth, mask, info: CameraInfo) -> SupervisionTargets:
+    @staticmethod
+    def _crop_and_scale_nearest(x: torch.Tensor, info: CameraInfo) -> torch.Tensor:
+        """(H, W, ...) -> the image's size: cropped to the tile multiple and, if the image was autoscaled, resampled by
+        nearest neighbour -- the pixels a nearest-neighbour resize of the image would pick, for any dtype (the pixel indices
+        are resized, not the values)."""
+        h = x.shape[0] - x.shape[0] % TILE_HEIGHT
+        w = x.shape[1] - x.shape[1] % TILE_WIDTH
+        x = x[:h, :w]
+        if max(h, w) > MAX_RESOLUTION_TRAIN:
+            import torchvision.transforms.functional as TF
+            idx = torch.arange(h * w, dtype=torch.float64).reshape(1, h, w)
+            idx = TF.resize(idx, size=1024, max_size=MAX_RESOLUTION_TRAIN, interpolation=TF.InterpolationMode.NEAREST,
+                            antialias=False)
+            idx = _crop_to_tiles(idx)[0].long()
+            x = x.reshape(h * w, *x.shape[2:])[idx]
+        if tuple(x.shape[:2]) != (info.camera_height, info.camera_width):
+            raise ValueError(f"target size {tuple(x.shape[:2])} does not match the image's "
+                             f"{(info.camera_height, info.camera_width)}")
+        return x.contiguous()
+
+    def _crop_and_scale_targets(self, depth, mask, labels, features, info: CameraInfo) -> SupervisionTargets:
         """The targets cropped to the tile multiple and, if the image was autoscaled, resized to its size."""
         out = []
         for x, nearest in ((depth, True), (mask, False)):
@@ -119,7 +156,8 @@ class ImagePoseDataset(torch.utils.data.Dataset):
                                      f"{(info.camera_height, info.camera_width)}")
                 x = x.contiguous()
             out.append(x)
-        return SupervisionTargets(depth=out[0], mask=out[1])
+        labels, features = (None if x is None else self._crop_and_scale_nearest(x, info) for x in (labels, features))
+        return SupervisionTargets(depth=out[0], mask=out[1], labels=labels, features=features)
 
     def __getitem__(self, idx: int):
         rec = self.records[idx]
@@ -132,11 +170,11 @@ class ImagePoseDataset(torch.utils.data.Dataset):
         K[0, :] = K[0, :] * image.shape[2] / rec["camera_width"]
         K[1, :] = K[1, :] * image.shape[1] / rec["camera_height"]
         if self.with_targets:
-            depth, mask = self._load_targets(rec, image.shape[1], image.shape[2])
+            targets = self._load_targets(rec, image.shape[1], image.shape[2])
         image = _crop_to_tiles(image)
         info = CameraInfo(camera_intrinsics=K, camera_height=image.shape[1], camera_width=image.shape[2],
                           camera_id=rec["camera_id"])
         image, info = self._autoscale_image_and_camera_info(image, info)
         if self.with_targets:
-            return image, q, t, info, self._crop_and_scale_targets(depth, mask, info)
+            return image, q, t, info, self._crop_and_scale_targets(*targets, info)
         return image, q, t, info

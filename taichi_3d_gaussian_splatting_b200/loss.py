@@ -165,9 +165,49 @@ def fused_image_loss(rasterized_image: torch.Tensor, ground_truth_image: torch.T
 @dataclass
 class SupervisionTargets:
     """Optional per-view targets besides the image: ``depth`` (H, W) float32 in point-cloud units along the optical axis
-    (0 or NaN = no measurement, e.g. sparse LiDAR) and ``mask`` (H, W) float32 in [0, 1] (1 = object)."""
+    (0 or NaN = no measurement, e.g. sparse LiDAR) and ``mask`` (H, W) float32 in [0, 1] (1 = object); for a loss on the
+    rendered per-Gaussian feature map (:func:`feature_loss`), ``labels`` (H, W) int32 class ids (outside [0, C) = no label)
+    or ``features`` (H, W, C) float32 (a pixel with a non-finite value = no target)."""
     depth: Optional[torch.Tensor] = None
     mask: Optional[torch.Tensor] = None
+    labels: Optional[torch.Tensor] = None
+    features: Optional[torch.Tensor] = None
+
+
+FEATURE_LOSSES = ("cross_entropy", "l2")
+
+
+def feature_loss(feature_map: torch.Tensor, targets: SupervisionTargets, kind: str, weight: float) -> torch.Tensor:
+    """The loss on the rendered (H, W, C) feature map ``F`` (the operator's ``point_extra_features`` output); the fused train
+    step (``gsb200_train_step_ext`` / ``csrc/feature_loss.cu``) computes the same:
+
+    * ``"cross_entropy"`` (semantic labels, C >= 2): ``weight * sum_labelled CE(softmax(F_p), label_p) / max(n_labelled, 1)``
+      on ``targets.labels`` (H, W) int32, a pixel labelled when ``0 <= label < C``;
+    * ``"l2"`` (distilled feature maps): ``weight * sum_supervised sum_c (F_pc - T_pc)^2 / max(n_supervised * C, 1)`` on
+      ``targets.features`` (H, W, C), a pixel supervised when all C of its values are finite.
+
+    Unsupervised pixels contribute nothing and get a zero gradient.  Returns the term as a 0-dim tensor."""
+    C = feature_map.shape[-1]
+    if kind == "cross_entropy":
+        if targets.labels is None:
+            raise ValueError('feature loss "cross_entropy" needs targets.labels')
+        if C < 2:
+            raise ValueError(f'feature loss "cross_entropy" needs C >= 2 channels, got {C}')
+        labels = targets.labels.long()
+        valid = (labels >= 0) & (labels < C)
+        safe = torch.where(valid, labels, torch.zeros_like(labels))
+        nll = -torch.log_softmax(feature_map, dim=-1).gather(-1, safe[..., None])[..., 0]  # max-subtracted log-sum-exp
+        err = torch.where(valid, nll, torch.zeros_like(nll))
+        return weight * err.sum() / valid.sum().clamp_min(1)
+    if kind == "l2":
+        if targets.features is None:
+            raise ValueError('feature loss "l2" needs targets.features')
+        T = targets.features
+        valid = torch.isfinite(T).all(dim=-1)
+        safe = torch.where(valid[..., None], T, torch.zeros_like(T))  # no NaN reaches the gradient of the unused branch
+        err = torch.where(valid[..., None], (feature_map - safe) ** 2, torch.zeros_like(T))
+        return weight * err.sum() / (valid.sum() * C).clamp_min(1)
+    raise ValueError(f"feature loss must be one of {FEATURE_LOSSES}, got {kind!r}")
 
 
 def _torch_image_loss(rasterized_image, ground_truth_image, lambda_value):

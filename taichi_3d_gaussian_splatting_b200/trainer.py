@@ -11,6 +11,10 @@ Optional supervision (an extension; ``TrainConfig.depth_loss_weight`` / ``mask_l
 ``SupervisionTargets`` as a fifth view element): a masked-L1 depth loss, an L1 mask loss on the accumulated alpha and
 training on a white or random background, with the same loss (``loss.supervision_loss``) in the autograd loop and in the
 fused step.
+Optional feature training (an extension; ``Scene.point_extra_features``, ``TrainConfig.feature_loss``, per-view
+``SupervisionTargets.labels`` / ``features``): per-Gaussian feature vectors rendered alongside the image, a cross-entropy or
+l2 loss on the rendered feature map (``loss.feature_loss``) and a third Adam on the features, kept in step with the scene
+through densification.
 The rasteriser is injected (default: the CUDA operator) so that tests can run the identical loop with the
 CPU oracle behind the same interface and compare PSNR trajectories.
 """
@@ -24,7 +28,7 @@ import torch.nn.functional as F
 from .Camera import CameraInfo
 from .densification import GaussianPointAdaptiveController
 from .GaussianPointCloudRasterisation import GaussianPointCloudRasterisation
-from .loss import LossFunction, SupervisionTargets, supervision_loss
+from .loss import FEATURE_LOSSES, LossFunction, SupervisionTargets, feature_loss, supervision_loss
 
 View = Tuple[torch.Tensor, torch.Tensor, torch.Tensor, CameraInfo]  # image (3,H,W) in [0,1], q (1,4), t (1,3), camera
 # ... optionally followed by a SupervisionTargets (depth and / or mask at the image's resolution)
@@ -52,9 +56,20 @@ def downsample_image_and_camera_info(image: torch.Tensor, camera_info: CameraInf
     return image, CameraInfo(camera_intrinsics=K, camera_height=h, camera_width=w, camera_id=camera_info.camera_id)
 
 
+def _nearest(x: torch.Tensor, h: int, w: int, hc: int, wc: int) -> torch.Tensor:
+    """(H, W, ...) -> (hc, wc, ...): the rows and columns ``F.interpolate(mode="nearest")`` picks for an (h, w) output,
+    cropped; exact for any dtype (the indices are resized, not the values)."""
+    rows = F.interpolate(torch.arange(x.shape[0], dtype=torch.float32, device=x.device)[None, None], size=h,
+                         mode="nearest")[0, 0, :hc].long()
+    cols = F.interpolate(torch.arange(x.shape[1], dtype=torch.float32, device=x.device)[None, None], size=w,
+                         mode="nearest")[0, 0, :wc].long()
+    return x[rows][:, cols].contiguous()
+
+
 def downsample_targets(targets: SupervisionTargets, camera_info: CameraInfo, downsample_factor: int) -> SupervisionTargets:
-    """The targets of a view at the schedule's resolution: the mask with the image's antialiased resize, the depth with
-    nearest neighbour (a sparse map stays sparse, no depth is blended across an edge); both cropped like the image."""
+    """The targets of a view at the schedule's resolution: the mask with the image's antialiased resize, the depth, the
+    labels and the feature map with nearest neighbour (a sparse map stays sparse, nothing is blended across an edge); all
+    cropped like the image."""
     h = camera_info.camera_height // downsample_factor
     w = camera_info.camera_width // downsample_factor
     hc, wc = h - h % 16, w - w % 16
@@ -64,7 +79,9 @@ def downsample_targets(targets: SupervisionTargets, camera_info: CameraInfo, dow
                              align_corners=False)[0, 0, :hc, :wc].contiguous()
     if targets.depth is not None:
         depth = F.interpolate(targets.depth[None, None], size=(h, w), mode="nearest")[0, 0, :hc, :wc].contiguous()
-    return SupervisionTargets(depth=depth, mask=mask)
+    labels = None if targets.labels is None else _nearest(targets.labels, h, w, hc, wc)
+    features = None if targets.features is None else _nearest(targets.features, h, w, hc, wc)
+    return SupervisionTargets(depth=depth, mask=mask, labels=labels, features=features)
 
 
 @dataclass
@@ -74,6 +91,7 @@ class Scene:
     point_cloud_features: torch.Tensor  # (N,56) leaf, requires_grad
     point_invalid_mask: torch.Tensor  # (N,) int8
     point_object_id: torch.Tensor  # (N,) int32
+    point_extra_features: Optional[torch.Tensor] = None  # (N, C) leaf, requires_grad: per-Gaussian feature vectors
 
 
 class GaussianPointCloudTrainer:
@@ -100,6 +118,12 @@ class GaussianPointCloudTrainer:
         depth_loss_weight: float = 0.
         mask_loss_weight: float = 0.
         background: str = "black"
+        # optional feature training (loss.feature_loss): "none", "cross_entropy" (labels) or "l2" (feature maps) on the
+        # rendered map of Scene.point_extra_features, its weight (> 0 when on), and the learning rate of the features' own
+        # Adam.  The default learning rate is a starting point, not tuned.
+        feature_loss: str = "none"
+        feature_loss_weight: float = 0.
+        extra_feature_learning_rate: float = 1e-2
 
     def __init__(self, config: "GaussianPointCloudTrainer.TrainConfig", scene: Scene, train_views: List[View],
                  rasterisation_factory: Optional[Callable] = None, generator: Optional[torch.Generator] = None,
@@ -130,6 +154,9 @@ class GaussianPointCloudTrainer:
             raise ValueError("mask_loss_weight > 0 needs a mask on every view")
         if config.background == "random" and any(tg.mask is None for tg in targets):
             raise ValueError('background="random" needs a mask on every view (the ground truth is composited by it)')
+        self._features = config.feature_loss != "none"
+        if self._features:
+            self._check_feature_config(config, scene, targets)
         self.config = config
         self._need_depth = config.depth_loss_weight > 0
         self._need_alpha = config.mask_loss_weight > 0 or config.background != "black"
@@ -151,7 +178,8 @@ class GaussianPointCloudTrainer:
             config=config.adaptive_controller_config,
             maintained_parameters=GaussianPointAdaptiveController.GaussianPointAdaptiveControllerMaintainedParameters(
                 pointcloud=scene.point_cloud, pointcloud_features=scene.point_cloud_features,
-                point_invalid_mask=scene.point_invalid_mask, point_object_id=scene.point_object_id),
+                point_invalid_mask=scene.point_invalid_mask, point_object_id=scene.point_object_id,
+                point_extra_features=scene.point_extra_features if self._features else None),
             generator=generator, fused_update=fused_controller_update)
         factory = rasterisation_factory or GaussianPointCloudRasterisation
         # the differentiable outputs only when a term needs them: injected factories without them keep working
@@ -164,6 +192,34 @@ class GaussianPointCloudTrainer:
         self._downsampled = {}
         self._view_generator = shuffle_generator
         self._view_order = None
+
+    @staticmethod
+    def _check_feature_config(config, scene: Scene, targets: List[SupervisionTargets]) -> None:
+        if config.feature_loss not in FEATURE_LOSSES:
+            raise ValueError(f"feature_loss must be one of {('none',) + FEATURE_LOSSES}, got {config.feature_loss!r}")
+        w = config.feature_loss_weight
+        if not (w > 0.0 and w < float("inf")):
+            raise ValueError(f"feature_loss_weight must be finite and > 0 with a feature loss, got {w}")
+        Fx = scene.point_extra_features
+        if Fx is None:
+            raise ValueError(f'feature_loss="{config.feature_loss}" needs Scene.point_extra_features')
+        if Fx.dim() != 2 or Fx.shape[0] != scene.point_cloud.shape[0] or not 1 <= Fx.shape[1] <= 16:
+            raise ValueError(f"point_extra_features must be (N, C) with 1 <= C <= 16, got {tuple(Fx.shape)}")
+        C = int(Fx.shape[1])
+        if config.feature_loss == "cross_entropy":
+            if C < 2:
+                raise ValueError(f'feature_loss="cross_entropy" needs C >= 2 channels, got {C}')
+            if any(tg.labels is None for tg in targets):
+                raise ValueError('feature_loss="cross_entropy" needs labels on every view')
+            # one host read for all views: a label >= C is a class the features cannot express, not "no label"
+            dev = targets[0].labels.device if targets else None
+            top = int(torch.stack([tg.labels.max().to(dev, torch.int64) for tg in targets]).max()) if targets else -1
+            if top >= C:
+                raise ValueError(f"labels must be < C = {C} (negative = no label), got {top}")
+        elif any(tg.features is None for tg in targets):
+            raise ValueError('feature_loss="l2" needs a feature map on every view')
+        elif any(tuple(tg.features.shape[-1:]) != (C,) for tg in targets):
+            raise ValueError(f"the feature maps of the views must have C = {C} channels")
 
     def _input(self, q, t, camera_info, band):
         s = self.scene
@@ -184,7 +240,7 @@ class GaussianPointCloudTrainer:
             if key not in self._downsampled:
                 image_ds, camera_ds = downsample_image_and_camera_info(image_gt, camera_info, downsample_factor)
                 self._downsampled[key] = (image_ds, camera_ds, downsample_targets(targets, camera_info, downsample_factor)
-                                          if self.supervised else targets)
+                                          if self.supervised or self._features else targets)
             image_gt, camera_info, targets = self._downsampled[key]
         return image_gt, q, t, camera_info, targets
 
@@ -208,7 +264,10 @@ class GaussianPointCloudTrainer:
         cfg = self.config
         step = FusedTrainStep(self.scene, cfg.rasterisation_config, cfg.loss_function_config.lambda_value,
                               controller=self.adaptive_controller, depth_weight=cfg.depth_loss_weight,
-                              mask_weight=cfg.mask_loss_weight)
+                              mask_weight=cfg.mask_loss_weight,
+                              **(dict(extra_features=self.scene.point_extra_features, feature_loss=cfg.feature_loss,
+                                      feature_weight=cfg.feature_loss_weight,
+                                      extra_feature_learning_rate=cfg.extra_feature_learning_rate) if self._features else {}))
         self.fused_train_step = step
         position_lr = cfg.position_learning_rate
         downsample_factor = cfg.initial_downsample_factor
@@ -218,7 +277,7 @@ class GaussianPointCloudTrainer:
             view_index = self._next_view_index(iteration)
             image_gt, q, t, camera_info, targets = self._view(view_index, downsample_factor)
             band = iteration // cfg.increase_color_max_sh_band_interval
-            if self.supervised:
+            if self.supervised or self._features:
                 step.run(image_gt, q, t, camera_info, band, cfg.feature_learning_rate, position_lr, targets=targets,
                          background=self._next_background())
             else:
@@ -236,6 +295,9 @@ class GaussianPointCloudTrainer:
                     total, mask_term, depth_term = step.supervision_loss.tolist()
                     entry["loss"] = total
                     self._supervised_history(entry, mask_term, depth_term)
+                if self._features:
+                    entry["feature_loss"] = float(step.feature_loss[0])
+                    entry["loss"] += entry["feature_loss"]
                 self.history.append(entry)
         return self.history
 
@@ -261,6 +323,8 @@ class GaussianPointCloudTrainer:
             Adam = torch.optim.Adam
         optimizer = Adam([self.scene.point_cloud_features], lr=cfg.feature_learning_rate, betas=(0.9, 0.999))
         position_optimizer = Adam([self.scene.point_cloud], lr=cfg.position_learning_rate, betas=(0.9, 0.999))
+        extra_optimizer = Adam([self.scene.point_extra_features], lr=cfg.extra_feature_learning_rate,
+                               betas=(0.9, 0.999)) if self._features else None
         scheduler = torch.optim.lr_scheduler.ExponentialLR(position_optimizer, gamma=cfg.position_learning_rate_decay_rate)
         downsample_factor = cfg.initial_downsample_factor
         for iteration in range(cfg.num_iterations):
@@ -268,12 +332,14 @@ class GaussianPointCloudTrainer:
                 downsample_factor //= 2
             optimizer.zero_grad()
             position_optimizer.zero_grad()
+            if extra_optimizer is not None:
+                extra_optimizer.zero_grad()
             view_index = self._next_view_index(iteration)
             image_gt, q, t, camera_info, targets = self._view(view_index, downsample_factor)
             band = iteration // cfg.increase_color_max_sh_band_interval
-            if self.supervised:
-                loss, l1_loss, mask_term, depth_term, image_pred = self._supervised_loss(q, t, camera_info, band, image_gt,
-                                                                                         targets)
+            if self.supervised or self._features:
+                loss, l1_loss, mask_term, depth_term, feature_term, image_pred = self._supervised_loss(
+                    q, t, camera_info, band, image_gt, targets)
             elif self.fused_image_loss:
                 image_pred, _, _ = self.rasterisation(self._input(q, t, camera_info, band))
                 loss, l1_loss, ssim_loss = self.loss_function.forward_rasterized(
@@ -289,6 +355,8 @@ class GaussianPointCloudTrainer:
             loss.backward()
             optimizer.step()
             position_optimizer.step()
+            if extra_optimizer is not None:
+                extra_optimizer.step()
             if iteration % cfg.position_learning_rate_decay_interval == 0:
                 scheduler.step()
             self.adaptive_controller.refinement()
@@ -298,15 +366,21 @@ class GaussianPointCloudTrainer:
                              num_valid_points=int((self.scene.point_invalid_mask == 0).sum()))
                 if self.supervised:
                     self._supervised_history(entry, mask_term.detach(), depth_term.detach())
+                if self._features:
+                    entry["feature_loss"] = float(feature_term.detach())
                 self.history.append(entry)
         return self.history
 
     def _supervised_loss(self, q, t, camera_info, band, image_gt, targets):
         """Forward with the differentiable outputs the terms need, then ``loss.supervision_loss`` with this trainer's image
-        loss (the torch one, or the fused kernels with ``fused_image_loss``; the scale regulariser if enabled).  Returns
-        (total, L1, mask term, depth term, the raw image as (3, H, W) for the PSNR log)."""
+        loss (the torch one, or the fused kernels with ``fused_image_loss``; the scale regulariser if enabled), plus
+        ``loss.feature_loss`` on the rendered feature map with a feature loss.  Returns (total, L1, mask term, depth term,
+        feature term, the raw image as (3, H, W) for the PSNR log)."""
         cfg = self.config
-        outs = self.rasterisation(self._input(q, t, camera_info, band))
+        if self._features:
+            outs = self.rasterisation(self._input(q, t, camera_info, band), point_extra_features=self.scene.point_extra_features)
+        else:
+            outs = self.rasterisation(self._input(q, t, camera_info, band))
         image_pred, depth = outs[0], outs[1]
         alpha = outs[3] if self._need_alpha else None
         regulariser = dict(point_invalid_mask=self.scene.point_invalid_mask, pointcloud_features=self.scene.point_cloud_features)
@@ -318,7 +392,11 @@ class GaussianPointCloudTrainer:
         total, l1, _, mask_term, depth_term = supervision_loss(
             image_pred, depth, alpha, image_gt, targets, self._next_background(), cfg.loss_function_config.lambda_value,
             cfg.depth_loss_weight, cfg.mask_loss_weight, image_loss=image_loss)
-        return total, l1, mask_term, depth_term, image_pred.detach().clamp(0, 1).permute(2, 0, 1)
+        feature_term = None
+        if self._features:
+            feature_term = feature_loss(outs[-1], targets, cfg.feature_loss, cfg.feature_loss_weight)
+            total = total + feature_term
+        return total, l1, mask_term, depth_term, feature_term, image_pred.detach().clamp(0, 1).permute(2, 0, 1)
 
     @torch.no_grad()
     def validation(self, views: Optional[List[View]] = None) -> float:
