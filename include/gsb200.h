@@ -205,7 +205,7 @@ const char *gsb200_last_error(void);
  * foreign-language binding verify its struct mirrors. */
 void gsb200_abi_sizes(int64_t *out3);
 /* ... and of the first n of {GsbWorkspaceLayout, GsbForwardArgs, GsbBackwardArgs, GsbExpandArgs, GsbTrainStepArgs,
- * GsbSupervisionArgs, GsbExtraFeatureArgs, GsbFeatureTrainArgs} */
+ * GsbSupervisionArgs, GsbExtraFeatureArgs, GsbFeatureTrainArgs, GsbPoseGradArgs} */
 void gsb200_abi_sizes_ext(int64_t *out, int32_t n);
 
 /* Workspace sizing.  far_plane*depth_to_sort_key_scale fixes the depth-key width; (H/16)*(W/16)
@@ -287,6 +287,38 @@ int gsb200_backward_ext(const GsbBackwardArgs *args,
                         const float *rasterized_depth,
                         const float *grad_pixel_accumulated_alpha,
                         const GsbExtraFeatureArgs *ext);             /* or NULL */
+
+/* Camera-pose gradients (an extension: the reference differentiates the scene only).  pose_kernel (csrc/preprocess.cu)
+ * maps (q_pc, t_pc) of object o to T = [W | tw] with qi = conj(q_pc), W = R(qi) (the GP3D:30-48 polynomial on the
+ * components as given) and tw = -R(qn) t_pc, qn = qi / |qi|; a point of the object is at pc = W xyz + tw in the camera.
+ * The pose gradient is the exact derivative of the rendered outputs with respect to q_pc and t_pc through this map, under
+ * the conventions of the point gradients: J inside Sigma' = J W Sigma W^T J^T, the SH view direction and the rescale factor
+ * are detached, the 0.99 clamp is straight-through.  Per in-camera point, with gp = dL/dpc (through uv by the full-K
+ * projection Jacobian, plus dL/dz of the depth term) and G the (g00, g01, g11) weighting of dL/dSigma':
+ *   dL/dW += gp xyz^T + 2 J^T G (J W) Sigma,   dL/dtw += gp,
+ * summed per object and taken through the map above.  No gradient factor is applied; every loss term the backward takes
+ * (image, depth, alpha, features) contributes.  For one object with a unit q_pc, dL/dt_pc = -sum_i dL/dxyz_i.
+ * The sum is deterministic: the per-point kernel runs on min(ceil(N/128), GSB_POSE_PARTIAL_BLOCKS) CTAs, each writes its
+ * per-object sums to `temp` in a fixed order, and a second kernel adds them in block order -- no float atomics. */
+#define GSB_POSE_MAX_OBJECTS 64        /* per-warp pose rows live in shared memory */
+#define GSB_POSE_PARTIAL_BLOCKS 2048
+typedef struct GsbPoseGradArgs {
+    const float *q_pointcloud_camera;  /* (num_objects,4): the forward's input */
+    float *grad_q_pointcloud_camera;   /* (num_objects,4) out, fully written */
+    float *grad_t_pointcloud_camera;   /* (num_objects,3) out, fully written */
+    void *temp;                        /* gsb200_pose_grad_temp_bytes(num_objects) bytes, 16-byte aligned */
+} GsbPoseGradArgs;
+/* GSB_POSE_PARTIAL_BLOCKS * num_objects * 12 floats (0 for num_objects < 1) */
+int64_t gsb200_pose_grad_temp_bytes(int32_t num_objects);
+/* gsb200_backward_ext that also writes the pose gradients of `pose`.  Everything else the call writes (dense gradients,
+ * hook tensors, controller accumulators) is bit-identical to gsb200_backward_ext's.  NULL pose: exactly
+ * gsb200_backward_ext.  With pose, before any CUDA call: GSB_EINVAL for a NULL q / output / temp pointer, a temp that is
+ * not 16-byte aligned or num_objects < 1; GSB_EUNSUPPORTED for num_objects > GSB_POSE_MAX_OBJECTS or
+ * GSB_FLAG_COMPACT_GRADS.  An image-only loss works with either loop-A kernel; the other terms keep their requirement of
+ * GSB_FLAG_BACKWARD_TRANSPOSED. */
+int gsb200_backward_pose(const GsbBackwardArgs *args, const float *grad_rasterized_depth, const float *rasterized_depth,
+                         const float *grad_pixel_accumulated_alpha, const GsbExtraFeatureArgs *ext,
+                         const GsbPoseGradArgs *pose); /* or NULL */
 
 int gsb200_expand_view_gradients(const GsbExpandArgs *args);
 

@@ -237,6 +237,7 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
         gradient_exchange=None,
         differentiable_depth: bool = False,
         differentiable_alpha: bool = False,
+        differentiable_pose: bool = False,
     ):
         """``exact_exp``: blend kernels use ``expf`` instead of ``ex2.approx`` (parity debugging).
         ``force_key64``: sort the reference's 64-bit ``tile << 32 | depth`` keys even when the live
@@ -267,7 +268,16 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
         on a background as ``image + (1 - S)[..., None] * bg``, trains xyz, q, s and the opacity through the blend weights;
         a loss on S alone works too.  Combines with ``differentiable_depth``.  The hook sees the alpha loss's share as it
         sees the image loss's share.  Same requirements as ``differentiable_depth``: ``ValueError`` with
-        ``backward_impl="butterfly"`` or ``config.rgb_only``."""
+        ``backward_impl="butterfly"`` or ``config.rgb_only``.
+        ``differentiable_pose``: ``backward`` also returns dL/d ``q_pointcloud_camera`` (K, 4) and dL/d
+        ``t_pointcloud_camera`` (K, 3) for whichever of them requires grad (an extension: the reference differentiates the
+        scene only) -- to refine noisy training poses, relocalise a camera against a trained scene, or track rigid objects
+        (one pose per ``point_object_id``).  The gradient is exact through the pose map of the forward (q is conjugated,
+        normalised for the translation and taken as given for the rotation), with the point gradients' conventions (J and
+        the SH view direction detached), and includes every loss term the backward takes (image, depth, alpha, features);
+        no gradient factor is applied (``gsb200_backward_pose``).  With a frozen scene (only q / t require grad) the backward
+        still runs.  At most 64 objects.  An image-only loss works with either backward kernel.  Off, a pose that requires
+        grad gets ``None``.  ``ValueError`` with ``config.rgb_only`` or a ``gradient_exchange``."""
         super().__init__()
         for name, on in (("differentiable_depth", differentiable_depth), ("differentiable_alpha", differentiable_alpha)):
             if on and backward_impl == "butterfly":
@@ -277,6 +287,11 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                 raise ValueError(f"{name} needs the auxiliary outputs: config.rgb_only=True renders none")
         self.differentiable_depth = bool(differentiable_depth)
         self.differentiable_alpha = bool(differentiable_alpha)
+        if differentiable_pose and config.rgb_only:
+            raise ValueError("differentiable_pose needs the auxiliary outputs: config.rgb_only=True renders none")
+        if differentiable_pose and gradient_exchange is not None:
+            raise ValueError("differentiable_pose is not supported with a gradient_exchange (view-parallel training)")
+        self.differentiable_pose = bool(differentiable_pose)
         self.config = config
         self.backward_valid_point_hook = backward_valid_point_hook
         self._flags = (_lib.GSB_FLAG_EXACT_EXP if exact_exp else 0) | (_lib.GSB_FLAG_FORCE_KEY64 if force_key64 else 0) | \
@@ -308,6 +323,7 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                 ctx.save_for_backward(pointcloud, pointcloud_features, point_object_id,
                                       t_pointcloud_camera, saved["camera_intrinsics"], acc_alpha,
                                       last_effective, frame.ws, *((depth,) if outer.differentiable_depth else ()),
+                                      *((q_pointcloud_camera,) if outer.differentiable_pose else ()),
                                       *((extra_features,) if extra_features is not None else ()))
                 ctx.frame = frame
                 ctx.num_objects = q_pointcloud_camera.shape[0]
@@ -329,9 +345,11 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                 # grad_extra: dL/d pixel_accumulated_alpha (differentiable_alpha), then dL/d the feature map (extra features)
                 grad_pixel_accumulated_alpha = grad_extra[0] if outer.differentiable_alpha else None
                 grad_feature_map = grad_extra[-1] if ctx.has_extra_features else None
-                grad_pointcloud = grad_pointcloud_features = grad_extra_features = None
-                # GPCR:1028; with extra features the backward also runs for them alone (frozen geometry)
-                if ctx.needs_input_grad[0] or ctx.needs_input_grad[1] or (ctx.has_extra_features and ctx.needs_input_grad[8]):
+                grad_pointcloud = grad_pointcloud_features = grad_extra_features = grad_q = grad_t = None
+                pose = outer.differentiable_pose and (ctx.needs_input_grad[4] or ctx.needs_input_grad[5])
+                # GPCR:1028; with extra features (or pose gradients) the backward also runs for them alone (frozen scene)
+                if ctx.needs_input_grad[0] or ctx.needs_input_grad[1] or (ctx.has_extra_features and ctx.needs_input_grad[8]) \
+                        or pose:
                     if outer.config.rgb_only:
                         # the reference leaves accumulated alpha / last-effective offsets uninitialised in
                         # this mode (GPCR:478-484), so its backward is undefined; refuse instead
@@ -341,8 +359,15 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                         frame = ctx.frame
                         grad_rasterized_image = torch.zeros((frame.height, frame.width, 3), dtype=torch.float32,
                                                             device=frame.ws.device)
-                    grad_pointcloud, grad_pointcloud_features, grad_extra_features = outer._run_backward(
-                        ctx, grad_rasterized_image, grad_rasterized_depth, grad_pixel_accumulated_alpha, grad_feature_map)
+                    grad_pointcloud, grad_pointcloud_features, grad_extra_features, grad_q, grad_t = outer._run_backward(
+                        ctx, grad_rasterized_image, grad_rasterized_depth, grad_pixel_accumulated_alpha, grad_feature_map, pose)
+                if pose:
+                    grad_q = grad_q if ctx.needs_input_grad[4] else None
+                    grad_t = grad_t if ctx.needs_input_grad[5] else None
+                    return ((grad_pointcloud if ctx.needs_input_grad[0] else None,
+                             grad_pointcloud_features if ctx.needs_input_grad[1] else None, None, None, grad_q, grad_t, None,
+                             None) + ((grad_extra_features if ctx.needs_input_grad[8] else None,) if ctx.has_extra_features
+                                      else ()))
                 if ctx.has_extra_features:  # frozen geometry: None for the scene tensors that do not need a gradient
                     return (grad_pointcloud if ctx.needs_input_grad[0] else None,
                             grad_pointcloud_features if ctx.needs_input_grad[1] else None, None, None, None, None, None, None,
@@ -480,9 +505,9 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
 
     # ------------------------------------------------------------------ backward plumbing
     def _run_backward(self, ctx, grad_rasterized_image, grad_rasterized_depth=None, grad_pixel_accumulated_alpha=None,
-                      grad_feature_map=None):
-        """Returns dL/dxyz, dL/dfeatures and, for a call with extra features, dL/d of them ((N, C); zeros when the feature map
-        was not used)."""
+                      grad_feature_map=None, pose=False):
+        """Returns dL/dxyz, dL/dfeatures, for a call with extra features dL/d of them ((N, C); zeros when the feature map
+        was not used), and with ``pose`` dL/dq_pointcloud_camera (K, 4) and dL/dt_pointcloud_camera (K, 3) (else None)."""
         cfg = self.config
         lib = _lib.load()
         saved = ctx.saved_tensors
@@ -490,6 +515,7 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
          last_effective, ws) = saved[:8]
         # differentiable_depth: the depth gradient (None when the loss does not use depth) and the forward's depth map
         depth = saved[8] if self.differentiable_depth and grad_rasterized_depth is not None else None
+        q_pointcloud_camera = saved[8 + int(self.differentiable_depth)] if self.differentiable_pose else None
         extra_features = saved[-1] if ctx.has_extra_features else None
         frame: Frame = ctx.frame
         device = pointcloud.device
@@ -547,7 +573,25 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                 C = extra_features.shape[1]
                 grad_extra_features = torch.zeros((N, C), dtype=torch.float32, device=device) if grad_feature_map is None \
                     else torch.empty((N, C), dtype=torch.float32, device=device)
-            if extra_features is not None and grad_feature_map is not None:
+            grad_q = grad_t = None
+            if pose:
+                n_obj = ctx.num_objects
+                q_pc = q_pointcloud_camera.detach().contiguous()
+                grad_q = torch.empty((n_obj, 4), dtype=torch.float32, device=device)
+                grad_t = torch.empty((n_obj, 3), dtype=torch.float32, device=device)
+                pose_temp = torch.empty((max(int(lib.gsb200_pose_grad_temp_bytes(n_obj)), 16) // 4,), dtype=torch.float32,
+                                        device=device)
+                pose_args = _lib.GsbPoseGradArgs(q_pointcloud_camera=_ptr(q_pc), grad_q_pointcloud_camera=_ptr(grad_q),
+                                                 grad_t_pointcloud_camera=_ptr(grad_t), temp=_ptr(pose_temp))
+                ext = None
+                if extra_features is not None and grad_feature_map is not None:
+                    grad_map = _f32(grad_feature_map)
+                    ext = _lib.GsbExtraFeatureArgs(channels=extra_features.shape[1], features=_ptr(extra_features),
+                                                   grad_rasterized=_ptr(grad_map), grad_features=_ptr(grad_extra_features))
+                _lib.check(lib.gsb200_backward_pose(ctypes.byref(args), _ptr(grad_depth), _ptr(depth), _ptr(grad_alpha),
+                                                    ctypes.byref(ext) if ext is not None else None,
+                                                    ctypes.byref(pose_args)), "gsb200_backward_pose")
+            elif extra_features is not None and grad_feature_map is not None:
                 grad_map = _f32(grad_feature_map)
                 ext = _lib.GsbExtraFeatureArgs(channels=extra_features.shape[1], features=_ptr(extra_features),
                                                grad_rasterized=_ptr(grad_map), grad_features=_ptr(grad_extra_features))
@@ -599,7 +643,7 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                     point_uv_in_camera=frame.point_uv.contiguous(),
                     point_depth=frame.point_in_camera[:, 2],
                 ))
-        return grad_pointcloud, grad_pointcloud_features, grad_extra_features
+        return grad_pointcloud, grad_pointcloud_features, grad_extra_features, grad_q, grad_t
 
     def backward_flags(self, frame_flags: int) -> int:
         """Flags of the backward call for a frame rendered with ``frame_flags`` (adds the experimental kernel selection)."""

@@ -105,6 +105,14 @@ class GsbFeatureTrainArgs(ctypes.Structure):
     ]
 
 
+class GsbPoseGradArgs(ctypes.Structure):
+    _fields_ = [
+        ("q_pointcloud_camera", c_vp), ("grad_q_pointcloud_camera", c_vp), ("grad_t_pointcloud_camera", c_vp), ("temp", c_vp),
+    ]
+
+
+GSB_POSE_MAX_OBJECTS = 64
+
 GSB_FEATURE_LOSS_CROSS_ENTROPY = 1
 GSB_FEATURE_LOSS_L2 = 2
 
@@ -127,7 +135,8 @@ EXPORTS = (
     "gsb200_forward_blend_work", "gsb200_backward_blend_work", "gsb200_device_selftest", "gsb200_expand_view_gradients",
     "gsb200_train_step", "gsb200_abi_sizes_ext", "gsb200_exchange_multimem", "gsb200_backward_with_depth",
     "gsb200_backward_aux", "gsb200_supervision_temp_bytes", "gsb200_train_step_aux", "gsb200_forward_ext",
-    "gsb200_backward_ext", "gsb200_feature_loss_temp_bytes", "gsb200_train_step_ext",
+    "gsb200_backward_ext", "gsb200_feature_loss_temp_bytes", "gsb200_train_step_ext", "gsb200_backward_pose",
+    "gsb200_pose_grad_temp_bytes",
 )
 
 _lib = None
@@ -161,6 +170,11 @@ def load() -> ctypes.CDLL:
     lib.gsb200_forward_ext.restype = ctypes.c_int
     lib.gsb200_backward_ext.argtypes = [ctypes.POINTER(GsbBackwardArgs), c_vp, c_vp, c_vp, ctypes.POINTER(GsbExtraFeatureArgs)]
     lib.gsb200_backward_ext.restype = ctypes.c_int
+    lib.gsb200_backward_pose.argtypes = [ctypes.POINTER(GsbBackwardArgs), c_vp, c_vp, c_vp, ctypes.POINTER(GsbExtraFeatureArgs),
+                                         ctypes.POINTER(GsbPoseGradArgs)]
+    lib.gsb200_backward_pose.restype = ctypes.c_int
+    lib.gsb200_pose_grad_temp_bytes.argtypes = [c_i32]
+    lib.gsb200_pose_grad_temp_bytes.restype = c_i64
     lib.gsb200_sort_temp_bytes.argtypes = [c_i64, c_i32]
     lib.gsb200_sort_temp_bytes.restype = c_i64
     lib.gsb200_sort_pairs.argtypes = [c_vp, c_vp, c_vp, c_vp, c_i64, c_i32, c_i32, c_vp, c_i64, c_vp]
@@ -241,6 +255,11 @@ def load() -> ctypes.CDLL:
     if sizes8[7] != ctypes.sizeof(GsbFeatureTrainArgs):
         raise RuntimeError(f"libgsb200.so ABI mismatch: sizeof(GsbFeatureTrainArgs) {sizes8[7]} != ctypes mirror "
                            f"{ctypes.sizeof(GsbFeatureTrainArgs)}")
+    sizes9 = (c_i64 * 9)()
+    lib.gsb200_abi_sizes_ext(sizes9, 9)
+    if sizes9[8] != ctypes.sizeof(GsbPoseGradArgs):
+        raise RuntimeError(f"libgsb200.so ABI mismatch: sizeof(GsbPoseGradArgs) {sizes9[8]} != ctypes mirror "
+                           f"{ctypes.sizeof(GsbPoseGradArgs)}")
     _lib = lib
     return lib
 

@@ -388,9 +388,14 @@ constexpr int PT_ROW_COMPACT = 20;  // COMPACT: 16 staged floats per row, same b
 // DEPTH = true (gsb200_backward_with_depth): word 11 of the accumulator row is dL/dz of the point's camera-space depth
 // (blend_bwd_transposed.cu), and z = W[2,:] xyz + t adds it to dL/dxyz along the third row of W -- before gx feeds the
 // dense gradient, the controller epilogue or the compact row.
-template <bool COMPACT, bool DEPTH = false>
-__global__ void __launch_bounds__(GSB_POINTS_THREADS, 6)  // 6 x 33 KB of staging per SM
-backward_points_kernel(const PointsBwdParams p) {
+// POSE = true (gsb200_backward_pose): each in-camera point also forms its 12 pose values -- dL/dW (9, row-major) and
+// dL/dtw (3) of its object's T = [W | tw] -- which the warp sums per object (fixed butterfly order) into the per-warp rows
+// s_pose[warp][object][12]; after the loop the CTA adds its warps' rows in warp order into its partial row block
+// pose_partials[blockIdx.x][object][12].  pose_finish_kernel adds the blocks in block order: no float atomics anywhere.
+constexpr int POSE_VALUES = 12;
+template <bool COMPACT, bool DEPTH, bool POSE>
+__device__ __forceinline__ void backward_points_body(const PointsBwdParams p, float *s_pose, float *pose_partials,
+                                                     int num_objects) {
     // One thread per scene row: rows outside the frustum get their zeros here (no separate memset of the
     // dense (N,3)/(N,56) gradients), rows inside get the chain rule.  A warp owns 32 consecutive rows, i.e. one
     // contiguous 7 KB piece of the (N,56) gradient and 384 B of the (N,3) one: each lane stages its row in
@@ -402,10 +407,17 @@ backward_points_kernel(const PointsBwdParams p) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     float *const my_feat = &s_feat[warp][lane * ROW];
     float *const my_xyz = &s_xyz[warp][lane * 3];
+    float *const my_pose = POSE ? s_pose + warp * (num_objects * POSE_VALUES) : nullptr;
+    if (POSE) {
+        for (int k = lane; k < num_objects * POSE_VALUES; k += 32) my_pose[k] = 0.0f;
+        __syncwarp();
+    }
     const long long stride = (long long)gridDim.x * blockDim.x;
     for (long long base = (long long)blockIdx.x * blockDim.x + warp * 32; base < p.N; base += stride) {
       const long long id = base + lane;
       const int o = id < p.N ? p.point_offset[id] : -1;
+      float pv[POSE ? POSE_VALUES : 1];
+      int pose_obj = -1;
       if (o < 0) {
           if (!COMPACT) { my_xyz[0] = 0.0f; my_xyz[1] = 0.0f; my_xyz[2] = 0.0f; }
 #pragma unroll
@@ -496,6 +508,37 @@ backward_points_kernel(const PointsBwdParams p) {
         // sigmoid'(.) from the stored colour: c (1 - c)  (UT:356-359)
         const float gcol[3] = {a1.y * (r2.x * (1.0f - r2.x)), a1.z * (r2.y * (1.0f - r2.y)),
                                a1.w * (r2.z * (1.0f - r2.z))};
+        if (POSE) {
+            // pc = W xyz + tw.  gp = dL/dpc through uv (and z with DEPTH): dL/dW += gp xyz^T, dL/dtw += gp.
+            // Sigma' = U Sigma U^T with U = J W (J detached): dL/dU = 2 G U Sigma, dL/dW += J^T (2 G U Sigma)
+            float gp[3];
+#pragma unroll
+            for (int r = 0; r < 3; ++r) gp[r] = dj[r] * a0.x + dj[3 + r] * a0.y;
+            if (DEPTH) gp[2] += a2.w;
+            float UM[6];  // U M, M = R diag(es)
+#pragma unroll
+            for (int a = 0; a < 2; ++a)
+#pragma unroll
+                for (int j = 0; j < 3; ++j)
+                    UM[a * 3 + j] = (U[a * 3] * R[j] + U[a * 3 + 1] * R[3 + j] + U[a * 3 + 2] * R[6 + j]) * es[j];
+            float B0[3], B1[3];  // G U Sigma = G (U M) M^T
+#pragma unroll
+            for (int c = 0; c < 3; ++c) {
+                const float A0 = UM[0] * (R[c * 3] * es[0]) + UM[1] * (R[c * 3 + 1] * es[1]) + UM[2] * (R[c * 3 + 2] * es[2]);
+                const float A1 = UM[3] * (R[c * 3] * es[0]) + UM[4] * (R[c * 3 + 1] * es[1]) + UM[5] * (R[c * 3 + 2] * es[2]);
+                B0[c] = g00 * A0 + g01 * A1;
+                B1[c] = g01 * A0 + g11 * A1;
+            }
+            const float xw[3] = {x, y, z};
+#pragma unroll
+            for (int c = 0; c < 3; ++c) {  // J = [J0 0 J2; 0 J4 J5]
+                pv[c] = gp[0] * xw[c] + 2.0f * (J[0] * B0[c]);
+                pv[3 + c] = gp[1] * xw[c] + 2.0f * (J[4] * B1[c]);
+                pv[6 + c] = gp[2] * xw[c] + 2.0f * (J[2] * B0[c] + J[5] * B1[c]);
+                pv[9 + c] = gp[c];
+            }
+            pose_obj = ob;
+        }
         if (p.ctl_num_in_camera != nullptr && !(p.skip_flag != nullptr && *p.skip_flag != 0)) {
             // GaussianPointAdaptiveController.update (:130-143) for this in-camera point: ids are unique, one thread per row,
             // so plain read-modify-writes.  a2.y = sum |d/duv| over pixels, a2.z = number of affected pixels (exact in f32)
@@ -540,6 +583,22 @@ backward_points_kernel(const PointsBwdParams p) {
         }
         }
       }
+      if (POSE) {
+          // one pass per object present in the warp (points of several objects may share a warp), lowest lane's first
+          unsigned int todo = __ballot_sync(0xffffffffu, pose_obj >= 0);
+          while (todo) {
+              const int cur = __shfl_sync(0xffffffffu, pose_obj, __ffs(todo) - 1);
+              const bool mine = pose_obj == cur;
+              todo &= ~__ballot_sync(0xffffffffu, mine);
+#pragma unroll
+              for (int k = 0; k < POSE_VALUES; ++k) {
+                  float v = mine ? pv[k] : 0.0f;
+#pragma unroll
+                  for (int d = 16; d > 0; d >>= 1) v += __shfl_xor_sync(0xffffffffu, v, d);
+                  if (lane == 0) my_pose[cur * POSE_VALUES + k] += v;
+              }
+          }
+      }
       __syncwarp();
       const long long rows = p.N - base < 32 ? p.N - base : 32;
       if (COMPACT) {
@@ -573,6 +632,100 @@ backward_points_kernel(const PointsBwdParams p) {
       }
       __syncwarp();
     }
+    if (POSE) {
+        __syncthreads();
+        float *const out = pose_partials + (size_t)blockIdx.x * num_objects * POSE_VALUES;
+        for (int k = threadIdx.x; k < num_objects * POSE_VALUES; k += blockDim.x) {
+            float s = s_pose[k];
+            for (int w = 1; w < GSB_POINTS_THREADS / 32; ++w) s += s_pose[w * num_objects * POSE_VALUES + k];
+            out[k] = s;
+        }
+    }
+}
+
+template <bool COMPACT, bool DEPTH = false>
+__global__ void __launch_bounds__(GSB_POINTS_THREADS, 6)  // 6 x 33 KB of staging per SM
+backward_points_kernel(const PointsBwdParams p) {
+    backward_points_body<COMPACT, DEPTH, false>(p, nullptr, nullptr, 0);
+}
+
+// The parameter block of the POSE instantiations: the default kernels keep PointsBwdParams as it is.
+struct PointsBwdPoseParams : PointsBwdParams {
+    float *pose_partials;  // (grid, num_objects, 12)
+    int num_objects;       // <= GSB_POSE_MAX_OBJECTS
+};
+
+template <bool DEPTH>
+__global__ void __launch_bounds__(GSB_POINTS_THREADS, 5)  // + 12 KB of per-warp pose rows
+backward_points_pose_kernel(const PointsBwdPoseParams p) {
+    __shared__ float s_pose[(GSB_POINTS_THREADS / 32) * GSB_POSE_MAX_OBJECTS * POSE_VALUES];
+    backward_points_body<false, DEPTH, true>(p, s_pose, p.pose_partials, p.num_objects);
+}
+
+// R(q) of GP3D:30-48 (xyzw, not normalised) and the gradient of sum_ij G_ij R(q)_ij with respect to q
+__device__ __forceinline__ void pose_rot(const float *q, float *R) {
+    const float x = q[0], y = q[1], z = q[2], w = q[3];
+    R[0] = 1 - 2 * (y * y + z * z); R[1] = 2 * (x * y - w * z);     R[2] = 2 * (x * z + w * y);
+    R[3] = 2 * (x * y + w * z);     R[4] = 1 - 2 * (x * x + z * z); R[5] = 2 * (y * z - w * x);
+    R[6] = 2 * (x * z - w * y);     R[7] = 2 * (y * z + w * x);     R[8] = 1 - 2 * (x * x + y * y);
+}
+__device__ __forceinline__ void pose_rot_grad(const float *q, const float *G, float *g) {
+    const float x = q[0], y = q[1], z = q[2], w = q[3];
+    g[0] = 2 * y * (G[1] + G[3]) + 2 * z * (G[2] + G[6]) - 4 * x * (G[4] + G[8]) + 2 * w * (G[7] - G[5]);
+    g[1] = 2 * x * (G[1] + G[3]) - 4 * y * (G[0] + G[8]) + 2 * z * (G[5] + G[7]) + 2 * w * (G[2] - G[6]);
+    g[2] = 2 * x * (G[2] + G[6]) + 2 * y * (G[5] + G[7]) - 4 * z * (G[0] + G[4]) + 2 * w * (G[3] - G[1]);
+    g[3] = 2 * x * (G[7] - G[5]) + 2 * y * (G[2] - G[6]) + 2 * z * (G[3] - G[1]);
+}
+
+// One CTA per object: adds the `blocks` partial rows of the object in a fixed order (strided per thread, then a fixed
+// shared-memory tree) and takes dL/dW, dL/dtw through pose_kernel's map (preprocess.cu) to dL/dq_pc, dL/dt_pc:
+// qi = conj(q_pc), W = R(qi), tw = -R(qn) t_pc with qn = qi / |qi|.  Writes every row, zeros when blocks == 0.
+constexpr int POSE_FINISH_THREADS = 128;
+__global__ void __launch_bounds__(POSE_FINISH_THREADS)
+pose_finish_kernel(const float *__restrict__ partials, int blocks, int num_objects, const float *__restrict__ q_pc,
+                   const float *__restrict__ t_pc, float *__restrict__ grad_q, float *__restrict__ grad_t) {
+    __shared__ float s_sum[POSE_FINISH_THREADS][POSE_VALUES + 1];
+    const int ob = blockIdx.x, tid = threadIdx.x;
+    float acc[POSE_VALUES];
+#pragma unroll
+    for (int k = 0; k < POSE_VALUES; ++k) acc[k] = 0.0f;
+    for (int b = tid; b < blocks; b += POSE_FINISH_THREADS) {
+        const float *row = partials + ((size_t)b * num_objects + ob) * POSE_VALUES;
+#pragma unroll
+        for (int k = 0; k < POSE_VALUES; ++k) acc[k] += row[k];
+    }
+#pragma unroll
+    for (int k = 0; k < POSE_VALUES; ++k) s_sum[tid][k] = acc[k];
+    __syncthreads();
+    for (int h = POSE_FINISH_THREADS / 2; h > 0; h >>= 1) {
+        if (tid < h)
+#pragma unroll
+            for (int k = 0; k < POSE_VALUES; ++k) s_sum[tid][k] += s_sum[tid + h][k];
+        __syncthreads();
+    }
+    if (tid != 0) return;
+    const float *gW = s_sum[0], *gtw = s_sum[0] + 9;
+    const float qi[4] = {-q_pc[4 * ob], -q_pc[4 * ob + 1], -q_pc[4 * ob + 2], q_pc[4 * ob + 3]};
+    const float t[3] = {t_pc[3 * ob], t_pc[3 * ob + 1], t_pc[3 * ob + 2]};
+    const float n = sqrtf(((qi[0] * qi[0] + qi[1] * qi[1]) + qi[2] * qi[2]) + qi[3] * qi[3]);
+    const float qn[4] = {qi[0] / n, qi[1] / n, qi[2] / n, qi[3] / n};
+    float g[4], gn[4], Rn[9], GRn[9];
+    pose_rot_grad(qi, gW, g);  // W = R(qi)
+    pose_rot(qn, Rn);          // tw = -R(qn) t
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        grad_t[3 * ob + c] = -(Rn[c] * gtw[0] + Rn[3 + c] * gtw[1] + Rn[6 + c] * gtw[2]);
+#pragma unroll
+        for (int r = 0; r < 3; ++r) GRn[r * 3 + c] = -gtw[r] * t[c];
+    }
+    pose_rot_grad(qn, GRn, gn);
+    const float dot = qn[0] * gn[0] + qn[1] * gn[1] + qn[2] * gn[2] + qn[3] * gn[3];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) g[k] += (gn[k] - qn[k] * dot) / n;  // d qn / d qi = (I - qn qn^T) / |qi|
+    grad_q[4 * ob] = -g[0];  // q_pc = conj(qi)
+    grad_q[4 * ob + 1] = -g[1];
+    grad_q[4 * ob + 2] = -g[2];
+    grad_q[4 * ob + 3] = g[3];
 }
 
 // ------------------------------------------------------------------ view-parallel exchange: rebuild the dense gradients
@@ -673,9 +826,7 @@ expand_view_gradients_kernel(const ExpandParams p) {
 #ifndef GSB_HOST_EMU
 static int first_cleared_of_band(int band) { return band <= 0 ? 1 : band == 1 ? 4 : band == 2 ? 9 : 16; }
 
-int launch_backward_points(const GsbBackwardArgs &a, const Workspace &ws, cudaStream_t stream, const long long *skip_flag,
-                           bool depth_grad) {
-    if (a.num_points <= 0) return GSB_OK;
+static PointsBwdParams make_points_params(const GsbBackwardArgs &a, const Workspace &ws, const long long *skip_flag) {
     PointsBwdParams p;
     p.ctl_num_in_camera = a.ctl_accumulated_num_in_camera;
     p.ctl_num_pixels = a.ctl_accumulated_num_pixels;
@@ -705,6 +856,13 @@ int launch_backward_points(const GsbBackwardArgs &a, const Workspace &ws, cudaSt
     p.grad_feat = a.grad_pointcloud_features;
     p.grad_sum_compact = a.grad_sum_compact;
     p.grad_color_compact = a.grad_color_compact;
+    return p;
+}
+
+int launch_backward_points(const GsbBackwardArgs &a, const Workspace &ws, cudaStream_t stream, const long long *skip_flag,
+                           bool depth_grad) {
+    if (a.num_points <= 0) return GSB_OK;
+    const PointsBwdParams p = make_points_params(a, ws, skip_flag);
     long long blocks = (a.num_points + GSB_POINTS_THREADS - 1) / GSB_POINTS_THREADS;
     const long long cap = 16LL * num_sms();
     if (blocks > cap) blocks = cap;
@@ -718,6 +876,28 @@ int launch_backward_points(const GsbBackwardArgs &a, const Workspace &ws, cudaSt
     } else {
         backward_points_kernel<false><<<(int)blocks, GSB_POINTS_THREADS, 0, stream>>>(p);
     }
+    GSB_CUDA_CHECK(cudaGetLastError());
+    return GSB_OK;
+}
+
+// The POSE per-point kernel on a grid that depends on N alone (at most GSB_POSE_PARTIAL_BLOCKS CTAs), so the summation
+// order of the pose gradient is the same on every device, then pose_finish_kernel.  The caller checked `pose`.
+int launch_backward_points_pose(const GsbBackwardArgs &a, const Workspace &ws, cudaStream_t stream, bool depth_grad,
+                                const GsbPoseGradArgs &pose) {
+    PointsBwdPoseParams p;
+    static_cast<PointsBwdParams &>(p) = make_points_params(a, ws, nullptr);
+    p.pose_partials = static_cast<float *>(pose.temp);
+    p.num_objects = a.num_objects;
+    long long blocks = a.num_points > 0 ? (a.num_points + GSB_POINTS_THREADS - 1) / GSB_POINTS_THREADS : 0;
+    if (blocks > GSB_POSE_PARTIAL_BLOCKS) blocks = GSB_POSE_PARTIAL_BLOCKS;
+    if (blocks > 0) {
+        if (depth_grad) backward_points_pose_kernel<true><<<(int)blocks, GSB_POINTS_THREADS, 0, stream>>>(p);
+        else backward_points_pose_kernel<false><<<(int)blocks, GSB_POINTS_THREADS, 0, stream>>>(p);
+        GSB_CUDA_CHECK(cudaGetLastError());
+    }
+    pose_finish_kernel<<<a.num_objects, POSE_FINISH_THREADS, 0, stream>>>(
+        p.pose_partials, (int)blocks, a.num_objects, pose.q_pointcloud_camera, a.t_pointcloud_camera,
+        pose.grad_q_pointcloud_camera, pose.grad_t_pointcloud_camera);
     GSB_CUDA_CHECK(cudaGetLastError());
     return GSB_OK;
 }

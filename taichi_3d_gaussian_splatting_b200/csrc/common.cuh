@@ -79,6 +79,10 @@ int launch_blend_backward(const GsbBackwardArgs &a, const Workspace &ws, cudaStr
                           const float *grad_alpha = nullptr, const GsbExtraFeatureArgs *ext = nullptr);
 int launch_backward_points(const GsbBackwardArgs &a, const Workspace &ws, cudaStream_t stream,
                            const long long *skip_flag = nullptr, bool depth_grad = false);
+// gsb200_backward_pose: the POSE per-point kernel (dense gradients as launch_backward_points, plus the per-CTA pose sums
+// in pose.temp) and the per-object finishing kernel; arguments checked by the caller
+int launch_backward_points_pose(const GsbBackwardArgs &a, const Workspace &ws, cudaStream_t stream, bool depth_grad,
+                                const GsbPoseGradArgs &pose);
 int launch_adam_step(float *param, const float *grad, float *exp_avg, float *exp_avg_sq, long long n, double lr, double beta1,
                      double beta2, double eps, int step, const long long *skip_flag, cudaStream_t stream);
 int launch_expand_view_gradients(const GsbExpandArgs &a, cudaStream_t stream);

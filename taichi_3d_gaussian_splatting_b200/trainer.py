@@ -15,6 +15,8 @@ Optional feature training (an extension; ``Scene.point_extra_features``, ``Train
 ``SupervisionTargets.labels`` / ``features``): per-Gaussian feature vectors rendered alongside the image, a cross-entropy or
 l2 loss on the rendered feature map (``loss.feature_loss``) and a third Adam on the features, kept in step with the scene
 through densification.
+Optional pose refinement (an extension; ``TrainConfig.pose_learning_rate``): the (q, t) of every training view but the
+first become trainable, differentiated by the operator's ``differentiable_pose`` and stepped by their own Adam.
 The rasteriser is injected (default: the CUDA operator) so that tests can run the identical loop with the
 CPU oracle behind the same interface and compare PSNR trajectories.
 """
@@ -124,6 +126,10 @@ class GaussianPointCloudTrainer:
         feature_loss: str = "none"
         feature_loss_weight: float = 0.
         extra_feature_learning_rate: float = 1e-2
+        # optional pose refinement: > 0 makes the (q, t) of training views 1..n leaf tensors (initialised from the views)
+        # trained by their own Adam at this rate, q renormalised after each step.  View 0's pose stays fixed and is the
+        # reference frame; the global scale of scene and translations is not pinned.  Not with fused_step.
+        pose_learning_rate: float = 0.
 
     def __init__(self, config: "GaussianPointCloudTrainer.TrainConfig", scene: Scene, train_views: List[View],
                  rasterisation_factory: Optional[Callable] = None, generator: Optional[torch.Generator] = None,
@@ -154,6 +160,15 @@ class GaussianPointCloudTrainer:
             raise ValueError("mask_loss_weight > 0 needs a mask on every view")
         if config.background == "random" and any(tg.mask is None for tg in targets):
             raise ValueError('background="random" needs a mask on every view (the ground truth is composited by it)')
+        if not (config.pose_learning_rate >= 0.0 and config.pose_learning_rate < float("inf")):
+            raise ValueError(f"pose_learning_rate must be finite and >= 0, got {config.pose_learning_rate}")
+        self._pose = config.pose_learning_rate > 0
+        if self._pose and fused_step:
+            raise ValueError("fused_step does not implement pose refinement (pose_learning_rate > 0)")
+        # the trainable poses: view 0 keeps its own tensors (the gauge), every other view gets leaf copies
+        self._poses = [(v[1], v[2]) if i == 0 or not self._pose else
+                       (v[1].detach().clone().requires_grad_(True), v[2].detach().clone().requires_grad_(True))
+                       for i, v in enumerate(train_views)]
         self._features = config.feature_loss != "none"
         if self._features:
             self._check_feature_config(config, scene, targets)
@@ -184,7 +199,8 @@ class GaussianPointCloudTrainer:
         factory = rasterisation_factory or GaussianPointCloudRasterisation
         # the differentiable outputs only when a term needs them: injected factories without them keep working
         extra = dict(**({"differentiable_depth": True} if self._need_depth else {}),
-                     **({"differentiable_alpha": True} if self._need_alpha else {}))
+                     **({"differentiable_alpha": True} if self._need_alpha else {}),
+                     **({"differentiable_pose": True} if self._pose else {}))
         self.rasterisation = factory(config=config.rasterisation_config,
                                      backward_valid_point_hook=self.adaptive_controller.update, **extra)
         self.loss_function = LossFunction(config=config.loss_function_config)
@@ -231,7 +247,8 @@ class GaussianPointCloudTrainer:
     def _view(self, view_index: int, downsample_factor: int):
         """(image, q, t, camera, targets) of a view at the schedule's resolution; resized once per (view, factor)."""
         view = self.train_views[view_index]
-        image_gt, q, t, camera_info = view[:4]
+        image_gt, _, _, camera_info = view[:4]
+        q, t = self._poses[view_index]
         targets = view[4] if len(view) > 4 and view[4] is not None else SupervisionTargets()
         if downsample_factor > 1:
             # the reference resizes the full-resolution frame in every iteration (GaussianPointTrainer.py:146-148); the
@@ -325,6 +342,8 @@ class GaussianPointCloudTrainer:
         position_optimizer = Adam([self.scene.point_cloud], lr=cfg.position_learning_rate, betas=(0.9, 0.999))
         extra_optimizer = Adam([self.scene.point_extra_features], lr=cfg.extra_feature_learning_rate,
                                betas=(0.9, 0.999)) if self._features else None
+        pose_optimizer = Adam([x for q, t in self._poses[1:] for x in (q, t)], lr=cfg.pose_learning_rate,
+                              betas=(0.9, 0.999)) if self._pose and len(self._poses) > 1 else None
         scheduler = torch.optim.lr_scheduler.ExponentialLR(position_optimizer, gamma=cfg.position_learning_rate_decay_rate)
         downsample_factor = cfg.initial_downsample_factor
         for iteration in range(cfg.num_iterations):
@@ -334,6 +353,8 @@ class GaussianPointCloudTrainer:
             position_optimizer.zero_grad()
             if extra_optimizer is not None:
                 extra_optimizer.zero_grad()
+            if pose_optimizer is not None:
+                pose_optimizer.zero_grad()
             view_index = self._next_view_index(iteration)
             image_gt, q, t, camera_info, targets = self._view(view_index, downsample_factor)
             band = iteration // cfg.increase_color_max_sh_band_interval
@@ -357,6 +378,11 @@ class GaussianPointCloudTrainer:
             position_optimizer.step()
             if extra_optimizer is not None:
                 extra_optimizer.step()
+            if pose_optimizer is not None:
+                pose_optimizer.step()
+                with torch.no_grad():
+                    for q_v, _ in self._poses[1:]:
+                        q_v.div_(q_v.norm(dim=-1, keepdim=True))
             if iteration % cfg.position_learning_rate_decay_interval == 0:
                 scheduler.step()
             self.adaptive_controller.refinement()
@@ -397,6 +423,10 @@ class GaussianPointCloudTrainer:
             feature_term = feature_loss(outs[-1], targets, cfg.feature_loss, cfg.feature_loss_weight)
             total = total + feature_term
         return total, l1, mask_term, depth_term, feature_term, image_pred.detach().clamp(0, 1).permute(2, 0, 1)
+
+    def refined_poses(self) -> List[Tuple[torch.Tensor, torch.Tensor]]:
+        """(q, t) of every training view as trained (detached copies; the views' own poses without pose refinement)."""
+        return [(q.detach().clone(), t.detach().clone()) for q, t in self._poses]
 
     @torch.no_grad()
     def validation(self, views: Optional[List[View]] = None) -> float:
