@@ -205,7 +205,7 @@ const char *gsb200_last_error(void);
  * foreign-language binding verify its struct mirrors. */
 void gsb200_abi_sizes(int64_t *out3);
 /* ... and of the first n of {GsbWorkspaceLayout, GsbForwardArgs, GsbBackwardArgs, GsbExpandArgs, GsbTrainStepArgs,
- * GsbSupervisionArgs, GsbExtraFeatureArgs, GsbFeatureTrainArgs, GsbPoseGradArgs} */
+ * GsbSupervisionArgs, GsbExtraFeatureArgs, GsbFeatureTrainArgs, GsbPoseGradArgs, GsbIntrinsicsGradArgs} */
 void gsb200_abi_sizes_ext(int64_t *out, int32_t n);
 
 /* Workspace sizing.  far_plane*depth_to_sort_key_scale fixes the depth-key width; (H/16)*(W/16)
@@ -319,6 +319,38 @@ int64_t gsb200_pose_grad_temp_bytes(int32_t num_objects);
 int gsb200_backward_pose(const GsbBackwardArgs *args, const float *grad_rasterized_depth, const float *rasterized_depth,
                          const float *grad_pixel_accumulated_alpha, const GsbExtraFeatureArgs *ext,
                          const GsbPoseGradArgs *pose); /* or NULL */
+
+/* Camera-intrinsics gradients (an extension: the reference differentiates the scene only).  The forward (preprocess.cu)
+ * reads K in two places: uv = (K pc)[:2] / z, which uses all six entries of rows 0 and 1, and J = [fx/z 0 -fx x/z^2;
+ * 0 fy/z -fy y/z^2] (fx = K[0][0], fy = K[1][1]; skew does not enter J) inside Sigma' = (J W) Sigma (J W)^T.  Row 2 is never
+ * read.  The intrinsics gradient is the exact derivative through both, under the conventions of the point and pose
+ * gradients: the dependence of J on pc is detached, so are the rescale factor, the radius and tile membership and the SH
+ * view direction; the 0.99 clamp is straight-through.  Per in-camera point, with guv = dL/duv of its accumulator row and
+ * B0, B1 the rows of G (J W) Sigma (the pose gradient's):
+ *   dL/dK[r][c] += guv_r pc_c / z                                 r in {0,1}, c in {0,1,2}
+ *   dL/dK[0][0] += 2 sum_c B0[c] (W[0][c]/z - x W[2][c]/z^2),   dL/dK[1][1] += 2 sum_c B1[c] (W[1][c]/z - y W[2][c]/z^2)
+ * summed over every in-camera point of every object (a frame has one K); dL/dK[2][.] = 0.  No gradient factor is applied;
+ * every loss term that reaches the accumulator rows (image, depth, alpha, features) contributes, and the depth term's direct
+ * dL/dz adds nothing (z does not depend on K).  The sum is deterministic: the per-point kernel runs on
+ * min(ceil(N/128), GSB_INTRINSICS_PARTIAL_BLOCKS) CTAs, each writes its sums to `temp`, and a second kernel adds them in
+ * block order -- no float atomics. */
+#define GSB_INTRINSICS_PARTIAL_BLOCKS 2048 /* = GSB_POSE_PARTIAL_BLOCKS: with both, one per-point pass */
+typedef struct GsbIntrinsicsGradArgs {
+    float *grad_camera_intrinsics; /* (3,3) out, fully written (row 2 zero) */
+    void *temp;                    /* gsb200_intrinsics_grad_temp_bytes() bytes, 16-byte aligned */
+} GsbIntrinsicsGradArgs;
+/* GSB_INTRINSICS_PARTIAL_BLOCKS * 6 floats */
+int64_t gsb200_intrinsics_grad_temp_bytes(void);
+/* gsb200_backward_pose that also writes the intrinsics gradient of `intrinsics`; with a pose as well, both come from one
+ * pass of the per-point kernel.  Everything else the call writes (dense gradients, hook tensors, controller accumulators,
+ * the pose gradients) is bit-identical to gsb200_backward_pose's.  NULL intrinsics: exactly gsb200_backward_pose, with the
+ * same kernels.  With intrinsics, before any CUDA call: GSB_EINVAL for a NULL output or temp pointer or a temp that is not
+ * 16-byte aligned; GSB_EUNSUPPORTED for GSB_FLAG_COMPACT_GRADS.  An image-only loss works with either loop-A kernel; the
+ * other terms keep their requirement of GSB_FLAG_BACKWARD_TRANSPOSED. */
+int gsb200_backward_calib(const GsbBackwardArgs *args, const float *grad_rasterized_depth, const float *rasterized_depth,
+                          const float *grad_pixel_accumulated_alpha, const GsbExtraFeatureArgs *ext,
+                          const GsbPoseGradArgs *pose,               /* or NULL */
+                          const GsbIntrinsicsGradArgs *intrinsics);  /* or NULL */
 
 int gsb200_expand_view_gradients(const GsbExpandArgs *args);
 

@@ -238,6 +238,7 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
         differentiable_depth: bool = False,
         differentiable_alpha: bool = False,
         differentiable_pose: bool = False,
+        differentiable_intrinsics: bool = False,
     ):
         """``exact_exp``: blend kernels use ``expf`` instead of ``ex2.approx`` (parity debugging).
         ``force_key64``: sort the reference's 64-bit ``tile << 32 | depth`` keys even when the live
@@ -277,7 +278,17 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
         the SH view direction detached), and includes every loss term the backward takes (image, depth, alpha, features);
         no gradient factor is applied (``gsb200_backward_pose``).  With a frozen scene (only q / t require grad) the backward
         still runs.  At most 64 objects.  An image-only loss works with either backward kernel.  Off, a pose that requires
-        grad gets ``None``.  ``ValueError`` with ``config.rgb_only`` or a ``gradient_exchange``."""
+        grad gets ``None``.  ``ValueError`` with ``config.rgb_only`` or a ``gradient_exchange``.
+        ``differentiable_intrinsics``: ``camera_info.camera_intrinsics`` becomes an input of the autograd graph, and
+        ``backward`` returns its (3, 3) gradient when it requires grad (an extension: the reference differentiates the scene
+        only) -- to calibrate focal length and principal point, alone or together with the poses, also against a frozen
+        scene and also for a K built by torch ops from learnable parameters.  The gradient is exact through the projection
+        uv = (K pc)[:2] / z (all six entries of rows 0 and 1) and through fx, fy inside J, with the conventions of the point
+        and pose gradients (J's dependence on pc, the rescale factor, tile membership and the SH view direction detached);
+        row 2 gets 0, and no gradient factor is applied (``gsb200_backward_calib``).  It includes every loss term the
+        backward takes (image, depth, alpha, features).  With ``differentiable_pose`` both come from one pass of the
+        per-point kernel.  An image-only loss works with either backward kernel.  Off, K gets no gradient.  ``ValueError``
+        with ``config.rgb_only`` or a ``gradient_exchange``."""
         super().__init__()
         for name, on in (("differentiable_depth", differentiable_depth), ("differentiable_alpha", differentiable_alpha)):
             if on and backward_impl == "butterfly":
@@ -292,6 +303,11 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
         if differentiable_pose and gradient_exchange is not None:
             raise ValueError("differentiable_pose is not supported with a gradient_exchange (view-parallel training)")
         self.differentiable_pose = bool(differentiable_pose)
+        if differentiable_intrinsics and config.rgb_only:
+            raise ValueError("differentiable_intrinsics needs the auxiliary outputs: config.rgb_only=True renders none")
+        if differentiable_intrinsics and gradient_exchange is not None:
+            raise ValueError("differentiable_intrinsics is not supported with a gradient_exchange (view-parallel training)")
+        self.differentiable_intrinsics = bool(differentiable_intrinsics)
         self.config = config
         self.backward_valid_point_hook = backward_valid_point_hook
         self._flags = (_lib.GSB_FLAG_EXACT_EXP if exact_exp else 0) | (_lib.GSB_FLAG_FORCE_KEY64 if force_key64 else 0) | \
@@ -315,7 +331,10 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
 
             @staticmethod
             def forward(ctx, pointcloud, pointcloud_features, point_invalid_mask, point_object_id,
-                        q_pointcloud_camera, t_pointcloud_camera, camera_info, color_max_sh_band, extra_features=None):
+                        q_pointcloud_camera, t_pointcloud_camera, camera_info, color_max_sh_band, extra_features=None,
+                        camera_intrinsics=None):
+                # camera_intrinsics (differentiable_intrinsics): camera_info.camera_intrinsics itself, passed again only so
+                # that autograd tracks it
                 outs, frame, saved = outer._run_forward(
                     pointcloud, pointcloud_features, point_invalid_mask, point_object_id,
                     q_pointcloud_camera, t_pointcloud_camera, camera_info, extra_features)
@@ -329,6 +348,7 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                 ctx.num_objects = q_pointcloud_camera.shape[0]
                 ctx.color_max_sh_band = color_max_sh_band
                 ctx.has_extra_features = extra_features is not None
+                ctx.intrinsics_input = camera_intrinsics is not None
                 if outer.differentiable_depth:
                     ctx.mark_non_differentiable(valid_count)
                 else:
@@ -347,9 +367,12 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                 grad_feature_map = grad_extra[-1] if ctx.has_extra_features else None
                 grad_pointcloud = grad_pointcloud_features = grad_extra_features = grad_q = grad_t = None
                 pose = outer.differentiable_pose and (ctx.needs_input_grad[4] or ctx.needs_input_grad[5])
-                # GPCR:1028; with extra features (or pose gradients) the backward also runs for them alone (frozen scene)
+                intrinsics = ctx.intrinsics_input and ctx.needs_input_grad[9]
+                grad_K = None
+                # GPCR:1028; with extra features (or pose / intrinsics gradients) the backward also runs for them alone
+                # (frozen scene)
                 if ctx.needs_input_grad[0] or ctx.needs_input_grad[1] or (ctx.has_extra_features and ctx.needs_input_grad[8]) \
-                        or pose:
+                        or pose or intrinsics:
                     if outer.config.rgb_only:
                         # the reference leaves accumulated alpha / last-effective offsets uninitialised in
                         # this mode (GPCR:478-484), so its backward is undefined; refuse instead
@@ -359,8 +382,16 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                         frame = ctx.frame
                         grad_rasterized_image = torch.zeros((frame.height, frame.width, 3), dtype=torch.float32,
                                                             device=frame.ws.device)
-                    grad_pointcloud, grad_pointcloud_features, grad_extra_features, grad_q, grad_t = outer._run_backward(
-                        ctx, grad_rasterized_image, grad_rasterized_depth, grad_pixel_accumulated_alpha, grad_feature_map, pose)
+                    grad_pointcloud, grad_pointcloud_features, grad_extra_features, grad_q, grad_t, grad_K = \
+                        outer._run_backward(ctx, grad_rasterized_image, grad_rasterized_depth, grad_pixel_accumulated_alpha,
+                                            grad_feature_map, pose, intrinsics)
+                if ctx.intrinsics_input:  # ten inputs: the extra features' slot (possibly None), then K
+                    return (grad_pointcloud if ctx.needs_input_grad[0] else None,
+                            grad_pointcloud_features if ctx.needs_input_grad[1] else None, None, None,
+                            grad_q if pose and ctx.needs_input_grad[4] else None,
+                            grad_t if pose and ctx.needs_input_grad[5] else None, None, None,
+                            grad_extra_features if ctx.has_extra_features and ctx.needs_input_grad[8] else None,
+                            grad_K if intrinsics else None)
                 if pose:
                     grad_q = grad_q if ctx.needs_input_grad[4] else None
                     grad_t = grad_t if ctx.needs_input_grad[5] else None
@@ -505,9 +536,10 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
 
     # ------------------------------------------------------------------ backward plumbing
     def _run_backward(self, ctx, grad_rasterized_image, grad_rasterized_depth=None, grad_pixel_accumulated_alpha=None,
-                      grad_feature_map=None, pose=False):
+                      grad_feature_map=None, pose=False, intrinsics=False):
         """Returns dL/dxyz, dL/dfeatures, for a call with extra features dL/d of them ((N, C); zeros when the feature map
-        was not used), and with ``pose`` dL/dq_pointcloud_camera (K, 4) and dL/dt_pointcloud_camera (K, 3) (else None)."""
+        was not used), with ``pose`` dL/dq_pointcloud_camera (K, 4) and dL/dt_pointcloud_camera (K, 3) (else None), and
+        with ``intrinsics`` dL/dcamera_intrinsics (3, 3) (else None)."""
         cfg = self.config
         lib = _lib.load()
         saved = ctx.saved_tensors
@@ -573,24 +605,38 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                 C = extra_features.shape[1]
                 grad_extra_features = torch.zeros((N, C), dtype=torch.float32, device=device) if grad_feature_map is None \
                     else torch.empty((N, C), dtype=torch.float32, device=device)
-            grad_q = grad_t = None
-            if pose:
-                n_obj = ctx.num_objects
-                q_pc = q_pointcloud_camera.detach().contiguous()
-                grad_q = torch.empty((n_obj, 4), dtype=torch.float32, device=device)
-                grad_t = torch.empty((n_obj, 3), dtype=torch.float32, device=device)
-                pose_temp = torch.empty((max(int(lib.gsb200_pose_grad_temp_bytes(n_obj)), 16) // 4,), dtype=torch.float32,
-                                        device=device)
-                pose_args = _lib.GsbPoseGradArgs(q_pointcloud_camera=_ptr(q_pc), grad_q_pointcloud_camera=_ptr(grad_q),
-                                                 grad_t_pointcloud_camera=_ptr(grad_t), temp=_ptr(pose_temp))
+            grad_q = grad_t = grad_K = None
+            if pose or intrinsics:
+                pose_args = intr_args = None
+                if pose:
+                    n_obj = ctx.num_objects
+                    q_pc = q_pointcloud_camera.detach().contiguous()
+                    grad_q = torch.empty((n_obj, 4), dtype=torch.float32, device=device)
+                    grad_t = torch.empty((n_obj, 3), dtype=torch.float32, device=device)
+                    pose_temp = torch.empty((max(int(lib.gsb200_pose_grad_temp_bytes(n_obj)), 16) // 4,),
+                                            dtype=torch.float32, device=device)
+                    pose_args = _lib.GsbPoseGradArgs(q_pointcloud_camera=_ptr(q_pc), grad_q_pointcloud_camera=_ptr(grad_q),
+                                                     grad_t_pointcloud_camera=_ptr(grad_t), temp=_ptr(pose_temp))
+                if intrinsics:
+                    grad_K = torch.empty((3, 3), dtype=torch.float32, device=device)
+                    intr_temp = torch.empty((int(lib.gsb200_intrinsics_grad_temp_bytes()) // 4,), dtype=torch.float32,
+                                            device=device)
+                    intr_args = _lib.GsbIntrinsicsGradArgs(grad_camera_intrinsics=_ptr(grad_K), temp=_ptr(intr_temp))
                 ext = None
                 if extra_features is not None and grad_feature_map is not None:
                     grad_map = _f32(grad_feature_map)
                     ext = _lib.GsbExtraFeatureArgs(channels=extra_features.shape[1], features=_ptr(extra_features),
                                                    grad_rasterized=_ptr(grad_map), grad_features=_ptr(grad_extra_features))
-                _lib.check(lib.gsb200_backward_pose(ctypes.byref(args), _ptr(grad_depth), _ptr(depth), _ptr(grad_alpha),
-                                                    ctypes.byref(ext) if ext is not None else None,
-                                                    ctypes.byref(pose_args)), "gsb200_backward_pose")
+                if intrinsics:
+                    _lib.check(lib.gsb200_backward_calib(
+                        ctypes.byref(args), _ptr(grad_depth), _ptr(depth), _ptr(grad_alpha),
+                        ctypes.byref(ext) if ext is not None else None,
+                        ctypes.byref(pose_args) if pose_args is not None else None, ctypes.byref(intr_args)),
+                        "gsb200_backward_calib")
+                else:
+                    _lib.check(lib.gsb200_backward_pose(ctypes.byref(args), _ptr(grad_depth), _ptr(depth), _ptr(grad_alpha),
+                                                        ctypes.byref(ext) if ext is not None else None,
+                                                        ctypes.byref(pose_args)), "gsb200_backward_pose")
             elif extra_features is not None and grad_feature_map is not None:
                 grad_map = _f32(grad_feature_map)
                 ext = _lib.GsbExtraFeatureArgs(channels=extra_features.shape[1], features=_ptr(extra_features),
@@ -643,7 +689,7 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                     point_uv_in_camera=frame.point_uv.contiguous(),
                     point_depth=frame.point_in_camera[:, 2],
                 ))
-        return grad_pointcloud, grad_pointcloud_features, grad_extra_features, grad_q, grad_t
+        return grad_pointcloud, grad_pointcloud_features, grad_extra_features, grad_q, grad_t, grad_K
 
     def backward_flags(self, frame_flags: int) -> int:
         """Flags of the backward call for a frame rendered with ``frame_flags`` (adds the experimental kernel selection)."""
@@ -669,6 +715,13 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
         camera_info = input_data.camera_info
         assert camera_info.camera_width % TILE_WIDTH == 0
         assert camera_info.camera_height % TILE_HEIGHT == 0
+        if self.differentiable_intrinsics:  # K as a tenth input, after the extra features' slot
+            if point_extra_features is not None:
+                self._check_extra_features(point_extra_features, input_data.point_cloud)
+            return self._module_function.apply(
+                input_data.point_cloud, input_data.point_cloud_features, input_data.point_invalid_mask,
+                input_data.point_object_id, input_data.q_pointcloud_camera, input_data.t_pointcloud_camera, camera_info,
+                input_data.color_max_sh_band, point_extra_features, camera_info.camera_intrinsics)
         if point_extra_features is not None:
             self._check_extra_features(point_extra_features, input_data.point_cloud)
             return self._module_function.apply(

@@ -113,6 +113,11 @@ class GsbPoseGradArgs(ctypes.Structure):
 
 GSB_POSE_MAX_OBJECTS = 64
 
+
+class GsbIntrinsicsGradArgs(ctypes.Structure):
+    _fields_ = [("grad_camera_intrinsics", c_vp), ("temp", c_vp)]
+
+
 GSB_FEATURE_LOSS_CROSS_ENTROPY = 1
 GSB_FEATURE_LOSS_L2 = 2
 
@@ -136,7 +141,7 @@ EXPORTS = (
     "gsb200_train_step", "gsb200_abi_sizes_ext", "gsb200_exchange_multimem", "gsb200_backward_with_depth",
     "gsb200_backward_aux", "gsb200_supervision_temp_bytes", "gsb200_train_step_aux", "gsb200_forward_ext",
     "gsb200_backward_ext", "gsb200_feature_loss_temp_bytes", "gsb200_train_step_ext", "gsb200_backward_pose",
-    "gsb200_pose_grad_temp_bytes",
+    "gsb200_pose_grad_temp_bytes", "gsb200_backward_calib", "gsb200_intrinsics_grad_temp_bytes",
 )
 
 _lib = None
@@ -175,6 +180,11 @@ def load() -> ctypes.CDLL:
     lib.gsb200_backward_pose.restype = ctypes.c_int
     lib.gsb200_pose_grad_temp_bytes.argtypes = [c_i32]
     lib.gsb200_pose_grad_temp_bytes.restype = c_i64
+    lib.gsb200_backward_calib.argtypes = [ctypes.POINTER(GsbBackwardArgs), c_vp, c_vp, c_vp, ctypes.POINTER(GsbExtraFeatureArgs),
+                                          ctypes.POINTER(GsbPoseGradArgs), ctypes.POINTER(GsbIntrinsicsGradArgs)]
+    lib.gsb200_backward_calib.restype = ctypes.c_int
+    lib.gsb200_intrinsics_grad_temp_bytes.argtypes = []
+    lib.gsb200_intrinsics_grad_temp_bytes.restype = c_i64
     lib.gsb200_sort_temp_bytes.argtypes = [c_i64, c_i32]
     lib.gsb200_sort_temp_bytes.restype = c_i64
     lib.gsb200_sort_pairs.argtypes = [c_vp, c_vp, c_vp, c_vp, c_i64, c_i32, c_i32, c_vp, c_i64, c_vp]
@@ -260,6 +270,11 @@ def load() -> ctypes.CDLL:
     if sizes9[8] != ctypes.sizeof(GsbPoseGradArgs):
         raise RuntimeError(f"libgsb200.so ABI mismatch: sizeof(GsbPoseGradArgs) {sizes9[8]} != ctypes mirror "
                            f"{ctypes.sizeof(GsbPoseGradArgs)}")
+    sizes10 = (c_i64 * 10)()
+    lib.gsb200_abi_sizes_ext(sizes10, 10)
+    if sizes10[9] != ctypes.sizeof(GsbIntrinsicsGradArgs):
+        raise RuntimeError(f"libgsb200.so ABI mismatch: sizeof(GsbIntrinsicsGradArgs) {sizes10[9]} != ctypes mirror "
+                           f"{ctypes.sizeof(GsbIntrinsicsGradArgs)}")
     _lib = lib
     return lib
 

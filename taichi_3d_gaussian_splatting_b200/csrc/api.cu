@@ -192,11 +192,11 @@ void gsb200_abi_sizes(int64_t *out3) {
 }
 
 void gsb200_abi_sizes_ext(int64_t *out, int32_t n) {
-    const int64_t all[9] = {(int64_t)sizeof(GsbWorkspaceLayout), (int64_t)sizeof(GsbForwardArgs), (int64_t)sizeof(GsbBackwardArgs),
-                            (int64_t)sizeof(GsbExpandArgs), (int64_t)sizeof(GsbTrainStepArgs), (int64_t)sizeof(GsbSupervisionArgs),
-                            (int64_t)sizeof(GsbExtraFeatureArgs), (int64_t)sizeof(GsbFeatureTrainArgs),
-                            (int64_t)sizeof(GsbPoseGradArgs)};
-    for (int i = 0; i < n && i < 9; ++i) out[i] = all[i];
+    const int64_t all[10] = {(int64_t)sizeof(GsbWorkspaceLayout), (int64_t)sizeof(GsbForwardArgs), (int64_t)sizeof(GsbBackwardArgs),
+                             (int64_t)sizeof(GsbExpandArgs), (int64_t)sizeof(GsbTrainStepArgs), (int64_t)sizeof(GsbSupervisionArgs),
+                             (int64_t)sizeof(GsbExtraFeatureArgs), (int64_t)sizeof(GsbFeatureTrainArgs),
+                             (int64_t)sizeof(GsbPoseGradArgs), (int64_t)sizeof(GsbIntrinsicsGradArgs)};
+    for (int i = 0; i < n && i < 10; ++i) out[i] = all[i];
 }
 
 int gsb200_workspace_layout(int64_t num_points, int32_t num_objects, int64_t key_capacity,
@@ -271,7 +271,8 @@ int gsb200_forward_ext(const GsbForwardArgs *a, const GsbExtraFeatureArgs *ext) 
 // term) or set.  The auxiliary terms are checked in gsb200_backward_ext.
 static int backward_impl(const GsbBackwardArgs *a, bool skip_on_overflow, const float *grad_depth = nullptr,
                          const float *depth = nullptr, const float *grad_alpha = nullptr,
-                         const GsbExtraFeatureArgs *ext = nullptr, const GsbPoseGradArgs *pose = nullptr) {
+                         const GsbExtraFeatureArgs *ext = nullptr, const GsbPoseGradArgs *pose = nullptr,
+                         const GsbIntrinsicsGradArgs *intr = nullptr) {
     if (!a) {
         set_error("backward: args is null");
         return GSB_EINVAL;
@@ -325,6 +326,7 @@ static int backward_impl(const GsbBackwardArgs *a, bool skip_on_overflow, const 
     if (ext && a->num_points > 0)  // the blend adds into the rows it reaches; every other row stays zero
         GSB_CUDA_CHECK(cudaMemsetAsync(ext->grad_features, 0, (size_t)a->num_points * ext->channels * 4, st));
     if ((rc = launch_blend_backward(*a, ws, st, grad_depth, depth, grad_alpha, ext)) != GSB_OK) return rc;
+    if (intr) return launch_backward_points_calib(*a, ws, st, grad_depth != nullptr, pose, *intr);
     if (pose) return launch_backward_points_pose(*a, ws, st, grad_depth != nullptr, *pose);
     return launch_backward_points(*a, ws, st, skip_on_overflow ? ws.counters + CNT_OVERFLOW : nullptr, grad_depth != nullptr);
 }
@@ -347,6 +349,31 @@ int64_t gsb200_pose_grad_temp_bytes(int32_t num_objects) {
 
 int gsb200_backward_pose(const GsbBackwardArgs *a, const float *grad_rasterized_depth, const float *rasterized_depth,
                          const float *grad_pixel_accumulated_alpha, const GsbExtraFeatureArgs *ext, const GsbPoseGradArgs *pose) {
+    return gsb200_backward_calib(a, grad_rasterized_depth, rasterized_depth, grad_pixel_accumulated_alpha, ext, pose, nullptr);
+}
+
+int64_t gsb200_intrinsics_grad_temp_bytes(void) {
+    return (int64_t)GSB_INTRINSICS_PARTIAL_BLOCKS * 6 * (int64_t)sizeof(float);
+}
+
+int gsb200_backward_calib(const GsbBackwardArgs *a, const float *grad_rasterized_depth, const float *rasterized_depth,
+                          const float *grad_pixel_accumulated_alpha, const GsbExtraFeatureArgs *ext, const GsbPoseGradArgs *pose,
+                          const GsbIntrinsicsGradArgs *intr) {
+    if (intr) {
+        if (!intr->grad_camera_intrinsics || !intr->temp) {
+            set_error("backward_calib: null grad_camera_intrinsics / temp pointer");
+            return GSB_EINVAL;
+        }
+        if (reinterpret_cast<uintptr_t>(intr->temp) % 16 != 0) {
+            set_error("backward_calib: the intrinsics temp must be 16-byte aligned");
+            return GSB_EINVAL;
+        }
+        if (a != nullptr && (a->flags & GSB_FLAG_COMPACT_GRADS)) {
+            set_error("backward_calib: the intrinsics gradient is not implemented for the compact rows of the view-parallel "
+                      "exchange (GSB_FLAG_COMPACT_GRADS)");
+            return GSB_EUNSUPPORTED;
+        }
+    }
     if (pose) {
         if (!pose->q_pointcloud_camera || !pose->grad_q_pointcloud_camera || !pose->grad_t_pointcloud_camera || !pose->temp) {
             set_error("backward_pose: null q_pointcloud_camera / grad_q_pointcloud_camera / grad_t_pointcloud_camera / temp "
@@ -396,7 +423,7 @@ int gsb200_backward_pose(const GsbBackwardArgs *a, const float *grad_rasterized_
                   "(GSB_FLAG_BACKWARD_TRANSPOSED); the butterfly kernel does not implement them");
         return GSB_EUNSUPPORTED;
     }
-    return backward_impl(a, false, grad_rasterized_depth, rasterized_depth, grad_pixel_accumulated_alpha, ext, pose);
+    return backward_impl(a, false, grad_rasterized_depth, rasterized_depth, grad_pixel_accumulated_alpha, ext, pose, intr);
 }
 
 int gsb200_backward_with_depth(const GsbBackwardArgs *a, const float *grad_rasterized_depth, const float *rasterized_depth) {

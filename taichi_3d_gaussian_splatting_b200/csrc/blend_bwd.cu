@@ -392,10 +392,33 @@ constexpr int PT_ROW_COMPACT = 20;  // COMPACT: 16 staged floats per row, same b
 // dL/dtw (3) of its object's T = [W | tw] -- which the warp sums per object (fixed butterfly order) into the per-warp rows
 // s_pose[warp][object][12]; after the loop the CTA adds its warps' rows in warp order into its partial row block
 // pose_partials[blockIdx.x][object][12].  pose_finish_kernel adds the blocks in block order: no float atomics anywhere.
+// INTR = true (gsb200_backward_calib): each in-camera point also forms its 6 intrinsics values -- dL/dK of rows 0 and 1,
+// row-major -- which the warp sums (fixed butterfly order, all objects together: a frame has one K) into the per-warp row
+// s_intr[warp][6]; after the loop the CTA adds its warps' rows in warp order into intr_partials[blockIdx.x][6], and
+// intrinsics_finish_kernel adds the blocks in block order.
 constexpr int POSE_VALUES = 12;
-template <bool COMPACT, bool DEPTH, bool POSE>
+constexpr int INTR_VALUES = 6;
+// B0, B1: the rows of G U Sigma (Sigma = M M^T, M = R diag(es)), so that dL/dU = 2 [B0; B1] for U = J W
+__device__ __forceinline__ void weighted_u_sigma(const float *U, const float *R, const float *es, float g00, float g01,
+                                                 float g11, float *B0, float *B1) {
+    float UM[6];  // U M, M = R diag(es)
+#pragma unroll
+    for (int a = 0; a < 2; ++a)
+#pragma unroll
+        for (int j = 0; j < 3; ++j)
+            UM[a * 3 + j] = (U[a * 3] * R[j] + U[a * 3 + 1] * R[3 + j] + U[a * 3 + 2] * R[6 + j]) * es[j];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {  // G U Sigma = G (U M) M^T
+        const float A0 = UM[0] * (R[c * 3] * es[0]) + UM[1] * (R[c * 3 + 1] * es[1]) + UM[2] * (R[c * 3 + 2] * es[2]);
+        const float A1 = UM[3] * (R[c * 3] * es[0]) + UM[4] * (R[c * 3 + 1] * es[1]) + UM[5] * (R[c * 3 + 2] * es[2]);
+        B0[c] = g00 * A0 + g01 * A1;
+        B1[c] = g01 * A0 + g11 * A1;
+    }
+}
+template <bool COMPACT, bool DEPTH, bool POSE, bool INTR = false>
 __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, float *s_pose, float *pose_partials,
-                                                     int num_objects) {
+                                                     int num_objects, float *s_intr = nullptr,
+                                                     float *intr_partials = nullptr) {
     // One thread per scene row: rows outside the frustum get their zeros here (no separate memset of the
     // dense (N,3)/(N,56) gradients), rows inside get the chain rule.  A warp owns 32 consecutive rows, i.e. one
     // contiguous 7 KB piece of the (N,56) gradient and 384 B of the (N,3) one: each lane stages its row in
@@ -412,12 +435,22 @@ __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, fl
         for (int k = lane; k < num_objects * POSE_VALUES; k += 32) my_pose[k] = 0.0f;
         __syncwarp();
     }
+    float *const my_intr = INTR ? s_intr + warp * INTR_VALUES : nullptr;
+    if (INTR) {
+        if (lane < INTR_VALUES) my_intr[lane] = 0.0f;
+        __syncwarp();
+    }
     const long long stride = (long long)gridDim.x * blockDim.x;
     for (long long base = (long long)blockIdx.x * blockDim.x + warp * 32; base < p.N; base += stride) {
       const long long id = base + lane;
       const int o = id < p.N ? p.point_offset[id] : -1;
       float pv[POSE ? POSE_VALUES : 1];
       int pose_obj = -1;
+      float iv[INTR ? INTR_VALUES : 1];  // zero for rows outside the frustum
+      if (INTR) {
+#pragma unroll
+          for (int k = 0; k < INTR_VALUES; ++k) iv[k] = 0.0f;
+      }
       if (o < 0) {
           if (!COMPACT) { my_xyz[0] = 0.0f; my_xyz[1] = 0.0f; my_xyz[2] = 0.0f; }
 #pragma unroll
@@ -515,20 +548,8 @@ __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, fl
 #pragma unroll
             for (int r = 0; r < 3; ++r) gp[r] = dj[r] * a0.x + dj[3 + r] * a0.y;
             if (DEPTH) gp[2] += a2.w;
-            float UM[6];  // U M, M = R diag(es)
-#pragma unroll
-            for (int a = 0; a < 2; ++a)
-#pragma unroll
-                for (int j = 0; j < 3; ++j)
-                    UM[a * 3 + j] = (U[a * 3] * R[j] + U[a * 3 + 1] * R[3 + j] + U[a * 3 + 2] * R[6 + j]) * es[j];
-            float B0[3], B1[3];  // G U Sigma = G (U M) M^T
-#pragma unroll
-            for (int c = 0; c < 3; ++c) {
-                const float A0 = UM[0] * (R[c * 3] * es[0]) + UM[1] * (R[c * 3 + 1] * es[1]) + UM[2] * (R[c * 3 + 2] * es[2]);
-                const float A1 = UM[3] * (R[c * 3] * es[0]) + UM[4] * (R[c * 3 + 1] * es[1]) + UM[5] * (R[c * 3 + 2] * es[2]);
-                B0[c] = g00 * A0 + g01 * A1;
-                B1[c] = g01 * A0 + g11 * A1;
-            }
+            float B0[3], B1[3];
+            weighted_u_sigma(U, R, es, g00, g01, g11, B0, B1);
             const float xw[3] = {x, y, z};
 #pragma unroll
             for (int c = 0; c < 3; ++c) {  // J = [J0 0 J2; 0 J4 J5]
@@ -538,6 +559,25 @@ __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, fl
                 pv[9 + c] = gp[c];
             }
             pose_obj = ob;
+        }
+        if (INTR) {
+            // uv = (K pc)[:2] / z: dL/dK[r][c] += guv_r pc_c / z.  Sigma' through J = [fx/z 0 -fx x/z^2; 0 fy/z -fy y/z^2]
+            // (pc detached in J): dL/dfx += 2 sum_c B0[c] (W[0][c]/z - x W[2][c]/z^2), dL/dfy likewise with B1 and row 1
+            float B0[3], B1[3];
+            weighted_u_sigma(U, R, es, g00, g01, g11, B0, B1);
+            const float ux = pcx * iz, uy = pcy * iz;
+            float sx0 = 0.0f, sy1 = 0.0f;
+#pragma unroll
+            for (int c = 0; c < 3; ++c) {
+                sx0 += B0[c] * (Wm[c] * iz - (pcx * Wm[6 + c]) * iz2);
+                sy1 += B1[c] * (Wm[3 + c] * iz - (pcy * Wm[6 + c]) * iz2);
+            }
+            iv[0] = a0.x * ux + 2.0f * sx0;
+            iv[1] = a0.x * uy;
+            iv[2] = a0.x;
+            iv[3] = a0.y * ux;
+            iv[4] = a0.y * uy + 2.0f * sy1;
+            iv[5] = a0.y;
         }
         if (p.ctl_num_in_camera != nullptr && !(p.skip_flag != nullptr && *p.skip_flag != 0)) {
             // GaussianPointAdaptiveController.update (:130-143) for this in-camera point: ids are unique, one thread per row,
@@ -599,6 +639,15 @@ __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, fl
               }
           }
       }
+      if (INTR) {
+#pragma unroll
+          for (int k = 0; k < INTR_VALUES; ++k) {
+              float v = iv[k];
+#pragma unroll
+              for (int d = 16; d > 0; d >>= 1) v += __shfl_xor_sync(0xffffffffu, v, d);
+              if (lane == 0) my_intr[k] += v;
+          }
+      }
       __syncwarp();
       const long long rows = p.N - base < 32 ? p.N - base : 32;
       if (COMPACT) {
@@ -639,6 +688,14 @@ __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, fl
             float s = s_pose[k];
             for (int w = 1; w < GSB_POINTS_THREADS / 32; ++w) s += s_pose[w * num_objects * POSE_VALUES + k];
             out[k] = s;
+        }
+    }
+    if (INTR) {
+        __syncthreads();
+        if (threadIdx.x < INTR_VALUES) {
+            float s = s_intr[threadIdx.x];
+            for (int w = 1; w < GSB_POINTS_THREADS / 32; ++w) s += s_intr[w * INTR_VALUES + threadIdx.x];
+            intr_partials[(size_t)blockIdx.x * INTR_VALUES + threadIdx.x] = s;
         }
     }
 }
@@ -726,6 +783,47 @@ pose_finish_kernel(const float *__restrict__ partials, int blocks, int num_objec
     grad_q[4 * ob + 1] = -g[1];
     grad_q[4 * ob + 2] = -g[2];
     grad_q[4 * ob + 3] = g[3];
+}
+
+// The parameter block of the INTR instantiations (pose_partials / num_objects are read only with POSE).
+struct PointsBwdCalibParams : PointsBwdPoseParams {
+    float *intr_partials;  // (grid, 6)
+};
+
+// Intrinsics alone (POSE = false) or pose and intrinsics in one pass over the scene rows (POSE = true).
+template <bool DEPTH, bool POSE>
+__global__ void __launch_bounds__(GSB_POINTS_THREADS, POSE ? 4 : 5)  // 6 or 18 values live across the SH epilogue
+backward_points_calib_kernel(const PointsBwdCalibParams p) {
+    __shared__ float s_pose[POSE ? (GSB_POINTS_THREADS / 32) * GSB_POSE_MAX_OBJECTS * POSE_VALUES : 1];
+    __shared__ float s_intr[(GSB_POINTS_THREADS / 32) * INTR_VALUES];
+    backward_points_body<false, DEPTH, POSE, true>(p, POSE ? s_pose : nullptr, p.pose_partials, p.num_objects, s_intr,
+                                                   p.intr_partials);
+}
+
+// One CTA: adds the `blocks` partial rows in a fixed order (strided per thread, then a fixed shared-memory tree) and
+// writes the whole (3,3) dL/dK, row 2 zero (the forward never reads it).  Zeros when blocks == 0.
+constexpr int INTR_FINISH_THREADS = 128;
+__global__ void __launch_bounds__(INTR_FINISH_THREADS)
+intrinsics_finish_kernel(const float *__restrict__ partials, int blocks, float *__restrict__ grad_K) {
+    __shared__ float s_sum[INTR_FINISH_THREADS][INTR_VALUES + 1];
+    const int tid = threadIdx.x;
+    float acc[INTR_VALUES];
+#pragma unroll
+    for (int k = 0; k < INTR_VALUES; ++k) acc[k] = 0.0f;
+    for (int b = tid; b < blocks; b += INTR_FINISH_THREADS) {
+#pragma unroll
+        for (int k = 0; k < INTR_VALUES; ++k) acc[k] += partials[(size_t)b * INTR_VALUES + k];
+    }
+#pragma unroll
+    for (int k = 0; k < INTR_VALUES; ++k) s_sum[tid][k] = acc[k];
+    __syncthreads();
+    for (int h = INTR_FINISH_THREADS / 2; h > 0; h >>= 1) {
+        if (tid < h)
+#pragma unroll
+            for (int k = 0; k < INTR_VALUES; ++k) s_sum[tid][k] += s_sum[tid + h][k];
+        __syncthreads();
+    }
+    if (tid < 9) grad_K[tid] = tid < INTR_VALUES ? s_sum[0][tid] : 0.0f;
 }
 
 // ------------------------------------------------------------------ view-parallel exchange: rebuild the dense gradients
@@ -898,6 +996,40 @@ int launch_backward_points_pose(const GsbBackwardArgs &a, const Workspace &ws, c
     pose_finish_kernel<<<a.num_objects, POSE_FINISH_THREADS, 0, stream>>>(
         p.pose_partials, (int)blocks, a.num_objects, pose.q_pointcloud_camera, a.t_pointcloud_camera,
         pose.grad_q_pointcloud_camera, pose.grad_t_pointcloud_camera);
+    GSB_CUDA_CHECK(cudaGetLastError());
+    return GSB_OK;
+}
+
+// The INTR per-point kernel (with the pose sums too when `pose` is set: one pass) on the POSE kernel's grid, then the
+// finishing kernels.  The caller checked `pose` and `intr`.
+int launch_backward_points_calib(const GsbBackwardArgs &a, const Workspace &ws, cudaStream_t stream, bool depth_grad,
+                                 const GsbPoseGradArgs *pose, const GsbIntrinsicsGradArgs &intr) {
+    static_assert(GSB_INTRINSICS_PARTIAL_BLOCKS == GSB_POSE_PARTIAL_BLOCKS, "the combined kernel has one grid");
+    PointsBwdCalibParams p;
+    static_cast<PointsBwdParams &>(p) = make_points_params(a, ws, nullptr);
+    p.pose_partials = pose ? static_cast<float *>(pose->temp) : nullptr;
+    p.num_objects = pose ? a.num_objects : 0;
+    p.intr_partials = static_cast<float *>(intr.temp);
+    long long blocks = a.num_points > 0 ? (a.num_points + GSB_POINTS_THREADS - 1) / GSB_POINTS_THREADS : 0;
+    if (blocks > GSB_INTRINSICS_PARTIAL_BLOCKS) blocks = GSB_INTRINSICS_PARTIAL_BLOCKS;
+    if (blocks > 0) {
+        if (pose) {
+            if (depth_grad) backward_points_calib_kernel<true, true><<<(int)blocks, GSB_POINTS_THREADS, 0, stream>>>(p);
+            else backward_points_calib_kernel<false, true><<<(int)blocks, GSB_POINTS_THREADS, 0, stream>>>(p);
+        } else {
+            if (depth_grad) backward_points_calib_kernel<true, false><<<(int)blocks, GSB_POINTS_THREADS, 0, stream>>>(p);
+            else backward_points_calib_kernel<false, false><<<(int)blocks, GSB_POINTS_THREADS, 0, stream>>>(p);
+        }
+        GSB_CUDA_CHECK(cudaGetLastError());
+    }
+    if (pose) {
+        pose_finish_kernel<<<a.num_objects, POSE_FINISH_THREADS, 0, stream>>>(
+            p.pose_partials, (int)blocks, a.num_objects, pose->q_pointcloud_camera, a.t_pointcloud_camera,
+            pose->grad_q_pointcloud_camera, pose->grad_t_pointcloud_camera);
+        GSB_CUDA_CHECK(cudaGetLastError());
+    }
+    intrinsics_finish_kernel<<<1, INTR_FINISH_THREADS, 0, stream>>>(p.intr_partials, (int)blocks,
+                                                                     intr.grad_camera_intrinsics);
     GSB_CUDA_CHECK(cudaGetLastError());
     return GSB_OK;
 }

@@ -83,6 +83,10 @@ int launch_backward_points(const GsbBackwardArgs &a, const Workspace &ws, cudaSt
 // in pose.temp) and the per-object finishing kernel; arguments checked by the caller
 int launch_backward_points_pose(const GsbBackwardArgs &a, const Workspace &ws, cudaStream_t stream, bool depth_grad,
                                 const GsbPoseGradArgs &pose);
+// gsb200_backward_calib with intrinsics: the INTR per-point kernel (with the pose sums as well when `pose` is set, in the
+// same pass) and the finishing kernels; arguments checked by the caller
+int launch_backward_points_calib(const GsbBackwardArgs &a, const Workspace &ws, cudaStream_t stream, bool depth_grad,
+                                 const GsbPoseGradArgs *pose, const GsbIntrinsicsGradArgs &intr);
 int launch_adam_step(float *param, const float *grad, float *exp_avg, float *exp_avg_sq, long long n, double lr, double beta1,
                      double beta2, double eps, int step, const long long *skip_flag, cudaStream_t stream);
 int launch_expand_view_gradients(const GsbExpandArgs &a, cudaStream_t stream);

@@ -17,6 +17,8 @@ l2 loss on the rendered feature map (``loss.feature_loss``) and a third Adam on 
 through densification.
 Optional pose refinement (an extension; ``TrainConfig.pose_learning_rate``): the (q, t) of every training view but the
 first become trainable, differentiated by the operator's ``differentiable_pose`` and stepped by their own Adam.
+Optional intrinsics refinement (an extension; ``TrainConfig.intrinsics_learning_rate``): per camera, a correction of the focal
+lengths and the principal point, differentiated by the operator's ``differentiable_intrinsics`` and stepped by its own Adam.
 The rasteriser is injected (default: the CUDA operator) so that tests can run the identical loop with the
 CPU oracle behind the same interface and compare PSNR trajectories.
 """
@@ -130,6 +132,11 @@ class GaussianPointCloudTrainer:
         # trained by their own Adam at this rate, q renormalised after each step.  View 0's pose stays fixed and is the
         # reference frame; the global scale of scene and translations is not pinned.  Not with fused_step.
         pose_learning_rate: float = 0.
+        # optional intrinsics refinement: > 0 gives every camera_id of the training views four leaf scalars, initialised to
+        # 0 and trained by their own Adam at this rate -- the log-scales of fx and fy, and the offsets of cx and cy in units
+        # of the view's full-resolution width and height.  Skew and K[1,0] are not trained.  Combines with
+        # pose_learning_rate.  Not with fused_step.
+        intrinsics_learning_rate: float = 0.
 
     def __init__(self, config: "GaussianPointCloudTrainer.TrainConfig", scene: Scene, train_views: List[View],
                  rasterisation_factory: Optional[Callable] = None, generator: Optional[torch.Generator] = None,
@@ -169,6 +176,19 @@ class GaussianPointCloudTrainer:
         self._poses = [(v[1], v[2]) if i == 0 or not self._pose else
                        (v[1].detach().clone().requires_grad_(True), v[2].detach().clone().requires_grad_(True))
                        for i, v in enumerate(train_views)]
+        if not (config.intrinsics_learning_rate >= 0.0 and config.intrinsics_learning_rate < float("inf")):
+            raise ValueError(f"intrinsics_learning_rate must be finite and >= 0, got {config.intrinsics_learning_rate}")
+        self._intr = config.intrinsics_learning_rate > 0
+        if self._intr and fused_step:
+            raise ValueError("fused_step does not implement intrinsics refinement (intrinsics_learning_rate > 0)")
+        # the trainable intrinsics corrections, one per camera_id: (log fx scale, log fy scale, cx / W, cy / H)
+        self._intrinsics = {}
+        if self._intr:
+            for v in train_views:
+                ci = v[3]
+                if ci.camera_id not in self._intrinsics:
+                    self._intrinsics[ci.camera_id] = torch.zeros(4, dtype=torch.float32, device=ci.camera_intrinsics.device,
+                                                                 requires_grad=True)
         self._features = config.feature_loss != "none"
         if self._features:
             self._check_feature_config(config, scene, targets)
@@ -200,7 +220,8 @@ class GaussianPointCloudTrainer:
         # the differentiable outputs only when a term needs them: injected factories without them keep working
         extra = dict(**({"differentiable_depth": True} if self._need_depth else {}),
                      **({"differentiable_alpha": True} if self._need_alpha else {}),
-                     **({"differentiable_pose": True} if self._pose else {}))
+                     **({"differentiable_pose": True} if self._pose else {}),
+                     **({"differentiable_intrinsics": True} if self._intr else {}))
         self.rasterisation = factory(config=config.rasterisation_config,
                                      backward_valid_point_hook=self.adaptive_controller.update, **extra)
         self.loss_function = LossFunction(config=config.loss_function_config)
@@ -260,6 +281,25 @@ class GaussianPointCloudTrainer:
                                           if self.supervised or self._features else targets)
             image_gt, camera_info, targets = self._downsampled[key]
         return image_gt, q, t, camera_info, targets
+
+    def _intrinsics_of(self, view_index: int, downsample_factor: int) -> torch.Tensor:
+        """The K of a view as trained, built by torch ops (differentiable in its camera's correction): the view's own
+        full-resolution K with fx, fy scaled by exp(log-scale) and cx, cy shifted by offset * (W, H), then fx, fy, cx, cy
+        divided by the downsample factor as ``downsample_image_and_camera_info`` does."""
+        ci = self.train_views[view_index][3]
+        K = ci.camera_intrinsics
+        corr = self._intrinsics[ci.camera_id]
+        rows, cols = torch.tensor([0, 1], device=K.device), torch.tensor([2, 2], device=K.device)
+        size = torch.tensor([float(ci.camera_width), float(ci.camera_height)], dtype=K.dtype, device=K.device)
+        scale = torch.ones_like(K).index_put((rows, rows), torch.exp(corr[:2]))
+        shift = torch.zeros_like(K).index_put((rows, cols), corr[2:] * size)
+        K = K * scale + shift
+        if downsample_factor > 1:
+            div = torch.ones_like(K).index_put((torch.tensor([0, 1, 0, 1], device=K.device),
+                                                torch.tensor([0, 1, 2, 2], device=K.device)),
+                                               torch.tensor(float(downsample_factor), dtype=K.dtype, device=K.device))
+            K = K / div
+        return K
 
     def _next_background(self) -> Optional[torch.Tensor]:
         """The background of this iteration: None (black), white, or a fresh colour drawn on the device."""
@@ -344,6 +384,8 @@ class GaussianPointCloudTrainer:
                                betas=(0.9, 0.999)) if self._features else None
         pose_optimizer = Adam([x for q, t in self._poses[1:] for x in (q, t)], lr=cfg.pose_learning_rate,
                               betas=(0.9, 0.999)) if self._pose and len(self._poses) > 1 else None
+        intrinsics_optimizer = Adam(list(self._intrinsics.values()), lr=cfg.intrinsics_learning_rate,
+                                    betas=(0.9, 0.999)) if self._intr else None
         scheduler = torch.optim.lr_scheduler.ExponentialLR(position_optimizer, gamma=cfg.position_learning_rate_decay_rate)
         downsample_factor = cfg.initial_downsample_factor
         for iteration in range(cfg.num_iterations):
@@ -355,8 +397,14 @@ class GaussianPointCloudTrainer:
                 extra_optimizer.zero_grad()
             if pose_optimizer is not None:
                 pose_optimizer.zero_grad()
+            if intrinsics_optimizer is not None:
+                intrinsics_optimizer.zero_grad()
             view_index = self._next_view_index(iteration)
             image_gt, q, t, camera_info, targets = self._view(view_index, downsample_factor)
+            if self._intr:  # built every iteration: the cached downsampled camera must not freeze K
+                camera_info = CameraInfo(camera_intrinsics=self._intrinsics_of(view_index, downsample_factor),
+                                         camera_height=camera_info.camera_height, camera_width=camera_info.camera_width,
+                                         camera_id=camera_info.camera_id)
             band = iteration // cfg.increase_color_max_sh_band_interval
             if self.supervised or self._features:
                 loss, l1_loss, mask_term, depth_term, feature_term, image_pred = self._supervised_loss(
@@ -383,6 +431,8 @@ class GaussianPointCloudTrainer:
                 with torch.no_grad():
                     for q_v, _ in self._poses[1:]:
                         q_v.div_(q_v.norm(dim=-1, keepdim=True))
+            if intrinsics_optimizer is not None:
+                intrinsics_optimizer.step()
             if iteration % cfg.position_learning_rate_decay_interval == 0:
                 scheduler.step()
             self.adaptive_controller.refinement()
@@ -427,6 +477,14 @@ class GaussianPointCloudTrainer:
     def refined_poses(self) -> List[Tuple[torch.Tensor, torch.Tensor]]:
         """(q, t) of every training view as trained (detached copies; the views' own poses without pose refinement)."""
         return [(q.detach().clone(), t.detach().clone()) for q, t in self._poses]
+
+    def refined_intrinsics(self) -> List[torch.Tensor]:
+        """The full-resolution (3, 3) K of every training view as trained (detached copies; the views' own K without
+        intrinsics refinement)."""
+        if not self._intr:
+            return [v[3].camera_intrinsics.detach().clone() for v in self.train_views]
+        with torch.no_grad():
+            return [self._intrinsics_of(i, 1).clone() for i in range(len(self.train_views))]
 
     @torch.no_grad()
     def validation(self, views: Optional[List[View]] = None) -> float:
