@@ -205,7 +205,7 @@ const char *gsb200_last_error(void);
  * foreign-language binding verify its struct mirrors. */
 void gsb200_abi_sizes(int64_t *out3);
 /* ... and of the first n of {GsbWorkspaceLayout, GsbForwardArgs, GsbBackwardArgs, GsbExpandArgs, GsbTrainStepArgs,
- * GsbSupervisionArgs, GsbExtraFeatureArgs, GsbFeatureTrainArgs, GsbPoseGradArgs, GsbIntrinsicsGradArgs} */
+ * GsbSupervisionArgs, GsbExtraFeatureArgs, GsbFeatureTrainArgs, GsbPoseGradArgs, GsbIntrinsicsGradArgs, GsbLensArgs} */
 void gsb200_abi_sizes_ext(int64_t *out, int32_t n);
 
 /* Workspace sizing.  far_plane*depth_to_sort_key_scale fixes the depth-key width; (H/16)*(W/16)
@@ -351,6 +351,41 @@ int gsb200_backward_calib(const GsbBackwardArgs *args, const float *grad_rasteri
                           const float *grad_pixel_accumulated_alpha, const GsbExtraFeatureArgs *ext,
                           const GsbPoseGradArgs *pose,               /* or NULL */
                           const GsbIntrinsicsGradArgs *intrinsics);  /* or NULL */
+
+/* Lens distortion (an extension: the reference projects through a pinhole).  The lens acts between the camera-frame point
+ * pc = (x, y, z) and K.  With xn = x/z, yn = y/z, r^2 = xn^2 + yn^2:
+ *   GSB_LENS_OPENCV (k1 k2 p1 p2 k3, OpenCV's distCoeffs order; COLMAP SIMPLE_RADIAL, RADIAL, OPENCV):
+ *     rad = 1 + k1 r^2 + k2 r^4 + k3 r^6,  xd = xn rad + 2 p1 xn yn + p2 (r^2 + 2 xn^2),  yd = yn rad + p1 (r^2 + 2 yn^2) + 2 p2 xn yn
+ *   GSB_LENS_FISHEYE (equidistant, k1 k2 k3 k4; COLMAP OPENCV_FISHEYE, cv2.fisheye; coefficients[4] must be 0):
+ *     theta = atan(r),  theta_d = theta (1 + k1 theta^2 + k2 theta^4 + k3 theta^6 + k4 theta^8),  (xd, yd) = (theta_d / r) (xn, yn)
+ *     (theta_d / r -> 1 on the optical axis; a series is used for small r)
+ *   u = K00 xd + K01 yd + K02,  v = K10 xd + K11 yd + K12   (today's (K pc)[:2] / z with (xn, yn) replaced by (xd, yd)).
+ * The covariance uses J = diag(fx, fy) D P with D = d(xd, yd)/d(xn, yn) and P = [1/z 0 -x/z^2; 0 1/z -y/z^2] (D = I is the
+ * pinhole J); the 0.3 low-pass, rescale, radius, bounding box and reach filter follow from Sigma' as for a pinhole.
+ * Validity: the radial map folds back beyond r_max -- for opencv the smallest positive root of 1 + 3 k1 r^2 + 5 k2 r^4 +
+ * 7 k3 r^6 (tangential terms ignored; none: unbounded), for fisheye tan(min(pi/2, smallest positive root of dtheta_d/dtheta)).
+ * The bound is computed once per call on the host in double and applied as an r^2 bound: a point with r^2 > r_max^2 is
+ * outside the frustum (no key, point_offset -1, zero gradient).  The near / far / image-border tests apply to the distorted
+ * (u, v).  Gradients: d uv / d pc = K[:2,:2] D P exactly; Sigma' uses the lens J; the conventions of the point gradients
+ * hold (J's dependence on pc, the SH view direction and rescale detached, the 0.99 clamp straight-through, the validity cut
+ * not differentiated).  No gradient with respect to the coefficients. */
+#define GSB_LENS_PINHOLE 0
+#define GSB_LENS_OPENCV 1
+#define GSB_LENS_FISHEYE 2
+typedef struct GsbLensArgs {
+    int32_t model;          /* GSB_LENS_* */
+    float coefficients[5];  /* opencv: k1 k2 p1 p2 k3; fisheye: k1 k2 k3 k4 0 */
+} GsbLensArgs;
+/* gsb200_forward_ext through the lens of `lens`.  NULL lens or GSB_LENS_PINHOLE: exactly gsb200_forward_ext.  Before any
+ * CUDA call: GSB_EINVAL for an unknown model, a non-finite coefficient or a non-zero unused coefficient. */
+int gsb200_forward_lens(const GsbForwardArgs *args, const GsbExtraFeatureArgs *ext, const GsbLensArgs *lens);
+/* gsb200_backward_ext of a frame rendered by gsb200_forward_lens with the same lens.  NULL lens or GSB_LENS_PINHOLE: exactly
+ * gsb200_backward_ext.  Before any CUDA call: the lens checks of gsb200_forward_lens, and GSB_EUNSUPPORTED with
+ * GSB_FLAG_COMPACT_GRADS (the view-parallel exchange does not rebuild lens gradients).  An image-only loss works with either
+ * loop-A kernel; the other terms keep their requirement of GSB_FLAG_BACKWARD_TRANSPOSED. */
+int gsb200_backward_lens(const GsbBackwardArgs *args, const float *grad_rasterized_depth, const float *rasterized_depth,
+                         const float *grad_pixel_accumulated_alpha, const GsbExtraFeatureArgs *ext,
+                         const GsbLensArgs *lens);  /* or NULL */
 
 int gsb200_expand_view_gradients(const GsbExpandArgs *args);
 

@@ -2,12 +2,66 @@
 
 Mirrors the reference's ``taichi_3d_gaussian_splatting/Camera.py:7-21`` (``CameraInfo`` is an
 argument of ``GaussianPointCloudRasterisationInput``; ``CameraView`` is imported beside it at
-GaussianPointCloudRasterisation.py:4).
+GaussianPointCloudRasterisation.py:4).  ``LensDistortion`` and ``CameraInfo.distortion`` are an extension: the reference
+projects through a pinhole only.
 """
+import math
 from dataclasses import dataclass
-from typing import Optional
+from typing import Optional, Sequence, Tuple
 
 import torch
+
+_LENS_COEFFICIENTS = {"opencv": 5, "fisheye": 4}
+
+
+@dataclass(frozen=True)
+class LensDistortion:
+    """A lens between the camera-frame point and K (definition in ``include/gsb200.h``), as host floats so that rendering a
+    view reads nothing back from the device.
+
+    ``model``: ``"opencv"`` -- coefficients ``(k1, k2, p1, p2, k3)`` in OpenCV's ``distCoeffs`` order (COLMAP
+    ``SIMPLE_RADIAL``, ``RADIAL``, ``OPENCV``) -- or ``"fisheye"`` -- ``(k1, k2, k3, k4)`` of the equidistant model (COLMAP
+    ``OPENCV_FISHEYE``, ``cv2.fisheye``).  The coefficients act on the normalised image plane (x/z, y/z), so resizing or
+    cropping an image changes K but not them."""
+    model: str
+    coefficients: Tuple[float, ...]
+
+    def __post_init__(self):
+        if self.model not in _LENS_COEFFICIENTS:
+            raise ValueError(f"lens model must be one of {tuple(_LENS_COEFFICIENTS)}, got {self.model!r}")
+        co = tuple(float(v) for v in self.coefficients)
+        if len(co) != _LENS_COEFFICIENTS[self.model]:
+            raise ValueError(f"the {self.model} lens takes {_LENS_COEFFICIENTS[self.model]} coefficients, got {len(co)}")
+        if not all(math.isfinite(v) for v in co):
+            raise ValueError(f"lens coefficients must be finite, got {co}")
+        object.__setattr__(self, "coefficients", co)
+
+    @staticmethod
+    def from_colmap(model_name: str, params: Sequence[float]) -> Tuple[torch.Tensor, Optional["LensDistortion"]]:
+        """(K (3,3) float32, lens or None) of a COLMAP camera: ``SIMPLE_PINHOLE`` (f cx cy), ``PINHOLE`` (fx fy cx cy),
+        ``SIMPLE_RADIAL`` (f cx cy k), ``RADIAL`` (f cx cy k1 k2), ``OPENCV`` (fx fy cx cy k1 k2 p1 p2) and
+        ``OPENCV_FISHEYE`` (fx fy cx cy k1 k2 k3 k4).  ``ValueError`` for any other model or a wrong parameter count."""
+        counts = {"SIMPLE_PINHOLE": 3, "PINHOLE": 4, "SIMPLE_RADIAL": 4, "RADIAL": 5, "OPENCV": 8, "OPENCV_FISHEYE": 8}
+        if model_name not in counts:
+            raise ValueError(f"unsupported COLMAP camera model {model_name!r}: expected one of {tuple(counts)}")
+        p = [float(v) for v in params]
+        if len(p) != counts[model_name]:
+            raise ValueError(f"COLMAP {model_name} has {counts[model_name]} parameters, got {len(p)}")
+        if model_name in ("SIMPLE_PINHOLE", "SIMPLE_RADIAL", "RADIAL"):
+            fx = fy = p[0]
+            cx, cy, rest = p[1], p[2], p[3:]
+        else:
+            fx, fy, cx, cy, rest = p[0], p[1], p[2], p[3], p[4:]
+        K = torch.tensor([[fx, 0.0, cx], [0.0, fy, cy], [0.0, 0.0, 1.0]], dtype=torch.float32)
+        if model_name == "SIMPLE_RADIAL":
+            return K, LensDistortion("opencv", (rest[0], 0.0, 0.0, 0.0, 0.0))
+        if model_name == "RADIAL":
+            return K, LensDistortion("opencv", (rest[0], rest[1], 0.0, 0.0, 0.0))
+        if model_name == "OPENCV":
+            return K, LensDistortion("opencv", tuple(rest) + (0.0,))
+        if model_name == "OPENCV_FISHEYE":
+            return K, LensDistortion("fisheye", tuple(rest))
+        return K, None
 
 
 @dataclass
@@ -16,6 +70,7 @@ class CameraInfo:
     camera_height: int
     camera_width: int
     camera_id: int
+    distortion: Optional[LensDistortion] = None  # extension: None is the reference's pinhole
 
 
 @dataclass

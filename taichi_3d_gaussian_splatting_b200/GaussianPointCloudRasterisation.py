@@ -345,6 +345,7 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                                       *((q_pointcloud_camera,) if outer.differentiable_pose else ()),
                                       *((extra_features,) if extra_features is not None else ()))
                 ctx.frame = frame
+                ctx.lens = saved["lens"]
                 ctx.num_objects = q_pointcloud_camera.shape[0]
                 ctx.color_max_sh_band = color_max_sh_band
                 ctx.has_extra_features = extra_features is not None
@@ -449,6 +450,7 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                      q_pointcloud_camera, t_pointcloud_camera, camera_info, extra_features=None):
         cfg = self.config
         lib = _lib.load()
+        lens = self._lens_args(camera_info)
         _require(pointcloud, "point_cloud", torch.float32, (3,))
         _require(pointcloud_features, "point_cloud_features", torch.float32, (56,))
         _require(point_invalid_mask, "point_invalid_mask", torch.int8)
@@ -512,7 +514,10 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                         host_counters=pinned.data_ptr(), host_counters_event=event.cuda_event)
                     # The whole frame is enqueued by this one call; the library copies {M, K, overflow} to pinned
                     # host memory right after the per-point stage and records `event` behind that copy.
-                    if ext is None:
+                    if lens is not None:
+                        _lib.check(lib.gsb200_forward_lens(ctypes.byref(args), ctypes.byref(ext) if ext is not None else None,
+                                                           ctypes.byref(lens)), "gsb200_forward_lens")
+                    elif ext is None:
                         _lib.check(lib.gsb200_forward(ctypes.byref(args)), "gsb200_forward")
                     else:  # the re-run after an overflow renders the feature map as well
                         _lib.check(lib.gsb200_forward_ext(ctypes.byref(args), ctypes.byref(ext)), "gsb200_forward_ext")
@@ -532,7 +537,20 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                 _PinnedCounters.release(device, readback)
         self.last_frame = frame
         outs = (image, depth, acc_alpha, last_effective, valid_count) + ((feature_map,) if feature_map is not None else ())
-        return outs, frame, {"camera_intrinsics": K}
+        return outs, frame, {"camera_intrinsics": K, "lens": lens}
+
+    def _lens_args(self, camera_info) -> Optional[_lib.GsbLensArgs]:
+        """The C lens argument of ``camera_info.distortion`` (None: the pinhole kernels), after the checks of the options
+        a lens does not combine with."""
+        distortion = getattr(camera_info, "distortion", None)
+        if distortion is None:
+            return None
+        for name, on in (("differentiable_pose", self.differentiable_pose),
+                         ("differentiable_intrinsics", self.differentiable_intrinsics),
+                         ("a gradient_exchange", self.gradient_exchange is not None)):
+            if on:
+                raise ValueError(f"a camera with lens distortion is not supported with {name}")
+        return _lib.lens_args(distortion)
 
     # ------------------------------------------------------------------ backward plumbing
     def _run_backward(self, ctx, grad_rasterized_image, grad_rasterized_depth=None, grad_pixel_accumulated_alpha=None,
@@ -606,7 +624,16 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                 grad_extra_features = torch.zeros((N, C), dtype=torch.float32, device=device) if grad_feature_map is None \
                     else torch.empty((N, C), dtype=torch.float32, device=device)
             grad_q = grad_t = grad_K = None
-            if pose or intrinsics:
+            if ctx.lens is not None:  # neither pose nor intrinsics gradients (refused in forward)
+                ext = None
+                if extra_features is not None and grad_feature_map is not None:
+                    grad_map = _f32(grad_feature_map)
+                    ext = _lib.GsbExtraFeatureArgs(channels=extra_features.shape[1], features=_ptr(extra_features),
+                                                   grad_rasterized=_ptr(grad_map), grad_features=_ptr(grad_extra_features))
+                _lib.check(lib.gsb200_backward_lens(ctypes.byref(args), _ptr(grad_depth), _ptr(depth), _ptr(grad_alpha),
+                                                    ctypes.byref(ext) if ext is not None else None, ctypes.byref(ctx.lens)),
+                           "gsb200_backward_lens")
+            elif pose or intrinsics:
                 pose_args = intr_args = None
                 if pose:
                     n_obj = ctx.num_objects
@@ -711,7 +738,11 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
         the backward runs for the features alone too.  Combines with ``differentiable_depth`` and ``differentiable_alpha``.
         ``ValueError`` with ``backward_impl="butterfly"``, ``config.rgb_only``, a ``gradient_exchange``, or a tensor of the
         wrong shape, dtype, device or layout.  The densification controller does not know these rows: a caller who clones,
-        splits or removes Gaussians must keep ``point_extra_features`` in step."""
+        splits or removes Gaussians must keep ``point_extra_features`` in step.
+        ``input_data.camera_info.distortion`` (an extension; ``Camera.LensDistortion``): render and differentiate through
+        an OpenCV radial-tangential or fisheye lens (``gsb200_forward_lens`` / ``gsb200_backward_lens``; definition in
+        ``include/gsb200.h``).  Every output and option above works with a lens, except ``differentiable_pose``,
+        ``differentiable_intrinsics`` and a ``gradient_exchange`` (``ValueError``); the coefficients get no gradient."""
         camera_info = input_data.camera_info
         assert camera_info.camera_width % TILE_WIDTH == 0
         assert camera_info.camera_height % TILE_HEIGHT == 0

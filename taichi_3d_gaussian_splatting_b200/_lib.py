@@ -118,6 +118,22 @@ class GsbIntrinsicsGradArgs(ctypes.Structure):
     _fields_ = [("grad_camera_intrinsics", c_vp), ("temp", c_vp)]
 
 
+class GsbLensArgs(ctypes.Structure):
+    _fields_ = [("model", c_i32), ("coefficients", c_f32 * 5)]
+
+
+GSB_LENS_PINHOLE = 0
+GSB_LENS_OPENCV = 1
+GSB_LENS_FISHEYE = 2
+
+
+def lens_args(distortion) -> GsbLensArgs:
+    """The C argument of a ``Camera.LensDistortion`` (host floats; unused coefficients 0)."""
+    model = {"opencv": GSB_LENS_OPENCV, "fisheye": GSB_LENS_FISHEYE}[distortion.model]
+    co = list(distortion.coefficients) + [0.0] * (5 - len(distortion.coefficients))
+    return GsbLensArgs(model=model, coefficients=(c_f32 * 5)(*co))
+
+
 GSB_FEATURE_LOSS_CROSS_ENTROPY = 1
 GSB_FEATURE_LOSS_L2 = 2
 
@@ -141,7 +157,8 @@ EXPORTS = (
     "gsb200_train_step", "gsb200_abi_sizes_ext", "gsb200_exchange_multimem", "gsb200_backward_with_depth",
     "gsb200_backward_aux", "gsb200_supervision_temp_bytes", "gsb200_train_step_aux", "gsb200_forward_ext",
     "gsb200_backward_ext", "gsb200_feature_loss_temp_bytes", "gsb200_train_step_ext", "gsb200_backward_pose",
-    "gsb200_pose_grad_temp_bytes", "gsb200_backward_calib", "gsb200_intrinsics_grad_temp_bytes",
+    "gsb200_pose_grad_temp_bytes", "gsb200_backward_calib", "gsb200_intrinsics_grad_temp_bytes", "gsb200_forward_lens",
+    "gsb200_backward_lens",
 )
 
 _lib = None
@@ -183,6 +200,12 @@ def load() -> ctypes.CDLL:
     lib.gsb200_backward_calib.argtypes = [ctypes.POINTER(GsbBackwardArgs), c_vp, c_vp, c_vp, ctypes.POINTER(GsbExtraFeatureArgs),
                                           ctypes.POINTER(GsbPoseGradArgs), ctypes.POINTER(GsbIntrinsicsGradArgs)]
     lib.gsb200_backward_calib.restype = ctypes.c_int
+    lib.gsb200_forward_lens.argtypes = [ctypes.POINTER(GsbForwardArgs), ctypes.POINTER(GsbExtraFeatureArgs),
+                                        ctypes.POINTER(GsbLensArgs)]
+    lib.gsb200_forward_lens.restype = ctypes.c_int
+    lib.gsb200_backward_lens.argtypes = [ctypes.POINTER(GsbBackwardArgs), c_vp, c_vp, c_vp, ctypes.POINTER(GsbExtraFeatureArgs),
+                                         ctypes.POINTER(GsbLensArgs)]
+    lib.gsb200_backward_lens.restype = ctypes.c_int
     lib.gsb200_intrinsics_grad_temp_bytes.argtypes = []
     lib.gsb200_intrinsics_grad_temp_bytes.restype = c_i64
     lib.gsb200_sort_temp_bytes.argtypes = [c_i64, c_i32]
@@ -275,6 +298,11 @@ def load() -> ctypes.CDLL:
     if sizes10[9] != ctypes.sizeof(GsbIntrinsicsGradArgs):
         raise RuntimeError(f"libgsb200.so ABI mismatch: sizeof(GsbIntrinsicsGradArgs) {sizes10[9]} != ctypes mirror "
                            f"{ctypes.sizeof(GsbIntrinsicsGradArgs)}")
+    sizes11 = (c_i64 * 11)()
+    lib.gsb200_abi_sizes_ext(sizes11, 11)
+    if sizes11[10] != ctypes.sizeof(GsbLensArgs):
+        raise RuntimeError(f"libgsb200.so ABI mismatch: sizeof(GsbLensArgs) {sizes11[10]} != ctypes mirror "
+                           f"{ctypes.sizeof(GsbLensArgs)}")
     _lib = lib
     return lib
 

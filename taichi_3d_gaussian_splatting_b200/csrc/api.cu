@@ -192,11 +192,11 @@ void gsb200_abi_sizes(int64_t *out3) {
 }
 
 void gsb200_abi_sizes_ext(int64_t *out, int32_t n) {
-    const int64_t all[10] = {(int64_t)sizeof(GsbWorkspaceLayout), (int64_t)sizeof(GsbForwardArgs), (int64_t)sizeof(GsbBackwardArgs),
+    const int64_t all[11] = {(int64_t)sizeof(GsbWorkspaceLayout), (int64_t)sizeof(GsbForwardArgs), (int64_t)sizeof(GsbBackwardArgs),
                              (int64_t)sizeof(GsbExpandArgs), (int64_t)sizeof(GsbTrainStepArgs), (int64_t)sizeof(GsbSupervisionArgs),
                              (int64_t)sizeof(GsbExtraFeatureArgs), (int64_t)sizeof(GsbFeatureTrainArgs),
-                             (int64_t)sizeof(GsbPoseGradArgs), (int64_t)sizeof(GsbIntrinsicsGradArgs)};
-    for (int i = 0; i < n && i < 10; ++i) out[i] = all[i];
+                             (int64_t)sizeof(GsbPoseGradArgs), (int64_t)sizeof(GsbIntrinsicsGradArgs), (int64_t)sizeof(GsbLensArgs)};
+    for (int i = 0; i < n && i < 11; ++i) out[i] = all[i];
 }
 
 int gsb200_workspace_layout(int64_t num_points, int32_t num_objects, int64_t key_capacity,
@@ -237,7 +237,42 @@ int gsb200_stage_blend(const GsbForwardArgs *a) {
 
 int gsb200_forward(const GsbForwardArgs *a) { return gsb200_forward_ext(a, nullptr); }
 
-int gsb200_forward_ext(const GsbForwardArgs *a, const GsbExtraFeatureArgs *ext) {
+// GsbLensArgs -> LensParams with the r^2 bound; GSB_EINVAL for an unknown model, a non-finite coefficient or a non-zero
+// unused one.  *out_lens stays NULL for a NULL lens or GSB_LENS_PINHOLE (the default kernels).
+static int check_lens(const char *what, const GsbLensArgs *lens, LensParams *params, const LensParams **out_lens) {
+    *out_lens = nullptr;
+    if (!lens) return GSB_OK;
+    if (lens->model != GSB_LENS_PINHOLE && lens->model != GSB_LENS_OPENCV && lens->model != GSB_LENS_FISHEYE) {
+        set_error("%s: unknown lens model %d", what, lens->model);
+        return GSB_EINVAL;
+    }
+    const int used = lens->model == GSB_LENS_OPENCV ? 5 : lens->model == GSB_LENS_FISHEYE ? 4 : 0;
+    for (int i = 0; i < 5; ++i) {
+        const float k = lens->coefficients[i];
+        if (!(k - k == 0.0f)) {
+            set_error("%s: lens coefficient %d is not finite", what, i);
+            return GSB_EINVAL;
+        }
+        if (i >= used && k != 0.0f) {
+            set_error("%s: lens coefficient %d is not used by model %d and must be 0", what, i, lens->model);
+            return GSB_EINVAL;
+        }
+    }
+    if (lens->model == GSB_LENS_PINHOLE) return GSB_OK;
+    params->model = lens->model;
+    for (int i = 0; i < 5; ++i) params->k[i] = lens->coefficients[i];
+    params->r2_max = (float)lens_r2_bound(lens->model, lens->coefficients);
+    *out_lens = params;
+    return GSB_OK;
+}
+
+int gsb200_forward_ext(const GsbForwardArgs *a, const GsbExtraFeatureArgs *ext) { return gsb200_forward_lens(a, ext, nullptr); }
+
+int gsb200_forward_lens(const GsbForwardArgs *a, const GsbExtraFeatureArgs *ext, const GsbLensArgs *lens_args) {
+    LensParams lens_params;
+    const LensParams *lens;
+    int lrc = check_lens("forward_lens", lens_args, &lens_params, &lens);
+    if (lrc != GSB_OK) return lrc;
     if (ext) {
         if (ext->channels < 1 || ext->channels > 16) {
             set_error("forward_ext: channels must be in 1..16 (got %d)", ext->channels);
@@ -256,7 +291,7 @@ int gsb200_forward_ext(const GsbForwardArgs *a, const GsbExtraFeatureArgs *ext) 
     int rc = resolve_fwd(a, &ws);
     if (rc != GSB_OK) return rc;
     cudaStream_t st = static_cast<cudaStream_t>(a->stream);
-    if ((rc = launch_preprocess(*a, ws, st)) != GSB_OK) return rc;
+    if ((rc = launch_preprocess(*a, ws, st, lens)) != GSB_OK) return rc;
     if (a->host_counters && a->host_counters_event) {
         GSB_CUDA_CHECK(cudaMemcpyAsync(a->host_counters, ws.counters, 4 * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
         GSB_CUDA_CHECK(cudaEventRecord(static_cast<cudaEvent_t>(a->host_counters_event), st));
@@ -272,7 +307,7 @@ int gsb200_forward_ext(const GsbForwardArgs *a, const GsbExtraFeatureArgs *ext) 
 static int backward_impl(const GsbBackwardArgs *a, bool skip_on_overflow, const float *grad_depth = nullptr,
                          const float *depth = nullptr, const float *grad_alpha = nullptr,
                          const GsbExtraFeatureArgs *ext = nullptr, const GsbPoseGradArgs *pose = nullptr,
-                         const GsbIntrinsicsGradArgs *intr = nullptr) {
+                         const GsbIntrinsicsGradArgs *intr = nullptr, const LensParams *lens = nullptr) {
     if (!a) {
         set_error("backward: args is null");
         return GSB_EINVAL;
@@ -326,6 +361,7 @@ static int backward_impl(const GsbBackwardArgs *a, bool skip_on_overflow, const 
     if (ext && a->num_points > 0)  // the blend adds into the rows it reaches; every other row stays zero
         GSB_CUDA_CHECK(cudaMemsetAsync(ext->grad_features, 0, (size_t)a->num_points * ext->channels * 4, st));
     if ((rc = launch_blend_backward(*a, ws, st, grad_depth, depth, grad_alpha, ext)) != GSB_OK) return rc;
+    if (lens) return launch_backward_points_lens(*a, ws, st, grad_depth != nullptr, *lens);
     if (intr) return launch_backward_points_calib(*a, ws, st, grad_depth != nullptr, pose, *intr);
     if (pose) return launch_backward_points_pose(*a, ws, st, grad_depth != nullptr, *pose);
     return launch_backward_points(*a, ws, st, skip_on_overflow ? ws.counters + CNT_OVERFLOW : nullptr, grad_depth != nullptr);
@@ -341,6 +377,27 @@ int gsb200_backward_aux(const GsbBackwardArgs *a, const float *grad_rasterized_d
 int gsb200_backward_ext(const GsbBackwardArgs *a, const float *grad_rasterized_depth, const float *rasterized_depth,
                         const float *grad_pixel_accumulated_alpha, const GsbExtraFeatureArgs *ext) {
     return gsb200_backward_pose(a, grad_rasterized_depth, rasterized_depth, grad_pixel_accumulated_alpha, ext, nullptr);
+}
+
+// gsb200_backward_calib's checks and dispatch; `lens` (gsb200_backward_lens, checked there) comes with neither pose nor
+// intrinsics
+static int backward_checked(const GsbBackwardArgs *a, const float *grad_rasterized_depth, const float *rasterized_depth,
+                            const float *grad_pixel_accumulated_alpha, const GsbExtraFeatureArgs *ext, const GsbPoseGradArgs *pose,
+                            const GsbIntrinsicsGradArgs *intr, const LensParams *lens);
+
+int gsb200_backward_lens(const GsbBackwardArgs *a, const float *grad_rasterized_depth, const float *rasterized_depth,
+                         const float *grad_pixel_accumulated_alpha, const GsbExtraFeatureArgs *ext, const GsbLensArgs *lens_args) {
+    LensParams lens_params;
+    const LensParams *lens;
+    int rc = check_lens("backward_lens", lens_args, &lens_params, &lens);
+    if (rc != GSB_OK) return rc;
+    if (!lens) return gsb200_backward_ext(a, grad_rasterized_depth, rasterized_depth, grad_pixel_accumulated_alpha, ext);
+    if (a != nullptr && (a->flags & GSB_FLAG_COMPACT_GRADS)) {
+        set_error("backward_lens: the lens gradient is not implemented for the compact rows of the view-parallel exchange "
+                  "(GSB_FLAG_COMPACT_GRADS)");
+        return GSB_EUNSUPPORTED;
+    }
+    return backward_checked(a, grad_rasterized_depth, rasterized_depth, grad_pixel_accumulated_alpha, ext, nullptr, nullptr, lens);
 }
 
 int64_t gsb200_pose_grad_temp_bytes(int32_t num_objects) {
@@ -359,6 +416,12 @@ int64_t gsb200_intrinsics_grad_temp_bytes(void) {
 int gsb200_backward_calib(const GsbBackwardArgs *a, const float *grad_rasterized_depth, const float *rasterized_depth,
                           const float *grad_pixel_accumulated_alpha, const GsbExtraFeatureArgs *ext, const GsbPoseGradArgs *pose,
                           const GsbIntrinsicsGradArgs *intr) {
+    return backward_checked(a, grad_rasterized_depth, rasterized_depth, grad_pixel_accumulated_alpha, ext, pose, intr, nullptr);
+}
+
+static int backward_checked(const GsbBackwardArgs *a, const float *grad_rasterized_depth, const float *rasterized_depth,
+                            const float *grad_pixel_accumulated_alpha, const GsbExtraFeatureArgs *ext, const GsbPoseGradArgs *pose,
+                            const GsbIntrinsicsGradArgs *intr, const LensParams *lens) {
     if (intr) {
         if (!intr->grad_camera_intrinsics || !intr->temp) {
             set_error("backward_calib: null grad_camera_intrinsics / temp pointer");
@@ -423,7 +486,7 @@ int gsb200_backward_calib(const GsbBackwardArgs *a, const float *grad_rasterized
                   "(GSB_FLAG_BACKWARD_TRANSPOSED); the butterfly kernel does not implement them");
         return GSB_EUNSUPPORTED;
     }
-    return backward_impl(a, false, grad_rasterized_depth, rasterized_depth, grad_pixel_accumulated_alpha, ext, pose, intr);
+    return backward_impl(a, false, grad_rasterized_depth, rasterized_depth, grad_pixel_accumulated_alpha, ext, pose, intr, lens);
 }
 
 int gsb200_backward_with_depth(const GsbBackwardArgs *a, const float *grad_rasterized_depth, const float *rasterized_depth) {

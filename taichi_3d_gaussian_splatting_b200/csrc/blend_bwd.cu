@@ -415,10 +415,14 @@ __device__ __forceinline__ void weighted_u_sigma(const float *U, const float *R,
         B1[c] = g01 * A0 + g11 * A1;
     }
 }
-template <bool COMPACT, bool DEPTH, bool POSE, bool INTR = false>
+// LENS = true (gsb200_backward_lens): the frame was projected through lens_distort (common.cuh), so d uv / d pc = K[:2,:2] D P
+// replaces the pinhole projection Jacobian and J = diag(fx, fy) D P replaces the pinhole J inside Sigma' (D at the point's
+// (xn, yn), detached like J).  Non-compact, without POSE / INTR.
+template <bool COMPACT, bool DEPTH, bool POSE, bool INTR = false, bool LENS = false>
 __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, float *s_pose, float *pose_partials,
                                                      int num_objects, float *s_intr = nullptr,
-                                                     float *intr_partials = nullptr) {
+                                                     float *intr_partials = nullptr, const LensParams lens = LensParams()) {
+    static_assert(!LENS || (!COMPACT && !POSE && !INTR), "the lens gradient is implemented for the dense rows alone");
     // One thread per scene row: rows outside the frustum get their zeros here (no separate memset of the
     // dense (N,3)/(N,56) gradients), rows inside get the chain rule.  A warp owns 32 consecutive rows, i.e. one
     // contiguous 7 KB piece of the (N,56) gradient and 384 B of the (N,3) one: each lane stages its row in
@@ -478,6 +482,20 @@ __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, fl
         const float iz = 1.0f / pcz, iz2 = iz * iz;
         float dj[6] = {Kc[0] * iz, Kc[1] * iz, (-Kc[0] * pcx - Kc[1] * pcy) * iz2,
                        Kc[3] * iz, Kc[4] * iz, (-Kc[3] * pcx - Kc[4] * pcy) * iz2};
+        float Jl[6];  // LENS: diag(fx, fy) D P, the J of Sigma' below
+        if (LENS) {
+            float ox, oy, D[4];  // D = d(xd, yd)/d(xn, yn) at the point
+            if (lens.model == GSB_LENS_FISHEYE) lens_distort<GSB_LENS_FISHEYE>(lens.k, pcx * iz, pcy * iz, ox, oy, D);
+            else lens_distort<GSB_LENS_OPENCV>(lens.k, pcx * iz, pcy * iz, ox, oy, D);
+            // K[:2,:2] D P: the pinhole expression with K[:2,:2] replaced by K[:2,:2] D (exactly K[:2,:2] for D = I)
+            const float A0 = Kc[0] * D[0] + Kc[1] * D[2], A1 = Kc[0] * D[1] + Kc[1] * D[3];
+            const float A3 = Kc[3] * D[0] + Kc[4] * D[2], A4 = Kc[3] * D[1] + Kc[4] * D[3];
+            dj[0] = A0 * iz; dj[1] = A1 * iz; dj[2] = (-A0 * pcx - A1 * pcy) * iz2;
+            dj[3] = A3 * iz; dj[4] = A4 * iz; dj[5] = (-A3 * pcx - A4 * pcy) * iz2;
+            const float F0 = Kc[0] * D[0], F1 = Kc[0] * D[1], F3 = Kc[4] * D[2], F4 = Kc[4] * D[3];  // likewise
+            Jl[0] = F0 * iz; Jl[1] = F1 * iz; Jl[2] = -(F0 * pcx + F1 * pcy) * iz2;
+            Jl[3] = F3 * iz; Jl[4] = F4 * iz; Jl[5] = -(F3 * pcx + F4 * pcy) * iz2;
+        }
         float gx[3];
 #pragma unroll
         for (int c = 0; c < 3; ++c) {
@@ -489,6 +507,10 @@ __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, fl
         // Sigma' = U Sigma U^T, U = J W with J from fx, fy only (GP3D:65-87, 237-331)
         const float fx = Kc[0], fy = Kc[4];
         float J[6] = {fx * iz, 0.0f, -(fx * pcx) * iz2, 0.0f, fy * iz, -(fy * pcy) * iz2};
+        if (LENS) {
+#pragma unroll
+            for (int k = 0; k < 6; ++k) J[k] = Jl[k];
+        }
         float U[6];
 #pragma unroll
         for (int c = 0; c < 3; ++c) {
@@ -717,6 +739,17 @@ __global__ void __launch_bounds__(GSB_POINTS_THREADS, 5)  // + 12 KB of per-warp
 backward_points_pose_kernel(const PointsBwdPoseParams p) {
     __shared__ float s_pose[(GSB_POINTS_THREADS / 32) * GSB_POSE_MAX_OBJECTS * POSE_VALUES];
     backward_points_body<false, DEPTH, true>(p, s_pose, p.pose_partials, p.num_objects);
+}
+
+// The parameter block of the LENS instantiations: the default kernels keep PointsBwdParams as it is.
+struct PointsBwdLensParams : PointsBwdParams {
+    LensParams lens;
+};
+
+template <bool DEPTH>
+__global__ void __launch_bounds__(GSB_POINTS_THREADS, 5)  // at 6 CTAs per SM the lens Jacobians spill 4-8 bytes
+backward_points_lens_kernel(const PointsBwdLensParams p) {
+    backward_points_body<false, DEPTH, false, false, true>(p, nullptr, nullptr, 0, nullptr, nullptr, p.lens);
 }
 
 // R(q) of GP3D:30-48 (xyzw, not normalised) and the gradient of sum_ij G_ij R(q)_ij with respect to q
@@ -974,6 +1007,21 @@ int launch_backward_points(const GsbBackwardArgs &a, const Workspace &ws, cudaSt
     } else {
         backward_points_kernel<false><<<(int)blocks, GSB_POINTS_THREADS, 0, stream>>>(p);
     }
+    GSB_CUDA_CHECK(cudaGetLastError());
+    return GSB_OK;
+}
+
+int launch_backward_points_lens(const GsbBackwardArgs &a, const Workspace &ws, cudaStream_t stream, bool depth_grad,
+                                const LensParams &lens) {
+    if (a.num_points <= 0) return GSB_OK;
+    PointsBwdLensParams p;
+    static_cast<PointsBwdParams &>(p) = make_points_params(a, ws, nullptr);
+    p.lens = lens;
+    long long blocks = (a.num_points + GSB_POINTS_THREADS - 1) / GSB_POINTS_THREADS;
+    const long long cap = 16LL * num_sms();
+    if (blocks > cap) blocks = cap;
+    if (depth_grad) backward_points_lens_kernel<true><<<(int)blocks, GSB_POINTS_THREADS, 0, stream>>>(p);
+    else backward_points_lens_kernel<false><<<(int)blocks, GSB_POINTS_THREADS, 0, stream>>>(p);
     GSB_CUDA_CHECK(cudaGetLastError());
     return GSB_OK;
 }

@@ -62,7 +62,9 @@ int resolve_workspace(void *base, int64_t bytes, int64_t N, int32_t n_obj, int64
                       Workspace *ws);
 
 // ---- stage launchers (each enqueues on `stream`, returns GSB_* code)
-int launch_preprocess(const GsbForwardArgs &a, const Workspace &ws, cudaStream_t stream);
+struct LensParams;
+// lens: the distortion of gsb200_forward_lens (checked there, r2_max set), or NULL for the pinhole kernel
+int launch_preprocess(const GsbForwardArgs &a, const Workspace &ws, cudaStream_t stream, const LensParams *lens = nullptr);
 int launch_sort(const Workspace &ws, int64_t key_capacity, cudaStream_t stream);
 int launch_tile_ranges(const Workspace &ws, int64_t key_capacity, int num_tiles, cudaStream_t stream);
 int launch_tile_ranges_raw(const long long *keys_i64, int64_t n, int *tile_start, int *tile_end,
@@ -79,6 +81,10 @@ int launch_blend_backward(const GsbBackwardArgs &a, const Workspace &ws, cudaStr
                           const float *grad_alpha = nullptr, const GsbExtraFeatureArgs *ext = nullptr);
 int launch_backward_points(const GsbBackwardArgs &a, const Workspace &ws, cudaStream_t stream,
                            const long long *skip_flag = nullptr, bool depth_grad = false);
+// gsb200_backward_lens: the LENS per-point kernel (dense gradients as launch_backward_points, d uv / d pc and J through the
+// lens); arguments checked by the caller
+int launch_backward_points_lens(const GsbBackwardArgs &a, const Workspace &ws, cudaStream_t stream, bool depth_grad,
+                                const LensParams &lens);
 // gsb200_backward_pose: the POSE per-point kernel (dense gradients as launch_backward_points, plus the per-CTA pose sums
 // in pose.temp) and the per-object finishing kernel; arguments checked by the caller
 int launch_backward_points_pose(const GsbBackwardArgs &a, const Workspace &ws, cudaStream_t stream, bool depth_grad,
@@ -254,6 +260,125 @@ __device__ __forceinline__ void fast_planes(const float4 r0, const float4 r1, fl
     s1 = make_float4((-0.5f * GSB_L2E) * r1.x, r1.y * r1.z, 1.0f - r1.z, r1.w);
 }
 #endif
+
+// ---- lens distortion (gsb200_forward_lens / gsb200_backward_lens; definition in include/gsb200.h).  The per-point forward
+// and the per-point backward both call lens_distort, so the position they project to and the Jacobian they differentiate
+// agree by construction.
+struct LensParams {
+    int model;     // GSB_LENS_OPENCV or GSB_LENS_FISHEYE
+    float k[5];    // opencv: k1 k2 p1 p2 k3; fisheye: k1 k2 k3 k4 0
+    float r2_max;  // r^2 bound of the region where the map does not fold back (inf: unbounded), lens_r2_bound
+};
+#if defined(__CUDACC__) || defined(GSB_HOST_EMU)
+// (xn, yn) -> the displacement (ox, oy) = (xd - xn, yd - yn) and D = d(xd, yd)/d(xn, yn), row-major 2x2.  The callers
+// project z (xn + ox, yn + oy, 1) = (x + z ox, y + z oy, z) and form K D, diag(fx, fy) D in the pinhole's expression shapes,
+// so that an opencv lens with all coefficients 0 (ox = oy = 0, D = I exactly) reproduces the pinhole path bit for bit.
+template <int MODEL>
+__device__ __forceinline__ void lens_distort(const float *k, float xn, float yn, float &ox, float &oy, float *D) {
+    const float r2 = xn * xn + yn * yn;
+    if (MODEL == GSB_LENS_OPENCV) {
+        const float k1 = k[0], k2 = k[1], p1 = k[2], p2 = k[3], k3 = k[4];
+        const float rad1 = r2 * (k1 + r2 * (k2 + r2 * k3));  // rad - 1
+        const float rad = 1.0f + rad1;
+        const float drad = k1 + r2 * (2.0f * k2 + r2 * (3.0f * k3));  // d rad / d r^2
+        ox = xn * rad1 + 2.0f * p1 * xn * yn + p2 * (r2 + 2.0f * xn * xn);
+        oy = yn * rad1 + p1 * (r2 + 2.0f * yn * yn) + 2.0f * p2 * xn * yn;
+        const float off = 2.0f * xn * yn * drad + 2.0f * (p1 * xn + p2 * yn);
+        D[0] = rad + 2.0f * xn * xn * drad + 2.0f * p1 * yn + 6.0f * p2 * xn;
+        D[1] = off;
+        D[2] = off;
+        D[3] = rad + 2.0f * yn * yn * drad + 6.0f * p1 * yn + 2.0f * p2 * xn;
+    } else {
+        // s = theta_d / r = A P(theta^2) with A = atan(r) / r, P(t) = 1 + k1 t + k2 t^2 + k3 t^3 + k4 t^4, and
+        // D = s I + g (xn, yn)^T (xn, yn) with g = (ds/dr) / r = (A'/r) P + 2 A^2 P'(theta^2) / (1 + r^2).
+        // A and A'/r are cancellation-free series for small r (both are even in r).
+        float A, Ar;
+        if (r2 < 0.04f) {
+            A = 1.0f + r2 * (-1.0f / 3.0f + r2 * (1.0f / 5.0f + r2 * (-1.0f / 7.0f + r2 * (1.0f / 9.0f + r2 * (-1.0f / 11.0f)))));
+            Ar = -2.0f / 3.0f + r2 * (4.0f / 5.0f + r2 * (-6.0f / 7.0f + r2 * (8.0f / 9.0f + r2 * (-10.0f / 11.0f))));
+        } else {
+            const float r = sqrtf(r2);
+            A = atanf(r) / r;
+            Ar = (1.0f / (1.0f + r2) - A) / r2;
+        }
+        const float t = A * A * r2;  // theta^2
+        const float P = 1.0f + t * (k[0] + t * (k[1] + t * (k[2] + t * k[3])));
+        const float dP = k[0] + t * (2.0f * k[1] + t * (3.0f * k[2] + t * (4.0f * k[3])));
+        const float s = A * P;
+        const float g = Ar * P + 2.0f * A * A * dP / (1.0f + r2);
+        ox = (s - 1.0f) * xn;
+        oy = (s - 1.0f) * yn;
+        D[0] = s + g * xn * xn;
+        D[1] = g * xn * yn;
+        D[2] = D[1];
+        D[3] = s + g * yn * yn;
+    }
+}
+#endif
+
+// Host, double: the r^2 bound of LensParams::r2_max (definition in include/gsb200.h), inf when the map never folds back.
+// The smallest positive root of the derivative polynomial in t = r^2 (opencv) or t = theta^2 (fisheye) is bracketed
+// between the roots of its derivative (recursively, degree <= 4) and bisected.
+static inline double lens_poly(const double *c, int deg, double t) {
+    double v = c[deg];
+    for (int i = deg - 1; i >= 0; --i) v = v * t + c[i];
+    return v;
+}
+// all roots of c[0] + c[1] t + ... + c[deg] t^deg in (lo, hi), ascending; returns their number
+static inline int lens_poly_roots(const double *c, int deg, double lo, double hi, double *out) {
+    while (deg > 0 && c[deg] == 0.0) --deg;
+    if (deg == 0) return 0;
+    double d[4], crit[4];
+    for (int i = 1; i <= deg; ++i) d[i - 1] = i * c[i];
+    const int nc = lens_poly_roots(d, deg - 1, lo, hi, crit);
+    double edges[6];
+    int ne = 0;
+    edges[ne++] = lo;
+    for (int i = 0; i < nc; ++i) edges[ne++] = crit[i];
+    edges[ne++] = hi;
+    int n = 0;
+    for (int i = 0; i + 1 < ne; ++i) {
+        double a = edges[i], b = edges[i + 1];
+        double fa = lens_poly(c, deg, a), fb = lens_poly(c, deg, b);
+        if (i > 0 && fa == 0.0) { out[n++] = a; continue; }  // a double root at a critical point
+        if ((fa < 0.0) == (fb < 0.0) || fb == 0.0) continue;
+        for (int it = 0; it < 200 && b - a > 0.0; ++it) {
+            const double m = 0.5 * (a + b);
+            if (m <= a || m >= b) break;
+            const double fm = lens_poly(c, deg, m);
+            if ((fm < 0.0) == (fa < 0.0)) { a = m; fa = fm; } else { b = m; }
+        }
+        out[n++] = 0.5 * (a + b);
+    }
+    return n;
+}
+static inline double lens_r2_bound(int model, const float *k) {
+    const double inf = __builtin_inf();
+    if (model == GSB_LENS_OPENCV) {
+        const double c[4] = {1.0, 3.0 * k[0], 5.0 * k[1], 7.0 * k[4]};  // d(r rad)/dr in t = r^2
+        double hi = 1.0;  // Cauchy bound of the positive roots
+        for (int i = 3; i >= 1; --i)
+            if (c[i] != 0.0) {
+                double m = 0.0;
+                for (int j = 0; j < i; ++j) m = fmax(m, fabs(c[j] / c[i]));
+                hi = 2.0 * (1.0 + m);
+                break;
+            }
+        double roots[4];
+        return lens_poly_roots(c, 3, 0.0, hi, roots) > 0 ? roots[0] : inf;
+    }
+    if (model == GSB_LENS_FISHEYE) {
+        const double half_pi = 1.5707963267948966;
+        const double c[5] = {1.0, 3.0 * k[0], 5.0 * k[1], 7.0 * k[2], 9.0 * k[3]};  // d theta_d / d theta in t = theta^2
+        double roots[4];
+        double theta = half_pi;
+        if (lens_poly_roots(c, 4, 0.0, half_pi * half_pi, roots) > 0) theta = fmin(theta, sqrt(roots[0]));
+        if (theta >= half_pi) return inf;  // tan(pi/2): every point in front of the camera
+        const double r = tan(theta);
+        return r * r;
+    }
+    return inf;
+}
 
 // ---- mbarrier + TMA 1-D bulk copy (global -> shared), used by the radix sort (key tiles) and the per-point stage (feature rows)
 #if defined(__CUDACC__) || defined(GSB_HOST_EMU)

@@ -188,9 +188,12 @@ __device__ __forceinline__ bool tile_reachable(const SplatReach &r, float u, flo
     return rect_reachable(r, X0, X0 + (float)(GSB_TILE_WIDTH - 1), Y0, Y0 + (float)(GSB_TILE_HEIGHT - 1));
 }
 
-template <typename KeyT>
-__global__ void __launch_bounds__(SCAN_BLOCK_THREADS, GSB_PRE_MIN_BLOCKS)
-preprocess_kernel(const PreParams p) {
+// The body of the per-point kernel.  LENS = GSB_LENS_PINHOLE is the default kernel; GSB_LENS_OPENCV / GSB_LENS_FISHEYE
+// (gsb200_forward_lens) project through lens_distort (common.cuh): the position is (K00 xd + K01 yd + K02, K10 xd + K11 yd +
+// K12), J = diag(fx, fy) D P, and a point with r^2 > lens.r2_max is outside the frustum.  Everything downstream of (u, v) and
+// J -- the record layout, the keys, the scan -- is the same for every model.
+template <typename KeyT, int LENS>
+__device__ __forceinline__ void preprocess_body(const PreParams p, const LensParams lens) {
     __shared__ unsigned int s_ticket;
     __shared__ unsigned long long s_warp_sums[SCAN_BLOCK_THREADS / 32];
     __shared__ unsigned long long s_block_exclusive;
@@ -245,10 +248,27 @@ preprocess_kernel(const PreParams p) {
         pc[0] = ((T[0] * x + T[1] * y) + T[2] * z) + T[3] * 1.0f;
         pc[1] = ((T[4] * x + T[5] * y) + T[6] * z) + T[7] * 1.0f;
         pc[2] = ((T[8] * x + T[9] * y) + T[10] * z) + T[11] * 1.0f;
-        float uv1[3];
-        matmul<3, 3, 1>(Kc, pc, uv1);
-        const float u = uv1[0] / pc[2], v = uv1[1] / pc[2];
-        in = pc[2] > p.near_plane && pc[2] < p.far_plane &&
+        float u, v;
+        float D[4] = {1.0f, 0.0f, 0.0f, 1.0f};  // d(xd, yd)/d(xn, yn)
+        bool lens_ok = true;
+        if (LENS == GSB_LENS_PINHOLE) {
+            float uv1[3];
+            matmul<3, 3, 1>(Kc, pc, uv1);
+            u = uv1[0] / pc[2];
+            v = uv1[1] / pc[2];
+        } else {
+            const float xn = pc[0] / pc[2], yn = pc[1] / pc[2];
+            lens_ok = xn * xn + yn * yn <= lens.r2_max;  // NaN (z = 0) fails as well
+            float ox, oy;
+            lens_distort<LENS>(lens.k, xn, yn, ox, oy, D);
+            // u = K00 xd + K01 yd + K02 as (K z (xd, yd, 1))[0] / z, the pinhole's arithmetic on the displaced point
+            const float pd[3] = {pc[0] + pc[2] * ox, pc[1] + pc[2] * oy, pc[2]};
+            float uv1[3];
+            matmul<3, 3, 1>(Kc, pd, uv1);
+            u = uv1[0] / pc[2];
+            v = uv1[1] / pc[2];
+        }
+        in = lens_ok && pc[2] > p.near_plane && pc[2] < p.far_plane &&
              u >= (float)(-GSB_TILE_WIDTH * GSB_BOUNDARY_TILES) &&
              u < (float)(p.W + GSB_TILE_WIDTH * GSB_BOUNDARY_TILES) &&
              v >= (float)(-GSB_TILE_HEIGHT * GSB_BOUNDARY_TILES) &&
@@ -270,6 +290,12 @@ preprocess_kernel(const PreParams p) {
             const float fx = Kc[0], fy = Kc[4];
             J[0] = fx / pc[2]; J[1] = 0.0f; J[2] = -(fx * pc[0]) / (pc[2] * pc[2]);
             J[3] = 0.0f; J[4] = fy / pc[2]; J[5] = -(fy * pc[1]) / (pc[2] * pc[2]);
+            if (LENS != GSB_LENS_PINHOLE) {  // J = diag(fx, fy) D P, P = [1/z 0 -x/z^2; 0 1/z -y/z^2]
+                J[0] = (fx * D[0]) / pc[2]; J[1] = (fx * D[1]) / pc[2];
+                J[2] = -(fx * (D[0] * pc[0] + D[1] * pc[1])) / (pc[2] * pc[2]);
+                J[3] = (fy * D[2]) / pc[2]; J[4] = (fy * D[3]) / pc[2];
+                J[5] = -(fy * (D[2] * pc[0] + D[3] * pc[1])) / (pc[2] * pc[2]);
+            }
             float R[9], S[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0}, RS[9], RSS[9], RT[9], Sigma[9];
             rotation_from_quaternion(qv.x, qv.y, qv.z, qv.w, R);
             S[0] = exp_cr(f[0]); S[4] = exp_cr(f[1]); S[8] = exp_cr(f[2]);
@@ -547,8 +573,25 @@ preprocess_kernel(const PreParams p) {
     }
 }
 
+template <typename KeyT>
+__global__ void __launch_bounds__(SCAN_BLOCK_THREADS, GSB_PRE_MIN_BLOCKS)
+preprocess_kernel(const PreParams p) {
+    preprocess_body<KeyT, GSB_LENS_PINHOLE>(p, LensParams());
+}
+
+// The parameter block of the lens instantiations: the default kernel keeps PreParams as it is.
+struct PreLensParams : PreParams {
+    LensParams lens;
+};
+
+template <typename KeyT, int LENS>
+__global__ void __launch_bounds__(SCAN_BLOCK_THREADS, GSB_PRE_MIN_BLOCKS)
+preprocess_lens_kernel(const PreLensParams p) {
+    preprocess_body<KeyT, LENS>(p, p.lens);
+}
+
 #ifndef GSB_HOST_EMU  // tests/simt compiles the kernels above as host C++ under the SIMT emulator
-int launch_preprocess(const GsbForwardArgs &a, const Workspace &ws, cudaStream_t stream) {
+int launch_preprocess(const GsbForwardArgs &a, const Workspace &ws, cudaStream_t stream, const LensParams *lens) {
     const GsbWorkspaceLayout &L = ws.layout;
     {
         // per-frame state to zero: [counters, sort_state) and [tile_start, zero_bytes) -- every offset is 256-B aligned
@@ -593,7 +636,21 @@ int launch_preprocess(const GsbForwardArgs &a, const Workspace &ws, cudaStream_t
     p.point_in_camera = ws.point_in_camera;
     p.keys = ws.keys_a;
     p.vals = ws.vals_a;
-    if (L.key_bytes == 4)
+    if (lens != nullptr) {
+        PreLensParams pl;
+        static_cast<PreParams &>(pl) = p;
+        pl.lens = *lens;
+        const bool fisheye = lens->model == GSB_LENS_FISHEYE;
+        if (L.key_bytes == 4) {
+            if (fisheye) preprocess_lens_kernel<unsigned int, GSB_LENS_FISHEYE><<<L.scan_blocks, SCAN_BLOCK_THREADS, 0, stream>>>(pl);
+            else preprocess_lens_kernel<unsigned int, GSB_LENS_OPENCV><<<L.scan_blocks, SCAN_BLOCK_THREADS, 0, stream>>>(pl);
+        } else {
+            if (fisheye)
+                preprocess_lens_kernel<unsigned long long, GSB_LENS_FISHEYE><<<L.scan_blocks, SCAN_BLOCK_THREADS, 0, stream>>>(pl);
+            else
+                preprocess_lens_kernel<unsigned long long, GSB_LENS_OPENCV><<<L.scan_blocks, SCAN_BLOCK_THREADS, 0, stream>>>(pl);
+        }
+    } else if (L.key_bytes == 4)
         preprocess_kernel<unsigned int><<<L.scan_blocks, SCAN_BLOCK_THREADS, 0, stream>>>(p);
     else
         preprocess_kernel<unsigned long long><<<L.scan_blocks, SCAN_BLOCK_THREADS, 0, stream>>>(p);

@@ -19,6 +19,9 @@ neighbour so that a sparse map stays sparse.  Two more optional keys carry targe
 ``labels_path`` (``.npy`` integer (H, W) class ids, read as int32; outside [0, C) = no label) and ``features_path``
 (``.npy`` float32 (H, W, C); NaN = no target), both at the resolution of the image on disk and cropped and autoscaled with
 the image by nearest neighbour.
+An optional record key ``distortion`` (an extension), ``{"model": "opencv" | "fisheye", "coefficients": [...]}``, gives the
+view's ``CameraInfo.distortion`` (``Camera.LensDistortion``).  The coefficients act on the normalised image plane, so
+rescaling, cropping and autoscale leave them unchanged.
 Pinned against the reference class itself: ``tests/golden/make_dataset_golden.py`` imports it (Taichi stubbed) and
 stores its outputs for a small generated dataset; ``tests/test_dataset_cpu.py`` compares.
 """
@@ -30,7 +33,7 @@ import numpy as np
 import torch
 import torch.utils.data
 
-from .Camera import CameraInfo
+from .Camera import CameraInfo, LensDistortion
 from .GaussianPointCloudRasterisation import TILE_HEIGHT, TILE_WIDTH
 from .loss import SupervisionTargets
 from .utils import SE3_to_quaternion_and_translation_torch
@@ -84,7 +87,17 @@ class ImagePoseDataset(torch.utils.data.Dataset):
         K[1, 1] *= sy
         K[1, 2] *= sy
         return resized, CameraInfo(camera_intrinsics=K, camera_height=resized.shape[1], camera_width=resized.shape[2],
-                                   camera_id=camera_info.camera_id)
+                                   camera_id=camera_info.camera_id, distortion=camera_info.distortion)
+
+    @staticmethod
+    def _distortion(rec: dict) -> Optional[LensDistortion]:
+        """The optional record key ``"distortion": {"model": "opencv" | "fisheye", "coefficients": [...]}``."""
+        d = rec.get("distortion")
+        if d is None:
+            return None
+        if not isinstance(d, dict) or "model" not in d or "coefficients" not in d:
+            raise ValueError(f'"distortion" must be {{"model": ..., "coefficients": [...]}}, got {d!r}')
+        return LensDistortion(d["model"], tuple(d["coefficients"]))
 
     def _path(self, path: str) -> str:
         if not os.path.isabs(path) and not os.path.exists(path):
@@ -173,7 +186,7 @@ class ImagePoseDataset(torch.utils.data.Dataset):
             targets = self._load_targets(rec, image.shape[1], image.shape[2])
         image = _crop_to_tiles(image)
         info = CameraInfo(camera_intrinsics=K, camera_height=image.shape[1], camera_width=image.shape[2],
-                          camera_id=rec["camera_id"])
+                          camera_id=rec["camera_id"], distortion=self._distortion(rec))
         image, info = self._autoscale_image_and_camera_info(image, info)
         if self.with_targets:
             return image, q, t, info, self._crop_and_scale_targets(*targets, info)

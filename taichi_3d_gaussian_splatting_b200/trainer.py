@@ -19,6 +19,9 @@ Optional pose refinement (an extension; ``TrainConfig.pose_learning_rate``): the
 first become trainable, differentiated by the operator's ``differentiable_pose`` and stepped by their own Adam.
 Optional intrinsics refinement (an extension; ``TrainConfig.intrinsics_learning_rate``): per camera, a correction of the focal
 lengths and the principal point, differentiated by the operator's ``differentiable_intrinsics`` and stepped by its own Adam.
+Views with lens distortion (an extension; ``CameraInfo.distortion``) train through their lens in the autograd loop; the
+downsampled camera keeps the coefficients (they act on the normalised image plane).  Not with ``fused_step``, pose or
+intrinsics refinement.
 The rasteriser is injected (default: the CUDA operator) so that tests can run the identical loop with the
 CPU oracle behind the same interface and compare PSNR trajectories.
 """
@@ -57,7 +60,9 @@ def downsample_image_and_camera_info(image: torch.Tensor, camera_info: CameraInf
     K[1, 1] /= downsample_factor
     K[0, 2] /= downsample_factor
     K[1, 2] /= downsample_factor
-    return image, CameraInfo(camera_intrinsics=K, camera_height=h, camera_width=w, camera_id=camera_info.camera_id)
+    # the lens coefficients act on the normalised image plane: resizing does not change them
+    return image, CameraInfo(camera_intrinsics=K, camera_height=h, camera_width=w, camera_id=camera_info.camera_id,
+                             distortion=camera_info.distortion)
 
 
 def _nearest(x: torch.Tensor, h: int, w: int, hc: int, wc: int) -> torch.Tensor:
@@ -181,6 +186,12 @@ class GaussianPointCloudTrainer:
         self._intr = config.intrinsics_learning_rate > 0
         if self._intr and fused_step:
             raise ValueError("fused_step does not implement intrinsics refinement (intrinsics_learning_rate > 0)")
+        # a view with lens distortion (CameraInfo.distortion) trains through the autograd loop alone
+        if any(getattr(v[3], "distortion", None) is not None for v in train_views):
+            for name, on in (("fused_step", fused_step), ("pose refinement (pose_learning_rate > 0)", self._pose),
+                             ("intrinsics refinement (intrinsics_learning_rate > 0)", self._intr)):
+                if on:
+                    raise ValueError(f"{name} is not supported with a distorted view (CameraInfo.distortion)")
         # the trainable intrinsics corrections, one per camera_id: (log fx scale, log fy scale, cx / W, cy / H)
         self._intrinsics = {}
         if self._intr:
