@@ -205,7 +205,8 @@ const char *gsb200_last_error(void);
  * foreign-language binding verify its struct mirrors. */
 void gsb200_abi_sizes(int64_t *out3);
 /* ... and of the first n of {GsbWorkspaceLayout, GsbForwardArgs, GsbBackwardArgs, GsbExpandArgs, GsbTrainStepArgs,
- * GsbSupervisionArgs, GsbExtraFeatureArgs, GsbFeatureTrainArgs, GsbPoseGradArgs, GsbIntrinsicsGradArgs, GsbLensArgs} */
+ * GsbSupervisionArgs, GsbExtraFeatureArgs, GsbFeatureTrainArgs, GsbPoseGradArgs, GsbIntrinsicsGradArgs, GsbLensArgs,
+ * GsbLensGradArgs} */
 void gsb200_abi_sizes_ext(int64_t *out, int32_t n);
 
 /* Workspace sizing.  far_plane*depth_to_sort_key_scale fixes the depth-key width; (H/16)*(W/16)
@@ -368,7 +369,7 @@ int gsb200_backward_calib(const GsbBackwardArgs *args, const float *grad_rasteri
  * outside the frustum (no key, point_offset -1, zero gradient).  The near / far / image-border tests apply to the distorted
  * (u, v).  Gradients: d uv / d pc = K[:2,:2] D P exactly; Sigma' uses the lens J; the conventions of the point gradients
  * hold (J's dependence on pc, the SH view direction and rescale detached, the 0.99 clamp straight-through, the validity cut
- * not differentiated).  No gradient with respect to the coefficients. */
+ * not differentiated).  The gradient with respect to the coefficients is opt-in: gsb200_backward_lens_grad below. */
 #define GSB_LENS_PINHOLE 0
 #define GSB_LENS_OPENCV 1
 #define GSB_LENS_FISHEYE 2
@@ -386,6 +387,40 @@ int gsb200_forward_lens(const GsbForwardArgs *args, const GsbExtraFeatureArgs *e
 int gsb200_backward_lens(const GsbBackwardArgs *args, const float *grad_rasterized_depth, const float *rasterized_depth,
                          const float *grad_pixel_accumulated_alpha, const GsbExtraFeatureArgs *ext,
                          const GsbLensArgs *lens);  /* or NULL */
+
+/* Lens-coefficient gradients (an extension).  The forward is gsb200_forward_lens, unchanged; it reads the coefficients in
+ * two places: the position u = K00 xd + K01 yd + K02, v = K10 xd + K11 yd + K12, and D = d(xd, yd)/d(xn, yn) inside
+ * J = diag(fx, fy) D P, Sigma' = (J W) Sigma (J W)^T.  The coefficient gradient is the exact derivative through both, under
+ * the conventions of the point, pose and intrinsics gradients: D is evaluated at the detached point but differentiated with
+ * respect to k; rescale, the radius, tile membership and the SH view direction are detached; the r_max validity cut is not
+ * differentiated (r_max is recomputed from the coefficients of each call); the 0.99 clamp is straight-through.  Per
+ * in-camera point, with guv = dL/duv of its accumulator row and B0, B1 the rows of G (J W) Sigma (so dL/d(J W) = 2 [B0; B1]):
+ *   dL/dk_i += guv^T K[:2,:2] d(xd, yd)/dk_i
+ *   dL/dJ = 2 [B0; B1] W^T,  dL/dD = diag(fx, fy) dL/dJ P^T,  dL/dk_i += <dL/dD, dD/dk_i>
+ * summed over every in-camera point of every object.  d(xd, yd)/dk and dD/dk are closed forms (lens_coefficient_grad in
+ * csrc/common.cuh): opencv d(xd, yd)/dk1 = r^2 (xn, yn), /dk2 = r^4 (xn, yn), /dk3 = r^6 (xn, yn), /dp1 = (2 xn yn,
+ * r^2 + 2 yn^2), /dp2 = (r^2 + 2 xn^2, 2 xn yn); fisheye with t = theta^2 and s = theta_d / r = A P(t): ds/dk_j = A t^j,
+ * dg/dk_j = (A'/r) t^j + 2 A^2 j t^(j-1) / (1 + r^2) for D = s I + g (xn, yn)^T (xn, yn).  No gradient factor is applied;
+ * every loss term that reaches the accumulator rows (image, depth, alpha, features) contributes, and the depth term's direct
+ * dL/dz adds nothing (z does not depend on k).  The sum is deterministic: the per-point kernel runs on
+ * min(ceil(N/128), GSB_LENS_GRAD_PARTIAL_BLOCKS) CTAs, each writes its sums to `temp`, and a second kernel adds them in block
+ * order -- no float atomics. */
+#define GSB_LENS_GRAD_PARTIAL_BLOCKS 2048
+typedef struct GsbLensGradArgs {
+    float *grad_coefficients; /* (5,) out, fully written in GsbLensArgs::coefficients' order; unused slots 0 */
+    void *temp;               /* gsb200_lens_grad_temp_bytes() bytes, 16-byte aligned */
+} GsbLensGradArgs;
+/* GSB_LENS_GRAD_PARTIAL_BLOCKS * 5 floats */
+int64_t gsb200_lens_grad_temp_bytes(void);
+/* gsb200_backward_lens that also writes the coefficient gradient of `lens` to `lens_grad`.  Everything else the call writes
+ * (dense gradients, hook tensors, controller accumulators) is bit-identical to gsb200_backward_lens's.  NULL lens_grad:
+ * exactly gsb200_backward_lens.  With lens_grad, before any CUDA call: the lens checks of gsb200_forward_lens; GSB_EINVAL for a
+ * NULL or pinhole lens, a NULL output or temp pointer, an output that is not 4-byte aligned or a temp that is not 16-byte
+ * aligned; GSB_EUNSUPPORTED for GSB_FLAG_COMPACT_GRADS.  An image-only loss works with either loop-A kernel; the other terms
+ * keep their requirement of GSB_FLAG_BACKWARD_TRANSPOSED. */
+int gsb200_backward_lens_grad(const GsbBackwardArgs *args, const float *grad_rasterized_depth, const float *rasterized_depth,
+                              const float *grad_pixel_accumulated_alpha, const GsbExtraFeatureArgs *ext,
+                              const GsbLensArgs *lens, const GsbLensGradArgs *lens_grad); /* lens_grad or NULL */
 
 int gsb200_expand_view_gradients(const GsbExpandArgs *args);
 

@@ -239,6 +239,7 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
         differentiable_alpha: bool = False,
         differentiable_pose: bool = False,
         differentiable_intrinsics: bool = False,
+        differentiable_distortion: bool = False,
     ):
         """``exact_exp``: blend kernels use ``expf`` instead of ``ex2.approx`` (parity debugging).
         ``force_key64``: sort the reference's 64-bit ``tile << 32 | depth`` keys even when the live
@@ -288,7 +289,16 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
         row 2 gets 0, and no gradient factor is applied (``gsb200_backward_calib``).  It includes every loss term the
         backward takes (image, depth, alpha, features).  With ``differentiable_pose`` both come from one pass of the
         per-point kernel.  An image-only loss works with either backward kernel.  Off, K gets no gradient.  ``ValueError``
-        with ``config.rgb_only`` or a ``gradient_exchange``."""
+        with ``config.rgb_only`` or a ``gradient_exchange``.
+        ``differentiable_distortion``: ``forward`` takes ``lens_coefficients``, the values of ``camera_info.distortion``'s
+        coefficients as an input of the autograd graph, and ``backward`` returns their gradient -- to refine a lens that is
+        roughly known (a pinhole or one-coefficient COLMAP model of a lens that distorts, a generic fisheye profile).  The
+        gradient is exact through the position and through D inside J, with the conventions of the point, pose and
+        intrinsics gradients (D at the detached point, rescale, tile membership and the SH view direction detached, the
+        r_max cut not differentiated); it includes every loss term the backward takes (image, depth, alpha, features), and no
+        gradient factor is applied (``gsb200_backward_lens_grad``).  An image-only loss works with either backward kernel.
+        ``ValueError`` with ``config.rgb_only`` or a ``gradient_exchange``; like every lens, not with
+        ``differentiable_pose`` or ``differentiable_intrinsics``."""
         super().__init__()
         for name, on in (("differentiable_depth", differentiable_depth), ("differentiable_alpha", differentiable_alpha)):
             if on and backward_impl == "butterfly":
@@ -308,6 +318,11 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
         if differentiable_intrinsics and gradient_exchange is not None:
             raise ValueError("differentiable_intrinsics is not supported with a gradient_exchange (view-parallel training)")
         self.differentiable_intrinsics = bool(differentiable_intrinsics)
+        if differentiable_distortion and config.rgb_only:
+            raise ValueError("differentiable_distortion needs the auxiliary outputs: config.rgb_only=True renders none")
+        if differentiable_distortion and gradient_exchange is not None:
+            raise ValueError("differentiable_distortion is not supported with a gradient_exchange (view-parallel training)")
+        self.differentiable_distortion = bool(differentiable_distortion)
         self.config = config
         self.backward_valid_point_hook = backward_valid_point_hook
         self._flags = (_lib.GSB_FLAG_EXACT_EXP if exact_exp else 0) | (_lib.GSB_FLAG_FORCE_KEY64 if force_key64 else 0) | \
@@ -332,12 +347,12 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
             @staticmethod
             def forward(ctx, pointcloud, pointcloud_features, point_invalid_mask, point_object_id,
                         q_pointcloud_camera, t_pointcloud_camera, camera_info, color_max_sh_band, extra_features=None,
-                        camera_intrinsics=None):
+                        camera_intrinsics=None, lens_coefficients=None):
                 # camera_intrinsics (differentiable_intrinsics): camera_info.camera_intrinsics itself, passed again only so
-                # that autograd tracks it
+                # that autograd tracks it; lens_coefficients (differentiable_distortion): the coefficients rendered
                 outs, frame, saved = outer._run_forward(
                     pointcloud, pointcloud_features, point_invalid_mask, point_object_id,
-                    q_pointcloud_camera, t_pointcloud_camera, camera_info, extra_features)
+                    q_pointcloud_camera, t_pointcloud_camera, camera_info, extra_features, lens_coefficients)
                 image, depth, acc_alpha, last_effective, valid_count = outs[:5]
                 ctx.save_for_backward(pointcloud, pointcloud_features, point_object_id,
                                       t_pointcloud_camera, saved["camera_intrinsics"], acc_alpha,
@@ -350,6 +365,9 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                 ctx.color_max_sh_band = color_max_sh_band
                 ctx.has_extra_features = extra_features is not None
                 ctx.intrinsics_input = camera_intrinsics is not None
+                ctx.lens_input = lens_coefficients is not None
+                if ctx.lens_input:
+                    ctx.lens_coefficients_like = (lens_coefficients.shape[0], lens_coefficients.device)
                 if outer.differentiable_depth:
                     ctx.mark_non_differentiable(valid_count)
                 else:
@@ -369,11 +387,12 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                 grad_pointcloud = grad_pointcloud_features = grad_extra_features = grad_q = grad_t = None
                 pose = outer.differentiable_pose and (ctx.needs_input_grad[4] or ctx.needs_input_grad[5])
                 intrinsics = ctx.intrinsics_input and ctx.needs_input_grad[9]
-                grad_K = None
+                lens_grad = ctx.lens_input and ctx.needs_input_grad[10]
+                grad_K = grad_k = None
                 # GPCR:1028; with extra features (or pose / intrinsics gradients) the backward also runs for them alone
                 # (frozen scene)
                 if ctx.needs_input_grad[0] or ctx.needs_input_grad[1] or (ctx.has_extra_features and ctx.needs_input_grad[8]) \
-                        or pose or intrinsics:
+                        or pose or intrinsics or lens_grad:
                     if outer.config.rgb_only:
                         # the reference leaves accumulated alpha / last-effective offsets uninitialised in
                         # this mode (GPCR:478-484), so its backward is undefined; refuse instead
@@ -383,9 +402,14 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                         frame = ctx.frame
                         grad_rasterized_image = torch.zeros((frame.height, frame.width, 3), dtype=torch.float32,
                                                             device=frame.ws.device)
-                    grad_pointcloud, grad_pointcloud_features, grad_extra_features, grad_q, grad_t, grad_K = \
+                    grad_pointcloud, grad_pointcloud_features, grad_extra_features, grad_q, grad_t, grad_K, grad_k = \
                         outer._run_backward(ctx, grad_rasterized_image, grad_rasterized_depth, grad_pixel_accumulated_alpha,
-                                            grad_feature_map, pose, intrinsics)
+                                            grad_feature_map, pose, intrinsics, lens_grad)
+                if ctx.lens_input:  # eleven inputs: the extra features' and K's slots (None with a lens), then the coefficients
+                    return (grad_pointcloud if ctx.needs_input_grad[0] else None,
+                            grad_pointcloud_features if ctx.needs_input_grad[1] else None, None, None, None, None, None, None,
+                            grad_extra_features if ctx.has_extra_features and ctx.needs_input_grad[8] else None, None,
+                            grad_k if lens_grad else None)
                 if ctx.intrinsics_input:  # ten inputs: the extra features' slot (possibly None), then K
                     return (grad_pointcloud if ctx.needs_input_grad[0] else None,
                             grad_pointcloud_features if ctx.needs_input_grad[1] else None, None, None,
@@ -447,10 +471,10 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
             raise ValueError("point_extra_features must be contiguous")
 
     def _run_forward(self, pointcloud, pointcloud_features, point_invalid_mask, point_object_id,
-                     q_pointcloud_camera, t_pointcloud_camera, camera_info, extra_features=None):
+                     q_pointcloud_camera, t_pointcloud_camera, camera_info, extra_features=None, lens_coefficients=None):
         cfg = self.config
         lib = _lib.load()
-        lens = self._lens_args(camera_info)
+        lens = self._lens_args(camera_info, lens_coefficients)
         _require(pointcloud, "point_cloud", torch.float32, (3,))
         _require(pointcloud_features, "point_cloud_features", torch.float32, (56,))
         _require(point_invalid_mask, "point_invalid_mask", torch.int8)
@@ -539,10 +563,16 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
         outs = (image, depth, acc_alpha, last_effective, valid_count) + ((feature_map,) if feature_map is not None else ())
         return outs, frame, {"camera_intrinsics": K, "lens": lens}
 
-    def _lens_args(self, camera_info) -> Optional[_lib.GsbLensArgs]:
+    def _lens_args(self, camera_info, lens_coefficients=None) -> Optional[_lib.GsbLensArgs]:
         """The C lens argument of ``camera_info.distortion`` (None: the pinhole kernels), after the checks of the options
-        a lens does not combine with."""
+        a lens does not combine with; with ``lens_coefficients`` (``differentiable_distortion``) its values replace the
+        record's coefficients (read on the host: free for a CPU tensor, one blocking 20-byte copy for a device tensor)."""
         distortion = getattr(camera_info, "distortion", None)
+        if lens_coefficients is not None:
+            if not self.differentiable_distortion:
+                raise ValueError("lens_coefficients needs differentiable_distortion=True")
+            if distortion is None:
+                raise ValueError("lens_coefficients was given for a camera with no lens (camera_info.distortion is None)")
         if distortion is None:
             return None
         for name, on in (("differentiable_pose", self.differentiable_pose),
@@ -550,14 +580,26 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                          ("a gradient_exchange", self.gradient_exchange is not None)):
             if on:
                 raise ValueError(f"a camera with lens distortion is not supported with {name}")
-        return _lib.lens_args(distortion)
+        if lens_coefficients is None:
+            return _lib.lens_args(distortion)
+        n = len(distortion.coefficients)
+        if not isinstance(lens_coefficients, torch.Tensor):
+            raise ValueError("lens_coefficients must be a torch.Tensor")
+        if tuple(lens_coefficients.shape) != (n,):
+            raise ValueError(f"lens_coefficients must have shape ({n},) for the {distortion.model} lens, got "
+                             f"{tuple(lens_coefficients.shape)}")
+        if lens_coefficients.dtype != torch.float32:
+            raise ValueError(f"lens_coefficients must be float32, got {lens_coefficients.dtype}")
+        values = lens_coefficients.detach().cpu().tolist()
+        return _lib.lens_args(type(distortion)(distortion.model, values))
 
     # ------------------------------------------------------------------ backward plumbing
     def _run_backward(self, ctx, grad_rasterized_image, grad_rasterized_depth=None, grad_pixel_accumulated_alpha=None,
-                      grad_feature_map=None, pose=False, intrinsics=False):
+                      grad_feature_map=None, pose=False, intrinsics=False, lens_grad=False):
         """Returns dL/dxyz, dL/dfeatures, for a call with extra features dL/d of them ((N, C); zeros when the feature map
-        was not used), with ``pose`` dL/dq_pointcloud_camera (K, 4) and dL/dt_pointcloud_camera (K, 3) (else None), and
-        with ``intrinsics`` dL/dcamera_intrinsics (3, 3) (else None)."""
+        was not used), with ``pose`` dL/dq_pointcloud_camera (K, 4) and dL/dt_pointcloud_camera (K, 3) (else None), with
+        ``intrinsics`` dL/dcamera_intrinsics (3, 3) (else None), and with ``lens_grad`` dL/dlens_coefficients on the
+        coefficient tensor's device (else None)."""
         cfg = self.config
         lib = _lib.load()
         saved = ctx.saved_tensors
@@ -623,16 +665,27 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                 C = extra_features.shape[1]
                 grad_extra_features = torch.zeros((N, C), dtype=torch.float32, device=device) if grad_feature_map is None \
                     else torch.empty((N, C), dtype=torch.float32, device=device)
-            grad_q = grad_t = grad_K = None
+            grad_q = grad_t = grad_K = grad_k = None
             if ctx.lens is not None:  # neither pose nor intrinsics gradients (refused in forward)
                 ext = None
                 if extra_features is not None and grad_feature_map is not None:
                     grad_map = _f32(grad_feature_map)
                     ext = _lib.GsbExtraFeatureArgs(channels=extra_features.shape[1], features=_ptr(extra_features),
                                                    grad_rasterized=_ptr(grad_map), grad_features=_ptr(grad_extra_features))
-                _lib.check(lib.gsb200_backward_lens(ctypes.byref(args), _ptr(grad_depth), _ptr(depth), _ptr(grad_alpha),
-                                                    ctypes.byref(ext) if ext is not None else None, ctypes.byref(ctx.lens)),
-                           "gsb200_backward_lens")
+                if lens_grad:
+                    grad_coefficients = torch.empty((5,), dtype=torch.float32, device=device)
+                    lens_temp = torch.empty((int(lib.gsb200_lens_grad_temp_bytes()) // 4,), dtype=torch.float32, device=device)
+                    lens_grad_args = _lib.GsbLensGradArgs(grad_coefficients=_ptr(grad_coefficients), temp=_ptr(lens_temp))
+                    _lib.check(lib.gsb200_backward_lens_grad(
+                        ctypes.byref(args), _ptr(grad_depth), _ptr(depth), _ptr(grad_alpha),
+                        ctypes.byref(ext) if ext is not None else None, ctypes.byref(ctx.lens), ctypes.byref(lens_grad_args)),
+                        "gsb200_backward_lens_grad")
+                    n, k_device = ctx.lens_coefficients_like
+                    grad_k = grad_coefficients[:n].to(k_device)
+                else:
+                    _lib.check(lib.gsb200_backward_lens(ctypes.byref(args), _ptr(grad_depth), _ptr(depth), _ptr(grad_alpha),
+                                                        ctypes.byref(ext) if ext is not None else None, ctypes.byref(ctx.lens)),
+                               "gsb200_backward_lens")
             elif pose or intrinsics:
                 pose_args = intr_args = None
                 if pose:
@@ -716,7 +769,7 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                     point_uv_in_camera=frame.point_uv.contiguous(),
                     point_depth=frame.point_in_camera[:, 2],
                 ))
-        return grad_pointcloud, grad_pointcloud_features, grad_extra_features, grad_q, grad_t, grad_K
+        return grad_pointcloud, grad_pointcloud_features, grad_extra_features, grad_q, grad_t, grad_K, grad_k
 
     def backward_flags(self, frame_flags: int) -> int:
         """Flags of the backward call for a frame rendered with ``frame_flags`` (adds the experimental kernel selection)."""
@@ -728,7 +781,7 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
 
     # ------------------------------------------------------------------ public forward (GPCR:1184-1204)
     def forward(self, input_data: "GaussianPointCloudRasterisation.GaussianPointCloudRasterisationInput",
-                point_extra_features: Optional[torch.Tensor] = None):
+                point_extra_features: Optional[torch.Tensor] = None, lens_coefficients: Optional[torch.Tensor] = None):
         """Returns (image, depth, pixel_valid_point_count), then pixel_accumulated_alpha with ``differentiable_alpha``.
         ``point_extra_features`` (an extension): an (N, C) float32 tensor of per-Gaussian values (1 <= C <= 16; semantic
         logits, instance encodings, distilled features, ...), contiguous, on the scene's device.  The output tuple then
@@ -742,10 +795,24 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
         ``input_data.camera_info.distortion`` (an extension; ``Camera.LensDistortion``): render and differentiate through
         an OpenCV radial-tangential or fisheye lens (``gsb200_forward_lens`` / ``gsb200_backward_lens``; definition in
         ``include/gsb200.h``).  Every output and option above works with a lens, except ``differentiable_pose``,
-        ``differentiable_intrinsics`` and a ``gradient_exchange`` (``ValueError``); the coefficients get no gradient."""
+        ``differentiable_intrinsics`` and a ``gradient_exchange`` (``ValueError``).
+        ``lens_coefficients`` (with ``differentiable_distortion``; an extension): a float32 tensor of the lens model's length
+        (5 for ``opencv``, 4 for ``fisheye``), on any device.  Its values are the coefficients rendered (``camera_info.
+        distortion`` supplies the model), and the backward returns dL/d ``lens_coefficients`` on the tensor's device.  The
+        values are read on the host: free for a CPU tensor, one blocking 20-byte copy for a device tensor.  ``ValueError``
+        for a camera with no lens, a tensor of the wrong length or dtype, or an operator without the option.  None: no
+        coefficient gradient."""
         camera_info = input_data.camera_info
         assert camera_info.camera_width % TILE_WIDTH == 0
         assert camera_info.camera_height % TILE_HEIGHT == 0
+        if lens_coefficients is not None:  # the extra features' and K's slots first (K is refused with a lens)
+            self._lens_args(camera_info, lens_coefficients)  # the argument checks, before any device work
+            if point_extra_features is not None:
+                self._check_extra_features(point_extra_features, input_data.point_cloud)
+            return self._module_function.apply(
+                input_data.point_cloud, input_data.point_cloud_features, input_data.point_invalid_mask,
+                input_data.point_object_id, input_data.q_pointcloud_camera, input_data.t_pointcloud_camera, camera_info,
+                input_data.color_max_sh_band, point_extra_features, None, lens_coefficients)
         if self.differentiable_intrinsics:  # K as a tenth input, after the extra features' slot
             if point_extra_features is not None:
                 self._check_extra_features(point_extra_features, input_data.point_cloud)

@@ -127,6 +127,10 @@ GSB_LENS_OPENCV = 1
 GSB_LENS_FISHEYE = 2
 
 
+class GsbLensGradArgs(ctypes.Structure):
+    _fields_ = [("grad_coefficients", c_vp), ("temp", c_vp)]
+
+
 def lens_args(distortion) -> GsbLensArgs:
     """The C argument of a ``Camera.LensDistortion`` (host floats; unused coefficients 0)."""
     model = {"opencv": GSB_LENS_OPENCV, "fisheye": GSB_LENS_FISHEYE}[distortion.model]
@@ -158,7 +162,7 @@ EXPORTS = (
     "gsb200_backward_aux", "gsb200_supervision_temp_bytes", "gsb200_train_step_aux", "gsb200_forward_ext",
     "gsb200_backward_ext", "gsb200_feature_loss_temp_bytes", "gsb200_train_step_ext", "gsb200_backward_pose",
     "gsb200_pose_grad_temp_bytes", "gsb200_backward_calib", "gsb200_intrinsics_grad_temp_bytes", "gsb200_forward_lens",
-    "gsb200_backward_lens",
+    "gsb200_backward_lens", "gsb200_backward_lens_grad", "gsb200_lens_grad_temp_bytes",
 )
 
 _lib = None
@@ -206,6 +210,12 @@ def load() -> ctypes.CDLL:
     lib.gsb200_backward_lens.argtypes = [ctypes.POINTER(GsbBackwardArgs), c_vp, c_vp, c_vp, ctypes.POINTER(GsbExtraFeatureArgs),
                                          ctypes.POINTER(GsbLensArgs)]
     lib.gsb200_backward_lens.restype = ctypes.c_int
+    lib.gsb200_backward_lens_grad.argtypes = [ctypes.POINTER(GsbBackwardArgs), c_vp, c_vp, c_vp,
+                                              ctypes.POINTER(GsbExtraFeatureArgs), ctypes.POINTER(GsbLensArgs),
+                                              ctypes.POINTER(GsbLensGradArgs)]
+    lib.gsb200_backward_lens_grad.restype = ctypes.c_int
+    lib.gsb200_lens_grad_temp_bytes.argtypes = []
+    lib.gsb200_lens_grad_temp_bytes.restype = c_i64
     lib.gsb200_intrinsics_grad_temp_bytes.argtypes = []
     lib.gsb200_intrinsics_grad_temp_bytes.restype = c_i64
     lib.gsb200_sort_temp_bytes.argtypes = [c_i64, c_i32]
@@ -303,6 +313,11 @@ def load() -> ctypes.CDLL:
     if sizes11[10] != ctypes.sizeof(GsbLensArgs):
         raise RuntimeError(f"libgsb200.so ABI mismatch: sizeof(GsbLensArgs) {sizes11[10]} != ctypes mirror "
                            f"{ctypes.sizeof(GsbLensArgs)}")
+    sizes12 = (c_i64 * 12)()
+    lib.gsb200_abi_sizes_ext(sizes12, 12)
+    if sizes12[11] != ctypes.sizeof(GsbLensGradArgs):
+        raise RuntimeError(f"libgsb200.so ABI mismatch: sizeof(GsbLensGradArgs) {sizes12[11]} != ctypes mirror "
+                           f"{ctypes.sizeof(GsbLensGradArgs)}")
     _lib = lib
     return lib
 

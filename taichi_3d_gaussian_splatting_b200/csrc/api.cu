@@ -192,11 +192,12 @@ void gsb200_abi_sizes(int64_t *out3) {
 }
 
 void gsb200_abi_sizes_ext(int64_t *out, int32_t n) {
-    const int64_t all[11] = {(int64_t)sizeof(GsbWorkspaceLayout), (int64_t)sizeof(GsbForwardArgs), (int64_t)sizeof(GsbBackwardArgs),
+    const int64_t all[12] = {(int64_t)sizeof(GsbWorkspaceLayout), (int64_t)sizeof(GsbForwardArgs), (int64_t)sizeof(GsbBackwardArgs),
                              (int64_t)sizeof(GsbExpandArgs), (int64_t)sizeof(GsbTrainStepArgs), (int64_t)sizeof(GsbSupervisionArgs),
                              (int64_t)sizeof(GsbExtraFeatureArgs), (int64_t)sizeof(GsbFeatureTrainArgs),
-                             (int64_t)sizeof(GsbPoseGradArgs), (int64_t)sizeof(GsbIntrinsicsGradArgs), (int64_t)sizeof(GsbLensArgs)};
-    for (int i = 0; i < n && i < 11; ++i) out[i] = all[i];
+                             (int64_t)sizeof(GsbPoseGradArgs), (int64_t)sizeof(GsbIntrinsicsGradArgs), (int64_t)sizeof(GsbLensArgs),
+                             (int64_t)sizeof(GsbLensGradArgs)};
+    for (int i = 0; i < n && i < 12; ++i) out[i] = all[i];
 }
 
 int gsb200_workspace_layout(int64_t num_points, int32_t num_objects, int64_t key_capacity,
@@ -307,7 +308,8 @@ int gsb200_forward_lens(const GsbForwardArgs *a, const GsbExtraFeatureArgs *ext,
 static int backward_impl(const GsbBackwardArgs *a, bool skip_on_overflow, const float *grad_depth = nullptr,
                          const float *depth = nullptr, const float *grad_alpha = nullptr,
                          const GsbExtraFeatureArgs *ext = nullptr, const GsbPoseGradArgs *pose = nullptr,
-                         const GsbIntrinsicsGradArgs *intr = nullptr, const LensParams *lens = nullptr) {
+                         const GsbIntrinsicsGradArgs *intr = nullptr, const LensParams *lens = nullptr,
+                         const GsbLensGradArgs *lens_grad = nullptr) {
     if (!a) {
         set_error("backward: args is null");
         return GSB_EINVAL;
@@ -361,6 +363,7 @@ static int backward_impl(const GsbBackwardArgs *a, bool skip_on_overflow, const 
     if (ext && a->num_points > 0)  // the blend adds into the rows it reaches; every other row stays zero
         GSB_CUDA_CHECK(cudaMemsetAsync(ext->grad_features, 0, (size_t)a->num_points * ext->channels * 4, st));
     if ((rc = launch_blend_backward(*a, ws, st, grad_depth, depth, grad_alpha, ext)) != GSB_OK) return rc;
+    if (lens && lens_grad) return launch_backward_points_lens_grad(*a, ws, st, grad_depth != nullptr, *lens, *lens_grad);
     if (lens) return launch_backward_points_lens(*a, ws, st, grad_depth != nullptr, *lens);
     if (intr) return launch_backward_points_calib(*a, ws, st, grad_depth != nullptr, pose, *intr);
     if (pose) return launch_backward_points_pose(*a, ws, st, grad_depth != nullptr, *pose);
@@ -380,10 +383,10 @@ int gsb200_backward_ext(const GsbBackwardArgs *a, const float *grad_rasterized_d
 }
 
 // gsb200_backward_calib's checks and dispatch; `lens` (gsb200_backward_lens, checked there) comes with neither pose nor
-// intrinsics
+// intrinsics, and `lens_grad` (gsb200_backward_lens_grad, checked there) only with `lens`
 static int backward_checked(const GsbBackwardArgs *a, const float *grad_rasterized_depth, const float *rasterized_depth,
                             const float *grad_pixel_accumulated_alpha, const GsbExtraFeatureArgs *ext, const GsbPoseGradArgs *pose,
-                            const GsbIntrinsicsGradArgs *intr, const LensParams *lens);
+                            const GsbIntrinsicsGradArgs *intr, const LensParams *lens, const GsbLensGradArgs *lens_grad = nullptr);
 
 int gsb200_backward_lens(const GsbBackwardArgs *a, const float *grad_rasterized_depth, const float *rasterized_depth,
                          const float *grad_pixel_accumulated_alpha, const GsbExtraFeatureArgs *ext, const GsbLensArgs *lens_args) {
@@ -398,6 +401,44 @@ int gsb200_backward_lens(const GsbBackwardArgs *a, const float *grad_rasterized_
         return GSB_EUNSUPPORTED;
     }
     return backward_checked(a, grad_rasterized_depth, rasterized_depth, grad_pixel_accumulated_alpha, ext, nullptr, nullptr, lens);
+}
+
+int64_t gsb200_lens_grad_temp_bytes(void) {
+    return (int64_t)GSB_LENS_GRAD_PARTIAL_BLOCKS * 5 * (int64_t)sizeof(float);
+}
+
+int gsb200_backward_lens_grad(const GsbBackwardArgs *a, const float *grad_rasterized_depth, const float *rasterized_depth,
+                              const float *grad_pixel_accumulated_alpha, const GsbExtraFeatureArgs *ext,
+                              const GsbLensArgs *lens_args, const GsbLensGradArgs *lens_grad) {
+    if (!lens_grad) return gsb200_backward_lens(a, grad_rasterized_depth, rasterized_depth, grad_pixel_accumulated_alpha, ext, lens_args);
+    LensParams lens_params;
+    const LensParams *lens;
+    int rc = check_lens("backward_lens_grad", lens_args, &lens_params, &lens);
+    if (rc != GSB_OK) return rc;
+    if (!lens) {
+        set_error("backward_lens_grad: the coefficient gradient needs an opencv or fisheye lens (got %s)",
+                  lens_args ? "GSB_LENS_PINHOLE" : "NULL");
+        return GSB_EINVAL;
+    }
+    if (!lens_grad->grad_coefficients || !lens_grad->temp) {
+        set_error("backward_lens_grad: null grad_coefficients / temp pointer");
+        return GSB_EINVAL;
+    }
+    if (reinterpret_cast<uintptr_t>(lens_grad->grad_coefficients) % 4 != 0) {
+        set_error("backward_lens_grad: grad_coefficients must be 4-byte aligned");
+        return GSB_EINVAL;
+    }
+    if (reinterpret_cast<uintptr_t>(lens_grad->temp) % 16 != 0) {
+        set_error("backward_lens_grad: the lens temp must be 16-byte aligned");
+        return GSB_EINVAL;
+    }
+    if (a != nullptr && (a->flags & GSB_FLAG_COMPACT_GRADS)) {
+        set_error("backward_lens_grad: the lens gradient is not implemented for the compact rows of the view-parallel exchange "
+                  "(GSB_FLAG_COMPACT_GRADS)");
+        return GSB_EUNSUPPORTED;
+    }
+    return backward_checked(a, grad_rasterized_depth, rasterized_depth, grad_pixel_accumulated_alpha, ext, nullptr, nullptr, lens,
+                            lens_grad);
 }
 
 int64_t gsb200_pose_grad_temp_bytes(int32_t num_objects) {
@@ -421,7 +462,7 @@ int gsb200_backward_calib(const GsbBackwardArgs *a, const float *grad_rasterized
 
 static int backward_checked(const GsbBackwardArgs *a, const float *grad_rasterized_depth, const float *rasterized_depth,
                             const float *grad_pixel_accumulated_alpha, const GsbExtraFeatureArgs *ext, const GsbPoseGradArgs *pose,
-                            const GsbIntrinsicsGradArgs *intr, const LensParams *lens) {
+                            const GsbIntrinsicsGradArgs *intr, const LensParams *lens, const GsbLensGradArgs *lens_grad) {
     if (intr) {
         if (!intr->grad_camera_intrinsics || !intr->temp) {
             set_error("backward_calib: null grad_camera_intrinsics / temp pointer");
@@ -486,7 +527,8 @@ static int backward_checked(const GsbBackwardArgs *a, const float *grad_rasteriz
                   "(GSB_FLAG_BACKWARD_TRANSPOSED); the butterfly kernel does not implement them");
         return GSB_EUNSUPPORTED;
     }
-    return backward_impl(a, false, grad_rasterized_depth, rasterized_depth, grad_pixel_accumulated_alpha, ext, pose, intr, lens);
+    return backward_impl(a, false, grad_rasterized_depth, rasterized_depth, grad_pixel_accumulated_alpha, ext, pose, intr, lens,
+                         lens_grad);
 }
 
 int gsb200_backward_with_depth(const GsbBackwardArgs *a, const float *grad_rasterized_depth, const float *rasterized_depth) {

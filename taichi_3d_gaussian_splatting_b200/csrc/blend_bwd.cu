@@ -418,11 +418,18 @@ __device__ __forceinline__ void weighted_u_sigma(const float *U, const float *R,
 // LENS = true (gsb200_backward_lens): the frame was projected through lens_distort (common.cuh), so d uv / d pc = K[:2,:2] D P
 // replaces the pinhole projection Jacobian and J = diag(fx, fy) D P replaces the pinhole J inside Sigma' (D at the point's
 // (xn, yn), detached like J).  Non-compact, without POSE / INTR.
-template <bool COMPACT, bool DEPTH, bool POSE, bool INTR = false, bool LENS = false>
+// LGRAD = true (gsb200_backward_lens_grad, with LENS): each in-camera point also forms its 5 coefficient values
+// (lens_coefficient_grad, common.cuh), which the warp sums (fixed butterfly order, all objects together: a frame has one lens)
+// into the per-warp row s_lgrad[warp][5]; after the loop the CTA adds its warps' rows in warp order into
+// lgrad_partials[blockIdx.x][5], and lens_grad_finish_kernel adds the blocks in block order.
+constexpr int LENS_GRAD_VALUES = 5;
+template <bool COMPACT, bool DEPTH, bool POSE, bool INTR = false, bool LENS = false, bool LGRAD = false>
 __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, float *s_pose, float *pose_partials,
                                                      int num_objects, float *s_intr = nullptr,
-                                                     float *intr_partials = nullptr, const LensParams lens = LensParams()) {
+                                                     float *intr_partials = nullptr, const LensParams lens = LensParams(),
+                                                     float *s_lgrad = nullptr, float *lgrad_partials = nullptr) {
     static_assert(!LENS || (!COMPACT && !POSE && !INTR), "the lens gradient is implemented for the dense rows alone");
+    static_assert(!LGRAD || LENS, "the coefficient gradient needs the lens path");
     // One thread per scene row: rows outside the frustum get their zeros here (no separate memset of the
     // dense (N,3)/(N,56) gradients), rows inside get the chain rule.  A warp owns 32 consecutive rows, i.e. one
     // contiguous 7 KB piece of the (N,56) gradient and 384 B of the (N,3) one: each lane stages its row in
@@ -444,6 +451,11 @@ __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, fl
         if (lane < INTR_VALUES) my_intr[lane] = 0.0f;
         __syncwarp();
     }
+    float *const my_lgrad = LGRAD ? s_lgrad + warp * LENS_GRAD_VALUES : nullptr;
+    if (LGRAD) {
+        if (lane < LENS_GRAD_VALUES) my_lgrad[lane] = 0.0f;
+        __syncwarp();
+    }
     const long long stride = (long long)gridDim.x * blockDim.x;
     for (long long base = (long long)blockIdx.x * blockDim.x + warp * 32; base < p.N; base += stride) {
       const long long id = base + lane;
@@ -454,6 +466,11 @@ __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, fl
       if (INTR) {
 #pragma unroll
           for (int k = 0; k < INTR_VALUES; ++k) iv[k] = 0.0f;
+      }
+      float lv[LGRAD ? LENS_GRAD_VALUES : 1];  // zero for rows outside the frustum
+      if (LGRAD) {
+#pragma unroll
+          for (int k = 0; k < LENS_GRAD_VALUES; ++k) lv[k] = 0.0f;
       }
       if (o < 0) {
           if (!COMPACT) { my_xyz[0] = 0.0f; my_xyz[1] = 0.0f; my_xyz[2] = 0.0f; }
@@ -601,6 +618,24 @@ __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, fl
             iv[4] = a0.y * uy + 2.0f * sy1;
             iv[5] = a0.y;
         }
+        if (LGRAD) {
+            // position: dL/d(xd, yd) = K[:2,:2]^T guv.  Sigma' through J = diag(fx, fy) D P (pc detached, D differentiated in k
+            // alone): dL/dJ = 2 [B0; B1] W^T, dL/dD = diag(fx, fy) dL/dJ P^T
+            float B0[3], B1[3];
+            weighted_u_sigma(U, R, es, g00, g01, g11, B0, B1);
+            float h0[3], h1[3];  // [B0; B1] W^T
+#pragma unroll
+            for (int j = 0; j < 3; ++j) {
+                h0[j] = B0[0] * Wm[3 * j] + B0[1] * Wm[3 * j + 1] + B0[2] * Wm[3 * j + 2];
+                h1[j] = B1[0] * Wm[3 * j] + B1[1] * Wm[3 * j + 1] + B1[2] * Wm[3 * j + 2];
+            }
+            const float gxd = Kc[0] * a0.x + Kc[3] * a0.y, gyd = Kc[1] * a0.x + Kc[4] * a0.y;
+            const float w00 = 2.0f * fx * (h0[0] * iz - (h0[2] * pcx) * iz2), w01 = 2.0f * fx * (h0[1] * iz - (h0[2] * pcy) * iz2);
+            const float w10 = 2.0f * fy * (h1[0] * iz - (h1[2] * pcx) * iz2), w11 = 2.0f * fy * (h1[1] * iz - (h1[2] * pcy) * iz2);
+            if (lens.model == GSB_LENS_FISHEYE)
+                lens_coefficient_grad<GSB_LENS_FISHEYE>(pcx * iz, pcy * iz, gxd, gyd, w00, w01 + w10, w11, lv);
+            else lens_coefficient_grad<GSB_LENS_OPENCV>(pcx * iz, pcy * iz, gxd, gyd, w00, w01 + w10, w11, lv);
+        }
         if (p.ctl_num_in_camera != nullptr && !(p.skip_flag != nullptr && *p.skip_flag != 0)) {
             // GaussianPointAdaptiveController.update (:130-143) for this in-camera point: ids are unique, one thread per row,
             // so plain read-modify-writes.  a2.y = sum |d/duv| over pixels, a2.z = number of affected pixels (exact in f32)
@@ -670,6 +705,15 @@ __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, fl
               if (lane == 0) my_intr[k] += v;
           }
       }
+      if (LGRAD) {
+#pragma unroll
+          for (int k = 0; k < LENS_GRAD_VALUES; ++k) {
+              float v = lv[k];
+#pragma unroll
+              for (int d = 16; d > 0; d >>= 1) v += __shfl_xor_sync(0xffffffffu, v, d);
+              if (lane == 0) my_lgrad[k] += v;
+          }
+      }
       __syncwarp();
       const long long rows = p.N - base < 32 ? p.N - base : 32;
       if (COMPACT) {
@@ -720,6 +764,14 @@ __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, fl
             intr_partials[(size_t)blockIdx.x * INTR_VALUES + threadIdx.x] = s;
         }
     }
+    if (LGRAD) {
+        __syncthreads();
+        if (threadIdx.x < LENS_GRAD_VALUES) {
+            float s = s_lgrad[threadIdx.x];
+            for (int w = 1; w < GSB_POINTS_THREADS / 32; ++w) s += s_lgrad[w * LENS_GRAD_VALUES + threadIdx.x];
+            lgrad_partials[(size_t)blockIdx.x * LENS_GRAD_VALUES + threadIdx.x] = s;
+        }
+    }
 }
 
 template <bool COMPACT, bool DEPTH = false>
@@ -750,6 +802,45 @@ template <bool DEPTH>
 __global__ void __launch_bounds__(GSB_POINTS_THREADS, 5)  // at 6 CTAs per SM the lens Jacobians spill 4-8 bytes
 backward_points_lens_kernel(const PointsBwdLensParams p) {
     backward_points_body<false, DEPTH, false, false, true>(p, nullptr, nullptr, 0, nullptr, nullptr, p.lens);
+}
+
+// The parameter block of the LGRAD instantiations.
+struct PointsBwdLensGradParams : PointsBwdLensParams {
+    float *lens_partials;  // (grid, 5)
+};
+
+template <bool DEPTH>
+__global__ void __launch_bounds__(GSB_POINTS_THREADS, 4)  // 5 values live across the SH epilogue: at 5 CTAs per SM it spills
+backward_points_lens_grad_kernel(const PointsBwdLensGradParams p) {
+    __shared__ float s_lgrad[(GSB_POINTS_THREADS / 32) * LENS_GRAD_VALUES];
+    backward_points_body<false, DEPTH, false, false, true, true>(p, nullptr, nullptr, 0, nullptr, nullptr, p.lens, s_lgrad,
+                                                                 p.lens_partials);
+}
+
+// One CTA: adds the `blocks` partial rows in a fixed order (strided per thread, then a fixed shared-memory tree) and writes
+// the 5 coefficient gradients (the unused fifth of a fisheye lens is a sum of zeros).  Zeros when blocks == 0.
+constexpr int LENS_GRAD_FINISH_THREADS = 128;
+__global__ void __launch_bounds__(LENS_GRAD_FINISH_THREADS)
+lens_grad_finish_kernel(const float *__restrict__ partials, int blocks, float *__restrict__ grad_coefficients) {
+    __shared__ float s_sum[LENS_GRAD_FINISH_THREADS][LENS_GRAD_VALUES + 1];
+    const int tid = threadIdx.x;
+    float acc[LENS_GRAD_VALUES];
+#pragma unroll
+    for (int k = 0; k < LENS_GRAD_VALUES; ++k) acc[k] = 0.0f;
+    for (int b = tid; b < blocks; b += LENS_GRAD_FINISH_THREADS) {
+#pragma unroll
+        for (int k = 0; k < LENS_GRAD_VALUES; ++k) acc[k] += partials[(size_t)b * LENS_GRAD_VALUES + k];
+    }
+#pragma unroll
+    for (int k = 0; k < LENS_GRAD_VALUES; ++k) s_sum[tid][k] = acc[k];
+    __syncthreads();
+    for (int h = LENS_GRAD_FINISH_THREADS / 2; h > 0; h >>= 1) {
+        if (tid < h)
+#pragma unroll
+            for (int k = 0; k < LENS_GRAD_VALUES; ++k) s_sum[tid][k] += s_sum[tid + h][k];
+        __syncthreads();
+    }
+    if (tid < LENS_GRAD_VALUES) grad_coefficients[tid] = s_sum[0][tid];
 }
 
 // R(q) of GP3D:30-48 (xyzw, not normalised) and the gradient of sum_ij G_ij R(q)_ij with respect to q
@@ -1022,6 +1113,28 @@ int launch_backward_points_lens(const GsbBackwardArgs &a, const Workspace &ws, c
     if (blocks > cap) blocks = cap;
     if (depth_grad) backward_points_lens_kernel<true><<<(int)blocks, GSB_POINTS_THREADS, 0, stream>>>(p);
     else backward_points_lens_kernel<false><<<(int)blocks, GSB_POINTS_THREADS, 0, stream>>>(p);
+    GSB_CUDA_CHECK(cudaGetLastError());
+    return GSB_OK;
+}
+
+// The LGRAD per-point kernel on a grid that depends on N alone (at most GSB_LENS_GRAD_PARTIAL_BLOCKS CTAs), so the
+// summation order of the coefficient gradient is the same on every device, then lens_grad_finish_kernel.  The caller checked
+// `lens_grad`.
+int launch_backward_points_lens_grad(const GsbBackwardArgs &a, const Workspace &ws, cudaStream_t stream, bool depth_grad,
+                                     const LensParams &lens, const GsbLensGradArgs &lens_grad) {
+    PointsBwdLensGradParams p;
+    static_cast<PointsBwdParams &>(p) = make_points_params(a, ws, nullptr);
+    p.lens = lens;
+    p.lens_partials = static_cast<float *>(lens_grad.temp);
+    long long blocks = a.num_points > 0 ? (a.num_points + GSB_POINTS_THREADS - 1) / GSB_POINTS_THREADS : 0;
+    if (blocks > GSB_LENS_GRAD_PARTIAL_BLOCKS) blocks = GSB_LENS_GRAD_PARTIAL_BLOCKS;
+    if (blocks > 0) {
+        if (depth_grad) backward_points_lens_grad_kernel<true><<<(int)blocks, GSB_POINTS_THREADS, 0, stream>>>(p);
+        else backward_points_lens_grad_kernel<false><<<(int)blocks, GSB_POINTS_THREADS, 0, stream>>>(p);
+        GSB_CUDA_CHECK(cudaGetLastError());
+    }
+    lens_grad_finish_kernel<<<1, LENS_GRAD_FINISH_THREADS, 0, stream>>>(p.lens_partials, (int)blocks,
+                                                                         lens_grad.grad_coefficients);
     GSB_CUDA_CHECK(cudaGetLastError());
     return GSB_OK;
 }

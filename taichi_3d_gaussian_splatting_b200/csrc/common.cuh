@@ -85,6 +85,10 @@ int launch_backward_points(const GsbBackwardArgs &a, const Workspace &ws, cudaSt
 // lens); arguments checked by the caller
 int launch_backward_points_lens(const GsbBackwardArgs &a, const Workspace &ws, cudaStream_t stream, bool depth_grad,
                                 const LensParams &lens);
+// gsb200_backward_lens_grad: the LENS per-point kernel that also sums the coefficient gradient (per-CTA rows in
+// lens_grad.temp), and the finishing kernel; arguments checked by the caller
+int launch_backward_points_lens_grad(const GsbBackwardArgs &a, const Workspace &ws, cudaStream_t stream, bool depth_grad,
+                                     const LensParams &lens, const GsbLensGradArgs &lens_grad);
 // gsb200_backward_pose: the POSE per-point kernel (dense gradients as launch_backward_points, plus the per-CTA pose sums
 // in pose.temp) and the per-object finishing kernel; arguments checked by the caller
 int launch_backward_points_pose(const GsbBackwardArgs &a, const Workspace &ws, cudaStream_t stream, bool depth_grad,
@@ -312,6 +316,51 @@ __device__ __forceinline__ void lens_distort(const float *k, float xn, float yn,
         D[1] = g * xn * yn;
         D[2] = D[1];
         D[3] = s + g * yn * yn;
+    }
+}
+// The coefficient gradient of lens_distort at (xn, yn) (gsb200_backward_lens_grad): given gx, gy = dL/d(xd, yd) and
+// w00, w01, w11 = dL/dD[0][0], dL/dD[0][1] + dL/dD[1][0], dL/dD[1][1] (D is symmetric in both models), writes
+// out[i] = gx dxd/dk_i + gy dyd/dk_i + <dL/dD, dD/dk_i> in LensParams::k's order (fisheye: out[4] = 0).  Both maps are linear
+// in the coefficients, so the columns d(xd, yd)/dk and dD/dk are closed forms in (xn, yn) alone:
+//   opencv, k_m = k1 k2 k3 (m = 1 2 3): d(xd, yd) = r^2m (xn, yn), dD = r^2m I + 2m r^2(m-1) (xn, yn)^T (xn, yn);
+//     p1: d(xd, yd) = (2 xn yn, r^2 + 2 yn^2), dD = [2 yn, 2 xn; 2 xn, 6 yn];  p2: (r^2 + 2 xn^2, 2 xn yn), [6 xn, 2 yn; 2 yn, 2 xn]
+//   fisheye, t = theta^2 (j = 1..4): ds/dk_j = A t^j, dg/dk_j = (A'/r) t^j + 2 A^2 j t^(j-1) / (1 + r^2), and with
+//     (xd, yd) = s (xn, yn), D = s I + g (xn, yn)^T (xn, yn): d(xd, yd) = ds (xn, yn), dD = ds I + dg (xn, yn)^T (xn, yn).
+// A and A'/r are lens_distort's (the same series below r^2 = 0.04).
+template <int MODEL>
+__device__ __forceinline__ void lens_coefficient_grad(float xn, float yn, float gx, float gy, float w00, float w01, float w11,
+                                                      float *out) {
+    const float r2 = xn * xn + yn * yn;
+    const float pos = gx * xn + gy * yn;                               // (gx, gy) . (xn, yn)
+    const float tr = w00 + w11;                                        // <dL/dD, I>
+    const float quad = w00 * xn * xn + w01 * xn * yn + w11 * yn * yn;  // <dL/dD, (xn, yn)^T (xn, yn)>
+    if (MODEL == GSB_LENS_OPENCV) {
+        const float r4 = r2 * r2;
+        out[0] = r2 * (pos + tr) + 2.0f * quad;
+        out[1] = r4 * (pos + tr) + 4.0f * r2 * quad;
+        out[2] = gx * (2.0f * xn * yn) + gy * (r2 + 2.0f * yn * yn) + 2.0f * w00 * yn + 2.0f * w01 * xn + 6.0f * w11 * yn;
+        out[3] = gx * (r2 + 2.0f * xn * xn) + gy * (2.0f * xn * yn) + 6.0f * w00 * xn + 2.0f * w01 * yn + 2.0f * w11 * xn;
+        out[4] = r4 * r2 * (pos + tr) + 6.0f * r4 * quad;
+    } else {
+        float A, Ar;
+        if (r2 < 0.04f) {
+            A = 1.0f + r2 * (-1.0f / 3.0f + r2 * (1.0f / 5.0f + r2 * (-1.0f / 7.0f + r2 * (1.0f / 9.0f + r2 * (-1.0f / 11.0f)))));
+            Ar = -2.0f / 3.0f + r2 * (4.0f / 5.0f + r2 * (-6.0f / 7.0f + r2 * (8.0f / 9.0f + r2 * (-10.0f / 11.0f))));
+        } else {
+            const float r = sqrtf(r2);
+            A = atanf(r) / r;
+            Ar = (1.0f / (1.0f + r2) - A) / r2;
+        }
+        const float t = A * A * r2;  // theta^2
+        const float c = 2.0f * A * A / (1.0f + r2);
+        float tj1 = 1.0f;  // t^(j-1)
+#pragma unroll
+        for (int j = 1; j <= 4; ++j) {
+            const float tj = tj1 * t;
+            out[j - 1] = A * tj * (pos + tr) + (Ar * tj + c * (float)j * tj1) * quad;
+            tj1 = tj;
+        }
+        out[4] = 0.0f;
     }
 }
 #endif

@@ -22,6 +22,8 @@ lengths and the principal point, differentiated by the operator's ``differentiab
 Views with lens distortion (an extension; ``CameraInfo.distortion``) train through their lens in the autograd loop; the
 downsampled camera keeps the coefficients (they act on the normalised image plane).  Not with ``fused_step``, pose or
 intrinsics refinement.
+Optional lens refinement (an extension; ``TrainConfig.distortion_learning_rate``): per camera with a lens, its coefficients,
+differentiated by the operator's ``differentiable_distortion`` and stepped by their own Adam.
 The rasteriser is injected (default: the CUDA operator) so that tests can run the identical loop with the
 CPU oracle behind the same interface and compare PSNR trajectories.
 """
@@ -32,7 +34,7 @@ from typing import Callable, List, Optional, Tuple
 import torch
 import torch.nn.functional as F
 
-from .Camera import CameraInfo
+from .Camera import CameraInfo, LensDistortion
 from .densification import GaussianPointAdaptiveController
 from .GaussianPointCloudRasterisation import GaussianPointCloudRasterisation
 from .loss import FEATURE_LOSSES, LossFunction, SupervisionTargets, feature_loss, supervision_loss
@@ -142,6 +144,11 @@ class GaussianPointCloudTrainer:
         # of the view's full-resolution width and height.  Skew and K[1,0] are not trained.  Combines with
         # pose_learning_rate.  Not with fused_step.
         intrinsics_learning_rate: float = 0.
+        # optional lens refinement: > 0 gives every camera_id whose training views have a lens (CameraInfo.distortion) one
+        # leaf tensor of its coefficients (5 for opencv, 4 for fisheye), initialised from the views' lens, kept on the host
+        # and trained by its own Adam at this rate.  The views of one camera_id must share their lens.  Not with fused_step,
+        # pose or intrinsics refinement (no distorted view combines with them).
+        distortion_learning_rate: float = 0.
 
     def __init__(self, config: "GaussianPointCloudTrainer.TrainConfig", scene: Scene, train_views: List[View],
                  rasterisation_factory: Optional[Callable] = None, generator: Optional[torch.Generator] = None,
@@ -200,6 +207,8 @@ class GaussianPointCloudTrainer:
                 if ci.camera_id not in self._intrinsics:
                     self._intrinsics[ci.camera_id] = torch.zeros(4, dtype=torch.float32, device=ci.camera_intrinsics.device,
                                                                  requires_grad=True)
+        self._distortion = self._distortion_leaves(config, train_views)
+        self._dist = config.distortion_learning_rate > 0
         self._features = config.feature_loss != "none"
         if self._features:
             self._check_feature_config(config, scene, targets)
@@ -232,7 +241,8 @@ class GaussianPointCloudTrainer:
         extra = dict(**({"differentiable_depth": True} if self._need_depth else {}),
                      **({"differentiable_alpha": True} if self._need_alpha else {}),
                      **({"differentiable_pose": True} if self._pose else {}),
-                     **({"differentiable_intrinsics": True} if self._intr else {}))
+                     **({"differentiable_intrinsics": True} if self._intr else {}),
+                     **({"differentiable_distortion": True} if self._dist else {}))
         self.rasterisation = factory(config=config.rasterisation_config,
                                      backward_valid_point_hook=self.adaptive_controller.update, **extra)
         self.loss_function = LossFunction(config=config.loss_function_config)
@@ -240,6 +250,27 @@ class GaussianPointCloudTrainer:
         self._downsampled = {}
         self._view_generator = shuffle_generator
         self._view_order = None
+
+    @staticmethod
+    def _distortion_leaves(config, train_views: List[View]) -> dict:
+        """The trainable lens coefficients, one float32 host leaf per camera_id with a lens ({} when lens refinement is off)."""
+        rate = config.distortion_learning_rate
+        if not (rate >= 0.0 and rate < float("inf")):
+            raise ValueError(f"distortion_learning_rate must be finite and >= 0, got {rate}")
+        if rate == 0:
+            return {}
+        lenses = {}
+        for v in train_views:
+            ci = v[3]
+            lenses.setdefault(ci.camera_id, set()).add(getattr(ci, "distortion", None))
+        for cid, found in lenses.items():
+            if len(found) > 1:
+                raise ValueError(f"the training views of camera_id {cid} have different lenses: {sorted(map(str, found))}")
+        leaves = {cid: torch.tensor(lens.coefficients, dtype=torch.float32, requires_grad=True)
+                  for cid, (lens,) in lenses.items() if lens is not None}
+        if not leaves:
+            raise ValueError("distortion_learning_rate > 0 needs a distorted training view (CameraInfo.distortion)")
+        return leaves
 
     @staticmethod
     def _check_feature_config(config, scene: Scene, targets: List[SupervisionTargets]) -> None:
@@ -397,6 +428,9 @@ class GaussianPointCloudTrainer:
                               betas=(0.9, 0.999)) if self._pose and len(self._poses) > 1 else None
         intrinsics_optimizer = Adam(list(self._intrinsics.values()), lr=cfg.intrinsics_learning_rate,
                                     betas=(0.9, 0.999)) if self._intr else None
+        # host tensors: torch's Adam whatever fused_adam says
+        distortion_optimizer = torch.optim.Adam(list(self._distortion.values()), lr=cfg.distortion_learning_rate,
+                                                betas=(0.9, 0.999)) if self._dist else None
         scheduler = torch.optim.lr_scheduler.ExponentialLR(position_optimizer, gamma=cfg.position_learning_rate_decay_rate)
         downsample_factor = cfg.initial_downsample_factor
         for iteration in range(cfg.num_iterations):
@@ -410,24 +444,34 @@ class GaussianPointCloudTrainer:
                 pose_optimizer.zero_grad()
             if intrinsics_optimizer is not None:
                 intrinsics_optimizer.zero_grad()
+            if distortion_optimizer is not None:
+                distortion_optimizer.zero_grad()
             view_index = self._next_view_index(iteration)
             image_gt, q, t, camera_info, targets = self._view(view_index, downsample_factor)
             if self._intr:  # built every iteration: the cached downsampled camera must not freeze K
                 camera_info = CameraInfo(camera_intrinsics=self._intrinsics_of(view_index, downsample_factor),
                                          camera_height=camera_info.camera_height, camera_width=camera_info.camera_width,
                                          camera_id=camera_info.camera_id)
+            lens_kw = {}
+            if self._dist and camera_info.distortion is not None:  # the lens as trained, the leaf as the autograd input
+                leaf = self._distortion[camera_info.camera_id]
+                camera_info = CameraInfo(camera_intrinsics=camera_info.camera_intrinsics,
+                                         camera_height=camera_info.camera_height, camera_width=camera_info.camera_width,
+                                         camera_id=camera_info.camera_id,
+                                         distortion=LensDistortion(camera_info.distortion.model, leaf.detach().tolist()))
+                lens_kw = {"lens_coefficients": leaf}
             band = iteration // cfg.increase_color_max_sh_band_interval
             if self.supervised or self._features:
                 loss, l1_loss, mask_term, depth_term, feature_term, image_pred = self._supervised_loss(
-                    q, t, camera_info, band, image_gt, targets)
+                    q, t, camera_info, band, image_gt, targets, lens_kw)
             elif self.fused_image_loss:
-                image_pred, _, _ = self.rasterisation(self._input(q, t, camera_info, band))
+                image_pred, _, _ = self.rasterisation(self._input(q, t, camera_info, band), **lens_kw)
                 loss, l1_loss, ssim_loss = self.loss_function.forward_rasterized(
                     image_pred, image_gt, point_invalid_mask=self.scene.point_invalid_mask,
                     pointcloud_features=self.scene.point_cloud_features)
                 image_pred = image_pred.detach().clamp(0, 1).permute(2, 0, 1) if log_interval else image_pred
             else:
-                image_pred, _, _ = self.rasterisation(self._input(q, t, camera_info, band))
+                image_pred, _, _ = self.rasterisation(self._input(q, t, camera_info, band), **lens_kw)
                 image_pred = torch.clamp(image_pred, min=0, max=1).permute(2, 0, 1)
                 loss, l1_loss, ssim_loss = self.loss_function(
                     image_pred, image_gt, point_invalid_mask=self.scene.point_invalid_mask,
@@ -444,6 +488,8 @@ class GaussianPointCloudTrainer:
                         q_v.div_(q_v.norm(dim=-1, keepdim=True))
             if intrinsics_optimizer is not None:
                 intrinsics_optimizer.step()
+            if distortion_optimizer is not None:
+                distortion_optimizer.step()
             if iteration % cfg.position_learning_rate_decay_interval == 0:
                 scheduler.step()
             self.adaptive_controller.refinement()
@@ -458,16 +504,19 @@ class GaussianPointCloudTrainer:
                 self.history.append(entry)
         return self.history
 
-    def _supervised_loss(self, q, t, camera_info, band, image_gt, targets):
+    def _supervised_loss(self, q, t, camera_info, band, image_gt, targets, lens_kw=None):
         """Forward with the differentiable outputs the terms need, then ``loss.supervision_loss`` with this trainer's image
         loss (the torch one, or the fused kernels with ``fused_image_loss``; the scale regulariser if enabled), plus
         ``loss.feature_loss`` on the rendered feature map with a feature loss.  Returns (total, L1, mask term, depth term,
-        feature term, the raw image as (3, H, W) for the PSNR log)."""
+        feature term, the raw image as (3, H, W) for the PSNR log).  ``lens_kw``: the operator's ``lens_coefficients``
+        argument with lens refinement."""
         cfg = self.config
+        lens_kw = lens_kw or {}
         if self._features:
-            outs = self.rasterisation(self._input(q, t, camera_info, band), point_extra_features=self.scene.point_extra_features)
+            outs = self.rasterisation(self._input(q, t, camera_info, band), point_extra_features=self.scene.point_extra_features,
+                                      **lens_kw)
         else:
-            outs = self.rasterisation(self._input(q, t, camera_info, band))
+            outs = self.rasterisation(self._input(q, t, camera_info, band), **lens_kw)
         image_pred, depth = outs[0], outs[1]
         alpha = outs[3] if self._need_alpha else None
         regulariser = dict(point_invalid_mask=self.scene.point_invalid_mask, pointcloud_features=self.scene.point_cloud_features)
@@ -496,6 +545,18 @@ class GaussianPointCloudTrainer:
             return [v[3].camera_intrinsics.detach().clone() for v in self.train_views]
         with torch.no_grad():
             return [self._intrinsics_of(i, 1).clone() for i in range(len(self.train_views))]
+
+    def refined_distortion(self) -> List[Optional[LensDistortion]]:
+        """The lens of every training view as trained (None for a view without one; the views' own lenses without lens
+        refinement)."""
+        out = []
+        for v in self.train_views:
+            ci = v[3]
+            lens = getattr(ci, "distortion", None)
+            if lens is not None and ci.camera_id in self._distortion:
+                lens = LensDistortion(lens.model, self._distortion[ci.camera_id].detach().tolist())
+            out.append(lens)
+        return out
 
     @torch.no_grad()
     def validation(self, views: Optional[List[View]] = None) -> float:
