@@ -206,7 +206,7 @@ const char *gsb200_last_error(void);
 void gsb200_abi_sizes(int64_t *out3);
 /* ... and of the first n of {GsbWorkspaceLayout, GsbForwardArgs, GsbBackwardArgs, GsbExpandArgs, GsbTrainStepArgs,
  * GsbSupervisionArgs, GsbExtraFeatureArgs, GsbFeatureTrainArgs, GsbPoseGradArgs, GsbIntrinsicsGradArgs, GsbLensArgs,
- * GsbLensGradArgs} */
+ * GsbLensGradArgs, GsbRollingShutterArgs, GsbRollingShutterGradArgs} */
 void gsb200_abi_sizes_ext(int64_t *out, int32_t n);
 
 /* Workspace sizing.  far_plane*depth_to_sort_key_scale fixes the depth-key width; (H/16)*(W/16)
@@ -421,6 +421,55 @@ int64_t gsb200_lens_grad_temp_bytes(void);
 int gsb200_backward_lens_grad(const GsbBackwardArgs *args, const float *grad_rasterized_depth, const float *rasterized_depth,
                               const float *grad_pixel_accumulated_alpha, const GsbExtraFeatureArgs *ext,
                               const GsbLensArgs *lens, const GsbLensGradArgs *lens_grad); /* lens_grad or NULL */
+
+/* Rolling shutter (an extension: the reference projects every point with one global-shutter pose).  A view carries a motion
+ * m = (v, w) (float32 x 6): the apparent motion of the scene in the camera frame over one full readout, top row to bottom
+ * row; v in scene units, w in radians.  The view's pose (q, t) is the pose at mid-readout.  With pc0 = W xyz + tw the camera-
+ * frame point of today and the row time tau in [-1/2, 1/2] (0 at the centre row):
+ *   pc(tau) = Rd(tau) pc0 + tau v,   Rd(tau) = exp(tau [w]x)   (Rodrigues; a series below |tau w|^2 = 0.01, so w = 0 is I)
+ *   row(p) = clamp(v_pix(p) / H - 1/2, -1/2, 1/2)   (v_pix: the row coordinate of p, through the lens if there is one;
+ *                                                    a NaN row clamps to -1/2)
+ *   tau_0 = 0,  tau_(k+1) = row(pc(tau_k)),  k < GSB_RS_ITERATIONS;  the point is rendered at pc(tau_3).
+ * Everything downstream uses pc(tau_3) and W_eff = Rd(tau_3) W: the near / far / border tests, the lens r_max test, (u, v),
+ * the depth and sort key, J and Sigma' = J W_eff Sigma W_eff^T J^T.  The SH view direction keeps the mid-readout camera centre.
+ * With m = 0, Rd = I and tau v = 0 exactly, so the rolling-shutter calls reproduce the global-shutter calls bit for bit.
+ * Gradients: tau is detached (like J, rescale and the SH direction); the point gradients flow through W_eff and pc(tau), and
+ * the per-point backward reads tau back from `row_time` instead of solving for it again.  The motion gradient (opt-in,
+ * GsbRollingShutterGradArgs), with gp = dL/dpc and [B0; B1] the rows of G (J W_eff) Sigma:
+ *   dL/dv = sum_i tau_i gp_i
+ *   dL/dRd_i = gp_i pc0_i^T + 2 J^T [B0; B1] W^T   (the full 2x3 J: with a lens it is not sparse)
+ *   dL/dw = sum_i tau_i J_r(tau_i w)^T a(Rd_i^T dL/dRd_i),  a(A) = (A32 - A23, A13 - A31, A21 - A12)
+ * summed over every in-camera point of every object (rolling_shutter_grad in csrc/common.cuh).  Every loss term that reaches
+ * the accumulator rows contributes (image, depth with its direct dL/dz, alpha, features).  The sum is deterministic: the
+ * per-point kernel runs on min(ceil(N/128), GSB_RS_GRAD_PARTIAL_BLOCKS) CTAs, each writes its sums to `temp`, and a second
+ * kernel adds them in block order -- no float atomics. */
+#define GSB_RS_ITERATIONS 3
+#define GSB_RS_GRAD_PARTIAL_BLOCKS 2048
+typedef struct GsbRollingShutterArgs {
+    float motion[6];  /* v (3), w (3) */
+    float *row_time;  /* (N,) float32, 4-byte aligned: written by the forward (tau_3 in camera, 0 outside the frustum), read
+                       * by the backward of the same frame */
+} GsbRollingShutterArgs;
+typedef struct GsbRollingShutterGradArgs {
+    float *grad_motion; /* (6,) out, dL/dv then dL/dw */
+    void *temp;         /* gsb200_rolling_shutter_grad_temp_bytes() bytes, 16-byte aligned */
+} GsbRollingShutterGradArgs;
+/* GSB_RS_GRAD_PARTIAL_BLOCKS * 6 floats */
+int64_t gsb200_rolling_shutter_grad_temp_bytes(void);
+/* gsb200_forward_lens through the rolling shutter of `rs`.  NULL rs: exactly gsb200_forward_lens.  Before any CUDA call: the
+ * lens checks of gsb200_forward_lens; GSB_EINVAL for a non-finite motion or a NULL or misaligned row_time. */
+int gsb200_forward_rolling_shutter(const GsbForwardArgs *args, const GsbExtraFeatureArgs *ext, const GsbLensArgs *lens,
+                                   const GsbRollingShutterArgs *rs);  /* lens, rs or NULL */
+/* gsb200_backward_lens of a frame rendered by gsb200_forward_rolling_shutter with the same lens and rs.  NULL rs: exactly
+ * gsb200_backward_lens.  NULL rs_grad: no motion gradient; every other output is bit-identical to the call with rs_grad.
+ * Before any CUDA call: the checks of gsb200_forward_rolling_shutter; GSB_EINVAL for an rs_grad without rs, a NULL output or
+ * temp pointer, an output that is not 4-byte aligned or a temp that is not 16-byte aligned; GSB_EUNSUPPORTED for
+ * GSB_FLAG_COMPACT_GRADS.  An image-only loss works with either loop-A kernel; the other terms keep their requirement of
+ * GSB_FLAG_BACKWARD_TRANSPOSED. */
+int gsb200_backward_rolling_shutter(const GsbBackwardArgs *args, const float *grad_rasterized_depth,
+                                    const float *rasterized_depth, const float *grad_pixel_accumulated_alpha,
+                                    const GsbExtraFeatureArgs *ext, const GsbLensArgs *lens, const GsbRollingShutterArgs *rs,
+                                    const GsbRollingShutterGradArgs *rs_grad);  /* lens, rs, rs_grad or NULL */
 
 int gsb200_expand_view_gradients(const GsbExpandArgs *args);
 

@@ -3,7 +3,8 @@
 Mirrors the reference's ``taichi_3d_gaussian_splatting/Camera.py:7-21`` (``CameraInfo`` is an
 argument of ``GaussianPointCloudRasterisationInput``; ``CameraView`` is imported beside it at
 GaussianPointCloudRasterisation.py:4).  ``LensDistortion`` and ``CameraInfo.distortion`` are an extension: the reference
-projects through a pinhole only.
+projects through a pinhole only.  ``RollingShutter`` and ``CameraInfo.rolling_shutter`` are an extension as well: the reference
+projects every row with one global-shutter pose.
 """
 import math
 from dataclasses import dataclass
@@ -64,6 +65,41 @@ class LensDistortion:
         return K, None
 
 
+@dataclass(frozen=True)
+class RollingShutter:
+    """The motion of a rolling-shutter view (definition in ``include/gsb200.h``), as host floats: ``linear`` = v (scene
+    units) and ``angular`` = w (radians), the apparent motion of the scene in the camera frame over one full readout, top row
+    to bottom row.  The view's pose is the pose at mid-readout.  Row time is normalised by the image height, so resizing or
+    cropping an image keeps the motion."""
+    linear: Tuple[float, float, float]
+    angular: Tuple[float, float, float]
+
+    def __post_init__(self):
+        for name in ("linear", "angular"):
+            v = tuple(float(x) for x in getattr(self, name))
+            if len(v) != 3:
+                raise ValueError(f"rolling-shutter {name} motion takes 3 values, got {len(v)}")
+            if not all(math.isfinite(x) for x in v):
+                raise ValueError(f"rolling-shutter {name} motion must be finite, got {v}")
+            object.__setattr__(self, name, v)
+
+    @staticmethod
+    def from_camera_velocity(linear_velocity: Sequence[float], angular_velocity: Sequence[float],
+                             readout_time: float) -> "RollingShutter":
+        """The motion of a camera moving at ``linear_velocity`` (scene units/s) and ``angular_velocity`` (rad/s), both in
+        the camera's own frame (what visual-inertial odometry and ARKit report), read out top to bottom in ``readout_time``
+        seconds: a static scene moves the other way in the camera frame, v = -T u and w = -T w_c."""
+        T = float(readout_time)
+        if not (math.isfinite(T) and T >= 0.0):
+            raise ValueError(f"readout_time must be finite and >= 0, got {readout_time}")
+        return RollingShutter(tuple(-T * float(x) for x in linear_velocity), tuple(-T * float(x) for x in angular_velocity))
+
+    @property
+    def motion(self) -> Tuple[float, ...]:
+        """(v, w) as six floats, the order of ``GsbRollingShutterArgs::motion``."""
+        return self.linear + self.angular
+
+
 @dataclass
 class CameraInfo:
     camera_intrinsics: torch.Tensor  # 3x3 f32 pinhole matrix (device tensor in the reference)
@@ -71,6 +107,7 @@ class CameraInfo:
     camera_width: int
     camera_id: int
     distortion: Optional[LensDistortion] = None  # extension: None is the reference's pinhole
+    rolling_shutter: Optional[RollingShutter] = None  # extension: None is the reference's global shutter
 
 
 @dataclass

@@ -20,6 +20,7 @@ Defined where the reference leaves memory uninitialised: an empty frame (no spla
 renders zeros, and with ``rgb_only=True`` the auxiliary outputs are zeros.
 """
 import ctypes
+import math
 import os
 import threading
 from dataclasses import dataclass
@@ -240,6 +241,7 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
         differentiable_pose: bool = False,
         differentiable_intrinsics: bool = False,
         differentiable_distortion: bool = False,
+        differentiable_rolling_shutter: bool = False,
     ):
         """``exact_exp``: blend kernels use ``expf`` instead of ``ex2.approx`` (parity debugging).
         ``force_key64``: sort the reference's 64-bit ``tile << 32 | depth`` keys even when the live
@@ -298,7 +300,14 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
         r_max cut not differentiated); it includes every loss term the backward takes (image, depth, alpha, features), and no
         gradient factor is applied (``gsb200_backward_lens_grad``).  An image-only loss works with either backward kernel.
         ``ValueError`` with ``config.rgb_only`` or a ``gradient_exchange``; like every lens, not with
-        ``differentiable_pose`` or ``differentiable_intrinsics``."""
+        ``differentiable_pose`` or ``differentiable_intrinsics``.
+        ``differentiable_rolling_shutter``: ``forward`` takes ``rolling_shutter_motion``, the values of
+        ``camera_info.rolling_shutter``'s motion (v, w) as an input of the autograd graph, and ``backward`` returns their
+        gradient -- to refine the camera motion of a phone, action-camera or drone view whose velocity is roughly known or
+        unknown.  The row time is detached; the gradient flows through pc(tau) and Rd(tau) W (``gsb200_backward_rolling_shutter``,
+        definition in ``include/gsb200.h``) and includes every loss term the backward takes (image, depth, alpha, features).
+        An image-only loss works with either backward kernel.  ``ValueError`` with ``config.rgb_only`` or a
+        ``gradient_exchange``."""
         super().__init__()
         for name, on in (("differentiable_depth", differentiable_depth), ("differentiable_alpha", differentiable_alpha)):
             if on and backward_impl == "butterfly":
@@ -323,6 +332,11 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
         if differentiable_distortion and gradient_exchange is not None:
             raise ValueError("differentiable_distortion is not supported with a gradient_exchange (view-parallel training)")
         self.differentiable_distortion = bool(differentiable_distortion)
+        if differentiable_rolling_shutter and config.rgb_only:
+            raise ValueError("differentiable_rolling_shutter needs the auxiliary outputs: config.rgb_only=True renders none")
+        if differentiable_rolling_shutter and gradient_exchange is not None:
+            raise ValueError("differentiable_rolling_shutter is not supported with a gradient_exchange (view-parallel training)")
+        self.differentiable_rolling_shutter = bool(differentiable_rolling_shutter)
         self.config = config
         self.backward_valid_point_hook = backward_valid_point_hook
         self._flags = (_lib.GSB_FLAG_EXACT_EXP if exact_exp else 0) | (_lib.GSB_FLAG_FORCE_KEY64 if force_key64 else 0) | \
@@ -347,12 +361,14 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
             @staticmethod
             def forward(ctx, pointcloud, pointcloud_features, point_invalid_mask, point_object_id,
                         q_pointcloud_camera, t_pointcloud_camera, camera_info, color_max_sh_band, extra_features=None,
-                        camera_intrinsics=None, lens_coefficients=None):
+                        camera_intrinsics=None, lens_coefficients=None, rolling_shutter_motion=None):
                 # camera_intrinsics (differentiable_intrinsics): camera_info.camera_intrinsics itself, passed again only so
-                # that autograd tracks it; lens_coefficients (differentiable_distortion): the coefficients rendered
+                # that autograd tracks it; lens_coefficients (differentiable_distortion): the coefficients rendered;
+                # rolling_shutter_motion (differentiable_rolling_shutter): the motion rendered
                 outs, frame, saved = outer._run_forward(
                     pointcloud, pointcloud_features, point_invalid_mask, point_object_id,
-                    q_pointcloud_camera, t_pointcloud_camera, camera_info, extra_features, lens_coefficients)
+                    q_pointcloud_camera, t_pointcloud_camera, camera_info, extra_features, lens_coefficients,
+                    rolling_shutter_motion)
                 image, depth, acc_alpha, last_effective, valid_count = outs[:5]
                 ctx.save_for_backward(pointcloud, pointcloud_features, point_object_id,
                                       t_pointcloud_camera, saved["camera_intrinsics"], acc_alpha,
@@ -361,6 +377,10 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                                       *((extra_features,) if extra_features is not None else ()))
                 ctx.frame = frame
                 ctx.lens = saved["lens"]
+                ctx.rolling_shutter = saved["rolling_shutter"]  # (GsbRollingShutterArgs, the row times it points at) or None
+                ctx.motion_input = rolling_shutter_motion is not None
+                if ctx.motion_input:
+                    ctx.motion_device = rolling_shutter_motion.device
                 ctx.num_objects = q_pointcloud_camera.shape[0]
                 ctx.color_max_sh_band = color_max_sh_band
                 ctx.has_extra_features = extra_features is not None
@@ -388,11 +408,12 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                 pose = outer.differentiable_pose and (ctx.needs_input_grad[4] or ctx.needs_input_grad[5])
                 intrinsics = ctx.intrinsics_input and ctx.needs_input_grad[9]
                 lens_grad = ctx.lens_input and ctx.needs_input_grad[10]
-                grad_K = grad_k = None
+                motion_grad = ctx.motion_input and ctx.needs_input_grad[11]
+                grad_K = grad_k = grad_m = None
                 # GPCR:1028; with extra features (or pose / intrinsics gradients) the backward also runs for them alone
                 # (frozen scene)
                 if ctx.needs_input_grad[0] or ctx.needs_input_grad[1] or (ctx.has_extra_features and ctx.needs_input_grad[8]) \
-                        or pose or intrinsics or lens_grad:
+                        or pose or intrinsics or lens_grad or motion_grad:
                     if outer.config.rgb_only:
                         # the reference leaves accumulated alpha / last-effective offsets uninitialised in
                         # this mode (GPCR:478-484), so its backward is undefined; refuse instead
@@ -402,9 +423,14 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                         frame = ctx.frame
                         grad_rasterized_image = torch.zeros((frame.height, frame.width, 3), dtype=torch.float32,
                                                             device=frame.ws.device)
-                    grad_pointcloud, grad_pointcloud_features, grad_extra_features, grad_q, grad_t, grad_K, grad_k = \
+                    grad_pointcloud, grad_pointcloud_features, grad_extra_features, grad_q, grad_t, grad_K, grad_k, grad_m = \
                         outer._run_backward(ctx, grad_rasterized_image, grad_rasterized_depth, grad_pixel_accumulated_alpha,
-                                            grad_feature_map, pose, intrinsics, lens_grad)
+                                            grad_feature_map, pose, intrinsics, lens_grad, motion_grad)
+                if ctx.motion_input:  # twelve inputs: the extra features', K's and the coefficients' slots (None), then m
+                    return (grad_pointcloud if ctx.needs_input_grad[0] else None,
+                            grad_pointcloud_features if ctx.needs_input_grad[1] else None, None, None, None, None, None, None,
+                            grad_extra_features if ctx.has_extra_features and ctx.needs_input_grad[8] else None, None, None,
+                            grad_m if motion_grad else None)
                 if ctx.lens_input:  # eleven inputs: the extra features' and K's slots (None with a lens), then the coefficients
                     return (grad_pointcloud if ctx.needs_input_grad[0] else None,
                             grad_pointcloud_features if ctx.needs_input_grad[1] else None, None, None, None, None, None, None,
@@ -471,10 +497,12 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
             raise ValueError("point_extra_features must be contiguous")
 
     def _run_forward(self, pointcloud, pointcloud_features, point_invalid_mask, point_object_id,
-                     q_pointcloud_camera, t_pointcloud_camera, camera_info, extra_features=None, lens_coefficients=None):
+                     q_pointcloud_camera, t_pointcloud_camera, camera_info, extra_features=None, lens_coefficients=None,
+                     rolling_shutter_motion=None):
         cfg = self.config
         lib = _lib.load()
         lens = self._lens_args(camera_info, lens_coefficients)
+        rs = self._rolling_shutter_args(camera_info, rolling_shutter_motion)
         _require(pointcloud, "point_cloud", torch.float32, (3,))
         _require(pointcloud_features, "point_cloud_features", torch.float32, (56,))
         _require(point_invalid_mask, "point_invalid_mask", torch.int8)
@@ -515,6 +543,10 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                 C = extra_features.shape[1]
                 feature_map = torch.empty((H, W, C), dtype=torch.float32, device=device)
                 ext = _lib.GsbExtraFeatureArgs(channels=C, features=_ptr(extra_features), rasterized=_ptr(feature_map))
+            row_time = None
+            if rs is not None:  # tau_3 of every scene row, read back by the backward of this frame
+                row_time = torch.empty((max(N, 1),), dtype=torch.float32, device=device)
+                rs.row_time = _ptr(row_time)
             readback = _PinnedCounters.acquire(device)
             pinned, event = readback
             retry_flag = 0
@@ -538,7 +570,12 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                         host_counters=pinned.data_ptr(), host_counters_event=event.cuda_event)
                     # The whole frame is enqueued by this one call; the library copies {M, K, overflow} to pinned
                     # host memory right after the per-point stage and records `event` behind that copy.
-                    if lens is not None:
+                    if rs is not None:
+                        _lib.check(lib.gsb200_forward_rolling_shutter(
+                            ctypes.byref(args), ctypes.byref(ext) if ext is not None else None,
+                            ctypes.byref(lens) if lens is not None else None, ctypes.byref(rs)),
+                            "gsb200_forward_rolling_shutter")
+                    elif lens is not None:
                         _lib.check(lib.gsb200_forward_lens(ctypes.byref(args), ctypes.byref(ext) if ext is not None else None,
                                                            ctypes.byref(lens)), "gsb200_forward_lens")
                     elif ext is None:
@@ -561,7 +598,8 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                 _PinnedCounters.release(device, readback)
         self.last_frame = frame
         outs = (image, depth, acc_alpha, last_effective, valid_count) + ((feature_map,) if feature_map is not None else ())
-        return outs, frame, {"camera_intrinsics": K, "lens": lens}
+        return outs, frame, {"camera_intrinsics": K, "lens": lens,
+                             "rolling_shutter": (rs, row_time) if rs is not None else None}
 
     def _lens_args(self, camera_info, lens_coefficients=None) -> Optional[_lib.GsbLensArgs]:
         """The C lens argument of ``camera_info.distortion`` (None: the pinhole kernels), after the checks of the options
@@ -593,13 +631,47 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
         values = lens_coefficients.detach().cpu().tolist()
         return _lib.lens_args(type(distortion)(distortion.model, values))
 
+    def _rolling_shutter_args(self, camera_info, motion=None) -> Optional[_lib.GsbRollingShutterArgs]:
+        """The C rolling-shutter argument of ``camera_info.rolling_shutter`` (None: the global-shutter kernels; row_time is
+        set by the caller), after the checks of the options a rolling shutter does not combine with; with ``motion``
+        (``differentiable_rolling_shutter``) its values replace the record's (read on the host: free for a CPU tensor, one
+        blocking 24-byte copy for a device tensor)."""
+        rolling_shutter = getattr(camera_info, "rolling_shutter", None)
+        if motion is not None:
+            if not self.differentiable_rolling_shutter:
+                raise ValueError("rolling_shutter_motion needs differentiable_rolling_shutter=True")
+            if rolling_shutter is None:
+                raise ValueError("rolling_shutter_motion was given for a camera without a rolling shutter "
+                                 "(camera_info.rolling_shutter is None)")
+        if rolling_shutter is None:
+            return None
+        for name, on in (("differentiable_pose", self.differentiable_pose),
+                         ("differentiable_intrinsics", self.differentiable_intrinsics),
+                         ("differentiable_distortion", self.differentiable_distortion),
+                         ("a gradient_exchange", self.gradient_exchange is not None)):
+            if on:
+                raise ValueError(f"a rolling-shutter camera is not supported with {name}")
+        values = rolling_shutter.motion
+        if motion is not None:
+            if not isinstance(motion, torch.Tensor):
+                raise ValueError("rolling_shutter_motion must be a torch.Tensor")
+            if tuple(motion.shape) != (6,):
+                raise ValueError(f"rolling_shutter_motion must have shape (6,), got {tuple(motion.shape)}")
+            if motion.dtype != torch.float32:
+                raise ValueError(f"rolling_shutter_motion must be float32, got {motion.dtype}")
+            values = motion.detach().cpu().tolist()
+            if not all(math.isfinite(v) for v in values):
+                raise ValueError(f"rolling_shutter_motion must be finite, got {values}")
+        return _lib.GsbRollingShutterArgs(motion=(ctypes.c_float * 6)(*values), row_time=None)
+
     # ------------------------------------------------------------------ backward plumbing
     def _run_backward(self, ctx, grad_rasterized_image, grad_rasterized_depth=None, grad_pixel_accumulated_alpha=None,
-                      grad_feature_map=None, pose=False, intrinsics=False, lens_grad=False):
+                      grad_feature_map=None, pose=False, intrinsics=False, lens_grad=False, motion_grad=False):
         """Returns dL/dxyz, dL/dfeatures, for a call with extra features dL/d of them ((N, C); zeros when the feature map
         was not used), with ``pose`` dL/dq_pointcloud_camera (K, 4) and dL/dt_pointcloud_camera (K, 3) (else None), with
-        ``intrinsics`` dL/dcamera_intrinsics (3, 3) (else None), and with ``lens_grad`` dL/dlens_coefficients on the
-        coefficient tensor's device (else None)."""
+        ``intrinsics`` dL/dcamera_intrinsics (3, 3) (else None), with ``lens_grad`` dL/dlens_coefficients on the
+        coefficient tensor's device (else None), and with ``motion_grad`` dL/drolling_shutter_motion on the motion tensor's
+        device (else None)."""
         cfg = self.config
         lib = _lib.load()
         saved = ctx.saved_tensors
@@ -665,8 +737,28 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                 C = extra_features.shape[1]
                 grad_extra_features = torch.zeros((N, C), dtype=torch.float32, device=device) if grad_feature_map is None \
                     else torch.empty((N, C), dtype=torch.float32, device=device)
-            grad_q = grad_t = grad_K = grad_k = None
-            if ctx.lens is not None:  # neither pose nor intrinsics gradients (refused in forward)
+            grad_q = grad_t = grad_K = grad_k = grad_m = None
+            if ctx.rolling_shutter is not None:  # neither pose, intrinsics nor lens gradients (refused in forward)
+                rs, _row_time = ctx.rolling_shutter
+                ext = None
+                if extra_features is not None and grad_feature_map is not None:
+                    grad_map = _f32(grad_feature_map)
+                    ext = _lib.GsbExtraFeatureArgs(channels=extra_features.shape[1], features=_ptr(extra_features),
+                                                   grad_rasterized=_ptr(grad_map), grad_features=_ptr(grad_extra_features))
+                rs_grad = None
+                if motion_grad:
+                    grad_motion = torch.empty((6,), dtype=torch.float32, device=device)
+                    rs_temp = torch.empty((int(lib.gsb200_rolling_shutter_grad_temp_bytes()) // 4,), dtype=torch.float32,
+                                          device=device)
+                    rs_grad = _lib.GsbRollingShutterGradArgs(grad_motion=_ptr(grad_motion), temp=_ptr(rs_temp))
+                _lib.check(lib.gsb200_backward_rolling_shutter(
+                    ctypes.byref(args), _ptr(grad_depth), _ptr(depth), _ptr(grad_alpha),
+                    ctypes.byref(ext) if ext is not None else None, ctypes.byref(ctx.lens) if ctx.lens is not None else None,
+                    ctypes.byref(rs), ctypes.byref(rs_grad) if rs_grad is not None else None),
+                    "gsb200_backward_rolling_shutter")
+                if motion_grad:
+                    grad_m = grad_motion.to(ctx.motion_device)
+            elif ctx.lens is not None:  # neither pose nor intrinsics gradients (refused in forward)
                 ext = None
                 if extra_features is not None and grad_feature_map is not None:
                     grad_map = _f32(grad_feature_map)
@@ -769,7 +861,7 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                     point_uv_in_camera=frame.point_uv.contiguous(),
                     point_depth=frame.point_in_camera[:, 2],
                 ))
-        return grad_pointcloud, grad_pointcloud_features, grad_extra_features, grad_q, grad_t, grad_K, grad_k
+        return grad_pointcloud, grad_pointcloud_features, grad_extra_features, grad_q, grad_t, grad_K, grad_k, grad_m
 
     def backward_flags(self, frame_flags: int) -> int:
         """Flags of the backward call for a frame rendered with ``frame_flags`` (adds the experimental kernel selection)."""
@@ -781,7 +873,8 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
 
     # ------------------------------------------------------------------ public forward (GPCR:1184-1204)
     def forward(self, input_data: "GaussianPointCloudRasterisation.GaussianPointCloudRasterisationInput",
-                point_extra_features: Optional[torch.Tensor] = None, lens_coefficients: Optional[torch.Tensor] = None):
+                point_extra_features: Optional[torch.Tensor] = None, lens_coefficients: Optional[torch.Tensor] = None,
+                rolling_shutter_motion: Optional[torch.Tensor] = None):
         """Returns (image, depth, pixel_valid_point_count), then pixel_accumulated_alpha with ``differentiable_alpha``.
         ``point_extra_features`` (an extension): an (N, C) float32 tensor of per-Gaussian values (1 <= C <= 16; semantic
         logits, instance encodings, distilled features, ...), contiguous, on the scene's device.  The output tuple then
@@ -801,10 +894,29 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
         distortion`` supplies the model), and the backward returns dL/d ``lens_coefficients`` on the tensor's device.  The
         values are read on the host: free for a CPU tensor, one blocking 20-byte copy for a device tensor.  ``ValueError``
         for a camera with no lens, a tensor of the wrong length or dtype, or an operator without the option.  None: no
-        coefficient gradient."""
+        coefficient gradient.
+        ``input_data.camera_info.rolling_shutter`` (an extension; ``Camera.RollingShutter``): render and differentiate each
+        point at its row time through the view's motion (``gsb200_forward_rolling_shutter`` /
+        ``gsb200_backward_rolling_shutter``; definition in ``include/gsb200.h``), with or without a lens.  ``last_frame``'s
+        ``point_in_camera`` and ``point_uv`` are the values at each point's row time.  Every output and option above works
+        with a rolling shutter, except ``differentiable_pose``, ``differentiable_intrinsics``, ``differentiable_distortion``
+        and a ``gradient_exchange`` (``ValueError``).
+        ``rolling_shutter_motion`` (with ``differentiable_rolling_shutter``; an extension): a (6,) float32 tensor (v, w) on
+        any device.  Its values are the motion rendered, and the backward returns dL/d ``rolling_shutter_motion`` on the
+        tensor's device.  The values are read on the host like ``lens_coefficients``.  ``ValueError`` for a camera without
+        a rolling shutter, a tensor of the wrong shape or dtype, or an operator without the option.  None: no motion
+        gradient."""
         camera_info = input_data.camera_info
         assert camera_info.camera_width % TILE_WIDTH == 0
         assert camera_info.camera_height % TILE_HEIGHT == 0
+        if rolling_shutter_motion is not None:  # the extra features', K's and the coefficients' slots first (all refused)
+            self._rolling_shutter_args(camera_info, rolling_shutter_motion)  # the argument checks, before any device work
+            if point_extra_features is not None:
+                self._check_extra_features(point_extra_features, input_data.point_cloud)
+            return self._module_function.apply(
+                input_data.point_cloud, input_data.point_cloud_features, input_data.point_invalid_mask,
+                input_data.point_object_id, input_data.q_pointcloud_camera, input_data.t_pointcloud_camera, camera_info,
+                input_data.color_max_sh_band, point_extra_features, None, None, rolling_shutter_motion)
         if lens_coefficients is not None:  # the extra features' and K's slots first (K is refused with a lens)
             self._lens_args(camera_info, lens_coefficients)  # the argument checks, before any device work
             if point_extra_features is not None:

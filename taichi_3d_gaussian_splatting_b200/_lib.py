@@ -131,6 +131,14 @@ class GsbLensGradArgs(ctypes.Structure):
     _fields_ = [("grad_coefficients", c_vp), ("temp", c_vp)]
 
 
+class GsbRollingShutterArgs(ctypes.Structure):
+    _fields_ = [("motion", c_f32 * 6), ("row_time", c_vp)]
+
+
+class GsbRollingShutterGradArgs(ctypes.Structure):
+    _fields_ = [("grad_motion", c_vp), ("temp", c_vp)]
+
+
 def lens_args(distortion) -> GsbLensArgs:
     """The C argument of a ``Camera.LensDistortion`` (host floats; unused coefficients 0)."""
     model = {"opencv": GSB_LENS_OPENCV, "fisheye": GSB_LENS_FISHEYE}[distortion.model]
@@ -162,7 +170,8 @@ EXPORTS = (
     "gsb200_backward_aux", "gsb200_supervision_temp_bytes", "gsb200_train_step_aux", "gsb200_forward_ext",
     "gsb200_backward_ext", "gsb200_feature_loss_temp_bytes", "gsb200_train_step_ext", "gsb200_backward_pose",
     "gsb200_pose_grad_temp_bytes", "gsb200_backward_calib", "gsb200_intrinsics_grad_temp_bytes", "gsb200_forward_lens",
-    "gsb200_backward_lens", "gsb200_backward_lens_grad", "gsb200_lens_grad_temp_bytes",
+    "gsb200_backward_lens", "gsb200_backward_lens_grad", "gsb200_lens_grad_temp_bytes", "gsb200_forward_rolling_shutter",
+    "gsb200_backward_rolling_shutter", "gsb200_rolling_shutter_grad_temp_bytes",
 )
 
 _lib = None
@@ -216,6 +225,16 @@ def load() -> ctypes.CDLL:
     lib.gsb200_backward_lens_grad.restype = ctypes.c_int
     lib.gsb200_lens_grad_temp_bytes.argtypes = []
     lib.gsb200_lens_grad_temp_bytes.restype = c_i64
+    lib.gsb200_forward_rolling_shutter.argtypes = [ctypes.POINTER(GsbForwardArgs), ctypes.POINTER(GsbExtraFeatureArgs),
+                                                   ctypes.POINTER(GsbLensArgs), ctypes.POINTER(GsbRollingShutterArgs)]
+    lib.gsb200_forward_rolling_shutter.restype = ctypes.c_int
+    lib.gsb200_backward_rolling_shutter.argtypes = [ctypes.POINTER(GsbBackwardArgs), c_vp, c_vp, c_vp,
+                                                    ctypes.POINTER(GsbExtraFeatureArgs), ctypes.POINTER(GsbLensArgs),
+                                                    ctypes.POINTER(GsbRollingShutterArgs),
+                                                    ctypes.POINTER(GsbRollingShutterGradArgs)]
+    lib.gsb200_backward_rolling_shutter.restype = ctypes.c_int
+    lib.gsb200_rolling_shutter_grad_temp_bytes.argtypes = []
+    lib.gsb200_rolling_shutter_grad_temp_bytes.restype = c_i64
     lib.gsb200_intrinsics_grad_temp_bytes.argtypes = []
     lib.gsb200_intrinsics_grad_temp_bytes.restype = c_i64
     lib.gsb200_sort_temp_bytes.argtypes = [c_i64, c_i32]
@@ -318,6 +337,12 @@ def load() -> ctypes.CDLL:
     if sizes12[11] != ctypes.sizeof(GsbLensGradArgs):
         raise RuntimeError(f"libgsb200.so ABI mismatch: sizeof(GsbLensGradArgs) {sizes12[11]} != ctypes mirror "
                            f"{ctypes.sizeof(GsbLensGradArgs)}")
+    sizes14 = (c_i64 * 14)()
+    lib.gsb200_abi_sizes_ext(sizes14, 14)
+    for i, mirror in ((12, GsbRollingShutterArgs), (13, GsbRollingShutterGradArgs)):
+        if sizes14[i] != ctypes.sizeof(mirror):
+            raise RuntimeError(f"libgsb200.so ABI mismatch: sizeof({mirror.__name__}) {sizes14[i]} != ctypes mirror "
+                               f"{ctypes.sizeof(mirror)}")
     _lib = lib
     return lib
 

@@ -192,12 +192,13 @@ void gsb200_abi_sizes(int64_t *out3) {
 }
 
 void gsb200_abi_sizes_ext(int64_t *out, int32_t n) {
-    const int64_t all[12] = {(int64_t)sizeof(GsbWorkspaceLayout), (int64_t)sizeof(GsbForwardArgs), (int64_t)sizeof(GsbBackwardArgs),
+    const int64_t all[14] = {(int64_t)sizeof(GsbWorkspaceLayout), (int64_t)sizeof(GsbForwardArgs), (int64_t)sizeof(GsbBackwardArgs),
                              (int64_t)sizeof(GsbExpandArgs), (int64_t)sizeof(GsbTrainStepArgs), (int64_t)sizeof(GsbSupervisionArgs),
                              (int64_t)sizeof(GsbExtraFeatureArgs), (int64_t)sizeof(GsbFeatureTrainArgs),
                              (int64_t)sizeof(GsbPoseGradArgs), (int64_t)sizeof(GsbIntrinsicsGradArgs), (int64_t)sizeof(GsbLensArgs),
-                             (int64_t)sizeof(GsbLensGradArgs)};
-    for (int i = 0; i < n && i < 12; ++i) out[i] = all[i];
+                             (int64_t)sizeof(GsbLensGradArgs), (int64_t)sizeof(GsbRollingShutterArgs),
+                             (int64_t)sizeof(GsbRollingShutterGradArgs)};
+    for (int i = 0; i < n && i < 14; ++i) out[i] = all[i];
 }
 
 int gsb200_workspace_layout(int64_t num_points, int32_t num_objects, int64_t key_capacity,
@@ -270,10 +271,48 @@ static int check_lens(const char *what, const GsbLensArgs *lens, LensParams *par
 int gsb200_forward_ext(const GsbForwardArgs *a, const GsbExtraFeatureArgs *ext) { return gsb200_forward_lens(a, ext, nullptr); }
 
 int gsb200_forward_lens(const GsbForwardArgs *a, const GsbExtraFeatureArgs *ext, const GsbLensArgs *lens_args) {
+    return gsb200_forward_rolling_shutter(a, ext, lens_args, nullptr);
+}
+
+// GsbRollingShutterArgs -> RsParams; GSB_EINVAL for a non-finite motion or a NULL or misaligned row_time.  *out_rs stays NULL
+// for a NULL rs.
+static int check_rs(const char *what, const GsbRollingShutterArgs *rs, RsParams *params, const RsParams **out_rs) {
+    *out_rs = nullptr;
+    if (!rs) return GSB_OK;
+    for (int i = 0; i < 6; ++i) {
+        const float m = rs->motion[i];
+        if (!(m - m == 0.0f)) {
+            set_error("%s: rolling-shutter motion %d is not finite", what, i);
+            return GSB_EINVAL;
+        }
+    }
+    if (!rs->row_time) {
+        set_error("%s: null row_time pointer", what);
+        return GSB_EINVAL;
+    }
+    if (reinterpret_cast<uintptr_t>(rs->row_time) % 4 != 0) {
+        set_error("%s: row_time must be 4-byte aligned", what);
+        return GSB_EINVAL;
+    }
+    for (int i = 0; i < 6; ++i) params->motion[i] = rs->motion[i];
+    params->row_time = rs->row_time;
+    *out_rs = params;
+    return GSB_OK;
+}
+
+int64_t gsb200_rolling_shutter_grad_temp_bytes(void) {
+    return (int64_t)GSB_RS_GRAD_PARTIAL_BLOCKS * 6 * (int64_t)sizeof(float);
+}
+
+int gsb200_forward_rolling_shutter(const GsbForwardArgs *a, const GsbExtraFeatureArgs *ext, const GsbLensArgs *lens_args,
+                                   const GsbRollingShutterArgs *rs_args) {
     LensParams lens_params;
     const LensParams *lens;
-    int lrc = check_lens("forward_lens", lens_args, &lens_params, &lens);
+    int lrc = check_lens(rs_args ? "forward_rolling_shutter" : "forward_lens", lens_args, &lens_params, &lens);
     if (lrc != GSB_OK) return lrc;
+    RsParams rs_params;
+    const RsParams *rs;
+    if ((lrc = check_rs("forward_rolling_shutter", rs_args, &rs_params, &rs)) != GSB_OK) return lrc;
     if (ext) {
         if (ext->channels < 1 || ext->channels > 16) {
             set_error("forward_ext: channels must be in 1..16 (got %d)", ext->channels);
@@ -292,7 +331,7 @@ int gsb200_forward_lens(const GsbForwardArgs *a, const GsbExtraFeatureArgs *ext,
     int rc = resolve_fwd(a, &ws);
     if (rc != GSB_OK) return rc;
     cudaStream_t st = static_cast<cudaStream_t>(a->stream);
-    if ((rc = launch_preprocess(*a, ws, st, lens)) != GSB_OK) return rc;
+    if ((rc = launch_preprocess(*a, ws, st, lens, rs)) != GSB_OK) return rc;
     if (a->host_counters && a->host_counters_event) {
         GSB_CUDA_CHECK(cudaMemcpyAsync(a->host_counters, ws.counters, 4 * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
         GSB_CUDA_CHECK(cudaEventRecord(static_cast<cudaEvent_t>(a->host_counters_event), st));
@@ -309,7 +348,8 @@ static int backward_impl(const GsbBackwardArgs *a, bool skip_on_overflow, const 
                          const float *depth = nullptr, const float *grad_alpha = nullptr,
                          const GsbExtraFeatureArgs *ext = nullptr, const GsbPoseGradArgs *pose = nullptr,
                          const GsbIntrinsicsGradArgs *intr = nullptr, const LensParams *lens = nullptr,
-                         const GsbLensGradArgs *lens_grad = nullptr) {
+                         const GsbLensGradArgs *lens_grad = nullptr, const RsParams *rs = nullptr,
+                         const GsbRollingShutterGradArgs *rs_grad = nullptr) {
     if (!a) {
         set_error("backward: args is null");
         return GSB_EINVAL;
@@ -363,6 +403,7 @@ static int backward_impl(const GsbBackwardArgs *a, bool skip_on_overflow, const 
     if (ext && a->num_points > 0)  // the blend adds into the rows it reaches; every other row stays zero
         GSB_CUDA_CHECK(cudaMemsetAsync(ext->grad_features, 0, (size_t)a->num_points * ext->channels * 4, st));
     if ((rc = launch_blend_backward(*a, ws, st, grad_depth, depth, grad_alpha, ext)) != GSB_OK) return rc;
+    if (rs) return launch_backward_points_rs(*a, ws, st, grad_depth != nullptr, lens, *rs, rs_grad);
     if (lens && lens_grad) return launch_backward_points_lens_grad(*a, ws, st, grad_depth != nullptr, *lens, *lens_grad);
     if (lens) return launch_backward_points_lens(*a, ws, st, grad_depth != nullptr, *lens);
     if (intr) return launch_backward_points_calib(*a, ws, st, grad_depth != nullptr, pose, *intr);
@@ -383,10 +424,51 @@ int gsb200_backward_ext(const GsbBackwardArgs *a, const float *grad_rasterized_d
 }
 
 // gsb200_backward_calib's checks and dispatch; `lens` (gsb200_backward_lens, checked there) comes with neither pose nor
-// intrinsics, and `lens_grad` (gsb200_backward_lens_grad, checked there) only with `lens`
+// intrinsics, `lens_grad` (gsb200_backward_lens_grad, checked there) only with `lens`, and `rs` / `rs_grad`
+// (gsb200_backward_rolling_shutter, checked there) with neither pose, intrinsics nor lens_grad
 static int backward_checked(const GsbBackwardArgs *a, const float *grad_rasterized_depth, const float *rasterized_depth,
                             const float *grad_pixel_accumulated_alpha, const GsbExtraFeatureArgs *ext, const GsbPoseGradArgs *pose,
-                            const GsbIntrinsicsGradArgs *intr, const LensParams *lens, const GsbLensGradArgs *lens_grad = nullptr);
+                            const GsbIntrinsicsGradArgs *intr, const LensParams *lens, const GsbLensGradArgs *lens_grad = nullptr,
+                            const RsParams *rs = nullptr, const GsbRollingShutterGradArgs *rs_grad = nullptr);
+
+int gsb200_backward_rolling_shutter(const GsbBackwardArgs *a, const float *grad_rasterized_depth, const float *rasterized_depth,
+                                    const float *grad_pixel_accumulated_alpha, const GsbExtraFeatureArgs *ext,
+                                    const GsbLensArgs *lens_args, const GsbRollingShutterArgs *rs_args,
+                                    const GsbRollingShutterGradArgs *rs_grad) {
+    if (!rs_args && rs_grad) {
+        set_error("backward_rolling_shutter: the motion gradient needs a rolling shutter (rs is NULL)");
+        return GSB_EINVAL;
+    }
+    if (!rs_args) return gsb200_backward_lens(a, grad_rasterized_depth, rasterized_depth, grad_pixel_accumulated_alpha, ext, lens_args);
+    LensParams lens_params;
+    const LensParams *lens;
+    int rc = check_lens("backward_rolling_shutter", lens_args, &lens_params, &lens);
+    if (rc != GSB_OK) return rc;
+    RsParams rs_params;
+    const RsParams *rs;
+    if ((rc = check_rs("backward_rolling_shutter", rs_args, &rs_params, &rs)) != GSB_OK) return rc;
+    if (rs_grad) {
+        if (!rs_grad->grad_motion || !rs_grad->temp) {
+            set_error("backward_rolling_shutter: null grad_motion / temp pointer");
+            return GSB_EINVAL;
+        }
+        if (reinterpret_cast<uintptr_t>(rs_grad->grad_motion) % 4 != 0) {
+            set_error("backward_rolling_shutter: grad_motion must be 4-byte aligned");
+            return GSB_EINVAL;
+        }
+        if (reinterpret_cast<uintptr_t>(rs_grad->temp) % 16 != 0) {
+            set_error("backward_rolling_shutter: the rolling-shutter temp must be 16-byte aligned");
+            return GSB_EINVAL;
+        }
+    }
+    if (a != nullptr && (a->flags & GSB_FLAG_COMPACT_GRADS)) {
+        set_error("backward_rolling_shutter: the rolling shutter is not implemented for the compact rows of the view-parallel "
+                  "exchange (GSB_FLAG_COMPACT_GRADS)");
+        return GSB_EUNSUPPORTED;
+    }
+    return backward_checked(a, grad_rasterized_depth, rasterized_depth, grad_pixel_accumulated_alpha, ext, nullptr, nullptr, lens,
+                            nullptr, rs, rs_grad);
+}
 
 int gsb200_backward_lens(const GsbBackwardArgs *a, const float *grad_rasterized_depth, const float *rasterized_depth,
                          const float *grad_pixel_accumulated_alpha, const GsbExtraFeatureArgs *ext, const GsbLensArgs *lens_args) {
@@ -462,7 +544,8 @@ int gsb200_backward_calib(const GsbBackwardArgs *a, const float *grad_rasterized
 
 static int backward_checked(const GsbBackwardArgs *a, const float *grad_rasterized_depth, const float *rasterized_depth,
                             const float *grad_pixel_accumulated_alpha, const GsbExtraFeatureArgs *ext, const GsbPoseGradArgs *pose,
-                            const GsbIntrinsicsGradArgs *intr, const LensParams *lens, const GsbLensGradArgs *lens_grad) {
+                            const GsbIntrinsicsGradArgs *intr, const LensParams *lens, const GsbLensGradArgs *lens_grad,
+                            const RsParams *rs, const GsbRollingShutterGradArgs *rs_grad) {
     if (intr) {
         if (!intr->grad_camera_intrinsics || !intr->temp) {
             set_error("backward_calib: null grad_camera_intrinsics / temp pointer");
@@ -528,7 +611,7 @@ static int backward_checked(const GsbBackwardArgs *a, const float *grad_rasteriz
         return GSB_EUNSUPPORTED;
     }
     return backward_impl(a, false, grad_rasterized_depth, rasterized_depth, grad_pixel_accumulated_alpha, ext, pose, intr, lens,
-                         lens_grad);
+                         lens_grad, rs, rs_grad);
 }
 
 int gsb200_backward_with_depth(const GsbBackwardArgs *a, const float *grad_rasterized_depth, const float *rasterized_depth) {

@@ -422,14 +422,28 @@ __device__ __forceinline__ void weighted_u_sigma(const float *U, const float *R,
 // (lens_coefficient_grad, common.cuh), which the warp sums (fixed butterfly order, all objects together: a frame has one lens)
 // into the per-warp row s_lgrad[warp][5]; after the loop the CTA adds its warps' rows in warp order into
 // lgrad_partials[blockIdx.x][5], and lens_grad_finish_kernel adds the blocks in block order.
+// RS = true (gsb200_backward_rolling_shutter): the frame was rendered through a rolling shutter (include/gsb200.h), so the
+// point's row time tau = rs.row_time[id] (written by the forward; detached) gives W_eff = Rd(tau) W, which replaces W in
+// d uv / d xyz, the depth term and U = J W_eff; point_in_camera already holds pc(tau).  Non-compact, without POSE / INTR /
+// LGRAD; with or without LENS.
+// MGRAD = true (with RS and rs_grad): each in-camera point also forms its 6 motion values (rolling_shutter_grad, common.cuh),
+// which the warp sums (fixed butterfly order, all objects together: a frame has one motion) into the per-warp row
+// s_mgrad[warp][6]; after the loop the CTA adds its warps' rows in warp order into mgrad_partials[blockIdx.x][6], and
+// rolling_shutter_grad_finish_kernel adds the blocks in block order.
 constexpr int LENS_GRAD_VALUES = 5;
-template <bool COMPACT, bool DEPTH, bool POSE, bool INTR = false, bool LENS = false, bool LGRAD = false>
+constexpr int RS_GRAD_VALUES = 6;
+template <bool COMPACT, bool DEPTH, bool POSE, bool INTR = false, bool LENS = false, bool LGRAD = false, bool RS = false,
+          bool MGRAD = false>
 __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, float *s_pose, float *pose_partials,
                                                      int num_objects, float *s_intr = nullptr,
                                                      float *intr_partials = nullptr, const LensParams lens = LensParams(),
-                                                     float *s_lgrad = nullptr, float *lgrad_partials = nullptr) {
+                                                     float *s_lgrad = nullptr, float *lgrad_partials = nullptr,
+                                                     const RsParams rs = RsParams(), float *s_mgrad = nullptr,
+                                                     float *mgrad_partials = nullptr) {
     static_assert(!LENS || (!COMPACT && !POSE && !INTR), "the lens gradient is implemented for the dense rows alone");
     static_assert(!LGRAD || LENS, "the coefficient gradient needs the lens path");
+    static_assert(!RS || (!COMPACT && !POSE && !INTR && !LGRAD), "the rolling shutter is implemented for the dense rows alone");
+    static_assert(!MGRAD || RS, "the motion gradient needs the rolling-shutter path");
     // One thread per scene row: rows outside the frustum get their zeros here (no separate memset of the
     // dense (N,3)/(N,56) gradients), rows inside get the chain rule.  A warp owns 32 consecutive rows, i.e. one
     // contiguous 7 KB piece of the (N,56) gradient and 384 B of the (N,3) one: each lane stages its row in
@@ -456,6 +470,11 @@ __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, fl
         if (lane < LENS_GRAD_VALUES) my_lgrad[lane] = 0.0f;
         __syncwarp();
     }
+    float *const my_mgrad = MGRAD ? s_mgrad + warp * RS_GRAD_VALUES : nullptr;
+    if (MGRAD) {
+        if (lane < RS_GRAD_VALUES) my_mgrad[lane] = 0.0f;
+        __syncwarp();
+    }
     const long long stride = (long long)gridDim.x * blockDim.x;
     for (long long base = (long long)blockIdx.x * blockDim.x + warp * 32; base < p.N; base += stride) {
       const long long id = base + lane;
@@ -471,6 +490,11 @@ __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, fl
       if (LGRAD) {
 #pragma unroll
           for (int k = 0; k < LENS_GRAD_VALUES; ++k) lv[k] = 0.0f;
+      }
+      float mv[MGRAD ? RS_GRAD_VALUES : 1];  // zero for rows outside the frustum
+      if (MGRAD) {
+#pragma unroll
+          for (int k = 0; k < RS_GRAD_VALUES; ++k) mv[k] = 0.0f;
       }
       if (o < 0) {
           if (!COMPACT) { my_xyz[0] = 0.0f; my_xyz[1] = 0.0f; my_xyz[2] = 0.0f; }
@@ -494,6 +518,17 @@ __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, fl
         const float4 *frow = reinterpret_cast<const float4 *>(p.features + (size_t)GSB_FEATURE_DIM * id);
         const float4 qv = __ldg(frow);
         const float4 sv = __ldg(frow + 1);  // s0 s1 s2 logit
+        float Wo[9], Rd[9], tau = 0.0f;  // RS: the object's W, Rd(tau) and the row time; Wm becomes W_eff = Rd W
+        if (RS) {
+            tau = rs.row_time[id];
+            rolling_shutter_rotation(tau, rs.motion + 3, Rd);
+#pragma unroll
+            for (int k = 0; k < 9; ++k) Wo[k] = Wm[k];
+#pragma unroll
+            for (int r = 0; r < 3; ++r)
+#pragma unroll
+                for (int c = 0; c < 3; ++c) Wm[3 * r + c] = (Rd[3 * r] * Wo[c] + Rd[3 * r + 1] * Wo[3 + c]) + Rd[3 * r + 2] * Wo[6 + c];
+        }
 
         // d uv / d xyz (GP3D:132-159): full-K projection Jacobian times W
         const float iz = 1.0f / pcz, iz2 = iz * iz;
@@ -636,6 +671,19 @@ __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, fl
                 lens_coefficient_grad<GSB_LENS_FISHEYE>(pcx * iz, pcy * iz, gxd, gyd, w00, w01 + w10, w11, lv);
             else lens_coefficient_grad<GSB_LENS_OPENCV>(pcx * iz, pcy * iz, gxd, gyd, w00, w01 + w10, w11, lv);
         }
+        if (MGRAD) {
+            // gp = dL/dpc(tau) through uv (and z with DEPTH); Sigma' = U Sigma U^T with U = J Rd W: dL/dU = 2 [B0; B1]
+            float gp[3];
+#pragma unroll
+            for (int r = 0; r < 3; ++r) gp[r] = dj[r] * a0.x + dj[3 + r] * a0.y;
+            if (DEPTH) gp[2] += a2.w;
+            float B0[3], B1[3];
+            weighted_u_sigma(U, R, es, g00, g01, g11, B0, B1);
+            const float pc0[3] = {((Wo[0] * x + Wo[1] * y) + Wo[2] * z) + pb->T[3],
+                                  ((Wo[3] * x + Wo[4] * y) + Wo[5] * z) + pb->T[7],
+                                  ((Wo[6] * x + Wo[7] * y) + Wo[8] * z) + pb->T[11]};
+            rolling_shutter_grad(tau, rs.motion + 3, Rd, pc0, gp, J, B0, B1, Wo, mv);
+        }
         if (p.ctl_num_in_camera != nullptr && !(p.skip_flag != nullptr && *p.skip_flag != 0)) {
             // GaussianPointAdaptiveController.update (:130-143) for this in-camera point: ids are unique, one thread per row,
             // so plain read-modify-writes.  a2.y = sum |d/duv| over pixels, a2.z = number of affected pixels (exact in f32)
@@ -714,6 +762,15 @@ __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, fl
               if (lane == 0) my_lgrad[k] += v;
           }
       }
+      if (MGRAD) {
+#pragma unroll
+          for (int k = 0; k < RS_GRAD_VALUES; ++k) {
+              float v = mv[k];
+#pragma unroll
+              for (int d = 16; d > 0; d >>= 1) v += __shfl_xor_sync(0xffffffffu, v, d);
+              if (lane == 0) my_mgrad[k] += v;
+          }
+      }
       __syncwarp();
       const long long rows = p.N - base < 32 ? p.N - base : 32;
       if (COMPACT) {
@@ -770,6 +827,14 @@ __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, fl
             float s = s_lgrad[threadIdx.x];
             for (int w = 1; w < GSB_POINTS_THREADS / 32; ++w) s += s_lgrad[w * LENS_GRAD_VALUES + threadIdx.x];
             lgrad_partials[(size_t)blockIdx.x * LENS_GRAD_VALUES + threadIdx.x] = s;
+        }
+    }
+    if (MGRAD) {
+        __syncthreads();
+        if (threadIdx.x < RS_GRAD_VALUES) {
+            float s = s_mgrad[threadIdx.x];
+            for (int w = 1; w < GSB_POINTS_THREADS / 32; ++w) s += s_mgrad[w * RS_GRAD_VALUES + threadIdx.x];
+            mgrad_partials[(size_t)blockIdx.x * RS_GRAD_VALUES + threadIdx.x] = s;
         }
     }
 }
@@ -841,6 +906,46 @@ lens_grad_finish_kernel(const float *__restrict__ partials, int blocks, float *_
         __syncthreads();
     }
     if (tid < LENS_GRAD_VALUES) grad_coefficients[tid] = s_sum[0][tid];
+}
+
+// The parameter block of the rolling-shutter instantiations (LENS = false ignores `lens`).
+struct PointsBwdRsParams : PointsBwdLensParams {
+    RsParams rs;
+    float *rs_partials;  // MGRAD: (grid, 6)
+};
+
+template <bool DEPTH, bool LENS, bool MGRAD>
+__global__ void __launch_bounds__(GSB_POINTS_THREADS, MGRAD ? 3 : 5)  // MGRAD: at 4 CTAs per SM the 6 values spill 4 bytes
+backward_points_rs_kernel(const PointsBwdRsParams p) {
+    __shared__ float s_mgrad[MGRAD ? (GSB_POINTS_THREADS / 32) * RS_GRAD_VALUES : 1];
+    backward_points_body<false, DEPTH, false, false, LENS, false, true, MGRAD>(p, nullptr, nullptr, 0, nullptr, nullptr, p.lens,
+                                                                              nullptr, nullptr, p.rs, s_mgrad, p.rs_partials);
+}
+
+// One CTA: adds the `blocks` partial rows in a fixed order (strided per thread, then a fixed shared-memory tree) and writes
+// the 6 motion gradients.  Zeros when blocks == 0.
+constexpr int RS_GRAD_FINISH_THREADS = 128;
+__global__ void __launch_bounds__(RS_GRAD_FINISH_THREADS)
+rolling_shutter_grad_finish_kernel(const float *__restrict__ partials, int blocks, float *__restrict__ grad_motion) {
+    __shared__ float s_sum[RS_GRAD_FINISH_THREADS][RS_GRAD_VALUES + 1];
+    const int tid = threadIdx.x;
+    float acc[RS_GRAD_VALUES];
+#pragma unroll
+    for (int k = 0; k < RS_GRAD_VALUES; ++k) acc[k] = 0.0f;
+    for (int b = tid; b < blocks; b += RS_GRAD_FINISH_THREADS) {
+#pragma unroll
+        for (int k = 0; k < RS_GRAD_VALUES; ++k) acc[k] += partials[(size_t)b * RS_GRAD_VALUES + k];
+    }
+#pragma unroll
+    for (int k = 0; k < RS_GRAD_VALUES; ++k) s_sum[tid][k] = acc[k];
+    __syncthreads();
+    for (int h = RS_GRAD_FINISH_THREADS / 2; h > 0; h >>= 1) {
+        if (tid < h)
+#pragma unroll
+            for (int k = 0; k < RS_GRAD_VALUES; ++k) s_sum[tid][k] += s_sum[tid + h][k];
+        __syncthreads();
+    }
+    if (tid < RS_GRAD_VALUES) grad_motion[tid] = s_sum[0][tid];
 }
 
 // R(q) of GP3D:30-48 (xyzw, not normalised) and the gradient of sum_ij G_ij R(q)_ij with respect to q
@@ -1136,6 +1241,45 @@ int launch_backward_points_lens_grad(const GsbBackwardArgs &a, const Workspace &
     lens_grad_finish_kernel<<<1, LENS_GRAD_FINISH_THREADS, 0, stream>>>(p.lens_partials, (int)blocks,
                                                                          lens_grad.grad_coefficients);
     GSB_CUDA_CHECK(cudaGetLastError());
+    return GSB_OK;
+}
+
+template <bool DEPTH, bool LENS>
+static void launch_rs_kernel(bool mgrad, int blocks, cudaStream_t stream, const PointsBwdRsParams &p) {
+    if (mgrad) backward_points_rs_kernel<DEPTH, LENS, true><<<blocks, GSB_POINTS_THREADS, 0, stream>>>(p);
+    else backward_points_rs_kernel<DEPTH, LENS, false><<<blocks, GSB_POINTS_THREADS, 0, stream>>>(p);
+}
+
+// The RS per-point kernel: without rs_grad on the grid of launch_backward_points_lens; with rs_grad (MGRAD) on a grid that
+// depends on N alone (at most GSB_RS_GRAD_PARTIAL_BLOCKS CTAs), so the summation order of the motion gradient is the same on
+// every device, then rolling_shutter_grad_finish_kernel.  Every per-row output is written by the row's own thread, so it does
+// not depend on the grid.  The caller checked the arguments.
+int launch_backward_points_rs(const GsbBackwardArgs &a, const Workspace &ws, cudaStream_t stream, bool depth_grad,
+                              const LensParams *lens, const RsParams &rs, const GsbRollingShutterGradArgs *rs_grad) {
+    PointsBwdRsParams p;
+    static_cast<PointsBwdParams &>(p) = make_points_params(a, ws, nullptr);
+    p.lens = lens != nullptr ? *lens : LensParams();
+    p.rs = rs;
+    p.rs_partials = rs_grad != nullptr ? static_cast<float *>(rs_grad->temp) : nullptr;
+    long long blocks = a.num_points > 0 ? (a.num_points + GSB_POINTS_THREADS - 1) / GSB_POINTS_THREADS : 0;
+    const long long cap = rs_grad != nullptr ? (long long)GSB_RS_GRAD_PARTIAL_BLOCKS : 16LL * num_sms();
+    if (blocks > cap) blocks = cap;
+    if (blocks > 0) {
+        const bool mgrad = rs_grad != nullptr;
+        if (lens != nullptr) {
+            if (depth_grad) launch_rs_kernel<true, true>(mgrad, (int)blocks, stream, p);
+            else launch_rs_kernel<false, true>(mgrad, (int)blocks, stream, p);
+        } else {
+            if (depth_grad) launch_rs_kernel<true, false>(mgrad, (int)blocks, stream, p);
+            else launch_rs_kernel<false, false>(mgrad, (int)blocks, stream, p);
+        }
+        GSB_CUDA_CHECK(cudaGetLastError());
+    }
+    if (rs_grad != nullptr) {
+        rolling_shutter_grad_finish_kernel<<<1, RS_GRAD_FINISH_THREADS, 0, stream>>>(p.rs_partials, (int)blocks,
+                                                                                     rs_grad->grad_motion);
+        GSB_CUDA_CHECK(cudaGetLastError());
+    }
     return GSB_OK;
 }
 

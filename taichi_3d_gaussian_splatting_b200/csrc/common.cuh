@@ -63,8 +63,11 @@ int resolve_workspace(void *base, int64_t bytes, int64_t N, int32_t n_obj, int64
 
 // ---- stage launchers (each enqueues on `stream`, returns GSB_* code)
 struct LensParams;
-// lens: the distortion of gsb200_forward_lens (checked there, r2_max set), or NULL for the pinhole kernel
-int launch_preprocess(const GsbForwardArgs &a, const Workspace &ws, cudaStream_t stream, const LensParams *lens = nullptr);
+struct RsParams;
+// lens: the distortion of gsb200_forward_lens (checked there, r2_max set), or NULL for the pinhole kernel; rs: the rolling
+// shutter of gsb200_forward_rolling_shutter (checked there), or NULL
+int launch_preprocess(const GsbForwardArgs &a, const Workspace &ws, cudaStream_t stream, const LensParams *lens = nullptr,
+                      const RsParams *rs = nullptr);
 int launch_sort(const Workspace &ws, int64_t key_capacity, cudaStream_t stream);
 int launch_tile_ranges(const Workspace &ws, int64_t key_capacity, int num_tiles, cudaStream_t stream);
 int launch_tile_ranges_raw(const long long *keys_i64, int64_t n, int *tile_start, int *tile_end,
@@ -89,6 +92,10 @@ int launch_backward_points_lens(const GsbBackwardArgs &a, const Workspace &ws, c
 // lens_grad.temp), and the finishing kernel; arguments checked by the caller
 int launch_backward_points_lens_grad(const GsbBackwardArgs &a, const Workspace &ws, cudaStream_t stream, bool depth_grad,
                                      const LensParams &lens, const GsbLensGradArgs &lens_grad);
+// gsb200_backward_rolling_shutter: the RS per-point kernel (lens: NULL for a pinhole), with rs_grad also the motion sums
+// (per-CTA rows in rs_grad->temp) and the finishing kernel; arguments checked by the caller
+int launch_backward_points_rs(const GsbBackwardArgs &a, const Workspace &ws, cudaStream_t stream, bool depth_grad,
+                              const LensParams *lens, const RsParams &rs, const GsbRollingShutterGradArgs *rs_grad);
 // gsb200_backward_pose: the POSE per-point kernel (dense gradients as launch_backward_points, plus the per-CTA pose sums
 // in pose.temp) and the per-object finishing kernel; arguments checked by the caller
 int launch_backward_points_pose(const GsbBackwardArgs &a, const Workspace &ws, cudaStream_t stream, bool depth_grad,
@@ -362,6 +369,79 @@ __device__ __forceinline__ void lens_coefficient_grad(float xn, float yn, float 
         }
         out[4] = 0.0f;
     }
+}
+#endif
+
+// ---- rolling shutter (gsb200_forward_rolling_shutter / gsb200_backward_rolling_shutter; definition in include/gsb200.h)
+struct RsParams {
+    float motion[6];  // v (3), w (3)
+    float *row_time;  // (N): written by the forward, read by the backward
+};
+#if defined(__CUDACC__) || defined(GSB_HOST_EMU)
+// A = sin(theta)/theta, B = (1 - cos(theta))/theta^2, C = (theta - sin(theta))/theta^3 of theta^2 = t2, by their series below
+// t2 = 0.01 (cancellation-free; t2 = 0 gives A = 1, B = 1/2 exactly)
+__device__ __forceinline__ void rs_series(float t2, float &A, float &B, float &C) {
+    if (t2 < 0.01f) {
+        A = 1.0f - (t2 / 6.0f) * (1.0f - t2 / 20.0f);
+        B = 0.5f * (1.0f - (t2 / 12.0f) * (1.0f - t2 / 30.0f));
+        C = (1.0f / 6.0f) * (1.0f - (t2 / 20.0f) * (1.0f - t2 / 42.0f));
+    } else {
+        const float th = sqrtf(t2);
+        const float s = sinf(th);
+        A = s / th;
+        B = (1.0f - cosf(th)) / t2;
+        C = (th - s) / (t2 * th);
+    }
+}
+// Rd(tau) = exp(tau [w]x) = I + A [p]x + B [p]x^2 with p = tau w, row-major.  w = 0 gives I exactly.
+__device__ __forceinline__ void rolling_shutter_rotation(float tau, const float *w, float *R) {
+    const float px = tau * w[0], py = tau * w[1], pz = tau * w[2];
+    float A, B, C;
+    rs_series(px * px + py * py + pz * pz, A, B, C);
+    R[0] = 1.0f - B * (py * py + pz * pz); R[1] = B * (px * py) - A * pz;        R[2] = B * (px * pz) + A * py;
+    R[3] = B * (px * py) + A * pz;        R[4] = 1.0f - B * (px * px + pz * pz); R[5] = B * (py * pz) - A * px;
+    R[6] = B * (px * pz) - A * py;        R[7] = B * (py * pz) + A * px;        R[8] = 1.0f - B * (px * px + py * py);
+}
+// pc(tau) = Rd pc0 + tau v
+__device__ __forceinline__ void rolling_shutter_point(const float *R, float tau, const float *v, const float *pc0, float *pc) {
+#pragma unroll
+    for (int r = 0; r < 3; ++r) pc[r] = ((R[3 * r] * pc0[0] + R[3 * r + 1] * pc0[1]) + R[3 * r + 2] * pc0[2]) + tau * v[r];
+}
+// The motion gradient of one in-camera point (gsb200_backward_rolling_shutter with rs_grad): out = (dL/dv, dL/dw) of the
+// definition in include/gsb200.h.  gp = dL/dpc, pc0 = W xyz + tw, R = Rd(tau), J the full 2x3 J (row-major), B0, B1 the rows of
+// G (J W_eff) Sigma, W the object's rotation (row-major).  dL/dRd = gp pc0^T + 2 J^T [B0; B1] W^T; with A = Rd^T dL/dRd and
+// a = (A21 - A12, A02 - A20, A10 - A01) (0-based), dL/dw = tau J_r(tau w)^T a, J_r^T a = a + B (p x a) + C p x (p x a).
+__device__ __forceinline__ void rolling_shutter_grad(float tau, const float *w, const float *R, const float *pc0, const float *gp,
+                                                     const float *J, const float *B0, const float *B1, const float *W,
+                                                     float *out) {
+    out[0] = tau * gp[0];
+    out[1] = tau * gp[1];
+    out[2] = tau * gp[2];
+    float h0[3], h1[3];  // [B0; B1] W^T
+#pragma unroll
+    for (int j = 0; j < 3; ++j) {
+        h0[j] = B0[0] * W[3 * j] + B0[1] * W[3 * j + 1] + B0[2] * W[3 * j + 2];
+        h1[j] = B1[0] * W[3 * j] + B1[1] * W[3 * j + 1] + B1[2] * W[3 * j + 2];
+    }
+    float G[9];
+#pragma unroll
+    for (int r = 0; r < 3; ++r)
+#pragma unroll
+        for (int j = 0; j < 3; ++j) G[3 * r + j] = gp[r] * pc0[j] + 2.0f * (J[r] * h0[j] + J[3 + r] * h1[j]);
+    float A[9];  // Rd^T G
+#pragma unroll
+    for (int r = 0; r < 3; ++r)
+#pragma unroll
+        for (int j = 0; j < 3; ++j) A[3 * r + j] = R[r] * G[j] + R[3 + r] * G[3 + j] + R[6 + r] * G[6 + j];
+    const float a0 = A[7] - A[5], a1 = A[2] - A[6], a2 = A[3] - A[1];
+    const float px = tau * w[0], py = tau * w[1], pz = tau * w[2];
+    float sA, sB, sC;
+    rs_series(px * px + py * py + pz * pz, sA, sB, sC);
+    const float c0 = py * a2 - pz * a1, c1 = pz * a0 - px * a2, c2 = px * a1 - py * a0;  // p x a
+    const float d0 = py * c2 - pz * c1, d1 = pz * c0 - px * c2, d2 = px * c1 - py * c0;  // p x (p x a)
+    out[3] = tau * (a0 + sB * c0 + sC * d0);
+    out[4] = tau * (a1 + sB * c1 + sC * d1);
+    out[5] = tau * (a2 + sB * c2 + sC * d2);
 }
 #endif
 

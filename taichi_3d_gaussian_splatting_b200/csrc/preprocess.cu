@@ -192,8 +192,12 @@ __device__ __forceinline__ bool tile_reachable(const SplatReach &r, float u, flo
 // (gsb200_forward_lens) project through lens_distort (common.cuh): the position is (K00 xd + K01 yd + K02, K10 xd + K11 yd +
 // K12), J = diag(fx, fy) D P, and a point with r^2 > lens.r2_max is outside the frustum.  Everything downstream of (u, v) and
 // J -- the record layout, the keys, the scan -- is the same for every model.
-template <typename KeyT, int LENS>
-__device__ __forceinline__ void preprocess_body(const PreParams p, const LensParams lens) {
+// ROLLING = true (gsb200_forward_rolling_shutter): the point is moved to its row time first (definition in include/gsb200.h).  The
+// GSB_RS_ITERATIONS fixed-point steps project pc(tau_k) through the same lens arithmetic as the position below, the point is
+// rendered at pc(tau_3), Sigma' uses W_eff = Rd(tau_3) W, and tau_3 (0 outside the frustum) goes to rs.row_time[i].  The SH
+// view direction keeps the mid-readout camera centre.
+template <typename KeyT, int LENS, bool ROLLING = false>
+__device__ __forceinline__ void preprocess_body(const PreParams p, const LensParams lens, const RsParams rs = RsParams()) {
     __shared__ unsigned int s_ticket;
     __shared__ unsigned long long s_warp_sums[SCAN_BLOCK_THREADS / 32];
     __shared__ unsigned long long s_block_exclusive;
@@ -214,6 +218,7 @@ __device__ __forceinline__ void preprocess_body(const PreParams p, const LensPar
     float4 r0 = make_float4(0, 0, 0, 0), r1 = r0, r2 = r0;
     float pc[3] = {0, 0, 0};
     float dir0 = 0.0f, dir1 = 0.0f, dir2 = 0.0f;  // unit view direction (GPCR:302), consumed by the SH stage
+    float tau = 0.0f;                             // ROLLING: the row time
 
     // Every global load of a point that depends on nothing but its index is issued HERE, in one go: the invalid mask, the
     // object id, the position and the first 32 bytes of the feature row (q | s, logit).  The kernel is bound by the latency
@@ -248,6 +253,27 @@ __device__ __forceinline__ void preprocess_body(const PreParams p, const LensPar
         pc[0] = ((T[0] * x + T[1] * y) + T[2] * z) + T[3] * 1.0f;
         pc[1] = ((T[4] * x + T[5] * y) + T[6] * z) + T[7] * 1.0f;
         pc[2] = ((T[8] * x + T[9] * y) + T[10] * z) + T[11] * 1.0f;
+        float Rd[9];  // ROLLING: Rd(tau_3)
+        if (ROLLING) {
+            const float pc0[3] = {pc[0], pc[1], pc[2]};
+#pragma unroll 1
+            for (int it = 0; it < GSB_RS_ITERATIONS; ++it) {
+                rolling_shutter_rotation(tau, rs.motion + 3, Rd);
+                float pt[3];
+                rolling_shutter_point(Rd, tau, rs.motion, pc0, pt);
+                float vp;  // the row coordinate of pc(tau), as v below
+                if (LENS == GSB_LENS_PINHOLE) {
+                    vp = ((Kc[3] * pt[0] + Kc[4] * pt[1]) + Kc[5] * pt[2]) / pt[2];
+                } else {
+                    float ox, oy, Dt[4];
+                    lens_distort<LENS>(lens.k, pt[0] / pt[2], pt[1] / pt[2], ox, oy, Dt);
+                    vp = ((Kc[3] * (pt[0] + pt[2] * ox) + Kc[4] * (pt[1] + pt[2] * oy)) + Kc[5] * pt[2]) / pt[2];
+                }
+                tau = fminf(fmaxf(vp / (float)p.H - 0.5f, -0.5f), 0.5f);  // fmaxf(NaN, -1/2) = -1/2
+            }
+            rolling_shutter_rotation(tau, rs.motion + 3, Rd);
+            rolling_shutter_point(Rd, tau, rs.motion, pc0, pc);
+        }
         float u, v;
         float D[4] = {1.0f, 0.0f, 0.0f, 1.0f};  // d(xd, yd)/d(xn, yn)
         bool lens_ok = true;
@@ -307,6 +333,12 @@ __device__ __forceinline__ void preprocess_body(const PreParams p, const LensPar
                 for (int b = 0; b < 3; ++b) RT[b * 3 + a] = R[a * 3 + b];
             matmul<3, 3, 3>(RSS, RT, Sigma);
             float Wm[9] = {T[0], T[1], T[2], T[4], T[5], T[6], T[8], T[9], T[10]};
+            if (ROLLING) {  // W_eff = Rd W
+                float We[9];
+                matmul<3, 3, 3>(Rd, Wm, We);
+#pragma unroll
+                for (int k = 0; k < 9; ++k) Wm[k] = We[k];
+            }
             float WT[9], JW[6], JWS[6], JWSW[6], JT[6], cov[4];
 #pragma unroll
             for (int a = 0; a < 3; ++a)
@@ -504,6 +536,7 @@ __device__ __forceinline__ void preprocess_body(const PreParams p, const LensPar
     const long long off = (long long)(excl >> CNT_SHIFT);
     const long long key_base = (long long)(excl & ((1ull << CNT_SHIFT) - 1));
     if (i < p.N) p.point_offset[i] = in ? (int)off : -1;
+    if (ROLLING && i < p.N) rs.row_time[i] = in ? tau : 0.0f;
     if (in) {
         p.point_id[off] = (int)i;
         p.num_tiles[off] = ntiles;
@@ -590,8 +623,20 @@ preprocess_lens_kernel(const PreLensParams p) {
     preprocess_body<KeyT, LENS>(p, p.lens);
 }
 
+// The parameter block of the rolling-shutter instantiations (LENS = GSB_LENS_PINHOLE ignores `lens`).
+struct PreRsParams : PreLensParams {
+    RsParams rs;
+};
+
+template <typename KeyT, int LENS>
+__global__ void __launch_bounds__(SCAN_BLOCK_THREADS, GSB_PRE_MIN_BLOCKS)
+preprocess_rs_kernel(const PreRsParams p) {
+    preprocess_body<KeyT, LENS, true>(p, p.lens, p.rs);
+}
+
 #ifndef GSB_HOST_EMU  // tests/simt compiles the kernels above as host C++ under the SIMT emulator
-int launch_preprocess(const GsbForwardArgs &a, const Workspace &ws, cudaStream_t stream, const LensParams *lens) {
+int launch_preprocess(const GsbForwardArgs &a, const Workspace &ws, cudaStream_t stream, const LensParams *lens,
+                      const RsParams *rs) {
     const GsbWorkspaceLayout &L = ws.layout;
     {
         // per-frame state to zero: [counters, sort_state) and [tile_start, zero_bytes) -- every offset is 256-B aligned
@@ -636,7 +681,23 @@ int launch_preprocess(const GsbForwardArgs &a, const Workspace &ws, cudaStream_t
     p.point_in_camera = ws.point_in_camera;
     p.keys = ws.keys_a;
     p.vals = ws.vals_a;
-    if (lens != nullptr) {
+    if (rs != nullptr) {
+        PreRsParams pr;
+        static_cast<PreParams &>(pr) = p;
+        pr.lens = lens != nullptr ? *lens : LensParams();
+        pr.rs = *rs;
+        const int model = lens != nullptr ? lens->model : GSB_LENS_PINHOLE;
+        const dim3 grid(L.scan_blocks), block(SCAN_BLOCK_THREADS);
+        if (L.key_bytes == 4) {
+            if (model == GSB_LENS_FISHEYE) preprocess_rs_kernel<unsigned int, GSB_LENS_FISHEYE><<<grid, block, 0, stream>>>(pr);
+            else if (model == GSB_LENS_OPENCV) preprocess_rs_kernel<unsigned int, GSB_LENS_OPENCV><<<grid, block, 0, stream>>>(pr);
+            else preprocess_rs_kernel<unsigned int, GSB_LENS_PINHOLE><<<grid, block, 0, stream>>>(pr);
+        } else {
+            if (model == GSB_LENS_FISHEYE) preprocess_rs_kernel<unsigned long long, GSB_LENS_FISHEYE><<<grid, block, 0, stream>>>(pr);
+            else if (model == GSB_LENS_OPENCV) preprocess_rs_kernel<unsigned long long, GSB_LENS_OPENCV><<<grid, block, 0, stream>>>(pr);
+            else preprocess_rs_kernel<unsigned long long, GSB_LENS_PINHOLE><<<grid, block, 0, stream>>>(pr);
+        }
+    } else if (lens != nullptr) {
         PreLensParams pl;
         static_cast<PreParams &>(pl) = p;
         pl.lens = *lens;

@@ -22,6 +22,10 @@ the image by nearest neighbour.
 An optional record key ``distortion`` (an extension), ``{"model": "opencv" | "fisheye", "coefficients": [...]}``, gives the
 view's ``CameraInfo.distortion`` (``Camera.LensDistortion``).  The coefficients act on the normalised image plane, so
 rescaling, cropping and autoscale leave them unchanged.
+An optional record key ``rolling_shutter`` (an extension), ``{"linear_velocity": [3], "angular_velocity": [3],
+"readout_time": s}``, gives the view's ``CameraInfo.rolling_shutter`` (``Camera.RollingShutter.from_camera_velocity``: the
+camera's own velocities in its frame, in scene units/s and rad/s, as visual-inertial odometry reports them, and the sensor's
+top-to-bottom readout time).  Row time is normalised by the image height, so rescaling and autoscale keep the motion.
 Pinned against the reference class itself: ``tests/golden/make_dataset_golden.py`` imports it (Taichi stubbed) and
 stores its outputs for a small generated dataset; ``tests/test_dataset_cpu.py`` compares.
 """
@@ -33,7 +37,7 @@ import numpy as np
 import torch
 import torch.utils.data
 
-from .Camera import CameraInfo, LensDistortion
+from .Camera import CameraInfo, LensDistortion, RollingShutter
 from .GaussianPointCloudRasterisation import TILE_HEIGHT, TILE_WIDTH
 from .loss import SupervisionTargets
 from .utils import SE3_to_quaternion_and_translation_torch
@@ -87,7 +91,8 @@ class ImagePoseDataset(torch.utils.data.Dataset):
         K[1, 1] *= sy
         K[1, 2] *= sy
         return resized, CameraInfo(camera_intrinsics=K, camera_height=resized.shape[1], camera_width=resized.shape[2],
-                                   camera_id=camera_info.camera_id, distortion=camera_info.distortion)
+                                   camera_id=camera_info.camera_id, distortion=camera_info.distortion,
+                                   rolling_shutter=camera_info.rolling_shutter)
 
     @staticmethod
     def _distortion(rec: dict) -> Optional[LensDistortion]:
@@ -98,6 +103,20 @@ class ImagePoseDataset(torch.utils.data.Dataset):
         if not isinstance(d, dict) or "model" not in d or "coefficients" not in d:
             raise ValueError(f'"distortion" must be {{"model": ..., "coefficients": [...]}}, got {d!r}')
         return LensDistortion(d["model"], tuple(d["coefficients"]))
+
+    @staticmethod
+    def _rolling_shutter(rec: dict) -> Optional[RollingShutter]:
+        """The optional record key ``"rolling_shutter": {"linear_velocity": [3], "angular_velocity": [3], "readout_time": s}``."""
+        r = rec.get("rolling_shutter")
+        if r is None:
+            return None
+        keys = ("linear_velocity", "angular_velocity", "readout_time")
+        if not isinstance(r, dict) or any(k not in r for k in keys):
+            raise ValueError(f'"rolling_shutter" must be {{"linear_velocity": [3], "angular_velocity": [3], "readout_time": s}}, '
+                             f'got {r!r}')
+        if len(r["linear_velocity"]) != 3 or len(r["angular_velocity"]) != 3:
+            raise ValueError(f'"rolling_shutter" velocities take 3 values each, got {r!r}')
+        return RollingShutter.from_camera_velocity(r["linear_velocity"], r["angular_velocity"], r["readout_time"])
 
     def _path(self, path: str) -> str:
         if not os.path.isabs(path) and not os.path.exists(path):
@@ -186,7 +205,8 @@ class ImagePoseDataset(torch.utils.data.Dataset):
             targets = self._load_targets(rec, image.shape[1], image.shape[2])
         image = _crop_to_tiles(image)
         info = CameraInfo(camera_intrinsics=K, camera_height=image.shape[1], camera_width=image.shape[2],
-                          camera_id=rec["camera_id"], distortion=self._distortion(rec))
+                          camera_id=rec["camera_id"], distortion=self._distortion(rec),
+                          rolling_shutter=self._rolling_shutter(rec))
         image, info = self._autoscale_image_and_camera_info(image, info)
         if self.with_targets:
             return image, q, t, info, self._crop_and_scale_targets(*targets, info)

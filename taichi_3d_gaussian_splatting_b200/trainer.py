@@ -24,6 +24,10 @@ downsampled camera keeps the coefficients (they act on the normalised image plan
 intrinsics refinement.
 Optional lens refinement (an extension; ``TrainConfig.distortion_learning_rate``): per camera with a lens, its coefficients,
 differentiated by the operator's ``differentiable_distortion`` and stepped by their own Adam.
+Views with a rolling shutter (an extension; ``CameraInfo.rolling_shutter``) train through it in the autograd loop; the
+downsampled camera keeps the motion (row time is normalised by the image height).  Not with ``fused_step``, pose, intrinsics
+or lens refinement.  Optional motion refinement (``TrainConfig.rolling_shutter_learning_rate``): per rolling-shutter view, its
+motion (v, w), differentiated by the operator's ``differentiable_rolling_shutter`` and stepped by its own Adam.
 The rasteriser is injected (default: the CUDA operator) so that tests can run the identical loop with the
 CPU oracle behind the same interface and compare PSNR trajectories.
 """
@@ -34,7 +38,7 @@ from typing import Callable, List, Optional, Tuple
 import torch
 import torch.nn.functional as F
 
-from .Camera import CameraInfo, LensDistortion
+from .Camera import CameraInfo, LensDistortion, RollingShutter
 from .densification import GaussianPointAdaptiveController
 from .GaussianPointCloudRasterisation import GaussianPointCloudRasterisation
 from .loss import FEATURE_LOSSES, LossFunction, SupervisionTargets, feature_loss, supervision_loss
@@ -62,9 +66,10 @@ def downsample_image_and_camera_info(image: torch.Tensor, camera_info: CameraInf
     K[1, 1] /= downsample_factor
     K[0, 2] /= downsample_factor
     K[1, 2] /= downsample_factor
-    # the lens coefficients act on the normalised image plane: resizing does not change them
+    # the lens coefficients act on the normalised image plane and row time is normalised by the height: resizing changes
+    # neither the lens nor the rolling-shutter motion
     return image, CameraInfo(camera_intrinsics=K, camera_height=h, camera_width=w, camera_id=camera_info.camera_id,
-                             distortion=camera_info.distortion)
+                             distortion=camera_info.distortion, rolling_shutter=camera_info.rolling_shutter)
 
 
 def _nearest(x: torch.Tensor, h: int, w: int, hc: int, wc: int) -> torch.Tensor:
@@ -149,6 +154,10 @@ class GaussianPointCloudTrainer:
         # and trained by its own Adam at this rate.  The views of one camera_id must share their lens.  Not with fused_step,
         # pose or intrinsics refinement (no distorted view combines with them).
         distortion_learning_rate: float = 0.
+        # optional motion refinement: > 0 gives every training view with a rolling shutter (CameraInfo.rolling_shutter) one
+        # (6,) leaf tensor of its motion (v, w), initialised from the view's, kept on the host and trained by its own Adam at
+        # this rate.  Not with fused_step, pose, intrinsics or lens refinement (no rolling-shutter view combines with them).
+        rolling_shutter_learning_rate: float = 0.
 
     def __init__(self, config: "GaussianPointCloudTrainer.TrainConfig", scene: Scene, train_views: List[View],
                  rasterisation_factory: Optional[Callable] = None, generator: Optional[torch.Generator] = None,
@@ -209,6 +218,15 @@ class GaussianPointCloudTrainer:
                                                                  requires_grad=True)
         self._distortion = self._distortion_leaves(config, train_views)
         self._dist = config.distortion_learning_rate > 0
+        # a view with a rolling shutter (CameraInfo.rolling_shutter) trains through the autograd loop alone
+        if any(getattr(v[3], "rolling_shutter", None) is not None for v in train_views):
+            for name, on in (("fused_step", fused_step), ("pose refinement (pose_learning_rate > 0)", self._pose),
+                             ("intrinsics refinement (intrinsics_learning_rate > 0)", self._intr),
+                             ("distortion refinement (distortion_learning_rate > 0)", self._dist)):
+                if on:
+                    raise ValueError(f"{name} is not supported with a rolling-shutter view (CameraInfo.rolling_shutter)")
+        self._rolling_shutter = self._rolling_shutter_leaves(config, train_views)
+        self._rs = config.rolling_shutter_learning_rate > 0
         self._features = config.feature_loss != "none"
         if self._features:
             self._check_feature_config(config, scene, targets)
@@ -242,7 +260,8 @@ class GaussianPointCloudTrainer:
                      **({"differentiable_alpha": True} if self._need_alpha else {}),
                      **({"differentiable_pose": True} if self._pose else {}),
                      **({"differentiable_intrinsics": True} if self._intr else {}),
-                     **({"differentiable_distortion": True} if self._dist else {}))
+                     **({"differentiable_distortion": True} if self._dist else {}),
+                     **({"differentiable_rolling_shutter": True} if self._rs else {}))
         self.rasterisation = factory(config=config.rasterisation_config,
                                      backward_valid_point_hook=self.adaptive_controller.update, **extra)
         self.loss_function = LossFunction(config=config.loss_function_config)
@@ -270,6 +289,22 @@ class GaussianPointCloudTrainer:
                   for cid, (lens,) in lenses.items() if lens is not None}
         if not leaves:
             raise ValueError("distortion_learning_rate > 0 needs a distorted training view (CameraInfo.distortion)")
+        return leaves
+
+    @staticmethod
+    def _rolling_shutter_leaves(config, train_views: List[View]) -> dict:
+        """The trainable motions, one float32 host leaf (6,) per rolling-shutter view, keyed by view index ({} when motion
+        refinement is off)."""
+        rate = config.rolling_shutter_learning_rate
+        if not (rate >= 0.0 and rate < float("inf")):
+            raise ValueError(f"rolling_shutter_learning_rate must be finite and >= 0, got {rate}")
+        if rate == 0:
+            return {}
+        leaves = {i: torch.tensor(v[3].rolling_shutter.motion, dtype=torch.float32, requires_grad=True)
+                  for i, v in enumerate(train_views) if getattr(v[3], "rolling_shutter", None) is not None}
+        if not leaves:
+            raise ValueError("rolling_shutter_learning_rate > 0 needs a rolling-shutter training view "
+                             "(CameraInfo.rolling_shutter)")
         return leaves
 
     @staticmethod
@@ -431,6 +466,9 @@ class GaussianPointCloudTrainer:
         # host tensors: torch's Adam whatever fused_adam says
         distortion_optimizer = torch.optim.Adam(list(self._distortion.values()), lr=cfg.distortion_learning_rate,
                                                 betas=(0.9, 0.999)) if self._dist else None
+        rolling_shutter_optimizer = torch.optim.Adam(list(self._rolling_shutter.values()),
+                                                     lr=cfg.rolling_shutter_learning_rate, betas=(0.9, 0.999)) \
+            if self._rs else None
         scheduler = torch.optim.lr_scheduler.ExponentialLR(position_optimizer, gamma=cfg.position_learning_rate_decay_rate)
         downsample_factor = cfg.initial_downsample_factor
         for iteration in range(cfg.num_iterations):
@@ -446,6 +484,8 @@ class GaussianPointCloudTrainer:
                 intrinsics_optimizer.zero_grad()
             if distortion_optimizer is not None:
                 distortion_optimizer.zero_grad()
+            if rolling_shutter_optimizer is not None:
+                rolling_shutter_optimizer.zero_grad()
             view_index = self._next_view_index(iteration)
             image_gt, q, t, camera_info, targets = self._view(view_index, downsample_factor)
             if self._intr:  # built every iteration: the cached downsampled camera must not freeze K
@@ -460,6 +500,14 @@ class GaussianPointCloudTrainer:
                                          camera_id=camera_info.camera_id,
                                          distortion=LensDistortion(camera_info.distortion.model, leaf.detach().tolist()))
                 lens_kw = {"lens_coefficients": leaf}
+            if self._rs and view_index in self._rolling_shutter:  # the motion as trained, the leaf as the autograd input
+                leaf = self._rolling_shutter[view_index]
+                values = leaf.detach().tolist()
+                camera_info = CameraInfo(camera_intrinsics=camera_info.camera_intrinsics,
+                                         camera_height=camera_info.camera_height, camera_width=camera_info.camera_width,
+                                         camera_id=camera_info.camera_id, distortion=camera_info.distortion,
+                                         rolling_shutter=RollingShutter(values[:3], values[3:]))
+                lens_kw = {"rolling_shutter_motion": leaf}
             band = iteration // cfg.increase_color_max_sh_band_interval
             if self.supervised or self._features:
                 loss, l1_loss, mask_term, depth_term, feature_term, image_pred = self._supervised_loss(
@@ -490,6 +538,8 @@ class GaussianPointCloudTrainer:
                 intrinsics_optimizer.step()
             if distortion_optimizer is not None:
                 distortion_optimizer.step()
+            if rolling_shutter_optimizer is not None:
+                rolling_shutter_optimizer.step()
             if iteration % cfg.position_learning_rate_decay_interval == 0:
                 scheduler.step()
             self.adaptive_controller.refinement()
@@ -556,6 +606,18 @@ class GaussianPointCloudTrainer:
             if lens is not None and ci.camera_id in self._distortion:
                 lens = LensDistortion(lens.model, self._distortion[ci.camera_id].detach().tolist())
             out.append(lens)
+        return out
+
+    def refined_rolling_shutter(self) -> List[Optional[RollingShutter]]:
+        """The rolling shutter of every training view as trained (None for a view without one; the views' own motions
+        without motion refinement)."""
+        out = []
+        for i, v in enumerate(self.train_views):
+            rs = getattr(v[3], "rolling_shutter", None)
+            if rs is not None and i in self._rolling_shutter:
+                values = self._rolling_shutter[i].detach().tolist()
+                rs = RollingShutter(values[:3], values[3:])
+            out.append(rs)
         return out
 
     @torch.no_grad()
