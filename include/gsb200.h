@@ -206,7 +206,7 @@ const char *gsb200_last_error(void);
 void gsb200_abi_sizes(int64_t *out3);
 /* ... and of the first n of {GsbWorkspaceLayout, GsbForwardArgs, GsbBackwardArgs, GsbExpandArgs, GsbTrainStepArgs,
  * GsbSupervisionArgs, GsbExtraFeatureArgs, GsbFeatureTrainArgs, GsbPoseGradArgs, GsbIntrinsicsGradArgs, GsbLensArgs,
- * GsbLensGradArgs, GsbRollingShutterArgs, GsbRollingShutterGradArgs} */
+ * GsbLensGradArgs, GsbRollingShutterArgs, GsbRollingShutterGradArgs, GsbAppearanceArgs} */
 void gsb200_abi_sizes_ext(int64_t *out, int32_t n);
 
 /* Workspace sizing.  far_plane*depth_to_sort_key_scale fixes the depth-key width; (H/16)*(W/16)
@@ -580,6 +580,60 @@ int64_t gsb200_feature_loss_temp_bytes(int32_t camera_height, int32_t camera_wid
  * GSB_FLAG_COMPACT_GRADS.  Deterministic: fixed grids and summation orders. */
 int gsb200_train_step_ext(const GsbTrainStepArgs *args, const GsbSupervisionArgs *supervision,
                           const GsbFeatureTrainArgs *features);
+
+/* Per-view appearance compensation (an extension): a bilateral grid (Wang et al., "Bilateral Guided Radiance Field
+ * Processing", SIGGRAPH 2024) of one view, G with shape (12, Gz, Gy, Gx), float32, contiguous: a 3x4 affine [A | b] (row-major)
+ * per node, Gx / Gy nodes across the image width / height, Gz over luminance; 1 <= Gx, Gy <= 64, 1 <= Gz <= 16.  For an
+ * image I (H,W,3), at pixel (px, py) with colour c:
+ *   gx = px (Gx-1) / max(W-1, 1),  gy = py (Gy-1) / max(H-1, 1)
+ *   lum = clamp(0.299 c_r + 0.587 c_g + 0.114 c_b, 0, 1),  gz = lum (Gz-1)
+ *   [A | b] = trilinear interpolation of G at (gx, gy, gz), the lower corner index clamped to n-2;  out = A c + b
+ * -- exactly F.grid_sample(G[None], (x, y, 2 lum - 1) in [-1, 1], mode="bilinear", align_corners=True,
+ * padding_mode="border").  The identity grid (A = I, b = 0) reproduces the image.  The backward gives dL/dG and dL/dc, the
+ * latter through A and, where 0 < lum < 1, through lum (the slope of the interpolation along z times (Gz-1) times
+ * (0.299, 0.587, 0.114)).  The TV prior is tv(G) = sum over the x, y and z axes of mean((G[i+1] - G[i])^2); an axis with one
+ * node contributes 0.  Deterministic: dL/dG is summed per grid cell in a fixed order, with no float atomics. */
+#define GSB_BILATERAL_GRID_MAX_XY 64
+#define GSB_BILATERAL_GRID_MAX_Z 16
+/* bytes of the backward's temp (per-CTA partial sums of dL/dG); 0 for a shape outside the limits */
+int64_t gsb200_bilateral_grid_temp_bytes(int32_t camera_height, int32_t camera_width, int32_t grid_x, int32_t grid_y,
+                                         int32_t grid_z);
+/* image_out (H,W,3) = the slice of `grid` applied to image (H,W,3).  GSB_EINVAL, before any CUDA call, for a shape outside
+ * the limits or a NULL or not 4-byte aligned pointer. */
+int gsb200_bilateral_grid_forward(const float *image, const float *grid, int32_t camera_height, int32_t camera_width,
+                                  int32_t grid_x, int32_t grid_y, int32_t grid_z, float *image_out, void *stream);
+/* From dL/dout (H,W,3): grad_image (H,W,3) = dL/dimage (it may alias grad_image_out: each pixel is read before it is
+ * written) and grad_grid (12,Gz,Gy,Gx) = dL/dG (overwritten).  GSB_EINVAL, before any CUDA call, for a shape outside the
+ * limits, a NULL or not 4-byte aligned pointer, or a temp that is NULL, not 16-byte aligned or smaller than
+ * gsb200_bilateral_grid_temp_bytes. */
+int gsb200_bilateral_grid_backward(const float *image, const float *grid, int32_t camera_height, int32_t camera_width,
+                                   int32_t grid_x, int32_t grid_y, int32_t grid_z, const float *grad_image_out,
+                                   float *grad_image, float *grad_grid, void *temp, int64_t temp_bytes, void *stream);
+
+/* The appearance grid of the view a fused train step trains on. */
+typedef struct GsbAppearanceArgs {
+    float *grid;                  /* (12,Gz,Gy,Gx) this view's grid, updated in place by its Adam step */
+    float *grad_grid;             /* (12,Gz,Gy,Gx) out: dL/dG (slice and TV) */
+    int32_t grid_x, grid_y, grid_z;
+    float tv_weight;              /* >= 0, finite */
+    float *exp_avg, *exp_avg_sq;  /* (12,Gz,Gy,Gx) this view's Adam moments, zero before its first step */
+    double learning_rate;         /* >= 0, finite; betas and eps are the train step's */
+    int32_t step;                 /* this view's own 1-based Adam step count */
+    float *image;                 /* (H,W,3) scratch: the sliced image I'' the image loss reads */
+    void *temp;                   /* gsb200_bilateral_grid_temp_bytes(H, W, Gx, Gy, Gz) bytes, 16-byte aligned */
+    int64_t temp_bytes;
+    float *loss_out1;             /* device: {tv_weight * tv(G)} */
+} GsbAppearanceArgs;
+/* gsb200_train_step_ext with the view's appearance grid: forward -> supervision pre-pass -> slice I'' = grid(I') of the image
+ * the loss would read (I' = I + (1 - S) bg with a background, else I) -> image loss on I'' -> slice backward (dL/dG, and
+ * dL/dI' in place over the image-loss gradient) -> TV (added into dL/dG, loss_out1) -> supervision post-pass (reads dL/dI')
+ * -> feature loss -> backward -> the Adam steps, then Adam on the grid; all of them skipped on the device after a
+ * key-capacity overflow.  The depth, mask and feature terms do not see the grid.  NULL appearance: exactly
+ * gsb200_train_step_ext.  GSB_EINVAL, before any CUDA call, for a shape outside the limits, a NULL or not 16-byte aligned
+ * grid, gradient, moment, image or temp pointer, a NULL loss_out1, a temp smaller than gsb200_bilateral_grid_temp_bytes,
+ * step < 1, or a TV weight or learning rate that is negative or not finite.  Deterministic. */
+int gsb200_train_step_appearance(const GsbTrainStepArgs *args, const GsbSupervisionArgs *supervision,
+                                 const GsbFeatureTrainArgs *features, const GsbAppearanceArgs *appearance);
 
 /* Individual stages (same workspace), for tests and profiling. */
 int gsb200_stage_preprocess(const GsbForwardArgs *args);   /* K1+P1+K2+K3+P2+K4 fused */

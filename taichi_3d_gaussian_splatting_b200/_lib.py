@@ -139,6 +139,14 @@ class GsbRollingShutterGradArgs(ctypes.Structure):
     _fields_ = [("grad_motion", c_vp), ("temp", c_vp)]
 
 
+class GsbAppearanceArgs(ctypes.Structure):
+    _fields_ = [
+        ("grid", c_vp), ("grad_grid", c_vp), ("grid_x", c_i32), ("grid_y", c_i32), ("grid_z", c_i32), ("tv_weight", c_f32),
+        ("exp_avg", c_vp), ("exp_avg_sq", c_vp), ("learning_rate", ctypes.c_double), ("step", c_i32), ("image", c_vp),
+        ("temp", c_vp), ("temp_bytes", c_i64), ("loss_out1", c_vp),
+    ]
+
+
 def lens_args(distortion) -> GsbLensArgs:
     """The C argument of a ``Camera.LensDistortion`` (host floats; unused coefficients 0)."""
     model = {"opencv": GSB_LENS_OPENCV, "fisheye": GSB_LENS_FISHEYE}[distortion.model]
@@ -171,7 +179,8 @@ EXPORTS = (
     "gsb200_backward_ext", "gsb200_feature_loss_temp_bytes", "gsb200_train_step_ext", "gsb200_backward_pose",
     "gsb200_pose_grad_temp_bytes", "gsb200_backward_calib", "gsb200_intrinsics_grad_temp_bytes", "gsb200_forward_lens",
     "gsb200_backward_lens", "gsb200_backward_lens_grad", "gsb200_lens_grad_temp_bytes", "gsb200_forward_rolling_shutter",
-    "gsb200_backward_rolling_shutter", "gsb200_rolling_shutter_grad_temp_bytes",
+    "gsb200_backward_rolling_shutter", "gsb200_rolling_shutter_grad_temp_bytes", "gsb200_bilateral_grid_temp_bytes",
+    "gsb200_bilateral_grid_forward", "gsb200_bilateral_grid_backward", "gsb200_train_step_appearance",
 )
 
 _lib = None
@@ -271,6 +280,15 @@ def load() -> ctypes.CDLL:
     lib.gsb200_train_step_ext.argtypes = [ctypes.POINTER(GsbTrainStepArgs), ctypes.POINTER(GsbSupervisionArgs),
                                           ctypes.POINTER(GsbFeatureTrainArgs)]
     lib.gsb200_train_step_ext.restype = ctypes.c_int
+    lib.gsb200_train_step_appearance.argtypes = [ctypes.POINTER(GsbTrainStepArgs), ctypes.POINTER(GsbSupervisionArgs),
+                                                 ctypes.POINTER(GsbFeatureTrainArgs), ctypes.POINTER(GsbAppearanceArgs)]
+    lib.gsb200_train_step_appearance.restype = ctypes.c_int
+    lib.gsb200_bilateral_grid_temp_bytes.argtypes = [c_i32] * 5
+    lib.gsb200_bilateral_grid_temp_bytes.restype = c_i64
+    lib.gsb200_bilateral_grid_forward.argtypes = [c_vp, c_vp] + [c_i32] * 5 + [c_vp, c_vp]
+    lib.gsb200_bilateral_grid_forward.restype = ctypes.c_int
+    lib.gsb200_bilateral_grid_backward.argtypes = [c_vp, c_vp] + [c_i32] * 5 + [c_vp, c_vp, c_vp, c_vp, c_i64, c_vp]
+    lib.gsb200_bilateral_grid_backward.restype = ctypes.c_int
     lib.gsb200_feature_loss_temp_bytes.argtypes = [c_i32, c_i32]
     lib.gsb200_feature_loss_temp_bytes.restype = c_i64
     lib.gsb200_supervision_temp_bytes.argtypes = [c_i32, c_i32]
@@ -343,6 +361,11 @@ def load() -> ctypes.CDLL:
         if sizes14[i] != ctypes.sizeof(mirror):
             raise RuntimeError(f"libgsb200.so ABI mismatch: sizeof({mirror.__name__}) {sizes14[i]} != ctypes mirror "
                                f"{ctypes.sizeof(mirror)}")
+    sizes15 = (c_i64 * 15)()
+    lib.gsb200_abi_sizes_ext(sizes15, 15)
+    if sizes15[14] != ctypes.sizeof(GsbAppearanceArgs):
+        raise RuntimeError(f"libgsb200.so ABI mismatch: sizeof(GsbAppearanceArgs) {sizes15[14]} != ctypes mirror "
+                           f"{ctypes.sizeof(GsbAppearanceArgs)}")
     _lib = lib
     return lib
 

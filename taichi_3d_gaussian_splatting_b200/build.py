@@ -32,6 +32,7 @@ SOURCES = {
     "image_loss.cu": [],
     "supervision_loss.cu": [],
     "feature_loss.cu": [],
+    "appearance.cu": [],
     "adam.cu": [],
     "controller.cu": [],
     "exchange.cu": [],

@@ -192,13 +192,13 @@ void gsb200_abi_sizes(int64_t *out3) {
 }
 
 void gsb200_abi_sizes_ext(int64_t *out, int32_t n) {
-    const int64_t all[14] = {(int64_t)sizeof(GsbWorkspaceLayout), (int64_t)sizeof(GsbForwardArgs), (int64_t)sizeof(GsbBackwardArgs),
+    const int64_t all[15] = {(int64_t)sizeof(GsbWorkspaceLayout), (int64_t)sizeof(GsbForwardArgs), (int64_t)sizeof(GsbBackwardArgs),
                              (int64_t)sizeof(GsbExpandArgs), (int64_t)sizeof(GsbTrainStepArgs), (int64_t)sizeof(GsbSupervisionArgs),
                              (int64_t)sizeof(GsbExtraFeatureArgs), (int64_t)sizeof(GsbFeatureTrainArgs),
                              (int64_t)sizeof(GsbPoseGradArgs), (int64_t)sizeof(GsbIntrinsicsGradArgs), (int64_t)sizeof(GsbLensArgs),
                              (int64_t)sizeof(GsbLensGradArgs), (int64_t)sizeof(GsbRollingShutterArgs),
-                             (int64_t)sizeof(GsbRollingShutterGradArgs)};
-    for (int i = 0; i < n && i < 14; ++i) out[i] = all[i];
+                             (int64_t)sizeof(GsbRollingShutterGradArgs), (int64_t)sizeof(GsbAppearanceArgs)};
+    for (int i = 0; i < n && i < 15; ++i) out[i] = all[i];
 }
 
 int gsb200_workspace_layout(int64_t num_points, int32_t num_objects, int64_t key_capacity,
@@ -677,7 +677,44 @@ static int check_feature_train_args(const GsbFeatureTrainArgs &x, const GsbBackw
     return GSB_OK;
 }
 
+// The appearance grid's own rules (gsb200_train_step_appearance); the frame's were checked before.
+static int check_appearance_args(const GsbAppearanceArgs &a, int H, int W) {
+    if (a.grid_x < 1 || a.grid_x > GSB_BILATERAL_GRID_MAX_XY || a.grid_y < 1 || a.grid_y > GSB_BILATERAL_GRID_MAX_XY ||
+        a.grid_z < 1 || a.grid_z > GSB_BILATERAL_GRID_MAX_Z) {
+        set_error("train_step_appearance: the grid must have 1 <= Gx, Gy <= %d and 1 <= Gz <= %d nodes (got %dx%dx%d)",
+                  GSB_BILATERAL_GRID_MAX_XY, GSB_BILATERAL_GRID_MAX_Z, a.grid_x, a.grid_y, a.grid_z);
+        return GSB_EINVAL;
+    }
+    if (!weight_ok(a.tv_weight) || !(a.learning_rate >= 0.0 && a.learning_rate <= 1.7976931348623157e308)) {
+        set_error("train_step_appearance: the TV weight and the learning rate must be finite and >= 0 (got %g, %g)",
+                  (double)a.tv_weight, a.learning_rate);
+        return GSB_EINVAL;
+    }
+    if (a.step < 1) {
+        set_error("train_step_appearance: the grid's step must be >= 1 (got %d)", a.step);
+        return GSB_EINVAL;
+    }
+    if (!a.grid || !a.grad_grid || !a.exp_avg || !a.exp_avg_sq || !a.image || !a.loss_out1 || !aligned16(a.grid) ||
+        !aligned16(a.grad_grid) || !aligned16(a.exp_avg) || !aligned16(a.exp_avg_sq) || !aligned16(a.image)) {
+        set_error("train_step_appearance: grid, grad_grid, exp_avg, exp_avg_sq and image must be 16-byte aligned, "
+                  "loss_out1 not NULL");
+        return GSB_EINVAL;
+    }
+    if (!a.temp || !aligned16(a.temp) ||
+        a.temp_bytes < gsb200_bilateral_grid_temp_bytes(H, W, a.grid_x, a.grid_y, a.grid_z)) {
+        set_error("train_step_appearance: temp null, not 16-byte aligned or smaller than gsb200_bilateral_grid_temp_bytes "
+                  "(temp_bytes=%lld)", (long long)a.temp_bytes);
+        return GSB_EINVAL;
+    }
+    return GSB_OK;
+}
+
 int gsb200_train_step_ext(const GsbTrainStepArgs *t, const GsbSupervisionArgs *s, const GsbFeatureTrainArgs *x) {
+    return gsb200_train_step_appearance(t, s, x, nullptr);
+}
+
+int gsb200_train_step_appearance(const GsbTrainStepArgs *t, const GsbSupervisionArgs *s, const GsbFeatureTrainArgs *x,
+                                 const GsbAppearanceArgs *app) {
     if (!t || !t->ground_truth_image || !t->loss_out3 || !t->loss_temp || !t->feature_exp_avg || !t->feature_exp_avg_sq ||
         !t->position_exp_avg || !t->position_exp_avg_sq || t->step < 1) {
         set_error("train_step: null pointer argument or step < 1");
@@ -741,6 +778,7 @@ int gsb200_train_step_ext(const GsbTrainStepArgs *t, const GsbSupervisionArgs *s
     const int H = f.camera_height, W = f.camera_width;
     int rc;
     if (x && (rc = check_feature_train_args(*x, b, H, W)) != GSB_OK) return rc;
+    if (app && (rc = check_appearance_args(*app, H, W)) != GSB_OK) return rc;
     const GsbExtraFeatureArgs *ext = x ? &x->features : nullptr;
     cudaStream_t st = static_cast<cudaStream_t>(f.stream);
     if ((rc = gsb200_forward_ext(&f, ext)) != GSB_OK) return rc;
@@ -748,9 +786,21 @@ int gsb200_train_step_ext(const GsbTrainStepArgs *t, const GsbSupervisionArgs *s
     if (supervised && (rc = launch_supervision_pre(*s, f.rasterized_image, t->ground_truth_image, f.pixel_accumulated_alpha,
                                                    f.rasterized_depth, H, W, st, &loss_image, &loss_gt)) != GSB_OK)
         return rc;
-    rc = gsb200_image_loss(loss_image, loss_gt, H, W, t->lambda_value, 1.0f, t->loss_out3,
+    const float *sliced_image = loss_image;  // I'' (the image loss's input)
+    if (app) {
+        if ((rc = launch_bilateral_grid_forward(loss_image, app->grid, H, W, app->grid_x, app->grid_y, app->grid_z, app->image,
+                                                st)) != GSB_OK)
+            return rc;
+        sliced_image = app->image;
+    }
+    rc = gsb200_image_loss(sliced_image, loss_gt, H, W, t->lambda_value, 1.0f, t->loss_out3,
                            const_cast<float *>(b.grad_rasterized_image), t->loss_temp, t->loss_temp_bytes, f.stream);
     if (rc != GSB_OK) return rc;
+    // dL/dG from dL/dI'' before dL/dI' replaces it in the same buffer; then the TV term into dL/dG
+    if (app && (rc = launch_bilateral_grid_backward(loss_image, app->grid, H, W, app->grid_x, app->grid_y, app->grid_z,
+                                                    b.grad_rasterized_image, const_cast<float *>(b.grad_rasterized_image),
+                                                    app->grad_grid, app->temp, app->tv_weight, app->loss_out1, st)) != GSB_OK)
+        return rc;
     if (supervised && (rc = launch_supervision_post(*s, f.rasterized_image, t->ground_truth_image, f.pixel_accumulated_alpha,
                                                     f.rasterized_depth, H, W, b.grad_rasterized_image, t->loss_out3, st)) != GSB_OK)
         return rc;
@@ -767,9 +817,15 @@ int gsb200_train_step_ext(const GsbTrainStepArgs *t, const GsbSupervisionArgs *s
     if (rc != GSB_OK) return rc;
     rc = launch_adam_step(const_cast<float *>(f.pointcloud), b.grad_pointcloud, t->position_exp_avg, t->position_exp_avg_sq,
                           (long long)f.num_points * 3, t->position_learning_rate, t->beta1, t->beta2, t->eps, t->step, skip, st);
-    if (rc != GSB_OK || !x) return rc;
-    return launch_adam_step(const_cast<float *>(ext->features), ext->grad_features, x->exp_avg, x->exp_avg_sq,
-                            (long long)f.num_points * ext->channels, x->learning_rate, t->beta1, t->beta2, t->eps, t->step, skip, st);
+    if (rc != GSB_OK) return rc;
+    if (x && (rc = launch_adam_step(const_cast<float *>(ext->features), ext->grad_features, x->exp_avg, x->exp_avg_sq,
+                                    (long long)f.num_points * ext->channels, x->learning_rate, t->beta1, t->beta2, t->eps,
+                                    t->step, skip, st)) != GSB_OK)
+        return rc;
+    if (!app) return GSB_OK;
+    return launch_adam_step(app->grid, app->grad_grid, app->exp_avg, app->exp_avg_sq,
+                            12LL * app->grid_z * app->grid_y * app->grid_x, app->learning_rate, t->beta1, t->beta2, t->eps,
+                            app->step, skip, st);
 }
 
 int gsb200_expand_view_gradients(const GsbExpandArgs *a) {

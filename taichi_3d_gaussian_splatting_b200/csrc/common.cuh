@@ -116,6 +116,12 @@ int launch_supervision_post(const GsbSupervisionArgs &s, const float *image, con
                             cudaStream_t stream);
 // feature_loss.cu: both passes of the feature term (arguments checked by gsb200_train_step_ext)
 int launch_feature_loss(const GsbFeatureTrainArgs &x, int H, int W, cudaStream_t stream);
+// appearance.cu: the bilateral-grid slice, its backward (+ the TV term when tv_out is set; arguments checked by the caller)
+int launch_bilateral_grid_forward(const float *image, const float *grid, int H, int W, int gx, int gy, int gz, float *out,
+                                  cudaStream_t stream);
+int launch_bilateral_grid_backward(const float *image, const float *grid, int H, int W, int gx, int gy, int gz,
+                                   const float *grad_out, float *grad_in, float *grad_grid, void *temp, float tv_weight,
+                                   float *tv_out, cudaStream_t stream);
 int launch_blend_forward_count(const GsbForwardArgs &a, const Workspace &ws, unsigned long long *counters_dev,
                                cudaStream_t stream);
 int launch_blend_backward_work(const GsbBackwardArgs &a, const Workspace &ws, unsigned long long *counters_dev,

@@ -18,6 +18,11 @@ an L1 mask loss on the accumulated alpha and training on a background colour, in
 Optional feature term (``extra_features``, ``feature_loss``, ``run(..., targets=SupervisionTargets(labels=... | features=...))``):
 per-Gaussian feature vectors F (N, C) rendered alongside the image, a cross-entropy or l2 loss on the rendered (H, W, C) map
 and an Adam step on F, in the same one call (``gsb200_train_step_ext``; ``loss.feature_loss`` states the loss in torch).
+
+Optional appearance grids (``appearance_grids``, ``run(..., appearance_view=i)``): one bilateral grid per training view
+(``appearance.apply_bilateral_grid``) slices the image the image loss reads, with a TV prior and an Adam step on the visited
+view's grid, in the same one call (``gsb200_train_step_appearance``).  Each view has its own Adam moments and its own step
+count, as torch's Adam gives one parameter per view that only steps when it has a gradient.
 """
 import ctypes
 import warnings
@@ -37,7 +42,9 @@ class FusedTrainStep:
     def __init__(self, scene, rasterisation_config, lambda_value: float = 0.2, controller=None, betas=(0.9, 0.999),
                  eps: float = 1e-8, key_capacity: Optional[int] = None, depth_weight: float = 0.0,
                  mask_weight: float = 0.0, extra_features: Optional[torch.Tensor] = None, feature_loss: Optional[str] = None,
-                 feature_weight: float = 1.0, extra_feature_learning_rate: float = 1e-2):
+                 feature_weight: float = 1.0, extra_feature_learning_rate: float = 1e-2,
+                 appearance_grids: Optional[torch.Tensor] = None, appearance_learning_rate: float = 2e-3,
+                 appearance_tv_weight: float = 10.0):
         """``scene``: object with ``point_cloud`` (N,3), ``point_cloud_features`` (N,56), ``point_invalid_mask``,
         ``point_object_id`` (CUDA, contiguous; updated in place).  ``controller``: a ``GaussianPointAdaptiveController`` whose
         six accumulators are updated by the backward epilogue (or ``None``).  ``depth_weight`` / ``mask_weight``: weights of
@@ -45,7 +52,9 @@ class FusedTrainStep:
         ``extra_features``: (N, C) float32 per-Gaussian feature vectors (CUDA, contiguous, 1 <= C <= 16; updated in place by
         their own Adam at ``extra_feature_learning_rate``), trained with ``feature_loss`` ("cross_entropy": needs
         ``targets.labels`` and C >= 2; "l2": needs ``targets.features``) weighted by ``feature_weight``
-        (``loss.feature_loss``)."""
+        (``loss.feature_loss``).  ``appearance_grids``: (V, 12, Gz, Gy, Gx) float32 per-view bilateral grids (CUDA,
+        contiguous; updated in place), trained at ``appearance_learning_rate`` with the TV weight ``appearance_tv_weight``;
+        ``run`` then needs ``appearance_view``."""
         for name, w in (("depth_weight", depth_weight), ("mask_weight", mask_weight)):
             if not (w >= 0.0 and w < float("inf")):
                 raise ValueError(f"{name} must be finite and >= 0, got {w}")
@@ -92,6 +101,17 @@ class FusedTrainStep:
                 raise ValueError(f"feature_weight must be finite and > 0, got {feature_weight}")
             self.extra_feature_exp_avg, self.extra_feature_exp_avg_sq = z(N, self.C), z(N, self.C)
             self.grad_extra_features = z(N, self.C)
+        self.appearance_grids = appearance_grids
+        if appearance_grids is not None:
+            self._check_appearance(appearance_grids, appearance_learning_rate, appearance_tv_weight)
+            self.appearance_learning_rate = float(appearance_learning_rate)
+            self.appearance_tv_weight = float(appearance_tv_weight)
+            V = appearance_grids.shape[0]
+            self.appearance_exp_avg = torch.zeros_like(appearance_grids)
+            self.appearance_exp_avg_sq = torch.zeros_like(appearance_grids)
+            self.appearance_steps = [0] * V  # each view's own Adam step count
+            self.grad_appearance_grid = torch.zeros_like(appearance_grids[0])
+        self.appearance_tv = z(1)  # {tv_weight * tv(G)} of the latest iteration with appearance (device)
         self._res = {}
         self._pinned = [torch.zeros(4, dtype=torch.int64).pin_memory() for _ in range(2)]
         self._events = [torch.cuda.Event() for _ in range(2)]
@@ -107,6 +127,18 @@ class FusedTrainStep:
         if F.dtype != torch.float32 or F.device != self.device or not F.is_contiguous() or F.data_ptr() % 16:
             raise ValueError(f"extra_features must be a contiguous, 16-byte aligned float32 tensor on {self.device}")
         return int(F.shape[1])
+
+    def _check_appearance(self, G, lr, tv_weight):
+        from .appearance import check_grid_shape
+        if not isinstance(G, torch.Tensor) or G.dim() != 5 or G.shape[0] < 1 or G.shape[1] != 12:
+            raise ValueError(f"appearance_grids must be a (V, 12, Gz, Gy, Gx) tensor, got "
+                             f"{tuple(G.shape) if isinstance(G, torch.Tensor) else type(G).__name__}")
+        check_grid_shape((G.shape[4], G.shape[3], G.shape[2]))
+        if G.dtype != torch.float32 or G.device != self.device or not G.is_contiguous() or G.data_ptr() % 16:
+            raise ValueError(f"appearance_grids must be a contiguous, 16-byte aligned float32 tensor on {self.device}")
+        for name, v in (("appearance_learning_rate", lr), ("appearance_tv_weight", tv_weight)):
+            if not (v >= 0.0 and v < float("inf")):
+                raise ValueError(f"{name} must be finite and >= 0, got {v}")
 
     # ------------------------------------------------------------------ per-resolution buffers
     def _buffers(self, H, W, n_obj):
@@ -130,6 +162,12 @@ class FusedTrainStep:
                 b.feature_map, b.grad_feature_map = e((H, W, self.C)), e((H, W, self.C))
                 b.feat_temp = torch.zeros((feat_bytes + 15) // 16 * 16, dtype=torch.uint8, device=dev)
                 b.feat_bytes = feat_bytes
+            if self.appearance_grids is not None:
+                gz, gy, gx = self.appearance_grids.shape[2:]
+                app_bytes = int(self._lib.gsb200_bilateral_grid_temp_bytes(H, W, gx, gy, gz))
+                b.sliced_image = e((H, W, 3))
+                b.app_temp = torch.zeros((app_bytes + 15) // 16 * 16, dtype=torch.uint8, device=dev)
+                b.app_bytes = app_bytes
             self._res[key] = b
         return b
 
@@ -150,12 +188,14 @@ class FusedTrainStep:
     # ------------------------------------------------------------------ one iteration
     def run(self, image_gt: torch.Tensor, q_pointcloud_camera: torch.Tensor, t_pointcloud_camera: torch.Tensor, camera_info,
             color_max_sh_band: int, feature_learning_rate: float, position_learning_rate: float,
-            targets: Optional[SupervisionTargets] = None, background: Optional[torch.Tensor] = None) -> None:
+            targets: Optional[SupervisionTargets] = None, background: Optional[torch.Tensor] = None,
+            appearance_view: Optional[int] = None) -> None:
         """``targets``: the view's depth and / or mask target ((H, W) float32 CUDA tensors) and, with ``extra_features``, its
         ``labels`` ((H, W) int32) or ``features`` ((H, W, C) float32); ``background``: a (3,) float32 CUDA tensor the image is
         composited on (read on the device when the step runs, so it may be refilled per iteration).  Without supervision
         terms or features this is ``gsb200_train_step``; with supervision terms ``gsb200_train_step_aux``; with features
-        ``gsb200_train_step_ext``."""
+        ``gsb200_train_step_ext``.  ``appearance_view``: with ``appearance_grids``, the index of the view whose grid slices
+        the image and takes an Adam step (``gsb200_train_step_appearance``)."""
         sc, cfg = self.scene, self.config
         H, W = int(camera_info.camera_height), int(camera_info.camera_width)
         if image_gt.shape != (3, H, W) or not image_gt.is_contiguous() or image_gt.dtype != torch.float32:
@@ -182,6 +222,13 @@ class FusedTrainStep:
                     or feat_t.device != image_gt.device:
                 raise ValueError(f'feature_loss "{self.feature_loss_kind}" needs {name}: a contiguous {dtype} {shape} '
                                  f"tensor on {image_gt.device}")
+        if self.appearance_grids is not None:
+            V = self.appearance_grids.shape[0]
+            if appearance_view is None or not 0 <= int(appearance_view) < V:
+                raise ValueError(f"appearance_grids needs appearance_view in 0..{V - 1}, got {appearance_view!r}")
+            appearance_view = int(appearance_view)
+        elif appearance_view is not None:
+            raise ValueError("appearance_view needs appearance_grids")
         self._check_previous()
         q, t = q_pointcloud_camera.contiguous(), t_pointcloud_camera.contiguous()
         K = camera_info.camera_intrinsics.contiguous()
@@ -237,6 +284,7 @@ class FusedTrainStep:
                     background=_ptr(background) if background is not None else None, depth_weight=self.depth_weight,
                     mask_weight=self.mask_weight, grad_depth=_ptr(b.grad_depth), grad_pixel_accumulated_alpha=_ptr(b.grad_alpha),
                     loss_out3=_ptr(self.supervision_loss), temp=_ptr(b.sup_temp), temp_bytes=b.sup_bytes)
+            fx = None
             if feat_t is not None:
                 ext = _lib.GsbExtraFeatureArgs(channels=self.C, features=_ptr(self.extra_features), rasterized=_ptr(b.feature_map),
                                                grad_rasterized=_ptr(b.grad_feature_map),
@@ -248,6 +296,20 @@ class FusedTrainStep:
                     loss_out2=_ptr(self.feature_loss), temp=_ptr(b.feat_temp), temp_bytes=b.feat_bytes,
                     exp_avg=_ptr(self.extra_feature_exp_avg), exp_avg_sq=_ptr(self.extra_feature_exp_avg_sq),
                     learning_rate=self.extra_feature_learning_rate)
+            if appearance_view is not None:
+                i = appearance_view
+                self.appearance_steps[i] += 1
+                gz, gy, gx = self.appearance_grids.shape[2:]
+                app = _lib.GsbAppearanceArgs(
+                    grid=_ptr(self.appearance_grids[i]), grad_grid=_ptr(self.grad_appearance_grid), grid_x=gx, grid_y=gy,
+                    grid_z=gz, tv_weight=self.appearance_tv_weight, exp_avg=_ptr(self.appearance_exp_avg[i]),
+                    exp_avg_sq=_ptr(self.appearance_exp_avg_sq[i]), learning_rate=self.appearance_learning_rate,
+                    step=self.appearance_steps[i], image=_ptr(b.sliced_image), temp=_ptr(b.app_temp), temp_bytes=b.app_bytes,
+                    loss_out1=_ptr(self.appearance_tv))
+                _lib.check(self._lib.gsb200_train_step_appearance(
+                    ctypes.byref(args), ctypes.byref(sup) if supervised else None, ctypes.byref(fx) if fx is not None else None,
+                    ctypes.byref(app)), "gsb200_train_step_appearance")
+            elif fx is not None:
                 _lib.check(self._lib.gsb200_train_step_ext(ctypes.byref(args), ctypes.byref(sup) if supervised else None,
                                                            ctypes.byref(fx)), "gsb200_train_step_ext")
             elif supervised:

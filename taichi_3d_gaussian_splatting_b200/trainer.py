@@ -28,6 +28,10 @@ Views with a rolling shutter (an extension; ``CameraInfo.rolling_shutter``) trai
 downsampled camera keeps the motion (row time is normalised by the image height).  Not with ``fused_step``, pose, intrinsics
 or lens refinement.  Optional motion refinement (``TrainConfig.rolling_shutter_learning_rate``): per rolling-shutter view, its
 motion (v, w), differentiated by the operator's ``differentiable_rolling_shutter`` and stepped by its own Adam.
+Optional appearance compensation (an extension; ``TrainConfig.appearance_grid``): one bilateral grid per training view
+(``appearance.apply_bilateral_grid``), initialised to the identity, slices the image the image loss sees (after the
+background composite), with a TV prior and its own Adam that steps only the visited view's grid.  It acts on the image alone,
+so it composes with every other option; ``validation`` renders the raw image (a held-out view has no grid).
 The rasteriser is injected (default: the CUDA operator) so that tests can run the identical loop with the
 CPU oracle behind the same interface and compare PSNR trajectories.
 """
@@ -38,6 +42,7 @@ from typing import Callable, List, Optional, Tuple
 import torch
 import torch.nn.functional as F
 
+from .appearance import apply_bilateral_grid, bilateral_grid_tv, check_grid_shape, identity_grids
 from .Camera import CameraInfo, LensDistortion, RollingShutter
 from .densification import GaussianPointAdaptiveController
 from .GaussianPointCloudRasterisation import GaussianPointCloudRasterisation
@@ -158,6 +163,13 @@ class GaussianPointCloudTrainer:
         # (6,) leaf tensor of its motion (v, w), initialised from the view's, kept on the host and trained by its own Adam at
         # this rate.  Not with fused_step, pose, intrinsics or lens refinement (no rolling-shutter view combines with them).
         rolling_shutter_learning_rate: float = 0.
+        # optional appearance compensation: (Gx, Gy, Gz) gives every training view one bilateral grid of that many nodes
+        # (1 <= Gx, Gy <= 64, 1 <= Gz <= 16; (1, 1, 1) is a per-view affine colour transform), initialised to the identity
+        # and trained by its own Adam at appearance_learning_rate with a TV prior of weight appearance_tv_weight.  The
+        # defaults are starting points, not tuned.
+        appearance_grid: Optional[Tuple[int, int, int]] = None
+        appearance_learning_rate: float = 2e-3
+        appearance_tv_weight: float = 10.0
 
     def __init__(self, config: "GaussianPointCloudTrainer.TrainConfig", scene: Scene, train_views: List[View],
                  rasterisation_factory: Optional[Callable] = None, generator: Optional[torch.Generator] = None,
@@ -227,6 +239,20 @@ class GaussianPointCloudTrainer:
                     raise ValueError(f"{name} is not supported with a rolling-shutter view (CameraInfo.rolling_shutter)")
         self._rolling_shutter = self._rolling_shutter_leaves(config, train_views)
         self._rs = config.rolling_shutter_learning_rate > 0
+        self._appearance = config.appearance_grid is not None
+        self._appearance_leaves = []
+        self._appearance_tensor = None
+        if self._appearance:
+            shape = check_grid_shape(config.appearance_grid)
+            for name in ("appearance_learning_rate", "appearance_tv_weight"):
+                v = getattr(config, name)
+                if not (v >= 0.0 and v < float("inf")):
+                    raise ValueError(f"{name} must be finite and >= 0, got {v}")
+            grids = identity_grids(len(train_views), shape, device=scene.point_cloud.device)
+            if fused_step:  # updated in place by the fused step
+                self._appearance_tensor = grids
+            else:  # one leaf per view: an optimiser over them steps only the leaves that got a gradient
+                self._appearance_leaves = [g.clone().requires_grad_(True) for g in grids]
         self._features = config.feature_loss != "none"
         if self._features:
             self._check_feature_config(config, scene, targets)
@@ -401,7 +427,10 @@ class GaussianPointCloudTrainer:
                               mask_weight=cfg.mask_loss_weight,
                               **(dict(extra_features=self.scene.point_extra_features, feature_loss=cfg.feature_loss,
                                       feature_weight=cfg.feature_loss_weight,
-                                      extra_feature_learning_rate=cfg.extra_feature_learning_rate) if self._features else {}))
+                                      extra_feature_learning_rate=cfg.extra_feature_learning_rate) if self._features else {}),
+                              **(dict(appearance_grids=self._appearance_tensor,
+                                      appearance_learning_rate=cfg.appearance_learning_rate,
+                                      appearance_tv_weight=cfg.appearance_tv_weight) if self._appearance else {}))
         self.fused_train_step = step
         position_lr = cfg.position_learning_rate
         downsample_factor = cfg.initial_downsample_factor
@@ -411,11 +440,12 @@ class GaussianPointCloudTrainer:
             view_index = self._next_view_index(iteration)
             image_gt, q, t, camera_info, targets = self._view(view_index, downsample_factor)
             band = iteration // cfg.increase_color_max_sh_band_interval
+            app_kw = {"appearance_view": view_index} if self._appearance else {}
             if self.supervised or self._features:
                 step.run(image_gt, q, t, camera_info, band, cfg.feature_learning_rate, position_lr, targets=targets,
-                         background=self._next_background())
+                         background=self._next_background(), **app_kw)
             else:
-                step.run(image_gt, q, t, camera_info, band, cfg.feature_learning_rate, position_lr)
+                step.run(image_gt, q, t, camera_info, band, cfg.feature_learning_rate, position_lr, **app_kw)
             if iteration % cfg.position_learning_rate_decay_interval == 0:  # ExponentialLR.step() after the optimiser step
                 position_lr *= cfg.position_learning_rate_decay_rate
             self.adaptive_controller.after_fused_update(step.hook_input)
@@ -432,6 +462,9 @@ class GaussianPointCloudTrainer:
                 if self._features:
                     entry["feature_loss"] = float(step.feature_loss[0])
                     entry["loss"] += entry["feature_loss"]
+                if self._appearance:
+                    entry["appearance_tv"] = float(step.appearance_tv[0])
+                    entry["loss"] += entry["appearance_tv"]
                 self.history.append(entry)
         return self.history
 
@@ -469,6 +502,8 @@ class GaussianPointCloudTrainer:
         rolling_shutter_optimizer = torch.optim.Adam(list(self._rolling_shutter.values()),
                                                      lr=cfg.rolling_shutter_learning_rate, betas=(0.9, 0.999)) \
             if self._rs else None
+        appearance_optimizer = Adam(self._appearance_leaves, lr=cfg.appearance_learning_rate, betas=(0.9, 0.999)) \
+            if self._appearance else None
         scheduler = torch.optim.lr_scheduler.ExponentialLR(position_optimizer, gamma=cfg.position_learning_rate_decay_rate)
         downsample_factor = cfg.initial_downsample_factor
         for iteration in range(cfg.num_iterations):
@@ -486,6 +521,8 @@ class GaussianPointCloudTrainer:
                 distortion_optimizer.zero_grad()
             if rolling_shutter_optimizer is not None:
                 rolling_shutter_optimizer.zero_grad()
+            if appearance_optimizer is not None:
+                appearance_optimizer.zero_grad()
             view_index = self._next_view_index(iteration)
             image_gt, q, t, camera_info, targets = self._view(view_index, downsample_factor)
             if self._intr:  # built every iteration: the cached downsampled camera must not freeze K
@@ -509,9 +546,9 @@ class GaussianPointCloudTrainer:
                                          rolling_shutter=RollingShutter(values[:3], values[3:]))
                 lens_kw = {"rolling_shutter_motion": leaf}
             band = iteration // cfg.increase_color_max_sh_band_interval
-            if self.supervised or self._features:
-                loss, l1_loss, mask_term, depth_term, feature_term, image_pred = self._supervised_loss(
-                    q, t, camera_info, band, image_gt, targets, lens_kw)
+            if self.supervised or self._features or self._appearance:
+                loss, l1_loss, mask_term, depth_term, feature_term, appearance_tv, image_pred = self._supervised_loss(
+                    q, t, camera_info, band, image_gt, targets, lens_kw, view_index)
             elif self.fused_image_loss:
                 image_pred, _, _ = self.rasterisation(self._input(q, t, camera_info, band), **lens_kw)
                 loss, l1_loss, ssim_loss = self.loss_function.forward_rasterized(
@@ -540,6 +577,8 @@ class GaussianPointCloudTrainer:
                 distortion_optimizer.step()
             if rolling_shutter_optimizer is not None:
                 rolling_shutter_optimizer.step()
+            if appearance_optimizer is not None:
+                appearance_optimizer.step()
             if iteration % cfg.position_learning_rate_decay_interval == 0:
                 scheduler.step()
             self.adaptive_controller.refinement()
@@ -551,15 +590,18 @@ class GaussianPointCloudTrainer:
                     self._supervised_history(entry, mask_term.detach(), depth_term.detach())
                 if self._features:
                     entry["feature_loss"] = float(feature_term.detach())
+                if self._appearance:
+                    entry["appearance_tv"] = float(appearance_tv.detach())
                 self.history.append(entry)
         return self.history
 
-    def _supervised_loss(self, q, t, camera_info, band, image_gt, targets, lens_kw=None):
+    def _supervised_loss(self, q, t, camera_info, band, image_gt, targets, lens_kw=None, view_index=None):
         """Forward with the differentiable outputs the terms need, then ``loss.supervision_loss`` with this trainer's image
         loss (the torch one, or the fused kernels with ``fused_image_loss``; the scale regulariser if enabled), plus
         ``loss.feature_loss`` on the rendered feature map with a feature loss.  Returns (total, L1, mask term, depth term,
-        feature term, the raw image as (3, H, W) for the PSNR log).  ``lens_kw``: the operator's ``lens_coefficients``
-        argument with lens refinement."""
+        feature term, the weighted TV term of the appearance grid, the raw image as (3, H, W) for the PSNR log).
+        ``lens_kw``: the operator's ``lens_coefficients`` argument with lens refinement.  With appearance grids the image
+        loss reads the image (after the background composite) sliced through the grid of ``view_index``."""
         cfg = self.config
         lens_kw = lens_kw or {}
         if self._features:
@@ -575,6 +617,12 @@ class GaussianPointCloudTrainer:
         else:
             image_loss = lambda pred, gt: self.loss_function(  # noqa: E731
                 torch.clamp(pred, min=0, max=1).permute(2, 0, 1), gt, **regulariser)
+        appearance_tv = None
+        if self._appearance:
+            grid = self._appearance_leaves[view_index]
+            raw_image_loss = image_loss
+            image_loss = lambda pred, gt: raw_image_loss(apply_bilateral_grid(pred, grid), gt)  # noqa: E731
+            appearance_tv = cfg.appearance_tv_weight * bilateral_grid_tv(grid)
         total, l1, _, mask_term, depth_term = supervision_loss(
             image_pred, depth, alpha, image_gt, targets, self._next_background(), cfg.loss_function_config.lambda_value,
             cfg.depth_loss_weight, cfg.mask_loss_weight, image_loss=image_loss)
@@ -582,7 +630,19 @@ class GaussianPointCloudTrainer:
         if self._features:
             feature_term = feature_loss(outs[-1], targets, cfg.feature_loss, cfg.feature_loss_weight)
             total = total + feature_term
-        return total, l1, mask_term, depth_term, feature_term, image_pred.detach().clamp(0, 1).permute(2, 0, 1)
+        if appearance_tv is not None:
+            total = total + appearance_tv
+        return (total, l1, mask_term, depth_term, feature_term, appearance_tv,
+                image_pred.detach().clamp(0, 1).permute(2, 0, 1))
+
+    def appearance_grids(self) -> Optional[torch.Tensor]:
+        """The (V, 12, Gz, Gy, Gx) appearance grids of the training views as trained (a detached copy; None without
+        appearance compensation)."""
+        if not self._appearance:
+            return None
+        if self._appearance_tensor is not None:
+            return self._appearance_tensor.detach().clone()
+        return torch.stack([g.detach() for g in self._appearance_leaves]).clone()
 
     def refined_poses(self) -> List[Tuple[torch.Tensor, torch.Tensor]]:
         """(q, t) of every training view as trained (detached copies; the views' own poses without pose refinement)."""
