@@ -208,6 +208,9 @@ void gsb200_abi_sizes(int64_t *out3);
  * GsbSupervisionArgs, GsbExtraFeatureArgs, GsbFeatureTrainArgs, GsbPoseGradArgs, GsbIntrinsicsGradArgs, GsbLensArgs,
  * GsbLensGradArgs, GsbRollingShutterArgs, GsbRollingShutterGradArgs, GsbAppearanceArgs} */
 void gsb200_abi_sizes_ext(int64_t *out, int32_t n);
+/* sizeof(GsbMcmcRelocateArgs), sizeof(GsbMcmcStepArgs).  A call of their own: the table of gsb200_abi_sizes_ext ends at
+ * GsbAppearanceArgs, and a binding may rely on slots past its end staying untouched. */
+void gsb200_abi_sizes_mcmc(int64_t *out2);
 
 /* Workspace sizing.  far_plane*depth_to_sort_key_scale fixes the depth-key width; (H/16)*(W/16)
  * the tile-id width; both <= 32 bits total selects 32-bit sort keys.
@@ -634,6 +637,93 @@ typedef struct GsbAppearanceArgs {
  * step < 1, or a TV weight or learning rate that is negative or not finite.  Deterministic. */
 int gsb200_train_step_appearance(const GsbTrainStepArgs *args, const GsbSupervisionArgs *supervision,
                                  const GsbFeatureTrainArgs *features, const GsbAppearanceArgs *appearance);
+
+/* MCMC densification (an extension; Kheradmand et al., "3D Gaussian Splatting as Markov Chain Monte Carlo", NeurIPS 2024):
+ * the per-iteration regularisers and position noise, and the relocation arithmetic of a refinement.  Row layout as
+ * everywhere: features[0:4] = q (xyzw), [4:7] = log-scale s, [7] = opacity logit; o = sigmoid(logit), scale = exp(s),
+ * Sigma = R(q / |q|) diag(exp(2 s)) R^T.  A row is valid when point_invalid_mask == 0; n_v = the number of valid rows (the
+ * host knows it: it changes only at a refinement).
+ *   Regularisers:  R = lambda_o sum_valid o_i / n_v + lambda_s sum_valid sum_j exp(s_ij) / (3 n_v)
+ *     dR/dlogit_i = lambda_o o_i (1 - o_i) / n_v,  dR/ds_ij = lambda_s exp(s_ij) / (3 n_v); invalid rows get nothing.  Plain
+ *     derivatives: the rasteriser's gradient factors (GsbBackwardArgs::grad_*_factor) do not apply to them.  n_v = 0: R = 0.
+ *   Position noise, after the optimiser step of iteration t, for every valid row i:
+ *     xyz_i += Sigma_i eps_i noise_scale g(o_i),  g(o) = 1 / (1 + exp(-gate_k ((1 - o) - (1 - min_opacity))))
+ *     (noise_scale = noise_lr * the position learning rate of the step; the paper: gate_k = 100, min_opacity = 0.005).
+ *     eps_i in R^3 is a pure function of (seed, t, i): x[0..3] = Philox4x32-10 (Salmon et al., SC 2011; multipliers
+ *     0xD2511F53, 0xCD9E8D57, key increments 0x9E3779B9, 0xBB67AE85) with key = {seed low, seed high 32 bits} and counter =
+ *     {i low, i high, t low, t high};  u_k = ((x[k] >> 9) + 0.5) 2^-23, exact in float32 and never 0 or 1 (a 24-bit mantissa
+ *     cannot hold (x >> 8) + 0.5);  Box-Muller:  eps = (r0 cos(2 pi u_1), r0 sin(2 pi u_1), r1 cos(2 pi u_3)),
+ *     r0 = sqrt(-2 ln u_0), r1 = sqrt(-2 ln u_2).  No state is kept: two calls with equal arguments are bit-identical.
+ *   Relocation (the paper's eq. 9), for a source that ends up as n copies (times drawn + 1, clamped to GSB_MCMC_N_MAX):
+ *     o_new = 1 - (1 - o)^(1/n),  D = sum_{i=1..n} sum_{k=0..i-1} C(i-1, k) (-1)^k o_new^(k+1) / sqrt(k+1),
+ *     s_new = s + log(o / D),  logit_new = logit(clamp(o_new, min_opacity, 1 - 1e-7));  evaluated in double (the sum
+ *     alternates); n = 1 is the identity to rounding (D = o). */
+#define GSB_MCMC_N_MAX 51
+/* bytes of the regulariser's temp (a ticket and per-CTA partial sums) */
+int64_t gsb200_mcmc_temp_bytes(void);
+/* Adds dR/dfeatures into columns 4..7 of grad_features (N,56) -- the gradient the backward has just written -- and writes
+ * terms_out2 = {opacity term, scale term} of R (device).  The sums are taken in double in a fixed order: bit-reproducible.
+ * temp: gsb200_mcmc_temp_bytes() bytes, its first 16 bytes zero before the first use (the call leaves them ready for the next
+ * one).  GSB_EINVAL, before any CUDA call, for num_points < 0, num_valid outside [0, num_points], a weight that is negative
+ * or not finite, or a NULL or not 16-byte aligned features, grad_features or temp pointer, a NULL mask or terms_out2. */
+int gsb200_mcmc_regulariser(const float *pointcloud_features, const int8_t *point_invalid_mask, float *grad_features,
+                            int64_t num_points, int64_t num_valid, float lambda_opacity, float lambda_scale,
+                            float *terms_out2, void *temp, void *stream);
+/* The position noise of iteration `step` on the valid rows of pointcloud (N,3), in place.  GSB_EINVAL, before any CUDA call,
+ * for num_points < 0, step < 0, a noise_scale, gate_k or min_opacity that is negative or not finite, a NULL pointer, a
+ * pointcloud that is not 4-byte aligned or features that are not 16-byte aligned. */
+int gsb200_mcmc_noise(float *pointcloud, const float *pointcloud_features, const int8_t *point_invalid_mask,
+                      int64_t num_points, float noise_scale, float gate_k, float min_opacity, uint64_t seed, int64_t step,
+                      void *stream);
+/* One relocation: first every drawn source row gets its new logit and log-scales from its draw count (in place) and its Adam
+ * moments zeroed; then, in stream order, every destination row becomes a copy of its source's updated row (xyz, the 56
+ * features, the object id, the extra-feature row when present), its mask byte is cleared and its moments are zeroed.  The
+ * caller guarantees: source ids unique, destination ids unique and disjoint from the source ids (no atomics are used).  A row
+ * id outside [0, num_points) is skipped on the device. */
+typedef struct GsbMcmcRelocateArgs {
+    int64_t num_points;
+    int64_t num_sources;
+    const int32_t *source_ids;        /* (num_sources,) rows that were drawn at least once */
+    const int32_t *source_counts;     /* (num_sources,) times drawn; the row ends up as count + 1 copies */
+    int64_t num_destinations;
+    const int32_t *destination_ids;   /* (num_destinations,) rows that are overwritten */
+    const int32_t *destination_sources; /* (num_destinations,) the row each one copies */
+    float *pointcloud;                /* (N,3) */
+    float *pointcloud_features;       /* (N,56), 16-byte aligned */
+    int8_t *point_invalid_mask;       /* (N,) */
+    int32_t *point_object_id;         /* (N,) */
+    float *extra_features;            /* (N,C) or NULL */
+    int32_t channels;                 /* C in 1..16 with extra_features */
+    float min_opacity;                /* in (0, 1) */
+    float *feature_exp_avg, *feature_exp_avg_sq;   /* (N,56) 16-byte aligned, or both NULL */
+    float *position_exp_avg, *position_exp_avg_sq; /* (N,3) or both NULL */
+    float *extra_exp_avg, *extra_exp_avg_sq;       /* (N,C) or both NULL (need extra_features) */
+    void *stream;
+} GsbMcmcRelocateArgs;
+/* GSB_EINVAL, before any CUDA call, for a NULL args, counts outside [0, num_points], a NULL id array with a non-zero count,
+ * a NULL scene tensor, features or feature moments that are not 16-byte aligned, C outside 1..16, a moment pair with one
+ * NULL half, extra moments without extra_features, or min_opacity outside (0, 1). */
+int gsb200_mcmc_relocate(const GsbMcmcRelocateArgs *args);
+
+/* The MCMC part of a fused train step. */
+typedef struct GsbMcmcStepArgs {
+    int64_t num_valid;                  /* n_v in [0, num_points] */
+    float lambda_opacity, lambda_scale; /* >= 0, finite */
+    float noise_scale;                  /* noise_lr * this step's position learning rate; >= 0, finite */
+    float gate_k, min_opacity;          /* >= 0, finite */
+    uint64_t seed;
+    int64_t step;                       /* the iteration t of the noise counter, >= 0 */
+    float *terms_out2;                  /* device: {opacity term, scale term} */
+    void *temp;                         /* gsb200_mcmc_temp_bytes(), 16-byte aligned, first 16 bytes zero before first use */
+} GsbMcmcStepArgs;
+/* gsb200_train_step_appearance with the MCMC per-iteration work: ... -> backward -> regulariser (adds into the dense feature
+ * gradient, writes terms_out2) -> the Adam steps -> position noise (reads the updated features).  Both new launches are
+ * skipped on the device after a key-capacity overflow, like the Adam steps.  NULL mcmc: exactly
+ * gsb200_train_step_appearance.  GSB_EINVAL, before any CUDA call, for the rules of gsb200_mcmc_regulariser and
+ * gsb200_mcmc_noise on the fields above. */
+int gsb200_train_step_mcmc(const GsbTrainStepArgs *args, const GsbSupervisionArgs *supervision,
+                           const GsbFeatureTrainArgs *features, const GsbAppearanceArgs *appearance,
+                           const GsbMcmcStepArgs *mcmc);
 
 /* Individual stages (same workspace), for tests and profiling. */
 int gsb200_stage_preprocess(const GsbForwardArgs *args);   /* K1+P1+K2+K3+P2+K4 fused */

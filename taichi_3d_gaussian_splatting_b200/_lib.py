@@ -147,6 +147,24 @@ class GsbAppearanceArgs(ctypes.Structure):
     ]
 
 
+class GsbMcmcRelocateArgs(ctypes.Structure):
+    _fields_ = [
+        ("num_points", c_i64), ("num_sources", c_i64), ("source_ids", c_vp), ("source_counts", c_vp),
+        ("num_destinations", c_i64), ("destination_ids", c_vp), ("destination_sources", c_vp), ("pointcloud", c_vp),
+        ("pointcloud_features", c_vp), ("point_invalid_mask", c_vp), ("point_object_id", c_vp), ("extra_features", c_vp),
+        ("channels", c_i32), ("min_opacity", c_f32), ("feature_exp_avg", c_vp), ("feature_exp_avg_sq", c_vp),
+        ("position_exp_avg", c_vp), ("position_exp_avg_sq", c_vp), ("extra_exp_avg", c_vp), ("extra_exp_avg_sq", c_vp),
+        ("stream", c_vp),
+    ]
+
+
+class GsbMcmcStepArgs(ctypes.Structure):
+    _fields_ = [
+        ("num_valid", c_i64), ("lambda_opacity", c_f32), ("lambda_scale", c_f32), ("noise_scale", c_f32), ("gate_k", c_f32),
+        ("min_opacity", c_f32), ("seed", ctypes.c_uint64), ("step", c_i64), ("terms_out2", c_vp), ("temp", c_vp),
+    ]
+
+
 def lens_args(distortion) -> GsbLensArgs:
     """The C argument of a ``Camera.LensDistortion`` (host floats; unused coefficients 0)."""
     model = {"opencv": GSB_LENS_OPENCV, "fisheye": GSB_LENS_FISHEYE}[distortion.model]
@@ -181,6 +199,8 @@ EXPORTS = (
     "gsb200_backward_lens", "gsb200_backward_lens_grad", "gsb200_lens_grad_temp_bytes", "gsb200_forward_rolling_shutter",
     "gsb200_backward_rolling_shutter", "gsb200_rolling_shutter_grad_temp_bytes", "gsb200_bilateral_grid_temp_bytes",
     "gsb200_bilateral_grid_forward", "gsb200_bilateral_grid_backward", "gsb200_train_step_appearance",
+    "gsb200_mcmc_temp_bytes", "gsb200_mcmc_regulariser", "gsb200_mcmc_noise", "gsb200_mcmc_relocate", "gsb200_train_step_mcmc",
+    "gsb200_abi_sizes_mcmc",
 )
 
 _lib = None
@@ -283,6 +303,18 @@ def load() -> ctypes.CDLL:
     lib.gsb200_train_step_appearance.argtypes = [ctypes.POINTER(GsbTrainStepArgs), ctypes.POINTER(GsbSupervisionArgs),
                                                  ctypes.POINTER(GsbFeatureTrainArgs), ctypes.POINTER(GsbAppearanceArgs)]
     lib.gsb200_train_step_appearance.restype = ctypes.c_int
+    lib.gsb200_train_step_mcmc.argtypes = [ctypes.POINTER(GsbTrainStepArgs), ctypes.POINTER(GsbSupervisionArgs),
+                                           ctypes.POINTER(GsbFeatureTrainArgs), ctypes.POINTER(GsbAppearanceArgs),
+                                           ctypes.POINTER(GsbMcmcStepArgs)]
+    lib.gsb200_train_step_mcmc.restype = ctypes.c_int
+    lib.gsb200_mcmc_temp_bytes.argtypes = []
+    lib.gsb200_mcmc_temp_bytes.restype = c_i64
+    lib.gsb200_mcmc_regulariser.argtypes = [c_vp, c_vp, c_vp, c_i64, c_i64, c_f32, c_f32, c_vp, c_vp, c_vp]
+    lib.gsb200_mcmc_regulariser.restype = ctypes.c_int
+    lib.gsb200_mcmc_noise.argtypes = [c_vp, c_vp, c_vp, c_i64, c_f32, c_f32, c_f32, ctypes.c_uint64, c_i64, c_vp]
+    lib.gsb200_mcmc_noise.restype = ctypes.c_int
+    lib.gsb200_mcmc_relocate.argtypes = [ctypes.POINTER(GsbMcmcRelocateArgs)]
+    lib.gsb200_mcmc_relocate.restype = ctypes.c_int
     lib.gsb200_bilateral_grid_temp_bytes.argtypes = [c_i32] * 5
     lib.gsb200_bilateral_grid_temp_bytes.restype = c_i64
     lib.gsb200_bilateral_grid_forward.argtypes = [c_vp, c_vp] + [c_i32] * 5 + [c_vp, c_vp]
@@ -366,6 +398,14 @@ def load() -> ctypes.CDLL:
     if sizes15[14] != ctypes.sizeof(GsbAppearanceArgs):
         raise RuntimeError(f"libgsb200.so ABI mismatch: sizeof(GsbAppearanceArgs) {sizes15[14]} != ctypes mirror "
                            f"{ctypes.sizeof(GsbAppearanceArgs)}")
+    lib.gsb200_abi_sizes_mcmc.argtypes = [ctypes.POINTER(c_i64)]
+    lib.gsb200_abi_sizes_mcmc.restype = None
+    sizes_mcmc = (c_i64 * 2)()
+    lib.gsb200_abi_sizes_mcmc(sizes_mcmc)
+    for i, mirror in ((0, GsbMcmcRelocateArgs), (1, GsbMcmcStepArgs)):
+        if sizes_mcmc[i] != ctypes.sizeof(mirror):
+            raise RuntimeError(f"libgsb200.so ABI mismatch: sizeof({mirror.__name__}) {sizes_mcmc[i]} != ctypes mirror "
+                               f"{ctypes.sizeof(mirror)}")
     _lib = lib
     return lib
 

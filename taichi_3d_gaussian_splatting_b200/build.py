@@ -34,6 +34,7 @@ SOURCES = {
     "feature_loss.cu": [],
     "appearance.cu": [],
     "adam.cu": [],
+    "mcmc.cu": [],
     "controller.cu": [],
     "exchange.cu": [],
 }

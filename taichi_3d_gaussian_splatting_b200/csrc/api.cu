@@ -201,6 +201,11 @@ void gsb200_abi_sizes_ext(int64_t *out, int32_t n) {
     for (int i = 0; i < n && i < 15; ++i) out[i] = all[i];
 }
 
+void gsb200_abi_sizes_mcmc(int64_t *out2) {
+    out2[0] = (int64_t)sizeof(GsbMcmcRelocateArgs);
+    out2[1] = (int64_t)sizeof(GsbMcmcStepArgs);
+}
+
 int gsb200_workspace_layout(int64_t num_points, int32_t num_objects, int64_t key_capacity,
                             int32_t camera_height, int32_t camera_width, float far_plane,
                             float depth_to_sort_key_scale, uint32_t flags, GsbWorkspaceLayout *out) {
@@ -715,6 +720,68 @@ int gsb200_train_step_ext(const GsbTrainStepArgs *t, const GsbSupervisionArgs *s
 
 int gsb200_train_step_appearance(const GsbTrainStepArgs *t, const GsbSupervisionArgs *s, const GsbFeatureTrainArgs *x,
                                  const GsbAppearanceArgs *app) {
+    return gsb200_train_step_mcmc(t, s, x, app, nullptr);
+}
+
+// The rules of the regulariser and of the noise (gsb200_mcmc_regulariser, gsb200_mcmc_noise, gsb200_train_step_mcmc).
+static int check_mcmc_regulariser(const char *what, int64_t N, int64_t num_valid, float lambda_opacity, float lambda_scale,
+                                  const float *terms_out, const void *temp) {
+    if (N < 0 || num_valid < 0 || num_valid > N) {
+        set_error("%s: num_valid must be in [0, num_points] (got %lld of %lld)", what, (long long)num_valid, (long long)N);
+        return GSB_EINVAL;
+    }
+    if (!weight_ok(lambda_opacity) || !weight_ok(lambda_scale)) {
+        set_error("%s: the opacity and scale weights must be finite and >= 0 (got %g, %g)", what, (double)lambda_opacity,
+                  (double)lambda_scale);
+        return GSB_EINVAL;
+    }
+    if (!terms_out || !temp || !aligned16(temp)) {
+        set_error("%s: terms_out2 NULL, or temp NULL or not 16-byte aligned", what);
+        return GSB_EINVAL;
+    }
+    return GSB_OK;
+}
+
+static int check_mcmc_noise(const char *what, int64_t N, float noise_scale, float gate_k, float min_opacity, int64_t step) {
+    if (N < 0 || step < 0) {
+        set_error("%s: num_points and the noise step must be >= 0 (got %lld, %lld)", what, (long long)N, (long long)step);
+        return GSB_EINVAL;
+    }
+    if (!weight_ok(noise_scale) || !weight_ok(gate_k) || !weight_ok(min_opacity)) {
+        set_error("%s: noise_scale, gate_k and min_opacity must be finite and >= 0 (got %g, %g, %g)", what, (double)noise_scale,
+                  (double)gate_k, (double)min_opacity);
+        return GSB_EINVAL;
+    }
+    return GSB_OK;
+}
+
+int gsb200_mcmc_regulariser(const float *features, const int8_t *invalid_mask, float *grad_features, int64_t N,
+                            int64_t num_valid, float lambda_opacity, float lambda_scale, float *terms_out2, void *temp,
+                            void *stream) {
+    int rc = check_mcmc_regulariser("mcmc_regulariser", N, num_valid, lambda_opacity, lambda_scale, terms_out2, temp);
+    if (rc != GSB_OK) return rc;
+    if (!features || !invalid_mask || !grad_features || !aligned16(features) || !aligned16(grad_features)) {
+        set_error("mcmc_regulariser: NULL pointer, or features / grad_features not 16-byte aligned");
+        return GSB_EINVAL;
+    }
+    return launch_mcmc_regulariser(features, invalid_mask, grad_features, N, num_valid, lambda_opacity, lambda_scale, terms_out2,
+                                   temp, nullptr, static_cast<cudaStream_t>(stream));
+}
+
+int gsb200_mcmc_noise(float *pointcloud, const float *features, const int8_t *invalid_mask, int64_t N, float noise_scale,
+                      float gate_k, float min_opacity, uint64_t seed, int64_t step, void *stream) {
+    int rc = check_mcmc_noise("mcmc_noise", N, noise_scale, gate_k, min_opacity, step);
+    if (rc != GSB_OK) return rc;
+    if (!pointcloud || !features || !invalid_mask || reinterpret_cast<uintptr_t>(pointcloud) % 4 || !aligned16(features)) {
+        set_error("mcmc_noise: NULL pointer, pointcloud not 4-byte aligned or features not 16-byte aligned");
+        return GSB_EINVAL;
+    }
+    return launch_mcmc_noise(pointcloud, features, invalid_mask, N, noise_scale, gate_k, min_opacity, seed, step, nullptr,
+                             static_cast<cudaStream_t>(stream));
+}
+
+int gsb200_train_step_mcmc(const GsbTrainStepArgs *t, const GsbSupervisionArgs *s, const GsbFeatureTrainArgs *x,
+                           const GsbAppearanceArgs *app, const GsbMcmcStepArgs *mc) {
     if (!t || !t->ground_truth_image || !t->loss_out3 || !t->loss_temp || !t->feature_exp_avg || !t->feature_exp_avg_sq ||
         !t->position_exp_avg || !t->position_exp_avg_sq || t->step < 1) {
         set_error("train_step: null pointer argument or step < 1");
@@ -779,6 +846,18 @@ int gsb200_train_step_appearance(const GsbTrainStepArgs *t, const GsbSupervision
     int rc;
     if (x && (rc = check_feature_train_args(*x, b, H, W)) != GSB_OK) return rc;
     if (app && (rc = check_appearance_args(*app, H, W)) != GSB_OK) return rc;
+    if (mc) {
+        if ((rc = check_mcmc_regulariser("train_step_mcmc", f.num_points, mc->num_valid, mc->lambda_opacity, mc->lambda_scale,
+                                         mc->terms_out2, mc->temp)) != GSB_OK)
+            return rc;
+        if ((rc = check_mcmc_noise("train_step_mcmc", f.num_points, mc->noise_scale, mc->gate_k, mc->min_opacity,
+                                   mc->step)) != GSB_OK)
+            return rc;
+        if (!f.point_invalid_mask || !aligned16(f.pointcloud_features) || !aligned16(b.grad_pointcloud_features)) {
+            set_error("train_step_mcmc: NULL invalid mask, or features / grad_features not 16-byte aligned");
+            return GSB_EINVAL;
+        }
+    }
     const GsbExtraFeatureArgs *ext = x ? &x->features : nullptr;
     cudaStream_t st = static_cast<cudaStream_t>(f.stream);
     if ((rc = gsb200_forward_ext(&f, ext)) != GSB_OK) return rc;
@@ -811,6 +890,10 @@ int gsb200_train_step_appearance(const GsbTrainStepArgs *t, const GsbSupervision
     Workspace ws;
     if ((rc = resolve_fwd(&f, &ws)) != GSB_OK) return rc;
     const long long *skip = ws.counters + CNT_OVERFLOW;
+    if (mc && (rc = launch_mcmc_regulariser(f.pointcloud_features, f.point_invalid_mask, b.grad_pointcloud_features,
+                                            f.num_points, mc->num_valid, mc->lambda_opacity, mc->lambda_scale, mc->terms_out2,
+                                            mc->temp, skip, st)) != GSB_OK)
+        return rc;
     rc = launch_adam_step(f.pointcloud_features, b.grad_pointcloud_features, t->feature_exp_avg, t->feature_exp_avg_sq,
                           (long long)f.num_points * GSB_FEATURE_DIM, t->feature_learning_rate, t->beta1, t->beta2, t->eps, t->step,
                           skip, st);
@@ -822,10 +905,13 @@ int gsb200_train_step_appearance(const GsbTrainStepArgs *t, const GsbSupervision
                                     (long long)f.num_points * ext->channels, x->learning_rate, t->beta1, t->beta2, t->eps,
                                     t->step, skip, st)) != GSB_OK)
         return rc;
-    if (!app) return GSB_OK;
-    return launch_adam_step(app->grid, app->grad_grid, app->exp_avg, app->exp_avg_sq,
-                            12LL * app->grid_z * app->grid_y * app->grid_x, app->learning_rate, t->beta1, t->beta2, t->eps,
-                            app->step, skip, st);
+    if (app && (rc = launch_adam_step(app->grid, app->grad_grid, app->exp_avg, app->exp_avg_sq,
+                                      12LL * app->grid_z * app->grid_y * app->grid_x, app->learning_rate, t->beta1, t->beta2,
+                                      t->eps, app->step, skip, st)) != GSB_OK)
+        return rc;
+    if (!mc) return GSB_OK;
+    return launch_mcmc_noise(const_cast<float *>(f.pointcloud), f.pointcloud_features, f.point_invalid_mask, f.num_points,
+                             mc->noise_scale, mc->gate_k, mc->min_opacity, mc->seed, mc->step, skip, st);
 }
 
 int gsb200_expand_view_gradients(const GsbExpandArgs *a) {

@@ -107,6 +107,13 @@ int launch_backward_points_calib(const GsbBackwardArgs &a, const Workspace &ws, 
 int launch_adam_step(float *param, const float *grad, float *exp_avg, float *exp_avg_sq, long long n, double lr, double beta1,
                      double beta2, double eps, int step, const long long *skip_flag, cudaStream_t stream);
 int launch_expand_view_gradients(const GsbExpandArgs &a, cudaStream_t stream);
+// MCMC densification (csrc/mcmc.cu); skip_flag as in launch_adam_step
+int launch_mcmc_regulariser(const float *features, const int8_t *invalid_mask, float *grad_features, long long N,
+                            long long num_valid, float lambda_opacity, float lambda_scale, float *terms_out, void *temp,
+                            const long long *skip_flag, cudaStream_t stream);
+int launch_mcmc_noise(float *pointcloud, const float *features, const int8_t *invalid_mask, long long N, float noise_scale,
+                      float gate_k, float min_opacity, unsigned long long seed, long long step, const long long *skip_flag,
+                      cudaStream_t stream);
 // supervision_loss.cu: the pre-pass returns the image and ground truth the image loss must read (composited or the inputs)
 int launch_supervision_pre(const GsbSupervisionArgs &s, const float *image, const float *gt, const float *alpha,
                            const float *depth, int H, int W, cudaStream_t stream, const float **loss_image,

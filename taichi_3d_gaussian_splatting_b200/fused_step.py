@@ -23,6 +23,11 @@ Optional appearance grids (``appearance_grids``, ``run(..., appearance_view=i)``
 (``appearance.apply_bilateral_grid``) slices the image the image loss reads, with a TV prior and an Adam step on the visited
 view's grid, in the same one call (``gsb200_train_step_appearance``).  Each view has its own Adam moments and its own step
 count, as torch's Adam gives one parameter per view that only steps when it has a gradient.
+
+Optional MCMC densification (``mcmc=MCMCConfig``, ``run(..., mcmc_num_valid=n_v)``): the opacity and scale regularisers are
+added to the feature gradient between the backward and the Adam steps and the covariance-shaped position noise after them, in
+the same one call (``gsb200_train_step_mcmc``; ``loss.mcmc_regulariser`` and ``mcmc.add_position_noise`` state them in torch).
+The refinements stay on the host (``mcmc.GaussianPointMCMCController.refinement(step.moments)``).
 """
 import ctypes
 import warnings
@@ -34,6 +39,7 @@ import torch
 from . import _lib
 from .GaussianPointCloudRasterisation import Frame, GaussianPointCloudRasterisation, _ptr
 from .loss import FEATURE_LOSSES, SupervisionTargets
+from .mcmc import GATE_K, MCMCMoments
 
 __all__ = ["FusedTrainStep", "SupervisionTargets"]
 
@@ -44,7 +50,7 @@ class FusedTrainStep:
                  mask_weight: float = 0.0, extra_features: Optional[torch.Tensor] = None, feature_loss: Optional[str] = None,
                  feature_weight: float = 1.0, extra_feature_learning_rate: float = 1e-2,
                  appearance_grids: Optional[torch.Tensor] = None, appearance_learning_rate: float = 2e-3,
-                 appearance_tv_weight: float = 10.0):
+                 appearance_tv_weight: float = 10.0, mcmc=None):
         """``scene``: object with ``point_cloud`` (N,3), ``point_cloud_features`` (N,56), ``point_invalid_mask``,
         ``point_object_id`` (CUDA, contiguous; updated in place).  ``controller``: a ``GaussianPointAdaptiveController`` whose
         six accumulators are updated by the backward epilogue (or ``None``).  ``depth_weight`` / ``mask_weight``: weights of
@@ -54,7 +60,7 @@ class FusedTrainStep:
         ``targets.labels`` and C >= 2; "l2": needs ``targets.features``) weighted by ``feature_weight``
         (``loss.feature_loss``).  ``appearance_grids``: (V, 12, Gz, Gy, Gx) float32 per-view bilateral grids (CUDA,
         contiguous; updated in place), trained at ``appearance_learning_rate`` with the TV weight ``appearance_tv_weight``;
-        ``run`` then needs ``appearance_view``."""
+        ``run`` then needs ``appearance_view``.  ``mcmc``: an ``mcmc.MCMCConfig``; ``run`` then needs ``mcmc_num_valid``."""
         for name, w in (("depth_weight", depth_weight), ("mask_weight", mask_weight)):
             if not (w >= 0.0 and w < float("inf")):
                 raise ValueError(f"{name} must be finite and >= 0, got {w}")
@@ -112,6 +118,10 @@ class FusedTrainStep:
             self.appearance_steps = [0] * V  # each view's own Adam step count
             self.grad_appearance_grid = torch.zeros_like(appearance_grids[0])
         self.appearance_tv = z(1)  # {tv_weight * tv(G)} of the latest iteration with appearance (device)
+        self.mcmc = mcmc.check() if mcmc is not None else None
+        self.mcmc_terms = z(2)  # {opacity term, scale term} of the latest iteration with MCMC (device)
+        if mcmc is not None:
+            self._mcmc_temp = torch.zeros(int(self._lib.gsb200_mcmc_temp_bytes()), dtype=torch.uint8, device=dev)
         self._res = {}
         self._pinned = [torch.zeros(4, dtype=torch.int64).pin_memory() for _ in range(2)]
         self._events = [torch.cuda.Event() for _ in range(2)]
@@ -189,13 +199,14 @@ class FusedTrainStep:
     def run(self, image_gt: torch.Tensor, q_pointcloud_camera: torch.Tensor, t_pointcloud_camera: torch.Tensor, camera_info,
             color_max_sh_band: int, feature_learning_rate: float, position_learning_rate: float,
             targets: Optional[SupervisionTargets] = None, background: Optional[torch.Tensor] = None,
-            appearance_view: Optional[int] = None) -> None:
+            appearance_view: Optional[int] = None, mcmc_num_valid: Optional[int] = None) -> None:
         """``targets``: the view's depth and / or mask target ((H, W) float32 CUDA tensors) and, with ``extra_features``, its
         ``labels`` ((H, W) int32) or ``features`` ((H, W, C) float32); ``background``: a (3,) float32 CUDA tensor the image is
         composited on (read on the device when the step runs, so it may be refilled per iteration).  Without supervision
         terms or features this is ``gsb200_train_step``; with supervision terms ``gsb200_train_step_aux``; with features
         ``gsb200_train_step_ext``.  ``appearance_view``: with ``appearance_grids``, the index of the view whose grid slices
-        the image and takes an Adam step (``gsb200_train_step_appearance``)."""
+        the image and takes an Adam step (``gsb200_train_step_appearance``).  ``mcmc_num_valid``: with ``mcmc``, the number
+        of valid rows n_v of the regularisers (``gsb200_train_step_mcmc``); the noise counter is the 0-based iteration."""
         sc, cfg = self.scene, self.config
         H, W = int(camera_info.camera_height), int(camera_info.camera_width)
         if image_gt.shape != (3, H, W) or not image_gt.is_contiguous() or image_gt.dtype != torch.float32:
@@ -229,6 +240,8 @@ class FusedTrainStep:
             appearance_view = int(appearance_view)
         elif appearance_view is not None:
             raise ValueError("appearance_view needs appearance_grids")
+        if (self.mcmc is None) != (mcmc_num_valid is None):
+            raise ValueError("mcmc and mcmc_num_valid must be given together")
         self._check_previous()
         q, t = q_pointcloud_camera.contiguous(), t_pointcloud_camera.contiguous()
         K = camera_info.camera_intrinsics.contiguous()
@@ -296,6 +309,7 @@ class FusedTrainStep:
                     loss_out2=_ptr(self.feature_loss), temp=_ptr(b.feat_temp), temp_bytes=b.feat_bytes,
                     exp_avg=_ptr(self.extra_feature_exp_avg), exp_avg_sq=_ptr(self.extra_feature_exp_avg_sq),
                     learning_rate=self.extra_feature_learning_rate)
+            app = None
             if appearance_view is not None:
                 i = appearance_view
                 self.appearance_steps[i] += 1
@@ -306,6 +320,16 @@ class FusedTrainStep:
                     exp_avg_sq=_ptr(self.appearance_exp_avg_sq[i]), learning_rate=self.appearance_learning_rate,
                     step=self.appearance_steps[i], image=_ptr(b.sliced_image), temp=_ptr(b.app_temp), temp_bytes=b.app_bytes,
                     loss_out1=_ptr(self.appearance_tv))
+            if self.mcmc is not None:
+                mc = self.mcmc
+                mcmc_args = _lib.GsbMcmcStepArgs(
+                    num_valid=int(mcmc_num_valid), lambda_opacity=mc.opacity_reg, lambda_scale=mc.scale_reg,
+                    noise_scale=mc.noise_lr * float(position_learning_rate), gate_k=GATE_K, min_opacity=mc.min_opacity,
+                    seed=int(mc.seed), step=self.step_count - 1, terms_out2=_ptr(self.mcmc_terms), temp=_ptr(self._mcmc_temp))
+                _lib.check(self._lib.gsb200_train_step_mcmc(
+                    ctypes.byref(args), ctypes.byref(sup) if supervised else None, ctypes.byref(fx) if fx is not None else None,
+                    ctypes.byref(app) if app is not None else None, ctypes.byref(mcmc_args)), "gsb200_train_step_mcmc")
+            elif app is not None:
                 _lib.check(self._lib.gsb200_train_step_appearance(
                     ctypes.byref(args), ctypes.byref(sup) if supervised else None, ctypes.byref(fx) if fx is not None else None,
                     ctypes.byref(app)), "gsb200_train_step_appearance")
@@ -319,6 +343,13 @@ class FusedTrainStep:
         self._pending[slot] = True
         self._last = SimpleNamespace(buffers=b, H=H, W=W, slot=slot, supervised=supervised,
                                      keep=(q, t, K, image_gt, depth_t, mask_t, background, feat_t))
+
+    @property
+    def moments(self) -> MCMCMoments:
+        """The Adam moments of this step, for ``GaussianPointMCMCController.refinement``."""
+        extra = (self.extra_feature_exp_avg, self.extra_feature_exp_avg_sq) if self.extra_features is not None else None
+        return MCMCMoments((self.feature_exp_avg, self.feature_exp_avg_sq), (self.position_exp_avg, self.position_exp_avg_sq),
+                           extra)
 
     # ------------------------------------------------------------------ the latest frame, on demand (these calls wait)
     @property

@@ -298,3 +298,54 @@ class LossFunction(nn.Module):
             s = pointcloud_features[point_invalid_mask == 0, 4:7]
             loss = loss + self.config.regularization_weight * torch.norm(torch.exp(s), dim=1).mean()
         return loss, l1, ld_ssim
+
+
+class _McmcRegulariser(torch.autograd.Function):
+    """The terms and their gradient in one launch of ``gsb200_mcmc_regulariser`` on a zero gradient buffer."""
+
+    @staticmethod
+    def forward(ctx, features, invalid_mask, lambda_opacity, lambda_scale, num_valid):
+        import ctypes
+        from . import _lib
+        lib = _lib.load()
+        feats = features.detach().contiguous()
+        grad = torch.zeros_like(feats)
+        terms = torch.empty(2, dtype=torch.float32, device=feats.device)
+        temp = torch.zeros(int(lib.gsb200_mcmc_temp_bytes()), dtype=torch.uint8, device=feats.device)
+        with torch.cuda.device(feats.device):
+            stream = torch.cuda.current_stream(feats.device).cuda_stream
+            _lib.check(lib.gsb200_mcmc_regulariser(feats.data_ptr(), invalid_mask.data_ptr(), grad.data_ptr(), feats.shape[0],
+                                                   int(num_valid), float(lambda_opacity), float(lambda_scale),
+                                                   terms.data_ptr(), temp.data_ptr(), ctypes.c_void_p(stream)),
+                       "gsb200_mcmc_regulariser")
+        ctx.save_for_backward(grad)
+        return terms
+
+    @staticmethod
+    def backward(ctx, grad_terms):
+        (grad,) = ctx.saved_tensors  # columns 4..6 carry the scale term's gradient, column 7 the opacity term's
+        scale = torch.cat([grad_terms[1].expand(3), grad_terms[0:1]])
+        out = torch.zeros_like(grad)
+        out[:, 4:8] = grad[:, 4:8] * scale
+        return out, None, None, None, None
+
+
+def mcmc_regulariser(pointcloud_features: torch.Tensor, point_invalid_mask: torch.Tensor, lambda_opacity: float = 0.01,
+                     lambda_scale: float = 0.01, num_valid: Optional[int] = None) -> torch.Tensor:
+    """The two L1 regularisers of MCMC densification (``mcmc.py``) as a (2,) tensor {opacity term, scale term}; their sum
+    is ``R = lambda_o sum_valid o_i / n_v + lambda_s sum_valid sum_j exp(s_ij) / (3 n_v)`` with o = sigmoid(features[:, 7]),
+    s = features[:, 4:7] and n_v the number of rows with ``point_invalid_mask == 0`` (``num_valid``, counted when not
+    given; 0 valid rows: both terms 0).  Differentiable in the features.  CUDA float32 tensors run the library's kernel
+    (``gsb200_mcmc_regulariser``, sums in double in a fixed order); CPU tensors the torch form, which is the kernel's
+    reference."""
+    valid = point_invalid_mask == 0
+    if num_valid is None:
+        num_valid = int(valid.sum())
+    if pointcloud_features.is_cuda:
+        if pointcloud_features.dtype != torch.float32:
+            raise ValueError("the CUDA regulariser takes float32 tensors")
+        return _McmcRegulariser.apply(pointcloud_features, point_invalid_mask, lambda_opacity, lambda_scale, num_valid)
+    n_v = max(int(num_valid), 1)
+    opacity = torch.sigmoid(pointcloud_features[:, 7])[valid].sum() * (lambda_opacity / n_v)
+    scale = torch.exp(pointcloud_features[:, 4:7])[valid].sum() * (lambda_scale / (3 * n_v))
+    return torch.stack([opacity, scale])

@@ -32,6 +32,11 @@ Optional appearance compensation (an extension; ``TrainConfig.appearance_grid``)
 (``appearance.apply_bilateral_grid``), initialised to the identity, slices the image the image loss sees (after the
 background composite), with a TV prior and its own Adam that steps only the visited view's grid.  It acts on the image alone,
 so it composes with every other option; ``validation`` renders the raw image (a held-out view has no grid).
+Optional MCMC densification (an extension; ``TrainConfig.densification="mcmc"``, ``mcmc_config``): the scene grows to a
+fixed budget by relocating dead Gaussians and adding 5 % per refinement (``mcmc.GaussianPointMCMCController``), with the
+opacity and scale regularisers in the loss and a covariance-shaped position noise after the optimiser step.  The adaptive
+controller and the backward hook are then not used.  Not with the optional scale regulariser of the loss function nor with a
+view-parallel gradient exchange.
 The rasteriser is injected (default: the CUDA operator) so that tests can run the identical loop with the
 CPU oracle behind the same interface and compare PSNR trajectories.
 """
@@ -46,11 +51,13 @@ from .appearance import apply_bilateral_grid, bilateral_grid_tv, check_grid_shap
 from .Camera import CameraInfo, LensDistortion, RollingShutter
 from .densification import GaussianPointAdaptiveController
 from .GaussianPointCloudRasterisation import GaussianPointCloudRasterisation
-from .loss import FEATURE_LOSSES, LossFunction, SupervisionTargets, feature_loss, supervision_loss
+from .loss import FEATURE_LOSSES, LossFunction, SupervisionTargets, feature_loss, mcmc_regulariser, supervision_loss
+from .mcmc import GATE_K, GaussianPointMCMCController, MCMCConfig, MCMCMoments, add_position_noise
 
 View = Tuple[torch.Tensor, torch.Tensor, torch.Tensor, CameraInfo]  # image (3,H,W) in [0,1], q (1,4), t (1,3), camera
 # ... optionally followed by a SupervisionTargets (depth and / or mask at the image's resolution)
 BACKGROUNDS = ("black", "white", "random")
+DENSIFICATIONS = ("adaptive", "mcmc")
 
 
 def psnr(pred: torch.Tensor, target: torch.Tensor) -> float:
@@ -170,6 +177,10 @@ class GaussianPointCloudTrainer:
         appearance_grid: Optional[Tuple[int, int, int]] = None
         appearance_learning_rate: float = 2e-3
         appearance_tv_weight: float = 10.0
+        # how the scene grows: "adaptive" (the reference's gradient-threshold controller, adaptive_controller_config) or
+        # "mcmc" (relocation, growth to mcmc_config.cap_max, regularisers and position noise; needs mcmc_config)
+        densification: str = "adaptive"
+        mcmc_config: Optional[MCMCConfig] = None
 
     def __init__(self, config: "GaussianPointCloudTrainer.TrainConfig", scene: Scene, train_views: List[View],
                  rasterisation_factory: Optional[Callable] = None, generator: Optional[torch.Generator] = None,
@@ -189,6 +200,16 @@ class GaussianPointCloudTrainer:
         each iteration on the device (no host wait; the autograd loop and the fused step draw the same colours)."""
         if config.background not in BACKGROUNDS:
             raise ValueError(f"background must be one of {BACKGROUNDS}, got {config.background!r}")
+        if config.densification not in DENSIFICATIONS:
+            raise ValueError(f"densification must be one of {DENSIFICATIONS}, got {config.densification!r}")
+        self._mcmc = config.densification == "mcmc"
+        if self._mcmc:
+            if not isinstance(config.mcmc_config, MCMCConfig):
+                raise ValueError('densification="mcmc" needs mcmc_config (an MCMCConfig with the budget cap_max)')
+            config.mcmc_config.check()
+            if config.loss_function_config.enable_regularization:
+                raise ValueError('densification="mcmc" has its own scale regulariser: switch off '
+                                 "loss_function_config.enable_regularization")
         for name in ("depth_loss_weight", "mask_loss_weight"):
             w = getattr(config, name)
             if not (w >= 0.0 and w < float("inf")):
@@ -273,13 +294,18 @@ class GaussianPointCloudTrainer:
         self.fused_adam = fused_adam
         self.scene = scene
         self.train_views = train_views
-        self.adaptive_controller = GaussianPointAdaptiveController(
-            config=config.adaptive_controller_config,
-            maintained_parameters=GaussianPointAdaptiveController.GaussianPointAdaptiveControllerMaintainedParameters(
-                pointcloud=scene.point_cloud, pointcloud_features=scene.point_cloud_features,
-                point_invalid_mask=scene.point_invalid_mask, point_object_id=scene.point_object_id,
-                point_extra_features=scene.point_extra_features if self._features else None),
-            generator=generator, fused_update=fused_controller_update)
+        maintained = GaussianPointAdaptiveController.GaussianPointAdaptiveControllerMaintainedParameters(
+            pointcloud=scene.point_cloud, pointcloud_features=scene.point_cloud_features,
+            point_invalid_mask=scene.point_invalid_mask, point_object_id=scene.point_object_id,
+            point_extra_features=scene.point_extra_features if self._features else None)
+        # one of the two: with MCMC there is no adaptive controller and no backward hook (no hook statistics)
+        self.adaptive_controller = self.mcmc_controller = None
+        if self._mcmc:
+            self.mcmc_controller = GaussianPointMCMCController(config.mcmc_config, maintained, generator=generator)
+        else:
+            self.adaptive_controller = GaussianPointAdaptiveController(
+                config=config.adaptive_controller_config, maintained_parameters=maintained, generator=generator,
+                fused_update=fused_controller_update)
         factory = rasterisation_factory or GaussianPointCloudRasterisation
         # the differentiable outputs only when a term needs them: injected factories without them keep working
         extra = dict(**({"differentiable_depth": True} if self._need_depth else {}),
@@ -289,7 +315,10 @@ class GaussianPointCloudTrainer:
                      **({"differentiable_distortion": True} if self._dist else {}),
                      **({"differentiable_rolling_shutter": True} if self._rs else {}))
         self.rasterisation = factory(config=config.rasterisation_config,
-                                     backward_valid_point_hook=self.adaptive_controller.update, **extra)
+                                     backward_valid_point_hook=None if self._mcmc else self.adaptive_controller.update,
+                                     **extra)
+        if self._mcmc and getattr(self.rasterisation, "gradient_exchange", None) is not None:
+            raise ValueError('densification="mcmc" is not implemented for the view-parallel gradient exchange')
         self.loss_function = LossFunction(config=config.loss_function_config)
         self.history: List[dict] = []
         self._downsampled = {}
@@ -424,7 +453,7 @@ class GaussianPointCloudTrainer:
         cfg = self.config
         step = FusedTrainStep(self.scene, cfg.rasterisation_config, cfg.loss_function_config.lambda_value,
                               controller=self.adaptive_controller, depth_weight=cfg.depth_loss_weight,
-                              mask_weight=cfg.mask_loss_weight,
+                              mask_weight=cfg.mask_loss_weight, mcmc=cfg.mcmc_config if self._mcmc else None,
                               **(dict(extra_features=self.scene.point_extra_features, feature_loss=cfg.feature_loss,
                                       feature_weight=cfg.feature_loss_weight,
                                       extra_feature_learning_rate=cfg.extra_feature_learning_rate) if self._features else {}),
@@ -441,6 +470,8 @@ class GaussianPointCloudTrainer:
             image_gt, q, t, camera_info, targets = self._view(view_index, downsample_factor)
             band = iteration // cfg.increase_color_max_sh_band_interval
             app_kw = {"appearance_view": view_index} if self._appearance else {}
+            if self._mcmc:
+                app_kw["mcmc_num_valid"] = self.mcmc_controller.num_valid
             if self.supervised or self._features:
                 step.run(image_gt, q, t, camera_info, band, cfg.feature_learning_rate, position_lr, targets=targets,
                          background=self._next_background(), **app_kw)
@@ -448,8 +479,11 @@ class GaussianPointCloudTrainer:
                 step.run(image_gt, q, t, camera_info, band, cfg.feature_learning_rate, position_lr, **app_kw)
             if iteration % cfg.position_learning_rate_decay_interval == 0:  # ExponentialLR.step() after the optimiser step
                 position_lr *= cfg.position_learning_rate_decay_rate
-            self.adaptive_controller.after_fused_update(step.hook_input)
-            self.adaptive_controller.refinement()
+            if self._mcmc:
+                self.mcmc_controller.refinement(step.moments)
+            else:
+                self.adaptive_controller.after_fused_update(step.hook_input)
+                self.adaptive_controller.refinement()
             if log_interval and iteration % log_interval == 0:
                 losses = step.loss.tolist()
                 entry = dict(iteration=iteration, loss=losses[0], l1=losses[1],
@@ -465,6 +499,9 @@ class GaussianPointCloudTrainer:
                 if self._appearance:
                     entry["appearance_tv"] = float(step.appearance_tv[0])
                     entry["loss"] += entry["appearance_tv"]
+                if self._mcmc:
+                    entry["mcmc_opacity_reg"], entry["mcmc_scale_reg"] = step.mcmc_terms.tolist()
+                    entry["loss"] += entry["mcmc_opacity_reg"] + entry["mcmc_scale_reg"]
                 self.history.append(entry)
         return self.history
 
@@ -561,6 +598,11 @@ class GaussianPointCloudTrainer:
                 loss, l1_loss, ssim_loss = self.loss_function(
                     image_pred, image_gt, point_invalid_mask=self.scene.point_invalid_mask,
                     pointcloud_features=self.scene.point_cloud_features)
+            if self._mcmc:
+                mc = cfg.mcmc_config
+                mcmc_terms = mcmc_regulariser(self.scene.point_cloud_features, self.scene.point_invalid_mask, mc.opacity_reg,
+                                              mc.scale_reg, num_valid=self.mcmc_controller.num_valid)
+                loss = loss + mcmc_terms.sum()
             loss.backward()
             optimizer.step()
             position_optimizer.step()
@@ -579,9 +621,16 @@ class GaussianPointCloudTrainer:
                 rolling_shutter_optimizer.step()
             if appearance_optimizer is not None:
                 appearance_optimizer.step()
+            if self._mcmc:  # the noise of iteration t at the position learning rate its optimiser step used
+                add_position_noise(self.scene.point_cloud, self.scene.point_cloud_features, self.scene.point_invalid_mask,
+                                   mc.noise_lr * position_optimizer.param_groups[0]["lr"], mc.seed, iteration, GATE_K,
+                                   mc.min_opacity)
             if iteration % cfg.position_learning_rate_decay_interval == 0:
                 scheduler.step()
-            self.adaptive_controller.refinement()
+            if self._mcmc:
+                self.mcmc_controller.refinement(MCMCMoments.of_optimizers(optimizer, position_optimizer, extra_optimizer))
+            else:
+                self.adaptive_controller.refinement()
             if log_interval and iteration % log_interval == 0:
                 entry = dict(iteration=iteration, loss=float(loss.detach()), l1=float(l1_loss.detach()),
                              psnr=psnr(image_pred.detach(), image_gt),
@@ -592,6 +641,8 @@ class GaussianPointCloudTrainer:
                     entry["feature_loss"] = float(feature_term.detach())
                 if self._appearance:
                     entry["appearance_tv"] = float(appearance_tv.detach())
+                if self._mcmc:
+                    entry["mcmc_opacity_reg"], entry["mcmc_scale_reg"] = mcmc_terms.detach().tolist()
                 self.history.append(entry)
         return self.history
 
