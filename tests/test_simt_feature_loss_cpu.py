@@ -50,7 +50,9 @@ def _check(out, term, grad, n_sup):
 KINDS_AND_CHANNELS = [("l2", 1)] + [(k, c) for k in ("cross_entropy", "l2") for c in (2, 3, 5, 8, 16)]
 
 
-@pytest.mark.parametrize("H,W", [(32, 48), (37, 29)])  # 37 x 29: odd, and not a multiple of the 256-thread CTA
+# 37 x 29: odd, and not a multiple of the 256-thread CTA.  272 x 976 = 265,472 pixels: more than the 1024 CTAs x 256 threads
+# of the capped grid, so both passes run their grid-stride loop twice, as on every real frame
+@pytest.mark.parametrize("H,W", [(32, 48), (37, 29), (272, 976)])
 @pytest.mark.parametrize("kind,C", KINDS_AND_CHANNELS)
 def test_feature_loss_source_matches_the_torch_loss(emu, kind, C, H, W):
     fmap, labels, target = _frame(H, W, C, H * 131 + W * 7 + C, kind)

@@ -69,7 +69,10 @@ CASES = {  # name: (depth weight, mask weight, background, mask given, depth kin
 }
 
 
-@pytest.mark.parametrize("H,W", [(32, 48), (37, 29)])  # 37 x 29: not a multiple of the 16-pixel tile, nor of 256 pixels
+# 37 x 29: not a multiple of the 16-pixel tile, nor of 256 pixels.  272 x 976 = 265,472 pixels: more than the 1024 CTAs x 256
+# threads of the capped grid, so both kernels run their grid-stride loop twice, as on every real frame (one emulated call
+# takes about 30 s on a CPU, so the repeated-call check stays on the small frames)
+@pytest.mark.parametrize("H,W", [(32, 48), (37, 29), (272, 976)])
 @pytest.mark.parametrize("name", sorted(CASES))
 def test_supervision_source_matches_the_torch_loss(emu, name, H, W):
     w_d, w_m, bg, with_mask, depth_kind = CASES[name]
@@ -79,9 +82,10 @@ def test_supervision_source_matches_the_torch_loss(emu, name, H, W):
     bg_arr = None if bg is None else np.array(bg, np.float32)
     temps = new_temps(emu, H, W)
     runs = [emulated_supervision_step(emu, image, gt, alpha, depth, d_target, mask, bg_arr, 0.2, w_d, w_m, temps=temps)
-            for _ in range(2)]
-    for a, b in zip(runs[0].__dict__.values(), runs[1].__dict__.values()):  # second call on the same temps: bit-identical
-        assert np.array_equal(a, b, equal_nan=True)
+            for _ in range(2 if H * W <= 256 * 1024 else 1)]
+    for again in runs[1:]:  # second call on the same temps: bit-identical
+        for a, b in zip(runs[0].__dict__.values(), again.__dict__.values()):
+            assert np.array_equal(a, b, equal_nan=True)
     out = runs[0]
     (total, l1, dssim, mterm, dterm), gI, gS, gD = _reference(image, gt, alpha, depth, d_target, mask, bg_arr, 0.2, w_d, w_m)
     assert abs(out.loss[0] - total) <= 2e-6 * max(1.0, abs(total)), (out.loss, total)
