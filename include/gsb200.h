@@ -725,6 +725,81 @@ int gsb200_train_step_mcmc(const GsbTrainStepArgs *args, const GsbSupervisionArg
                            const GsbFeatureTrainArgs *features, const GsbAppearanceArgs *appearance,
                            const GsbMcmcStepArgs *mcmc);
 
+/* 3D smoothing filter (an extension; Yu et al., "Mip-Splatting: Alias-free 3D Gaussian Splatting", CVPR 2024): every row
+ * is convolved in world space with an isotropic Gaussian whose std sigma_i >= 0 (scene units) is set by the finest sampling
+ * interval of the training views that see it, so that a scene rendered closer, at a larger focal length or at a higher
+ * resolution than any training view holds no frequency those views did not constrain.  filter3d is a float32 (N,) array,
+ * read-only and never differentiated; a NaN or negative entry is read as 0, invalid rows are never read.  Row layout as
+ * everywhere: features[4:7] = s (log-scales), features[7] = logit, o = sigmoid(logit).  With e_j = exp(s_j)^2 and
+ * e^_j = e_j + sigma^2:
+ *   rendered scale   s^_j = sqrt(e^_j)            (R orthogonal: Sigma^ = R diag(e^) R^T = Sigma + sigma^2 I exactly)
+ *   compensation     c = sqrt((e_0/e^_0)(e_1/e^_1)(e_2/e^_2)) in (0, 1]   (a product of ratios: no overflow)
+ *   rendered opacity o^ = o c
+ * Everything downstream of Sigma uses Sigma^ (J, Sigma', the compensated 0.3 low-pass, the radius, the tile box and the reach
+ * filter).  c is folded into the record's rescale slot (r1.y = rescale c) and r1.z keeps the raw o, so the blend's
+ * rescale * opacity product is rescale * o^ and no blend kernel changes; sigma = 0 leaves a row exactly as without the
+ * filter.  The per-point backward uses s^ in M = R diag(s^) and
+ *   dL/ds_j = (sum_l dM_lj R_lj) s^_j (e_j / e^_j) + G_a sigma^2 / e^_j,   dL/dlogit unchanged,
+ * where G_a = sum over pixels of dL/dalpha alpha is recovered as glogit / fl(1 - o) with o read from the frame's record; where
+ * fl(1 - o) = 0 (logit >~ 17.3) the compensation term of that row is dropped.  The gradient factors apply as without the
+ * filter; rescale, J(pc) and the SH direction stay detached.  Not implemented with camera-parameter gradients (pose,
+ * intrinsics, lens coefficients, motion) or the compact rows of the view-parallel exchange. */
+typedef struct GsbFilter3dArgs {
+    const float *filter3d;  /* (N,) sigma_i, 4-byte aligned */
+} GsbFilter3dArgs;
+/* gsb200_forward_rolling_shutter with the 3D filter.  NULL filter: exactly gsb200_forward_rolling_shutter.  GSB_EINVAL,
+ * before any CUDA call, for a NULL or not 4-byte aligned filter3d. */
+int gsb200_forward_filter3d(const GsbForwardArgs *args, const GsbExtraFeatureArgs *ext, const GsbLensArgs *lens,
+                            const GsbRollingShutterArgs *rs, const GsbFilter3dArgs *filter);
+/* gsb200_backward_rolling_shutter without the motion gradient, with the 3D filter the frame was rendered with (the same
+ * array).  NULL filter: exactly gsb200_backward_rolling_shutter(..., NULL).  GSB_EINVAL, before any CUDA call, for a NULL or
+ * not 4-byte aligned filter3d; GSB_EUNSUPPORTED with GSB_FLAG_COMPACT_GRADS. */
+int gsb200_backward_filter3d(const GsbBackwardArgs *args, const float *grad_rasterized_depth, const float *rasterized_depth,
+                             const float *grad_pixel_accumulated_alpha, const GsbExtraFeatureArgs *ext, const GsbLensArgs *lens,
+                             const GsbRollingShutterArgs *rs, const GsbFilter3dArgs *filter);
+/* gsb200_train_step_mcmc with the 3D filter in its forward and backward.  NULL filter: exactly gsb200_train_step_mcmc.
+ * GSB_EINVAL, before any CUDA call, for a NULL or not 4-byte aligned filter3d. */
+int gsb200_train_step_filter3d(const GsbTrainStepArgs *args, const GsbSupervisionArgs *supervision,
+                               const GsbFeatureTrainArgs *features, const GsbAppearanceArgs *appearance,
+                               const GsbMcmcStepArgs *mcmc, const GsbFilter3dArgs *filter);
+/* The filter from the training views.  For a valid row i and a view v with full-resolution K_v, W_v, H_v and the pose of the
+ * row's object in that view, mapped as the rasteriser maps it (the forward's pose kernel):
+ *   pc = T x,  (u, v) = (K pc)[:2] / z   (pinhole, float32, the preprocess's operation order)
+ *   v sees i  iff  z > near_plane  and  -0.15 W <= u <= 1.15 W  and  -0.15 H <= v <= 1.15 H   (bounds formed in float32)
+ *   d_i = min over the views that see i of z / f_v,  f_v = fmaxf(K00, K11)   (a view with f_v <= 0 sees nothing, and
+ *   neither does one with a NaN K00 or K11: u or v is then NaN); a row whose object id is outside [0, num_objects) matches
+ *   no view
+ *   a valid row no view sees gets the largest d of the seen rows; if no row is seen, every row gets 0
+ *   filter3d_i = sqrt(variance) d_i  (variance in pixels^2 at the finest view; the paper's value is 0.2);  invalid rows: 0.
+ * The paper takes the minimum distance over one focal length; this takes the per-view z / f, which equals it for views of
+ * one focal length and is the sampling interval itself when they differ.  Every step is a min or a max: bit-deterministic.
+ * The views' pose blocks, K, W and H are staged through shared memory in chunks, so any number of views and objects works.
+ * Lens distortion and rolling shutters are not modelled here: callers pass the pinhole K and the mid-readout pose. */
+typedef struct GsbFilter3dViewsArgs {
+    int64_t num_points;
+    const float *pointcloud;            /* (N,3) */
+    const int8_t *point_invalid_mask;   /* (N,) */
+    const int32_t *point_object_id;     /* (N,) in [0, num_objects) */
+    int32_t num_objects;                /* >= 1 */
+    int32_t num_views;                  /* >= 1 */
+    const float *q_pointcloud_camera;   /* (V, num_objects, 4) xyzw, camera -> pointcloud, as the forward takes them */
+    const float *t_pointcloud_camera;   /* (V, num_objects, 3) */
+    const float *camera_intrinsics;     /* (V, 3, 3) full resolution */
+    const int32_t *camera_size;         /* (V, 2) {W, H}, full resolution */
+    float near_plane;                   /* finite, >= 0 */
+    float variance;                     /* finite, >= 0 */
+    float *filter3d;                    /* (N,) out, 4-byte aligned */
+    void *temp;                         /* gsb200_filter3d_temp_bytes(V, num_objects) bytes, 16-byte aligned */
+    int64_t temp_bytes;
+    void *stream;
+} GsbFilter3dViewsArgs;
+int64_t gsb200_filter3d_temp_bytes(int32_t num_views, int32_t num_objects);
+/* GSB_EINVAL, before any CUDA call, for a NULL args, num_points < 0, num_views < 1, num_objects < 1, a NULL or misaligned
+ * pointer, a temp smaller than gsb200_filter3d_temp_bytes, or a near plane or variance that is negative or not finite. */
+int gsb200_filter3d_from_views(const GsbFilter3dViewsArgs *args);
+/* sizeof(GsbFilter3dArgs), sizeof(GsbFilter3dViewsArgs) */
+void gsb200_abi_sizes_filter3d(int64_t *out2);
+
 /* Individual stages (same workspace), for tests and profiling. */
 int gsb200_stage_preprocess(const GsbForwardArgs *args);   /* K1+P1+K2+K3+P2+K4 fused */
 int gsb200_stage_sort(const GsbForwardArgs *args);         /* P3 */

@@ -361,14 +361,16 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
             @staticmethod
             def forward(ctx, pointcloud, pointcloud_features, point_invalid_mask, point_object_id,
                         q_pointcloud_camera, t_pointcloud_camera, camera_info, color_max_sh_band, extra_features=None,
-                        camera_intrinsics=None, lens_coefficients=None, rolling_shutter_motion=None):
+                        camera_intrinsics=None, lens_coefficients=None, rolling_shutter_motion=None, point_filter_3d=None):
                 # camera_intrinsics (differentiable_intrinsics): camera_info.camera_intrinsics itself, passed again only so
                 # that autograd tracks it; lens_coefficients (differentiable_distortion): the coefficients rendered;
-                # rolling_shutter_motion (differentiable_rolling_shutter): the motion rendered
+                # rolling_shutter_motion (differentiable_rolling_shutter): the motion rendered; point_filter_3d: the 3D
+                # smoothing filter (never differentiated)
                 outs, frame, saved = outer._run_forward(
                     pointcloud, pointcloud_features, point_invalid_mask, point_object_id,
                     q_pointcloud_camera, t_pointcloud_camera, camera_info, extra_features, lens_coefficients,
-                    rolling_shutter_motion)
+                    rolling_shutter_motion, point_filter_3d)
+                ctx.filter_3d = point_filter_3d  # read by the backward of this frame (the forward's array)
                 image, depth, acc_alpha, last_effective, valid_count = outs[:5]
                 ctx.save_for_backward(pointcloud, pointcloud_features, point_object_id,
                                       t_pointcloud_camera, saved["camera_intrinsics"], acc_alpha,
@@ -400,7 +402,14 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                 return result
 
             @staticmethod
-            def backward(ctx, grad_rasterized_image, grad_rasterized_depth, grad_pixel_valid_point_count, *grad_extra):
+            def backward(ctx, *grads):
+                result = _module_function._grads(ctx, *grads)
+                if ctx.filter_3d is not None:  # thirteen inputs: the filter's slot ends the list and gets no gradient
+                    result = tuple(result) + (None,) * (13 - len(result))
+                return result
+
+            @staticmethod
+            def _grads(ctx, grad_rasterized_image, grad_rasterized_depth, grad_pixel_valid_point_count, *grad_extra):
                 # grad_extra: dL/d pixel_accumulated_alpha (differentiable_alpha), then dL/d the feature map (extra features)
                 grad_pixel_accumulated_alpha = grad_extra[0] if outer.differentiable_alpha else None
                 grad_feature_map = grad_extra[-1] if ctx.has_extra_features else None
@@ -496,9 +505,31 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
         if not extra_features.is_contiguous():
             raise ValueError("point_extra_features must be contiguous")
 
+    def _check_filter_3d(self, point_filter_3d, pointcloud):
+        """The ``point_filter_3d`` argument of ``forward``: (N,) float32, contiguous, on the scene's device, and an operator
+        without camera-parameter gradients or a gradient exchange."""
+        for name, on in (("differentiable_pose", self.differentiable_pose),
+                         ("differentiable_intrinsics", self.differentiable_intrinsics),
+                         ("differentiable_distortion", self.differentiable_distortion),
+                         ("differentiable_rolling_shutter", self.differentiable_rolling_shutter),
+                         ("a gradient_exchange", self.gradient_exchange is not None)):
+            if on:
+                raise ValueError(f"point_filter_3d is not supported with {name}")
+        if not isinstance(point_filter_3d, torch.Tensor):
+            raise ValueError("point_filter_3d must be a torch.Tensor")
+        N = pointcloud.shape[0]
+        if tuple(point_filter_3d.shape) != (N,):
+            raise ValueError(f"point_filter_3d must have shape ({N},), got {tuple(point_filter_3d.shape)}")
+        if point_filter_3d.dtype != torch.float32:
+            raise ValueError(f"point_filter_3d must be float32, got {point_filter_3d.dtype}")
+        if point_filter_3d.device != pointcloud.device:
+            raise ValueError(f"point_filter_3d must be on {pointcloud.device}, got {point_filter_3d.device}")
+        if not point_filter_3d.is_contiguous():
+            raise ValueError("point_filter_3d must be contiguous")
+
     def _run_forward(self, pointcloud, pointcloud_features, point_invalid_mask, point_object_id,
                      q_pointcloud_camera, t_pointcloud_camera, camera_info, extra_features=None, lens_coefficients=None,
-                     rolling_shutter_motion=None):
+                     rolling_shutter_motion=None, point_filter_3d=None):
         cfg = self.config
         lib = _lib.load()
         lens = self._lens_args(camera_info, lens_coefficients)
@@ -570,7 +601,12 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                         host_counters=pinned.data_ptr(), host_counters_event=event.cuda_event)
                     # The whole frame is enqueued by this one call; the library copies {M, K, overflow} to pinned
                     # host memory right after the per-point stage and records `event` behind that copy.
-                    if rs is not None:
+                    if point_filter_3d is not None:
+                        _lib.check(lib.gsb200_forward_filter3d(
+                            ctypes.byref(args), ctypes.byref(ext) if ext is not None else None,
+                            ctypes.byref(lens) if lens is not None else None, ctypes.byref(rs) if rs is not None else None,
+                            ctypes.byref(_lib.GsbFilter3dArgs(filter3d=_ptr(point_filter_3d)))), "gsb200_forward_filter3d")
+                    elif rs is not None:
                         _lib.check(lib.gsb200_forward_rolling_shutter(
                             ctypes.byref(args), ctypes.byref(ext) if ext is not None else None,
                             ctypes.byref(lens) if lens is not None else None, ctypes.byref(rs)),
@@ -738,7 +774,19 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                 grad_extra_features = torch.zeros((N, C), dtype=torch.float32, device=device) if grad_feature_map is None \
                     else torch.empty((N, C), dtype=torch.float32, device=device)
             grad_q = grad_t = grad_K = grad_k = grad_m = None
-            if ctx.rolling_shutter is not None:  # neither pose, intrinsics nor lens gradients (refused in forward)
+            if ctx.filter_3d is not None:  # no camera-parameter gradient (refused in forward)
+                ext = None
+                if extra_features is not None and grad_feature_map is not None:
+                    grad_map = _f32(grad_feature_map)
+                    ext = _lib.GsbExtraFeatureArgs(channels=extra_features.shape[1], features=_ptr(extra_features),
+                                                   grad_rasterized=_ptr(grad_map), grad_features=_ptr(grad_extra_features))
+                rs = ctx.rolling_shutter[0] if ctx.rolling_shutter is not None else None
+                _lib.check(lib.gsb200_backward_filter3d(
+                    ctypes.byref(args), _ptr(grad_depth), _ptr(depth), _ptr(grad_alpha),
+                    ctypes.byref(ext) if ext is not None else None, ctypes.byref(ctx.lens) if ctx.lens is not None else None,
+                    ctypes.byref(rs) if rs is not None else None,
+                    ctypes.byref(_lib.GsbFilter3dArgs(filter3d=_ptr(ctx.filter_3d)))), "gsb200_backward_filter3d")
+            elif ctx.rolling_shutter is not None:  # neither pose, intrinsics nor lens gradients (refused in forward)
                 rs, _row_time = ctx.rolling_shutter
                 ext = None
                 if extra_features is not None and grad_feature_map is not None:
@@ -874,7 +922,7 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
     # ------------------------------------------------------------------ public forward (GPCR:1184-1204)
     def forward(self, input_data: "GaussianPointCloudRasterisation.GaussianPointCloudRasterisationInput",
                 point_extra_features: Optional[torch.Tensor] = None, lens_coefficients: Optional[torch.Tensor] = None,
-                rolling_shutter_motion: Optional[torch.Tensor] = None):
+                rolling_shutter_motion: Optional[torch.Tensor] = None, point_filter_3d: Optional[torch.Tensor] = None):
         """Returns (image, depth, pixel_valid_point_count), then pixel_accumulated_alpha with ``differentiable_alpha``.
         ``point_extra_features`` (an extension): an (N, C) float32 tensor of per-Gaussian values (1 <= C <= 16; semantic
         logits, instance encodings, distilled features, ...), contiguous, on the scene's device.  The output tuple then
@@ -905,10 +953,33 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
         any device.  Its values are the motion rendered, and the backward returns dL/d ``rolling_shutter_motion`` on the
         tensor's device.  The values are read on the host like ``lens_coefficients``.  ``ValueError`` for a camera without
         a rolling shutter, a tensor of the wrong shape or dtype, or an operator without the option.  None: no motion
-        gradient."""
+        gradient.
+        ``point_filter_3d`` (an extension; ``mip_filter.compute_filter_3d``): an (N,) float32 tensor of per-Gaussian 3D
+        smoothing filter stds sigma >= 0, contiguous, on the scene's device.  Every Gaussian is rendered convolved with an
+        isotropic Gaussian of std sigma: scales sqrt(exp(s)^2 + sigma^2) and opacity o times the compensation c
+        (``gsb200_forward_filter3d`` / ``gsb200_backward_filter3d``; definition in ``include/gsb200.h``); the stored rows are
+        not changed, and the gradients are with respect to them.  The filter gets no gradient.  Works with extra features,
+        depth, alpha, every lens, a rolling shutter and either backward kernel for an image-only loss.  ``ValueError`` with
+        ``differentiable_pose``, ``differentiable_intrinsics``, ``differentiable_distortion``,
+        ``differentiable_rolling_shutter``, a ``gradient_exchange``, ``lens_coefficients``, ``rolling_shutter_motion``, or a
+        tensor of the wrong shape, dtype, device or layout."""
         camera_info = input_data.camera_info
         assert camera_info.camera_width % TILE_WIDTH == 0
         assert camera_info.camera_height % TILE_HEIGHT == 0
+        if point_filter_3d is not None:  # lens coefficients, K and the motion are refused with it: their slots are None
+            for name, value in (("lens_coefficients", lens_coefficients), ("rolling_shutter_motion", rolling_shutter_motion)):
+                if value is not None:
+                    raise ValueError(f"point_filter_3d is not supported with {name} (no camera-parameter gradient with the "
+                                     "filter)")
+            self._check_filter_3d(point_filter_3d, input_data.point_cloud)
+            if point_extra_features is not None:
+                self._check_extra_features(point_extra_features, input_data.point_cloud)
+            self._lens_args(camera_info)  # the lens and rolling-shutter checks, before any device work
+            self._rolling_shutter_args(camera_info)
+            return self._module_function.apply(
+                input_data.point_cloud, input_data.point_cloud_features, input_data.point_invalid_mask,
+                input_data.point_object_id, input_data.q_pointcloud_camera, input_data.t_pointcloud_camera, camera_info,
+                input_data.color_max_sh_band, point_extra_features, None, None, None, point_filter_3d)
         if rolling_shutter_motion is not None:  # the extra features', K's and the coefficients' slots first (all refused)
             self._rolling_shutter_args(camera_info, rolling_shutter_motion)  # the argument checks, before any device work
             if point_extra_features is not None:

@@ -165,6 +165,19 @@ class GsbMcmcStepArgs(ctypes.Structure):
     ]
 
 
+class GsbFilter3dArgs(ctypes.Structure):
+    _fields_ = [("filter3d", c_vp)]
+
+
+class GsbFilter3dViewsArgs(ctypes.Structure):
+    _fields_ = [
+        ("num_points", c_i64), ("pointcloud", c_vp), ("point_invalid_mask", c_vp), ("point_object_id", c_vp),
+        ("num_objects", c_i32), ("num_views", c_i32), ("q_pointcloud_camera", c_vp), ("t_pointcloud_camera", c_vp),
+        ("camera_intrinsics", c_vp), ("camera_size", c_vp), ("near_plane", c_f32), ("variance", c_f32), ("filter3d", c_vp),
+        ("temp", c_vp), ("temp_bytes", c_i64), ("stream", c_vp),
+    ]
+
+
 def lens_args(distortion) -> GsbLensArgs:
     """The C argument of a ``Camera.LensDistortion`` (host floats; unused coefficients 0)."""
     model = {"opencv": GSB_LENS_OPENCV, "fisheye": GSB_LENS_FISHEYE}[distortion.model]
@@ -200,7 +213,8 @@ EXPORTS = (
     "gsb200_backward_rolling_shutter", "gsb200_rolling_shutter_grad_temp_bytes", "gsb200_bilateral_grid_temp_bytes",
     "gsb200_bilateral_grid_forward", "gsb200_bilateral_grid_backward", "gsb200_train_step_appearance",
     "gsb200_mcmc_temp_bytes", "gsb200_mcmc_regulariser", "gsb200_mcmc_noise", "gsb200_mcmc_relocate", "gsb200_train_step_mcmc",
-    "gsb200_abi_sizes_mcmc",
+    "gsb200_abi_sizes_mcmc", "gsb200_forward_filter3d", "gsb200_backward_filter3d", "gsb200_train_step_filter3d",
+    "gsb200_filter3d_temp_bytes", "gsb200_filter3d_from_views", "gsb200_abi_sizes_filter3d",
 )
 
 _lib = None
@@ -307,6 +321,22 @@ def load() -> ctypes.CDLL:
                                            ctypes.POINTER(GsbFeatureTrainArgs), ctypes.POINTER(GsbAppearanceArgs),
                                            ctypes.POINTER(GsbMcmcStepArgs)]
     lib.gsb200_train_step_mcmc.restype = ctypes.c_int
+    lib.gsb200_forward_filter3d.argtypes = [ctypes.POINTER(GsbForwardArgs), ctypes.POINTER(GsbExtraFeatureArgs),
+                                            ctypes.POINTER(GsbLensArgs), ctypes.POINTER(GsbRollingShutterArgs),
+                                            ctypes.POINTER(GsbFilter3dArgs)]
+    lib.gsb200_forward_filter3d.restype = ctypes.c_int
+    lib.gsb200_backward_filter3d.argtypes = [ctypes.POINTER(GsbBackwardArgs), c_vp, c_vp, c_vp, ctypes.POINTER(GsbExtraFeatureArgs),
+                                             ctypes.POINTER(GsbLensArgs), ctypes.POINTER(GsbRollingShutterArgs),
+                                             ctypes.POINTER(GsbFilter3dArgs)]
+    lib.gsb200_backward_filter3d.restype = ctypes.c_int
+    lib.gsb200_train_step_filter3d.argtypes = [ctypes.POINTER(GsbTrainStepArgs), ctypes.POINTER(GsbSupervisionArgs),
+                                               ctypes.POINTER(GsbFeatureTrainArgs), ctypes.POINTER(GsbAppearanceArgs),
+                                               ctypes.POINTER(GsbMcmcStepArgs), ctypes.POINTER(GsbFilter3dArgs)]
+    lib.gsb200_train_step_filter3d.restype = ctypes.c_int
+    lib.gsb200_filter3d_temp_bytes.argtypes = [c_i32, c_i32]
+    lib.gsb200_filter3d_temp_bytes.restype = c_i64
+    lib.gsb200_filter3d_from_views.argtypes = [ctypes.POINTER(GsbFilter3dViewsArgs)]
+    lib.gsb200_filter3d_from_views.restype = ctypes.c_int
     lib.gsb200_mcmc_temp_bytes.argtypes = []
     lib.gsb200_mcmc_temp_bytes.restype = c_i64
     lib.gsb200_mcmc_regulariser.argtypes = [c_vp, c_vp, c_vp, c_i64, c_i64, c_f32, c_f32, c_vp, c_vp, c_vp]
@@ -405,6 +435,14 @@ def load() -> ctypes.CDLL:
     for i, mirror in ((0, GsbMcmcRelocateArgs), (1, GsbMcmcStepArgs)):
         if sizes_mcmc[i] != ctypes.sizeof(mirror):
             raise RuntimeError(f"libgsb200.so ABI mismatch: sizeof({mirror.__name__}) {sizes_mcmc[i]} != ctypes mirror "
+                               f"{ctypes.sizeof(mirror)}")
+    lib.gsb200_abi_sizes_filter3d.argtypes = [ctypes.POINTER(c_i64)]
+    lib.gsb200_abi_sizes_filter3d.restype = None
+    sizes_filter = (c_i64 * 2)()
+    lib.gsb200_abi_sizes_filter3d(sizes_filter)
+    for i, mirror in ((0, GsbFilter3dArgs), (1, GsbFilter3dViewsArgs)):
+        if sizes_filter[i] != ctypes.sizeof(mirror):
+            raise RuntimeError(f"libgsb200.so ABI mismatch: sizeof({mirror.__name__}) {sizes_filter[i]} != ctypes mirror "
                                f"{ctypes.sizeof(mirror)}")
     _lib = lib
     return lib

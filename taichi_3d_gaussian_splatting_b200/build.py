@@ -2,7 +2,7 @@
 
     python -m taichi_3d_gaussian_splatting_b200.build [--force] [--verbose]
 
-``preprocess.cu`` is compiled with ``-fmad=false`` so that every per-point discrete decision is
+``preprocess.cu`` and ``filter3d.cu`` are compiled with ``-fmad=false`` so that every per-point discrete decision is
 bit-reproducible against the CPU oracle; the blend kernels use default FMA contraction.
 """
 import hashlib
@@ -35,6 +35,7 @@ SOURCES = {
     "appearance.cu": [],
     "adam.cu": [],
     "mcmc.cu": [],
+    "filter3d.cu": ["-fmad=false"],
     "controller.cu": [],
     "exchange.cu": [],
 }

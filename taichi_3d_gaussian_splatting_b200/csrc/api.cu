@@ -206,6 +206,11 @@ void gsb200_abi_sizes_mcmc(int64_t *out2) {
     out2[1] = (int64_t)sizeof(GsbMcmcStepArgs);
 }
 
+void gsb200_abi_sizes_filter3d(int64_t *out2) {
+    out2[0] = (int64_t)sizeof(GsbFilter3dArgs);
+    out2[1] = (int64_t)sizeof(GsbFilter3dViewsArgs);
+}
+
 int gsb200_workspace_layout(int64_t num_points, int32_t num_objects, int64_t key_capacity,
                             int32_t camera_height, int32_t camera_width, float far_plane,
                             float depth_to_sort_key_scale, uint32_t flags, GsbWorkspaceLayout *out) {
@@ -311,6 +316,27 @@ int64_t gsb200_rolling_shutter_grad_temp_bytes(void) {
 
 int gsb200_forward_rolling_shutter(const GsbForwardArgs *a, const GsbExtraFeatureArgs *ext, const GsbLensArgs *lens_args,
                                    const GsbRollingShutterArgs *rs_args) {
+    return gsb200_forward_filter3d(a, ext, lens_args, rs_args, nullptr);
+}
+
+// GsbFilter3dArgs -> the (N,) filter array; GSB_EINVAL for a NULL or not 4-byte aligned array.  *out stays NULL for a NULL
+// filter.
+static int check_filter3d(const char *what, const GsbFilter3dArgs *filter, const float **out) {
+    *out = nullptr;
+    if (!filter) return GSB_OK;
+    if (!filter->filter3d || reinterpret_cast<uintptr_t>(filter->filter3d) % 4 != 0) {
+        set_error("%s: filter3d is NULL or not 4-byte aligned", what);
+        return GSB_EINVAL;
+    }
+    *out = filter->filter3d;
+    return GSB_OK;
+}
+
+int gsb200_forward_filter3d(const GsbForwardArgs *a, const GsbExtraFeatureArgs *ext, const GsbLensArgs *lens_args,
+                            const GsbRollingShutterArgs *rs_args, const GsbFilter3dArgs *filter) {
+    const float *filter3d;
+    int frc = check_filter3d("forward_filter3d", filter, &filter3d);
+    if (frc != GSB_OK) return frc;
     LensParams lens_params;
     const LensParams *lens;
     int lrc = check_lens(rs_args ? "forward_rolling_shutter" : "forward_lens", lens_args, &lens_params, &lens);
@@ -336,7 +362,7 @@ int gsb200_forward_rolling_shutter(const GsbForwardArgs *a, const GsbExtraFeatur
     int rc = resolve_fwd(a, &ws);
     if (rc != GSB_OK) return rc;
     cudaStream_t st = static_cast<cudaStream_t>(a->stream);
-    if ((rc = launch_preprocess(*a, ws, st, lens, rs)) != GSB_OK) return rc;
+    if ((rc = launch_preprocess(*a, ws, st, lens, rs, filter3d)) != GSB_OK) return rc;
     if (a->host_counters && a->host_counters_event) {
         GSB_CUDA_CHECK(cudaMemcpyAsync(a->host_counters, ws.counters, 4 * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
         GSB_CUDA_CHECK(cudaEventRecord(static_cast<cudaEvent_t>(a->host_counters_event), st));
@@ -354,7 +380,7 @@ static int backward_impl(const GsbBackwardArgs *a, bool skip_on_overflow, const 
                          const GsbExtraFeatureArgs *ext = nullptr, const GsbPoseGradArgs *pose = nullptr,
                          const GsbIntrinsicsGradArgs *intr = nullptr, const LensParams *lens = nullptr,
                          const GsbLensGradArgs *lens_grad = nullptr, const RsParams *rs = nullptr,
-                         const GsbRollingShutterGradArgs *rs_grad = nullptr) {
+                         const GsbRollingShutterGradArgs *rs_grad = nullptr, const float *filter3d = nullptr) {
     if (!a) {
         set_error("backward: args is null");
         return GSB_EINVAL;
@@ -408,6 +434,9 @@ static int backward_impl(const GsbBackwardArgs *a, bool skip_on_overflow, const 
     if (ext && a->num_points > 0)  // the blend adds into the rows it reaches; every other row stays zero
         GSB_CUDA_CHECK(cudaMemsetAsync(ext->grad_features, 0, (size_t)a->num_points * ext->channels * 4, st));
     if ((rc = launch_blend_backward(*a, ws, st, grad_depth, depth, grad_alpha, ext)) != GSB_OK) return rc;
+    if (filter3d)
+        return launch_backward_points_filter(*a, ws, st, skip_on_overflow ? ws.counters + CNT_OVERFLOW : nullptr,
+                                             grad_depth != nullptr, lens, rs, filter3d);
     if (rs) return launch_backward_points_rs(*a, ws, st, grad_depth != nullptr, lens, *rs, rs_grad);
     if (lens && lens_grad) return launch_backward_points_lens_grad(*a, ws, st, grad_depth != nullptr, *lens, *lens_grad);
     if (lens) return launch_backward_points_lens(*a, ws, st, grad_depth != nullptr, *lens);
@@ -434,7 +463,32 @@ int gsb200_backward_ext(const GsbBackwardArgs *a, const float *grad_rasterized_d
 static int backward_checked(const GsbBackwardArgs *a, const float *grad_rasterized_depth, const float *rasterized_depth,
                             const float *grad_pixel_accumulated_alpha, const GsbExtraFeatureArgs *ext, const GsbPoseGradArgs *pose,
                             const GsbIntrinsicsGradArgs *intr, const LensParams *lens, const GsbLensGradArgs *lens_grad = nullptr,
-                            const RsParams *rs = nullptr, const GsbRollingShutterGradArgs *rs_grad = nullptr);
+                            const RsParams *rs = nullptr, const GsbRollingShutterGradArgs *rs_grad = nullptr,
+                            const float *filter3d = nullptr);
+
+int gsb200_backward_filter3d(const GsbBackwardArgs *a, const float *grad_rasterized_depth, const float *rasterized_depth,
+                             const float *grad_pixel_accumulated_alpha, const GsbExtraFeatureArgs *ext, const GsbLensArgs *lens_args,
+                             const GsbRollingShutterArgs *rs_args, const GsbFilter3dArgs *filter) {
+    if (!filter)
+        return gsb200_backward_rolling_shutter(a, grad_rasterized_depth, rasterized_depth, grad_pixel_accumulated_alpha, ext,
+                                               lens_args, rs_args, nullptr);
+    const float *filter3d;
+    int rc = check_filter3d("backward_filter3d", filter, &filter3d);
+    if (rc != GSB_OK) return rc;
+    LensParams lens_params;
+    const LensParams *lens;
+    if ((rc = check_lens("backward_filter3d", lens_args, &lens_params, &lens)) != GSB_OK) return rc;
+    RsParams rs_params;
+    const RsParams *rs;
+    if ((rc = check_rs("backward_filter3d", rs_args, &rs_params, &rs)) != GSB_OK) return rc;
+    if (a != nullptr && (a->flags & GSB_FLAG_COMPACT_GRADS)) {
+        set_error("backward_filter3d: the 3D filter is not implemented for the compact rows of the view-parallel exchange "
+                  "(GSB_FLAG_COMPACT_GRADS)");
+        return GSB_EUNSUPPORTED;
+    }
+    return backward_checked(a, grad_rasterized_depth, rasterized_depth, grad_pixel_accumulated_alpha, ext, nullptr, nullptr, lens,
+                            nullptr, rs, nullptr, filter3d);
+}
 
 int gsb200_backward_rolling_shutter(const GsbBackwardArgs *a, const float *grad_rasterized_depth, const float *rasterized_depth,
                                     const float *grad_pixel_accumulated_alpha, const GsbExtraFeatureArgs *ext,
@@ -550,7 +604,7 @@ int gsb200_backward_calib(const GsbBackwardArgs *a, const float *grad_rasterized
 static int backward_checked(const GsbBackwardArgs *a, const float *grad_rasterized_depth, const float *rasterized_depth,
                             const float *grad_pixel_accumulated_alpha, const GsbExtraFeatureArgs *ext, const GsbPoseGradArgs *pose,
                             const GsbIntrinsicsGradArgs *intr, const LensParams *lens, const GsbLensGradArgs *lens_grad,
-                            const RsParams *rs, const GsbRollingShutterGradArgs *rs_grad) {
+                            const RsParams *rs, const GsbRollingShutterGradArgs *rs_grad, const float *filter3d) {
     if (intr) {
         if (!intr->grad_camera_intrinsics || !intr->temp) {
             set_error("backward_calib: null grad_camera_intrinsics / temp pointer");
@@ -616,7 +670,7 @@ static int backward_checked(const GsbBackwardArgs *a, const float *grad_rasteriz
         return GSB_EUNSUPPORTED;
     }
     return backward_impl(a, false, grad_rasterized_depth, rasterized_depth, grad_pixel_accumulated_alpha, ext, pose, intr, lens,
-                         lens_grad, rs, rs_grad);
+                         lens_grad, rs, rs_grad, filter3d);
 }
 
 int gsb200_backward_with_depth(const GsbBackwardArgs *a, const float *grad_rasterized_depth, const float *rasterized_depth) {
@@ -782,6 +836,14 @@ int gsb200_mcmc_noise(float *pointcloud, const float *features, const int8_t *in
 
 int gsb200_train_step_mcmc(const GsbTrainStepArgs *t, const GsbSupervisionArgs *s, const GsbFeatureTrainArgs *x,
                            const GsbAppearanceArgs *app, const GsbMcmcStepArgs *mc) {
+    return gsb200_train_step_filter3d(t, s, x, app, mc, nullptr);
+}
+
+int gsb200_train_step_filter3d(const GsbTrainStepArgs *t, const GsbSupervisionArgs *s, const GsbFeatureTrainArgs *x,
+                               const GsbAppearanceArgs *app, const GsbMcmcStepArgs *mc, const GsbFilter3dArgs *filter) {
+    const float *filter3d;
+    int frc = check_filter3d("train_step_filter3d", filter, &filter3d);
+    if (frc != GSB_OK) return frc;
     if (!t || !t->ground_truth_image || !t->loss_out3 || !t->loss_temp || !t->feature_exp_avg || !t->feature_exp_avg_sq ||
         !t->position_exp_avg || !t->position_exp_avg_sq || t->step < 1) {
         set_error("train_step: null pointer argument or step < 1");
@@ -860,7 +922,7 @@ int gsb200_train_step_mcmc(const GsbTrainStepArgs *t, const GsbSupervisionArgs *
     }
     const GsbExtraFeatureArgs *ext = x ? &x->features : nullptr;
     cudaStream_t st = static_cast<cudaStream_t>(f.stream);
-    if ((rc = gsb200_forward_ext(&f, ext)) != GSB_OK) return rc;
+    if ((rc = gsb200_forward_filter3d(&f, ext, nullptr, nullptr, filter)) != GSB_OK) return rc;
     const float *loss_image = f.rasterized_image, *loss_gt = t->ground_truth_image;
     if (supervised && (rc = launch_supervision_pre(*s, f.rasterized_image, t->ground_truth_image, f.pixel_accumulated_alpha,
                                                    f.rasterized_depth, H, W, st, &loss_image, &loss_gt)) != GSB_OK)
@@ -885,7 +947,8 @@ int gsb200_train_step_mcmc(const GsbTrainStepArgs *t, const GsbSupervisionArgs *
         return rc;
     if (x && (rc = launch_feature_loss(*x, H, W, st)) != GSB_OK) return rc;
     if ((rc = backward_impl(&b, true, depth_on ? s->grad_depth : nullptr, depth_on ? f.rasterized_depth : nullptr,
-                            alpha_on ? s->grad_pixel_accumulated_alpha : nullptr, ext)) != GSB_OK)
+                            alpha_on ? s->grad_pixel_accumulated_alpha : nullptr, ext, nullptr, nullptr, nullptr, nullptr,
+                            nullptr, nullptr, filter3d)) != GSB_OK)
         return rc;
     Workspace ws;
     if ((rc = resolve_fwd(&f, &ws)) != GSB_OK) return rc;

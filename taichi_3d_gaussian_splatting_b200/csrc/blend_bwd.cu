@@ -430,20 +430,28 @@ __device__ __forceinline__ void weighted_u_sigma(const float *U, const float *R,
 // which the warp sums (fixed butterfly order, all objects together: a frame has one motion) into the per-warp row
 // s_mgrad[warp][6]; after the loop the CTA adds its warps' rows in warp order into mgrad_partials[blockIdx.x][6], and
 // rolling_shutter_grad_finish_kernel adds the blocks in block order.
+// FILTER = true (gsb200_backward_filter3d): the frame was rendered with the 3D smoothing filter sigma = fmaxf(filter3d[id], 0)
+// (include/gsb200.h): s^_j = sqrt(e_j + sigma^2), e_j = exp(s_j)^2, replaces exp(s_j) in M = R diag(s^), and
+//   dL/ds_j = (sum_l dM_lj R_lj) s^_j (e_j / e^_j) + G_a sigma^2 / e^_j,   G_a = glogit / fl(1 - o)
+// where o is the record's raw opacity r1.z (the float the blend multiplied by); the compensation term is dropped where
+// fl(1 - o) = 0.  dL/dlogit is unchanged: the compensation c does not depend on the logit.  Non-compact, without POSE / INTR /
+// LGRAD / MGRAD.
 constexpr int LENS_GRAD_VALUES = 5;
 constexpr int RS_GRAD_VALUES = 6;
 template <bool COMPACT, bool DEPTH, bool POSE, bool INTR = false, bool LENS = false, bool LGRAD = false, bool RS = false,
-          bool MGRAD = false>
+          bool MGRAD = false, bool FILTER = false>
 __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, float *s_pose, float *pose_partials,
                                                      int num_objects, float *s_intr = nullptr,
                                                      float *intr_partials = nullptr, const LensParams lens = LensParams(),
                                                      float *s_lgrad = nullptr, float *lgrad_partials = nullptr,
                                                      const RsParams rs = RsParams(), float *s_mgrad = nullptr,
-                                                     float *mgrad_partials = nullptr) {
+                                                     float *mgrad_partials = nullptr, const float *filter3d = nullptr) {
     static_assert(!LENS || (!COMPACT && !POSE && !INTR), "the lens gradient is implemented for the dense rows alone");
     static_assert(!LGRAD || LENS, "the coefficient gradient needs the lens path");
     static_assert(!RS || (!COMPACT && !POSE && !INTR && !LGRAD), "the rolling shutter is implemented for the dense rows alone");
     static_assert(!MGRAD || RS, "the motion gradient needs the rolling-shutter path");
+    static_assert(!FILTER || (!COMPACT && !POSE && !INTR && !LGRAD && !MGRAD),
+                  "the 3D filter is implemented for the dense rows without camera gradients");
     // One thread per scene row: rows outside the frustum get their zeros here (no separate memset of the
     // dense (N,3)/(N,56) gradients), rows inside get the chain rule.  A warp owns 32 consecutive rows, i.e. one
     // contiguous 7 KB piece of the (N,56) gradient and 384 B of the (N,3) one: each lane stages its row in
@@ -585,7 +593,25 @@ __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, fl
         R[0] = 1 - 2 * (qy * qy + qz * qz); R[1] = 2 * (qx * qy - qw * qz); R[2] = 2 * (qx * qz + qw * qy);
         R[3] = 2 * (qx * qy + qw * qz); R[4] = 1 - 2 * (qx * qx + qz * qz); R[5] = 2 * (qy * qz - qw * qx);
         R[6] = 2 * (qx * qz - qw * qy); R[7] = 2 * (qy * qz + qw * qx); R[8] = 1 - 2 * (qx * qx + qy * qy);
-        const float es[3] = {expf(sv.x), expf(sv.y), expf(sv.z)};
+        float es[3] = {expf(sv.x), expf(sv.y), expf(sv.z)};  // FILTER: s^
+        float fr[3] = {1.0f, 1.0f, 1.0f}, fcomp[3] = {0.0f, 0.0f, 0.0f};  // FILTER: e / e^ and G_a sigma^2 / e^
+        bool filtered = false;  // FILTER: sigma > 0 (sigma = 0 leaves the row's gradient exactly as unfiltered)
+        if (FILTER) {
+            const float sg = fmaxf(filter3d[id], 0.0f);  // NaN -> 0, as the forward
+            const float s2 = sg * sg;
+            filtered = s2 > 0.0f;
+            if (filtered) {
+                const float one_minus_o = 1.0f - __ldg(p.records + 3 * (size_t)o + 1).z;
+                const float g_alpha = one_minus_o != 0.0f ? a2.x / one_minus_o : 0.0f;
+#pragma unroll
+                for (int j = 0; j < 3; ++j) {
+                    const float e = es[j] * es[j], eh = e + s2;
+                    fr[j] = e / eh;
+                    fcomp[j] = g_alpha * (s2 / eh);
+                    es[j] = sqrtf(eh);
+                }
+            }
+        }
         // dL/dM = (V + V^T) M,  M_ij = R_ij es_j
         float dM[9];
 #pragma unroll
@@ -601,6 +627,10 @@ __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, fl
         float gs[3];
 #pragma unroll
         for (int j = 0; j < 3; ++j) gs[j] = (dM[j] * R[j] + dM[3 + j] * R[3 + j] + dM[6 + j] * R[6 + j]) * es[j];
+        if (FILTER && filtered) {
+#pragma unroll
+            for (int j = 0; j < 3; ++j) gs[j] = gs[j] * fr[j] + fcomp[j];
+        }
         // d/dq = sum_ij dM_ij es_j dR_ij/dq  (table GP3D:316-329)
         const float sx = es[0], sy = es[1], sz = es[2];
         float gq[4];
@@ -920,6 +950,28 @@ backward_points_rs_kernel(const PointsBwdRsParams p) {
     __shared__ float s_mgrad[MGRAD ? (GSB_POINTS_THREADS / 32) * RS_GRAD_VALUES : 1];
     backward_points_body<false, DEPTH, false, false, LENS, false, true, MGRAD>(p, nullptr, nullptr, 0, nullptr, nullptr, p.lens,
                                                                               nullptr, nullptr, p.rs, s_mgrad, p.rs_partials);
+}
+
+// The parameter blocks of the FILTER instantiations (LENS = false ignores `lens`).
+struct PointsBwdFilterParams : PointsBwdLensParams {
+    const float *filter3d;
+};
+struct PointsBwdRsFilterParams : PointsBwdRsParams {
+    const float *filter3d;
+};
+
+template <bool DEPTH, bool LENS>
+__global__ void __launch_bounds__(GSB_POINTS_THREADS, LENS ? 5 : 6)
+backward_points_filter_kernel(const PointsBwdFilterParams p) {
+    backward_points_body<false, DEPTH, false, false, LENS, false, false, false, true>(
+        p, nullptr, nullptr, 0, nullptr, nullptr, p.lens, nullptr, nullptr, RsParams(), nullptr, nullptr, p.filter3d);
+}
+
+template <bool DEPTH, bool LENS>
+__global__ void __launch_bounds__(GSB_POINTS_THREADS, 5)
+backward_points_rs_filter_kernel(const PointsBwdRsFilterParams p) {
+    backward_points_body<false, DEPTH, false, false, LENS, false, true, false, true>(
+        p, nullptr, nullptr, 0, nullptr, nullptr, p.lens, nullptr, nullptr, p.rs, nullptr, nullptr, p.filter3d);
 }
 
 // One CTA: adds the `blocks` partial rows in a fixed order (strided per thread, then a fixed shared-memory tree) and writes
@@ -1280,6 +1332,46 @@ int launch_backward_points_rs(const GsbBackwardArgs &a, const Workspace &ws, cud
                                                                                      rs_grad->grad_motion);
         GSB_CUDA_CHECK(cudaGetLastError());
     }
+    return GSB_OK;
+}
+
+// The FILTER per-point kernels on the grid of launch_backward_points (lens: NULL for a pinhole; rs: NULL for a global
+// shutter); skip_flag as in launch_backward_points.  The caller checked the arguments.
+int launch_backward_points_filter(const GsbBackwardArgs &a, const Workspace &ws, cudaStream_t stream, const long long *skip_flag,
+                                  bool depth_grad, const LensParams *lens, const RsParams *rs, const float *filter3d) {
+    if (a.num_points <= 0) return GSB_OK;
+    long long blocks = (a.num_points + GSB_POINTS_THREADS - 1) / GSB_POINTS_THREADS;
+    const long long cap = 16LL * num_sms();
+    if (blocks > cap) blocks = cap;
+    const int g = (int)blocks;
+    if (rs != nullptr) {
+        PointsBwdRsFilterParams p;
+        static_cast<PointsBwdParams &>(p) = make_points_params(a, ws, skip_flag);
+        p.lens = lens != nullptr ? *lens : LensParams();
+        p.rs = *rs;
+        p.rs_partials = nullptr;
+        p.filter3d = filter3d;
+        if (lens != nullptr) {
+            if (depth_grad) backward_points_rs_filter_kernel<true, true><<<g, GSB_POINTS_THREADS, 0, stream>>>(p);
+            else backward_points_rs_filter_kernel<false, true><<<g, GSB_POINTS_THREADS, 0, stream>>>(p);
+        } else {
+            if (depth_grad) backward_points_rs_filter_kernel<true, false><<<g, GSB_POINTS_THREADS, 0, stream>>>(p);
+            else backward_points_rs_filter_kernel<false, false><<<g, GSB_POINTS_THREADS, 0, stream>>>(p);
+        }
+    } else {
+        PointsBwdFilterParams p;
+        static_cast<PointsBwdParams &>(p) = make_points_params(a, ws, skip_flag);
+        p.lens = lens != nullptr ? *lens : LensParams();
+        p.filter3d = filter3d;
+        if (lens != nullptr) {
+            if (depth_grad) backward_points_filter_kernel<true, true><<<g, GSB_POINTS_THREADS, 0, stream>>>(p);
+            else backward_points_filter_kernel<false, true><<<g, GSB_POINTS_THREADS, 0, stream>>>(p);
+        } else {
+            if (depth_grad) backward_points_filter_kernel<true, false><<<g, GSB_POINTS_THREADS, 0, stream>>>(p);
+            else backward_points_filter_kernel<false, false><<<g, GSB_POINTS_THREADS, 0, stream>>>(p);
+        }
+    }
+    GSB_CUDA_CHECK(cudaGetLastError());
     return GSB_OK;
 }
 

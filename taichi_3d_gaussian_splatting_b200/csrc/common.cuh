@@ -65,9 +65,12 @@ int resolve_workspace(void *base, int64_t bytes, int64_t N, int32_t n_obj, int64
 struct LensParams;
 struct RsParams;
 // lens: the distortion of gsb200_forward_lens (checked there, r2_max set), or NULL for the pinhole kernel; rs: the rolling
-// shutter of gsb200_forward_rolling_shutter (checked there), or NULL
+// shutter of gsb200_forward_rolling_shutter (checked there), or NULL; filter3d: the (N,) 3D smoothing filter of
+// gsb200_forward_filter3d (checked there), or NULL
 int launch_preprocess(const GsbForwardArgs &a, const Workspace &ws, cudaStream_t stream, const LensParams *lens = nullptr,
-                      const RsParams *rs = nullptr);
+                      const RsParams *rs = nullptr, const float *filter3d = nullptr);
+// the pose blocks of n (q, t) pairs (pose_kernel without the per-frame clears)
+int launch_pose_blocks(const float *q_pc, const float *t_pc, int n, PoseBlock *poses, cudaStream_t stream);
 int launch_sort(const Workspace &ws, int64_t key_capacity, cudaStream_t stream);
 int launch_tile_ranges(const Workspace &ws, int64_t key_capacity, int num_tiles, cudaStream_t stream);
 int launch_tile_ranges_raw(const long long *keys_i64, int64_t n, int *tile_start, int *tile_end,
@@ -96,6 +99,12 @@ int launch_backward_points_lens_grad(const GsbBackwardArgs &a, const Workspace &
 // (per-CTA rows in rs_grad->temp) and the finishing kernel; arguments checked by the caller
 int launch_backward_points_rs(const GsbBackwardArgs &a, const Workspace &ws, cudaStream_t stream, bool depth_grad,
                               const LensParams *lens, const RsParams &rs, const GsbRollingShutterGradArgs *rs_grad);
+// gsb200_backward_filter3d: the FILTER per-point kernels (lens: NULL for a pinhole; rs: NULL for a global shutter; dense
+// gradients as launch_backward_points, skip_flag likewise); arguments checked by the caller
+int launch_backward_points_filter(const GsbBackwardArgs &a, const Workspace &ws, cudaStream_t stream, const long long *skip_flag,
+                                  bool depth_grad, const LensParams *lens, const RsParams *rs, const float *filter3d);
+// gsb200_filter3d_from_views (csrc/filter3d.cu; arguments checked by the caller)
+int launch_filter3d_from_views(const GsbFilter3dViewsArgs &a, cudaStream_t stream);
 // gsb200_backward_pose: the POSE per-point kernel (dense gradients as launch_backward_points, plus the per-CTA pose sums
 // in pose.temp) and the per-object finishing kernel; arguments checked by the caller
 int launch_backward_points_pose(const GsbBackwardArgs &a, const Workspace &ws, cudaStream_t stream, bool depth_grad,

@@ -196,8 +196,13 @@ __device__ __forceinline__ bool tile_reachable(const SplatReach &r, float u, flo
 // GSB_RS_ITERATIONS fixed-point steps project pc(tau_k) through the same lens arithmetic as the position below, the point is
 // rendered at pc(tau_3), Sigma' uses W_eff = Rd(tau_3) W, and tau_3 (0 outside the frustum) goes to rs.row_time[i].  The SH
 // view direction keeps the mid-readout camera centre.
-template <typename KeyT, int LENS, bool ROLLING = false>
-__device__ __forceinline__ void preprocess_body(const PreParams p, const LensParams lens, const RsParams rs = RsParams()) {
+// FILTER = true (gsb200_forward_filter3d): the row's 3D smoothing filter sigma = fmaxf(filter3d[i], 0) (definition in
+// include/gsb200.h) widens the scales to s^_j = sqrt(exp(s_j)^2 + sigma^2) before Sigma is formed, and the compensation
+// c = sqrt(prod_j exp(s_j)^2 / s^_j^2) is folded into the record's rescale slot (r1.y = rescale c; r1.z keeps the raw
+// opacity), so the blend kernels read rescale * o * c unchanged.  sigma = 0 leaves the row untouched.
+template <typename KeyT, int LENS, bool ROLLING = false, bool FILTER = false>
+__device__ __forceinline__ void preprocess_body(const PreParams p, const LensParams lens, const RsParams rs = RsParams(),
+                                                const float *filter3d = nullptr) {
     __shared__ unsigned int s_ticket;
     __shared__ unsigned long long s_warp_sums[SCAN_BLOCK_THREADS / 32];
     __shared__ unsigned long long s_block_exclusive;
@@ -230,6 +235,7 @@ __device__ __forceinline__ void preprocess_body(const PreParams p, const LensPar
     int h_ob = 0;
     float h_x = 0.0f, h_y = 0.0f, h_z = 0.0f;
     float4 h_q = make_float4(0, 0, 0, 0), h_sl = h_q;
+    float h_sigma = 0.0f;  // FILTER
     if (i < p.N) {
         h_inv = p.invalid[i];
         h_ob = p.obj_id[i];
@@ -239,6 +245,7 @@ __device__ __forceinline__ void preprocess_body(const PreParams p, const LensPar
         const float4 *hrow = reinterpret_cast<const float4 *>(p.features + (size_t)GSB_FEATURE_DIM * i);
         h_q = hrow[0];           // plain load: this thread rewrites the row's q below
         h_sl = __ldg(hrow + 1);  // s0 s1 s2 logit
+        if (FILTER) h_sigma = __ldg(&filter3d[i]);
     }
     if (i < p.N && h_inv != 1) {
         const PoseBlock *pb = p.poses + h_ob;
@@ -325,6 +332,21 @@ __device__ __forceinline__ void preprocess_body(const PreParams p, const LensPar
             float R[9], S[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0}, RS[9], RSS[9], RT[9], Sigma[9];
             rotation_from_quaternion(qv.x, qv.y, qv.z, qv.w, R);
             S[0] = exp_cr(f[0]); S[4] = exp_cr(f[1]); S[8] = exp_cr(f[2]);
+            float filter_c = 1.0f;  // FILTER: the opacity compensation c
+            if (FILTER) {
+                const float sg = fmaxf(h_sigma, 0.0f);  // NaN -> 0
+                const float s2 = sg * sg;
+                if (s2 > 0.0f) {
+                    float ratio = 1.0f;
+#pragma unroll
+                    for (int j = 0; j < 3; ++j) {
+                        const float e = S[4 * j] * S[4 * j], eh = e + s2;
+                        ratio = ratio * (e / eh);  // a product of ratios in (0, 1]: no overflow
+                        S[4 * j] = sqrtf(eh);
+                    }
+                    filter_c = sqrtf(ratio);
+                }
+            }
             matmul<3, 3, 3>(R, S, RS);
             matmul<3, 3, 3>(RS, S, RSS);  // S^T == S (diagonal)
 #pragma unroll
@@ -373,10 +395,11 @@ __device__ __forceinline__ void preprocess_body(const PreParams p, const LensPar
             ntiles = (max_tu - min_tu) * (max_tv - min_tv);
             // reach-test parameters of this splat; the (tile, splat) tests themselves are done cooperatively by
             // the warp below (one lane per PAIR, not per splat)
-            reach = make_splat_reach(inv_det * c11, inv_det * (-c01), inv_det * c00, rescale * opacity);
+            const float rescale_c = FILTER ? rescale * filter_c : rescale;
+            reach = make_splat_reach(inv_det * c11, inv_det * (-c01), inv_det * c00, rescale_c * opacity);
             if (!p.filter_tiles) reach.mode = 2;
             r0 = make_float4(u, v, inv_det * c11, inv_det * (-c01));
-            r1 = make_float4(inv_det * c00, rescale, opacity, pc[2]);
+            r1 = make_float4(inv_det * c00, rescale_c, opacity, pc[2]);
             r2.w = radius;
         }
     }
@@ -634,9 +657,55 @@ preprocess_rs_kernel(const PreRsParams p) {
     preprocess_body<KeyT, LENS, true>(p, p.lens, p.rs);
 }
 
+// The parameter blocks of the FILTER instantiations (the other kernels keep theirs as they are).  The lens block's
+// LENS = GSB_LENS_PINHOLE instantiation ignores `lens`.
+struct PreFilterParams : PreLensParams {
+    const float *filter3d;
+};
+struct PreRsFilterParams : PreRsParams {
+    const float *filter3d;
+};
+
+template <typename KeyT, int LENS>
+__global__ void __launch_bounds__(SCAN_BLOCK_THREADS, GSB_PRE_MIN_BLOCKS)
+preprocess_filter_kernel(const PreFilterParams p) {
+    preprocess_body<KeyT, LENS, false, true>(p, p.lens, RsParams(), p.filter3d);
+}
+
+template <typename KeyT, int LENS>
+__global__ void __launch_bounds__(SCAN_BLOCK_THREADS, GSB_PRE_MIN_BLOCKS)
+preprocess_rs_filter_kernel(const PreRsFilterParams p) {
+    preprocess_body<KeyT, LENS, true, true>(p, p.lens, p.rs, p.filter3d);
+}
+
 #ifndef GSB_HOST_EMU  // tests/simt compiles the kernels above as host C++ under the SIMT emulator
+// The pose blocks of n (q, t) pairs without clearing anything (gsb200_filter3d_from_views: one per view and object).
+int launch_pose_blocks(const float *q_pc, const float *t_pc, int n, PoseBlock *poses, cudaStream_t stream) {
+    if (n <= 0) return GSB_OK;
+    pose_kernel<<<(n + 63) / 64, 64, 0, stream>>>(q_pc, t_pc, n, poses);
+    GSB_CUDA_CHECK(cudaGetLastError());
+    return GSB_OK;
+}
+
+template <typename KeyT>
+static void launch_filter_kernel(int model, bool rolling, dim3 grid, dim3 block, cudaStream_t stream,
+                                 const PreRsFilterParams &pr) {
+    if (rolling) {
+        if (model == GSB_LENS_FISHEYE) preprocess_rs_filter_kernel<KeyT, GSB_LENS_FISHEYE><<<grid, block, 0, stream>>>(pr);
+        else if (model == GSB_LENS_OPENCV) preprocess_rs_filter_kernel<KeyT, GSB_LENS_OPENCV><<<grid, block, 0, stream>>>(pr);
+        else preprocess_rs_filter_kernel<KeyT, GSB_LENS_PINHOLE><<<grid, block, 0, stream>>>(pr);
+        return;
+    }
+    PreFilterParams pf;
+    static_cast<PreLensParams &>(pf) = static_cast<const PreLensParams &>(pr);
+    pf.filter3d = pr.filter3d;
+    if (model == GSB_LENS_FISHEYE) preprocess_filter_kernel<KeyT, GSB_LENS_FISHEYE><<<grid, block, 0, stream>>>(pf);
+    else if (model == GSB_LENS_OPENCV) preprocess_filter_kernel<KeyT, GSB_LENS_OPENCV><<<grid, block, 0, stream>>>(pf);
+    else preprocess_filter_kernel<KeyT, GSB_LENS_PINHOLE><<<grid, block, 0, stream>>>(pf);
+}
+
 int launch_preprocess(const GsbForwardArgs &a, const Workspace &ws, cudaStream_t stream, const LensParams *lens,
-                      const RsParams *rs) {
+                      const RsParams *rs, const float *filter3d) {
     const GsbWorkspaceLayout &L = ws.layout;
     {
         // per-frame state to zero: [counters, sort_state) and [tile_start, zero_bytes) -- every offset is 256-B aligned
@@ -681,7 +750,17 @@ int launch_preprocess(const GsbForwardArgs &a, const Workspace &ws, cudaStream_t
     p.point_in_camera = ws.point_in_camera;
     p.keys = ws.keys_a;
     p.vals = ws.vals_a;
-    if (rs != nullptr) {
+    if (filter3d != nullptr) {
+        PreRsFilterParams pr;
+        static_cast<PreParams &>(pr) = p;
+        pr.lens = lens != nullptr ? *lens : LensParams();
+        pr.rs = rs != nullptr ? *rs : RsParams();
+        pr.filter3d = filter3d;
+        const int model = lens != nullptr ? lens->model : GSB_LENS_PINHOLE;
+        const dim3 grid(L.scan_blocks), block(SCAN_BLOCK_THREADS);
+        if (L.key_bytes == 4) launch_filter_kernel<unsigned int>(model, rs != nullptr, grid, block, stream, pr);
+        else launch_filter_kernel<unsigned long long>(model, rs != nullptr, grid, block, stream, pr);
+    } else if (rs != nullptr) {
         PreRsParams pr;
         static_cast<PreParams &>(pr) = p;
         pr.lens = lens != nullptr ? *lens : LensParams();

@@ -199,14 +199,17 @@ class FusedTrainStep:
     def run(self, image_gt: torch.Tensor, q_pointcloud_camera: torch.Tensor, t_pointcloud_camera: torch.Tensor, camera_info,
             color_max_sh_band: int, feature_learning_rate: float, position_learning_rate: float,
             targets: Optional[SupervisionTargets] = None, background: Optional[torch.Tensor] = None,
-            appearance_view: Optional[int] = None, mcmc_num_valid: Optional[int] = None) -> None:
+            appearance_view: Optional[int] = None, mcmc_num_valid: Optional[int] = None,
+            filter_3d: Optional[torch.Tensor] = None) -> None:
         """``targets``: the view's depth and / or mask target ((H, W) float32 CUDA tensors) and, with ``extra_features``, its
         ``labels`` ((H, W) int32) or ``features`` ((H, W, C) float32); ``background``: a (3,) float32 CUDA tensor the image is
         composited on (read on the device when the step runs, so it may be refilled per iteration).  Without supervision
         terms or features this is ``gsb200_train_step``; with supervision terms ``gsb200_train_step_aux``; with features
         ``gsb200_train_step_ext``.  ``appearance_view``: with ``appearance_grids``, the index of the view whose grid slices
         the image and takes an Adam step (``gsb200_train_step_appearance``).  ``mcmc_num_valid``: with ``mcmc``, the number
-        of valid rows n_v of the regularisers (``gsb200_train_step_mcmc``); the noise counter is the 0-based iteration."""
+        of valid rows n_v of the regularisers (``gsb200_train_step_mcmc``); the noise counter is the 0-based iteration.
+        ``filter_3d``: the (N,) float32 3D smoothing filter of the rows (``mip_filter.compute_filter_3d``), contiguous, on the
+        scene's device; the forward and the backward render through it (``gsb200_train_step_filter3d``)."""
         sc, cfg = self.scene, self.config
         H, W = int(camera_info.camera_height), int(camera_info.camera_width)
         if image_gt.shape != (3, H, W) or not image_gt.is_contiguous() or image_gt.dtype != torch.float32:
@@ -242,6 +245,9 @@ class FusedTrainStep:
             raise ValueError("appearance_view needs appearance_grids")
         if (self.mcmc is None) != (mcmc_num_valid is None):
             raise ValueError("mcmc and mcmc_num_valid must be given together")
+        if filter_3d is not None and (tuple(filter_3d.shape) != (self.N,) or filter_3d.dtype != torch.float32
+                                      or not filter_3d.is_contiguous() or filter_3d.device != image_gt.device):
+            raise ValueError(f"filter_3d must be a contiguous float32 ({self.N},) tensor on {image_gt.device}")
         self._check_previous()
         q, t = q_pointcloud_camera.contiguous(), t_pointcloud_camera.contiguous()
         K = camera_info.camera_intrinsics.contiguous()
@@ -320,12 +326,20 @@ class FusedTrainStep:
                     exp_avg_sq=_ptr(self.appearance_exp_avg_sq[i]), learning_rate=self.appearance_learning_rate,
                     step=self.appearance_steps[i], image=_ptr(b.sliced_image), temp=_ptr(b.app_temp), temp_bytes=b.app_bytes,
                     loss_out1=_ptr(self.appearance_tv))
+            mcmc_args = None
             if self.mcmc is not None:
                 mc = self.mcmc
                 mcmc_args = _lib.GsbMcmcStepArgs(
                     num_valid=int(mcmc_num_valid), lambda_opacity=mc.opacity_reg, lambda_scale=mc.scale_reg,
                     noise_scale=mc.noise_lr * float(position_learning_rate), gate_k=GATE_K, min_opacity=mc.min_opacity,
                     seed=int(mc.seed), step=self.step_count - 1, terms_out2=_ptr(self.mcmc_terms), temp=_ptr(self._mcmc_temp))
+            if filter_3d is not None:
+                _lib.check(self._lib.gsb200_train_step_filter3d(
+                    ctypes.byref(args), ctypes.byref(sup) if supervised else None, ctypes.byref(fx) if fx is not None else None,
+                    ctypes.byref(app) if app is not None else None,
+                    ctypes.byref(mcmc_args) if mcmc_args is not None else None,
+                    ctypes.byref(_lib.GsbFilter3dArgs(filter3d=_ptr(filter_3d)))), "gsb200_train_step_filter3d")
+            elif mcmc_args is not None:
                 _lib.check(self._lib.gsb200_train_step_mcmc(
                     ctypes.byref(args), ctypes.byref(sup) if supervised else None, ctypes.byref(fx) if fx is not None else None,
                     ctypes.byref(app) if app is not None else None, ctypes.byref(mcmc_args)), "gsb200_train_step_mcmc")
@@ -342,7 +356,7 @@ class FusedTrainStep:
                 _lib.check(self._lib.gsb200_train_step(ctypes.byref(args)), "gsb200_train_step")
         self._pending[slot] = True
         self._last = SimpleNamespace(buffers=b, H=H, W=W, slot=slot, supervised=supervised,
-                                     keep=(q, t, K, image_gt, depth_t, mask_t, background, feat_t))
+                                     keep=(q, t, K, image_gt, depth_t, mask_t, background, feat_t, filter_3d))
 
     @property
     def moments(self) -> MCMCMoments:

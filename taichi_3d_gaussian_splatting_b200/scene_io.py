@@ -185,8 +185,14 @@ class GaussianPointCloudScene(nn.Module):
         return scene
 
     # GaussianPointCloudScene.py:148-181 (official 3DGS layout)
-    def to_ply(self, path: str):
+    def to_ply(self, path: str, filter_3d: Optional[torch.Tensor] = None):
+        """``filter_3d``: the (N,) 3D smoothing filter of the rows (``mip_filter``; e.g. ``trainer.filter_3d()``), baked into
+        ``scale_*`` and ``opacity`` so that any 3DGS viewer shows the filtered scene.  None: the rows as they are."""
         xyz, feat = self._valid()
+        if filter_3d is not None:
+            from .mip_filter import bake_filter_3d
+            keep = (self.point_invalid_mask == 0).cpu()
+            feat = bake_filter_3d(feat, filter_3d.detach().cpu()[keep])
         sh = feat[:, 8:].reshape(-1, 3, 16).numpy()
         cols = {"x": xyz[:, 0], "y": xyz[:, 1], "z": xyz[:, 2]}
         for k in ("nx", "ny", "nz"):

@@ -53,6 +53,7 @@ from .densification import GaussianPointAdaptiveController
 from .GaussianPointCloudRasterisation import GaussianPointCloudRasterisation
 from .loss import FEATURE_LOSSES, LossFunction, SupervisionTargets, feature_loss, mcmc_regulariser, supervision_loss
 from .mcmc import GATE_K, GaussianPointMCMCController, MCMCConfig, MCMCMoments, add_position_noise
+from .mip_filter import compute_filter_3d
 
 View = Tuple[torch.Tensor, torch.Tensor, torch.Tensor, CameraInfo]  # image (3,H,W) in [0,1], q (1,4), t (1,3), camera
 # ... optionally followed by a SupervisionTargets (depth and / or mask at the image's resolution)
@@ -181,6 +182,15 @@ class GaussianPointCloudTrainer:
         # "mcmc" (relocation, growth to mcmc_config.cap_max, regularisers and position noise; needs mcmc_config)
         densification: str = "adaptive"
         mcmc_config: Optional[MCMCConfig] = None
+        # optional 3D smoothing filter (Mip-Splatting, mip_filter.py): every Gaussian is rendered convolved with an isotropic
+        # Gaussian sized by the finest sampling interval of the full-resolution training views that see it (variance in
+        # pixels^2, the paper's 0.2), recomputed before the first iteration, after every refinement and every
+        # mip_filter_interval iterations.  Not with pose, intrinsics, lens or motion refinement, fisheye training views or
+        # the view-parallel exchange.  OpenCV-lens and rolling-shutter views use the pinhole test at the mid-readout pose
+        # (an approximation).
+        mip_filter_3d: bool = False
+        mip_filter_variance: float = 0.2
+        mip_filter_interval: int = 100
 
     def __init__(self, config: "GaussianPointCloudTrainer.TrainConfig", scene: Scene, train_views: List[View],
                  rasterisation_factory: Optional[Callable] = None, generator: Optional[torch.Generator] = None,
@@ -260,6 +270,24 @@ class GaussianPointCloudTrainer:
                     raise ValueError(f"{name} is not supported with a rolling-shutter view (CameraInfo.rolling_shutter)")
         self._rolling_shutter = self._rolling_shutter_leaves(config, train_views)
         self._rs = config.rolling_shutter_learning_rate > 0
+        self._mip = bool(config.mip_filter_3d)
+        self._filter_3d = None
+        if self._mip:
+            v = config.mip_filter_variance
+            if not (isinstance(v, (int, float)) and math.isfinite(v) and v >= 0):
+                raise ValueError(f"mip_filter_variance must be finite and >= 0, got {v}")
+            if not (isinstance(config.mip_filter_interval, int) and config.mip_filter_interval >= 1):
+                raise ValueError(f"mip_filter_interval must be an int >= 1, got {config.mip_filter_interval!r}")
+            for name, on in (("pose refinement (pose_learning_rate > 0)", self._pose),
+                             ("intrinsics refinement (intrinsics_learning_rate > 0)", self._intr),
+                             ("distortion refinement (distortion_learning_rate > 0)", config.distortion_learning_rate > 0),
+                             ("motion refinement (rolling_shutter_learning_rate > 0)", self._rs)):
+                if on:
+                    raise ValueError(f"mip_filter_3d is not supported with {name}: the filter is computed from fixed "
+                                     "training cameras")
+            if any(getattr(getattr(v[3], "distortion", None), "model", None) == "fisheye" for v in train_views):
+                raise ValueError("mip_filter_3d does not support fisheye training views: the filter's pinhole frustum test "
+                                 "is wrong for them")
         self._appearance = config.appearance_grid is not None
         self._appearance_leaves = []
         self._appearance_tensor = None
@@ -319,6 +347,8 @@ class GaussianPointCloudTrainer:
                                      **extra)
         if self._mcmc and getattr(self.rasterisation, "gradient_exchange", None) is not None:
             raise ValueError('densification="mcmc" is not implemented for the view-parallel gradient exchange')
+        if self._mip and getattr(self.rasterisation, "gradient_exchange", None) is not None:
+            raise ValueError("mip_filter_3d is not implemented for the view-parallel gradient exchange")
         self.loss_function = LossFunction(config=config.loss_function_config)
         self.history: List[dict] = []
         self._downsampled = {}
@@ -433,6 +463,36 @@ class GaussianPointCloudTrainer:
             K = K / div
         return K
 
+    def _update_filter_3d(self) -> None:
+        """The 3D filter of the current rows from the full-resolution training views (``mip_filter.compute_filter_3d``)."""
+        views = [(q, t, v[3]) for (q, t), v in zip(self._poses, self.train_views)]
+        self._filter_3d = compute_filter_3d(self.scene.point_cloud, self.scene.point_invalid_mask, self.scene.point_object_id,
+                                            views, self.config.rasterisation_config.near_plane, self.config.mip_filter_variance)
+
+    def _after_refinement(self, iteration: int) -> None:
+        """Recomputes the 3D filter after a refinement that may have moved rows (densification, MCMC relocation and growth)
+        and every ``mip_filter_interval`` iterations."""
+        if not self._mip:
+            return
+        if self._mcmc:
+            c = self.mcmc_controller
+            refined = c.config.refine_start <= c.iteration_counter < c.config.refine_stop and \
+                c.iteration_counter % c.config.refine_every == 0
+        else:
+            c = self.adaptive_controller
+            refined = c.iteration_counter >= c.config.num_iterations_warm_up and \
+                c.iteration_counter % c.config.num_iterations_densify == 0
+        if refined or (iteration + 1) % self.config.mip_filter_interval == 0:
+            self._update_filter_3d()
+
+    def _filter_kw(self) -> dict:
+        return {"point_filter_3d": self._filter_3d} if self._mip else {}
+
+    def filter_3d(self) -> Optional[torch.Tensor]:
+        """The (N,) 3D filter the latest iteration rendered with (a detached copy; None without ``mip_filter_3d``).
+        ``GaussianPointCloudScene.to_ply(path, filter_3d=...)`` bakes it into an export."""
+        return None if self._filter_3d is None else self._filter_3d.detach().clone()
+
     def _next_background(self) -> Optional[torch.Tensor]:
         """The background of this iteration: None (black), white, or a fresh colour drawn on the device."""
         if self.config.background == "random":
@@ -463,6 +523,8 @@ class GaussianPointCloudTrainer:
         self.fused_train_step = step
         position_lr = cfg.position_learning_rate
         downsample_factor = cfg.initial_downsample_factor
+        if self._mip:
+            self._update_filter_3d()
         for iteration in range(cfg.num_iterations):
             if iteration % cfg.half_downsample_factor_interval == 0 and iteration > 0 and downsample_factor > 1:
                 downsample_factor //= 2
@@ -472,6 +534,8 @@ class GaussianPointCloudTrainer:
             app_kw = {"appearance_view": view_index} if self._appearance else {}
             if self._mcmc:
                 app_kw["mcmc_num_valid"] = self.mcmc_controller.num_valid
+            if self._mip:
+                app_kw["filter_3d"] = self._filter_3d
             if self.supervised or self._features:
                 step.run(image_gt, q, t, camera_info, band, cfg.feature_learning_rate, position_lr, targets=targets,
                          background=self._next_background(), **app_kw)
@@ -484,6 +548,7 @@ class GaussianPointCloudTrainer:
             else:
                 self.adaptive_controller.after_fused_update(step.hook_input)
                 self.adaptive_controller.refinement()
+            self._after_refinement(iteration)
             if log_interval and iteration % log_interval == 0:
                 losses = step.loss.tolist()
                 entry = dict(iteration=iteration, loss=losses[0], l1=losses[1],
@@ -543,6 +608,8 @@ class GaussianPointCloudTrainer:
             if self._appearance else None
         scheduler = torch.optim.lr_scheduler.ExponentialLR(position_optimizer, gamma=cfg.position_learning_rate_decay_rate)
         downsample_factor = cfg.initial_downsample_factor
+        if self._mip:
+            self._update_filter_3d()
         for iteration in range(cfg.num_iterations):
             if iteration % cfg.half_downsample_factor_interval == 0 and iteration > 0 and downsample_factor > 1:
                 downsample_factor //= 2
@@ -566,7 +633,7 @@ class GaussianPointCloudTrainer:
                 camera_info = CameraInfo(camera_intrinsics=self._intrinsics_of(view_index, downsample_factor),
                                          camera_height=camera_info.camera_height, camera_width=camera_info.camera_width,
                                          camera_id=camera_info.camera_id)
-            lens_kw = {}
+            lens_kw = self._filter_kw()
             if self._dist and camera_info.distortion is not None:  # the lens as trained, the leaf as the autograd input
                 leaf = self._distortion[camera_info.camera_id]
                 camera_info = CameraInfo(camera_intrinsics=camera_info.camera_intrinsics,
@@ -631,6 +698,7 @@ class GaussianPointCloudTrainer:
                 self.mcmc_controller.refinement(MCMCMoments.of_optimizers(optimizer, position_optimizer, extra_optimizer))
             else:
                 self.adaptive_controller.refinement()
+            self._after_refinement(iteration)
             if log_interval and iteration % log_interval == 0:
                 entry = dict(iteration=iteration, loss=float(loss.detach()), l1=float(l1_loss.detach()),
                              psnr=psnr(image_pred.detach(), image_gt),
@@ -735,10 +803,12 @@ class GaussianPointCloudTrainer:
     def validation(self, views: Optional[List[View]] = None) -> float:
         """Mean PSNR over the views at full resolution (GaussianPointTrainer.py:334-415 without the logging)."""
         views = views if views is not None else self.train_views
+        if self._mip and self._filter_3d is None:
+            self._update_filter_3d()
         total = 0.0
         for view in views:
             image_gt, q, t, camera_info = view[:4]
-            outs = self.rasterisation(self._input(q, t, camera_info, 3))
+            outs = self.rasterisation(self._input(q, t, camera_info, 3), **self._filter_kw())
             image_pred = outs[0]
             if self.config.background != "black":
                 # white: the prediction on white and the ground truth composited by its mask; random: both on black
