@@ -800,6 +800,55 @@ int gsb200_filter3d_from_views(const GsbFilter3dViewsArgs *args);
 /* sizeof(GsbFilter3dArgs), sizeof(GsbFilter3dViewsArgs) */
 void gsb200_abi_sizes_filter3d(int64_t *out2);
 
+/* Per-pixel weights of the image loss (an extension), for images whose views hold transient distractors (people, cars,
+ * shadows that are in one photo and not the next).  For the image x (H,W,3) the image loss reads (the sliced image with an
+ * appearance grid, the composited one with a background) and its ground truth g (3,H,W), with s (H,W) the static weight
+ * (1 everywhere when NULL):
+ *   r = (|c0 - g0| + |c1 - g1| + |c2 - g2|) / 3 in float32 in this order, c = clamp(x, 0, 1);  bin = min(floor(4096 r), 4095)
+ *   b = the smallest bin with (float)cum(b) >= q (float)n, cum the histogram of the bins of the n pixels with s > 0
+ *   raw inlier: bin <= b
+ *   3x3 inlier: (float)(raw inliers) >= box_threshold (float)(neighbours), over the in-image 3x3 neighbours with s > 0
+ *   patch inlier: every pixel of a 16x16 tile, when (float)(3x3 inliers) >= patch_threshold (float)(pixels) over the
+ *                 tile's pixels with s > 0
+ *   w = s [3x3 inlier or patch inlier] with the robust mask (RobustNeRF, Sabour et al., CVPR 2023, section 4), else w = s.
+ * The image loss runs unchanged on x' = w c + (1 - w) g (no FMA contraction: it rounds like torch), so a pixel of weight 0
+ * is its ground truth and adds nothing to either term, and dL/dx = w 1[0 <= x <= 1] dL/dx'.  The normalisation stays over
+ * all pixels.  stats_out2 = {inlier fraction sum[w > 0 among s > 0] / n (0 when n = 0), threshold (b + 1) / 4096 (1 without
+ * the robust mask)}.  Integer counts only: two calls are bit-identical.  H and W must be multiples of 16. */
+typedef struct GsbRobustLossArgs {
+    const float *static_weight;   /* (H,W) in [0,1], or NULL: 1 everywhere */
+    int32_t robust;               /* 1: the inlier mask of this iteration's residual; 0: w = s */
+    float inlier_quantile;        /* q in (0, 1] (robust only) */
+    float box_threshold;          /* in [0, 1] (robust only) */
+    float patch_threshold;        /* in [0, 1] (robust only) */
+    float *weight_out;            /* (H,W) out: w */
+    float *composite;             /* (H,W,3) scratch out: x' */
+    void *temp;                   /* gsb200_robust_temp_bytes(H, W), 16-byte aligned, zero before the first use */
+    int64_t temp_bytes;
+    float *stats_out2;            /* device: {inlier fraction, threshold} */
+} GsbRobustLossArgs;
+/* bytes of the temp; 0 unless H and W are positive multiples of 16 */
+int64_t gsb200_robust_temp_bytes(int32_t camera_height, int32_t camera_width);
+/* gsb200_image_loss with the weights: robust pre-passes -> image loss on (x', gt) -> dL/dx into grad_rasterized_image.
+ * The rules of gsb200_train_step_robust on `robust`, and those of gsb200_image_loss; grad_rasterized_image must not be NULL. */
+int gsb200_robust_image_loss(const float *rasterized_image, const float *ground_truth_image, int32_t camera_height,
+                             int32_t camera_width, float lambda_value, const GsbRobustLossArgs *robust, float *loss_out3,
+                             float *grad_rasterized_image, void *temp, int64_t temp_bytes, void *stream);
+/* gsb200_train_step_filter3d with the weights: ... -> supervision pre-pass -> slice -> robust pre-passes on the image the
+ * loss reads -> image loss on x' -> robust post-pass (dL/dx' -> dL/dx in place) -> slice backward -> supervision post-pass
+ * -> ...  The depth, mask and feature terms are not weighted.  The pre- and post-passes run on a key-capacity overflow too;
+ * they write only the weight, the composite and the stats, so the iteration stays a no-op.  NULL robust: exactly
+ * gsb200_train_step_filter3d.  GSB_EINVAL, before any CUDA call, for robust not 0 or 1, a quantile outside (0, 1] or a
+ * threshold outside [0, 1] with the robust mask, H or W not a multiple of 16, a NULL weight_out, composite or stats_out2,
+ * a static weight, weight_out or composite not 4-byte aligned, a temp that is NULL, not 16-byte aligned or smaller
+ * than gsb200_robust_temp_bytes, or a loss_temp of the train step that is not 16-byte aligned or smaller than
+ * gsb200_image_loss_temp_bytes. */
+int gsb200_train_step_robust(const GsbTrainStepArgs *args, const GsbSupervisionArgs *supervision,
+                             const GsbFeatureTrainArgs *features, const GsbAppearanceArgs *appearance,
+                             const GsbMcmcStepArgs *mcmc, const GsbFilter3dArgs *filter, const GsbRobustLossArgs *robust);
+/* sizeof(GsbRobustLossArgs) */
+void gsb200_abi_sizes_robust(int64_t *out1);
+
 /* Individual stages (same workspace), for tests and profiling. */
 int gsb200_stage_preprocess(const GsbForwardArgs *args);   /* K1+P1+K2+K3+P2+K4 fused */
 int gsb200_stage_sort(const GsbForwardArgs *args);         /* P3 */

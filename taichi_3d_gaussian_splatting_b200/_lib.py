@@ -169,6 +169,14 @@ class GsbFilter3dArgs(ctypes.Structure):
     _fields_ = [("filter3d", c_vp)]
 
 
+class GsbRobustLossArgs(ctypes.Structure):
+    _fields_ = [
+        ("static_weight", c_vp), ("robust", c_i32), ("inlier_quantile", c_f32), ("box_threshold", c_f32),
+        ("patch_threshold", c_f32), ("weight_out", c_vp), ("composite", c_vp), ("temp", c_vp), ("temp_bytes", c_i64),
+        ("stats_out2", c_vp),
+    ]
+
+
 class GsbFilter3dViewsArgs(ctypes.Structure):
     _fields_ = [
         ("num_points", c_i64), ("pointcloud", c_vp), ("point_invalid_mask", c_vp), ("point_object_id", c_vp),
@@ -214,7 +222,8 @@ EXPORTS = (
     "gsb200_bilateral_grid_forward", "gsb200_bilateral_grid_backward", "gsb200_train_step_appearance",
     "gsb200_mcmc_temp_bytes", "gsb200_mcmc_regulariser", "gsb200_mcmc_noise", "gsb200_mcmc_relocate", "gsb200_train_step_mcmc",
     "gsb200_abi_sizes_mcmc", "gsb200_forward_filter3d", "gsb200_backward_filter3d", "gsb200_train_step_filter3d",
-    "gsb200_filter3d_temp_bytes", "gsb200_filter3d_from_views", "gsb200_abi_sizes_filter3d",
+    "gsb200_filter3d_temp_bytes", "gsb200_filter3d_from_views", "gsb200_abi_sizes_filter3d", "gsb200_robust_temp_bytes",
+    "gsb200_robust_image_loss", "gsb200_train_step_robust", "gsb200_abi_sizes_robust",
 )
 
 _lib = None
@@ -333,6 +342,16 @@ def load() -> ctypes.CDLL:
                                                ctypes.POINTER(GsbFeatureTrainArgs), ctypes.POINTER(GsbAppearanceArgs),
                                                ctypes.POINTER(GsbMcmcStepArgs), ctypes.POINTER(GsbFilter3dArgs)]
     lib.gsb200_train_step_filter3d.restype = ctypes.c_int
+    lib.gsb200_train_step_robust.argtypes = [ctypes.POINTER(GsbTrainStepArgs), ctypes.POINTER(GsbSupervisionArgs),
+                                             ctypes.POINTER(GsbFeatureTrainArgs), ctypes.POINTER(GsbAppearanceArgs),
+                                             ctypes.POINTER(GsbMcmcStepArgs), ctypes.POINTER(GsbFilter3dArgs),
+                                             ctypes.POINTER(GsbRobustLossArgs)]
+    lib.gsb200_train_step_robust.restype = ctypes.c_int
+    lib.gsb200_robust_temp_bytes.argtypes = [c_i32, c_i32]
+    lib.gsb200_robust_temp_bytes.restype = c_i64
+    lib.gsb200_robust_image_loss.argtypes = [c_vp, c_vp, c_i32, c_i32, c_f32, ctypes.POINTER(GsbRobustLossArgs), c_vp, c_vp,
+                                             c_vp, c_i64, c_vp]
+    lib.gsb200_robust_image_loss.restype = ctypes.c_int
     lib.gsb200_filter3d_temp_bytes.argtypes = [c_i32, c_i32]
     lib.gsb200_filter3d_temp_bytes.restype = c_i64
     lib.gsb200_filter3d_from_views.argtypes = [ctypes.POINTER(GsbFilter3dViewsArgs)]
@@ -444,6 +463,13 @@ def load() -> ctypes.CDLL:
         if sizes_filter[i] != ctypes.sizeof(mirror):
             raise RuntimeError(f"libgsb200.so ABI mismatch: sizeof({mirror.__name__}) {sizes_filter[i]} != ctypes mirror "
                                f"{ctypes.sizeof(mirror)}")
+    lib.gsb200_abi_sizes_robust.argtypes = [ctypes.POINTER(c_i64)]
+    lib.gsb200_abi_sizes_robust.restype = None
+    sizes_robust = (c_i64 * 1)()
+    lib.gsb200_abi_sizes_robust(sizes_robust)
+    if sizes_robust[0] != ctypes.sizeof(GsbRobustLossArgs):
+        raise RuntimeError(f"libgsb200.so ABI mismatch: sizeof(GsbRobustLossArgs) {sizes_robust[0]} != ctypes mirror "
+                           f"{ctypes.sizeof(GsbRobustLossArgs)}")
     _lib = lib
     return lib
 

@@ -2,8 +2,8 @@
 
     python -m taichi_3d_gaussian_splatting_b200.build [--force] [--verbose]
 
-``preprocess.cu`` and ``filter3d.cu`` are compiled with ``-fmad=false`` so that every per-point discrete decision is
-bit-reproducible against the CPU oracle; the blend kernels use default FMA contraction.
+``preprocess.cu``, ``filter3d.cu`` and ``robust_loss.cu`` are compiled with ``-fmad=false`` so that every per-point discrete decision is
+bit-reproducible against the CPU oracle (and the loss weights' composite against torch); the blend kernels use default FMA contraction.
 """
 import hashlib
 import os
@@ -36,6 +36,7 @@ SOURCES = {
     "adam.cu": [],
     "mcmc.cu": [],
     "filter3d.cu": ["-fmad=false"],
+    "robust_loss.cu": ["-fmad=false"],
     "controller.cu": [],
     "exchange.cu": [],
 }

@@ -841,6 +841,69 @@ int gsb200_train_step_mcmc(const GsbTrainStepArgs *t, const GsbSupervisionArgs *
 
 int gsb200_train_step_filter3d(const GsbTrainStepArgs *t, const GsbSupervisionArgs *s, const GsbFeatureTrainArgs *x,
                                const GsbAppearanceArgs *app, const GsbMcmcStepArgs *mc, const GsbFilter3dArgs *filter) {
+    return gsb200_train_step_robust(t, s, x, app, mc, filter, nullptr);
+}
+
+// The loss weights' own rules (gsb200_train_step_robust, gsb200_robust_image_loss).
+static int check_robust_args(const char *what, const GsbRobustLossArgs &r, int H, int W) {
+    if (r.robust != 0 && r.robust != 1) {
+        set_error("%s: robust must be 0 or 1 (got %d)", what, r.robust);
+        return GSB_EINVAL;
+    }
+    if (r.robust && (!(r.inlier_quantile > 0.0f && r.inlier_quantile <= 1.0f) ||
+                     !(r.box_threshold >= 0.0f && r.box_threshold <= 1.0f) ||
+                     !(r.patch_threshold >= 0.0f && r.patch_threshold <= 1.0f))) {
+        set_error("%s: the inlier quantile must be in (0, 1] and the thresholds in [0, 1] (got %g, %g, %g)", what,
+                  (double)r.inlier_quantile, (double)r.box_threshold, (double)r.patch_threshold);
+        return GSB_EINVAL;
+    }
+    if (H < 16 || W < 16 || H % 16 || W % 16) {
+        set_error("%s: the loss weights need H and W to be multiples of 16 (got %dx%d)", what, H, W);
+        return GSB_EINVAL;
+    }
+    const auto aligned4 = [](const void *p) { return reinterpret_cast<uintptr_t>(p) % 4 == 0; };
+    if (!r.weight_out || !r.composite || !r.stats_out2 || !aligned4(r.static_weight) || !aligned4(r.weight_out) ||
+        !aligned4(r.composite)) {
+        set_error("%s: NULL weight_out, composite or stats_out2, or a static weight, weight_out or composite that is not "
+                  "4-byte aligned", what);
+        return GSB_EINVAL;
+    }
+    if (!r.temp || !aligned16(r.temp) || r.temp_bytes < gsb200_robust_temp_bytes(H, W)) {
+        set_error("%s: temp null, not 16-byte aligned or smaller than gsb200_robust_temp_bytes(H, W) (temp_bytes=%lld)", what,
+                  (long long)r.temp_bytes);
+        return GSB_EINVAL;
+    }
+    return GSB_OK;
+}
+
+int gsb200_robust_image_loss(const float *rasterized_image, const float *ground_truth_image, int32_t camera_height,
+                             int32_t camera_width, float lambda_value, const GsbRobustLossArgs *robust, float *loss_out3,
+                             float *grad_rasterized_image, void *temp, int64_t temp_bytes, void *stream) {
+    if (!robust || !rasterized_image || !ground_truth_image || !grad_rasterized_image) {
+        set_error("robust_image_loss: NULL robust, image, ground truth or gradient");
+        return GSB_EINVAL;
+    }
+    int rc = check_robust_args("robust_image_loss", *robust, camera_height, camera_width);
+    if (rc != GSB_OK) return rc;
+    if (!loss_out3 || !temp || temp_bytes < gsb200_image_loss_temp_bytes(camera_height, camera_width) || !aligned16(temp)) {
+        set_error("robust_image_loss: loss_out3 NULL, or the image loss's temp null, not 16-byte aligned or too small "
+                  "(temp_bytes=%lld)", (long long)temp_bytes);
+        return GSB_EINVAL;
+    }
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if ((rc = launch_robust_pre(*robust, rasterized_image, ground_truth_image, camera_height, camera_width, st)) != GSB_OK)
+        return rc;
+    if ((rc = gsb200_image_loss(robust->composite, ground_truth_image, camera_height, camera_width, lambda_value, 1.0f,
+                                loss_out3, grad_rasterized_image, temp, temp_bytes, stream)) != GSB_OK)
+        return rc;
+    return launch_robust_post(*robust, rasterized_image, camera_height, camera_width, grad_rasterized_image, st);
+}
+
+void gsb200_abi_sizes_robust(int64_t *out1) { out1[0] = (int64_t)sizeof(GsbRobustLossArgs); }
+
+int gsb200_train_step_robust(const GsbTrainStepArgs *t, const GsbSupervisionArgs *s, const GsbFeatureTrainArgs *x,
+                             const GsbAppearanceArgs *app, const GsbMcmcStepArgs *mc, const GsbFilter3dArgs *filter,
+                             const GsbRobustLossArgs *robust) {
     const float *filter3d;
     int frc = check_filter3d("train_step_filter3d", filter, &filter3d);
     if (frc != GSB_OK) return frc;
@@ -920,6 +983,15 @@ int gsb200_train_step_filter3d(const GsbTrainStepArgs *t, const GsbSupervisionAr
             return GSB_EINVAL;
         }
     }
+    if (robust) {
+        if ((rc = check_robust_args("train_step_robust", *robust, H, W)) != GSB_OK) return rc;
+        // the image loss runs between the robust pre- and post-passes: its rules are checked before either is launched
+        if (t->loss_temp_bytes < gsb200_image_loss_temp_bytes(H, W) || !aligned16(t->loss_temp)) {
+            set_error("train_step_robust: the image loss's temp is not 16-byte aligned or smaller than "
+                      "gsb200_image_loss_temp_bytes(H, W) (loss_temp_bytes=%lld)", (long long)t->loss_temp_bytes);
+            return GSB_EINVAL;
+        }
+    }
     const GsbExtraFeatureArgs *ext = x ? &x->features : nullptr;
     cudaStream_t st = static_cast<cudaStream_t>(f.stream);
     if ((rc = gsb200_forward_filter3d(&f, ext, nullptr, nullptr, filter)) != GSB_OK) return rc;
@@ -934,9 +1006,14 @@ int gsb200_train_step_filter3d(const GsbTrainStepArgs *t, const GsbSupervisionAr
             return rc;
         sliced_image = app->image;
     }
-    rc = gsb200_image_loss(sliced_image, loss_gt, H, W, t->lambda_value, 1.0f, t->loss_out3,
+    if (robust && (rc = launch_robust_pre(*robust, sliced_image, loss_gt, H, W, st)) != GSB_OK) return rc;
+    rc = gsb200_image_loss(robust ? robust->composite : sliced_image, loss_gt, H, W, t->lambda_value, 1.0f, t->loss_out3,
                            const_cast<float *>(b.grad_rasterized_image), t->loss_temp, t->loss_temp_bytes, f.stream);
     if (rc != GSB_OK) return rc;
+    // dL/dx' -> dL/dx of the image the loss read, before the slice backward and the supervision post-pass read it
+    if (robust && (rc = launch_robust_post(*robust, sliced_image, H, W, const_cast<float *>(b.grad_rasterized_image), st)) !=
+                      GSB_OK)
+        return rc;
     // dL/dG from dL/dI'' before dL/dI' replaces it in the same buffer; then the TV term into dL/dG
     if (app && (rc = launch_bilateral_grid_backward(loss_image, app->grid, H, W, app->grid_x, app->grid_y, app->grid_z,
                                                     b.grad_rasterized_image, const_cast<float *>(b.grad_rasterized_image),

@@ -132,6 +132,10 @@ int launch_supervision_post(const GsbSupervisionArgs &s, const float *image, con
                             cudaStream_t stream);
 // feature_loss.cu: both passes of the feature term (arguments checked by gsb200_train_step_ext)
 int launch_feature_loss(const GsbFeatureTrainArgs &x, int H, int W, cudaStream_t stream);
+// Per-pixel loss weights (csrc/robust_loss.cu); arguments checked by the caller.  pre: w and x' from the image the loss
+// reads; post: dL/dx' -> dL/dx in place, and the stats
+int launch_robust_pre(const GsbRobustLossArgs &r, const float *image, const float *gt, int H, int W, cudaStream_t stream);
+int launch_robust_post(const GsbRobustLossArgs &r, const float *image, int H, int W, float *grad, cudaStream_t stream);
 // appearance.cu: the bilateral-grid slice, its backward (+ the TV term when tv_out is set; arguments checked by the caller)
 int launch_bilateral_grid_forward(const float *image, const float *grid, int H, int W, int gx, int gy, int gz, float *out,
                                   cudaStream_t stream);

@@ -28,6 +28,11 @@ Optional MCMC densification (``mcmc=MCMCConfig``, ``run(..., mcmc_num_valid=n_v)
 added to the feature gradient between the backward and the Adam steps and the covariance-shaped position noise after them, in
 the same one call (``gsb200_train_step_mcmc``; ``loss.mcmc_regulariser`` and ``mcmc.add_position_noise`` state them in torch).
 The refinements stay on the host (``mcmc.GaussianPointMCMCController.refinement(step.moments)``).
+
+Optional per-pixel weights of the image loss (``robust=RobustLossConfig``, ``run(..., targets=SupervisionTargets(loss_weight=
+...), robust_active=)``): a static weight per view and / or RobustNeRF's trimmed inlier mask of this iteration's residual, both
+computed on the device in the same one call (``gsb200_train_step_robust``; ``loss.robust_weight`` states them in torch).
+``step.loss_weight`` holds the latest weight map and ``step.robust_stats`` {inlier fraction, threshold}.
 """
 import ctypes
 import warnings
@@ -38,7 +43,7 @@ import torch
 
 from . import _lib
 from .GaussianPointCloudRasterisation import Frame, GaussianPointCloudRasterisation, _ptr
-from .loss import FEATURE_LOSSES, SupervisionTargets
+from .loss import FEATURE_LOSSES, RobustLossConfig, SupervisionTargets
 from .mcmc import GATE_K, MCMCMoments
 
 __all__ = ["FusedTrainStep", "SupervisionTargets"]
@@ -50,7 +55,7 @@ class FusedTrainStep:
                  mask_weight: float = 0.0, extra_features: Optional[torch.Tensor] = None, feature_loss: Optional[str] = None,
                  feature_weight: float = 1.0, extra_feature_learning_rate: float = 1e-2,
                  appearance_grids: Optional[torch.Tensor] = None, appearance_learning_rate: float = 2e-3,
-                 appearance_tv_weight: float = 10.0, mcmc=None):
+                 appearance_tv_weight: float = 10.0, mcmc=None, robust: Optional[RobustLossConfig] = None):
         """``scene``: object with ``point_cloud`` (N,3), ``point_cloud_features`` (N,56), ``point_invalid_mask``,
         ``point_object_id`` (CUDA, contiguous; updated in place).  ``controller``: a ``GaussianPointAdaptiveController`` whose
         six accumulators are updated by the backward epilogue (or ``None``).  ``depth_weight`` / ``mask_weight``: weights of
@@ -60,7 +65,9 @@ class FusedTrainStep:
         ``targets.labels`` and C >= 2; "l2": needs ``targets.features``) weighted by ``feature_weight``
         (``loss.feature_loss``).  ``appearance_grids``: (V, 12, Gz, Gy, Gx) float32 per-view bilateral grids (CUDA,
         contiguous; updated in place), trained at ``appearance_learning_rate`` with the TV weight ``appearance_tv_weight``;
-        ``run`` then needs ``appearance_view``.  ``mcmc``: an ``mcmc.MCMCConfig``; ``run`` then needs ``mcmc_num_valid``."""
+        ``run`` then needs ``appearance_view``.  ``mcmc``: an ``mcmc.MCMCConfig``; ``run`` then needs ``mcmc_num_valid``.
+        ``robust``: a ``loss.RobustLossConfig``; the image loss then drops the outliers of RobustNeRF's inlier mask in the
+        iterations ``run(robust_active=...)`` selects (``start_iteration`` is the caller's to honour)."""
         for name, w in (("depth_weight", depth_weight), ("mask_weight", mask_weight)):
             if not (w >= 0.0 and w < float("inf")):
                 raise ValueError(f"{name} must be finite and >= 0, got {w}")
@@ -118,6 +125,10 @@ class FusedTrainStep:
             self.appearance_steps = [0] * V  # each view's own Adam step count
             self.grad_appearance_grid = torch.zeros_like(appearance_grids[0])
         self.appearance_tv = z(1)  # {tv_weight * tv(G)} of the latest iteration with appearance (device)
+        if robust is not None and not isinstance(robust, RobustLossConfig):
+            raise ValueError(f"robust must be a RobustLossConfig, got {type(robust).__name__}")
+        self.robust = robust
+        self.robust_stats = z(2)  # {inlier fraction, threshold} of the latest iteration with loss weights (device)
         self.mcmc = mcmc.check() if mcmc is not None else None
         self.mcmc_terms = z(2)  # {opacity term, scale term} of the latest iteration with MCMC (device)
         if mcmc is not None:
@@ -200,7 +211,7 @@ class FusedTrainStep:
             color_max_sh_band: int, feature_learning_rate: float, position_learning_rate: float,
             targets: Optional[SupervisionTargets] = None, background: Optional[torch.Tensor] = None,
             appearance_view: Optional[int] = None, mcmc_num_valid: Optional[int] = None,
-            filter_3d: Optional[torch.Tensor] = None) -> None:
+            filter_3d: Optional[torch.Tensor] = None, robust_active: Optional[bool] = None) -> None:
         """``targets``: the view's depth and / or mask target ((H, W) float32 CUDA tensors) and, with ``extra_features``, its
         ``labels`` ((H, W) int32) or ``features`` ((H, W, C) float32); ``background``: a (3,) float32 CUDA tensor the image is
         composited on (read on the device when the step runs, so it may be refilled per iteration).  Without supervision
@@ -209,7 +220,10 @@ class FusedTrainStep:
         the image and takes an Adam step (``gsb200_train_step_appearance``).  ``mcmc_num_valid``: with ``mcmc``, the number
         of valid rows n_v of the regularisers (``gsb200_train_step_mcmc``); the noise counter is the 0-based iteration.
         ``filter_3d``: the (N,) float32 3D smoothing filter of the rows (``mip_filter.compute_filter_3d``), contiguous, on the
-        scene's device; the forward and the backward render through it (``gsb200_train_step_filter3d``)."""
+        scene's device; the forward and the backward render through it (``gsb200_train_step_filter3d``).
+        ``targets.loss_weight``: the view's static (H, W) float32 weight of the image loss in [0, 1] (always used when given);
+        ``robust_active``: whether this iteration applies the ``robust`` inlier mask (default: when ``robust`` is set).  With
+        either, the image loss is weighted per pixel (``gsb200_train_step_robust``)."""
         sc, cfg = self.scene, self.config
         H, W = int(camera_info.camera_height), int(camera_info.camera_width)
         if image_gt.shape != (3, H, W) or not image_gt.is_contiguous() or image_gt.dtype != torch.float32:
@@ -245,6 +259,17 @@ class FusedTrainStep:
             raise ValueError("appearance_view needs appearance_grids")
         if (self.mcmc is None) != (mcmc_num_valid is None):
             raise ValueError("mcmc and mcmc_num_valid must be given together")
+        if robust_active is None:
+            robust_active = self.robust is not None
+        elif robust_active and self.robust is None:
+            raise ValueError("robust_active needs FusedTrainStep(robust=RobustLossConfig(...))")
+        static_w = targets.loss_weight
+        if static_w is not None and (tuple(static_w.shape) != (H, W) or not static_w.is_contiguous()
+                                     or static_w.dtype != torch.float32 or static_w.device != image_gt.device):
+            raise ValueError(f"targets.loss_weight must be a contiguous float32 ({H}, {W}) tensor on {image_gt.device}")
+        weighted = bool(robust_active) or static_w is not None
+        if weighted and (H % 16 or W % 16):
+            raise ValueError(f"the loss weights need H and W to be multiples of 16, got {H}x{W}")
         if filter_3d is not None and (tuple(filter_3d.shape) != (self.N,) or filter_3d.dtype != torch.float32
                                       or not filter_3d.is_contiguous() or filter_3d.device != image_gt.device):
             raise ValueError(f"filter_3d must be a contiguous float32 ({self.N},) tensor on {image_gt.device}")
@@ -333,7 +358,25 @@ class FusedTrainStep:
                     num_valid=int(mcmc_num_valid), lambda_opacity=mc.opacity_reg, lambda_scale=mc.scale_reg,
                     noise_scale=mc.noise_lr * float(position_learning_rate), gate_k=GATE_K, min_opacity=mc.min_opacity,
                     seed=int(mc.seed), step=self.step_count - 1, terms_out2=_ptr(self.mcmc_terms), temp=_ptr(self._mcmc_temp))
-            if filter_3d is not None:
+            if weighted:
+                if not hasattr(b, "robust_temp"):
+                    rl_bytes = int(self._lib.gsb200_robust_temp_bytes(H, W))
+                    b.loss_weight = torch.empty((H, W), dtype=torch.float32, device=self.device)
+                    b.composite = torch.empty((H, W, 3), dtype=torch.float32, device=self.device)
+                    b.robust_temp = torch.zeros(rl_bytes, dtype=torch.uint8, device=self.device)
+                cfg_r = self.robust or RobustLossConfig()
+                rob = _lib.GsbRobustLossArgs(
+                    static_weight=_ptr(static_w) if static_w is not None else None, robust=int(bool(robust_active)),
+                    inlier_quantile=cfg_r.inlier_quantile, box_threshold=cfg_r.box_threshold,
+                    patch_threshold=cfg_r.patch_threshold, weight_out=_ptr(b.loss_weight), composite=_ptr(b.composite),
+                    temp=_ptr(b.robust_temp), temp_bytes=b.robust_temp.numel(), stats_out2=_ptr(self.robust_stats))
+                _lib.check(self._lib.gsb200_train_step_robust(
+                    ctypes.byref(args), ctypes.byref(sup) if supervised else None, ctypes.byref(fx) if fx is not None else None,
+                    ctypes.byref(app) if app is not None else None,
+                    ctypes.byref(mcmc_args) if mcmc_args is not None else None,
+                    ctypes.byref(_lib.GsbFilter3dArgs(filter3d=_ptr(filter_3d))) if filter_3d is not None else None,
+                    ctypes.byref(rob)), "gsb200_train_step_robust")
+            elif filter_3d is not None:
                 _lib.check(self._lib.gsb200_train_step_filter3d(
                     ctypes.byref(args), ctypes.byref(sup) if supervised else None, ctypes.byref(fx) if fx is not None else None,
                     ctypes.byref(app) if app is not None else None,
@@ -355,8 +398,8 @@ class FusedTrainStep:
             else:
                 _lib.check(self._lib.gsb200_train_step(ctypes.byref(args)), "gsb200_train_step")
         self._pending[slot] = True
-        self._last = SimpleNamespace(buffers=b, H=H, W=W, slot=slot, supervised=supervised,
-                                     keep=(q, t, K, image_gt, depth_t, mask_t, background, feat_t, filter_3d))
+        self._last = SimpleNamespace(buffers=b, H=H, W=W, slot=slot, supervised=supervised, weighted=weighted,
+                                     keep=(q, t, K, image_gt, depth_t, mask_t, background, feat_t, filter_3d, static_w))
 
     @property
     def moments(self) -> MCMCMoments:
@@ -370,6 +413,11 @@ class FusedTrainStep:
     def image(self) -> torch.Tensor:
         """(H,W,3) rasterised image of the latest iteration (before the clamp)."""
         return self._last.buffers.image
+
+    @property
+    def loss_weight(self) -> Optional[torch.Tensor]:
+        """(H,W) per-pixel weight w of the image loss of the latest iteration (None when it had no loss weights)."""
+        return self._last.buffers.loss_weight if self._last is not None and self._last.weighted else None
 
     @property
     def feature_map(self) -> torch.Tensor:

@@ -18,7 +18,9 @@ grey mask), cropped and autoscaled with the image: the mask with the image's ant
 neighbour so that a sparse map stays sparse.  Two more optional keys carry targets for per-Gaussian feature training:
 ``labels_path`` (``.npy`` integer (H, W) class ids, read as int32; outside [0, C) = no label) and ``features_path``
 (``.npy`` float32 (H, W, C); NaN = no target), both at the resolution of the image on disk and cropped and autoscaled with
-the image by nearest neighbour.
+the image by nearest neighbour.  The optional key ``loss_weight_path`` gives the view's per-pixel weight of the image loss
+(``SupervisionTargets.loss_weight``, 0 = ignore the pixel, e.g. a segmentation mask of people or cars): an image read like
+``mask_path`` or a ``.npy`` float32 (H, W), with values in [0, 1], cropped and autoscaled like the mask.
 An optional record key ``distortion`` (an extension), ``{"model": "opencv" | "fisheye", "coefficients": [...]}``, gives the
 view's ``CameraInfo.distortion`` (``Camera.LensDistortion``).  The coefficients act on the normalised image plane, so
 rescaling, cropping and autoscale leave them unchanged.
@@ -135,8 +137,8 @@ class ImagePoseDataset(torch.utils.data.Dataset):
         return x
 
     def _load_targets(self, rec: dict, height: int, width: int) -> Tuple[torch.Tensor, ...]:
-        """(depth, mask, labels, features) at the resolution of the image on disk, or None each: depth and mask (H, W)
-        float32, labels (H, W) int32, features (H, W, C) float32."""
+        """(depth, mask, labels, features, loss_weight) at the resolution of the image on disk, or None each: depth, mask
+        and loss_weight (H, W) float32, labels (H, W) int32, features (H, W, C) float32."""
         depth = mask = None
         if rec.get("depth_path"):
             depth = torch.from_numpy(np.ascontiguousarray(np.load(self._path(rec["depth_path"])), dtype=np.float32))
@@ -149,7 +151,19 @@ class ImagePoseDataset(torch.utils.data.Dataset):
                 raise ValueError(f"{rec['mask_path']}: mask is {tuple(mask.shape)}, the image is {(height, width)}")
         labels = self._load_npy(rec, "labels_path", np.int32, height, width, "label map")
         features = self._load_npy(rec, "features_path", np.float32, height, width, "feature map")
-        return depth, mask, labels, features
+        loss_weight = None
+        if rec.get("loss_weight_path"):
+            path = self._path(rec["loss_weight_path"])
+            if path.endswith(".npy"):
+                loss_weight = torch.from_numpy(np.ascontiguousarray(np.load(path), dtype=np.float32))
+            else:
+                loss_weight = _load_image(path)[-1].contiguous()
+            if tuple(loss_weight.shape) != (height, width):
+                raise ValueError(f"{rec['loss_weight_path']}: loss weight is {tuple(loss_weight.shape)}, the image is "
+                                 f"{(height, width)}")
+            if not bool(((loss_weight >= 0) & (loss_weight <= 1)).all()):
+                raise ValueError(f"{rec['loss_weight_path']}: loss weights must lie in [0, 1]")
+        return depth, mask, labels, features, loss_weight
 
     @staticmethod
     def _crop_and_scale_nearest(x: torch.Tensor, info: CameraInfo) -> torch.Tensor:
@@ -171,10 +185,10 @@ class ImagePoseDataset(torch.utils.data.Dataset):
                              f"{(info.camera_height, info.camera_width)}")
         return x.contiguous()
 
-    def _crop_and_scale_targets(self, depth, mask, labels, features, info: CameraInfo) -> SupervisionTargets:
+    def _crop_and_scale_targets(self, depth, mask, labels, features, loss_weight, info: CameraInfo) -> SupervisionTargets:
         """The targets cropped to the tile multiple and, if the image was autoscaled, resized to its size."""
         out = []
-        for x, nearest in ((depth, True), (mask, False)):
+        for x, nearest in ((depth, True), (mask, False), (loss_weight, False)):
             if x is not None:
                 x = _crop_to_tiles(x[None])[0]
                 if max(x.shape[0], x.shape[1]) > MAX_RESOLUTION_TRAIN:
@@ -189,7 +203,7 @@ class ImagePoseDataset(torch.utils.data.Dataset):
                 x = x.contiguous()
             out.append(x)
         labels, features = (None if x is None else self._crop_and_scale_nearest(x, info) for x in (labels, features))
-        return SupervisionTargets(depth=out[0], mask=out[1], labels=labels, features=features)
+        return SupervisionTargets(depth=out[0], mask=out[1], labels=labels, features=features, loss_weight=out[2])
 
     def __getitem__(self, idx: int):
         rec = self.records[idx]

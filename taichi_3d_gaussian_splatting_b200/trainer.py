@@ -37,6 +37,12 @@ fixed budget by relocating dead Gaussians and adding 5 % per refinement (``mcmc.
 opacity and scale regularisers in the loss and a covariance-shaped position noise after the optimiser step.  The adaptive
 controller and the backward hook are then not used.  Not with the optional scale regulariser of the loss function nor with a
 view-parallel gradient exchange.
+Optional per-pixel weights of the image loss (an extension; ``TrainConfig.robust_loss``, per-view
+``SupervisionTargets.loss_weight``): transient distractors (people, cars, shadows in one view only) are dropped from the
+image loss by RobustNeRF's trimmed inlier mask of each iteration's residual and / or by a static weight per view
+(``loss.robust_weight``), in the autograd loop (torch form, inside the appearance grid's wrapper) and in the fused step
+(``gsb200_train_step_robust``).  The depth, mask and feature terms are not weighted; ``validation`` is unchanged.  Not with
+the view-parallel gradient exchange.
 The rasteriser is injected (default: the CUDA operator) so that tests can run the identical loop with the
 CPU oracle behind the same interface and compare PSNR trajectories.
 """
@@ -51,7 +57,8 @@ from .appearance import apply_bilateral_grid, bilateral_grid_tv, check_grid_shap
 from .Camera import CameraInfo, LensDistortion, RollingShutter
 from .densification import GaussianPointAdaptiveController
 from .GaussianPointCloudRasterisation import GaussianPointCloudRasterisation
-from .loss import FEATURE_LOSSES, LossFunction, SupervisionTargets, feature_loss, mcmc_regulariser, supervision_loss
+from .loss import (FEATURE_LOSSES, LossFunction, RobustLossConfig, SupervisionTargets, feature_loss, mcmc_regulariser,
+                   robust_composite, robust_weight, supervision_loss)
 from .mcmc import GATE_K, GaussianPointMCMCController, MCMCConfig, MCMCMoments, add_position_noise
 from .mip_filter import compute_filter_3d
 
@@ -96,9 +103,9 @@ def _nearest(x: torch.Tensor, h: int, w: int, hc: int, wc: int) -> torch.Tensor:
 
 
 def downsample_targets(targets: SupervisionTargets, camera_info: CameraInfo, downsample_factor: int) -> SupervisionTargets:
-    """The targets of a view at the schedule's resolution: the mask with the image's antialiased resize, the depth, the
-    labels and the feature map with nearest neighbour (a sparse map stays sparse, nothing is blended across an edge); all
-    cropped like the image."""
+    """The targets of a view at the schedule's resolution: the mask and the loss weight with the image's antialiased resize,
+    the depth, the labels and the feature map with nearest neighbour (a sparse map stays sparse, nothing is blended across
+    an edge); all cropped like the image."""
     h = camera_info.camera_height // downsample_factor
     w = camera_info.camera_width // downsample_factor
     hc, wc = h - h % 16, w - w % 16
@@ -110,7 +117,11 @@ def downsample_targets(targets: SupervisionTargets, camera_info: CameraInfo, dow
         depth = F.interpolate(targets.depth[None, None], size=(h, w), mode="nearest")[0, 0, :hc, :wc].contiguous()
     labels = None if targets.labels is None else _nearest(targets.labels, h, w, hc, wc)
     features = None if targets.features is None else _nearest(targets.features, h, w, hc, wc)
-    return SupervisionTargets(depth=depth, mask=mask, labels=labels, features=features)
+    loss_weight = None
+    if targets.loss_weight is not None:
+        loss_weight = F.interpolate(targets.loss_weight[None, None], size=(h, w), mode="bilinear", antialias=True,
+                                    align_corners=False)[0, 0, :hc, :wc].contiguous()
+    return SupervisionTargets(depth=depth, mask=mask, labels=labels, features=features, loss_weight=loss_weight)
 
 
 @dataclass
@@ -191,6 +202,10 @@ class GaussianPointCloudTrainer:
         mip_filter_3d: bool = False
         mip_filter_variance: float = 0.2
         mip_filter_interval: int = 100
+        # optional robust image loss against transient distractors (RobustNeRF's trimmed inlier mask, loss.robust_weight),
+        # from robust_loss.start_iteration on.  A view whose targets carry loss_weight is weighted by it in any case.  Not
+        # with the view-parallel exchange.
+        robust_loss: Optional[RobustLossConfig] = None
 
     def __init__(self, config: "GaussianPointCloudTrainer.TrainConfig", scene: Scene, train_views: List[View],
                  rasterisation_factory: Optional[Callable] = None, generator: Optional[torch.Generator] = None,
@@ -305,6 +320,11 @@ class GaussianPointCloudTrainer:
         self._features = config.feature_loss != "none"
         if self._features:
             self._check_feature_config(config, scene, targets)
+        if config.robust_loss is not None and not isinstance(config.robust_loss, RobustLossConfig):
+            raise ValueError(f"robust_loss must be a RobustLossConfig, got {type(config.robust_loss).__name__}")
+        # per-pixel weights of the image loss: the robust mask and / or a view's static loss_weight
+        self._weighted = config.robust_loss is not None or any(tg.loss_weight is not None for tg in targets)
+        self._robust_stats = None
         self.config = config
         self._need_depth = config.depth_loss_weight > 0
         self._need_alpha = config.mask_loss_weight > 0 or config.background != "black"
@@ -349,6 +369,9 @@ class GaussianPointCloudTrainer:
             raise ValueError('densification="mcmc" is not implemented for the view-parallel gradient exchange')
         if self._mip and getattr(self.rasterisation, "gradient_exchange", None) is not None:
             raise ValueError("mip_filter_3d is not implemented for the view-parallel gradient exchange")
+        if self._weighted and getattr(self.rasterisation, "gradient_exchange", None) is not None:
+            raise ValueError("robust_loss and per-view loss_weight targets are not implemented for the view-parallel "
+                             "gradient exchange")
         self.loss_function = LossFunction(config=config.loss_function_config)
         self.history: List[dict] = []
         self._downsampled = {}
@@ -440,7 +463,7 @@ class GaussianPointCloudTrainer:
             if key not in self._downsampled:
                 image_ds, camera_ds = downsample_image_and_camera_info(image_gt, camera_info, downsample_factor)
                 self._downsampled[key] = (image_ds, camera_ds, downsample_targets(targets, camera_info, downsample_factor)
-                                          if self.supervised or self._features else targets)
+                                          if self.supervised or self._features or self._weighted else targets)
             image_gt, camera_info, targets = self._downsampled[key]
         return image_gt, q, t, camera_info, targets
 
@@ -514,6 +537,7 @@ class GaussianPointCloudTrainer:
         step = FusedTrainStep(self.scene, cfg.rasterisation_config, cfg.loss_function_config.lambda_value,
                               controller=self.adaptive_controller, depth_weight=cfg.depth_loss_weight,
                               mask_weight=cfg.mask_loss_weight, mcmc=cfg.mcmc_config if self._mcmc else None,
+                              robust=cfg.robust_loss,
                               **(dict(extra_features=self.scene.point_extra_features, feature_loss=cfg.feature_loss,
                                       feature_weight=cfg.feature_loss_weight,
                                       extra_feature_learning_rate=cfg.extra_feature_learning_rate) if self._features else {}),
@@ -536,7 +560,9 @@ class GaussianPointCloudTrainer:
                 app_kw["mcmc_num_valid"] = self.mcmc_controller.num_valid
             if self._mip:
                 app_kw["filter_3d"] = self._filter_3d
-            if self.supervised or self._features:
+            if cfg.robust_loss is not None:
+                app_kw["robust_active"] = iteration >= cfg.robust_loss.start_iteration
+            if self.supervised or self._features or self._weighted:
                 step.run(image_gt, q, t, camera_info, band, cfg.feature_learning_rate, position_lr, targets=targets,
                          background=self._next_background(), **app_kw)
             else:
@@ -567,6 +593,8 @@ class GaussianPointCloudTrainer:
                 if self._mcmc:
                     entry["mcmc_opacity_reg"], entry["mcmc_scale_reg"] = step.mcmc_terms.tolist()
                     entry["loss"] += entry["mcmc_opacity_reg"] + entry["mcmc_scale_reg"]
+                if self._weighted:
+                    entry["robust_inlier_fraction"] = float(step.robust_stats[0]) if step.loss_weight is not None else 1.0
                 self.history.append(entry)
         return self.history
 
@@ -650,9 +678,10 @@ class GaussianPointCloudTrainer:
                                          rolling_shutter=RollingShutter(values[:3], values[3:]))
                 lens_kw = {"rolling_shutter_motion": leaf}
             band = iteration // cfg.increase_color_max_sh_band_interval
-            if self.supervised or self._features or self._appearance:
+            if self.supervised or self._features or self._appearance or self._weighted:
+                robust_active = cfg.robust_loss is not None and iteration >= cfg.robust_loss.start_iteration
                 loss, l1_loss, mask_term, depth_term, feature_term, appearance_tv, image_pred = self._supervised_loss(
-                    q, t, camera_info, band, image_gt, targets, lens_kw, view_index)
+                    q, t, camera_info, band, image_gt, targets, lens_kw, view_index, robust_active)
             elif self.fused_image_loss:
                 image_pred, _, _ = self.rasterisation(self._input(q, t, camera_info, band), **lens_kw)
                 loss, l1_loss, ssim_loss = self.loss_function.forward_rasterized(
@@ -711,16 +740,21 @@ class GaussianPointCloudTrainer:
                     entry["appearance_tv"] = float(appearance_tv.detach())
                 if self._mcmc:
                     entry["mcmc_opacity_reg"], entry["mcmc_scale_reg"] = mcmc_terms.detach().tolist()
+                if self._weighted:
+                    entry["robust_inlier_fraction"] = float(self._robust_stats[0]) if self._robust_stats is not None else 1.0
                 self.history.append(entry)
         return self.history
 
-    def _supervised_loss(self, q, t, camera_info, band, image_gt, targets, lens_kw=None, view_index=None):
+    def _supervised_loss(self, q, t, camera_info, band, image_gt, targets, lens_kw=None, view_index=None,
+                         robust_active=False):
         """Forward with the differentiable outputs the terms need, then ``loss.supervision_loss`` with this trainer's image
         loss (the torch one, or the fused kernels with ``fused_image_loss``; the scale regulariser if enabled), plus
         ``loss.feature_loss`` on the rendered feature map with a feature loss.  Returns (total, L1, mask term, depth term,
         feature term, the weighted TV term of the appearance grid, the raw image as (3, H, W) for the PSNR log).
         ``lens_kw``: the operator's ``lens_coefficients`` argument with lens refinement.  With appearance grids the image
-        loss reads the image (after the background composite) sliced through the grid of ``view_index``."""
+        loss reads the image (after the background composite) sliced through the grid of ``view_index``.  With loss weights
+        (the view's ``targets.loss_weight``, and the robust mask when ``robust_active``) the image loss reads the composite
+        ``loss.robust_composite`` of that image under ``loss.robust_weight``."""
         cfg = self.config
         lens_kw = lens_kw or {}
         if self._features:
@@ -736,6 +770,15 @@ class GaussianPointCloudTrainer:
         else:
             image_loss = lambda pred, gt: self.loss_function(  # noqa: E731
                 torch.clamp(pred, min=0, max=1).permute(2, 0, 1), gt, **regulariser)
+        self._robust_stats = None
+        static_w = targets.loss_weight if targets is not None else None
+        if robust_active or static_w is not None:
+            weighted_image_loss = image_loss
+            robust_cfg = cfg.robust_loss if robust_active else None
+
+            def image_loss(pred, gt):
+                w, self._robust_stats = robust_weight(pred.detach(), gt, static_w, robust_cfg)
+                return weighted_image_loss(robust_composite(pred, gt, w), gt)
         appearance_tv = None
         if self._appearance:
             grid = self._appearance_leaves[view_index]
