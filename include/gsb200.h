@@ -474,6 +474,55 @@ int gsb200_backward_rolling_shutter(const GsbBackwardArgs *args, const float *gr
                                     const GsbExtraFeatureArgs *ext, const GsbLensArgs *lens, const GsbRollingShutterArgs *rs,
                                     const GsbRollingShutterGradArgs *rs_grad);  /* lens, rs, rs_grad or NULL */
 
+/* Motion blur (an extension: the reference renders every view as if the shutter were instantaneous).  A view may carry an
+ * exposure motion m_b = (v, w) (float32 x 6): the apparent motion of the scene in the camera frame over the whole exposure,
+ * in the convention of GsbRollingShutterArgs::motion; the view's pose is the pose at mid-exposure.  With pc the camera-frame
+ * point as rendered without blur (with a rolling shutter: pc(tau_3), and W is W_eff) and Jp = d(u, v)/d pc the full position
+ * Jacobian (full K, and the lens D when there is one):
+ *   d = Jp (v + w x pc)                  the screen displacement of the splat centre over the exposure
+ *   B = d d^T / 12                       the second moment of a uniform sweep t in [-1/2, 1/2]
+ *   conic = (Sigma_d + B)^-1,  Sigma_d = Sigma' + 0.3 I
+ *   rescale slot = rescale c_b,  rescale = sqrt(det Sigma' / det Sigma_d) (detached),  c_b = sqrt(det Sigma_d / det(Sigma_d + B))
+ *   radius (and the tile square) from Sigma' + B; the reach test runs on the blurred conic
+ * c_b keeps each splat's integrated weight over the sweep.  m_b = 0 takes the un-blurred arithmetic: records, keys, images and
+ * every gradient are those of the call without blur, bit for bit.  The model replaces the box-shaped streak by a Gaussian of
+ * equal variance, linearises the screen trajectory at mid-exposure and composites time-averaged splats.
+ * Only +-m_b is observable (B depends on d d^T alone), and dB/dm_b = 0 at m_b = 0: refining m_b needs a non-zero start.
+ * Gradients: d is detached with respect to the point (like J, tau and rescale).  With G = dL/dSigma' of the blend and
+ * G_a = glogit / fl(1 - o) (the 3D filter's recovery of sum dL/dalpha alpha; dropped where fl(1 - o) = 0):
+ *   dL/dSigma' = G + G_a/2 (Sigma_d^-1 - (Sigma_d + B)^-1)
+ *   dL/dd = G d / 6 - G_a/12 (Sigma_d + B)^-1 d,   g = Jp^T dL/dd
+ *   dL/dv = sum_i g_i,   dL/dw = sum_i pc_i x g_i
+ * summed over every in-camera point of every object (GsbMotionBlurGradArgs; every loss term that reaches the accumulator rows
+ * contributes).  The sum is deterministic as the rolling shutter's: min(ceil(N/128), GSB_RS_GRAD_PARTIAL_BLOCKS) per-CTA rows
+ * in `temp`, added in block order by a second kernel.  Not implemented with the 3D filter, the rolling-shutter motion
+ * gradient, pose / intrinsics / lens-coefficient gradients or the compact rows of the view-parallel exchange. */
+typedef struct GsbMotionBlurArgs {
+    float motion[6];  /* v (3), w (3) over the whole exposure */
+} GsbMotionBlurArgs;
+typedef struct GsbMotionBlurGradArgs {
+    float *grad_motion; /* (6,) out, dL/dv then dL/dw */
+    void *temp;         /* gsb200_motion_blur_grad_temp_bytes() bytes, 16-byte aligned */
+} GsbMotionBlurGradArgs;
+/* GSB_RS_GRAD_PARTIAL_BLOCKS * 6 floats */
+int64_t gsb200_motion_blur_grad_temp_bytes(void);
+/* sizeof(GsbMotionBlurArgs), sizeof(GsbMotionBlurGradArgs) (a call of their own, like gsb200_abi_sizes_mcmc) */
+void gsb200_abi_sizes_motion_blur(int64_t *out2);
+/* gsb200_forward_rolling_shutter with the exposure motion of `blur`.  NULL blur: exactly gsb200_forward_rolling_shutter.
+ * Before any CUDA call: the checks of gsb200_forward_rolling_shutter; GSB_EINVAL for a non-finite motion. */
+int gsb200_forward_motion_blur(const GsbForwardArgs *args, const GsbExtraFeatureArgs *ext, const GsbLensArgs *lens,
+                               const GsbRollingShutterArgs *rs, const GsbMotionBlurArgs *blur);  /* lens, rs, blur or NULL */
+/* gsb200_backward_rolling_shutter (without the rolling-shutter motion gradient) of a frame rendered by
+ * gsb200_forward_motion_blur with the same lens, rs and blur.  NULL blur: exactly gsb200_backward_rolling_shutter(..., NULL).
+ * NULL blur_grad: no motion gradient; every other output is bit-identical to the call with blur_grad.  Before any CUDA call:
+ * the checks of gsb200_forward_motion_blur; GSB_EINVAL for a blur_grad without blur, a NULL output or temp pointer, an output
+ * that is not 4-byte aligned or a temp that is not 16-byte aligned; GSB_EUNSUPPORTED for GSB_FLAG_COMPACT_GRADS.  An
+ * image-only loss works with either loop-A kernel; the other terms keep their requirement of GSB_FLAG_BACKWARD_TRANSPOSED. */
+int gsb200_backward_motion_blur(const GsbBackwardArgs *args, const float *grad_rasterized_depth, const float *rasterized_depth,
+                                const float *grad_pixel_accumulated_alpha, const GsbExtraFeatureArgs *ext,
+                                const GsbLensArgs *lens, const GsbRollingShutterArgs *rs, const GsbMotionBlurArgs *blur,
+                                const GsbMotionBlurGradArgs *blur_grad);  /* lens, rs, blur, blur_grad or NULL */
+
 int gsb200_expand_view_gradients(const GsbExpandArgs *args);
 
 /* The two collectives of the compact exchange as ONE hand-written kernel over NVSwitch multicast memory (NVLS; csrc/exchange.cu):

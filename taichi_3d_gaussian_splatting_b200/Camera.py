@@ -4,7 +4,8 @@ Mirrors the reference's ``taichi_3d_gaussian_splatting/Camera.py:7-21`` (``Camer
 argument of ``GaussianPointCloudRasterisationInput``; ``CameraView`` is imported beside it at
 GaussianPointCloudRasterisation.py:4).  ``LensDistortion`` and ``CameraInfo.distortion`` are an extension: the reference
 projects through a pinhole only.  ``RollingShutter`` and ``CameraInfo.rolling_shutter`` are an extension as well: the reference
-projects every row with one global-shutter pose.
+projects every row with one global-shutter pose.  So are ``MotionBlur`` and ``CameraInfo.motion_blur``: the reference renders every
+view as if the shutter were instantaneous.
 """
 import math
 from dataclasses import dataclass
@@ -100,6 +101,76 @@ class RollingShutter:
         return self.linear + self.angular
 
 
+@dataclass(frozen=True)
+class MotionBlur:
+    """The exposure motion of a blurred view (definition in ``include/gsb200.h``), as host floats: ``linear`` = v (scene
+    units) and ``angular`` = w (radians), the apparent motion of the scene in the camera frame over the whole exposure, in the
+    convention of ``RollingShutter``.  The view's pose is the pose at mid-exposure.
+
+    Two properties of the model: only +-m is observable (the blur depends on d d^T, so m and -m render the same), and the
+    blur's gradient with respect to m vanishes at m = 0, so refining it needs a non-zero start (from visual-inertial
+    odometry through ``from_camera_velocity``, or from neighbouring frames through ``between_poses``)."""
+    linear: Tuple[float, float, float]
+    angular: Tuple[float, float, float]
+
+    def __post_init__(self):
+        for name in ("linear", "angular"):
+            v = tuple(float(x) for x in getattr(self, name))
+            if len(v) != 3:
+                raise ValueError(f"motion-blur {name} motion takes 3 values, got {len(v)}")
+            if not all(math.isfinite(x) for x in v):
+                raise ValueError(f"motion-blur {name} motion must be finite, got {v}")
+            object.__setattr__(self, name, v)
+
+    @staticmethod
+    def from_camera_velocity(linear_velocity: Sequence[float], angular_velocity: Sequence[float],
+                             exposure_time: float) -> "MotionBlur":
+        """The exposure motion of a camera moving at ``linear_velocity`` (scene units/s) and ``angular_velocity`` (rad/s),
+        both in the camera's own frame (what visual-inertial odometry and ARKit report), with the shutter open for
+        ``exposure_time`` seconds: a static scene moves the other way in the camera frame, v = -T u and w = -T w_c."""
+        T = float(exposure_time)
+        if not (math.isfinite(T) and T >= 0.0):
+            raise ValueError(f"exposure_time must be finite and >= 0, got {exposure_time}")
+        return MotionBlur(tuple(-T * float(x) for x in linear_velocity), tuple(-T * float(x) for x in angular_velocity))
+
+    @staticmethod
+    def between_poses(T_before: torch.Tensor, T_after: torch.Tensor, fraction: float) -> "MotionBlur":
+        """The exposure motion of a view between two frames of a video at constant velocity, ``fraction`` = exposure time
+        / frame interval.  ``T_before`` and ``T_after`` are the 4x4 camera -> scene transforms (``CameraView.
+        T_pointcloud_camera``) of the earlier and the later frame.  A = T_after^-1 T_before = [R_A | t_A] maps camera-frame
+        points of the earlier frame to the later one, and the motion is (fraction t_A, fraction log R_A): exact for this
+        model's motion pc(t) = exp(t [w]x) pc + t v at constant velocity."""
+        f = float(fraction)
+        if not (math.isfinite(f) and f >= 0.0):
+            raise ValueError(f"fraction must be finite and >= 0, got {fraction}")
+        Tb = torch.as_tensor(T_before, dtype=torch.float64).cpu()
+        Ta = torch.as_tensor(T_after, dtype=torch.float64).cpu()
+        if Tb.shape != (4, 4) or Ta.shape != (4, 4):
+            raise ValueError(f"T_before and T_after must be 4x4, got {tuple(Tb.shape)} and {tuple(Ta.shape)}")
+        A = torch.linalg.inv(Ta) @ Tb
+        R, t = A[:3, :3], A[:3, 3]
+        # log R: the axis-angle vector (theta in [0, pi]), by the skew part away from pi and the symmetric part near it
+        c = float(torch.clamp((torch.trace(R) - 1.0) / 2.0, -1.0, 1.0))
+        theta = math.acos(c)
+        skew = torch.stack([R[2, 1] - R[1, 2], R[0, 2] - R[2, 0], R[1, 0] - R[0, 1]])
+        if theta < 1e-6:
+            w = 0.5 * skew
+        elif math.pi - theta > 1e-4:
+            w = (theta / (2.0 * math.sin(theta))) * skew
+        else:
+            B = (R + torch.eye(3, dtype=torch.float64)) / 2.0
+            k = int(torch.argmax(torch.diagonal(B)))
+            axis = B[:, k] / torch.sqrt(B[k, k])
+            axis = axis * torch.sign(torch.dot(axis, skew)) if float(torch.dot(axis, skew)) != 0.0 else axis
+            w = theta * axis
+        return MotionBlur(tuple((f * t).tolist()), tuple((f * w).tolist()))
+
+    @property
+    def motion(self) -> Tuple[float, ...]:
+        """(v, w) as six floats, the order of ``GsbMotionBlurArgs::motion``."""
+        return self.linear + self.angular
+
+
 @dataclass
 class CameraInfo:
     camera_intrinsics: torch.Tensor  # 3x3 f32 pinhole matrix (device tensor in the reference)
@@ -108,6 +179,7 @@ class CameraInfo:
     camera_id: int
     distortion: Optional[LensDistortion] = None  # extension: None is the reference's pinhole
     rolling_shutter: Optional[RollingShutter] = None  # extension: None is the reference's global shutter
+    motion_blur: Optional[MotionBlur] = None  # extension: None is the reference's instantaneous exposure
 
 
 @dataclass

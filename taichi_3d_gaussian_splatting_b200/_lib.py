@@ -139,6 +139,14 @@ class GsbRollingShutterGradArgs(ctypes.Structure):
     _fields_ = [("grad_motion", c_vp), ("temp", c_vp)]
 
 
+class GsbMotionBlurArgs(ctypes.Structure):
+    _fields_ = [("motion", c_f32 * 6)]
+
+
+class GsbMotionBlurGradArgs(ctypes.Structure):
+    _fields_ = [("grad_motion", c_vp), ("temp", c_vp)]
+
+
 class GsbAppearanceArgs(ctypes.Structure):
     _fields_ = [
         ("grid", c_vp), ("grad_grid", c_vp), ("grid_x", c_i32), ("grid_y", c_i32), ("grid_z", c_i32), ("tv_weight", c_f32),
@@ -223,7 +231,8 @@ EXPORTS = (
     "gsb200_mcmc_temp_bytes", "gsb200_mcmc_regulariser", "gsb200_mcmc_noise", "gsb200_mcmc_relocate", "gsb200_train_step_mcmc",
     "gsb200_abi_sizes_mcmc", "gsb200_forward_filter3d", "gsb200_backward_filter3d", "gsb200_train_step_filter3d",
     "gsb200_filter3d_temp_bytes", "gsb200_filter3d_from_views", "gsb200_abi_sizes_filter3d", "gsb200_robust_temp_bytes",
-    "gsb200_robust_image_loss", "gsb200_train_step_robust", "gsb200_abi_sizes_robust",
+    "gsb200_robust_image_loss", "gsb200_train_step_robust", "gsb200_abi_sizes_robust", "gsb200_forward_motion_blur",
+    "gsb200_backward_motion_blur", "gsb200_motion_blur_grad_temp_bytes", "gsb200_abi_sizes_motion_blur",
 )
 
 _lib = None
@@ -287,6 +296,17 @@ def load() -> ctypes.CDLL:
     lib.gsb200_backward_rolling_shutter.restype = ctypes.c_int
     lib.gsb200_rolling_shutter_grad_temp_bytes.argtypes = []
     lib.gsb200_rolling_shutter_grad_temp_bytes.restype = c_i64
+    lib.gsb200_forward_motion_blur.argtypes = [ctypes.POINTER(GsbForwardArgs), ctypes.POINTER(GsbExtraFeatureArgs),
+                                               ctypes.POINTER(GsbLensArgs), ctypes.POINTER(GsbRollingShutterArgs),
+                                               ctypes.POINTER(GsbMotionBlurArgs)]
+    lib.gsb200_forward_motion_blur.restype = ctypes.c_int
+    lib.gsb200_backward_motion_blur.argtypes = [ctypes.POINTER(GsbBackwardArgs), c_vp, c_vp, c_vp,
+                                                ctypes.POINTER(GsbExtraFeatureArgs), ctypes.POINTER(GsbLensArgs),
+                                                ctypes.POINTER(GsbRollingShutterArgs), ctypes.POINTER(GsbMotionBlurArgs),
+                                                ctypes.POINTER(GsbMotionBlurGradArgs)]
+    lib.gsb200_backward_motion_blur.restype = ctypes.c_int
+    lib.gsb200_motion_blur_grad_temp_bytes.argtypes = []
+    lib.gsb200_motion_blur_grad_temp_bytes.restype = c_i64
     lib.gsb200_intrinsics_grad_temp_bytes.argtypes = []
     lib.gsb200_intrinsics_grad_temp_bytes.restype = c_i64
     lib.gsb200_sort_temp_bytes.argtypes = [c_i64, c_i32]
@@ -447,6 +467,14 @@ def load() -> ctypes.CDLL:
     if sizes15[14] != ctypes.sizeof(GsbAppearanceArgs):
         raise RuntimeError(f"libgsb200.so ABI mismatch: sizeof(GsbAppearanceArgs) {sizes15[14]} != ctypes mirror "
                            f"{ctypes.sizeof(GsbAppearanceArgs)}")
+    lib.gsb200_abi_sizes_motion_blur.argtypes = [ctypes.POINTER(c_i64)]
+    lib.gsb200_abi_sizes_motion_blur.restype = None
+    sizes_blur = (c_i64 * 2)()
+    lib.gsb200_abi_sizes_motion_blur(sizes_blur)
+    for i, mirror in ((0, GsbMotionBlurArgs), (1, GsbMotionBlurGradArgs)):
+        if sizes_blur[i] != ctypes.sizeof(mirror):
+            raise RuntimeError(f"libgsb200.so ABI mismatch: sizeof({mirror.__name__}) {sizes_blur[i]} != ctypes mirror "
+                               f"{ctypes.sizeof(mirror)}")
     lib.gsb200_abi_sizes_mcmc.argtypes = [ctypes.POINTER(c_i64)]
     lib.gsb200_abi_sizes_mcmc.restype = None
     sizes_mcmc = (c_i64 * 2)()

@@ -206,6 +206,11 @@ void gsb200_abi_sizes_mcmc(int64_t *out2) {
     out2[1] = (int64_t)sizeof(GsbMcmcStepArgs);
 }
 
+void gsb200_abi_sizes_motion_blur(int64_t *out2) {
+    out2[0] = (int64_t)sizeof(GsbMotionBlurArgs);
+    out2[1] = (int64_t)sizeof(GsbMotionBlurGradArgs);
+}
+
 void gsb200_abi_sizes_filter3d(int64_t *out2) {
     out2[0] = (int64_t)sizeof(GsbFilter3dArgs);
     out2[1] = (int64_t)sizeof(GsbFilter3dViewsArgs);
@@ -332,11 +337,50 @@ static int check_filter3d(const char *what, const GsbFilter3dArgs *filter, const
     return GSB_OK;
 }
 
+// GsbMotionBlurArgs -> BlurParams; GSB_EINVAL for a non-finite motion.  *out_blur stays NULL for a NULL blur.
+static int check_blur(const char *what, const GsbMotionBlurArgs *blur, BlurParams *params, const BlurParams **out_blur) {
+    *out_blur = nullptr;
+    if (!blur) return GSB_OK;
+    for (int i = 0; i < 6; ++i) {
+        const float m = blur->motion[i];
+        if (!(m - m == 0.0f)) {
+            set_error("%s: exposure motion %d is not finite", what, i);
+            return GSB_EINVAL;
+        }
+        params->motion[i] = m;
+    }
+    *out_blur = params;
+    return GSB_OK;
+}
+
+int64_t gsb200_motion_blur_grad_temp_bytes(void) {
+    return (int64_t)GSB_RS_GRAD_PARTIAL_BLOCKS * 6 * (int64_t)sizeof(float);
+}
+
+// The forward of gsb200_forward_filter3d / gsb200_forward_motion_blur after their own checks (filter3d and blur: checked, at
+// most one of them set)
+static int forward_checked(const GsbForwardArgs *a, const GsbExtraFeatureArgs *ext, const GsbLensArgs *lens_args,
+                           const GsbRollingShutterArgs *rs_args, const float *filter3d, const BlurParams *blur);
+
 int gsb200_forward_filter3d(const GsbForwardArgs *a, const GsbExtraFeatureArgs *ext, const GsbLensArgs *lens_args,
                             const GsbRollingShutterArgs *rs_args, const GsbFilter3dArgs *filter) {
     const float *filter3d;
     int frc = check_filter3d("forward_filter3d", filter, &filter3d);
     if (frc != GSB_OK) return frc;
+    return forward_checked(a, ext, lens_args, rs_args, filter3d, nullptr);
+}
+
+int gsb200_forward_motion_blur(const GsbForwardArgs *a, const GsbExtraFeatureArgs *ext, const GsbLensArgs *lens_args,
+                               const GsbRollingShutterArgs *rs_args, const GsbMotionBlurArgs *blur_args) {
+    BlurParams blur_params;
+    const BlurParams *blur;
+    int rc = check_blur("forward_motion_blur", blur_args, &blur_params, &blur);
+    if (rc != GSB_OK) return rc;
+    return forward_checked(a, ext, lens_args, rs_args, nullptr, blur);
+}
+
+static int forward_checked(const GsbForwardArgs *a, const GsbExtraFeatureArgs *ext, const GsbLensArgs *lens_args,
+                           const GsbRollingShutterArgs *rs_args, const float *filter3d, const BlurParams *blur) {
     LensParams lens_params;
     const LensParams *lens;
     int lrc = check_lens(rs_args ? "forward_rolling_shutter" : "forward_lens", lens_args, &lens_params, &lens);
@@ -362,7 +406,7 @@ int gsb200_forward_filter3d(const GsbForwardArgs *a, const GsbExtraFeatureArgs *
     int rc = resolve_fwd(a, &ws);
     if (rc != GSB_OK) return rc;
     cudaStream_t st = static_cast<cudaStream_t>(a->stream);
-    if ((rc = launch_preprocess(*a, ws, st, lens, rs, filter3d)) != GSB_OK) return rc;
+    if ((rc = launch_preprocess(*a, ws, st, lens, rs, filter3d, blur)) != GSB_OK) return rc;
     if (a->host_counters && a->host_counters_event) {
         GSB_CUDA_CHECK(cudaMemcpyAsync(a->host_counters, ws.counters, 4 * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
         GSB_CUDA_CHECK(cudaEventRecord(static_cast<cudaEvent_t>(a->host_counters_event), st));
@@ -380,7 +424,8 @@ static int backward_impl(const GsbBackwardArgs *a, bool skip_on_overflow, const 
                          const GsbExtraFeatureArgs *ext = nullptr, const GsbPoseGradArgs *pose = nullptr,
                          const GsbIntrinsicsGradArgs *intr = nullptr, const LensParams *lens = nullptr,
                          const GsbLensGradArgs *lens_grad = nullptr, const RsParams *rs = nullptr,
-                         const GsbRollingShutterGradArgs *rs_grad = nullptr, const float *filter3d = nullptr) {
+                         const GsbRollingShutterGradArgs *rs_grad = nullptr, const float *filter3d = nullptr,
+                         const BlurParams *blur = nullptr, const GsbMotionBlurGradArgs *blur_grad = nullptr) {
     if (!a) {
         set_error("backward: args is null");
         return GSB_EINVAL;
@@ -434,6 +479,7 @@ static int backward_impl(const GsbBackwardArgs *a, bool skip_on_overflow, const 
     if (ext && a->num_points > 0)  // the blend adds into the rows it reaches; every other row stays zero
         GSB_CUDA_CHECK(cudaMemsetAsync(ext->grad_features, 0, (size_t)a->num_points * ext->channels * 4, st));
     if ((rc = launch_blend_backward(*a, ws, st, grad_depth, depth, grad_alpha, ext)) != GSB_OK) return rc;
+    if (blur) return launch_backward_points_blur(*a, ws, st, grad_depth != nullptr, lens, rs, *blur, blur_grad);
     if (filter3d)
         return launch_backward_points_filter(*a, ws, st, skip_on_overflow ? ws.counters + CNT_OVERFLOW : nullptr,
                                              grad_depth != nullptr, lens, rs, filter3d);
@@ -464,7 +510,52 @@ static int backward_checked(const GsbBackwardArgs *a, const float *grad_rasteriz
                             const float *grad_pixel_accumulated_alpha, const GsbExtraFeatureArgs *ext, const GsbPoseGradArgs *pose,
                             const GsbIntrinsicsGradArgs *intr, const LensParams *lens, const GsbLensGradArgs *lens_grad = nullptr,
                             const RsParams *rs = nullptr, const GsbRollingShutterGradArgs *rs_grad = nullptr,
-                            const float *filter3d = nullptr);
+                            const float *filter3d = nullptr, const BlurParams *blur = nullptr,
+                            const GsbMotionBlurGradArgs *blur_grad = nullptr);
+
+int gsb200_backward_motion_blur(const GsbBackwardArgs *a, const float *grad_rasterized_depth, const float *rasterized_depth,
+                                const float *grad_pixel_accumulated_alpha, const GsbExtraFeatureArgs *ext,
+                                const GsbLensArgs *lens_args, const GsbRollingShutterArgs *rs_args,
+                                const GsbMotionBlurArgs *blur_args, const GsbMotionBlurGradArgs *blur_grad) {
+    if (!blur_args && blur_grad) {
+        set_error("backward_motion_blur: the exposure-motion gradient needs a motion blur (blur is NULL)");
+        return GSB_EINVAL;
+    }
+    if (!blur_args)
+        return gsb200_backward_rolling_shutter(a, grad_rasterized_depth, rasterized_depth, grad_pixel_accumulated_alpha, ext,
+                                               lens_args, rs_args, nullptr);
+    LensParams lens_params;
+    const LensParams *lens;
+    int rc = check_lens("backward_motion_blur", lens_args, &lens_params, &lens);
+    if (rc != GSB_OK) return rc;
+    RsParams rs_params;
+    const RsParams *rs;
+    if ((rc = check_rs("backward_motion_blur", rs_args, &rs_params, &rs)) != GSB_OK) return rc;
+    BlurParams blur_params;
+    const BlurParams *blur;
+    if ((rc = check_blur("backward_motion_blur", blur_args, &blur_params, &blur)) != GSB_OK) return rc;
+    if (blur_grad) {
+        if (!blur_grad->grad_motion || !blur_grad->temp) {
+            set_error("backward_motion_blur: null grad_motion / temp pointer");
+            return GSB_EINVAL;
+        }
+        if (reinterpret_cast<uintptr_t>(blur_grad->grad_motion) % 4 != 0) {
+            set_error("backward_motion_blur: grad_motion must be 4-byte aligned");
+            return GSB_EINVAL;
+        }
+        if (reinterpret_cast<uintptr_t>(blur_grad->temp) % 16 != 0) {
+            set_error("backward_motion_blur: the motion-blur temp must be 16-byte aligned");
+            return GSB_EINVAL;
+        }
+    }
+    if (a != nullptr && (a->flags & GSB_FLAG_COMPACT_GRADS)) {
+        set_error("backward_motion_blur: the motion blur is not implemented for the compact rows of the view-parallel exchange "
+                  "(GSB_FLAG_COMPACT_GRADS)");
+        return GSB_EUNSUPPORTED;
+    }
+    return backward_checked(a, grad_rasterized_depth, rasterized_depth, grad_pixel_accumulated_alpha, ext, nullptr, nullptr, lens,
+                            nullptr, rs, nullptr, nullptr, blur, blur_grad);
+}
 
 int gsb200_backward_filter3d(const GsbBackwardArgs *a, const float *grad_rasterized_depth, const float *rasterized_depth,
                              const float *grad_pixel_accumulated_alpha, const GsbExtraFeatureArgs *ext, const GsbLensArgs *lens_args,
@@ -604,7 +695,8 @@ int gsb200_backward_calib(const GsbBackwardArgs *a, const float *grad_rasterized
 static int backward_checked(const GsbBackwardArgs *a, const float *grad_rasterized_depth, const float *rasterized_depth,
                             const float *grad_pixel_accumulated_alpha, const GsbExtraFeatureArgs *ext, const GsbPoseGradArgs *pose,
                             const GsbIntrinsicsGradArgs *intr, const LensParams *lens, const GsbLensGradArgs *lens_grad,
-                            const RsParams *rs, const GsbRollingShutterGradArgs *rs_grad, const float *filter3d) {
+                            const RsParams *rs, const GsbRollingShutterGradArgs *rs_grad, const float *filter3d,
+                            const BlurParams *blur, const GsbMotionBlurGradArgs *blur_grad) {
     if (intr) {
         if (!intr->grad_camera_intrinsics || !intr->temp) {
             set_error("backward_calib: null grad_camera_intrinsics / temp pointer");
@@ -670,7 +762,7 @@ static int backward_checked(const GsbBackwardArgs *a, const float *grad_rasteriz
         return GSB_EUNSUPPORTED;
     }
     return backward_impl(a, false, grad_rasterized_depth, rasterized_depth, grad_pixel_accumulated_alpha, ext, pose, intr, lens,
-                         lens_grad, rs, rs_grad, filter3d);
+                         lens_grad, rs, rs_grad, filter3d, blur, blur_grad);
 }
 
 int gsb200_backward_with_depth(const GsbBackwardArgs *a, const float *grad_rasterized_depth, const float *rasterized_depth) {

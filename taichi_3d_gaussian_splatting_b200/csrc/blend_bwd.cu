@@ -436,22 +436,35 @@ __device__ __forceinline__ void weighted_u_sigma(const float *U, const float *R,
 // where o is the record's raw opacity r1.z (the float the blend multiplied by); the compensation term is dropped where
 // fl(1 - o) = 0.  dL/dlogit is unchanged: the compensation c does not depend on the logit.  Non-compact, without POSE / INTR /
 // LGRAD / MGRAD.
+// BLUR = true (gsb200_backward_motion_blur): the frame was rendered with the exposure motion m_b = blur.motion
+// (include/gsb200.h): the conic was (Sigma_d + B)^-1 with B = d d^T / 12, d = Jp (v + w x pc) (detached, from dj and
+// point_in_camera), and the rescale slot carried c_b.  G reaches Sigma' unchanged (B is additive), plus the compensation's
+// G_a/2 (Sigma_d^-1 - (Sigma_d + B)^-1) with G_a = glogit / fl(1 - o) (dropped where fl(1 - o) = 0), before V = U^T G U
+// (motion_blur_grad, common.cuh).  A view with m_b = 0 takes the un-blurred arithmetic.  Non-compact, without POSE / INTR /
+// LGRAD / MGRAD / FILTER; with or without LENS and RS.
+// BGRAD = true (with BLUR and blur_grad): each in-camera point also forms dL/dv = g and dL/dw = pc x g with g = Jp^T dL/dd,
+// which go through the rows of MGRAD: s_mgrad, mgrad_partials and rolling_shutter_grad_finish_kernel.
 constexpr int LENS_GRAD_VALUES = 5;
 constexpr int RS_GRAD_VALUES = 6;
 template <bool COMPACT, bool DEPTH, bool POSE, bool INTR = false, bool LENS = false, bool LGRAD = false, bool RS = false,
-          bool MGRAD = false, bool FILTER = false>
+          bool MGRAD = false, bool FILTER = false, bool BLUR = false, bool BGRAD = false>
 __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, float *s_pose, float *pose_partials,
                                                      int num_objects, float *s_intr = nullptr,
                                                      float *intr_partials = nullptr, const LensParams lens = LensParams(),
                                                      float *s_lgrad = nullptr, float *lgrad_partials = nullptr,
                                                      const RsParams rs = RsParams(), float *s_mgrad = nullptr,
-                                                     float *mgrad_partials = nullptr, const float *filter3d = nullptr) {
+                                                     float *mgrad_partials = nullptr, const float *filter3d = nullptr,
+                                                     const BlurParams blur = BlurParams()) {
     static_assert(!LENS || (!COMPACT && !POSE && !INTR), "the lens gradient is implemented for the dense rows alone");
     static_assert(!LGRAD || LENS, "the coefficient gradient needs the lens path");
     static_assert(!RS || (!COMPACT && !POSE && !INTR && !LGRAD), "the rolling shutter is implemented for the dense rows alone");
     static_assert(!MGRAD || RS, "the motion gradient needs the rolling-shutter path");
     static_assert(!FILTER || (!COMPACT && !POSE && !INTR && !LGRAD && !MGRAD),
                   "the 3D filter is implemented for the dense rows without camera gradients");
+    static_assert(!BLUR || (!COMPACT && !POSE && !INTR && !LGRAD && !MGRAD && !FILTER),
+                  "the motion blur is implemented for the dense rows without other camera gradients or the 3D filter");
+    static_assert(!BGRAD || BLUR, "the exposure-motion gradient needs the motion-blur path");
+    constexpr bool CAM6 = MGRAD || BGRAD;  // a 6-value motion gradient (rolling shutter or exposure)
     // One thread per scene row: rows outside the frustum get their zeros here (no separate memset of the
     // dense (N,3)/(N,56) gradients), rows inside get the chain rule.  A warp owns 32 consecutive rows, i.e. one
     // contiguous 7 KB piece of the (N,56) gradient and 384 B of the (N,3) one: each lane stages its row in
@@ -478,8 +491,8 @@ __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, fl
         if (lane < LENS_GRAD_VALUES) my_lgrad[lane] = 0.0f;
         __syncwarp();
     }
-    float *const my_mgrad = MGRAD ? s_mgrad + warp * RS_GRAD_VALUES : nullptr;
-    if (MGRAD) {
+    float *const my_mgrad = CAM6 ? s_mgrad + warp * RS_GRAD_VALUES : nullptr;
+    if (CAM6) {
         if (lane < RS_GRAD_VALUES) my_mgrad[lane] = 0.0f;
         __syncwarp();
     }
@@ -499,8 +512,8 @@ __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, fl
 #pragma unroll
           for (int k = 0; k < LENS_GRAD_VALUES; ++k) lv[k] = 0.0f;
       }
-      float mv[MGRAD ? RS_GRAD_VALUES : 1];  // zero for rows outside the frustum
-      if (MGRAD) {
+      float mv[CAM6 ? RS_GRAD_VALUES : 1];  // zero for rows outside the frustum
+      if (CAM6) {
 #pragma unroll
           for (int k = 0; k < RS_GRAD_VALUES; ++k) mv[k] = 0.0f;
       }
@@ -577,7 +590,37 @@ __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, fl
             U[c] = J[0] * Wm[c] + J[1] * Wm[3 + c] + J[2] * Wm[6 + c];
             U[3 + c] = J[3] * Wm[c] + J[4] * Wm[3 + c] + J[5] * Wm[6 + c];
         }
-        const float g00 = 0.5f * a0.z, g01 = 0.5f * a0.w, g11 = 0.5f * a1.x;  // UT:345's 1/2, see the blend loop
+        float g00 = 0.5f * a0.z, g01 = 0.5f * a0.w, g11 = 0.5f * a1.x;  // UT:345's 1/2, see the blend loop
+        if (BLUR && motion_blur_on(blur.motion)) {
+            // Sigma' = (U M)(U M)^T, M = R(q) diag(exp(s)) (the rows of R and exp(s) as below)
+            const float bx = qv.x, by = qv.y, bz = qv.z, bw = qv.w;
+            const float Rb[9] = {1 - 2 * (by * by + bz * bz), 2 * (bx * by - bw * bz), 2 * (bx * bz + bw * by),
+                                 2 * (bx * by + bw * bz), 1 - 2 * (bx * bx + bz * bz), 2 * (by * bz - bw * bx),
+                                 2 * (bx * bz - bw * by), 2 * (by * bz + bw * bx), 1 - 2 * (bx * bx + by * by)};
+            const float eb[3] = {expf(sv.x), expf(sv.y), expf(sv.z)};
+            float UM[6];
+#pragma unroll
+            for (int a = 0; a < 2; ++a)
+#pragma unroll
+                for (int j = 0; j < 3; ++j)
+                    UM[a * 3 + j] = (U[a * 3] * Rb[j] + U[a * 3 + 1] * Rb[3 + j] + U[a * 3 + 2] * Rb[6 + j]) * eb[j];
+            const float s00 = UM[0] * UM[0] + UM[1] * UM[1] + UM[2] * UM[2];
+            const float s01 = UM[0] * UM[3] + UM[1] * UM[4] + UM[2] * UM[5];
+            const float s11 = UM[3] * UM[3] + UM[4] * UM[4] + UM[5] * UM[5];
+            const float pcv[3] = {pcx, pcy, pcz};
+            float d0, d1, gd0, gd1;
+            motion_blur_velocity(dj, pcv, blur.motion, d0, d1);
+            const float one_minus_o = 1.0f - __ldg(p.records + 3 * (size_t)o + 1).z;
+            const float g_alpha = one_minus_o != 0.0f ? a2.x / one_minus_o : 0.0f;
+            motion_blur_grad(s00, s01, s11, d0, d1, g_alpha, g00, g01, g11, gd0, gd1);
+            if (BGRAD) {  // g = Jp^T dL/dd: dL/dv = g, dL/dw = pc x g
+                const float q0 = dj[0] * gd0 + dj[3] * gd1, q1 = dj[1] * gd0 + dj[4] * gd1, q2 = dj[2] * gd0 + dj[5] * gd1;
+                mv[0] = q0; mv[1] = q1; mv[2] = q2;
+                mv[3] = pcy * q2 - pcz * q1;
+                mv[4] = pcz * q0 - pcx * q2;
+                mv[5] = pcx * q1 - pcy * q0;
+            }
+        }
         // V = U^T G U  (dL/dSigma with the (g00,g01,g01,g11) weighting of GPCR:716-721)
         float V[9];
 #pragma unroll
@@ -792,7 +835,7 @@ __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, fl
               if (lane == 0) my_lgrad[k] += v;
           }
       }
-      if (MGRAD) {
+      if (CAM6) {
 #pragma unroll
           for (int k = 0; k < RS_GRAD_VALUES; ++k) {
               float v = mv[k];
@@ -859,7 +902,7 @@ __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, fl
             lgrad_partials[(size_t)blockIdx.x * LENS_GRAD_VALUES + threadIdx.x] = s;
         }
     }
-    if (MGRAD) {
+    if (CAM6) {
         __syncthreads();
         if (threadIdx.x < RS_GRAD_VALUES) {
             float s = s_mgrad[threadIdx.x];
@@ -974,8 +1017,22 @@ backward_points_rs_filter_kernel(const PointsBwdRsFilterParams p) {
         p, nullptr, nullptr, 0, nullptr, nullptr, p.lens, nullptr, nullptr, p.rs, nullptr, nullptr, p.filter3d);
 }
 
+// The parameter block of the BLUR instantiations (LENS = false ignores `lens`, RS = false ignores `rs`; rs_partials: the
+// BGRAD rows).
+struct PointsBwdBlurParams : PointsBwdRsParams {
+    BlurParams blur;
+};
+
+template <bool DEPTH, bool LENS, bool RS, bool BGRAD>
+__global__ void __launch_bounds__(GSB_POINTS_THREADS, BGRAD ? 3 : 5)
+backward_points_blur_kernel(const PointsBwdBlurParams p) {
+    __shared__ float s_mgrad[BGRAD ? (GSB_POINTS_THREADS / 32) * RS_GRAD_VALUES : 1];
+    backward_points_body<false, DEPTH, false, false, LENS, false, RS, false, false, true, BGRAD>(
+        p, nullptr, nullptr, 0, nullptr, nullptr, p.lens, nullptr, nullptr, p.rs, s_mgrad, p.rs_partials, nullptr, p.blur);
+}
+
 // One CTA: adds the `blocks` partial rows in a fixed order (strided per thread, then a fixed shared-memory tree) and writes
-// the 6 motion gradients.  Zeros when blocks == 0.
+// the 6 motion gradients (of the rolling shutter or of the exposure).  Zeros when blocks == 0.
 constexpr int RS_GRAD_FINISH_THREADS = 128;
 __global__ void __launch_bounds__(RS_GRAD_FINISH_THREADS)
 rolling_shutter_grad_finish_kernel(const float *__restrict__ partials, int blocks, float *__restrict__ grad_motion) {
@@ -1330,6 +1387,46 @@ int launch_backward_points_rs(const GsbBackwardArgs &a, const Workspace &ws, cud
     if (rs_grad != nullptr) {
         rolling_shutter_grad_finish_kernel<<<1, RS_GRAD_FINISH_THREADS, 0, stream>>>(p.rs_partials, (int)blocks,
                                                                                      rs_grad->grad_motion);
+        GSB_CUDA_CHECK(cudaGetLastError());
+    }
+    return GSB_OK;
+}
+
+template <bool DEPTH, bool LENS, bool RS>
+static void launch_blur_kernel(bool bgrad, int blocks, cudaStream_t stream, const PointsBwdBlurParams &p) {
+    if (bgrad) backward_points_blur_kernel<DEPTH, LENS, RS, true><<<blocks, GSB_POINTS_THREADS, 0, stream>>>(p);
+    else backward_points_blur_kernel<DEPTH, LENS, RS, false><<<blocks, GSB_POINTS_THREADS, 0, stream>>>(p);
+}
+
+// The BLUR per-point kernel on the grid of launch_backward_points_rs (at most GSB_RS_GRAD_PARTIAL_BLOCKS CTAs with blur_grad),
+// then with blur_grad rolling_shutter_grad_finish_kernel.  The caller checked the arguments.
+int launch_backward_points_blur(const GsbBackwardArgs &a, const Workspace &ws, cudaStream_t stream, bool depth_grad,
+                                const LensParams *lens, const RsParams *rs, const BlurParams &blur,
+                                const GsbMotionBlurGradArgs *blur_grad) {
+    PointsBwdBlurParams p;
+    static_cast<PointsBwdParams &>(p) = make_points_params(a, ws, nullptr);
+    p.lens = lens != nullptr ? *lens : LensParams();
+    p.rs = rs != nullptr ? *rs : RsParams();
+    p.rs_partials = blur_grad != nullptr ? static_cast<float *>(blur_grad->temp) : nullptr;
+    p.blur = blur;
+    long long blocks = a.num_points > 0 ? (a.num_points + GSB_POINTS_THREADS - 1) / GSB_POINTS_THREADS : 0;
+    const long long cap = blur_grad != nullptr ? (long long)GSB_RS_GRAD_PARTIAL_BLOCKS : 16LL * num_sms();
+    if (blocks > cap) blocks = cap;
+    if (blocks > 0) {
+        const bool bgrad = blur_grad != nullptr, l = lens != nullptr, r = rs != nullptr;
+        const int g = (int)blocks;
+        if (depth_grad) {
+            if (l) r ? launch_blur_kernel<true, true, true>(bgrad, g, stream, p) : launch_blur_kernel<true, true, false>(bgrad, g, stream, p);
+            else r ? launch_blur_kernel<true, false, true>(bgrad, g, stream, p) : launch_blur_kernel<true, false, false>(bgrad, g, stream, p);
+        } else {
+            if (l) r ? launch_blur_kernel<false, true, true>(bgrad, g, stream, p) : launch_blur_kernel<false, true, false>(bgrad, g, stream, p);
+            else r ? launch_blur_kernel<false, false, true>(bgrad, g, stream, p) : launch_blur_kernel<false, false, false>(bgrad, g, stream, p);
+        }
+        GSB_CUDA_CHECK(cudaGetLastError());
+    }
+    if (blur_grad != nullptr) {
+        rolling_shutter_grad_finish_kernel<<<1, RS_GRAD_FINISH_THREADS, 0, stream>>>(p.rs_partials, (int)blocks,
+                                                                                     blur_grad->grad_motion);
         GSB_CUDA_CHECK(cudaGetLastError());
     }
     return GSB_OK;

@@ -64,11 +64,13 @@ int resolve_workspace(void *base, int64_t bytes, int64_t N, int32_t n_obj, int64
 // ---- stage launchers (each enqueues on `stream`, returns GSB_* code)
 struct LensParams;
 struct RsParams;
+struct BlurParams;
 // lens: the distortion of gsb200_forward_lens (checked there, r2_max set), or NULL for the pinhole kernel; rs: the rolling
 // shutter of gsb200_forward_rolling_shutter (checked there), or NULL; filter3d: the (N,) 3D smoothing filter of
-// gsb200_forward_filter3d (checked there), or NULL
+// gsb200_forward_filter3d (checked there), or NULL; blur: the exposure motion of gsb200_forward_motion_blur (checked there,
+// never together with filter3d), or NULL
 int launch_preprocess(const GsbForwardArgs &a, const Workspace &ws, cudaStream_t stream, const LensParams *lens = nullptr,
-                      const RsParams *rs = nullptr, const float *filter3d = nullptr);
+                      const RsParams *rs = nullptr, const float *filter3d = nullptr, const BlurParams *blur = nullptr);
 // the pose blocks of n (q, t) pairs (pose_kernel without the per-frame clears)
 int launch_pose_blocks(const float *q_pc, const float *t_pc, int n, PoseBlock *poses, cudaStream_t stream);
 int launch_sort(const Workspace &ws, int64_t key_capacity, cudaStream_t stream);
@@ -103,6 +105,12 @@ int launch_backward_points_rs(const GsbBackwardArgs &a, const Workspace &ws, cud
 // gradients as launch_backward_points, skip_flag likewise); arguments checked by the caller
 int launch_backward_points_filter(const GsbBackwardArgs &a, const Workspace &ws, cudaStream_t stream, const long long *skip_flag,
                                   bool depth_grad, const LensParams *lens, const RsParams *rs, const float *filter3d);
+// gsb200_backward_motion_blur: the BLUR per-point kernel (lens: NULL for a pinhole; rs: NULL for a global shutter), with
+// blur_grad also the motion sums (per-CTA rows in blur_grad->temp) and the rolling-shutter finishing kernel; arguments
+// checked by the caller
+int launch_backward_points_blur(const GsbBackwardArgs &a, const Workspace &ws, cudaStream_t stream, bool depth_grad,
+                                const LensParams *lens, const RsParams *rs, const BlurParams &blur,
+                                const GsbMotionBlurGradArgs *blur_grad);
 // gsb200_filter3d_from_views (csrc/filter3d.cu; arguments checked by the caller)
 int launch_filter3d_from_views(const GsbFilter3dViewsArgs &a, cudaStream_t stream);
 // gsb200_backward_pose: the POSE per-point kernel (dense gradients as launch_backward_points, plus the per-CTA pose sums
@@ -468,6 +476,44 @@ __device__ __forceinline__ void rolling_shutter_grad(float tau, const float *w, 
     out[3] = tau * (a0 + sB * c0 + sC * d0);
     out[4] = tau * (a1 + sB * c1 + sC * d1);
     out[5] = tau * (a2 + sB * c2 + sC * d2);
+}
+#endif
+
+// ---- motion blur (gsb200_forward_motion_blur / gsb200_backward_motion_blur; definition in include/gsb200.h)
+struct BlurParams {
+    float motion[6];  // v (3), w (3) over the whole exposure
+};
+#if defined(__CUDACC__) || defined(GSB_HOST_EMU)
+// m != 0.  A view with m = 0 takes the un-blurred arithmetic, so it reproduces the kernels without blur bit for bit.
+__device__ __forceinline__ bool motion_blur_on(const float *m) {
+    return m[0] != 0.0f || m[1] != 0.0f || m[2] != 0.0f || m[3] != 0.0f || m[4] != 0.0f || m[5] != 0.0f;
+}
+// d = Jp (v + w x pc): the screen displacement of the splat centre over the exposure (dj: the full 2x3 position Jacobian
+// d(u, v)/d pc, row-major)
+__device__ __forceinline__ void motion_blur_velocity(const float *dj, const float *pc, const float *m, float &d0, float &d1) {
+    const float u0 = m[0] + (m[4] * pc[2] - m[5] * pc[1]);
+    const float u1 = m[1] + (m[5] * pc[0] - m[3] * pc[2]);
+    const float u2 = m[2] + (m[3] * pc[1] - m[4] * pc[0]);
+    d0 = (dj[0] * u0 + dj[1] * u1) + dj[2] * u2;
+    d1 = (dj[3] * u0 + dj[4] * u1) + dj[5] * u2;
+}
+// The backward of the blur of one in-camera point.  (s00, s01, s11) = Sigma', (d0, d1) = d, g_alpha = G_a; on entry
+// (g00, g01, g11) = G = dL/d(Sigma_d + B), on exit dL/dSigma' = G + G_a/2 (Sigma_d^-1 - (Sigma_d + B)^-1) (the compensation
+// c_b); (gd0, gd1) = dL/dd = G d / 6 - G_a/12 (Sigma_d + B)^-1 d.
+__device__ __forceinline__ void motion_blur_grad(float s00, float s01, float s11, float d0, float d1, float g_alpha, float &g00,
+                                                 float &g01, float &g11, float &gd0, float &gd1) {
+    const float a00 = s00 + 0.3f, a11 = s11 + 0.3f;  // Sigma_d
+    const float b00 = a00 + (d0 * d0) / 12.0f, b01 = s01 + (d0 * d1) / 12.0f, b11 = a11 + (d1 * d1) / 12.0f;  // Sigma_d + B
+    const float ia = 1.0f / (a00 * a11 - s01 * s01), ib = 1.0f / (b00 * b11 - b01 * b01);
+    const float i00 = ib * b11, i01 = -ib * b01, i11 = ib * b00;  // (Sigma_d + B)^-1
+    const float Gd0 = g00 * d0 + g01 * d1, Gd1 = g01 * d0 + g11 * d1;
+    const float Id0 = i00 * d0 + i01 * d1, Id1 = i01 * d0 + i11 * d1;
+    gd0 = Gd0 / 6.0f - (g_alpha / 12.0f) * Id0;
+    gd1 = Gd1 / 6.0f - (g_alpha / 12.0f) * Id1;
+    const float h = 0.5f * g_alpha;
+    g00 += h * (ia * a11 - i00);
+    g01 += h * (-ia * s01 - i01);
+    g11 += h * (ia * a00 - i11);
 }
 #endif
 

@@ -200,9 +200,14 @@ __device__ __forceinline__ bool tile_reachable(const SplatReach &r, float u, flo
 // include/gsb200.h) widens the scales to s^_j = sqrt(exp(s_j)^2 + sigma^2) before Sigma is formed, and the compensation
 // c = sqrt(prod_j exp(s_j)^2 / s^_j^2) is folded into the record's rescale slot (r1.y = rescale c; r1.z keeps the raw
 // opacity), so the blend kernels read rescale * o * c unchanged.  sigma = 0 leaves the row untouched.
-template <typename KeyT, int LENS, bool ROLLING = false, bool FILTER = false>
+// BLUR = true (gsb200_forward_motion_blur): the splat is widened by the exposure motion (definition in include/gsb200.h).
+// d = Jp (v + w x pc) with the full position Jacobian Jp at the rendered pc, B = d d^T / 12; the conic is (Sigma_d + B)^-1,
+// the rescale slot holds rescale c_b with c_b = sqrt(det Sigma_d / det(Sigma_d + B)), and the radius comes from Sigma' + B.
+// A view with m = 0 takes the un-blurred arithmetic.  Not with FILTER.
+template <typename KeyT, int LENS, bool ROLLING = false, bool FILTER = false, bool BLUR = false>
 __device__ __forceinline__ void preprocess_body(const PreParams p, const LensParams lens, const RsParams rs = RsParams(),
-                                                const float *filter3d = nullptr) {
+                                                const float *filter3d = nullptr, const BlurParams blur = BlurParams()) {
+    static_assert(!(BLUR && FILTER), "the motion blur is not implemented with the 3D filter");
     __shared__ unsigned int s_ticket;
     __shared__ unsigned long long s_warp_sums[SCAN_BLOCK_THREADS / 32];
     __shared__ unsigned long long s_block_exclusive;
@@ -376,10 +381,31 @@ __device__ __forceinline__ void preprocess_body(const PreParams p, const LensPar
             const float det_pre = c00 * c11 - c01 * c10;
             c00 += 0.3f;
             c11 += 0.3f;
-            const float det = c00 * c11 - c01 * c10;
+            float det = c00 * c11 - c01 * c10;
             const float rescale = sqrtf(fmaxf(0.0f, det_pre / det));
+            float blur_c = 1.0f;  // BLUR: the compensation c_b
+            const bool blurred = BLUR && motion_blur_on(blur.motion);
+            if (blurred) {
+                // Jp = K[:2,:2] D P, the expression of the backward's d uv / d pc
+                float A0 = Kc[0], A1 = Kc[1], A3 = Kc[3], A4 = Kc[4];
+                if (LENS != GSB_LENS_PINHOLE) {
+                    A0 = Kc[0] * D[0] + Kc[1] * D[2]; A1 = Kc[0] * D[1] + Kc[1] * D[3];
+                    A3 = Kc[3] * D[0] + Kc[4] * D[2]; A4 = Kc[3] * D[1] + Kc[4] * D[3];
+                }
+                const float iz = 1.0f / pc[2], iz2 = iz * iz;
+                const float dj[6] = {A0 * iz, A1 * iz, (-A0 * pc[0] - A1 * pc[1]) * iz2,
+                                     A3 * iz, A4 * iz, (-A3 * pc[0] - A4 * pc[1]) * iz2};
+                float d0, d1;
+                motion_blur_velocity(dj, pc, blur.motion, d0, d1);
+                const float b00 = (d0 * d0) / 12.0f, b01 = (d0 * d1) / 12.0f, b11 = (d1 * d1) / 12.0f;
+                c00 += b00; c01 += b01; c10 += b01; c11 += b11;
+                cov[0] += b00; cov[1] += b01; cov[2] += b01; cov[3] += b11;  // the radius below: Sigma' + B
+                const float det_b = c00 * c11 - c01 * c10;
+                blur_c = sqrtf(det / det_b);  // in (0, 1]: B is positive semi-definite
+                det = det_b;
+            }
             const float inv_det = 1.0f / det;
-            // GPCR:311-315 radius from the un-blurred covariance
+            // GPCR:311-315 radius from the un-blurred covariance (with BLUR: from Sigma' + B)
             const float ca = cov[0], cd = cov[3];
             const float large = (ca + cd + sqrtf((ca - cd) * (ca - cd) + 4.0f * cov[1] * cov[2])) / 2.0f;
             const float radius = sqrtf(large) * 3.0f;
@@ -395,7 +421,7 @@ __device__ __forceinline__ void preprocess_body(const PreParams p, const LensPar
             ntiles = (max_tu - min_tu) * (max_tv - min_tv);
             // reach-test parameters of this splat; the (tile, splat) tests themselves are done cooperatively by
             // the warp below (one lane per PAIR, not per splat)
-            const float rescale_c = FILTER ? rescale * filter_c : rescale;
+            const float rescale_c = FILTER ? rescale * filter_c : blurred ? rescale * blur_c : rescale;
             reach = make_splat_reach(inv_det * c11, inv_det * (-c01), inv_det * c00, rescale_c * opacity);
             if (!p.filter_tiles) reach.mode = 2;
             r0 = make_float4(u, v, inv_det * c11, inv_det * (-c01));
@@ -678,6 +704,17 @@ preprocess_rs_filter_kernel(const PreRsFilterParams p) {
     preprocess_body<KeyT, LENS, true, true>(p, p.lens, p.rs, p.filter3d);
 }
 
+// The parameter block of the BLUR instantiations (LENS = GSB_LENS_PINHOLE ignores `lens`, ROLLING = false ignores `rs`).
+struct PreBlurParams : PreRsParams {
+    BlurParams blur;
+};
+
+template <typename KeyT, int LENS, bool ROLLING>
+__global__ void __launch_bounds__(SCAN_BLOCK_THREADS, GSB_PRE_MIN_BLOCKS)
+preprocess_blur_kernel(const PreBlurParams p) {
+    preprocess_body<KeyT, LENS, ROLLING, false, true>(p, p.lens, p.rs, nullptr, p.blur);
+}
+
 #ifndef GSB_HOST_EMU  // tests/simt compiles the kernels above as host C++ under the SIMT emulator
 // The pose blocks of n (q, t) pairs without clearing anything (gsb200_filter3d_from_views: one per view and object).
 int launch_pose_blocks(const float *q_pc, const float *t_pc, int n, PoseBlock *poses, cudaStream_t stream) {
@@ -704,8 +741,21 @@ static void launch_filter_kernel(int model, bool rolling, dim3 grid, dim3 block,
     else preprocess_filter_kernel<KeyT, GSB_LENS_PINHOLE><<<grid, block, 0, stream>>>(pf);
 }
 
+template <typename KeyT>
+static void launch_blur_kernel(int model, bool rolling, dim3 grid, dim3 block, cudaStream_t stream, const PreBlurParams &pb) {
+    if (rolling) {
+        if (model == GSB_LENS_FISHEYE) preprocess_blur_kernel<KeyT, GSB_LENS_FISHEYE, true><<<grid, block, 0, stream>>>(pb);
+        else if (model == GSB_LENS_OPENCV) preprocess_blur_kernel<KeyT, GSB_LENS_OPENCV, true><<<grid, block, 0, stream>>>(pb);
+        else preprocess_blur_kernel<KeyT, GSB_LENS_PINHOLE, true><<<grid, block, 0, stream>>>(pb);
+    } else {
+        if (model == GSB_LENS_FISHEYE) preprocess_blur_kernel<KeyT, GSB_LENS_FISHEYE, false><<<grid, block, 0, stream>>>(pb);
+        else if (model == GSB_LENS_OPENCV) preprocess_blur_kernel<KeyT, GSB_LENS_OPENCV, false><<<grid, block, 0, stream>>>(pb);
+        else preprocess_blur_kernel<KeyT, GSB_LENS_PINHOLE, false><<<grid, block, 0, stream>>>(pb);
+    }
+}
+
 int launch_preprocess(const GsbForwardArgs &a, const Workspace &ws, cudaStream_t stream, const LensParams *lens,
-                      const RsParams *rs, const float *filter3d) {
+                      const RsParams *rs, const float *filter3d, const BlurParams *blur) {
     const GsbWorkspaceLayout &L = ws.layout;
     {
         // per-frame state to zero: [counters, sort_state) and [tile_start, zero_bytes) -- every offset is 256-B aligned
@@ -750,7 +800,17 @@ int launch_preprocess(const GsbForwardArgs &a, const Workspace &ws, cudaStream_t
     p.point_in_camera = ws.point_in_camera;
     p.keys = ws.keys_a;
     p.vals = ws.vals_a;
-    if (filter3d != nullptr) {
+    if (blur != nullptr) {
+        PreBlurParams pb;
+        static_cast<PreParams &>(pb) = p;
+        pb.lens = lens != nullptr ? *lens : LensParams();
+        pb.rs = rs != nullptr ? *rs : RsParams();
+        pb.blur = *blur;
+        const int model = lens != nullptr ? lens->model : GSB_LENS_PINHOLE;
+        const dim3 grid(L.scan_blocks), block(SCAN_BLOCK_THREADS);
+        if (L.key_bytes == 4) launch_blur_kernel<unsigned int>(model, rs != nullptr, grid, block, stream, pb);
+        else launch_blur_kernel<unsigned long long>(model, rs != nullptr, grid, block, stream, pb);
+    } else if (filter3d != nullptr) {
         PreRsFilterParams pr;
         static_cast<PreParams &>(pr) = p;
         pr.lens = lens != nullptr ? *lens : LensParams();

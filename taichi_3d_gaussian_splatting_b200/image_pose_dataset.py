@@ -28,6 +28,10 @@ An optional record key ``rolling_shutter`` (an extension), ``{"linear_velocity":
 "readout_time": s}``, gives the view's ``CameraInfo.rolling_shutter`` (``Camera.RollingShutter.from_camera_velocity``: the
 camera's own velocities in its frame, in scene units/s and rad/s, as visual-inertial odometry reports them, and the sensor's
 top-to-bottom readout time).  Row time is normalised by the image height, so rescaling and autoscale keep the motion.
+An optional record key ``motion_blur`` (an extension), ``{"linear_velocity": [3], "angular_velocity": [3],
+"exposure_time": s}``, gives the view's ``CameraInfo.motion_blur`` (``Camera.MotionBlur.from_camera_velocity``: the camera's
+own velocities as for ``rolling_shutter``, and the time the shutter was open).  The motion is in the camera frame, so
+rescaling and autoscale keep it.
 Pinned against the reference class itself: ``tests/golden/make_dataset_golden.py`` imports it (Taichi stubbed) and
 stores its outputs for a small generated dataset; ``tests/test_dataset_cpu.py`` compares.
 """
@@ -39,7 +43,7 @@ import numpy as np
 import torch
 import torch.utils.data
 
-from .Camera import CameraInfo, LensDistortion, RollingShutter
+from .Camera import CameraInfo, LensDistortion, MotionBlur, RollingShutter
 from .GaussianPointCloudRasterisation import TILE_HEIGHT, TILE_WIDTH
 from .loss import SupervisionTargets
 from .utils import SE3_to_quaternion_and_translation_torch
@@ -94,7 +98,7 @@ class ImagePoseDataset(torch.utils.data.Dataset):
         K[1, 2] *= sy
         return resized, CameraInfo(camera_intrinsics=K, camera_height=resized.shape[1], camera_width=resized.shape[2],
                                    camera_id=camera_info.camera_id, distortion=camera_info.distortion,
-                                   rolling_shutter=camera_info.rolling_shutter)
+                                   rolling_shutter=camera_info.rolling_shutter, motion_blur=camera_info.motion_blur)
 
     @staticmethod
     def _distortion(rec: dict) -> Optional[LensDistortion]:
@@ -119,6 +123,20 @@ class ImagePoseDataset(torch.utils.data.Dataset):
         if len(r["linear_velocity"]) != 3 or len(r["angular_velocity"]) != 3:
             raise ValueError(f'"rolling_shutter" velocities take 3 values each, got {r!r}')
         return RollingShutter.from_camera_velocity(r["linear_velocity"], r["angular_velocity"], r["readout_time"])
+
+    @staticmethod
+    def _motion_blur(rec: dict) -> Optional[MotionBlur]:
+        """The optional record key ``"motion_blur": {"linear_velocity": [3], "angular_velocity": [3], "exposure_time": s}``."""
+        r = rec.get("motion_blur")
+        if r is None:
+            return None
+        keys = ("linear_velocity", "angular_velocity", "exposure_time")
+        if not isinstance(r, dict) or any(k not in r for k in keys):
+            raise ValueError(f'"motion_blur" must be {{"linear_velocity": [3], "angular_velocity": [3], "exposure_time": s}}, '
+                             f'got {r!r}')
+        if len(r["linear_velocity"]) != 3 or len(r["angular_velocity"]) != 3:
+            raise ValueError(f'"motion_blur" velocities take 3 values each, got {r!r}')
+        return MotionBlur.from_camera_velocity(r["linear_velocity"], r["angular_velocity"], r["exposure_time"])
 
     def _path(self, path: str) -> str:
         if not os.path.isabs(path) and not os.path.exists(path):
@@ -220,7 +238,7 @@ class ImagePoseDataset(torch.utils.data.Dataset):
         image = _crop_to_tiles(image)
         info = CameraInfo(camera_intrinsics=K, camera_height=image.shape[1], camera_width=image.shape[2],
                           camera_id=rec["camera_id"], distortion=self._distortion(rec),
-                          rolling_shutter=self._rolling_shutter(rec))
+                          rolling_shutter=self._rolling_shutter(rec), motion_blur=self._motion_blur(rec))
         image, info = self._autoscale_image_and_camera_info(image, info)
         if self.with_targets:
             return image, q, t, info, self._crop_and_scale_targets(*targets, info)

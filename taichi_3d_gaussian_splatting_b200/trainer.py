@@ -28,6 +28,13 @@ Views with a rolling shutter (an extension; ``CameraInfo.rolling_shutter``) trai
 downsampled camera keeps the motion (row time is normalised by the image height).  Not with ``fused_step``, pose, intrinsics
 or lens refinement.  Optional motion refinement (``TrainConfig.rolling_shutter_learning_rate``): per rolling-shutter view, its
 motion (v, w), differentiated by the operator's ``differentiable_rolling_shutter`` and stepped by its own Adam.
+Views with motion blur (an extension; ``CameraInfo.motion_blur``) train through it in the autograd loop, with or without a
+rolling shutter; the downsampled camera keeps the exposure motion (it is in the camera frame).  Not with ``fused_step``,
+``mip_filter_3d``, pose, intrinsics, lens or rolling-shutter motion refinement, or the view-parallel exchange.  Optional
+exposure-motion refinement (``TrainConfig.motion_blur_learning_rate``): per blurred view, its exposure motion (v, w),
+differentiated by the operator's ``differentiable_motion_blur`` and stepped by its own Adam; it needs a non-zero start (the
+gradient vanishes at zero motion), e.g. ``Camera.MotionBlur.between_poses`` of the neighbouring frames.  ``validation``
+renders every view as its camera says: blurred views blurred.
 Optional appearance compensation (an extension; ``TrainConfig.appearance_grid``): one bilateral grid per training view
 (``appearance.apply_bilateral_grid``), initialised to the identity, slices the image the image loss sees (after the
 background composite), with a TV prior and its own Adam that steps only the visited view's grid.  It acts on the image alone,
@@ -54,7 +61,7 @@ import torch
 import torch.nn.functional as F
 
 from .appearance import apply_bilateral_grid, bilateral_grid_tv, check_grid_shape, identity_grids
-from .Camera import CameraInfo, LensDistortion, RollingShutter
+from .Camera import CameraInfo, LensDistortion, MotionBlur, RollingShutter
 from .densification import GaussianPointAdaptiveController
 from .GaussianPointCloudRasterisation import GaussianPointCloudRasterisation
 from .loss import (FEATURE_LOSSES, LossFunction, RobustLossConfig, SupervisionTargets, feature_loss, mcmc_regulariser,
@@ -86,10 +93,11 @@ def downsample_image_and_camera_info(image: torch.Tensor, camera_info: CameraInf
     K[1, 1] /= downsample_factor
     K[0, 2] /= downsample_factor
     K[1, 2] /= downsample_factor
-    # the lens coefficients act on the normalised image plane and row time is normalised by the height: resizing changes
-    # neither the lens nor the rolling-shutter motion
+    # the lens coefficients act on the normalised image plane, row time is normalised by the height and the exposure motion
+    # is in the camera frame: resizing changes neither the lens, the rolling-shutter motion nor the exposure motion
     return image, CameraInfo(camera_intrinsics=K, camera_height=h, camera_width=w, camera_id=camera_info.camera_id,
-                             distortion=camera_info.distortion, rolling_shutter=camera_info.rolling_shutter)
+                             distortion=camera_info.distortion, rolling_shutter=camera_info.rolling_shutter,
+                             motion_blur=camera_info.motion_blur)
 
 
 def _nearest(x: torch.Tensor, h: int, w: int, hc: int, wc: int) -> torch.Tensor:
@@ -182,6 +190,11 @@ class GaussianPointCloudTrainer:
         # (6,) leaf tensor of its motion (v, w), initialised from the view's, kept on the host and trained by its own Adam at
         # this rate.  Not with fused_step, pose, intrinsics or lens refinement (no rolling-shutter view combines with them).
         rolling_shutter_learning_rate: float = 0.
+        # optional exposure-motion refinement: > 0 gives every training view with motion blur (CameraInfo.motion_blur) one
+        # (6,) leaf tensor of its exposure motion (v, w), initialised from the view's, kept on the host and trained by its own
+        # Adam at this rate.  The start must not be zero (the blur's gradient vanishes there).  Not with fused_step,
+        # mip_filter_3d, pose, intrinsics, lens or rolling-shutter motion refinement.
+        motion_blur_learning_rate: float = 0.
         # optional appearance compensation: (Gx, Gy, Gz) gives every training view one bilateral grid of that many nodes
         # (1 <= Gx, Gy <= 64, 1 <= Gz <= 16; (1, 1, 1) is a per-view affine colour transform), initialised to the identity
         # and trained by its own Adam at appearance_learning_rate with a TV prior of weight appearance_tv_weight.  The
@@ -285,6 +298,18 @@ class GaussianPointCloudTrainer:
                     raise ValueError(f"{name} is not supported with a rolling-shutter view (CameraInfo.rolling_shutter)")
         self._rolling_shutter = self._rolling_shutter_leaves(config, train_views)
         self._rs = config.rolling_shutter_learning_rate > 0
+        # a view with motion blur (CameraInfo.motion_blur) trains through the autograd loop alone
+        self._blurred = any(getattr(v[3], "motion_blur", None) is not None for v in train_views)
+        if self._blurred:
+            for name, on in (("fused_step", fused_step), ("mip_filter_3d", bool(config.mip_filter_3d)),
+                             ("pose refinement (pose_learning_rate > 0)", self._pose),
+                             ("intrinsics refinement (intrinsics_learning_rate > 0)", self._intr),
+                             ("distortion refinement (distortion_learning_rate > 0)", self._dist),
+                             ("motion refinement (rolling_shutter_learning_rate > 0)", self._rs)):
+                if on:
+                    raise ValueError(f"{name} is not supported with a motion-blurred view (CameraInfo.motion_blur)")
+        self._motion_blur = self._motion_blur_leaves(config, train_views)
+        self._mb = config.motion_blur_learning_rate > 0
         self._mip = bool(config.mip_filter_3d)
         self._filter_3d = None
         if self._mip:
@@ -361,12 +386,16 @@ class GaussianPointCloudTrainer:
                      **({"differentiable_pose": True} if self._pose else {}),
                      **({"differentiable_intrinsics": True} if self._intr else {}),
                      **({"differentiable_distortion": True} if self._dist else {}),
-                     **({"differentiable_rolling_shutter": True} if self._rs else {}))
+                     **({"differentiable_rolling_shutter": True} if self._rs else {}),
+                     **({"differentiable_motion_blur": True} if self._mb else {}))
         self.rasterisation = factory(config=config.rasterisation_config,
                                      backward_valid_point_hook=None if self._mcmc else self.adaptive_controller.update,
                                      **extra)
         if self._mcmc and getattr(self.rasterisation, "gradient_exchange", None) is not None:
             raise ValueError('densification="mcmc" is not implemented for the view-parallel gradient exchange')
+        if self._blurred and getattr(self.rasterisation, "gradient_exchange", None) is not None:
+            raise ValueError("a motion-blurred view (CameraInfo.motion_blur) is not supported with the view-parallel "
+                             "gradient exchange")
         if self._mip and getattr(self.rasterisation, "gradient_exchange", None) is not None:
             raise ValueError("mip_filter_3d is not implemented for the view-parallel gradient exchange")
         if self._weighted and getattr(self.rasterisation, "gradient_exchange", None) is not None:
@@ -413,6 +442,21 @@ class GaussianPointCloudTrainer:
         if not leaves:
             raise ValueError("rolling_shutter_learning_rate > 0 needs a rolling-shutter training view "
                              "(CameraInfo.rolling_shutter)")
+        return leaves
+
+    @staticmethod
+    def _motion_blur_leaves(config, train_views: List[View]) -> dict:
+        """The trainable exposure motions, one float32 host leaf (6,) per blurred view, keyed by view index ({} when
+        exposure-motion refinement is off)."""
+        rate = config.motion_blur_learning_rate
+        if not (rate >= 0.0 and rate < float("inf")):
+            raise ValueError(f"motion_blur_learning_rate must be finite and >= 0, got {rate}")
+        if rate == 0:
+            return {}
+        leaves = {i: torch.tensor(v[3].motion_blur.motion, dtype=torch.float32, requires_grad=True)
+                  for i, v in enumerate(train_views) if getattr(v[3], "motion_blur", None) is not None}
+        if not leaves:
+            raise ValueError("motion_blur_learning_rate > 0 needs a motion-blurred training view (CameraInfo.motion_blur)")
         return leaves
 
     @staticmethod
@@ -632,6 +676,8 @@ class GaussianPointCloudTrainer:
         rolling_shutter_optimizer = torch.optim.Adam(list(self._rolling_shutter.values()),
                                                      lr=cfg.rolling_shutter_learning_rate, betas=(0.9, 0.999)) \
             if self._rs else None
+        motion_blur_optimizer = torch.optim.Adam(list(self._motion_blur.values()), lr=cfg.motion_blur_learning_rate,
+                                                 betas=(0.9, 0.999)) if self._mb else None
         appearance_optimizer = Adam(self._appearance_leaves, lr=cfg.appearance_learning_rate, betas=(0.9, 0.999)) \
             if self._appearance else None
         scheduler = torch.optim.lr_scheduler.ExponentialLR(position_optimizer, gamma=cfg.position_learning_rate_decay_rate)
@@ -653,6 +699,8 @@ class GaussianPointCloudTrainer:
                 distortion_optimizer.zero_grad()
             if rolling_shutter_optimizer is not None:
                 rolling_shutter_optimizer.zero_grad()
+            if motion_blur_optimizer is not None:
+                motion_blur_optimizer.zero_grad()
             if appearance_optimizer is not None:
                 appearance_optimizer.zero_grad()
             view_index = self._next_view_index(iteration)
@@ -677,6 +725,15 @@ class GaussianPointCloudTrainer:
                                          camera_id=camera_info.camera_id, distortion=camera_info.distortion,
                                          rolling_shutter=RollingShutter(values[:3], values[3:]))
                 lens_kw = {"rolling_shutter_motion": leaf}
+            if self._mb and view_index in self._motion_blur:  # the exposure motion as trained, the leaf as the autograd input
+                leaf = self._motion_blur[view_index]
+                values = leaf.detach().tolist()
+                camera_info = CameraInfo(camera_intrinsics=camera_info.camera_intrinsics,
+                                         camera_height=camera_info.camera_height, camera_width=camera_info.camera_width,
+                                         camera_id=camera_info.camera_id, distortion=camera_info.distortion,
+                                         rolling_shutter=camera_info.rolling_shutter,
+                                         motion_blur=MotionBlur(values[:3], values[3:]))
+                lens_kw = {"exposure_motion": leaf}
             band = iteration // cfg.increase_color_max_sh_band_interval
             if self.supervised or self._features or self._appearance or self._weighted:
                 robust_active = cfg.robust_loss is not None and iteration >= cfg.robust_loss.start_iteration
@@ -715,6 +772,8 @@ class GaussianPointCloudTrainer:
                 distortion_optimizer.step()
             if rolling_shutter_optimizer is not None:
                 rolling_shutter_optimizer.step()
+            if motion_blur_optimizer is not None:
+                motion_blur_optimizer.step()
             if appearance_optimizer is not None:
                 appearance_optimizer.step()
             if self._mcmc:  # the noise of iteration t at the position learning rate its optimiser step used
@@ -840,6 +899,18 @@ class GaussianPointCloudTrainer:
                 values = self._rolling_shutter[i].detach().tolist()
                 rs = RollingShutter(values[:3], values[3:])
             out.append(rs)
+        return out
+
+    def refined_motion_blur(self) -> List[Optional[MotionBlur]]:
+        """The motion blur of every training view as trained (None for a view without one; the views' own exposure motions
+        without exposure-motion refinement)."""
+        out = []
+        for i, v in enumerate(self.train_views):
+            mb = getattr(v[3], "motion_blur", None)
+            if mb is not None and i in self._motion_blur:
+                values = self._motion_blur[i].detach().tolist()
+                mb = MotionBlur(values[:3], values[3:])
+            out.append(mb)
         return out
 
     @torch.no_grad()
