@@ -523,6 +523,56 @@ int gsb200_backward_motion_blur(const GsbBackwardArgs *args, const float *grad_r
                                 const GsbLensArgs *lens, const GsbRollingShutterArgs *rs, const GsbMotionBlurArgs *blur,
                                 const GsbMotionBlurGradArgs *blur_grad);  /* lens, rs, blur, blur_grad or NULL */
 
+/* Depth of field (an extension: the reference renders through an ideal pinhole).  A view may carry a thin lens (a, rho)
+ * (float32 x 2): a the aperture diameter in scene units, rho = 1 / focus distance in 1/scene units (0: focused at infinity).
+ * Both live on the normalised image plane, so downsampling, crop and autoscale leave them unchanged.  With pc the rendered
+ * camera-frame point (pc(tau_3) with a rolling shutter), z = pc.z and M = K[:2,:2] (K[:2,:2] D with a lens, the 2x2 factor of
+ * Jp above):
+ *   beta = a^2 (rho - 1/z)^2 / 16        the per-axis variance of a uniform disk of diameter a |rho - 1/z| on the normalised plane
+ *   B_d = beta M M^T,  B = B_m + B_d     (B_m the motion blur's d d^T / 12 when the view also has one, else 0)
+ * and the conic, rescale slot (c_b), radius, tile square and reach test follow from Sigma_d + B as for the motion blur.  The
+ * model is exact at the level of the covariance: an aperture sample s moves the camera centre by s and, to keep the focal
+ * plane fixed, the principal point by M s rho, so a point moves by M s (rho - 1/z) and its covariance over the disk is B_d.
+ * The blur diameter in pixels is a f_px |rho - 1/z|.  It approximates the disk by a Gaussian of equal variance, composites
+ * defocused splats instead of averaging composited frames (no partial occlusion at depth edges) and, with a lens, maps the
+ * disk through the lens Jacobian at the point.  a = 0 takes the arithmetic without defocus: records, keys, images and every
+ * gradient are those of gsb200_forward_motion_blur / gsb200_backward_motion_blur, bit for bit.
+ * Only |a| is observable, and both parameter gradients vanish at a = 0: refinement needs a non-zero start.  rho is
+ * identifiable only from a view spanning a range of depths: points in front of and behind the focal plane blur alike.
+ * Gradients: beta is detached with respect to the point (like J and d).  With G and G_a as for the motion blur:
+ *   G_B = G - G_a/2 (Sigma_d + B)^-1,   dL/dbeta = <G_B, M M^T>
+ *   dL/da = sum_i dL/dbeta_i a (rho - 1/z_i)^2 / 8,   dL/drho = sum_i dL/dbeta_i a^2 (rho - 1/z_i) / 8
+ * over every in-camera point (GsbDefocusGradArgs), deterministic as the motion blur's: the per-CTA rows in `temp` and the
+ * block-order finishing kernel.  dL/dSigma' has the motion blur's form with this B.  Not implemented with the 3D filter,
+ * camera-parameter gradients (pose, intrinsics, lens coefficients, rolling-shutter or exposure motion) or the compact rows of
+ * the view-parallel exchange. */
+typedef struct GsbDefocusArgs {
+    float aperture;       /* a, scene units */
+    float inverse_focus;  /* rho = 1 / focus distance */
+} GsbDefocusArgs;
+typedef struct GsbDefocusGradArgs {
+    float *grad; /* (2,) out, dL/da, dL/drho */
+    void *temp;  /* gsb200_defocus_grad_temp_bytes() bytes, 16-byte aligned */
+} GsbDefocusGradArgs;
+/* (GSB_RS_GRAD_PARTIAL_BLOCKS + 1) * 6 floats: the per-CTA rows and the finished row */
+int64_t gsb200_defocus_grad_temp_bytes(void);
+/* sizeof(GsbDefocusArgs), sizeof(GsbDefocusGradArgs) (a call of their own, like gsb200_abi_sizes_motion_blur) */
+void gsb200_abi_sizes_defocus(int64_t *out2);
+/* gsb200_forward_motion_blur with the thin lens of `defocus`.  NULL defocus: exactly gsb200_forward_motion_blur.  Before any
+ * CUDA call: the checks of gsb200_forward_motion_blur; GSB_EINVAL for a non-finite a or rho. */
+int gsb200_forward_defocus(const GsbForwardArgs *args, const GsbExtraFeatureArgs *ext, const GsbLensArgs *lens,
+                           const GsbRollingShutterArgs *rs, const GsbMotionBlurArgs *blur,
+                           const GsbDefocusArgs *defocus);  /* lens, rs, blur, defocus or NULL */
+/* gsb200_backward_motion_blur (without the exposure-motion gradient) of a frame rendered by gsb200_forward_defocus with the
+ * same lens, rs, blur and defocus.  NULL defocus: exactly gsb200_backward_motion_blur(..., blur, NULL).  NULL defocus_grad: no
+ * (a, rho) gradient; every other output is bit-identical to the call with defocus_grad.  Before any CUDA call: the checks of
+ * gsb200_forward_defocus; GSB_EINVAL for a defocus_grad without defocus, a NULL output or temp pointer, an output that is not
+ * 4-byte aligned or a temp that is not 16-byte aligned; GSB_EUNSUPPORTED for GSB_FLAG_COMPACT_GRADS. */
+int gsb200_backward_defocus(const GsbBackwardArgs *args, const float *grad_rasterized_depth, const float *rasterized_depth,
+                            const float *grad_pixel_accumulated_alpha, const GsbExtraFeatureArgs *ext, const GsbLensArgs *lens,
+                            const GsbRollingShutterArgs *rs, const GsbMotionBlurArgs *blur, const GsbDefocusArgs *defocus,
+                            const GsbDefocusGradArgs *defocus_grad);  /* lens, rs, blur, defocus, defocus_grad or NULL */
+
 int gsb200_expand_view_gradients(const GsbExpandArgs *args);
 
 /* The two collectives of the compact exchange as ONE hand-written kernel over NVSwitch multicast memory (NVLS; csrc/exchange.cu):

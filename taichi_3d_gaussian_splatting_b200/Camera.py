@@ -5,7 +5,8 @@ argument of ``GaussianPointCloudRasterisationInput``; ``CameraView`` is imported
 GaussianPointCloudRasterisation.py:4).  ``LensDistortion`` and ``CameraInfo.distortion`` are an extension: the reference
 projects through a pinhole only.  ``RollingShutter`` and ``CameraInfo.rolling_shutter`` are an extension as well: the reference
 projects every row with one global-shutter pose.  So are ``MotionBlur`` and ``CameraInfo.motion_blur``: the reference renders every
-view as if the shutter were instantaneous.
+view as if the shutter were instantaneous; and ``Defocus`` and ``CameraInfo.defocus``: the reference renders through an ideal
+pinhole, sharp at every depth.
 """
 import math
 from dataclasses import dataclass
@@ -171,6 +172,45 @@ class MotionBlur:
         return self.linear + self.angular
 
 
+@dataclass(frozen=True)
+class Defocus:
+    """The thin lens of a view with depth of field (definition in ``include/gsb200.h``), as host floats: ``aperture`` = a, the
+    aperture (entrance pupil) diameter in scene units, and ``focus_distance`` in scene units (``math.inf``: focused at
+    infinity).  A point at depth z is blurred to a disk of a f_px |1/focus_distance - 1/z| pixels.  Both values live on the
+    normalised image plane, so downsampling, crop and autoscale keep them.
+
+    Two properties of the model: only |a| is observable, and both parameter gradients vanish at a = 0, so refining them needs a
+    non-zero start; the focus distance is identifiable only from a view that spans a range of depths (points in front of and
+    behind the focal plane blur alike)."""
+    aperture: float
+    focus_distance: float = math.inf
+
+    def __post_init__(self):
+        a, d = float(self.aperture), float(self.focus_distance)
+        if not (math.isfinite(a) and a >= 0.0):
+            raise ValueError(f"defocus aperture must be finite and >= 0, got {self.aperture}")
+        if not (d > 0.0):  # inf allowed, NaN refused
+            raise ValueError(f"defocus focus_distance must be > 0 (inf allowed), got {self.focus_distance}")
+        object.__setattr__(self, "aperture", a)
+        object.__setattr__(self, "focus_distance", d)
+
+    @staticmethod
+    def from_lens(focal_length_mm: float, f_number: float, focus_distance: float, units_per_metre: float) -> "Defocus":
+        """The thin lens of a photo's EXIF values: the focal length in mm, the f-number N and the focus (subject) distance in
+        metres (``math.inf`` for infinity), for a scene ``units_per_metre`` scene units to the metre.  The entrance pupil's
+        diameter is f / N."""
+        f, n, d, u = float(focal_length_mm), float(f_number), float(focus_distance), float(units_per_metre)
+        for name, v in (("focal_length_mm", f), ("f_number", n), ("units_per_metre", u)):
+            if not (math.isfinite(v) and v > 0.0):
+                raise ValueError(f"{name} must be finite and > 0, got {v}")
+        return Defocus((f / 1000.0) / n * u, d * u)
+
+    @property
+    def parameters(self) -> Tuple[float, float]:
+        """(a, rho) with rho = 1 / focus distance, the order of ``GsbDefocusArgs``."""
+        return self.aperture, 1.0 / self.focus_distance
+
+
 @dataclass
 class CameraInfo:
     camera_intrinsics: torch.Tensor  # 3x3 f32 pinhole matrix (device tensor in the reference)
@@ -180,6 +220,7 @@ class CameraInfo:
     distortion: Optional[LensDistortion] = None  # extension: None is the reference's pinhole
     rolling_shutter: Optional[RollingShutter] = None  # extension: None is the reference's global shutter
     motion_blur: Optional[MotionBlur] = None  # extension: None is the reference's instantaneous exposure
+    defocus: Optional[Defocus] = None  # extension: None is the reference's pinhole, sharp at every depth
 
 
 @dataclass

@@ -243,6 +243,7 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
         differentiable_distortion: bool = False,
         differentiable_rolling_shutter: bool = False,
         differentiable_motion_blur: bool = False,
+        differentiable_defocus: bool = False,
     ):
         """``exact_exp``: blend kernels use ``expf`` instead of ``ex2.approx`` (parity debugging).
         ``force_key64``: sort the reference's 64-bit ``tile << 32 | depth`` keys even when the live
@@ -314,7 +315,13 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
         motion of a blurred view from a non-zero start (the gradient vanishes at zero motion).  d is detached; the gradient
         flows through B = d d^T / 12 and the compensation c_b (``gsb200_backward_motion_blur``, definition in
         ``include/gsb200.h``) and includes every loss term the backward takes (image, depth, alpha, features).  An image-only
-        loss works with either backward kernel.  ``ValueError`` with ``config.rgb_only`` or a ``gradient_exchange``."""
+        loss works with either backward kernel.  ``ValueError`` with ``config.rgb_only`` or a ``gradient_exchange``.
+        ``differentiable_defocus``: ``forward`` takes ``defocus_parameters``, the values (a, rho) of ``camera_info.defocus``
+        as an input of the autograd graph, and ``backward`` returns their gradient -- to refine the aperture and focus
+        distance of a defocused view from a non-zero aperture (both gradients vanish at a = 0).  beta is detached with respect
+        to the point; the gradient flows through B_d = beta M M^T and the compensation c_b (``gsb200_backward_defocus``,
+        definition in ``include/gsb200.h``) and includes every loss term the backward takes (image, depth, alpha, features).
+        ``ValueError`` with ``config.rgb_only`` or a ``gradient_exchange``."""
         super().__init__()
         for name, on in (("differentiable_depth", differentiable_depth), ("differentiable_alpha", differentiable_alpha)):
             if on and backward_impl == "butterfly":
@@ -349,6 +356,11 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
         if differentiable_motion_blur and gradient_exchange is not None:
             raise ValueError("differentiable_motion_blur is not supported with a gradient_exchange (view-parallel training)")
         self.differentiable_motion_blur = bool(differentiable_motion_blur)
+        if differentiable_defocus and config.rgb_only:
+            raise ValueError("differentiable_defocus needs the auxiliary outputs: config.rgb_only=True renders none")
+        if differentiable_defocus and gradient_exchange is not None:
+            raise ValueError("differentiable_defocus is not supported with a gradient_exchange (view-parallel training)")
+        self.differentiable_defocus = bool(differentiable_defocus)
         self.config = config
         self.backward_valid_point_hook = backward_valid_point_hook
         self._flags = (_lib.GSB_FLAG_EXACT_EXP if exact_exp else 0) | (_lib.GSB_FLAG_FORCE_KEY64 if force_key64 else 0) | \
@@ -374,16 +386,16 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
             def forward(ctx, pointcloud, pointcloud_features, point_invalid_mask, point_object_id,
                         q_pointcloud_camera, t_pointcloud_camera, camera_info, color_max_sh_band, extra_features=None,
                         camera_intrinsics=None, lens_coefficients=None, rolling_shutter_motion=None, point_filter_3d=None,
-                        exposure_motion=None):
+                        exposure_motion=None, defocus_parameters=None):
                 # camera_intrinsics (differentiable_intrinsics): camera_info.camera_intrinsics itself, passed again only so
                 # that autograd tracks it; lens_coefficients (differentiable_distortion): the coefficients rendered;
                 # rolling_shutter_motion (differentiable_rolling_shutter): the motion rendered; point_filter_3d: the 3D
                 # smoothing filter (never differentiated); exposure_motion (differentiable_motion_blur): the exposure motion
-                # rendered
+                # rendered; defocus_parameters (differentiable_defocus): the (a, rho) rendered
                 outs, frame, saved = outer._run_forward(
                     pointcloud, pointcloud_features, point_invalid_mask, point_object_id,
                     q_pointcloud_camera, t_pointcloud_camera, camera_info, extra_features, lens_coefficients,
-                    rolling_shutter_motion, point_filter_3d, exposure_motion)
+                    rolling_shutter_motion, point_filter_3d, exposure_motion, defocus_parameters)
                 ctx.filter_3d = point_filter_3d  # read by the backward of this frame (the forward's array)
                 image, depth, acc_alpha, last_effective, valid_count = outs[:5]
                 ctx.save_for_backward(pointcloud, pointcloud_features, point_object_id,
@@ -401,6 +413,10 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                 ctx.blur_input = exposure_motion is not None
                 if ctx.blur_input:
                     ctx.blur_device = exposure_motion.device
+                ctx.defocus = saved["defocus"]  # GsbDefocusArgs or None
+                ctx.defocus_input = defocus_parameters is not None
+                if ctx.defocus_input:
+                    ctx.defocus_device = defocus_parameters.device
                 ctx.num_objects = q_pointcloud_camera.shape[0]
                 ctx.color_max_sh_band = color_max_sh_band
                 ctx.has_extra_features = extra_features is not None
@@ -422,6 +438,9 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
             @staticmethod
             def backward(ctx, *grads):
                 result = _module_function._grads(ctx, *grads)
+                if ctx.defocus_input:  # fifteen inputs: the slots before (a, rho) get no gradient here
+                    result, grad_d = result
+                    return tuple(result) + (None,) * (14 - len(result)) + (grad_d,)
                 if ctx.blur_input:  # fourteen inputs: the slots before the exposure motion get no gradient here
                     result, grad_b = result
                     return tuple(result) + (None,) * (13 - len(result)) + (grad_b,)
@@ -440,11 +459,12 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                 lens_grad = ctx.lens_input and ctx.needs_input_grad[10]
                 motion_grad = ctx.motion_input and ctx.needs_input_grad[11]
                 blur_grad = ctx.blur_input and ctx.needs_input_grad[13]
-                grad_K = grad_k = grad_m = grad_b = None
+                defocus_grad = ctx.defocus_input and ctx.needs_input_grad[14]
+                grad_K = grad_k = grad_m = grad_b = grad_d = None
                 # GPCR:1028; with extra features (or pose / intrinsics gradients) the backward also runs for them alone
                 # (frozen scene)
                 if ctx.needs_input_grad[0] or ctx.needs_input_grad[1] or (ctx.has_extra_features and ctx.needs_input_grad[8]) \
-                        or pose or intrinsics or lens_grad or motion_grad or blur_grad:
+                        or pose or intrinsics or lens_grad or motion_grad or blur_grad or defocus_grad:
                     if outer.config.rgb_only:
                         # the reference leaves accumulated alpha / last-effective offsets uninitialised in
                         # this mode (GPCR:478-484), so its backward is undefined; refuse instead
@@ -455,9 +475,14 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                         grad_rasterized_image = torch.zeros((frame.height, frame.width, 3), dtype=torch.float32,
                                                             device=frame.ws.device)
                     grad_pointcloud, grad_pointcloud_features, grad_extra_features, grad_q, grad_t, grad_K, grad_k, grad_m, \
-                        grad_b = outer._run_backward(ctx, grad_rasterized_image, grad_rasterized_depth,
-                                                     grad_pixel_accumulated_alpha, grad_feature_map, pose, intrinsics,
-                                                     lens_grad, motion_grad, blur_grad)
+                        grad_b, grad_d = outer._run_backward(ctx, grad_rasterized_image, grad_rasterized_depth,
+                                                             grad_pixel_accumulated_alpha, grad_feature_map, pose, intrinsics,
+                                                             lens_grad, motion_grad, blur_grad, defocus_grad)
+                if ctx.defocus_input:  # (a, rho)'s gradient goes back beside the leading slots (see backward)
+                    return ((grad_pointcloud if ctx.needs_input_grad[0] else None,
+                             grad_pointcloud_features if ctx.needs_input_grad[1] else None, None, None, None, None, None, None,
+                             grad_extra_features if ctx.has_extra_features and ctx.needs_input_grad[8] else None),
+                            grad_d if defocus_grad else None)
                 if ctx.blur_input:  # the exposure motion's gradient goes back beside the leading slots (see backward)
                     return ((grad_pointcloud if ctx.needs_input_grad[0] else None,
                              grad_pointcloud_features if ctx.needs_input_grad[1] else None, None, None, None, None, None, None,
@@ -557,12 +582,13 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
 
     def _run_forward(self, pointcloud, pointcloud_features, point_invalid_mask, point_object_id,
                      q_pointcloud_camera, t_pointcloud_camera, camera_info, extra_features=None, lens_coefficients=None,
-                     rolling_shutter_motion=None, point_filter_3d=None, exposure_motion=None):
+                     rolling_shutter_motion=None, point_filter_3d=None, exposure_motion=None, defocus_parameters=None):
         cfg = self.config
         lib = _lib.load()
         lens = self._lens_args(camera_info, lens_coefficients)
         rs = self._rolling_shutter_args(camera_info, rolling_shutter_motion)
         blur = self._motion_blur_args(camera_info, exposure_motion, rolling_shutter_motion, point_filter_3d)
+        defocus = self._defocus_args(camera_info, defocus_parameters, rolling_shutter_motion, point_filter_3d, exposure_motion)
         _require(pointcloud, "point_cloud", torch.float32, (3,))
         _require(pointcloud_features, "point_cloud_features", torch.float32, (56,))
         _require(point_invalid_mask, "point_invalid_mask", torch.int8)
@@ -630,7 +656,12 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                         host_counters=pinned.data_ptr(), host_counters_event=event.cuda_event)
                     # The whole frame is enqueued by this one call; the library copies {M, K, overflow} to pinned
                     # host memory right after the per-point stage and records `event` behind that copy.
-                    if blur is not None:
+                    if defocus is not None:
+                        _lib.check(lib.gsb200_forward_defocus(
+                            ctypes.byref(args), ctypes.byref(ext) if ext is not None else None,
+                            ctypes.byref(lens) if lens is not None else None, ctypes.byref(rs) if rs is not None else None,
+                            ctypes.byref(blur) if blur is not None else None, ctypes.byref(defocus)), "gsb200_forward_defocus")
+                    elif blur is not None:
                         _lib.check(lib.gsb200_forward_motion_blur(
                             ctypes.byref(args), ctypes.byref(ext) if ext is not None else None,
                             ctypes.byref(lens) if lens is not None else None, ctypes.byref(rs) if rs is not None else None,
@@ -669,7 +700,8 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
         self.last_frame = frame
         outs = (image, depth, acc_alpha, last_effective, valid_count) + ((feature_map,) if feature_map is not None else ())
         return outs, frame, {"camera_intrinsics": K, "lens": lens,
-                             "rolling_shutter": (rs, row_time) if rs is not None else None, "motion_blur": blur}
+                             "rolling_shutter": (rs, row_time) if rs is not None else None, "motion_blur": blur,
+                             "defocus": defocus}
 
     def _lens_args(self, camera_info, lens_coefficients=None) -> Optional[_lib.GsbLensArgs]:
         """The C lens argument of ``camera_info.distortion`` (None: the pinhole kernels), after the checks of the options
@@ -768,15 +800,51 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                 raise ValueError(f"exposure_motion must be finite, got {values}")
         return _lib.GsbMotionBlurArgs(motion=(ctypes.c_float * 6)(*values))
 
+    def _defocus_args(self, camera_info, parameters=None, rolling_shutter_motion=None, point_filter_3d=None,
+                      exposure_motion=None) -> Optional[_lib.GsbDefocusArgs]:
+        """The C defocus argument of ``camera_info.defocus`` (None: the kernels without defocus), after the checks of the
+        options a defocus does not combine with; with ``parameters`` (``differentiable_defocus``) its values (a, rho) replace
+        the record's (read on the host like ``exposure_motion``)."""
+        defocus = getattr(camera_info, "defocus", None)
+        if parameters is not None:
+            if not self.differentiable_defocus:
+                raise ValueError("defocus_parameters needs differentiable_defocus=True")
+            if defocus is None:
+                raise ValueError("defocus_parameters was given for a camera without defocus (camera_info.defocus is None)")
+        if defocus is None:
+            return None
+        for name, on in (("differentiable_pose", self.differentiable_pose),
+                         ("differentiable_intrinsics", self.differentiable_intrinsics),
+                         ("differentiable_distortion", self.differentiable_distortion),
+                         ("a gradient_exchange", self.gradient_exchange is not None),
+                         ("point_filter_3d", point_filter_3d is not None),
+                         ("rolling_shutter_motion (one camera gradient per call)", rolling_shutter_motion is not None),
+                         ("exposure_motion (one camera gradient per call)", exposure_motion is not None)):
+            if on:
+                raise ValueError(f"a defocused camera is not supported with {name}")
+        values = defocus.parameters
+        if parameters is not None:
+            if not isinstance(parameters, torch.Tensor):
+                raise ValueError("defocus_parameters must be a torch.Tensor")
+            if tuple(parameters.shape) != (2,):
+                raise ValueError(f"defocus_parameters must have shape (2,), got {tuple(parameters.shape)}")
+            if parameters.dtype != torch.float32:
+                raise ValueError(f"defocus_parameters must be float32, got {parameters.dtype}")
+            values = parameters.detach().cpu().tolist()
+            if not all(math.isfinite(v) for v in values):
+                raise ValueError(f"defocus_parameters must be finite, got {values}")
+        return _lib.GsbDefocusArgs(aperture=values[0], inverse_focus=values[1])
+
     # ------------------------------------------------------------------ backward plumbing
     def _run_backward(self, ctx, grad_rasterized_image, grad_rasterized_depth=None, grad_pixel_accumulated_alpha=None,
                       grad_feature_map=None, pose=False, intrinsics=False, lens_grad=False, motion_grad=False,
-                      blur_grad=False):
+                      blur_grad=False, defocus_grad=False):
         """Returns dL/dxyz, dL/dfeatures, for a call with extra features dL/d of them ((N, C); zeros when the feature map
         was not used), with ``pose`` dL/dq_pointcloud_camera (K, 4) and dL/dt_pointcloud_camera (K, 3) (else None), with
         ``intrinsics`` dL/dcamera_intrinsics (3, 3) (else None), with ``lens_grad`` dL/dlens_coefficients on the
         coefficient tensor's device (else None), with ``motion_grad`` dL/drolling_shutter_motion on the motion tensor's
-        device (else None), and with ``blur_grad`` dL/dexposure_motion on that tensor's device (else None)."""
+        device (else None), with ``blur_grad`` dL/dexposure_motion on that tensor's device (else None), and with
+        ``defocus_grad`` dL/ddefocus_parameters on that tensor's device (else None)."""
         cfg = self.config
         lib = _lib.load()
         saved = ctx.saved_tensors
@@ -842,8 +910,29 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                 C = extra_features.shape[1]
                 grad_extra_features = torch.zeros((N, C), dtype=torch.float32, device=device) if grad_feature_map is None \
                     else torch.empty((N, C), dtype=torch.float32, device=device)
-            grad_q = grad_t = grad_K = grad_k = grad_m = grad_b = None
-            if ctx.motion_blur is not None:  # no other camera-parameter gradient (refused in forward)
+            grad_q = grad_t = grad_K = grad_k = grad_m = grad_b = grad_d = None
+            if ctx.defocus is not None:  # no other camera-parameter gradient (refused in forward)
+                ext = None
+                if extra_features is not None and grad_feature_map is not None:
+                    grad_map = _f32(grad_feature_map)
+                    ext = _lib.GsbExtraFeatureArgs(channels=extra_features.shape[1], features=_ptr(extra_features),
+                                                   grad_rasterized=_ptr(grad_map), grad_features=_ptr(grad_extra_features))
+                rs = ctx.rolling_shutter[0] if ctx.rolling_shutter is not None else None
+                defocus_grad_args = None
+                if defocus_grad:
+                    grad_defocus = torch.empty((2,), dtype=torch.float32, device=device)
+                    defocus_temp = torch.empty((int(lib.gsb200_defocus_grad_temp_bytes()) // 4,), dtype=torch.float32,
+                                               device=device)
+                    defocus_grad_args = _lib.GsbDefocusGradArgs(grad=_ptr(grad_defocus), temp=_ptr(defocus_temp))
+                _lib.check(lib.gsb200_backward_defocus(
+                    ctypes.byref(args), _ptr(grad_depth), _ptr(depth), _ptr(grad_alpha),
+                    ctypes.byref(ext) if ext is not None else None, ctypes.byref(ctx.lens) if ctx.lens is not None else None,
+                    ctypes.byref(rs) if rs is not None else None,
+                    ctypes.byref(ctx.motion_blur) if ctx.motion_blur is not None else None, ctypes.byref(ctx.defocus),
+                    ctypes.byref(defocus_grad_args) if defocus_grad_args is not None else None), "gsb200_backward_defocus")
+                if defocus_grad:
+                    grad_d = grad_defocus.to(ctx.defocus_device)
+            elif ctx.motion_blur is not None:  # no other camera-parameter gradient (refused in forward)
                 ext = None
                 if extra_features is not None and grad_feature_map is not None:
                     grad_map = _f32(grad_feature_map)
@@ -998,7 +1087,8 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                     point_uv_in_camera=frame.point_uv.contiguous(),
                     point_depth=frame.point_in_camera[:, 2],
                 ))
-        return grad_pointcloud, grad_pointcloud_features, grad_extra_features, grad_q, grad_t, grad_K, grad_k, grad_m, grad_b
+        return grad_pointcloud, grad_pointcloud_features, grad_extra_features, grad_q, grad_t, grad_K, grad_k, grad_m, grad_b, \
+            grad_d
 
     def backward_flags(self, frame_flags: int) -> int:
         """Flags of the backward call for a frame rendered with ``frame_flags`` (adds the experimental kernel selection)."""
@@ -1012,7 +1102,7 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
     def forward(self, input_data: "GaussianPointCloudRasterisation.GaussianPointCloudRasterisationInput",
                 point_extra_features: Optional[torch.Tensor] = None, lens_coefficients: Optional[torch.Tensor] = None,
                 rolling_shutter_motion: Optional[torch.Tensor] = None, point_filter_3d: Optional[torch.Tensor] = None,
-                exposure_motion: Optional[torch.Tensor] = None):
+                exposure_motion: Optional[torch.Tensor] = None, defocus_parameters: Optional[torch.Tensor] = None):
         """Returns (image, depth, pixel_valid_point_count), then pixel_accumulated_alpha with ``differentiable_alpha``.
         ``point_extra_features`` (an extension): an (N, C) float32 tensor of per-Gaussian values (1 <= C <= 16; semantic
         logits, instance encodings, distilled features, ...), contiguous, on the scene's device.  The output tuple then
@@ -1062,10 +1152,42 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
         ``exposure_motion`` (with ``differentiable_motion_blur``; an extension): a (6,) float32 tensor (v, w) on any device.
         Its values are the exposure motion rendered, and the backward returns dL/d ``exposure_motion`` on the tensor's
         device.  ``ValueError`` for a camera without motion blur, a tensor of the wrong shape or dtype, or an operator without
-        the option.  None: no motion gradient."""
+        the option.  None: no motion gradient.
+        ``input_data.camera_info.defocus`` (an extension; ``Camera.Defocus``): render and differentiate the view through a
+        thin lens, each splat widened by its defocus blur (``gsb200_forward_defocus`` / ``gsb200_backward_defocus``;
+        definition in ``include/gsb200.h``), with or without a lens, a rolling shutter and motion blur.  Every output and
+        option above works with it, except ``differentiable_pose``, ``differentiable_intrinsics``,
+        ``differentiable_distortion``, a ``gradient_exchange``, ``point_filter_3d``, ``rolling_shutter_motion`` and
+        ``exposure_motion`` (``ValueError``).  A pinhole render of the same view is the camera with ``defocus=None``; a
+        refocused one is the camera with another ``Defocus``.
+        ``defocus_parameters`` (with ``differentiable_defocus``; an extension): a (2,) float32 tensor (a, rho) on any
+        device.  Its values are the aperture and inverse focus distance rendered (a negative a renders as |a|), and the
+        backward returns dL/d ``defocus_parameters`` on the tensor's device.  ``ValueError`` for a camera without defocus, a
+        tensor of the wrong shape or dtype, or an operator without the option.  None: no defocus gradient."""
         camera_info = input_data.camera_info
         assert camera_info.camera_width % TILE_WIDTH == 0
         assert camera_info.camera_height % TILE_HEIGHT == 0
+        if getattr(camera_info, "defocus", None) is not None or defocus_parameters is not None:
+            # the argument checks, before any device work; K, the coefficients, both motions and the filter are refused,
+            # so their slots are None
+            self._defocus_args(camera_info, defocus_parameters, rolling_shutter_motion, point_filter_3d, exposure_motion)
+            self._motion_blur_args(camera_info)
+            self._lens_args(camera_info, lens_coefficients)
+            self._rolling_shutter_args(camera_info)
+            if lens_coefficients is not None:
+                raise ValueError("a defocused camera is not supported with lens_coefficients")
+            if point_extra_features is not None:
+                self._check_extra_features(point_extra_features, input_data.point_cloud)
+            tail = (None,) * 5 + (defocus_parameters,) if defocus_parameters is not None else ()
+            if point_extra_features is not None or tail:
+                return self._module_function.apply(
+                    input_data.point_cloud, input_data.point_cloud_features, input_data.point_invalid_mask,
+                    input_data.point_object_id, input_data.q_pointcloud_camera, input_data.t_pointcloud_camera, camera_info,
+                    input_data.color_max_sh_band, point_extra_features, *tail)
+            return self._module_function.apply(
+                input_data.point_cloud, input_data.point_cloud_features, input_data.point_invalid_mask,
+                input_data.point_object_id, input_data.q_pointcloud_camera, input_data.t_pointcloud_camera, camera_info,
+                input_data.color_max_sh_band)
         if getattr(camera_info, "motion_blur", None) is not None or exposure_motion is not None:
             # the argument checks, before any device work; K, the coefficients, the row-time motion and the filter are
             # refused, so their slots are None

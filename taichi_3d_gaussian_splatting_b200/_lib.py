@@ -147,6 +147,14 @@ class GsbMotionBlurGradArgs(ctypes.Structure):
     _fields_ = [("grad_motion", c_vp), ("temp", c_vp)]
 
 
+class GsbDefocusArgs(ctypes.Structure):
+    _fields_ = [("aperture", c_f32), ("inverse_focus", c_f32)]
+
+
+class GsbDefocusGradArgs(ctypes.Structure):
+    _fields_ = [("grad", c_vp), ("temp", c_vp)]
+
+
 class GsbAppearanceArgs(ctypes.Structure):
     _fields_ = [
         ("grid", c_vp), ("grad_grid", c_vp), ("grid_x", c_i32), ("grid_y", c_i32), ("grid_z", c_i32), ("tv_weight", c_f32),
@@ -233,6 +241,7 @@ EXPORTS = (
     "gsb200_filter3d_temp_bytes", "gsb200_filter3d_from_views", "gsb200_abi_sizes_filter3d", "gsb200_robust_temp_bytes",
     "gsb200_robust_image_loss", "gsb200_train_step_robust", "gsb200_abi_sizes_robust", "gsb200_forward_motion_blur",
     "gsb200_backward_motion_blur", "gsb200_motion_blur_grad_temp_bytes", "gsb200_abi_sizes_motion_blur",
+    "gsb200_forward_defocus", "gsb200_backward_defocus", "gsb200_defocus_grad_temp_bytes", "gsb200_abi_sizes_defocus",
 )
 
 _lib = None
@@ -307,6 +316,17 @@ def load() -> ctypes.CDLL:
     lib.gsb200_backward_motion_blur.restype = ctypes.c_int
     lib.gsb200_motion_blur_grad_temp_bytes.argtypes = []
     lib.gsb200_motion_blur_grad_temp_bytes.restype = c_i64
+    lib.gsb200_forward_defocus.argtypes = [ctypes.POINTER(GsbForwardArgs), ctypes.POINTER(GsbExtraFeatureArgs),
+                                           ctypes.POINTER(GsbLensArgs), ctypes.POINTER(GsbRollingShutterArgs),
+                                           ctypes.POINTER(GsbMotionBlurArgs), ctypes.POINTER(GsbDefocusArgs)]
+    lib.gsb200_forward_defocus.restype = ctypes.c_int
+    lib.gsb200_backward_defocus.argtypes = [ctypes.POINTER(GsbBackwardArgs), c_vp, c_vp, c_vp,
+                                            ctypes.POINTER(GsbExtraFeatureArgs), ctypes.POINTER(GsbLensArgs),
+                                            ctypes.POINTER(GsbRollingShutterArgs), ctypes.POINTER(GsbMotionBlurArgs),
+                                            ctypes.POINTER(GsbDefocusArgs), ctypes.POINTER(GsbDefocusGradArgs)]
+    lib.gsb200_backward_defocus.restype = ctypes.c_int
+    lib.gsb200_defocus_grad_temp_bytes.argtypes = []
+    lib.gsb200_defocus_grad_temp_bytes.restype = c_i64
     lib.gsb200_intrinsics_grad_temp_bytes.argtypes = []
     lib.gsb200_intrinsics_grad_temp_bytes.restype = c_i64
     lib.gsb200_sort_temp_bytes.argtypes = [c_i64, c_i32]
@@ -474,6 +494,14 @@ def load() -> ctypes.CDLL:
     for i, mirror in ((0, GsbMotionBlurArgs), (1, GsbMotionBlurGradArgs)):
         if sizes_blur[i] != ctypes.sizeof(mirror):
             raise RuntimeError(f"libgsb200.so ABI mismatch: sizeof({mirror.__name__}) {sizes_blur[i]} != ctypes mirror "
+                               f"{ctypes.sizeof(mirror)}")
+    lib.gsb200_abi_sizes_defocus.argtypes = [ctypes.POINTER(c_i64)]
+    lib.gsb200_abi_sizes_defocus.restype = None
+    sizes_defocus = (c_i64 * 2)()
+    lib.gsb200_abi_sizes_defocus(sizes_defocus)
+    for i, mirror in ((0, GsbDefocusArgs), (1, GsbDefocusGradArgs)):
+        if sizes_defocus[i] != ctypes.sizeof(mirror):
+            raise RuntimeError(f"libgsb200.so ABI mismatch: sizeof({mirror.__name__}) {sizes_defocus[i]} != ctypes mirror "
                                f"{ctypes.sizeof(mirror)}")
     lib.gsb200_abi_sizes_mcmc.argtypes = [ctypes.POINTER(c_i64)]
     lib.gsb200_abi_sizes_mcmc.restype = None

@@ -211,6 +211,11 @@ void gsb200_abi_sizes_motion_blur(int64_t *out2) {
     out2[1] = (int64_t)sizeof(GsbMotionBlurGradArgs);
 }
 
+void gsb200_abi_sizes_defocus(int64_t *out2) {
+    out2[0] = (int64_t)sizeof(GsbDefocusArgs);
+    out2[1] = (int64_t)sizeof(GsbDefocusGradArgs);
+}
+
 void gsb200_abi_sizes_filter3d(int64_t *out2) {
     out2[0] = (int64_t)sizeof(GsbFilter3dArgs);
     out2[1] = (int64_t)sizeof(GsbFilter3dViewsArgs);
@@ -357,10 +362,31 @@ int64_t gsb200_motion_blur_grad_temp_bytes(void) {
     return (int64_t)GSB_RS_GRAD_PARTIAL_BLOCKS * 6 * (int64_t)sizeof(float);
 }
 
-// The forward of gsb200_forward_filter3d / gsb200_forward_motion_blur after their own checks (filter3d and blur: checked, at
-// most one of them set)
+// GsbDefocusArgs -> DefocusParams; GSB_EINVAL for a non-finite a or rho.  *out_defocus stays NULL for a NULL defocus.
+static int check_defocus(const char *what, const GsbDefocusArgs *defocus, DefocusParams *params,
+                         const DefocusParams **out_defocus) {
+    *out_defocus = nullptr;
+    if (!defocus) return GSB_OK;
+    const float a = defocus->aperture, rho = defocus->inverse_focus;
+    if (!(a - a == 0.0f) || !(rho - rho == 0.0f)) {
+        set_error("%s: aperture / inverse_focus is not finite", what);
+        return GSB_EINVAL;
+    }
+    params->aperture = a;
+    params->inverse_focus = rho;
+    *out_defocus = params;
+    return GSB_OK;
+}
+
+int64_t gsb200_defocus_grad_temp_bytes(void) {
+    return ((int64_t)GSB_RS_GRAD_PARTIAL_BLOCKS + 1) * 6 * (int64_t)sizeof(float);
+}
+
+// The forward of gsb200_forward_filter3d / gsb200_forward_motion_blur / gsb200_forward_defocus after their own checks
+// (filter3d and blur / defocus: checked, never together)
 static int forward_checked(const GsbForwardArgs *a, const GsbExtraFeatureArgs *ext, const GsbLensArgs *lens_args,
-                           const GsbRollingShutterArgs *rs_args, const float *filter3d, const BlurParams *blur);
+                           const GsbRollingShutterArgs *rs_args, const float *filter3d, const BlurParams *blur,
+                           const DefocusParams *defocus = nullptr);
 
 int gsb200_forward_filter3d(const GsbForwardArgs *a, const GsbExtraFeatureArgs *ext, const GsbLensArgs *lens_args,
                             const GsbRollingShutterArgs *rs_args, const GsbFilter3dArgs *filter) {
@@ -379,8 +405,23 @@ int gsb200_forward_motion_blur(const GsbForwardArgs *a, const GsbExtraFeatureArg
     return forward_checked(a, ext, lens_args, rs_args, nullptr, blur);
 }
 
+int gsb200_forward_defocus(const GsbForwardArgs *a, const GsbExtraFeatureArgs *ext, const GsbLensArgs *lens_args,
+                           const GsbRollingShutterArgs *rs_args, const GsbMotionBlurArgs *blur_args,
+                           const GsbDefocusArgs *defocus_args) {
+    if (!defocus_args) return gsb200_forward_motion_blur(a, ext, lens_args, rs_args, blur_args);
+    BlurParams blur_params;
+    const BlurParams *blur;
+    int rc = check_blur("forward_defocus", blur_args, &blur_params, &blur);
+    if (rc != GSB_OK) return rc;
+    DefocusParams defocus_params;
+    const DefocusParams *defocus;
+    if ((rc = check_defocus("forward_defocus", defocus_args, &defocus_params, &defocus)) != GSB_OK) return rc;
+    return forward_checked(a, ext, lens_args, rs_args, nullptr, blur, defocus);
+}
+
 static int forward_checked(const GsbForwardArgs *a, const GsbExtraFeatureArgs *ext, const GsbLensArgs *lens_args,
-                           const GsbRollingShutterArgs *rs_args, const float *filter3d, const BlurParams *blur) {
+                           const GsbRollingShutterArgs *rs_args, const float *filter3d, const BlurParams *blur,
+                           const DefocusParams *defocus) {
     LensParams lens_params;
     const LensParams *lens;
     int lrc = check_lens(rs_args ? "forward_rolling_shutter" : "forward_lens", lens_args, &lens_params, &lens);
@@ -406,7 +447,7 @@ static int forward_checked(const GsbForwardArgs *a, const GsbExtraFeatureArgs *e
     int rc = resolve_fwd(a, &ws);
     if (rc != GSB_OK) return rc;
     cudaStream_t st = static_cast<cudaStream_t>(a->stream);
-    if ((rc = launch_preprocess(*a, ws, st, lens, rs, filter3d, blur)) != GSB_OK) return rc;
+    if ((rc = launch_preprocess(*a, ws, st, lens, rs, filter3d, blur, defocus)) != GSB_OK) return rc;
     if (a->host_counters && a->host_counters_event) {
         GSB_CUDA_CHECK(cudaMemcpyAsync(a->host_counters, ws.counters, 4 * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
         GSB_CUDA_CHECK(cudaEventRecord(static_cast<cudaEvent_t>(a->host_counters_event), st));
@@ -425,7 +466,8 @@ static int backward_impl(const GsbBackwardArgs *a, bool skip_on_overflow, const 
                          const GsbIntrinsicsGradArgs *intr = nullptr, const LensParams *lens = nullptr,
                          const GsbLensGradArgs *lens_grad = nullptr, const RsParams *rs = nullptr,
                          const GsbRollingShutterGradArgs *rs_grad = nullptr, const float *filter3d = nullptr,
-                         const BlurParams *blur = nullptr, const GsbMotionBlurGradArgs *blur_grad = nullptr) {
+                         const BlurParams *blur = nullptr, const GsbMotionBlurGradArgs *blur_grad = nullptr,
+                         const DefocusParams *defocus = nullptr, const GsbDefocusGradArgs *defocus_grad = nullptr) {
     if (!a) {
         set_error("backward: args is null");
         return GSB_EINVAL;
@@ -479,6 +521,9 @@ static int backward_impl(const GsbBackwardArgs *a, bool skip_on_overflow, const 
     if (ext && a->num_points > 0)  // the blend adds into the rows it reaches; every other row stays zero
         GSB_CUDA_CHECK(cudaMemsetAsync(ext->grad_features, 0, (size_t)a->num_points * ext->channels * 4, st));
     if ((rc = launch_blend_backward(*a, ws, st, grad_depth, depth, grad_alpha, ext)) != GSB_OK) return rc;
+    if (defocus)  // a NULL blur is zero motion
+        return launch_backward_points_blur(*a, ws, st, grad_depth != nullptr, lens, rs, blur ? *blur : BlurParams{}, nullptr,
+                                           defocus, defocus_grad);
     if (blur) return launch_backward_points_blur(*a, ws, st, grad_depth != nullptr, lens, rs, *blur, blur_grad);
     if (filter3d)
         return launch_backward_points_filter(*a, ws, st, skip_on_overflow ? ws.counters + CNT_OVERFLOW : nullptr,
@@ -511,7 +556,8 @@ static int backward_checked(const GsbBackwardArgs *a, const float *grad_rasteriz
                             const GsbIntrinsicsGradArgs *intr, const LensParams *lens, const GsbLensGradArgs *lens_grad = nullptr,
                             const RsParams *rs = nullptr, const GsbRollingShutterGradArgs *rs_grad = nullptr,
                             const float *filter3d = nullptr, const BlurParams *blur = nullptr,
-                            const GsbMotionBlurGradArgs *blur_grad = nullptr);
+                            const GsbMotionBlurGradArgs *blur_grad = nullptr, const DefocusParams *defocus = nullptr,
+                            const GsbDefocusGradArgs *defocus_grad = nullptr);
 
 int gsb200_backward_motion_blur(const GsbBackwardArgs *a, const float *grad_rasterized_depth, const float *rasterized_depth,
                                 const float *grad_pixel_accumulated_alpha, const GsbExtraFeatureArgs *ext,
@@ -555,6 +601,54 @@ int gsb200_backward_motion_blur(const GsbBackwardArgs *a, const float *grad_rast
     }
     return backward_checked(a, grad_rasterized_depth, rasterized_depth, grad_pixel_accumulated_alpha, ext, nullptr, nullptr, lens,
                             nullptr, rs, nullptr, nullptr, blur, blur_grad);
+}
+
+int gsb200_backward_defocus(const GsbBackwardArgs *a, const float *grad_rasterized_depth, const float *rasterized_depth,
+                            const float *grad_pixel_accumulated_alpha, const GsbExtraFeatureArgs *ext,
+                            const GsbLensArgs *lens_args, const GsbRollingShutterArgs *rs_args,
+                            const GsbMotionBlurArgs *blur_args, const GsbDefocusArgs *defocus_args,
+                            const GsbDefocusGradArgs *defocus_grad) {
+    if (!defocus_args && defocus_grad) {
+        set_error("backward_defocus: the defocus gradient needs a defocus (defocus is NULL)");
+        return GSB_EINVAL;
+    }
+    if (!defocus_args)
+        return gsb200_backward_motion_blur(a, grad_rasterized_depth, rasterized_depth, grad_pixel_accumulated_alpha, ext,
+                                           lens_args, rs_args, blur_args, nullptr);
+    LensParams lens_params;
+    const LensParams *lens;
+    int rc = check_lens("backward_defocus", lens_args, &lens_params, &lens);
+    if (rc != GSB_OK) return rc;
+    RsParams rs_params;
+    const RsParams *rs;
+    if ((rc = check_rs("backward_defocus", rs_args, &rs_params, &rs)) != GSB_OK) return rc;
+    BlurParams blur_params;
+    const BlurParams *blur;
+    if ((rc = check_blur("backward_defocus", blur_args, &blur_params, &blur)) != GSB_OK) return rc;
+    DefocusParams defocus_params;
+    const DefocusParams *defocus;
+    if ((rc = check_defocus("backward_defocus", defocus_args, &defocus_params, &defocus)) != GSB_OK) return rc;
+    if (defocus_grad) {
+        if (!defocus_grad->grad || !defocus_grad->temp) {
+            set_error("backward_defocus: null grad / temp pointer");
+            return GSB_EINVAL;
+        }
+        if (reinterpret_cast<uintptr_t>(defocus_grad->grad) % 4 != 0) {
+            set_error("backward_defocus: grad must be 4-byte aligned");
+            return GSB_EINVAL;
+        }
+        if (reinterpret_cast<uintptr_t>(defocus_grad->temp) % 16 != 0) {
+            set_error("backward_defocus: the defocus temp must be 16-byte aligned");
+            return GSB_EINVAL;
+        }
+    }
+    if (a != nullptr && (a->flags & GSB_FLAG_COMPACT_GRADS)) {
+        set_error("backward_defocus: the defocus is not implemented for the compact rows of the view-parallel exchange "
+                  "(GSB_FLAG_COMPACT_GRADS)");
+        return GSB_EUNSUPPORTED;
+    }
+    return backward_checked(a, grad_rasterized_depth, rasterized_depth, grad_pixel_accumulated_alpha, ext, nullptr, nullptr, lens,
+                            nullptr, rs, nullptr, nullptr, blur, nullptr, defocus, defocus_grad);
 }
 
 int gsb200_backward_filter3d(const GsbBackwardArgs *a, const float *grad_rasterized_depth, const float *rasterized_depth,
@@ -696,7 +790,8 @@ static int backward_checked(const GsbBackwardArgs *a, const float *grad_rasteriz
                             const float *grad_pixel_accumulated_alpha, const GsbExtraFeatureArgs *ext, const GsbPoseGradArgs *pose,
                             const GsbIntrinsicsGradArgs *intr, const LensParams *lens, const GsbLensGradArgs *lens_grad,
                             const RsParams *rs, const GsbRollingShutterGradArgs *rs_grad, const float *filter3d,
-                            const BlurParams *blur, const GsbMotionBlurGradArgs *blur_grad) {
+                            const BlurParams *blur, const GsbMotionBlurGradArgs *blur_grad, const DefocusParams *defocus,
+                            const GsbDefocusGradArgs *defocus_grad) {
     if (intr) {
         if (!intr->grad_camera_intrinsics || !intr->temp) {
             set_error("backward_calib: null grad_camera_intrinsics / temp pointer");
@@ -762,7 +857,7 @@ static int backward_checked(const GsbBackwardArgs *a, const float *grad_rasteriz
         return GSB_EUNSUPPORTED;
     }
     return backward_impl(a, false, grad_rasterized_depth, rasterized_depth, grad_pixel_accumulated_alpha, ext, pose, intr, lens,
-                         lens_grad, rs, rs_grad, filter3d, blur, blur_grad);
+                         lens_grad, rs, rs_grad, filter3d, blur, blur_grad, defocus, defocus_grad);
 }
 
 int gsb200_backward_with_depth(const GsbBackwardArgs *a, const float *grad_rasterized_depth, const float *rasterized_depth) {

@@ -444,17 +444,24 @@ __device__ __forceinline__ void weighted_u_sigma(const float *U, const float *R,
 // LGRAD / MGRAD / FILTER; with or without LENS and RS.
 // BGRAD = true (with BLUR and blur_grad): each in-camera point also forms dL/dv = g and dL/dw = pc x g with g = Jp^T dL/dd,
 // which go through the rows of MGRAD: s_mgrad, mgrad_partials and rolling_shutter_grad_finish_kernel.
+// DEFOCUS = true (with BLUR; gsb200_backward_defocus): B also carries the thin lens' B_d = beta M M^T (include/gsb200.h; beta
+// detached, at pcz).  With G_B = G - G_a/2 (Sigma_d + B)^-1 (blur_cov_grad, common.cuh), dL/dSigma' is that of BLUR with this
+// B.  A view with a = 0 takes the arithmetic without defocus.  Not with BGRAD.
+// DGRAD = true (with DEFOCUS and defocus_grad): each in-camera point also forms dL/da = dL/dbeta a (rho - 1/z)^2 / 8 and
+// dL/drho = dL/dbeta a^2 (rho - 1/z) / 8 with dL/dbeta = <G_B, M M^T>, in the first two values of the rows of MGRAD.
 constexpr int LENS_GRAD_VALUES = 5;
 constexpr int RS_GRAD_VALUES = 6;
 template <bool COMPACT, bool DEPTH, bool POSE, bool INTR = false, bool LENS = false, bool LGRAD = false, bool RS = false,
-          bool MGRAD = false, bool FILTER = false, bool BLUR = false, bool BGRAD = false>
+          bool MGRAD = false, bool FILTER = false, bool BLUR = false, bool BGRAD = false, bool DEFOCUS = false,
+          bool DGRAD = false>
 __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, float *s_pose, float *pose_partials,
                                                      int num_objects, float *s_intr = nullptr,
                                                      float *intr_partials = nullptr, const LensParams lens = LensParams(),
                                                      float *s_lgrad = nullptr, float *lgrad_partials = nullptr,
                                                      const RsParams rs = RsParams(), float *s_mgrad = nullptr,
                                                      float *mgrad_partials = nullptr, const float *filter3d = nullptr,
-                                                     const BlurParams blur = BlurParams()) {
+                                                     const BlurParams blur = BlurParams(),
+                                                     const DefocusParams defocus = DefocusParams()) {
     static_assert(!LENS || (!COMPACT && !POSE && !INTR), "the lens gradient is implemented for the dense rows alone");
     static_assert(!LGRAD || LENS, "the coefficient gradient needs the lens path");
     static_assert(!RS || (!COMPACT && !POSE && !INTR && !LGRAD), "the rolling shutter is implemented for the dense rows alone");
@@ -464,7 +471,9 @@ __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, fl
     static_assert(!BLUR || (!COMPACT && !POSE && !INTR && !LGRAD && !MGRAD && !FILTER),
                   "the motion blur is implemented for the dense rows without other camera gradients or the 3D filter");
     static_assert(!BGRAD || BLUR, "the exposure-motion gradient needs the motion-blur path");
-    constexpr bool CAM6 = MGRAD || BGRAD;  // a 6-value motion gradient (rolling shutter or exposure)
+    static_assert(!DEFOCUS || (BLUR && !BGRAD), "the defocus runs on the motion-blur path, without the exposure-motion gradient");
+    static_assert(!DGRAD || DEFOCUS, "the defocus gradient needs the defocus path");
+    constexpr bool CAM6 = MGRAD || BGRAD || DGRAD;  // the rows of a camera gradient (rolling shutter, exposure or defocus)
     // One thread per scene row: rows outside the frustum get their zeros here (no separate memset of the
     // dense (N,3)/(N,56) gradients), rows inside get the chain rule.  A warp owns 32 consecutive rows, i.e. one
     // contiguous 7 KB piece of the (N,56) gradient and 384 B of the (N,3) one: each lane stages its row in
@@ -556,6 +565,7 @@ __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, fl
         float dj[6] = {Kc[0] * iz, Kc[1] * iz, (-Kc[0] * pcx - Kc[1] * pcy) * iz2,
                        Kc[3] * iz, Kc[4] * iz, (-Kc[3] * pcx - Kc[4] * pcy) * iz2};
         float Jl[6];  // LENS: diag(fx, fy) D P, the J of Sigma' below
+        float Mk[4] = {Kc[0], Kc[1], Kc[3], Kc[4]};  // DEFOCUS: M = K[:2,:2] (K[:2,:2] D with LENS)
         if (LENS) {
             float ox, oy, D[4];  // D = d(xd, yd)/d(xn, yn) at the point
             if (lens.model == GSB_LENS_FISHEYE) lens_distort<GSB_LENS_FISHEYE>(lens.k, pcx * iz, pcy * iz, ox, oy, D);
@@ -563,6 +573,7 @@ __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, fl
             // K[:2,:2] D P: the pinhole expression with K[:2,:2] replaced by K[:2,:2] D (exactly K[:2,:2] for D = I)
             const float A0 = Kc[0] * D[0] + Kc[1] * D[2], A1 = Kc[0] * D[1] + Kc[1] * D[3];
             const float A3 = Kc[3] * D[0] + Kc[4] * D[2], A4 = Kc[3] * D[1] + Kc[4] * D[3];
+            Mk[0] = A0; Mk[1] = A1; Mk[2] = A3; Mk[3] = A4;
             dj[0] = A0 * iz; dj[1] = A1 * iz; dj[2] = (-A0 * pcx - A1 * pcy) * iz2;
             dj[3] = A3 * iz; dj[4] = A4 * iz; dj[5] = (-A3 * pcx - A4 * pcy) * iz2;
             const float F0 = Kc[0] * D[0], F1 = Kc[0] * D[1], F3 = Kc[4] * D[2], F4 = Kc[4] * D[3];  // likewise
@@ -591,7 +602,9 @@ __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, fl
             U[3 + c] = J[3] * Wm[c] + J[4] * Wm[3 + c] + J[5] * Wm[6 + c];
         }
         float g00 = 0.5f * a0.z, g01 = 0.5f * a0.w, g11 = 0.5f * a1.x;  // UT:345's 1/2, see the blend loop
-        if (BLUR && motion_blur_on(blur.motion)) {
+        const bool moving = BLUR && motion_blur_on(blur.motion);
+        const bool defocused = DEFOCUS && defocus.aperture != 0.0f;
+        if (moving || defocused) {
             // Sigma' = (U M)(U M)^T, M = R(q) diag(exp(s)) (the rows of R and exp(s) as below)
             const float bx = qv.x, by = qv.y, bz = qv.z, bw = qv.w;
             const float Rb[9] = {1 - 2 * (by * by + bz * bz), 2 * (bx * by - bw * bz), 2 * (bx * bz + bw * by),
@@ -608,17 +621,33 @@ __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, fl
             const float s01 = UM[0] * UM[3] + UM[1] * UM[4] + UM[2] * UM[5];
             const float s11 = UM[3] * UM[3] + UM[4] * UM[4] + UM[5] * UM[5];
             const float pcv[3] = {pcx, pcy, pcz};
-            float d0, d1, gd0, gd1;
-            motion_blur_velocity(dj, pcv, blur.motion, d0, d1);
+            float d0 = 0.0f, d1 = 0.0f, gd0, gd1;
+            if (moving) motion_blur_velocity(dj, pcv, blur.motion, d0, d1);
             const float one_minus_o = 1.0f - __ldg(p.records + 3 * (size_t)o + 1).z;
             const float g_alpha = one_minus_o != 0.0f ? a2.x / one_minus_o : 0.0f;
-            motion_blur_grad(s00, s01, s11, d0, d1, g_alpha, g00, g01, g11, gd0, gd1);
-            if (BGRAD) {  // g = Jp^T dL/dd: dL/dv = g, dL/dw = pc x g
-                const float q0 = dj[0] * gd0 + dj[3] * gd1, q1 = dj[1] * gd0 + dj[4] * gd1, q2 = dj[2] * gd0 + dj[5] * gd1;
-                mv[0] = q0; mv[1] = q1; mv[2] = q2;
-                mv[3] = pcy * q2 - pcz * q1;
-                mv[4] = pcz * q0 - pcx * q2;
-                mv[5] = pcx * q1 - pcy * q0;
+            if (!defocused) {
+                motion_blur_grad(s00, s01, s11, d0, d1, g_alpha, g00, g01, g11, gd0, gd1);
+                if (BGRAD) {  // g = Jp^T dL/dd: dL/dv = g, dL/dw = pc x g
+                    const float q0 = dj[0] * gd0 + dj[3] * gd1, q1 = dj[1] * gd0 + dj[4] * gd1, q2 = dj[2] * gd0 + dj[5] * gd1;
+                    mv[0] = q0; mv[1] = q1; mv[2] = q2;
+                    mv[3] = pcy * q2 - pcz * q1;
+                    mv[4] = pcz * q0 - pcx * q2;
+                    mv[5] = pcx * q1 - pcy * q0;
+                }
+            } else {  // B = d d^T / 12 (zero without motion) + beta M M^T
+                const float P00 = Mk[0] * Mk[0] + Mk[1] * Mk[1], P01 = Mk[0] * Mk[2] + Mk[1] * Mk[3],
+                            P11 = Mk[2] * Mk[2] + Mk[3] * Mk[3];
+                const float beta = defocus_variance(defocus, pcz);
+                const float b00 = (d0 * d0) / 12.0f + beta * P00, b01 = (d0 * d1) / 12.0f + beta * P01,
+                            b11 = (d1 * d1) / 12.0f + beta * P11;
+                float h00, h01, h11;
+                blur_cov_grad(s00, s01, s11, b00, b01, b11, g_alpha, g00, g01, g11, h00, h01, h11);
+                if (DGRAD) {
+                    const float gbeta = h00 * P00 + 2.0f * (h01 * P01) + h11 * P11;
+                    const float e = defocus.inverse_focus - 1.0f / pcz, a = defocus.aperture;
+                    mv[0] = gbeta * (a * (e * e)) / 8.0f;
+                    mv[1] = gbeta * ((a * a) * e) / 8.0f;
+                }
             }
         }
         // V = U^T G U  (dL/dSigma with the (g00,g01,g01,g11) weighting of GPCR:716-721)
@@ -1018,17 +1047,19 @@ backward_points_rs_filter_kernel(const PointsBwdRsFilterParams p) {
 }
 
 // The parameter block of the BLUR instantiations (LENS = false ignores `lens`, RS = false ignores `rs`; rs_partials: the
-// BGRAD rows).
+// BGRAD or DGRAD rows; DEFOCUS = false ignores `defocus`).
 struct PointsBwdBlurParams : PointsBwdRsParams {
     BlurParams blur;
+    DefocusParams defocus;
 };
 
-template <bool DEPTH, bool LENS, bool RS, bool BGRAD>
-__global__ void __launch_bounds__(GSB_POINTS_THREADS, BGRAD ? 3 : 5)
+template <bool DEPTH, bool LENS, bool RS, bool BGRAD, bool DEFOCUS = false, bool DGRAD = false>
+__global__ void __launch_bounds__(GSB_POINTS_THREADS, BGRAD || DGRAD ? 3 : 5)
 backward_points_blur_kernel(const PointsBwdBlurParams p) {
-    __shared__ float s_mgrad[BGRAD ? (GSB_POINTS_THREADS / 32) * RS_GRAD_VALUES : 1];
-    backward_points_body<false, DEPTH, false, false, LENS, false, RS, false, false, true, BGRAD>(
-        p, nullptr, nullptr, 0, nullptr, nullptr, p.lens, nullptr, nullptr, p.rs, s_mgrad, p.rs_partials, nullptr, p.blur);
+    __shared__ float s_mgrad[BGRAD || DGRAD ? (GSB_POINTS_THREADS / 32) * RS_GRAD_VALUES : 1];
+    backward_points_body<false, DEPTH, false, false, LENS, false, RS, false, false, true, BGRAD, DEFOCUS, DGRAD>(
+        p, nullptr, nullptr, 0, nullptr, nullptr, p.lens, nullptr, nullptr, p.rs, s_mgrad, p.rs_partials, nullptr, p.blur,
+        p.defocus);
 }
 
 // One CTA: adds the `blocks` partial rows in a fixed order (strided per thread, then a fixed shared-memory tree) and writes
@@ -1392,42 +1423,55 @@ int launch_backward_points_rs(const GsbBackwardArgs &a, const Workspace &ws, cud
     return GSB_OK;
 }
 
+// mode 0: BLUR, 1: BGRAD, 2: DEFOCUS, 3: DEFOCUS and DGRAD
 template <bool DEPTH, bool LENS, bool RS>
-static void launch_blur_kernel(bool bgrad, int blocks, cudaStream_t stream, const PointsBwdBlurParams &p) {
-    if (bgrad) backward_points_blur_kernel<DEPTH, LENS, RS, true><<<blocks, GSB_POINTS_THREADS, 0, stream>>>(p);
+static void launch_blur_kernel(int mode, int blocks, cudaStream_t stream, const PointsBwdBlurParams &p) {
+    if (mode == 1) backward_points_blur_kernel<DEPTH, LENS, RS, true><<<blocks, GSB_POINTS_THREADS, 0, stream>>>(p);
+    else if (mode == 2) backward_points_blur_kernel<DEPTH, LENS, RS, false, true, false><<<blocks, GSB_POINTS_THREADS, 0, stream>>>(p);
+    else if (mode == 3) backward_points_blur_kernel<DEPTH, LENS, RS, false, true, true><<<blocks, GSB_POINTS_THREADS, 0, stream>>>(p);
     else backward_points_blur_kernel<DEPTH, LENS, RS, false><<<blocks, GSB_POINTS_THREADS, 0, stream>>>(p);
 }
 
-// The BLUR per-point kernel on the grid of launch_backward_points_rs (at most GSB_RS_GRAD_PARTIAL_BLOCKS CTAs with blur_grad),
-// then with blur_grad rolling_shutter_grad_finish_kernel.  The caller checked the arguments.
+// The BLUR per-point kernel on the grid of launch_backward_points_rs (at most GSB_RS_GRAD_PARTIAL_BLOCKS CTAs with blur_grad
+// or defocus_grad), then with either rolling_shutter_grad_finish_kernel.  With defocus_grad the finished row goes to the slot
+// after the per-CTA rows in defocus_grad->temp and its first two values (dL/da, dL/drho) to defocus_grad->grad.  The caller
+// checked the arguments.
 int launch_backward_points_blur(const GsbBackwardArgs &a, const Workspace &ws, cudaStream_t stream, bool depth_grad,
                                 const LensParams *lens, const RsParams *rs, const BlurParams &blur,
-                                const GsbMotionBlurGradArgs *blur_grad) {
+                                const GsbMotionBlurGradArgs *blur_grad, const DefocusParams *defocus,
+                                const GsbDefocusGradArgs *defocus_grad) {
     PointsBwdBlurParams p;
     static_cast<PointsBwdParams &>(p) = make_points_params(a, ws, nullptr);
     p.lens = lens != nullptr ? *lens : LensParams();
     p.rs = rs != nullptr ? *rs : RsParams();
-    p.rs_partials = blur_grad != nullptr ? static_cast<float *>(blur_grad->temp) : nullptr;
+    p.rs_partials = blur_grad != nullptr ? static_cast<float *>(blur_grad->temp)
+                    : defocus_grad != nullptr ? static_cast<float *>(defocus_grad->temp) : nullptr;
     p.blur = blur;
+    p.defocus = defocus != nullptr ? *defocus : DefocusParams();
+    const bool cam_grad = blur_grad != nullptr || defocus_grad != nullptr;
     long long blocks = a.num_points > 0 ? (a.num_points + GSB_POINTS_THREADS - 1) / GSB_POINTS_THREADS : 0;
-    const long long cap = blur_grad != nullptr ? (long long)GSB_RS_GRAD_PARTIAL_BLOCKS : 16LL * num_sms();
+    const long long cap = cam_grad ? (long long)GSB_RS_GRAD_PARTIAL_BLOCKS : 16LL * num_sms();
     if (blocks > cap) blocks = cap;
     if (blocks > 0) {
-        const bool bgrad = blur_grad != nullptr, l = lens != nullptr, r = rs != nullptr;
+        const int mode = defocus != nullptr ? (defocus_grad != nullptr ? 3 : 2) : blur_grad != nullptr ? 1 : 0;
+        const bool l = lens != nullptr, r = rs != nullptr;
         const int g = (int)blocks;
         if (depth_grad) {
-            if (l) r ? launch_blur_kernel<true, true, true>(bgrad, g, stream, p) : launch_blur_kernel<true, true, false>(bgrad, g, stream, p);
-            else r ? launch_blur_kernel<true, false, true>(bgrad, g, stream, p) : launch_blur_kernel<true, false, false>(bgrad, g, stream, p);
+            if (l) r ? launch_blur_kernel<true, true, true>(mode, g, stream, p) : launch_blur_kernel<true, true, false>(mode, g, stream, p);
+            else r ? launch_blur_kernel<true, false, true>(mode, g, stream, p) : launch_blur_kernel<true, false, false>(mode, g, stream, p);
         } else {
-            if (l) r ? launch_blur_kernel<false, true, true>(bgrad, g, stream, p) : launch_blur_kernel<false, true, false>(bgrad, g, stream, p);
-            else r ? launch_blur_kernel<false, false, true>(bgrad, g, stream, p) : launch_blur_kernel<false, false, false>(bgrad, g, stream, p);
+            if (l) r ? launch_blur_kernel<false, true, true>(mode, g, stream, p) : launch_blur_kernel<false, true, false>(mode, g, stream, p);
+            else r ? launch_blur_kernel<false, false, true>(mode, g, stream, p) : launch_blur_kernel<false, false, false>(mode, g, stream, p);
         }
         GSB_CUDA_CHECK(cudaGetLastError());
     }
-    if (blur_grad != nullptr) {
-        rolling_shutter_grad_finish_kernel<<<1, RS_GRAD_FINISH_THREADS, 0, stream>>>(p.rs_partials, (int)blocks,
-                                                                                     blur_grad->grad_motion);
+    if (cam_grad) {
+        float *const row = blur_grad != nullptr ? blur_grad->grad_motion
+                                                : p.rs_partials + (size_t)GSB_RS_GRAD_PARTIAL_BLOCKS * RS_GRAD_VALUES;
+        rolling_shutter_grad_finish_kernel<<<1, RS_GRAD_FINISH_THREADS, 0, stream>>>(p.rs_partials, (int)blocks, row);
         GSB_CUDA_CHECK(cudaGetLastError());
+        if (defocus_grad != nullptr)
+            GSB_CUDA_CHECK(cudaMemcpyAsync(defocus_grad->grad, row, 2 * sizeof(float), cudaMemcpyDeviceToDevice, stream));
     }
     return GSB_OK;
 }

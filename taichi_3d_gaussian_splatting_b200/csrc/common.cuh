@@ -65,12 +65,15 @@ int resolve_workspace(void *base, int64_t bytes, int64_t N, int32_t n_obj, int64
 struct LensParams;
 struct RsParams;
 struct BlurParams;
+struct DefocusParams;
 // lens: the distortion of gsb200_forward_lens (checked there, r2_max set), or NULL for the pinhole kernel; rs: the rolling
 // shutter of gsb200_forward_rolling_shutter (checked there), or NULL; filter3d: the (N,) 3D smoothing filter of
 // gsb200_forward_filter3d (checked there), or NULL; blur: the exposure motion of gsb200_forward_motion_blur (checked there,
-// never together with filter3d), or NULL
+// never together with filter3d), or NULL; defocus: the thin lens of gsb200_forward_defocus (checked there, never together with
+// filter3d; a NULL blur is then zero motion), or NULL
 int launch_preprocess(const GsbForwardArgs &a, const Workspace &ws, cudaStream_t stream, const LensParams *lens = nullptr,
-                      const RsParams *rs = nullptr, const float *filter3d = nullptr, const BlurParams *blur = nullptr);
+                      const RsParams *rs = nullptr, const float *filter3d = nullptr, const BlurParams *blur = nullptr,
+                      const DefocusParams *defocus = nullptr);
 // the pose blocks of n (q, t) pairs (pose_kernel without the per-frame clears)
 int launch_pose_blocks(const float *q_pc, const float *t_pc, int n, PoseBlock *poses, cudaStream_t stream);
 int launch_sort(const Workspace &ws, int64_t key_capacity, cudaStream_t stream);
@@ -108,9 +111,13 @@ int launch_backward_points_filter(const GsbBackwardArgs &a, const Workspace &ws,
 // gsb200_backward_motion_blur: the BLUR per-point kernel (lens: NULL for a pinhole; rs: NULL for a global shutter), with
 // blur_grad also the motion sums (per-CTA rows in blur_grad->temp) and the rolling-shutter finishing kernel; arguments
 // checked by the caller
+// defocus (gsb200_backward_defocus): the thin lens of the frame, or NULL; defocus_grad (with defocus, never with blur_grad):
+// the (a, rho) sums through the same rows and finishing kernel, the finished row's first two values copied to
+// defocus_grad->grad
 int launch_backward_points_blur(const GsbBackwardArgs &a, const Workspace &ws, cudaStream_t stream, bool depth_grad,
                                 const LensParams *lens, const RsParams *rs, const BlurParams &blur,
-                                const GsbMotionBlurGradArgs *blur_grad);
+                                const GsbMotionBlurGradArgs *blur_grad, const DefocusParams *defocus = nullptr,
+                                const GsbDefocusGradArgs *defocus_grad = nullptr);
 // gsb200_filter3d_from_views (csrc/filter3d.cu; arguments checked by the caller)
 int launch_filter3d_from_views(const GsbFilter3dViewsArgs &a, cudaStream_t stream);
 // gsb200_backward_pose: the POSE per-point kernel (dense gradients as launch_backward_points, plus the per-CTA pose sums
@@ -511,6 +518,37 @@ __device__ __forceinline__ void motion_blur_grad(float s00, float s01, float s11
     gd0 = Gd0 / 6.0f - (g_alpha / 12.0f) * Id0;
     gd1 = Gd1 / 6.0f - (g_alpha / 12.0f) * Id1;
     const float h = 0.5f * g_alpha;
+    g00 += h * (ia * a11 - i00);
+    g01 += h * (-ia * s01 - i01);
+    g11 += h * (ia * a00 - i11);
+}
+#endif
+
+// ---- defocus (gsb200_forward_defocus / gsb200_backward_defocus; definition in include/gsb200.h)
+struct DefocusParams {
+    float aperture = 0.0f;       // a, scene units
+    float inverse_focus = 0.0f;  // rho = 1 / focus distance
+};
+#if defined(__CUDACC__) || defined(GSB_HOST_EMU)
+// beta = a^2 (rho - 1/z)^2 / 16: the per-axis variance, on the normalised image plane, of the aperture disk's image of a point
+// at depth z.  B_d = beta M M^T with M = K[:2,:2] (K[:2,:2] D with a lens).
+__device__ __forceinline__ float defocus_variance(const DefocusParams &f, float z) {
+    const float e = f.inverse_focus - 1.0f / z;
+    return (f.aperture * f.aperture) * (e * e) / 16.0f;
+}
+// The backward of a blur B (the sum of the motion's and the defocus' terms) of one in-camera point: (s00, s01, s11) = Sigma',
+// (b00, b01, b11) = B, g_alpha = G_a; on entry (g00, g01, g11) = G = dL/d(Sigma_d + B), on exit dL/dSigma' = G + G_a/2
+// (Sigma_d^-1 - (Sigma_d + B)^-1); (h00, h01, h11) = G_B = dL/dB = G - G_a/2 (Sigma_d + B)^-1, the c_b term included.
+__device__ __forceinline__ void blur_cov_grad(float s00, float s01, float s11, float b00, float b01, float b11, float g_alpha,
+                                              float &g00, float &g01, float &g11, float &h00, float &h01, float &h11) {
+    const float a00 = s00 + 0.3f, a11 = s11 + 0.3f;  // Sigma_d
+    const float c00 = a00 + b00, c01 = s01 + b01, c11 = a11 + b11;  // Sigma_d + B
+    const float ia = 1.0f / (a00 * a11 - s01 * s01), ib = 1.0f / (c00 * c11 - c01 * c01);
+    const float i00 = ib * c11, i01 = -ib * c01, i11 = ib * c00;  // (Sigma_d + B)^-1
+    const float h = 0.5f * g_alpha;
+    h00 = g00 - h * i00;
+    h01 = g01 - h * i01;
+    h11 = g11 - h * i11;
     g00 += h * (ia * a11 - i00);
     g01 += h * (-ia * s01 - i01);
     g11 += h * (ia * a00 - i11);

@@ -204,10 +204,15 @@ __device__ __forceinline__ bool tile_reachable(const SplatReach &r, float u, flo
 // d = Jp (v + w x pc) with the full position Jacobian Jp at the rendered pc, B = d d^T / 12; the conic is (Sigma_d + B)^-1,
 // the rescale slot holds rescale c_b with c_b = sqrt(det Sigma_d / det(Sigma_d + B)), and the radius comes from Sigma' + B.
 // A view with m = 0 takes the un-blurred arithmetic.  Not with FILTER.
-template <typename KeyT, int LENS, bool ROLLING = false, bool FILTER = false, bool BLUR = false>
+// DEFOCUS = true (with BLUR; gsb200_forward_defocus): B also carries the thin lens' B_d = beta M M^T, beta = a^2 (rho - 1/z)^2
+// / 16 at the rendered z, M = K[:2,:2] (K[:2,:2] D with a lens): B = B_m + B_d, and the conic, c_b, radius and reach follow
+// from Sigma_d + B as above.  A view with a = 0 takes the arithmetic without defocus.
+template <typename KeyT, int LENS, bool ROLLING = false, bool FILTER = false, bool BLUR = false, bool DEFOCUS = false>
 __device__ __forceinline__ void preprocess_body(const PreParams p, const LensParams lens, const RsParams rs = RsParams(),
-                                                const float *filter3d = nullptr, const BlurParams blur = BlurParams()) {
+                                                const float *filter3d = nullptr, const BlurParams blur = BlurParams(),
+                                                const DefocusParams defocus = DefocusParams()) {
     static_assert(!(BLUR && FILTER), "the motion blur is not implemented with the 3D filter");
+    static_assert(!DEFOCUS || BLUR, "the defocus runs on the motion-blur path");
     __shared__ unsigned int s_ticket;
     __shared__ unsigned long long s_warp_sums[SCAN_BLOCK_THREADS / 32];
     __shared__ unsigned long long s_block_exclusive;
@@ -384,7 +389,9 @@ __device__ __forceinline__ void preprocess_body(const PreParams p, const LensPar
             float det = c00 * c11 - c01 * c10;
             const float rescale = sqrtf(fmaxf(0.0f, det_pre / det));
             float blur_c = 1.0f;  // BLUR: the compensation c_b
-            const bool blurred = BLUR && motion_blur_on(blur.motion);
+            const bool moving = BLUR && motion_blur_on(blur.motion);
+            const bool defocused = DEFOCUS && defocus.aperture != 0.0f;
+            const bool blurred = moving || defocused;
             if (blurred) {
                 // Jp = K[:2,:2] D P, the expression of the backward's d uv / d pc
                 float A0 = Kc[0], A1 = Kc[1], A3 = Kc[3], A4 = Kc[4];
@@ -392,12 +399,21 @@ __device__ __forceinline__ void preprocess_body(const PreParams p, const LensPar
                     A0 = Kc[0] * D[0] + Kc[1] * D[2]; A1 = Kc[0] * D[1] + Kc[1] * D[3];
                     A3 = Kc[3] * D[0] + Kc[4] * D[2]; A4 = Kc[3] * D[1] + Kc[4] * D[3];
                 }
-                const float iz = 1.0f / pc[2], iz2 = iz * iz;
-                const float dj[6] = {A0 * iz, A1 * iz, (-A0 * pc[0] - A1 * pc[1]) * iz2,
-                                     A3 * iz, A4 * iz, (-A3 * pc[0] - A4 * pc[1]) * iz2};
-                float d0, d1;
-                motion_blur_velocity(dj, pc, blur.motion, d0, d1);
-                const float b00 = (d0 * d0) / 12.0f, b01 = (d0 * d1) / 12.0f, b11 = (d1 * d1) / 12.0f;
+                float b00 = 0.0f, b01 = 0.0f, b11 = 0.0f;
+                if (moving) {
+                    const float iz = 1.0f / pc[2], iz2 = iz * iz;
+                    const float dj[6] = {A0 * iz, A1 * iz, (-A0 * pc[0] - A1 * pc[1]) * iz2,
+                                         A3 * iz, A4 * iz, (-A3 * pc[0] - A4 * pc[1]) * iz2};
+                    float d0, d1;
+                    motion_blur_velocity(dj, pc, blur.motion, d0, d1);
+                    b00 = (d0 * d0) / 12.0f; b01 = (d0 * d1) / 12.0f; b11 = (d1 * d1) / 12.0f;
+                }
+                if (defocused) {  // + beta M M^T, M = (A0 A1; A3 A4)
+                    const float beta = defocus_variance(defocus, pc[2]);
+                    b00 += beta * (A0 * A0 + A1 * A1);
+                    b01 += beta * (A0 * A3 + A1 * A4);
+                    b11 += beta * (A3 * A3 + A4 * A4);
+                }
                 c00 += b00; c01 += b01; c10 += b01; c11 += b11;
                 cov[0] += b00; cov[1] += b01; cov[2] += b01; cov[3] += b11;  // the radius below: Sigma' + B
                 const float det_b = c00 * c11 - c01 * c10;
@@ -705,14 +721,16 @@ preprocess_rs_filter_kernel(const PreRsFilterParams p) {
 }
 
 // The parameter block of the BLUR instantiations (LENS = GSB_LENS_PINHOLE ignores `lens`, ROLLING = false ignores `rs`).
+// DEFOCUS = false ignores `defocus`.
 struct PreBlurParams : PreRsParams {
     BlurParams blur;
+    DefocusParams defocus;
 };
 
-template <typename KeyT, int LENS, bool ROLLING>
+template <typename KeyT, int LENS, bool ROLLING, bool DEFOCUS = false>
 __global__ void __launch_bounds__(SCAN_BLOCK_THREADS, GSB_PRE_MIN_BLOCKS)
 preprocess_blur_kernel(const PreBlurParams p) {
-    preprocess_body<KeyT, LENS, ROLLING, false, true>(p, p.lens, p.rs, nullptr, p.blur);
+    preprocess_body<KeyT, LENS, ROLLING, false, true, DEFOCUS>(p, p.lens, p.rs, nullptr, p.blur, p.defocus);
 }
 
 #ifndef GSB_HOST_EMU  // tests/simt compiles the kernels above as host C++ under the SIMT emulator
@@ -741,21 +759,21 @@ static void launch_filter_kernel(int model, bool rolling, dim3 grid, dim3 block,
     else preprocess_filter_kernel<KeyT, GSB_LENS_PINHOLE><<<grid, block, 0, stream>>>(pf);
 }
 
-template <typename KeyT>
+template <typename KeyT, bool DEFOCUS>
 static void launch_blur_kernel(int model, bool rolling, dim3 grid, dim3 block, cudaStream_t stream, const PreBlurParams &pb) {
     if (rolling) {
-        if (model == GSB_LENS_FISHEYE) preprocess_blur_kernel<KeyT, GSB_LENS_FISHEYE, true><<<grid, block, 0, stream>>>(pb);
-        else if (model == GSB_LENS_OPENCV) preprocess_blur_kernel<KeyT, GSB_LENS_OPENCV, true><<<grid, block, 0, stream>>>(pb);
-        else preprocess_blur_kernel<KeyT, GSB_LENS_PINHOLE, true><<<grid, block, 0, stream>>>(pb);
+        if (model == GSB_LENS_FISHEYE) preprocess_blur_kernel<KeyT, GSB_LENS_FISHEYE, true, DEFOCUS><<<grid, block, 0, stream>>>(pb);
+        else if (model == GSB_LENS_OPENCV) preprocess_blur_kernel<KeyT, GSB_LENS_OPENCV, true, DEFOCUS><<<grid, block, 0, stream>>>(pb);
+        else preprocess_blur_kernel<KeyT, GSB_LENS_PINHOLE, true, DEFOCUS><<<grid, block, 0, stream>>>(pb);
     } else {
-        if (model == GSB_LENS_FISHEYE) preprocess_blur_kernel<KeyT, GSB_LENS_FISHEYE, false><<<grid, block, 0, stream>>>(pb);
-        else if (model == GSB_LENS_OPENCV) preprocess_blur_kernel<KeyT, GSB_LENS_OPENCV, false><<<grid, block, 0, stream>>>(pb);
-        else preprocess_blur_kernel<KeyT, GSB_LENS_PINHOLE, false><<<grid, block, 0, stream>>>(pb);
+        if (model == GSB_LENS_FISHEYE) preprocess_blur_kernel<KeyT, GSB_LENS_FISHEYE, false, DEFOCUS><<<grid, block, 0, stream>>>(pb);
+        else if (model == GSB_LENS_OPENCV) preprocess_blur_kernel<KeyT, GSB_LENS_OPENCV, false, DEFOCUS><<<grid, block, 0, stream>>>(pb);
+        else preprocess_blur_kernel<KeyT, GSB_LENS_PINHOLE, false, DEFOCUS><<<grid, block, 0, stream>>>(pb);
     }
 }
 
 int launch_preprocess(const GsbForwardArgs &a, const Workspace &ws, cudaStream_t stream, const LensParams *lens,
-                      const RsParams *rs, const float *filter3d, const BlurParams *blur) {
+                      const RsParams *rs, const float *filter3d, const BlurParams *blur, const DefocusParams *defocus) {
     const GsbWorkspaceLayout &L = ws.layout;
     {
         // per-frame state to zero: [counters, sort_state) and [tile_start, zero_bytes) -- every offset is 256-B aligned
@@ -800,16 +818,23 @@ int launch_preprocess(const GsbForwardArgs &a, const Workspace &ws, cudaStream_t
     p.point_in_camera = ws.point_in_camera;
     p.keys = ws.keys_a;
     p.vals = ws.vals_a;
-    if (blur != nullptr) {
+    if (blur != nullptr || defocus != nullptr) {
         PreBlurParams pb;
         static_cast<PreParams &>(pb) = p;
         pb.lens = lens != nullptr ? *lens : LensParams();
         pb.rs = rs != nullptr ? *rs : RsParams();
-        pb.blur = *blur;
+        pb.blur = blur != nullptr ? *blur : BlurParams{};  // zero motion: the defocus alone
+        pb.defocus = defocus != nullptr ? *defocus : DefocusParams();
         const int model = lens != nullptr ? lens->model : GSB_LENS_PINHOLE;
         const dim3 grid(L.scan_blocks), block(SCAN_BLOCK_THREADS);
-        if (L.key_bytes == 4) launch_blur_kernel<unsigned int>(model, rs != nullptr, grid, block, stream, pb);
-        else launch_blur_kernel<unsigned long long>(model, rs != nullptr, grid, block, stream, pb);
+        const bool r = rs != nullptr;
+        if (defocus != nullptr) {
+            if (L.key_bytes == 4) launch_blur_kernel<unsigned int, true>(model, r, grid, block, stream, pb);
+            else launch_blur_kernel<unsigned long long, true>(model, r, grid, block, stream, pb);
+        } else {
+            if (L.key_bytes == 4) launch_blur_kernel<unsigned int, false>(model, r, grid, block, stream, pb);
+            else launch_blur_kernel<unsigned long long, false>(model, r, grid, block, stream, pb);
+        }
     } else if (filter3d != nullptr) {
         PreRsFilterParams pr;
         static_cast<PreParams &>(pr) = p;

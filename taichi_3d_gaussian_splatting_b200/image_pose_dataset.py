@@ -32,6 +32,9 @@ An optional record key ``motion_blur`` (an extension), ``{"linear_velocity": [3]
 "exposure_time": s}``, gives the view's ``CameraInfo.motion_blur`` (``Camera.MotionBlur.from_camera_velocity``: the camera's
 own velocities as for ``rolling_shutter``, and the time the shutter was open).  The motion is in the camera frame, so
 rescaling and autoscale keep it.
+An optional record key ``defocus`` (an extension), ``{"aperture": a, "focus_distance": d}``, gives the view's
+``CameraInfo.defocus`` (``Camera.Defocus``: the aperture diameter and the focus distance in scene units; ``Camera.Defocus.
+from_lens`` converts EXIF values).  Both act on the normalised image plane, so rescaling and autoscale keep them.
 Pinned against the reference class itself: ``tests/golden/make_dataset_golden.py`` imports it (Taichi stubbed) and
 stores its outputs for a small generated dataset; ``tests/test_dataset_cpu.py`` compares.
 """
@@ -43,7 +46,7 @@ import numpy as np
 import torch
 import torch.utils.data
 
-from .Camera import CameraInfo, LensDistortion, MotionBlur, RollingShutter
+from .Camera import CameraInfo, Defocus, LensDistortion, MotionBlur, RollingShutter
 from .GaussianPointCloudRasterisation import TILE_HEIGHT, TILE_WIDTH
 from .loss import SupervisionTargets
 from .utils import SE3_to_quaternion_and_translation_torch
@@ -98,7 +101,8 @@ class ImagePoseDataset(torch.utils.data.Dataset):
         K[1, 2] *= sy
         return resized, CameraInfo(camera_intrinsics=K, camera_height=resized.shape[1], camera_width=resized.shape[2],
                                    camera_id=camera_info.camera_id, distortion=camera_info.distortion,
-                                   rolling_shutter=camera_info.rolling_shutter, motion_blur=camera_info.motion_blur)
+                                   rolling_shutter=camera_info.rolling_shutter, motion_blur=camera_info.motion_blur,
+                                   defocus=camera_info.defocus)
 
     @staticmethod
     def _distortion(rec: dict) -> Optional[LensDistortion]:
@@ -137,6 +141,16 @@ class ImagePoseDataset(torch.utils.data.Dataset):
         if len(r["linear_velocity"]) != 3 or len(r["angular_velocity"]) != 3:
             raise ValueError(f'"motion_blur" velocities take 3 values each, got {r!r}')
         return MotionBlur.from_camera_velocity(r["linear_velocity"], r["angular_velocity"], r["exposure_time"])
+
+    @staticmethod
+    def _defocus(rec: dict) -> Optional[Defocus]:
+        """The optional record key ``"defocus": {"aperture": a, "focus_distance": d}`` (scene units)."""
+        r = rec.get("defocus")
+        if r is None:
+            return None
+        if not isinstance(r, dict) or any(k not in r for k in ("aperture", "focus_distance")):
+            raise ValueError(f'"defocus" must be {{"aperture": a, "focus_distance": d}}, got {r!r}')
+        return Defocus(r["aperture"], r["focus_distance"])
 
     def _path(self, path: str) -> str:
         if not os.path.isabs(path) and not os.path.exists(path):
@@ -238,7 +252,8 @@ class ImagePoseDataset(torch.utils.data.Dataset):
         image = _crop_to_tiles(image)
         info = CameraInfo(camera_intrinsics=K, camera_height=image.shape[1], camera_width=image.shape[2],
                           camera_id=rec["camera_id"], distortion=self._distortion(rec),
-                          rolling_shutter=self._rolling_shutter(rec), motion_blur=self._motion_blur(rec))
+                          rolling_shutter=self._rolling_shutter(rec), motion_blur=self._motion_blur(rec),
+                          defocus=self._defocus(rec))
         image, info = self._autoscale_image_and_camera_info(image, info)
         if self.with_targets:
             return image, q, t, info, self._crop_and_scale_targets(*targets, info)

@@ -30,7 +30,7 @@ class SyntheticScene:
             self.point_cloud.to(device), self.point_cloud_features.to(device),
             self.point_invalid_mask.to(device), self.point_object_id.to(device),
             CameraInfo(ci.camera_intrinsics.to(device), ci.camera_height, ci.camera_width, ci.camera_id, ci.distortion,
-                       ci.rolling_shutter, ci.motion_blur),
+                       ci.rolling_shutter, ci.motion_blur, ci.defocus),
             self.q_pointcloud_camera.to(device), self.t_pointcloud_camera.to(device))
 
 

@@ -35,6 +35,12 @@ exposure-motion refinement (``TrainConfig.motion_blur_learning_rate``): per blur
 differentiated by the operator's ``differentiable_motion_blur`` and stepped by its own Adam; it needs a non-zero start (the
 gradient vanishes at zero motion), e.g. ``Camera.MotionBlur.between_poses`` of the neighbouring frames.  ``validation``
 renders every view as its camera says: blurred views blurred.
+Views with depth of field (an extension; ``CameraInfo.defocus``) train through it in the autograd loop, with or without a lens,
+a rolling shutter and motion blur; the downsampled camera keeps (a, rho) (they act on the normalised image plane).  Not with
+``fused_step``, ``mip_filter_3d``, pose, intrinsics, lens, rolling-shutter motion or exposure-motion refinement, or the
+view-parallel exchange.  Optional defocus refinement (``TrainConfig.defocus_learning_rate``): per defocused view, its (a, rho),
+differentiated by the operator's ``differentiable_defocus`` and stepped by its own Adam; it needs a non-zero aperture (both
+gradients vanish at a = 0).  ``validation`` renders every view as its camera says: defocused views defocused.
 Optional appearance compensation (an extension; ``TrainConfig.appearance_grid``): one bilateral grid per training view
 (``appearance.apply_bilateral_grid``), initialised to the identity, slices the image the image loss sees (after the
 background composite), with a TV prior and its own Adam that steps only the visited view's grid.  It acts on the image alone,
@@ -61,7 +67,7 @@ import torch
 import torch.nn.functional as F
 
 from .appearance import apply_bilateral_grid, bilateral_grid_tv, check_grid_shape, identity_grids
-from .Camera import CameraInfo, LensDistortion, MotionBlur, RollingShutter
+from .Camera import CameraInfo, Defocus, LensDistortion, MotionBlur, RollingShutter
 from .densification import GaussianPointAdaptiveController
 from .GaussianPointCloudRasterisation import GaussianPointCloudRasterisation
 from .loss import (FEATURE_LOSSES, LossFunction, RobustLossConfig, SupervisionTargets, feature_loss, mcmc_regulariser,
@@ -93,11 +99,12 @@ def downsample_image_and_camera_info(image: torch.Tensor, camera_info: CameraInf
     K[1, 1] /= downsample_factor
     K[0, 2] /= downsample_factor
     K[1, 2] /= downsample_factor
-    # the lens coefficients act on the normalised image plane, row time is normalised by the height and the exposure motion
-    # is in the camera frame: resizing changes neither the lens, the rolling-shutter motion nor the exposure motion
+    # the lens coefficients and the thin lens act on the normalised image plane, row time is normalised by the height and the
+    # exposure motion is in the camera frame: resizing changes neither the lens, the rolling-shutter motion, the exposure
+    # motion nor the defocus
     return image, CameraInfo(camera_intrinsics=K, camera_height=h, camera_width=w, camera_id=camera_info.camera_id,
                              distortion=camera_info.distortion, rolling_shutter=camera_info.rolling_shutter,
-                             motion_blur=camera_info.motion_blur)
+                             motion_blur=camera_info.motion_blur, defocus=camera_info.defocus)
 
 
 def _nearest(x: torch.Tensor, h: int, w: int, hc: int, wc: int) -> torch.Tensor:
@@ -195,6 +202,11 @@ class GaussianPointCloudTrainer:
         # Adam at this rate.  The start must not be zero (the blur's gradient vanishes there).  Not with fused_step,
         # mip_filter_3d, pose, intrinsics, lens or rolling-shutter motion refinement.
         motion_blur_learning_rate: float = 0.
+        # optional defocus refinement: > 0 gives every training view with depth of field (CameraInfo.defocus) one (2,) leaf
+        # tensor of its (a, rho), initialised from the view's, kept on the host and trained by its own Adam at this rate.  The
+        # aperture must not start at zero (both gradients vanish there).  Not with fused_step, mip_filter_3d, pose,
+        # intrinsics, lens, rolling-shutter motion or exposure-motion refinement.
+        defocus_learning_rate: float = 0.
         # optional appearance compensation: (Gx, Gy, Gz) gives every training view one bilateral grid of that many nodes
         # (1 <= Gx, Gy <= 64, 1 <= Gz <= 16; (1, 1, 1) is a per-view affine colour transform), initialised to the identity
         # and trained by its own Adam at appearance_learning_rate with a TV prior of weight appearance_tv_weight.  The
@@ -310,6 +322,19 @@ class GaussianPointCloudTrainer:
                     raise ValueError(f"{name} is not supported with a motion-blurred view (CameraInfo.motion_blur)")
         self._motion_blur = self._motion_blur_leaves(config, train_views)
         self._mb = config.motion_blur_learning_rate > 0
+        # a view with depth of field (CameraInfo.defocus) trains through the autograd loop alone
+        self._defocused = any(getattr(v[3], "defocus", None) is not None for v in train_views)
+        if self._defocused:
+            for name, on in (("fused_step", fused_step), ("mip_filter_3d", bool(config.mip_filter_3d)),
+                             ("pose refinement (pose_learning_rate > 0)", self._pose),
+                             ("intrinsics refinement (intrinsics_learning_rate > 0)", self._intr),
+                             ("distortion refinement (distortion_learning_rate > 0)", self._dist),
+                             ("motion refinement (rolling_shutter_learning_rate > 0)", self._rs),
+                             ("exposure-motion refinement (motion_blur_learning_rate > 0)", self._mb)):
+                if on:
+                    raise ValueError(f"{name} is not supported with a defocused view (CameraInfo.defocus)")
+        self._defocus = self._defocus_leaves(config, train_views)
+        self._df = config.defocus_learning_rate > 0
         self._mip = bool(config.mip_filter_3d)
         self._filter_3d = None
         if self._mip:
@@ -387,12 +412,15 @@ class GaussianPointCloudTrainer:
                      **({"differentiable_intrinsics": True} if self._intr else {}),
                      **({"differentiable_distortion": True} if self._dist else {}),
                      **({"differentiable_rolling_shutter": True} if self._rs else {}),
-                     **({"differentiable_motion_blur": True} if self._mb else {}))
+                     **({"differentiable_motion_blur": True} if self._mb else {}),
+                     **({"differentiable_defocus": True} if self._df else {}))
         self.rasterisation = factory(config=config.rasterisation_config,
                                      backward_valid_point_hook=None if self._mcmc else self.adaptive_controller.update,
                                      **extra)
         if self._mcmc and getattr(self.rasterisation, "gradient_exchange", None) is not None:
             raise ValueError('densification="mcmc" is not implemented for the view-parallel gradient exchange')
+        if self._defocused and getattr(self.rasterisation, "gradient_exchange", None) is not None:
+            raise ValueError("a defocused view (CameraInfo.defocus) is not supported with the view-parallel gradient exchange")
         if self._blurred and getattr(self.rasterisation, "gradient_exchange", None) is not None:
             raise ValueError("a motion-blurred view (CameraInfo.motion_blur) is not supported with the view-parallel "
                              "gradient exchange")
@@ -442,6 +470,21 @@ class GaussianPointCloudTrainer:
         if not leaves:
             raise ValueError("rolling_shutter_learning_rate > 0 needs a rolling-shutter training view "
                              "(CameraInfo.rolling_shutter)")
+        return leaves
+
+    @staticmethod
+    def _defocus_leaves(config, train_views: List[View]) -> dict:
+        """The trainable thin lenses, one float32 host leaf (a, rho) per defocused view, keyed by view index ({} when defocus
+        refinement is off)."""
+        rate = config.defocus_learning_rate
+        if not (rate >= 0.0 and rate < float("inf")):
+            raise ValueError(f"defocus_learning_rate must be finite and >= 0, got {rate}")
+        if rate == 0:
+            return {}
+        leaves = {i: torch.tensor(v[3].defocus.parameters, dtype=torch.float32, requires_grad=True)
+                  for i, v in enumerate(train_views) if getattr(v[3], "defocus", None) is not None}
+        if not leaves:
+            raise ValueError("defocus_learning_rate > 0 needs a defocused training view (CameraInfo.defocus)")
         return leaves
 
     @staticmethod
@@ -678,6 +721,8 @@ class GaussianPointCloudTrainer:
             if self._rs else None
         motion_blur_optimizer = torch.optim.Adam(list(self._motion_blur.values()), lr=cfg.motion_blur_learning_rate,
                                                  betas=(0.9, 0.999)) if self._mb else None
+        defocus_optimizer = torch.optim.Adam(list(self._defocus.values()), lr=cfg.defocus_learning_rate,
+                                             betas=(0.9, 0.999)) if self._df else None
         appearance_optimizer = Adam(self._appearance_leaves, lr=cfg.appearance_learning_rate, betas=(0.9, 0.999)) \
             if self._appearance else None
         scheduler = torch.optim.lr_scheduler.ExponentialLR(position_optimizer, gamma=cfg.position_learning_rate_decay_rate)
@@ -701,6 +746,8 @@ class GaussianPointCloudTrainer:
                 rolling_shutter_optimizer.zero_grad()
             if motion_blur_optimizer is not None:
                 motion_blur_optimizer.zero_grad()
+            if defocus_optimizer is not None:
+                defocus_optimizer.zero_grad()
             if appearance_optimizer is not None:
                 appearance_optimizer.zero_grad()
             view_index = self._next_view_index(iteration)
@@ -734,6 +781,8 @@ class GaussianPointCloudTrainer:
                                          rolling_shutter=camera_info.rolling_shutter,
                                          motion_blur=MotionBlur(values[:3], values[3:]))
                 lens_kw = {"exposure_motion": leaf}
+            if self._df and view_index in self._defocus:  # the leaf's values are rendered, and it is the autograd input
+                lens_kw = {"defocus_parameters": self._defocus[view_index]}
             band = iteration // cfg.increase_color_max_sh_band_interval
             if self.supervised or self._features or self._appearance or self._weighted:
                 robust_active = cfg.robust_loss is not None and iteration >= cfg.robust_loss.start_iteration
@@ -774,6 +823,8 @@ class GaussianPointCloudTrainer:
                 rolling_shutter_optimizer.step()
             if motion_blur_optimizer is not None:
                 motion_blur_optimizer.step()
+            if defocus_optimizer is not None:
+                defocus_optimizer.step()
             if appearance_optimizer is not None:
                 appearance_optimizer.step()
             if self._mcmc:  # the noise of iteration t at the position learning rate its optimiser step used
@@ -911,6 +962,19 @@ class GaussianPointCloudTrainer:
                 values = self._motion_blur[i].detach().tolist()
                 mb = MotionBlur(values[:3], values[3:])
             out.append(mb)
+        return out
+
+    def refined_defocus(self) -> List[Optional[Defocus]]:
+        """The defocus of every training view as trained (None for a view without one; the views' own without defocus
+        refinement): Defocus(|a|, 1 / rho), with a focus at infinity for rho <= 0 (a focus beyond infinity is the nearest
+        physical thin lens)."""
+        out = []
+        for i, v in enumerate(self.train_views):
+            d = getattr(v[3], "defocus", None)
+            if d is not None and i in self._defocus:
+                a, rho = self._defocus[i].detach().tolist()
+                d = Defocus(abs(a), 1.0 / rho if rho > 0.0 else math.inf)
+            out.append(d)
         return out
 
     @torch.no_grad()
