@@ -391,6 +391,36 @@ int gsb200_backward_lens(const GsbBackwardArgs *args, const float *grad_rasteriz
                          const float *grad_pixel_accumulated_alpha, const GsbExtraFeatureArgs *ext,
                          const GsbLensArgs *lens);  /* or NULL */
 
+/* Equirectangular 360-degree panoramas (an extension: the reference projects through a pinhole).  Camera frame as everywhere
+ * (x right, y down, z forward).  With rho = sqrt(x^2 + z^2) and r = sqrt(rho^2 + y^2):
+ *   lon = atan2(x, z),  lat = atan2(y, rho),  u = K00 lon + K02 reduced into [0, W),  v = K11 lat + K12.
+ * A full panorama has K00 = W / 2pi, K11 = H / pi, K02 = W / 2, K12 = H / 2; the image centre looks along +z.
+ * Covariance: Sigma' = J W Sigma W^T J^T with J = diag(K00, K11) [z/rho^2 0 -x/rho^2; -x y/(r^2 rho) rho/r^2 -z y/(r^2 rho)]
+ * (the local affine projection); the 0.3 low-pass, rescale, 3-sigma radius and reach filter are the pinhole's.
+ * In view: near < r < far and rho > GSB_EQUIRECT_POLE_EPSILON r (a cone of half-angle ~0.057 degrees around each pole, where
+ * lon is undefined, is culled).  Points behind the camera are in view.  The depth is the ray distance r: in the sort key,
+ * the record's depth slot, the depth output and the hook's point_depth.
+ * Seam: the footprint's tile columns are not clamped to the image; a footprint wider than the panorama is cut to the W/16
+ * columns whose centres lie within W/2 of u.  The reach filter runs in these unwrapped columns, and the key's tile column is
+ * taken modulo W/16.  The blend kernels stage each splat at the copy of u nearest the tile's centre column,
+ * u + W rint((tile centre - u) / W); the per-pixel arithmetic is unchanged, and dL/du does not change under the shift.
+ * Gradients: d(u, v)/d pc = J exactly (J's dependence on pc detached inside Sigma', as for every model); the depth gradient
+ * enters pc along pc / r.  Known limit: the affine approximation degrades towards the poles, where a Gaussian is drawn across
+ * up to the full width of its rows; outputs and gradients stay finite there. */
+#define GSB_EQUIRECT_POLE_EPSILON 1e-3f
+/* |2 pi K00 - W| <= GSB_EQUIRECT_FX_TOLERANCE W: the panorama covers 360 degrees */
+#define GSB_EQUIRECT_FX_TOLERANCE 1e-4f
+/* gsb200_forward_ext of an equirectangular view.  Before any kernel runs: GSB_EINVAL when W is not a multiple of 16 or for
+ * the checks of gsb200_forward_ext; then K (device memory, like every call's) is read back -- 36 bytes and one
+ * synchronisation of args->stream -- and GSB_EINVAL when |2 pi K00 - W| > GSB_EQUIRECT_FX_TOLERANCE W, K01 or K10 is not 0,
+ * K's last row is not (0, 0, 1), or an entry is not finite. */
+int gsb200_forward_equirect(const GsbForwardArgs *args, const GsbExtraFeatureArgs *ext);
+/* gsb200_backward_ext of a frame rendered by gsb200_forward_equirect.  The checks of gsb200_forward_equirect, and before any
+ * CUDA call GSB_EUNSUPPORTED with GSB_FLAG_COMPACT_GRADS (the view-parallel exchange) or without
+ * GSB_FLAG_BACKWARD_TRANSPOSED (the butterfly loop A does not wrap the seam). */
+int gsb200_backward_equirect(const GsbBackwardArgs *args, const float *grad_rasterized_depth, const float *rasterized_depth,
+                             const float *grad_pixel_accumulated_alpha, const GsbExtraFeatureArgs *ext);
+
 /* Lens-coefficient gradients (an extension).  The forward is gsb200_forward_lens, unchanged; it reads the coefficients in
  * two places: the position u = K00 xd + K01 yd + K02, v = K10 xd + K11 yd + K12, and D = d(xd, yd)/d(xn, yn) inside
  * J = diag(fx, fy) D P, Sigma' = (J W) Sigma (J W)^T.  The coefficient gradient is the exact derivative through both, under

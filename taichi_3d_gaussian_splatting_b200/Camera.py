@@ -14,7 +14,7 @@ from typing import Optional, Sequence, Tuple
 
 import torch
 
-_LENS_COEFFICIENTS = {"opencv": 5, "fisheye": 4}
+_LENS_COEFFICIENTS = {"opencv": 5, "fisheye": 4, "equirectangular": 0}
 
 
 @dataclass(frozen=True)
@@ -25,7 +25,12 @@ class LensDistortion:
     ``model``: ``"opencv"`` -- coefficients ``(k1, k2, p1, p2, k3)`` in OpenCV's ``distCoeffs`` order (COLMAP
     ``SIMPLE_RADIAL``, ``RADIAL``, ``OPENCV``) -- or ``"fisheye"`` -- ``(k1, k2, k3, k4)`` of the equidistant model (COLMAP
     ``OPENCV_FISHEYE``, ``cv2.fisheye``).  The coefficients act on the normalised image plane (x/z, y/z), so resizing or
-    cropping an image changes K but not them."""
+    cropping an image changes K but not them.
+
+    ``"equirectangular"`` (no coefficients) is the 360-degree panorama of Insta360, Ricoh Theta, GoPro Max and drone panorama
+    modes: u = fx atan2(x, z) + cx (wrapped into [0, W)), v = fy atan2(y, sqrt(x^2 + z^2)) + cy, with 2 pi fx = W (definition in
+    ``include/gsb200.h``; K from ``equirectangular_intrinsics``).  It renders and trains the point gradients only: no pose,
+    intrinsics or lens gradient, rolling shutter, motion blur, defocus, 3D filter or view-parallel exchange."""
     model: str
     coefficients: Tuple[float, ...]
 
@@ -38,6 +43,16 @@ class LensDistortion:
         if not all(math.isfinite(v) for v in co):
             raise ValueError(f"lens coefficients must be finite, got {co}")
         object.__setattr__(self, "coefficients", co)
+
+    @staticmethod
+    def equirectangular_intrinsics(width: int, height: int) -> torch.Tensor:
+        """K (3,3) float32 of a full equirectangular panorama: fx = W / 2pi, fy = H / pi, (cx, cy) = (W / 2, H / 2), so the image
+        spans 360 x 180 degrees and its centre looks along +z."""
+        w, h = int(width), int(height)
+        if w <= 0 or h <= 0:
+            raise ValueError(f"width and height must be positive, got {width} x {height}")
+        return torch.tensor([[w / (2.0 * math.pi), 0.0, w / 2.0], [0.0, h / math.pi, h / 2.0], [0.0, 0.0, 1.0]],
+                            dtype=torch.float32)
 
     @staticmethod
     def from_colmap(model_name: str, params: Sequence[float]) -> Tuple[torch.Tensor, Optional["LensDistortion"]]:

@@ -39,6 +39,16 @@ _RECORD_FLOATS = 12
 _ACCUM_FLOATS = 12
 
 
+# The lens argument of an equirectangular view: it has no GsbLensArgs and goes through gsb200_forward_equirect /
+# gsb200_backward_equirect
+_EQUIRECT = "equirectangular"
+
+
+def _is_equirect(camera_info) -> bool:
+    distortion = getattr(camera_info, "distortion", None)
+    return distortion is not None and distortion.model == "equirectangular"
+
+
 def _ptr(t: Optional[torch.Tensor]) -> Optional[int]:
     return None if t is None else t.data_ptr()
 
@@ -656,7 +666,10 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                         host_counters=pinned.data_ptr(), host_counters_event=event.cuda_event)
                     # The whole frame is enqueued by this one call; the library copies {M, K, overflow} to pinned
                     # host memory right after the per-point stage and records `event` behind that copy.
-                    if defocus is not None:
+                    if lens is _EQUIRECT:
+                        _lib.check(lib.gsb200_forward_equirect(ctypes.byref(args), ctypes.byref(ext) if ext is not None else None),
+                                   "gsb200_forward_equirect")
+                    elif defocus is not None:
                         _lib.check(lib.gsb200_forward_defocus(
                             ctypes.byref(args), ctypes.byref(ext) if ext is not None else None,
                             ctypes.byref(lens) if lens is not None else None, ctypes.byref(rs) if rs is not None else None,
@@ -715,6 +728,9 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                 raise ValueError("lens_coefficients was given for a camera with no lens (camera_info.distortion is None)")
         if distortion is None:
             return None
+        if distortion.model == "equirectangular":
+            self._check_equirect(camera_info, lens_coefficients)
+            return _EQUIRECT
         for name, on in (("differentiable_pose", self.differentiable_pose),
                          ("differentiable_intrinsics", self.differentiable_intrinsics),
                          ("a gradient_exchange", self.gradient_exchange is not None)):
@@ -732,6 +748,31 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
             raise ValueError(f"lens_coefficients must be float32, got {lens_coefficients.dtype}")
         values = lens_coefficients.detach().cpu().tolist()
         return _lib.lens_args(type(distortion)(distortion.model, values))
+
+    def _check_equirect(self, camera_info, lens_coefficients=None, rolling_shutter_motion=None, point_filter_3d=None,
+                        exposure_motion=None, defocus_parameters=None) -> None:
+        """``ValueError`` for what an equirectangular view does not combine with (include/gsb200.h): camera-parameter
+        gradients, the other camera extensions, the 3D filter, the view-parallel exchange and the butterfly backward."""
+        for name, on in (("differentiable_pose", self.differentiable_pose),
+                         ("differentiable_intrinsics", self.differentiable_intrinsics),
+                         ("differentiable_distortion", self.differentiable_distortion),
+                         ("differentiable_rolling_shutter", self.differentiable_rolling_shutter),
+                         ("differentiable_motion_blur", self.differentiable_motion_blur),
+                         ("differentiable_defocus", self.differentiable_defocus),
+                         ("a gradient_exchange", self.gradient_exchange is not None),
+                         ("backward_impl='butterfly'", self.backward_impl == "butterfly"),
+                         ("a rolling shutter (camera_info.rolling_shutter)", getattr(camera_info, "rolling_shutter", None) is not None),
+                         ("motion blur (camera_info.motion_blur)", getattr(camera_info, "motion_blur", None) is not None),
+                         ("defocus (camera_info.defocus)", getattr(camera_info, "defocus", None) is not None),
+                         ("lens_coefficients", lens_coefficients is not None),
+                         ("rolling_shutter_motion", rolling_shutter_motion is not None),
+                         ("point_filter_3d", point_filter_3d is not None),
+                         ("exposure_motion", exposure_motion is not None),
+                         ("defocus_parameters", defocus_parameters is not None)):
+            if on:
+                raise ValueError(f"an equirectangular camera is not supported with {name}")
+        if int(camera_info.camera_width) % TILE_WIDTH != 0:
+            raise ValueError(f"an equirectangular view's width must be a multiple of {TILE_WIDTH}, got {camera_info.camera_width}")
 
     def _rolling_shutter_args(self, camera_info, motion=None) -> Optional[_lib.GsbRollingShutterArgs]:
         """The C rolling-shutter argument of ``camera_info.rolling_shutter`` (None: the global-shutter kernels; row_time is
@@ -911,7 +952,16 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                 grad_extra_features = torch.zeros((N, C), dtype=torch.float32, device=device) if grad_feature_map is None \
                     else torch.empty((N, C), dtype=torch.float32, device=device)
             grad_q = grad_t = grad_K = grad_k = grad_m = grad_b = grad_d = None
-            if ctx.defocus is not None:  # no other camera-parameter gradient (refused in forward)
+            if ctx.lens is _EQUIRECT:  # no camera-parameter gradient or other extension (refused in forward)
+                ext = None
+                if extra_features is not None and grad_feature_map is not None:
+                    grad_map = _f32(grad_feature_map)
+                    ext = _lib.GsbExtraFeatureArgs(channels=extra_features.shape[1], features=_ptr(extra_features),
+                                                   grad_rasterized=_ptr(grad_map), grad_features=_ptr(grad_extra_features))
+                _lib.check(lib.gsb200_backward_equirect(ctypes.byref(args), _ptr(grad_depth), _ptr(depth), _ptr(grad_alpha),
+                                                        ctypes.byref(ext) if ext is not None else None),
+                           "gsb200_backward_equirect")
+            elif ctx.defocus is not None:  # no other camera-parameter gradient (refused in forward)
                 ext = None
                 if extra_features is not None and grad_feature_map is not None:
                     grad_map = _f32(grad_feature_map)
@@ -1085,7 +1135,7 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                     num_overlap_tiles=frame.num_overlap_tiles,
                     num_affected_pixels=acc[:, 10].round().to(torch.int32),
                     point_uv_in_camera=frame.point_uv.contiguous(),
-                    point_depth=frame.point_in_camera[:, 2],
+                    point_depth=frame.records[:, 7] if ctx.lens is _EQUIRECT else frame.point_in_camera[:, 2],
                 ))
         return grad_pointcloud, grad_pointcloud_features, grad_extra_features, grad_q, grad_t, grad_K, grad_k, grad_m, grad_b, \
             grad_d
@@ -1165,6 +1215,9 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
         backward returns dL/d ``defocus_parameters`` on the tensor's device.  ``ValueError`` for a camera without defocus, a
         tensor of the wrong shape or dtype, or an operator without the option.  None: no defocus gradient."""
         camera_info = input_data.camera_info
+        if _is_equirect(camera_info):  # the argument checks, before any device work
+            self._check_equirect(camera_info, lens_coefficients, rolling_shutter_motion, point_filter_3d, exposure_motion,
+                                 defocus_parameters)
         assert camera_info.camera_width % TILE_WIDTH == 0
         assert camera_info.camera_height % TILE_HEIGHT == 0
         if getattr(camera_info, "defocus", None) is not None or defocus_parameters is not None:

@@ -203,7 +203,8 @@ class GsbFilter3dViewsArgs(ctypes.Structure):
 
 
 def lens_args(distortion) -> GsbLensArgs:
-    """The C argument of a ``Camera.LensDistortion`` (host floats; unused coefficients 0)."""
+    """The C argument of a ``Camera.LensDistortion`` (host floats; unused coefficients 0).  The equirectangular model has
+    none: it goes through ``gsb200_forward_equirect`` / ``gsb200_backward_equirect``."""
     model = {"opencv": GSB_LENS_OPENCV, "fisheye": GSB_LENS_FISHEYE}[distortion.model]
     co = list(distortion.coefficients) + [0.0] * (5 - len(distortion.coefficients))
     return GsbLensArgs(model=model, coefficients=(c_f32 * 5)(*co))
@@ -242,6 +243,7 @@ EXPORTS = (
     "gsb200_robust_image_loss", "gsb200_train_step_robust", "gsb200_abi_sizes_robust", "gsb200_forward_motion_blur",
     "gsb200_backward_motion_blur", "gsb200_motion_blur_grad_temp_bytes", "gsb200_abi_sizes_motion_blur",
     "gsb200_forward_defocus", "gsb200_backward_defocus", "gsb200_defocus_grad_temp_bytes", "gsb200_abi_sizes_defocus",
+    "gsb200_forward_equirect", "gsb200_backward_equirect",
 )
 
 _lib = None
@@ -289,6 +291,11 @@ def load() -> ctypes.CDLL:
     lib.gsb200_backward_lens.argtypes = [ctypes.POINTER(GsbBackwardArgs), c_vp, c_vp, c_vp, ctypes.POINTER(GsbExtraFeatureArgs),
                                          ctypes.POINTER(GsbLensArgs)]
     lib.gsb200_backward_lens.restype = ctypes.c_int
+    lib.gsb200_forward_equirect.argtypes = [ctypes.POINTER(GsbForwardArgs), ctypes.POINTER(GsbExtraFeatureArgs)]
+    lib.gsb200_forward_equirect.restype = ctypes.c_int
+    lib.gsb200_backward_equirect.argtypes = [ctypes.POINTER(GsbBackwardArgs), c_vp, c_vp, c_vp,
+                                             ctypes.POINTER(GsbExtraFeatureArgs)]
+    lib.gsb200_backward_equirect.restype = ctypes.c_int
     lib.gsb200_backward_lens_grad.argtypes = [ctypes.POINTER(GsbBackwardArgs), c_vp, c_vp, c_vp,
                                               ctypes.POINTER(GsbExtraFeatureArgs), ctypes.POINTER(GsbLensArgs),
                                               ctypes.POINTER(GsbLensGradArgs)]

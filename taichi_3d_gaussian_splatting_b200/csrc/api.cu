@@ -1,4 +1,5 @@
 // api.cu -- extern "C" entry points of libgsb200.so (see include/gsb200.h).
+#include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
@@ -458,8 +459,10 @@ static int forward_checked(const GsbForwardArgs *a, const GsbExtraFeatureArgs *e
     return launch_blend_forward(*a, ws, st, ext);
 }
 
+static int check_equirect_intrinsics(const char *what, const float *K_dev, int W, void *stream);
+
 // grad_depth / depth: both NULL (no depth term), or both set; grad_alpha: NULL (no alpha term) or set; ext: NULL (no feature
-// term) or set.  The auxiliary terms are checked in gsb200_backward_ext.
+// term) or set; equirect: the WRAP loop A and the EQUI per-point kernel of gsb200_backward_equirect (checked there).  The auxiliary terms are checked in gsb200_backward_ext.
 static int backward_impl(const GsbBackwardArgs *a, bool skip_on_overflow, const float *grad_depth = nullptr,
                          const float *depth = nullptr, const float *grad_alpha = nullptr,
                          const GsbExtraFeatureArgs *ext = nullptr, const GsbPoseGradArgs *pose = nullptr,
@@ -467,7 +470,8 @@ static int backward_impl(const GsbBackwardArgs *a, bool skip_on_overflow, const 
                          const GsbLensGradArgs *lens_grad = nullptr, const RsParams *rs = nullptr,
                          const GsbRollingShutterGradArgs *rs_grad = nullptr, const float *filter3d = nullptr,
                          const BlurParams *blur = nullptr, const GsbMotionBlurGradArgs *blur_grad = nullptr,
-                         const DefocusParams *defocus = nullptr, const GsbDefocusGradArgs *defocus_grad = nullptr) {
+                         const DefocusParams *defocus = nullptr, const GsbDefocusGradArgs *defocus_grad = nullptr,
+                         bool equirect = false) {
     if (!a) {
         set_error("backward: args is null");
         return GSB_EINVAL;
@@ -515,12 +519,15 @@ static int backward_impl(const GsbBackwardArgs *a, bool skip_on_overflow, const 
                                a->key_capacity, a->camera_height, a->camera_width, a->far_plane,
                                a->depth_to_sort_key_scale, a->flags, &ws);
     if (rc != GSB_OK) return rc;
+    if (equirect && (rc = check_equirect_intrinsics("backward_equirect", a->camera_intrinsics, a->camera_width, a->stream)) != GSB_OK)
+        return rc;
     cudaStream_t st = static_cast<cudaStream_t>(a->stream);
     if (a->accum_rows > 0)
         GSB_CUDA_CHECK(cudaMemsetAsync(a->accum, 0, (size_t)a->accum_rows * GSB_ACCUM_FLOATS * 4, st));
     if (ext && a->num_points > 0)  // the blend adds into the rows it reaches; every other row stays zero
         GSB_CUDA_CHECK(cudaMemsetAsync(ext->grad_features, 0, (size_t)a->num_points * ext->channels * 4, st));
-    if ((rc = launch_blend_backward(*a, ws, st, grad_depth, depth, grad_alpha, ext)) != GSB_OK) return rc;
+    if ((rc = launch_blend_backward(*a, ws, st, grad_depth, depth, grad_alpha, ext, equirect)) != GSB_OK) return rc;
+    if (equirect) return launch_backward_points_equirect(*a, ws, st, grad_depth != nullptr);
     if (defocus)  // a NULL blur is zero motion
         return launch_backward_points_blur(*a, ws, st, grad_depth != nullptr, lens, rs, blur ? *blur : BlurParams{}, nullptr,
                                            defocus, defocus_grad);
@@ -858,6 +865,118 @@ static int backward_checked(const GsbBackwardArgs *a, const float *grad_rasteriz
     }
     return backward_impl(a, false, grad_rasterized_depth, rasterized_depth, grad_pixel_accumulated_alpha, ext, pose, intr, lens,
                          lens_grad, rs, rs_grad, filter3d, blur, blur_grad, defocus, defocus_grad);
+}
+
+// The intrinsics of an equirectangular view (include/gsb200.h), read back from the device: 2 pi K00 = W within
+// GSB_EQUIRECT_FX_TOLERANCE, no skew, last row (0, 0, 1), every entry finite.  LensParams{LENS_EQUIRECT} selects the kernels.
+static int check_equirect_intrinsics(const char *what, const float *K_dev, int W, void *stream) {
+    float K[9];
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    GSB_CUDA_CHECK(cudaMemcpyAsync(K, K_dev, sizeof(K), cudaMemcpyDeviceToHost, st));
+    GSB_CUDA_CHECK(cudaStreamSynchronize(st));
+    for (int i = 0; i < 9; ++i)
+        if (!(K[i] - K[i] == 0.0f)) {
+            set_error("%s: camera_intrinsics[%d] is not finite", what, i);
+            return GSB_EINVAL;
+        }
+    if (K[1] != 0.0f || K[3] != 0.0f) {
+        set_error("%s: the equirectangular camera has no skew (K01 = %g, K10 = %g)", what, (double)K[1], (double)K[3]);
+        return GSB_EINVAL;
+    }
+    if (K[6] != 0.0f || K[7] != 0.0f || K[8] != 1.0f) {
+        set_error("%s: K's last row must be (0, 0, 1)", what);
+        return GSB_EINVAL;
+    }
+    const double full = 2.0 * 3.14159265358979323846 * (double)K[0];
+    if (!(fabs(full - (double)W) <= (double)GSB_EQUIRECT_FX_TOLERANCE * (double)W)) {
+        set_error("%s: 2 pi K00 = %g must equal the width %d (a full 360-degree panorama, tolerance %g W)", what, full, W,
+                  (double)GSB_EQUIRECT_FX_TOLERANCE);
+        return GSB_EINVAL;
+    }
+    return GSB_OK;
+}
+
+static int check_equirect_width(const char *what, int W) {
+    if (W <= 0 || W % GSB_TILE_WIDTH != 0) {
+        set_error("%s: the panorama's width must be a positive multiple of %d (got %d)", what, GSB_TILE_WIDTH, W);
+        return GSB_EINVAL;
+    }
+    return GSB_OK;
+}
+
+int gsb200_forward_equirect(const GsbForwardArgs *a, const GsbExtraFeatureArgs *ext) {
+    int rc = check_forward_args(a);
+    if (rc != GSB_OK) return rc;
+    if ((rc = check_equirect_width("forward_equirect", a->camera_width)) != GSB_OK) return rc;
+    if (ext) {
+        if (ext->channels < 1 || ext->channels > 16) {
+            set_error("forward_equirect: channels must be in 1..16 (got %d)", ext->channels);
+            return GSB_EINVAL;
+        }
+        if (!ext->features || !ext->rasterized) {
+            set_error("forward_equirect: null features / rasterized pointer");
+            return GSB_EINVAL;
+        }
+        if (a->rgb_only) {
+            set_error("forward_equirect: the feature map needs the full forward (rgb_only is set)");
+            return GSB_EINVAL;
+        }
+    }
+    Workspace ws;
+    if ((rc = resolve_fwd(a, &ws)) != GSB_OK) return rc;
+    if ((rc = check_equirect_intrinsics("forward_equirect", a->camera_intrinsics, a->camera_width, a->stream)) != GSB_OK) return rc;
+    cudaStream_t st = static_cast<cudaStream_t>(a->stream);
+    LensParams equirect{};
+    equirect.model = LENS_EQUIRECT;
+    if ((rc = launch_preprocess(*a, ws, st, &equirect)) != GSB_OK) return rc;
+    if (a->host_counters && a->host_counters_event) {
+        GSB_CUDA_CHECK(cudaMemcpyAsync(a->host_counters, ws.counters, 4 * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+        GSB_CUDA_CHECK(cudaEventRecord(static_cast<cudaEvent_t>(a->host_counters_event), st));
+    }
+    if ((rc = launch_sort(ws, a->key_capacity, st)) != GSB_OK) return rc;
+    const int T = (a->camera_height / GSB_TILE_HEIGHT) * (a->camera_width / GSB_TILE_WIDTH);
+    if ((rc = launch_tile_ranges(ws, a->key_capacity, T, st)) != GSB_OK) return rc;
+    return launch_blend_forward(*a, ws, st, ext, true);
+}
+
+int gsb200_backward_equirect(const GsbBackwardArgs *a, const float *grad_rasterized_depth, const float *rasterized_depth,
+                             const float *grad_pixel_accumulated_alpha, const GsbExtraFeatureArgs *ext) {
+    if (!a) {
+        set_error("backward_equirect: args is null");
+        return GSB_EINVAL;
+    }
+    int rc = check_equirect_width("backward_equirect", a->camera_width);
+    if (rc != GSB_OK) return rc;
+    if (!a->camera_intrinsics) {
+        set_error("backward_equirect: null camera_intrinsics");
+        return GSB_EINVAL;
+    }
+    if (a->flags & GSB_FLAG_COMPACT_GRADS) {
+        set_error("backward_equirect: the panorama is not implemented for the compact rows of the view-parallel exchange "
+                  "(GSB_FLAG_COMPACT_GRADS)");
+        return GSB_EUNSUPPORTED;
+    }
+    if (!(a->flags & GSB_FLAG_BACKWARD_TRANSPOSED)) {
+        set_error("backward_equirect: the panorama needs the transposed backward kernel (GSB_FLAG_BACKWARD_TRANSPOSED); the "
+                  "butterfly kernel does not wrap the seam");
+        return GSB_EUNSUPPORTED;
+    }
+    if ((grad_rasterized_depth == nullptr) != (rasterized_depth == nullptr)) {
+        set_error("backward_equirect: grad_rasterized_depth and rasterized_depth must be both NULL or both set");
+        return GSB_EINVAL;
+    }
+    if (ext) {
+        if (ext->channels < 1 || ext->channels > 16) {
+            set_error("backward_equirect: channels must be in 1..16 (got %d)", ext->channels);
+            return GSB_EINVAL;
+        }
+        if (!ext->features || !ext->grad_rasterized || !ext->grad_features) {
+            set_error("backward_equirect: null features / grad_rasterized / grad_features pointer");
+            return GSB_EINVAL;
+        }
+    }
+    return backward_impl(a, false, grad_rasterized_depth, rasterized_depth, grad_pixel_accumulated_alpha, ext, nullptr, nullptr,
+                         nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, true);
 }
 
 int gsb200_backward_with_depth(const GsbBackwardArgs *a, const float *grad_rasterized_depth, const float *rasterized_depth) {

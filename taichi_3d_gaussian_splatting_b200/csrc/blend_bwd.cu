@@ -283,7 +283,7 @@ static BlendBwdParams make_blend_bwd_params(const GsbBackwardArgs &a, const Work
 }
 
 int launch_blend_backward(const GsbBackwardArgs &a, const Workspace &ws, cudaStream_t stream, const float *grad_depth,
-                          const float *depth, const float *grad_alpha, const GsbExtraFeatureArgs *ext) {
+                          const float *depth, const float *grad_alpha, const GsbExtraFeatureArgs *ext, bool wrap) {
     BlendBwdParams p;
     p.H = a.camera_height;
     p.W = a.camera_width;
@@ -308,7 +308,7 @@ int launch_blend_backward(const GsbBackwardArgs &a, const Workspace &ws, cudaStr
     if (a.flags & GSB_FLAG_BACKWARD_TRANSPOSED)  // experimental, see blend_bwd_transposed.cu
         return launch_blend_backward_transposed(p, tiles, (a.flags & GSB_FLAG_EXACT_EXP) != 0,
                                                 (a.flags & GSB_FLAG_NO_HOOK_STATS) == 0, stream, grad_depth != nullptr,
-                                                grad_alpha != nullptr, ext ? &feat : nullptr);
+                                                grad_alpha != nullptr, ext ? &feat : nullptr, wrap);
     const bool exact = (a.flags & GSB_FLAG_EXACT_EXP) != 0;
     if (a.flags & GSB_FLAG_NO_HOOK_STATS) {  // opt-in
         if (exact) blend_backward_kernel<true, false><<<tiles, GSB_TILE_PIXELS, 0, stream>>>(p);
@@ -451,9 +451,12 @@ __device__ __forceinline__ void weighted_u_sigma(const float *U, const float *R,
 // dL/drho = dL/dbeta a^2 (rho - 1/z) / 8 with dL/dbeta = <G_B, M M^T>, in the first two values of the rows of MGRAD.
 constexpr int LENS_GRAD_VALUES = 5;
 constexpr int RS_GRAD_VALUES = 6;
+// EQUI = true (gsb200_backward_equirect): the frame is an equirectangular panorama (include/gsb200.h): d uv / d pc and the J
+// of Sigma' are both equirect_jacobian at point_in_camera (J detached, as for every model), and with DEPTH word 11 is dL/dr
+// of the ray distance, which enters pc along pc / r.  Non-compact, without any other camera path or gradient.
 template <bool COMPACT, bool DEPTH, bool POSE, bool INTR = false, bool LENS = false, bool LGRAD = false, bool RS = false,
           bool MGRAD = false, bool FILTER = false, bool BLUR = false, bool BGRAD = false, bool DEFOCUS = false,
-          bool DGRAD = false>
+          bool DGRAD = false, bool EQUI = false>
 __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, float *s_pose, float *pose_partials,
                                                      int num_objects, float *s_intr = nullptr,
                                                      float *intr_partials = nullptr, const LensParams lens = LensParams(),
@@ -473,6 +476,8 @@ __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, fl
     static_assert(!BGRAD || BLUR, "the exposure-motion gradient needs the motion-blur path");
     static_assert(!DEFOCUS || (BLUR && !BGRAD), "the defocus runs on the motion-blur path, without the exposure-motion gradient");
     static_assert(!DGRAD || DEFOCUS, "the defocus gradient needs the defocus path");
+    static_assert(!EQUI || (!COMPACT && !POSE && !INTR && !LENS && !RS && !FILTER && !BLUR),
+                  "the panorama is implemented for the dense rows without the other camera paths");
     constexpr bool CAM6 = MGRAD || BGRAD || DGRAD;  // the rows of a camera gradient (rolling shutter, exposure or defocus)
     // One thread per scene row: rows outside the frustum get their zeros here (no separate memset of the
     // dense (N,3)/(N,56) gradients), rows inside get the chain rule.  A warp owns 32 consecutive rows, i.e. one
@@ -580,13 +585,21 @@ __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, fl
             Jl[0] = F0 * iz; Jl[1] = F1 * iz; Jl[2] = -(F0 * pcx + F1 * pcy) * iz2;
             Jl[3] = F3 * iz; Jl[4] = F4 * iz; Jl[5] = -(F3 * pcx + F4 * pcy) * iz2;
         }
+        float eq_r = 1.0f;  // EQUI: the ray distance r
+        if (EQUI) {  // d uv / d pc = J of the panorama
+            const float pcv[3] = {pcx, pcy, pcz};
+            const float rho = sqrtf(pcx * pcx + pcz * pcz);
+            eq_r = sqrtf(rho * rho + pcy * pcy);
+            equirect_jacobian(Kc[0], Kc[4], pcv, rho, eq_r, dj);
+        }
         float gx[3];
 #pragma unroll
         for (int c = 0; c < 3; ++c) {
             const float d0 = dj[0] * Wm[c] + dj[1] * Wm[3 + c] + dj[2] * Wm[6 + c];
             const float d1 = dj[3] * Wm[c] + dj[4] * Wm[3 + c] + dj[5] * Wm[6 + c];
             gx[c] = a0.x * d0 + a0.y * d1;
-            if (DEPTH) gx[c] += a2.w * Wm[6 + c];
+            if (DEPTH && !EQUI) gx[c] += a2.w * Wm[6 + c];
+            if (DEPTH && EQUI) gx[c] += a2.w * (((pcx * Wm[c] + pcy * Wm[3 + c]) + pcz * Wm[6 + c]) / eq_r);  // dr/dpc = pc / r
         }
         // Sigma' = U Sigma U^T, U = J W with J from fx, fy only (GP3D:65-87, 237-331)
         const float fx = Kc[0], fy = Kc[4];
@@ -594,6 +607,10 @@ __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, fl
         if (LENS) {
 #pragma unroll
             for (int k = 0; k < 6; ++k) J[k] = Jl[k];
+        }
+        if (EQUI) {
+#pragma unroll
+            for (int k = 0; k < 6; ++k) J[k] = dj[k];
         }
         float U[6];
 #pragma unroll
@@ -984,6 +1001,13 @@ backward_points_lens_grad_kernel(const PointsBwdLensGradParams p) {
                                                                  p.lens_partials);
 }
 
+template <bool DEPTH>
+__global__ void __launch_bounds__(GSB_POINTS_THREADS, 6)
+backward_points_equirect_kernel(const PointsBwdParams p) {
+    backward_points_body<false, DEPTH, false, false, false, false, false, false, false, false, false, false, false, true>(
+        p, nullptr, nullptr, 0);
+}
+
 // One CTA: adds the `blocks` partial rows in a fixed order (strided per thread, then a fixed shared-memory tree) and writes
 // the 5 coefficient gradients (the unused fifth of a fisheye lens is a sum of zeros).  Zeros when blocks == 0.
 constexpr int LENS_GRAD_FINISH_THREADS = 128;
@@ -1343,6 +1367,18 @@ int launch_backward_points(const GsbBackwardArgs &a, const Workspace &ws, cudaSt
     } else {
         backward_points_kernel<false><<<(int)blocks, GSB_POINTS_THREADS, 0, stream>>>(p);
     }
+    GSB_CUDA_CHECK(cudaGetLastError());
+    return GSB_OK;
+}
+
+int launch_backward_points_equirect(const GsbBackwardArgs &a, const Workspace &ws, cudaStream_t stream, bool depth_grad) {
+    if (a.num_points <= 0) return GSB_OK;
+    const PointsBwdParams p = make_points_params(a, ws, nullptr);
+    long long blocks = (a.num_points + GSB_POINTS_THREADS - 1) / GSB_POINTS_THREADS;
+    const long long cap = 16LL * num_sms();
+    if (blocks > cap) blocks = cap;
+    if (depth_grad) backward_points_equirect_kernel<true><<<(int)blocks, GSB_POINTS_THREADS, 0, stream>>>(p);
+    else backward_points_equirect_kernel<false><<<(int)blocks, GSB_POINTS_THREADS, 0, stream>>>(p);
     GSB_CUDA_CHECK(cudaGetLastError());
     return GSB_OK;
 }

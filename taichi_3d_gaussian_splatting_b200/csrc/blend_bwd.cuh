@@ -64,7 +64,7 @@ __device__ __forceinline__ float sqrt_approx(float x) {  // MUFU.RSQ based, ~1 u
 
 int launch_blend_backward_transposed(const BlendBwdParams &p, int tiles, bool exact_exp, bool stats,
                                      cudaStream_t stream, bool depth = false, bool alpha = false,
-                                     const BlendFeatureParams *feat = nullptr);
+                                     const BlendFeatureParams *feat = nullptr, bool wrap = false);
 int launch_blend_backward_count(const BlendBwdParams &p, int tiles, cudaStream_t stream);
 
 }  // namespace gsb

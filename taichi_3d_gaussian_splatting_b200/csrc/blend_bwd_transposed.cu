@@ -38,6 +38,8 @@
 //     one shuffle level, then RED.ADD (F32x4 where C % 4 == 0) into the (N,C) rows.
 // The feature buffers are appended to the dynamic shared-memory image (TbFeat) and the kernel is compiled for 2 CTAs per
 // SM (DESIGN section 3); the existing buffers, the accumulator rows and the workspace are unchanged.
+// WRAP = true (gsb200_backward_equirect): the panorama's seam, staged as in the forward (equirect_wrap_u, common.cuh): every
+// later use of u -- phase 1's d0 and phase 2's row offsets -- sees the copy nearest the tile, and dL/du is unchanged by the shift.
 #include <type_traits>
 
 #include "blend_bwd.cuh"
@@ -151,7 +153,7 @@ __device__ __forceinline__ float keep_if_contributing(float P, int idx, int last
 template <int CF>
 using TbParams = typename std::conditional<CF == 0, BlendBwdParams, BlendBwdFeatParams>::type;
 
-template <bool EXACT_EXP, bool STATS, bool COUNT = false, bool DEPTH = false, bool ALPHA = false, int CF = 0>
+template <bool EXACT_EXP, bool STATS, bool COUNT = false, bool DEPTH = false, bool ALPHA = false, int CF = 0, bool WRAP = false>
 __global__ void __launch_bounds__(GSB_TILE_PIXELS, tb_min_blocks(CF))
 blend_backward_transposed_kernel(const TbParams<CF> p) {
     static_assert(!(COUNT && (DEPTH || ALPHA || CF)), "the work-counter diagnostic runs the default arithmetic only");
@@ -248,7 +250,9 @@ blend_backward_transposed_kernel(const TbParams<CF> p) {
                 if (idx >= block_start) {
                     const int o = __ldg(&p.sorted_vals[idx]);
                     const float4 *rec = p.records + 3 * (size_t)o;
-                    const float4 r0 = __ldg(rec), r1 = __ldg(rec + 1);
+                    float4 r0 = __ldg(rec);
+                    const float4 r1 = __ldg(rec + 1);
+                    if (WRAP) r0.x = equirect_wrap_u(r0.x, S.origin.x, (float)p.W);
                     if (EXACT_EXP) {
                         s_r0[tid] = r0;
                         s_r1[tid] = r1;
@@ -582,57 +586,65 @@ blend_backward_transposed_kernel(const TbParams<CF> p) {
 }
 
 #ifndef GSB_HOST_EMU
-template <bool EXACT_EXP, bool STATS, bool DEPTH = false, bool ALPHA = false, int CF = 0>
+template <bool EXACT_EXP, bool STATS, bool DEPTH = false, bool ALPHA = false, int CF = 0, bool WRAP = false>
 static int launch_tb(const TbParams<CF> &p, int tiles, cudaStream_t stream) {
     static bool configured = false;  // one device per process (one process per GPU)
     if (!configured) {
-        GSB_CUDA_CHECK(cudaFuncSetAttribute(blend_backward_transposed_kernel<EXACT_EXP, STATS, false, DEPTH, ALPHA, CF>,
+        GSB_CUDA_CHECK(cudaFuncSetAttribute(blend_backward_transposed_kernel<EXACT_EXP, STATS, false, DEPTH, ALPHA, CF, WRAP>,
                                             cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tb_smem_bytes<CF>()));
         configured = true;
     }
-    blend_backward_transposed_kernel<EXACT_EXP, STATS, false, DEPTH, ALPHA, CF>
+    blend_backward_transposed_kernel<EXACT_EXP, STATS, false, DEPTH, ALPHA, CF, WRAP>
         <<<tiles, GSB_TILE_PIXELS, tb_smem_bytes<CF>(), stream>>>(p);
     GSB_CUDA_CHECK(cudaGetLastError());
     return GSB_OK;
 }
 
-template <bool DEPTH, bool ALPHA, int CF = 0>
+template <bool DEPTH, bool ALPHA, int CF = 0, bool WRAP = false>
 static int launch_tb_terms(const TbParams<CF> &p, int tiles, bool exact_exp, bool stats, cudaStream_t stream) {
     if (exact_exp)
-        return stats ? launch_tb<true, true, DEPTH, ALPHA, CF>(p, tiles, stream)
-                     : launch_tb<true, false, DEPTH, ALPHA, CF>(p, tiles, stream);
-    return stats ? launch_tb<false, true, DEPTH, ALPHA, CF>(p, tiles, stream)
-                 : launch_tb<false, false, DEPTH, ALPHA, CF>(p, tiles, stream);
+        return stats ? launch_tb<true, true, DEPTH, ALPHA, CF, WRAP>(p, tiles, stream)
+                     : launch_tb<true, false, DEPTH, ALPHA, CF, WRAP>(p, tiles, stream);
+    return stats ? launch_tb<false, true, DEPTH, ALPHA, CF, WRAP>(p, tiles, stream)
+                 : launch_tb<false, false, DEPTH, ALPHA, CF, WRAP>(p, tiles, stream);
 }
 
-template <int CF>
+template <int CF, bool WRAP = false>
 static int launch_tb_features(const BlendBwdFeatParams &p, int tiles, bool exact_exp, bool stats, cudaStream_t stream, bool depth,
                               bool alpha) {
     if (alpha)
-        return depth ? launch_tb_terms<true, true, CF>(p, tiles, exact_exp, stats, stream)
-                     : launch_tb_terms<false, true, CF>(p, tiles, exact_exp, stats, stream);
-    return depth ? launch_tb_terms<true, false, CF>(p, tiles, exact_exp, stats, stream)
-                 : launch_tb_terms<false, false, CF>(p, tiles, exact_exp, stats, stream);
+        return depth ? launch_tb_terms<true, true, CF, WRAP>(p, tiles, exact_exp, stats, stream)
+                     : launch_tb_terms<false, true, CF, WRAP>(p, tiles, exact_exp, stats, stream);
+    return depth ? launch_tb_terms<true, false, CF, WRAP>(p, tiles, exact_exp, stats, stream)
+                 : launch_tb_terms<false, false, CF, WRAP>(p, tiles, exact_exp, stats, stream);
 }
 
-// depth = true: p.grad_depth and p.depth must be set (the DEPTH instantiations); alpha = true: p.grad_alpha (ALPHA);
-// feat: the feature channels, C in 1..16 (the CF instantiation of width 4, 8 or 16), or NULL
-int launch_blend_backward_transposed(const BlendBwdParams &p, int tiles, bool exact_exp, bool stats,
-                                     cudaStream_t stream, bool depth, bool alpha, const BlendFeatureParams *feat) {
+template <bool WRAP>
+static int launch_tb_all(const BlendBwdParams &p, int tiles, bool exact_exp, bool stats, cudaStream_t stream, bool depth,
+                         bool alpha, const BlendFeatureParams *feat) {
     if (feat) {
         BlendBwdFeatParams fp;
         static_cast<BlendBwdParams &>(fp) = p;
         fp.feat = *feat;
         const int C = feat->channels;
-        return C <= 4 ? launch_tb_features<4>(fp, tiles, exact_exp, stats, stream, depth, alpha)
-             : C <= 8 ? launch_tb_features<8>(fp, tiles, exact_exp, stats, stream, depth, alpha)
-                      : launch_tb_features<16>(fp, tiles, exact_exp, stats, stream, depth, alpha);
+        return C <= 4 ? launch_tb_features<4, WRAP>(fp, tiles, exact_exp, stats, stream, depth, alpha)
+             : C <= 8 ? launch_tb_features<8, WRAP>(fp, tiles, exact_exp, stats, stream, depth, alpha)
+                      : launch_tb_features<16, WRAP>(fp, tiles, exact_exp, stats, stream, depth, alpha);
     }
     if (alpha)
-        return depth ? launch_tb_terms<true, true>(p, tiles, exact_exp, stats, stream)
-                     : launch_tb_terms<false, true>(p, tiles, exact_exp, stats, stream);
-    return depth ? launch_tb_terms<true, false>(p, tiles, exact_exp, stats, stream)
-                 : launch_tb_terms<false, false>(p, tiles, exact_exp, stats, stream);
+        return depth ? launch_tb_terms<true, true, 0, WRAP>(p, tiles, exact_exp, stats, stream)
+                     : launch_tb_terms<false, true, 0, WRAP>(p, tiles, exact_exp, stats, stream);
+    return depth ? launch_tb_terms<true, false, 0, WRAP>(p, tiles, exact_exp, stats, stream)
+                 : launch_tb_terms<false, false, 0, WRAP>(p, tiles, exact_exp, stats, stream);
+}
+
+// depth = true: p.grad_depth and p.depth must be set (the DEPTH instantiations); alpha = true: p.grad_alpha (ALPHA);
+// feat: the feature channels, C in 1..16 (the CF instantiation of width 4, 8 or 16), or NULL; wrap: the WRAP instantiations
+// (an equirectangular frame)
+int launch_blend_backward_transposed(const BlendBwdParams &p, int tiles, bool exact_exp, bool stats,
+                                     cudaStream_t stream, bool depth, bool alpha, const BlendFeatureParams *feat, bool wrap) {
+    return wrap ? launch_tb_all<true>(p, tiles, exact_exp, stats, stream, depth, alpha, feat)
+                : launch_tb_all<false>(p, tiles, exact_exp, stats, stream, depth, alpha, feat);
 }
 
 // Diagnostic: loop A with GPU-side work counters (default arithmetic, no hook statistics): counters[0] = (warp, splat)

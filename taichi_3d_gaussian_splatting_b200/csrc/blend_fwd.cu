@@ -108,7 +108,9 @@ constexpr int fw_feature_smem_bytes(int cf) { return 2 * GSB_TILE_PIXELS * cf * 
 
 // CF (4, 8 or 16; 0 = no features): compile-time width of the per-Gaussian feature vector (gsb200_forward_ext).  The
 // runtime C <= CF is padded with zeros in shared memory and registers; nothing past C is read or written in global memory.
-template <bool RGB_ONLY, bool EXACT_EXP, bool COUNT = false, int CF = 0>
+// WRAP = true (gsb200_forward_equirect): the panorama's seam -- each splat is staged at the copy of its u nearest the tile
+// (equirect_wrap_u, common.cuh), before the fast planes and the patch mask are formed; the per-pixel loop is unchanged.
+template <bool RGB_ONLY, bool EXACT_EXP, bool COUNT = false, int CF = 0, bool WRAP = false>
 __global__ void __launch_bounds__(GSB_TILE_PIXELS, fw_min_blocks(CF, EXACT_EXP))
 blend_forward_kernel(const FwParams<CF> p) {
     static_assert(CF == 0 || (CF % 4 == 0 && !RGB_ONLY && !COUNT), "features: whole float4 groups, full outputs only");
@@ -155,7 +157,9 @@ blend_forward_kernel(const FwParams<CF> p) {
         if (idx < end) {
             const int o = __ldg(&p.sorted_vals[idx]);
             const float4 *rec = p.records + 3 * (size_t)o;
-            const float4 r0 = __ldg(rec), r1 = __ldg(rec + 1);
+            float4 r0 = __ldg(rec);
+            const float4 r1 = __ldg(rec + 1);
+            if (WRAP) r0.x = equirect_wrap_u(r0.x, tile_x0, (float)p.W);
             if (EXACT_EXP) {
                 s_r0[tid] = r0;
                 s_r1[tid] = r1;
@@ -338,25 +342,52 @@ blend_forward_kernel(const FwParams<CF> p) {
 }
 
 #ifndef GSB_HOST_EMU
-template <bool EXACT_EXP, int CF>
+template <bool EXACT_EXP, int CF, bool WRAP = false>
 static int launch_fwd_features(const BlendFwdFeatParams &p, int tiles, cudaStream_t stream) {
     static bool configured = false;  // one device per process (one process per GPU)
     if (!configured) {
-        GSB_CUDA_CHECK(cudaFuncSetAttribute(blend_forward_kernel<false, EXACT_EXP, false, CF>,
+        GSB_CUDA_CHECK(cudaFuncSetAttribute(blend_forward_kernel<false, EXACT_EXP, false, CF, WRAP>,
                                             cudaFuncAttributeMaxDynamicSharedMemorySize, fw_feature_smem_bytes(CF)));
         configured = true;
     }
-    blend_forward_kernel<false, EXACT_EXP, false, CF><<<tiles, GSB_TILE_PIXELS, fw_feature_smem_bytes(CF), stream>>>(p);
+    blend_forward_kernel<false, EXACT_EXP, false, CF, WRAP><<<tiles, GSB_TILE_PIXELS, fw_feature_smem_bytes(CF), stream>>>(p);
     GSB_CUDA_CHECK(cudaGetLastError());
     return GSB_OK;
 }
 
-template <int CF>
+template <int CF, bool WRAP = false>
 static int launch_fwd_features(const BlendFwdFeatParams &p, int tiles, bool exact, cudaStream_t stream) {
-    return exact ? launch_fwd_features<true, CF>(p, tiles, stream) : launch_fwd_features<false, CF>(p, tiles, stream);
+    return exact ? launch_fwd_features<true, CF, WRAP>(p, tiles, stream) : launch_fwd_features<false, CF, WRAP>(p, tiles, stream);
 }
 
-int launch_blend_forward(const GsbForwardArgs &a, const Workspace &ws, cudaStream_t stream, const GsbExtraFeatureArgs *ext) {
+// The WRAP instantiations of gsb200_forward_equirect (the default ones stay as they are)
+static int launch_blend_forward_wrap(const BlendFwdParams &p, int tiles, bool exact, bool rgb_only, const GsbExtraFeatureArgs *ext,
+                                     const Workspace &ws, cudaStream_t stream) {
+    if (ext) {
+        BlendFwdFeatParams fp;
+        static_cast<BlendFwdParams &>(fp) = p;
+        fp.channels = ext->channels;
+        fp.point_id = ws.point_id;
+        fp.features = ext->features;
+        fp.out_features = ext->rasterized;
+        const int C = ext->channels;
+        return C <= 4 ? launch_fwd_features<4, true>(fp, tiles, exact, stream)
+             : C <= 8 ? launch_fwd_features<8, true>(fp, tiles, exact, stream)
+                      : launch_fwd_features<16, true>(fp, tiles, exact, stream);
+    }
+    if (rgb_only) {
+        if (exact) blend_forward_kernel<true, true, false, 0, true><<<tiles, GSB_TILE_PIXELS, 0, stream>>>(p);
+        else blend_forward_kernel<true, false, false, 0, true><<<tiles, GSB_TILE_PIXELS, 0, stream>>>(p);
+    } else {
+        if (exact) blend_forward_kernel<false, true, false, 0, true><<<tiles, GSB_TILE_PIXELS, 0, stream>>>(p);
+        else blend_forward_kernel<false, false, false, 0, true><<<tiles, GSB_TILE_PIXELS, 0, stream>>>(p);
+    }
+    GSB_CUDA_CHECK(cudaGetLastError());
+    return GSB_OK;
+}
+
+int launch_blend_forward(const GsbForwardArgs &a, const Workspace &ws, cudaStream_t stream, const GsbExtraFeatureArgs *ext,
+                         bool wrap) {
     BlendFwdParams p;
     p.H = a.camera_height;
     p.W = a.camera_width;
@@ -374,6 +405,7 @@ int launch_blend_forward(const GsbForwardArgs &a, const Workspace &ws, cudaStrea
     const int tiles = p.tiles_x * (a.camera_height / GSB_TILE_HEIGHT);
     if (tiles <= 0) return GSB_OK;
     const bool exact = (a.flags & GSB_FLAG_EXACT_EXP) != 0;
+    if (wrap) return launch_blend_forward_wrap(p, tiles, exact, a.rgb_only != 0, ext, ws, stream);
     if (ext) {  // checked by gsb200_forward_ext: 1 <= C <= 16, not rgb_only
         BlendFwdFeatParams fp;
         static_cast<BlendFwdParams &>(fp) = p;

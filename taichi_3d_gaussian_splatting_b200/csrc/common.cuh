@@ -80,16 +80,21 @@ int launch_sort(const Workspace &ws, int64_t key_capacity, cudaStream_t stream);
 int launch_tile_ranges(const Workspace &ws, int64_t key_capacity, int num_tiles, cudaStream_t stream);
 int launch_tile_ranges_raw(const long long *keys_i64, int64_t n, int *tile_start, int *tile_end,
                            int num_tiles, cudaStream_t stream);
-// ext: the per-Gaussian feature vectors to blend alongside the image (gsb200_forward_ext, checked there), or NULL
+// ext: the per-Gaussian feature vectors to blend alongside the image (gsb200_forward_ext, checked there), or NULL; wrap: the
+// WRAP instantiations of an equirectangular frame (gsb200_forward_equirect)
 int launch_blend_forward(const GsbForwardArgs &a, const Workspace &ws, cudaStream_t stream,
-                         const GsbExtraFeatureArgs *ext = nullptr);
+                         const GsbExtraFeatureArgs *ext = nullptr, bool wrap = false);
 // grad_depth / depth: the (H,W) depth gradient and the forward's depth output (gsb200_backward_aux; transposed
 // kernel only), or both NULL.  grad_alpha: the (H,W) gradient of the accumulated alpha (transposed kernel only), or NULL.
 // ext: the feature-map gradient and the (N,C) output rows, zeroed by the caller (transposed kernel only), or NULL.
-// depth_grad: the accumulator rows carry dL/dz in word 11.
+// depth_grad: the accumulator rows carry dL/dz in word 11.  wrap: the WRAP instantiations of the transposed kernel for an
+// equirectangular frame (gsb200_backward_equirect; the butterfly kernel has none)
 int launch_blend_backward(const GsbBackwardArgs &a, const Workspace &ws, cudaStream_t stream,
                           const float *grad_depth = nullptr, const float *depth = nullptr,
-                          const float *grad_alpha = nullptr, const GsbExtraFeatureArgs *ext = nullptr);
+                          const float *grad_alpha = nullptr, const GsbExtraFeatureArgs *ext = nullptr, bool wrap = false);
+// gsb200_backward_equirect: the EQUIRECT per-point kernel (dense gradients as launch_backward_points, d uv / d pc and J of the
+// panorama, depth r); arguments checked by the caller
+int launch_backward_points_equirect(const GsbBackwardArgs &a, const Workspace &ws, cudaStream_t stream, bool depth_grad);
 int launch_backward_points(const GsbBackwardArgs &a, const Workspace &ws, cudaStream_t stream,
                            const long long *skip_flag = nullptr, bool depth_grad = false);
 // gsb200_backward_lens: the LENS per-point kernel (dense gradients as launch_backward_points, d uv / d pc and J through the
@@ -552,6 +557,42 @@ __device__ __forceinline__ void blur_cov_grad(float s00, float s01, float s11, f
     g00 += h * (ia * a11 - i00);
     g01 += h * (-ia * s01 - i01);
     g11 += h * (ia * a00 - i11);
+}
+#endif
+
+// ---- equirectangular panoramas (gsb200_forward_equirect / gsb200_backward_equirect; definition in include/gsb200.h).
+// LENS_EQUIRECT is an internal model code of the per-point kernels' LENS switch and of LensParams::model, never a GsbLensArgs
+// value: gsb200_forward_lens keeps refusing every model code it does not know.
+constexpr int LENS_EQUIRECT = 0x45510;
+#if defined(__CUDACC__) || defined(GSB_HOST_EMU)
+// The projection of a camera-frame point: rho = |(x, z)|, r = |pc|, u = fx atan2(x, z) + cx reduced into [0, W),
+// v = fy atan2(y, rho) + cy.  Returns whether the point is in view (near < r < far, rho > GSB_EQUIRECT_POLE_EPSILON r; NaN
+// fails).
+__device__ __forceinline__ bool equirect_project(const float *Kc, int W, float near_plane, float far_plane, const float *pc,
+                                                 float &u, float &v, float &rho, float &r) {
+    const float x = pc[0], y = pc[1], z = pc[2];
+    const float rho2 = x * x + z * z;
+    rho = sqrtf(rho2);
+    r = sqrtf(rho2 + y * y);
+    const float Wf = (float)W;
+    u = Kc[0] * atan2f(x, z) + Kc[2];
+    u = u - Wf * floorf(u / Wf);
+    if (u >= Wf) u = u - Wf;  // a tiny negative u rounds to W
+    v = Kc[4] * atan2f(y, rho) + Kc[5];
+    return r > near_plane && r < far_plane && rho > GSB_EQUIRECT_POLE_EPSILON * r;
+}
+// J = d(u, v)/d pc = diag(fx, fy) [z/rho^2 0 -x/rho^2; -x y/(r^2 rho) rho/r^2 -z y/(r^2 rho)], row-major 2x3: the Jacobian of
+// Sigma' (pc detached, DESIGN section 3) and, with pc live, the position's
+__device__ __forceinline__ void equirect_jacobian(float fx, float fy, const float *pc, float rho, float r, float *J) {
+    const float x = pc[0], y = pc[1], z = pc[2];
+    const float irho2 = 1.0f / (rho * rho), ir2 = 1.0f / (r * r);
+    const float t = (y * ir2) / rho;
+    J[0] = fx * (z * irho2); J[1] = 0.0f; J[2] = -(fx * (x * irho2));
+    J[3] = -(fy * (x * t)); J[4] = fy * (rho * ir2); J[5] = -(fy * (z * t));
+}
+// The copy of a splat centre u nearest the tile column whose pixels start at tile_x0 (the blend kernels' WRAP staging)
+__device__ __forceinline__ float equirect_wrap_u(float u, float tile_x0, float W) {
+    return u + W * rintf(((tile_x0 + 0.5f * (float)GSB_TILE_WIDTH) - u) / W);
 }
 #endif
 

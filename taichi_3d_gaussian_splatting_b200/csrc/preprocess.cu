@@ -154,6 +154,22 @@ __device__ __forceinline__ void bounding_box(float u, float v, float radii, int 
     d = min(max((int)floorf(max_v / (float)GSB_TILE_HEIGHT) + 1, c + 1), th);
 }
 
+// The tile columns [a, b) of an equirectangular footprint (u in [0, W)): not clamped to the image, and a footprint wider than
+// the panorama is cut to the W/16 columns whose centres lie within W/2 of u, so that every column of the window is the copy
+// the blend kernels stage the splat at (equirect_wrap_u).  NaN or inf radii take the whole row.
+__device__ __forceinline__ void equirect_columns(float u, float radii, int W, int &a, int &b) {
+    radii = fmaxf(radii, 1.0f);
+    const int tw = W / GSB_TILE_WIDTH;
+    const float fa = floorf((u - radii) / (float)GSB_TILE_WIDTH), fb = floorf((u + radii) / (float)GSB_TILE_WIDTH) + 1.0f;
+    if (fb - fa <= (float)tw) {
+        a = (int)fa;
+        b = (int)fb;
+    } else {
+        a = (int)ceilf((u - 0.5f * (float)W - 0.5f * (float)GSB_TILE_WIDTH) / (float)GSB_TILE_WIDTH);
+        b = a + tw;
+    }
+}
+
 #ifndef GSB_PRE_MIN_BLOCKS
 #define GSB_PRE_MIN_BLOCKS 5
 #endif
@@ -207,12 +223,18 @@ __device__ __forceinline__ bool tile_reachable(const SplatReach &r, float u, flo
 // DEFOCUS = true (with BLUR; gsb200_forward_defocus): B also carries the thin lens' B_d = beta M M^T, beta = a^2 (rho - 1/z)^2
 // / 16 at the rendered z, M = K[:2,:2] (K[:2,:2] D with a lens): B = B_m + B_d, and the conic, c_b, radius and reach follow
 // from Sigma_d + B as above.  A view with a = 0 takes the arithmetic without defocus.
+// LENS = LENS_EQUIRECT (gsb200_forward_equirect): the equirectangular panorama (definition in include/gsb200.h).  (u, v), the
+// in-view test and J come from equirect_project / equirect_jacobian (common.cuh), the depth is the ray distance r (record,
+// sort key, CNT_MAX_DEPTH_KEY), the footprint's columns from equirect_columns, and the key's tile column is taken modulo
+// W/16.  Not with ROLLING, FILTER or BLUR.
 template <typename KeyT, int LENS, bool ROLLING = false, bool FILTER = false, bool BLUR = false, bool DEFOCUS = false>
 __device__ __forceinline__ void preprocess_body(const PreParams p, const LensParams lens, const RsParams rs = RsParams(),
                                                 const float *filter3d = nullptr, const BlurParams blur = BlurParams(),
                                                 const DefocusParams defocus = DefocusParams()) {
     static_assert(!(BLUR && FILTER), "the motion blur is not implemented with the 3D filter");
     static_assert(!DEFOCUS || BLUR, "the defocus runs on the motion-blur path");
+    constexpr bool EQUIRECT = LENS == LENS_EQUIRECT;
+    static_assert(!EQUIRECT || (!ROLLING && !FILTER && !BLUR), "the panorama is implemented without the camera extensions");
     __shared__ unsigned int s_ticket;
     __shared__ unsigned long long s_warp_sums[SCAN_BLOCK_THREADS / 32];
     __shared__ unsigned long long s_block_exclusive;
@@ -234,6 +256,7 @@ __device__ __forceinline__ void preprocess_body(const PreParams p, const LensPar
     float pc[3] = {0, 0, 0};
     float dir0 = 0.0f, dir1 = 0.0f, dir2 = 0.0f;  // unit view direction (GPCR:302), consumed by the SH stage
     float tau = 0.0f;                             // ROLLING: the row time
+    float depth = 0.0f, eq_rho = 0.0f;            // EQUIRECT: the ray distance r and rho = |(x, z)|
 
     // Every global load of a point that depends on nothing but its index is issued HERE, in one go: the invalid mask, the
     // object id, the position and the first 32 bytes of the feature row (q | s, logit).  The kernel is bound by the latency
@@ -294,7 +317,11 @@ __device__ __forceinline__ void preprocess_body(const PreParams p, const LensPar
         float u, v;
         float D[4] = {1.0f, 0.0f, 0.0f, 1.0f};  // d(xd, yd)/d(xn, yn)
         bool lens_ok = true;
-        if (LENS == GSB_LENS_PINHOLE) {
+        if (EQUIRECT) {
+            in = equirect_project(Kc, p.W, p.near_plane, p.far_plane, pc, u, v, eq_rho, depth) &&
+                 v >= (float)(-GSB_TILE_HEIGHT * GSB_BOUNDARY_TILES) &&
+                 v < (float)(p.H + GSB_TILE_HEIGHT * GSB_BOUNDARY_TILES);
+        } else if (LENS == GSB_LENS_PINHOLE) {
             float uv1[3];
             matmul<3, 3, 1>(Kc, pc, uv1);
             u = uv1[0] / pc[2];
@@ -311,11 +338,14 @@ __device__ __forceinline__ void preprocess_body(const PreParams p, const LensPar
             u = uv1[0] / pc[2];
             v = uv1[1] / pc[2];
         }
-        in = lens_ok && pc[2] > p.near_plane && pc[2] < p.far_plane &&
-             u >= (float)(-GSB_TILE_WIDTH * GSB_BOUNDARY_TILES) &&
-             u < (float)(p.W + GSB_TILE_WIDTH * GSB_BOUNDARY_TILES) &&
-             v >= (float)(-GSB_TILE_HEIGHT * GSB_BOUNDARY_TILES) &&
-             v < (float)(p.H + GSB_TILE_HEIGHT * GSB_BOUNDARY_TILES);
+        if (!EQUIRECT) {
+            depth = pc[2];
+            in = lens_ok && pc[2] > p.near_plane && pc[2] < p.far_plane &&
+                 u >= (float)(-GSB_TILE_WIDTH * GSB_BOUNDARY_TILES) &&
+                 u < (float)(p.W + GSB_TILE_WIDTH * GSB_BOUNDARY_TILES) &&
+                 v >= (float)(-GSB_TILE_HEIGHT * GSB_BOUNDARY_TILES) &&
+                 v < (float)(p.H + GSB_TILE_HEIGHT * GSB_BOUNDARY_TILES);
+        }
         if (in) {
             float4 *frow = reinterpret_cast<float4 *>(p.features + (size_t)GSB_FEATURE_DIM * i);
             float4 qv = h_q;
@@ -339,6 +369,7 @@ __device__ __forceinline__ void preprocess_body(const PreParams p, const LensPar
                 J[3] = (fy * D[2]) / pc[2]; J[4] = (fy * D[3]) / pc[2];
                 J[5] = -(fy * (D[2] * pc[0] + D[3] * pc[1])) / (pc[2] * pc[2]);
             }
+            if (EQUIRECT) equirect_jacobian(fx, fy, pc, eq_rho, depth, J);
             float R[9], S[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0}, RS[9], RSS[9], RT[9], Sigma[9];
             rotation_from_quaternion(qv.x, qv.y, qv.z, qv.w, R);
             S[0] = exp_cr(f[0]); S[4] = exp_cr(f[1]); S[8] = exp_cr(f[2]);
@@ -434,6 +465,7 @@ __device__ __forceinline__ void preprocess_body(const PreParams p, const LensPar
             dx = dinv * dx; dy = dinv * dy; dz = dinv * dz;
             dir0 = dx; dir1 = dy; dir2 = dz;
             bounding_box(u, v, radius, p.W, p.H, min_tu, max_tu, min_tv, max_tv);
+            if (EQUIRECT) equirect_columns(u, radius, p.W, min_tu, max_tu);
             ntiles = (max_tu - min_tu) * (max_tv - min_tv);
             // reach-test parameters of this splat; the (tile, splat) tests themselves are done cooperatively by
             // the warp below (one lane per PAIR, not per splat)
@@ -441,7 +473,7 @@ __device__ __forceinline__ void preprocess_body(const PreParams p, const LensPar
             reach = make_splat_reach(inv_det * c11, inv_det * (-c01), inv_det * c00, rescale_c * opacity);
             if (!p.filter_tiles) reach.mode = 2;
             r0 = make_float4(u, v, inv_det * c11, inv_det * (-c01));
-            r1 = make_float4(inv_det * c00, rescale_c, opacity, pc[2]);
+            r1 = make_float4(inv_det * c00, rescale_c, opacity, EQUIRECT ? depth : pc[2]);
             r2.w = radius;
         }
     }
@@ -617,7 +649,7 @@ __device__ __forceinline__ void preprocess_body(const PreParams p, const LensPar
     // (tile_u outer, tile_v inner) order.  The key ranges of the warp's splats are adjacent (prefix sum), so
     // dealing the keys round-robin to the lanes makes the stores contiguous and the work balanced.
     {
-        const int depth_key = (int)(pc[2] * p.depth_scale);
+        const int depth_key = (int)((EQUIRECT ? depth : pc[2]) * p.depth_scale);
         st.depth_key[lane] = depth_key;
         {   // largest depth key of the frame -> CNT_MAX_DEPTH_KEY: the sort runs only the passes its live bits need
             int wmax = in ? depth_key : 0;
@@ -663,7 +695,7 @@ __device__ __forceinline__ void preprocess_body(const PreParams p, const LensPar
             const int tu = st.min_tu[lo] + du, tv = st.min_tv[lo] + (idx - du * ntv_o);
             const long long pos = st.key_base[lo] + j;
             if (pos < p.key_store_limit) {
-                const KeyT tile = (KeyT)(tu + tv * tiles_x);
+                const KeyT tile = EQUIRECT ? (KeyT)((tu % tiles_x + tiles_x) % tiles_x + tv * tiles_x) : (KeyT)(tu + tv * tiles_x);
                 keys[pos] = (tile << p.depth_bits) | (KeyT)(unsigned int)st.depth_key[lo];
                 p.vals[pos] = st.off[lo];
             }
@@ -731,6 +763,12 @@ template <typename KeyT, int LENS, bool ROLLING, bool DEFOCUS = false>
 __global__ void __launch_bounds__(SCAN_BLOCK_THREADS, GSB_PRE_MIN_BLOCKS)
 preprocess_blur_kernel(const PreBlurParams p) {
     preprocess_body<KeyT, LENS, ROLLING, false, true, DEFOCUS>(p, p.lens, p.rs, nullptr, p.blur, p.defocus);
+}
+
+template <typename KeyT>
+__global__ void __launch_bounds__(SCAN_BLOCK_THREADS, GSB_PRE_MIN_BLOCKS)
+preprocess_equirect_kernel(const PreParams p) {
+    preprocess_body<KeyT, LENS_EQUIRECT>(p, LensParams());
 }
 
 #ifndef GSB_HOST_EMU  // tests/simt compiles the kernels above as host C++ under the SIMT emulator
@@ -861,6 +899,9 @@ int launch_preprocess(const GsbForwardArgs &a, const Workspace &ws, cudaStream_t
             else if (model == GSB_LENS_OPENCV) preprocess_rs_kernel<unsigned long long, GSB_LENS_OPENCV><<<grid, block, 0, stream>>>(pr);
             else preprocess_rs_kernel<unsigned long long, GSB_LENS_PINHOLE><<<grid, block, 0, stream>>>(pr);
         }
+    } else if (lens != nullptr && lens->model == LENS_EQUIRECT) {  // gsb200_forward_equirect: no other extension
+        if (L.key_bytes == 4) preprocess_equirect_kernel<unsigned int><<<L.scan_blocks, SCAN_BLOCK_THREADS, 0, stream>>>(p);
+        else preprocess_equirect_kernel<unsigned long long><<<L.scan_blocks, SCAN_BLOCK_THREADS, 0, stream>>>(p);
     } else if (lens != nullptr) {
         PreLensParams pl;
         static_cast<PreParams &>(pl) = p;

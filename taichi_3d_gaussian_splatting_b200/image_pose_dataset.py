@@ -24,6 +24,9 @@ the image by nearest neighbour.  The optional key ``loss_weight_path`` gives the
 An optional record key ``distortion`` (an extension), ``{"model": "opencv" | "fisheye", "coefficients": [...]}``, gives the
 view's ``CameraInfo.distortion`` (``Camera.LensDistortion``).  The coefficients act on the normalised image plane, so
 rescaling, cropping and autoscale leave them unchanged.
+With ``"model": "equirectangular"`` and ``"coefficients": []`` the view is a 360-degree panorama: its width is resized (not
+cropped) to a multiple of 16, autoscale resizes it the same way, and fx is set so that 2 pi fx = W; its targets are resized
+with it (the depth, labels and features by nearest neighbour).
 An optional record key ``rolling_shutter`` (an extension), ``{"linear_velocity": [3], "angular_velocity": [3],
 "readout_time": s}``, gives the view's ``CameraInfo.rolling_shutter`` (``Camera.RollingShutter.from_camera_velocity``: the
 camera's own velocities in its frame, in scene units/s and rad/s, as visual-inertial odometry reports them, and the sensor's
@@ -39,6 +42,7 @@ Pinned against the reference class itself: ``tests/golden/make_dataset_golden.py
 stores its outputs for a small generated dataset; ``tests/test_dataset_cpu.py`` compares.
 """
 import json
+import math
 import os
 from typing import List, Optional, Tuple
 
@@ -59,6 +63,27 @@ def _crop_to_tiles(image: torch.Tensor) -> torch.Tensor:
     h = image.shape[1] - image.shape[1] % TILE_HEIGHT
     w = image.shape[2] - image.shape[2] % TILE_WIDTH
     return image[:3, :h, :w].contiguous()
+
+
+def _is_equirect(info: CameraInfo) -> bool:
+    return info.distortion is not None and info.distortion.model == "equirectangular"
+
+
+def _resize_equirect(image: torch.Tensor, info: CameraInfo, h: int, w: int) -> Tuple[torch.Tensor, CameraInfo]:
+    """An equirectangular view resized (antialiased) to (h, w), multiples of 16: every column is kept, fx = W / 2pi, cx
+    and fy, cy scale with the size."""
+    import torchvision.transforms.functional as TF
+    if (h, w) != (image.shape[1], image.shape[2]):
+        image = TF.resize(image[:3], size=[h, w], antialias=True)
+    K = info.camera_intrinsics.clone()
+    sy = h / info.camera_height
+    K[0, 2] *= w / info.camera_width
+    K[0, 0] = w / (2.0 * math.pi)
+    K[1, 1] *= sy
+    K[1, 2] *= sy
+    return image[:3].contiguous(), CameraInfo(camera_intrinsics=K, camera_height=h, camera_width=w, camera_id=info.camera_id,
+                                              distortion=info.distortion, rolling_shutter=info.rolling_shutter,
+                                              motion_blur=info.motion_blur, defocus=info.defocus)
 
 
 def _load_image(path: str) -> torch.Tensor:
@@ -90,6 +115,10 @@ class ImagePoseDataset(torch.utils.data.Dataset):
         if max(camera_info.camera_height, camera_info.camera_width) <= MAX_RESOLUTION_TRAIN:
             return image, camera_info
         import torchvision.transforms.functional as TF
+        if _is_equirect(camera_info):  # the size the resize below would give, then its tile multiple
+            h, w = TF.resize(torch.zeros(1, camera_info.camera_height, camera_info.camera_width), size=1024,
+                             max_size=MAX_RESOLUTION_TRAIN, antialias=False).shape[1:]
+            return _resize_equirect(image, camera_info, h - h % TILE_HEIGHT, w - w % TILE_WIDTH)
         resized = TF.resize(image, size=1024, max_size=MAX_RESOLUTION_TRAIN, antialias=True)
         sy = resized.shape[1] / camera_info.camera_height
         sx = resized.shape[2] / camera_info.camera_width
@@ -106,7 +135,8 @@ class ImagePoseDataset(torch.utils.data.Dataset):
 
     @staticmethod
     def _distortion(rec: dict) -> Optional[LensDistortion]:
-        """The optional record key ``"distortion": {"model": "opencv" | "fisheye", "coefficients": [...]}``."""
+        """The optional record key ``"distortion": {"model": "opencv" | "fisheye" | "equirectangular", "coefficients":
+        [...]}``."""
         d = rec.get("distortion")
         if d is None:
             return None
@@ -217,8 +247,30 @@ class ImagePoseDataset(torch.utils.data.Dataset):
                              f"{(info.camera_height, info.camera_width)}")
         return x.contiguous()
 
+    @staticmethod
+    def _resize_equirect_targets(depth, mask, labels, features, loss_weight, info: CameraInfo) -> SupervisionTargets:
+        """The targets of an equirectangular view resized to its size: the mask and the loss weight antialiased, the depth,
+        the labels and the features by nearest neighbour (the pixel indices are resized)."""
+        import torchvision.transforms.functional as TF
+        h, w = info.camera_height, info.camera_width
+
+        def nearest(x):
+            if x is None:
+                return None
+            idx = torch.arange(x.shape[0] * x.shape[1], dtype=torch.float64).reshape(1, x.shape[0], x.shape[1])
+            idx = TF.resize(idx, size=[h, w], interpolation=TF.InterpolationMode.NEAREST, antialias=False)[0].long()
+            return x.reshape(x.shape[0] * x.shape[1], *x.shape[2:])[idx].contiguous()
+
+        def smooth(x):
+            return None if x is None else TF.resize(x[None], size=[h, w], antialias=True)[0].contiguous()
+
+        return SupervisionTargets(depth=nearest(depth), mask=smooth(mask), labels=nearest(labels), features=nearest(features),
+                                  loss_weight=smooth(loss_weight))
+
     def _crop_and_scale_targets(self, depth, mask, labels, features, loss_weight, info: CameraInfo) -> SupervisionTargets:
         """The targets cropped to the tile multiple and, if the image was autoscaled, resized to its size."""
+        if _is_equirect(info):
+            return self._resize_equirect_targets(depth, mask, labels, features, loss_weight, info)
         out = []
         for x, nearest in ((depth, True), (mask, False), (loss_weight, False)):
             if x is not None:
@@ -249,11 +301,19 @@ class ImagePoseDataset(torch.utils.data.Dataset):
         K[1, :] = K[1, :] * image.shape[1] / rec["camera_height"]
         if self.with_targets:
             targets = self._load_targets(rec, image.shape[1], image.shape[2])
-        image = _crop_to_tiles(image)
-        info = CameraInfo(camera_intrinsics=K, camera_height=image.shape[1], camera_width=image.shape[2],
-                          camera_id=rec["camera_id"], distortion=self._distortion(rec),
-                          rolling_shutter=self._rolling_shutter(rec), motion_blur=self._motion_blur(rec),
-                          defocus=self._defocus(rec))
+        distortion = self._distortion(rec)
+        if distortion is not None and distortion.model == "equirectangular":
+            info = CameraInfo(camera_intrinsics=K, camera_height=image.shape[1], camera_width=image.shape[2],
+                              camera_id=rec["camera_id"], distortion=distortion, rolling_shutter=self._rolling_shutter(rec),
+                              motion_blur=self._motion_blur(rec), defocus=self._defocus(rec))
+            h, w = image.shape[1], image.shape[2]
+            image, info = _resize_equirect(image, info, h - h % TILE_HEIGHT, w - w % TILE_WIDTH)
+        else:
+            image = _crop_to_tiles(image)
+            info = CameraInfo(camera_intrinsics=K, camera_height=image.shape[1], camera_width=image.shape[2],
+                              camera_id=rec["camera_id"], distortion=distortion,
+                              rolling_shutter=self._rolling_shutter(rec), motion_blur=self._motion_blur(rec),
+                              defocus=self._defocus(rec))
         image, info = self._autoscale_image_and_camera_info(image, info)
         if self.with_targets:
             return image, q, t, info, self._crop_and_scale_targets(*targets, info)

@@ -86,10 +86,34 @@ def psnr(pred: torch.Tensor, target: torch.Tensor) -> float:
     return float("inf") if mse == 0 else -10.0 * math.log10(mse)
 
 
-def downsample_image_and_camera_info(image: torch.Tensor, camera_info: CameraInfo, downsample_factor: int):
-    """GaussianPointTrainer.py:98-116: antialiased resize, crop to multiples of 16, scale fx fy cx cy."""
+def _is_equirect(camera_info: CameraInfo) -> bool:
+    return getattr(getattr(camera_info, "distortion", None), "model", None) == "equirectangular"
+
+
+def _downsampled_size(camera_info: CameraInfo, downsample_factor: int):
+    """(h, w) of the resize: the schedule's size, or for an equirectangular view its tile multiple, so that the panorama
+    keeps covering 360 degrees instead of losing columns to the crop."""
     h = camera_info.camera_height // downsample_factor
     w = camera_info.camera_width // downsample_factor
+    if _is_equirect(camera_info):
+        h, w = h - h % 16, w - w % 16
+    return h, w
+
+
+def downsample_image_and_camera_info(image: torch.Tensor, camera_info: CameraInfo, downsample_factor: int):
+    """GaussianPointTrainer.py:98-116: antialiased resize, crop to multiples of 16, scale fx fy cx cy.  An equirectangular
+    view is resized straight to multiples of 16 and keeps 2 pi fx = W."""
+    h, w = _downsampled_size(camera_info, downsample_factor)
+    if _is_equirect(camera_info):
+        image = F.interpolate(image[None], size=(h, w), mode="bilinear", antialias=True, align_corners=False)[0]
+        K = camera_info.camera_intrinsics.clone()
+        sy = h / camera_info.camera_height
+        K[0, 2] *= w / camera_info.camera_width
+        K[0, 0] = w / (2.0 * math.pi)
+        K[1, 1] *= sy
+        K[1, 2] *= sy
+        return image[:3].contiguous(), CameraInfo(camera_intrinsics=K, camera_height=h, camera_width=w,
+                                                  camera_id=camera_info.camera_id, distortion=camera_info.distortion)
     image = F.interpolate(image[None], size=(h, w), mode="bilinear", antialias=True, align_corners=False)[0]
     w -= w % 16
     h -= h % 16
@@ -121,8 +145,7 @@ def downsample_targets(targets: SupervisionTargets, camera_info: CameraInfo, dow
     """The targets of a view at the schedule's resolution: the mask and the loss weight with the image's antialiased resize,
     the depth, the labels and the feature map with nearest neighbour (a sparse map stays sparse, nothing is blended across
     an edge); all cropped like the image."""
-    h = camera_info.camera_height // downsample_factor
-    w = camera_info.camera_width // downsample_factor
+    h, w = _downsampled_size(camera_info, downsample_factor)
     hc, wc = h - h % 16, w - w % 16
     mask = depth = None
     if targets.mask is not None:
@@ -301,6 +324,18 @@ class GaussianPointCloudTrainer:
                                                                  requires_grad=True)
         self._distortion = self._distortion_leaves(config, train_views)
         self._dist = config.distortion_learning_rate > 0
+        # an equirectangular view (CameraInfo.distortion, model "equirectangular") trains the points alone, through the
+        # autograd loop
+        if any(_is_equirect(v[3]) for v in train_views):
+            for name, on in (("fused_step", fused_step), ("mip_filter_3d", bool(config.mip_filter_3d)),
+                             ("pose refinement (pose_learning_rate > 0)", self._pose),
+                             ("intrinsics refinement (intrinsics_learning_rate > 0)", self._intr),
+                             ("distortion refinement (distortion_learning_rate > 0)", config.distortion_learning_rate > 0),
+                             ("motion refinement (rolling_shutter_learning_rate > 0)", config.rolling_shutter_learning_rate > 0),
+                             ("exposure-motion refinement (motion_blur_learning_rate > 0)", config.motion_blur_learning_rate > 0),
+                             ("defocus refinement (defocus_learning_rate > 0)", config.defocus_learning_rate > 0)):
+                if on:
+                    raise ValueError(f"{name} is not supported with an equirectangular view")
         # a view with a rolling shutter (CameraInfo.rolling_shutter) trains through the autograd loop alone
         if any(getattr(v[3], "rolling_shutter", None) is not None for v in train_views):
             for name, on in (("fused_step", fused_step), ("pose refinement (pose_learning_rate > 0)", self._pose),
