@@ -929,6 +929,31 @@ int gsb200_filter3d_from_views(const GsbFilter3dViewsArgs *args);
 /* sizeof(GsbFilter3dArgs), sizeof(GsbFilter3dViewsArgs) */
 void gsb200_abi_sizes_filter3d(int64_t *out2);
 
+/* Orthographic (parallel-projection) views (an extension: the reference projects through a pinhole).  Camera frame as
+ * everywhere (x right, y down, z forward), pc = W xyz + t:
+ *   u = K00 x + K01 y + K02,  v = K10 x + K11 y + K12   (K[:2] (x, y, 1), no divide; K's last row is not read)
+ * so fx = K00 and fy = K11 are pixels per scene unit.  Covariance: Sigma' = J W Sigma W^T J^T with J = K[:2,:2] [I2 0], which
+ * does not depend on pc: d(u, v)/d pc = J exactly and nothing is detached through J.  The 0.3 low-pass, rescale, 3-sigma radius,
+ * bounding box and reach filter are the pinhole's.  In view: near < z < far and (u, v) inside the image plus the boundary tiles,
+ * as the pinhole.  The depth is z: sort key, depth output, depth gradient and the hook's point_depth.  SH view direction: the
+ * camera's forward axis in the object's frame, row 2 of W, the same for every point (detached, as in every model).
+ * Pose and intrinsics gradients follow the pinhole's conventions with this J:
+ *   dL/dK[r][c] = sum guv_r (x, y, 1)_c + 2 sum_j B_r[j] W[c][j] (c = 0, 1),  B = G (J W) Sigma;  row 2 of dL/dK is zero.
+ * Known limit: a translation along the viewing axis changes only z, so it reaches the image only through the sort order and the
+ * depth output; the pose gradient along that axis comes from the depth term alone. */
+/* gsb200_forward_ext of an orthographic view, with the 3D smoothing filter of gsb200_forward_filter3d when `filter` is set (or
+ * NULL).  Before any CUDA call: the checks of gsb200_forward_filter3d; K is not read back and nothing synchronises. */
+int gsb200_forward_ortho(const GsbForwardArgs *args, const GsbExtraFeatureArgs *ext, const GsbFilter3dArgs *filter);
+/* gsb200_backward_calib of a frame rendered by gsb200_forward_ortho with the same filter; filter, pose and intrinsics may each be
+ * NULL.  Before any CUDA call: GSB_EUNSUPPORTED with GSB_FLAG_COMPACT_GRADS or for a filter together with a pose or intrinsics
+ * gradient, and GSB_EINVAL under the rules of gsb200_backward_filter3d and gsb200_backward_calib.  An image-only loss works with
+ * either loop-A kernel; the other terms keep their requirement of GSB_FLAG_BACKWARD_TRANSPOSED.  The pose and intrinsics sums
+ * are deterministic (per-CTA rows and finishing kernels, as gsb200_backward_calib). */
+int gsb200_backward_ortho(const GsbBackwardArgs *args, const float *grad_rasterized_depth, const float *rasterized_depth,
+                          const float *grad_pixel_accumulated_alpha, const GsbExtraFeatureArgs *ext,
+                          const GsbFilter3dArgs *filter, const GsbPoseGradArgs *pose,
+                          const GsbIntrinsicsGradArgs *intrinsics);
+
 /* Per-pixel weights of the image loss (an extension), for images whose views hold transient distractors (people, cars,
  * shadows that are in one photo and not the next).  For the image x (H,W,3) the image loss reads (the sliced image with an
  * appearance grid, the composited one with a background) and its ground truth g (3,H,W), with s (H,W) the static weight

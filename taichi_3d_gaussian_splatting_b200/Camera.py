@@ -6,7 +6,8 @@ GaussianPointCloudRasterisation.py:4).  ``LensDistortion`` and ``CameraInfo.dist
 projects through a pinhole only.  ``RollingShutter`` and ``CameraInfo.rolling_shutter`` are an extension as well: the reference
 projects every row with one global-shutter pose.  So are ``MotionBlur`` and ``CameraInfo.motion_blur``: the reference renders every
 view as if the shutter were instantaneous; and ``Defocus`` and ``CameraInfo.defocus``: the reference renders through an ideal
-pinhole, sharp at every depth.
+pinhole, sharp at every depth.  ``LensDistortion("orthographic", ())`` and ``orthographic_view`` are an extension too: the
+reference has no parallel projection.
 """
 import math
 from dataclasses import dataclass
@@ -14,7 +15,7 @@ from typing import Optional, Sequence, Tuple
 
 import torch
 
-_LENS_COEFFICIENTS = {"opencv": 5, "fisheye": 4, "equirectangular": 0}
+_LENS_COEFFICIENTS = {"opencv": 5, "fisheye": 4, "equirectangular": 0, "orthographic": 0}
 
 
 @dataclass(frozen=True)
@@ -30,7 +31,14 @@ class LensDistortion:
     ``"equirectangular"`` (no coefficients) is the 360-degree panorama of Insta360, Ricoh Theta, GoPro Max and drone panorama
     modes: u = fx atan2(x, z) + cx (wrapped into [0, W)), v = fy atan2(y, sqrt(x^2 + z^2)) + cy, with 2 pi fx = W (definition in
     ``include/gsb200.h``; K from ``equirectangular_intrinsics``).  It renders and trains the point gradients only: no pose,
-    intrinsics or lens gradient, rolling shutter, motion blur, defocus, 3D filter or view-parallel exchange."""
+    intrinsics or lens gradient, rolling shutter, motion blur, defocus, 3D filter or view-parallel exchange.
+
+    ``"orthographic"`` (no coefficients) is the parallel projection of orthophotos, orthorectified aerial tiles, satellite
+    crops and CAD renders: u = K00 x + K01 y + K02, v = K10 x + K11 y + K12 of the camera-frame point, no divide, so fx and fy
+    are pixels per scene unit (definition in ``include/gsb200.h``; K from ``orthographic_intrinsics``).  Depth is z, and the SH
+    colour is seen along the camera's forward axis.  It renders and trains the point, pose and intrinsics gradients, with
+    depth, alpha, features and the 3D filter (the filter without camera gradients); no lens gradient, rolling shutter, motion
+    blur, defocus or view-parallel exchange."""
     model: str
     coefficients: Tuple[float, ...]
 
@@ -53,6 +61,17 @@ class LensDistortion:
             raise ValueError(f"width and height must be positive, got {width} x {height}")
         return torch.tensor([[w / (2.0 * math.pi), 0.0, w / 2.0], [0.0, h / math.pi, h / 2.0], [0.0, 0.0, 1.0]],
                             dtype=torch.float32)
+
+    @staticmethod
+    def orthographic_intrinsics(width: int, height: int, pixel_size: float) -> torch.Tensor:
+        """K (3,3) float32 of an orthographic view: fx = fy = 1 / pixel_size (pixels per scene unit; ``pixel_size`` is the
+        ground sampling distance of an orthophoto) and the principal point at the image centre."""
+        w, h, d = int(width), int(height), float(pixel_size)
+        if w <= 0 or h <= 0:
+            raise ValueError(f"width and height must be positive, got {width} x {height}")
+        if not (math.isfinite(d) and d > 0.0):
+            raise ValueError(f"pixel_size must be finite and > 0, got {pixel_size}")
+        return torch.tensor([[1.0 / d, 0.0, w / 2.0], [0.0, 1.0 / d, h / 2.0], [0.0, 0.0, 1.0]], dtype=torch.float32)
 
     @staticmethod
     def from_colmap(model_name: str, params: Sequence[float]) -> Tuple[torch.Tensor, Optional["LensDistortion"]]:
@@ -245,3 +264,34 @@ class CameraView:
     camera_id: int
     image_id: int
     timestamp: Optional[int] = None
+
+
+def orthographic_view(centre: Sequence[float], forward: Sequence[float], up: Sequence[float], width: int, height: int,
+                      pixel_size: float, camera_id: int = 0) -> Tuple[torch.Tensor, torch.Tensor, CameraInfo]:
+    """(q_pointcloud_camera (1,4) xyzw, t_pointcloud_camera (1,3), CameraInfo) of an orthographic camera at ``centre`` looking
+    along ``forward``, with ``up`` toward the top of the image (made orthogonal to ``forward``), ``pixel_size`` scene units per
+    pixel.  The orthophoto recipe: a nadir view (``forward`` = -``up`` of the scene, ``up`` any horizontal direction that
+    should point to the top of the image) above the scene; where alpha >= 1/2 the surface height is centre . up_scene - depth.
+    ``camera_id`` keys the trainer's intrinsics correction: give orthographic views an id of their own when they train
+    beside pinhole views, so that refining the pixel size does not move a lens' focal length.  ``ValueError`` for a zero or
+    non-finite direction, or ``up`` parallel to ``forward``."""
+    from .utils import rotation_matrix_to_quaternion_torch
+    c = torch.as_tensor(centre, dtype=torch.float64).reshape(3)
+    f = torch.as_tensor(forward, dtype=torch.float64).reshape(3)
+    u = torch.as_tensor(up, dtype=torch.float64).reshape(3)
+    if not (bool(torch.isfinite(c).all()) and bool(torch.isfinite(f).all()) and bool(torch.isfinite(u).all())):
+        raise ValueError("centre, forward and up must be finite")
+    if float(f.norm()) == 0.0:
+        raise ValueError("forward must not be zero")
+    z = f / f.norm()
+    down = -(u - torch.dot(u, z) * z)  # the camera's y axis points down the image
+    if float(down.norm()) <= 1e-9 * max(float(u.norm()), 1e-300):
+        raise ValueError("up must not be zero or parallel to forward")
+    y = down / down.norm()
+    x = torch.linalg.cross(y, z)
+    R = torch.stack([x, y, z], dim=1)  # columns: the camera axes in the scene frame
+    q = rotation_matrix_to_quaternion_torch(R[None]).to(torch.float32)
+    K = LensDistortion.orthographic_intrinsics(width, height, pixel_size)
+    ci = CameraInfo(camera_intrinsics=K, camera_height=int(height), camera_width=int(width), camera_id=int(camera_id),
+                    distortion=LensDistortion("orthographic", ()))
+    return q.contiguous(), c.to(torch.float32)[None].contiguous(), ci

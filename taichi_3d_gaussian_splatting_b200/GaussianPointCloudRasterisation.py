@@ -49,6 +49,16 @@ def _is_equirect(camera_info) -> bool:
     return distortion is not None and distortion.model == "equirectangular"
 
 
+# The lens argument of an orthographic view: it has no GsbLensArgs and goes through gsb200_forward_ortho /
+# gsb200_backward_ortho
+_ORTHO = "orthographic"
+
+
+def _is_ortho(camera_info) -> bool:
+    distortion = getattr(camera_info, "distortion", None)
+    return distortion is not None and distortion.model == "orthographic"
+
+
 def _ptr(t: Optional[torch.Tensor]) -> Optional[int]:
     return None if t is None else t.data_ptr()
 
@@ -669,6 +679,11 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                     if lens is _EQUIRECT:
                         _lib.check(lib.gsb200_forward_equirect(ctypes.byref(args), ctypes.byref(ext) if ext is not None else None),
                                    "gsb200_forward_equirect")
+                    elif lens is _ORTHO:
+                        _lib.check(lib.gsb200_forward_ortho(
+                            ctypes.byref(args), ctypes.byref(ext) if ext is not None else None,
+                            ctypes.byref(_lib.GsbFilter3dArgs(filter3d=_ptr(point_filter_3d)))
+                            if point_filter_3d is not None else None), "gsb200_forward_ortho")
                     elif defocus is not None:
                         _lib.check(lib.gsb200_forward_defocus(
                             ctypes.byref(args), ctypes.byref(ext) if ext is not None else None,
@@ -731,6 +746,9 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
         if distortion.model == "equirectangular":
             self._check_equirect(camera_info, lens_coefficients)
             return _EQUIRECT
+        if distortion.model == "orthographic":
+            self._check_ortho(camera_info, lens_coefficients)
+            return _ORTHO
         for name, on in (("differentiable_pose", self.differentiable_pose),
                          ("differentiable_intrinsics", self.differentiable_intrinsics),
                          ("a gradient_exchange", self.gradient_exchange is not None)):
@@ -773,6 +791,26 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                 raise ValueError(f"an equirectangular camera is not supported with {name}")
         if int(camera_info.camera_width) % TILE_WIDTH != 0:
             raise ValueError(f"an equirectangular view's width must be a multiple of {TILE_WIDTH}, got {camera_info.camera_width}")
+
+    def _check_ortho(self, camera_info, lens_coefficients=None, rolling_shutter_motion=None, exposure_motion=None,
+                     defocus_parameters=None) -> None:
+        """``ValueError`` for what an orthographic view does not combine with (include/gsb200.h): the lens-coefficient,
+        rolling-shutter, motion-blur and defocus gradients and records, and the view-parallel exchange.  The 3D filter with
+        camera-parameter gradients is refused by ``_check_filter_3d``."""
+        for name, on in (("differentiable_distortion", self.differentiable_distortion),
+                         ("differentiable_rolling_shutter", self.differentiable_rolling_shutter),
+                         ("differentiable_motion_blur", self.differentiable_motion_blur),
+                         ("differentiable_defocus", self.differentiable_defocus),
+                         ("a gradient_exchange", self.gradient_exchange is not None),
+                         ("a rolling shutter (camera_info.rolling_shutter)", getattr(camera_info, "rolling_shutter", None) is not None),
+                         ("motion blur (camera_info.motion_blur)", getattr(camera_info, "motion_blur", None) is not None),
+                         ("defocus (camera_info.defocus)", getattr(camera_info, "defocus", None) is not None),
+                         ("lens_coefficients", lens_coefficients is not None),
+                         ("rolling_shutter_motion", rolling_shutter_motion is not None),
+                         ("exposure_motion", exposure_motion is not None),
+                         ("defocus_parameters", defocus_parameters is not None)):
+            if on:
+                raise ValueError(f"an orthographic camera is not supported with {name}")
 
     def _rolling_shutter_args(self, camera_info, motion=None) -> Optional[_lib.GsbRollingShutterArgs]:
         """The C rolling-shutter argument of ``camera_info.rolling_shutter`` (None: the global-shutter kernels; row_time is
@@ -961,6 +999,33 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                 _lib.check(lib.gsb200_backward_equirect(ctypes.byref(args), _ptr(grad_depth), _ptr(depth), _ptr(grad_alpha),
                                                         ctypes.byref(ext) if ext is not None else None),
                            "gsb200_backward_equirect")
+            elif ctx.lens is _ORTHO:  # the 3D filter, pose and intrinsics gradients (the filter never with the latter two)
+                pose_args = intr_args = None
+                if pose:
+                    n_obj = ctx.num_objects
+                    q_pc = q_pointcloud_camera.detach().contiguous()
+                    grad_q = torch.empty((n_obj, 4), dtype=torch.float32, device=device)
+                    grad_t = torch.empty((n_obj, 3), dtype=torch.float32, device=device)
+                    pose_temp = torch.empty((max(int(lib.gsb200_pose_grad_temp_bytes(n_obj)), 16) // 4,),
+                                            dtype=torch.float32, device=device)
+                    pose_args = _lib.GsbPoseGradArgs(q_pointcloud_camera=_ptr(q_pc), grad_q_pointcloud_camera=_ptr(grad_q),
+                                                     grad_t_pointcloud_camera=_ptr(grad_t), temp=_ptr(pose_temp))
+                if intrinsics:
+                    grad_K = torch.empty((3, 3), dtype=torch.float32, device=device)
+                    intr_temp = torch.empty((int(lib.gsb200_intrinsics_grad_temp_bytes()) // 4,), dtype=torch.float32,
+                                            device=device)
+                    intr_args = _lib.GsbIntrinsicsGradArgs(grad_camera_intrinsics=_ptr(grad_K), temp=_ptr(intr_temp))
+                ext = None
+                if extra_features is not None and grad_feature_map is not None:
+                    grad_map = _f32(grad_feature_map)
+                    ext = _lib.GsbExtraFeatureArgs(channels=extra_features.shape[1], features=_ptr(extra_features),
+                                                   grad_rasterized=_ptr(grad_map), grad_features=_ptr(grad_extra_features))
+                _lib.check(lib.gsb200_backward_ortho(
+                    ctypes.byref(args), _ptr(grad_depth), _ptr(depth), _ptr(grad_alpha),
+                    ctypes.byref(ext) if ext is not None else None,
+                    ctypes.byref(_lib.GsbFilter3dArgs(filter3d=_ptr(ctx.filter_3d))) if ctx.filter_3d is not None else None,
+                    ctypes.byref(pose_args) if pose_args is not None else None,
+                    ctypes.byref(intr_args) if intr_args is not None else None), "gsb200_backward_ortho")
             elif ctx.defocus is not None:  # no other camera-parameter gradient (refused in forward)
                 ext = None
                 if extra_features is not None and grad_feature_map is not None:
@@ -1213,11 +1278,21 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
         ``defocus_parameters`` (with ``differentiable_defocus``; an extension): a (2,) float32 tensor (a, rho) on any
         device.  Its values are the aperture and inverse focus distance rendered (a negative a renders as |a|), and the
         backward returns dL/d ``defocus_parameters`` on the tensor's device.  ``ValueError`` for a camera without defocus, a
-        tensor of the wrong shape or dtype, or an operator without the option.  None: no defocus gradient."""
+        tensor of the wrong shape or dtype, or an operator without the option.  None: no defocus gradient.
+        ``camera_info.distortion = LensDistortion("orthographic", ())`` (an extension): render and differentiate a parallel
+        projection (``gsb200_forward_ortho`` / ``gsb200_backward_ortho``; definition in ``include/gsb200.h``).  Depth is z,
+        and the SH colour is seen along the camera's forward axis.  Works with extra features, depth, alpha,
+        ``differentiable_pose``, ``differentiable_intrinsics``, ``point_filter_3d`` (not with the two camera gradients) and
+        either backward kernel for an image-only loss.  ``ValueError``, before any device work, with
+        ``differentiable_distortion``, ``differentiable_rolling_shutter``, ``differentiable_motion_blur``,
+        ``differentiable_defocus``, a ``gradient_exchange``, a rolling shutter, motion blur or defocus on the camera, or their
+        tensors."""
         camera_info = input_data.camera_info
         if _is_equirect(camera_info):  # the argument checks, before any device work
             self._check_equirect(camera_info, lens_coefficients, rolling_shutter_motion, point_filter_3d, exposure_motion,
                                  defocus_parameters)
+        if _is_ortho(camera_info):
+            self._check_ortho(camera_info, lens_coefficients, rolling_shutter_motion, exposure_motion, defocus_parameters)
         assert camera_info.camera_width % TILE_WIDTH == 0
         assert camera_info.camera_height % TILE_HEIGHT == 0
         if getattr(camera_info, "defocus", None) is not None or defocus_parameters is not None:

@@ -243,7 +243,7 @@ EXPORTS = (
     "gsb200_robust_image_loss", "gsb200_train_step_robust", "gsb200_abi_sizes_robust", "gsb200_forward_motion_blur",
     "gsb200_backward_motion_blur", "gsb200_motion_blur_grad_temp_bytes", "gsb200_abi_sizes_motion_blur",
     "gsb200_forward_defocus", "gsb200_backward_defocus", "gsb200_defocus_grad_temp_bytes", "gsb200_abi_sizes_defocus",
-    "gsb200_forward_equirect", "gsb200_backward_equirect",
+    "gsb200_forward_equirect", "gsb200_backward_equirect", "gsb200_forward_ortho", "gsb200_backward_ortho",
 )
 
 _lib = None
@@ -385,6 +385,13 @@ def load() -> ctypes.CDLL:
                                              ctypes.POINTER(GsbLensArgs), ctypes.POINTER(GsbRollingShutterArgs),
                                              ctypes.POINTER(GsbFilter3dArgs)]
     lib.gsb200_backward_filter3d.restype = ctypes.c_int
+    lib.gsb200_forward_ortho.argtypes = [ctypes.POINTER(GsbForwardArgs), ctypes.POINTER(GsbExtraFeatureArgs),
+                                         ctypes.POINTER(GsbFilter3dArgs)]
+    lib.gsb200_forward_ortho.restype = ctypes.c_int
+    lib.gsb200_backward_ortho.argtypes = [ctypes.POINTER(GsbBackwardArgs), c_vp, c_vp, c_vp, ctypes.POINTER(GsbExtraFeatureArgs),
+                                          ctypes.POINTER(GsbFilter3dArgs), ctypes.POINTER(GsbPoseGradArgs),
+                                          ctypes.POINTER(GsbIntrinsicsGradArgs)]
+    lib.gsb200_backward_ortho.restype = ctypes.c_int
     lib.gsb200_train_step_filter3d.argtypes = [ctypes.POINTER(GsbTrainStepArgs), ctypes.POINTER(GsbSupervisionArgs),
                                                ctypes.POINTER(GsbFeatureTrainArgs), ctypes.POINTER(GsbAppearanceArgs),
                                                ctypes.POINTER(GsbMcmcStepArgs), ctypes.POINTER(GsbFilter3dArgs)]

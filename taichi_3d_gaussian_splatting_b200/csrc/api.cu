@@ -385,9 +385,10 @@ int64_t gsb200_defocus_grad_temp_bytes(void) {
 
 // The forward of gsb200_forward_filter3d / gsb200_forward_motion_blur / gsb200_forward_defocus after their own checks
 // (filter3d and blur / defocus: checked, never together)
+// (model: an internal projection that replaces lens_args, gsb200_forward_ortho's)
 static int forward_checked(const GsbForwardArgs *a, const GsbExtraFeatureArgs *ext, const GsbLensArgs *lens_args,
                            const GsbRollingShutterArgs *rs_args, const float *filter3d, const BlurParams *blur,
-                           const DefocusParams *defocus = nullptr);
+                           const DefocusParams *defocus = nullptr, const LensParams *model = nullptr);
 
 int gsb200_forward_filter3d(const GsbForwardArgs *a, const GsbExtraFeatureArgs *ext, const GsbLensArgs *lens_args,
                             const GsbRollingShutterArgs *rs_args, const GsbFilter3dArgs *filter) {
@@ -422,11 +423,12 @@ int gsb200_forward_defocus(const GsbForwardArgs *a, const GsbExtraFeatureArgs *e
 
 static int forward_checked(const GsbForwardArgs *a, const GsbExtraFeatureArgs *ext, const GsbLensArgs *lens_args,
                            const GsbRollingShutterArgs *rs_args, const float *filter3d, const BlurParams *blur,
-                           const DefocusParams *defocus) {
+                           const DefocusParams *defocus, const LensParams *model) {
     LensParams lens_params;
     const LensParams *lens;
     int lrc = check_lens(rs_args ? "forward_rolling_shutter" : "forward_lens", lens_args, &lens_params, &lens);
     if (lrc != GSB_OK) return lrc;
+    if (model) lens = model;
     RsParams rs_params;
     const RsParams *rs;
     if ((lrc = check_rs("forward_rolling_shutter", rs_args, &rs_params, &rs)) != GSB_OK) return lrc;
@@ -471,7 +473,7 @@ static int backward_impl(const GsbBackwardArgs *a, bool skip_on_overflow, const 
                          const GsbRollingShutterGradArgs *rs_grad = nullptr, const float *filter3d = nullptr,
                          const BlurParams *blur = nullptr, const GsbMotionBlurGradArgs *blur_grad = nullptr,
                          const DefocusParams *defocus = nullptr, const GsbDefocusGradArgs *defocus_grad = nullptr,
-                         bool equirect = false) {
+                         bool equirect = false, bool ortho = false) {
     if (!a) {
         set_error("backward: args is null");
         return GSB_EINVAL;
@@ -528,6 +530,7 @@ static int backward_impl(const GsbBackwardArgs *a, bool skip_on_overflow, const 
         GSB_CUDA_CHECK(cudaMemsetAsync(ext->grad_features, 0, (size_t)a->num_points * ext->channels * 4, st));
     if ((rc = launch_blend_backward(*a, ws, st, grad_depth, depth, grad_alpha, ext, equirect)) != GSB_OK) return rc;
     if (equirect) return launch_backward_points_equirect(*a, ws, st, grad_depth != nullptr);
+    if (ortho) return launch_backward_points_ortho(*a, ws, st, grad_depth != nullptr, pose, intr, filter3d);
     if (defocus)  // a NULL blur is zero motion
         return launch_backward_points_blur(*a, ws, st, grad_depth != nullptr, lens, rs, blur ? *blur : BlurParams{}, nullptr,
                                            defocus, defocus_grad);
@@ -564,7 +567,7 @@ static int backward_checked(const GsbBackwardArgs *a, const float *grad_rasteriz
                             const RsParams *rs = nullptr, const GsbRollingShutterGradArgs *rs_grad = nullptr,
                             const float *filter3d = nullptr, const BlurParams *blur = nullptr,
                             const GsbMotionBlurGradArgs *blur_grad = nullptr, const DefocusParams *defocus = nullptr,
-                            const GsbDefocusGradArgs *defocus_grad = nullptr);
+                            const GsbDefocusGradArgs *defocus_grad = nullptr, bool ortho = false);
 
 int gsb200_backward_motion_blur(const GsbBackwardArgs *a, const float *grad_rasterized_depth, const float *rasterized_depth,
                                 const float *grad_pixel_accumulated_alpha, const GsbExtraFeatureArgs *ext,
@@ -798,7 +801,7 @@ static int backward_checked(const GsbBackwardArgs *a, const float *grad_rasteriz
                             const GsbIntrinsicsGradArgs *intr, const LensParams *lens, const GsbLensGradArgs *lens_grad,
                             const RsParams *rs, const GsbRollingShutterGradArgs *rs_grad, const float *filter3d,
                             const BlurParams *blur, const GsbMotionBlurGradArgs *blur_grad, const DefocusParams *defocus,
-                            const GsbDefocusGradArgs *defocus_grad) {
+                            const GsbDefocusGradArgs *defocus_grad, bool ortho) {
     if (intr) {
         if (!intr->grad_camera_intrinsics || !intr->temp) {
             set_error("backward_calib: null grad_camera_intrinsics / temp pointer");
@@ -864,7 +867,7 @@ static int backward_checked(const GsbBackwardArgs *a, const float *grad_rasteriz
         return GSB_EUNSUPPORTED;
     }
     return backward_impl(a, false, grad_rasterized_depth, rasterized_depth, grad_pixel_accumulated_alpha, ext, pose, intr, lens,
-                         lens_grad, rs, rs_grad, filter3d, blur, blur_grad, defocus, defocus_grad);
+                         lens_grad, rs, rs_grad, filter3d, blur, blur_grad, defocus, defocus_grad, false, ortho);
 }
 
 // The intrinsics of an equirectangular view (include/gsb200.h), read back from the device: 2 pi K00 = W within
@@ -977,6 +980,34 @@ int gsb200_backward_equirect(const GsbBackwardArgs *a, const float *grad_rasteri
     }
     return backward_impl(a, false, grad_rasterized_depth, rasterized_depth, grad_pixel_accumulated_alpha, ext, nullptr, nullptr,
                          nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, true);
+}
+
+int gsb200_forward_ortho(const GsbForwardArgs *a, const GsbExtraFeatureArgs *ext, const GsbFilter3dArgs *filter) {
+    const float *filter3d;
+    int rc = check_filter3d("forward_ortho", filter, &filter3d);
+    if (rc != GSB_OK) return rc;
+    LensParams ortho{};
+    ortho.model = LENS_ORTHO;
+    return forward_checked(a, ext, nullptr, nullptr, filter3d, nullptr, nullptr, &ortho);
+}
+
+int gsb200_backward_ortho(const GsbBackwardArgs *a, const float *grad_rasterized_depth, const float *rasterized_depth,
+                          const float *grad_pixel_accumulated_alpha, const GsbExtraFeatureArgs *ext, const GsbFilter3dArgs *filter,
+                          const GsbPoseGradArgs *pose, const GsbIntrinsicsGradArgs *intr) {
+    const float *filter3d;
+    int rc = check_filter3d("backward_ortho", filter, &filter3d);
+    if (rc != GSB_OK) return rc;
+    if (a != nullptr && (a->flags & GSB_FLAG_COMPACT_GRADS)) {
+        set_error("backward_ortho: the orthographic view is not implemented for the compact rows of the view-parallel exchange "
+                  "(GSB_FLAG_COMPACT_GRADS)");
+        return GSB_EUNSUPPORTED;
+    }
+    if (filter3d && (pose || intr)) {
+        set_error("backward_ortho: the 3D filter is not implemented with the pose or intrinsics gradient");
+        return GSB_EUNSUPPORTED;
+    }
+    return backward_checked(a, grad_rasterized_depth, rasterized_depth, grad_pixel_accumulated_alpha, ext, pose, intr, nullptr,
+                            nullptr, nullptr, nullptr, filter3d, nullptr, nullptr, nullptr, nullptr, true);
 }
 
 int gsb200_backward_with_depth(const GsbBackwardArgs *a, const float *grad_rasterized_depth, const float *rasterized_depth) {

@@ -454,9 +454,14 @@ constexpr int RS_GRAD_VALUES = 6;
 // EQUI = true (gsb200_backward_equirect): the frame is an equirectangular panorama (include/gsb200.h): d uv / d pc and the J
 // of Sigma' are both equirect_jacobian at point_in_camera (J detached, as for every model), and with DEPTH word 11 is dL/dr
 // of the ray distance, which enters pc along pc / r.  Non-compact, without any other camera path or gradient.
+// ORTHO = true (gsb200_backward_ortho): the frame is an orthographic view (include/gsb200.h): d uv / d pc and the J of Sigma'
+// are both K[:2,:2] [I 0], exact (J does not depend on pc), the depth term is the pinhole's along z, and the SH basis is taken
+// along row 2 of W.  With POSE, J enters dL/dW through all four of its entries: dL/dW[r] = gp_r xyz + 2 sum_a J[a][r] B_a.  With
+// INTR: dL/dK[r][c] = guv_r (x, y, 1)_c + 2 sum_j B_r[j] W[c][j] for c in {0, 1}.  Non-compact; with or without DEPTH, FILTER,
+// POSE and INTR (FILTER never with POSE or INTR); without the other camera paths.
 template <bool COMPACT, bool DEPTH, bool POSE, bool INTR = false, bool LENS = false, bool LGRAD = false, bool RS = false,
           bool MGRAD = false, bool FILTER = false, bool BLUR = false, bool BGRAD = false, bool DEFOCUS = false,
-          bool DGRAD = false, bool EQUI = false>
+          bool DGRAD = false, bool EQUI = false, bool ORTHO = false>
 __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, float *s_pose, float *pose_partials,
                                                      int num_objects, float *s_intr = nullptr,
                                                      float *intr_partials = nullptr, const LensParams lens = LensParams(),
@@ -478,6 +483,8 @@ __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, fl
     static_assert(!DGRAD || DEFOCUS, "the defocus gradient needs the defocus path");
     static_assert(!EQUI || (!COMPACT && !POSE && !INTR && !LENS && !RS && !FILTER && !BLUR),
                   "the panorama is implemented for the dense rows without the other camera paths");
+    static_assert(!ORTHO || (!COMPACT && !LENS && !RS && !BLUR && !EQUI),
+                  "the orthographic view is implemented for the dense rows without the other camera paths");
     constexpr bool CAM6 = MGRAD || BGRAD || DGRAD;  // the rows of a camera gradient (rolling shutter, exposure or defocus)
     // One thread per scene row: rows outside the frustum get their zeros here (no separate memset of the
     // dense (N,3)/(N,56) gradients), rows inside get the chain rule.  A warp owns 32 consecutive rows, i.e. one
@@ -592,6 +599,10 @@ __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, fl
             eq_r = sqrtf(rho * rho + pcy * pcy);
             equirect_jacobian(Kc[0], Kc[4], pcv, rho, eq_r, dj);
         }
+        if (ORTHO) {  // d uv / d pc = K[:2,:2] [I 0]
+            dj[0] = Kc[0]; dj[1] = Kc[1]; dj[2] = 0.0f;
+            dj[3] = Kc[3]; dj[4] = Kc[4]; dj[5] = 0.0f;
+        }
         float gx[3];
 #pragma unroll
         for (int c = 0; c < 3; ++c) {
@@ -608,7 +619,7 @@ __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, fl
 #pragma unroll
             for (int k = 0; k < 6; ++k) J[k] = Jl[k];
         }
-        if (EQUI) {
+        if (EQUI || ORTHO) {
 #pragma unroll
             for (int k = 0; k < 6; ++k) J[k] = dj[k];
         }
@@ -745,10 +756,16 @@ __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, fl
             weighted_u_sigma(U, R, es, g00, g01, g11, B0, B1);
             const float xw[3] = {x, y, z};
 #pragma unroll
-            for (int c = 0; c < 3; ++c) {  // J = [J0 0 J2; 0 J4 J5]
-                pv[c] = gp[0] * xw[c] + 2.0f * (J[0] * B0[c]);
-                pv[3 + c] = gp[1] * xw[c] + 2.0f * (J[4] * B1[c]);
-                pv[6 + c] = gp[2] * xw[c] + 2.0f * (J[2] * B0[c] + J[5] * B1[c]);
+            for (int c = 0; c < 3; ++c) {  // J = [J0 0 J2; 0 J4 J5]; ORTHO: J = [J0 J1 0; J3 J4 0]
+                if (ORTHO) {
+                    pv[c] = gp[0] * xw[c] + 2.0f * (J[0] * B0[c] + J[3] * B1[c]);
+                    pv[3 + c] = gp[1] * xw[c] + 2.0f * (J[1] * B0[c] + J[4] * B1[c]);
+                    pv[6 + c] = gp[2] * xw[c];
+                } else {
+                    pv[c] = gp[0] * xw[c] + 2.0f * (J[0] * B0[c]);
+                    pv[3 + c] = gp[1] * xw[c] + 2.0f * (J[4] * B1[c]);
+                    pv[6 + c] = gp[2] * xw[c] + 2.0f * (J[2] * B0[c] + J[5] * B1[c]);
+                }
                 pv[9 + c] = gp[c];
             }
             pose_obj = ob;
@@ -758,6 +775,24 @@ __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, fl
             // (pc detached in J): dL/dfx += 2 sum_c B0[c] (W[0][c]/z - x W[2][c]/z^2), dL/dfy likewise with B1 and row 1
             float B0[3], B1[3];
             weighted_u_sigma(U, R, es, g00, g01, g11, B0, B1);
+            if (ORTHO) {
+                // uv = K[:2] (x, y, 1): dL/dK[r][c] += guv_r (x, y, 1)_c.  Sigma' through J = K[:2,:2] [I 0]:
+                // dL/dK[r][c] += 2 sum_j B_r[j] W[c][j] for c in {0, 1}
+                float s00 = 0.0f, s01 = 0.0f, s10 = 0.0f, s11 = 0.0f;
+#pragma unroll
+                for (int c = 0; c < 3; ++c) {
+                    s00 += B0[c] * Wm[c];
+                    s01 += B0[c] * Wm[3 + c];
+                    s10 += B1[c] * Wm[c];
+                    s11 += B1[c] * Wm[3 + c];
+                }
+                iv[0] = a0.x * pcx + 2.0f * s00;
+                iv[1] = a0.x * pcy + 2.0f * s01;
+                iv[2] = a0.x;
+                iv[3] = a0.y * pcx + 2.0f * s10;
+                iv[4] = a0.y * pcy + 2.0f * s11;
+                iv[5] = a0.y;
+            } else {
             const float ux = pcx * iz, uy = pcy * iz;
             float sx0 = 0.0f, sy1 = 0.0f;
 #pragma unroll
@@ -771,6 +806,7 @@ __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, fl
             iv[3] = a0.y * ux;
             iv[4] = a0.y * uy + 2.0f * sy1;
             iv[5] = a0.y;
+            }
         }
         if (LGRAD) {
             // position: dL/d(xd, yd) = K[:2,:2]^T guv.  Sigma' through J = diag(fx, fy) D P (pc detached, D differentiated in k
@@ -827,7 +863,8 @@ __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, fl
         } else {
         // SH basis along xyz - camera centre (GPCR:731-732, 749; SH:10-32)
         float sh[16];
-        sh_basis(x - p.t_pc_cam[3 * ob], y - p.t_pc_cam[3 * ob + 1], z - p.t_pc_cam[3 * ob + 2], sh);
+        if (ORTHO) sh_basis(Wm[6], Wm[7], Wm[8], sh);  // the camera's forward axis, as the forward
+        else sh_basis(x - p.t_pc_cam[3 * ob], y - p.t_pc_cam[3 * ob + 1], z - p.t_pc_cam[3 * ob + 2], sh);
 
         my_xyz[0] = gx[0]; my_xyz[1] = gx[1]; my_xyz[2] = gx[2];
         float4 *gf = reinterpret_cast<float4 *>(my_feat);
@@ -1191,6 +1228,22 @@ backward_points_calib_kernel(const PointsBwdCalibParams p) {
     __shared__ float s_intr[(GSB_POINTS_THREADS / 32) * INTR_VALUES];
     backward_points_body<false, DEPTH, POSE, true>(p, POSE ? s_pose : nullptr, p.pose_partials, p.num_objects, s_intr,
                                                    p.intr_partials);
+}
+
+// The parameter block of the ORTHO instantiations (pose_partials / num_objects read only with POSE, intr_partials only with
+// INTR, filter3d only with FILTER).
+struct PointsBwdOrthoParams : PointsBwdCalibParams {
+    const float *filter3d;
+};
+
+template <bool DEPTH, bool POSE, bool INTR, bool FILTER>
+__global__ void __launch_bounds__(GSB_POINTS_THREADS, POSE && INTR ? 4 : POSE || INTR ? 5 : 6)  // as the pinhole's kernels
+backward_points_ortho_kernel(const PointsBwdOrthoParams p) {
+    __shared__ float s_pose[POSE ? (GSB_POINTS_THREADS / 32) * GSB_POSE_MAX_OBJECTS * POSE_VALUES : 1];
+    __shared__ float s_intr[INTR ? (GSB_POINTS_THREADS / 32) * INTR_VALUES : 1];
+    backward_points_body<false, DEPTH, POSE, INTR, false, false, false, false, FILTER, false, false, false, false, false, true>(
+        p, POSE ? s_pose : nullptr, p.pose_partials, p.num_objects, INTR ? s_intr : nullptr, p.intr_partials, LensParams(),
+        nullptr, nullptr, RsParams(), nullptr, nullptr, p.filter3d);
 }
 
 // One CTA: adds the `blocks` partial rows in a fixed order (strided per thread, then a fixed shared-memory tree) and
@@ -1605,6 +1658,51 @@ int launch_backward_points_calib(const GsbBackwardArgs &a, const Workspace &ws, 
     intrinsics_finish_kernel<<<1, INTR_FINISH_THREADS, 0, stream>>>(p.intr_partials, (int)blocks,
                                                                      intr.grad_camera_intrinsics);
     GSB_CUDA_CHECK(cudaGetLastError());
+    return GSB_OK;
+}
+
+template <bool DEPTH>
+static void launch_ortho_kernel(bool pose, bool intr, bool filter, int blocks, cudaStream_t stream,
+                                const PointsBwdOrthoParams &p) {
+    if (filter) backward_points_ortho_kernel<DEPTH, false, false, true><<<blocks, GSB_POINTS_THREADS, 0, stream>>>(p);
+    else if (pose && intr) backward_points_ortho_kernel<DEPTH, true, true, false><<<blocks, GSB_POINTS_THREADS, 0, stream>>>(p);
+    else if (pose) backward_points_ortho_kernel<DEPTH, true, false, false><<<blocks, GSB_POINTS_THREADS, 0, stream>>>(p);
+    else if (intr) backward_points_ortho_kernel<DEPTH, false, true, false><<<blocks, GSB_POINTS_THREADS, 0, stream>>>(p);
+    else backward_points_ortho_kernel<DEPTH, false, false, false><<<blocks, GSB_POINTS_THREADS, 0, stream>>>(p);
+}
+
+// The ORTHO per-point kernel: without camera gradients on the grid of launch_backward_points; with pose or intrinsics on the
+// POSE kernel's grid (it depends on N alone), then the finishing kernels, as launch_backward_points_calib.  filter3d never comes
+// with pose or intr.  The caller checked the arguments.
+int launch_backward_points_ortho(const GsbBackwardArgs &a, const Workspace &ws, cudaStream_t stream, bool depth_grad,
+                                 const GsbPoseGradArgs *pose, const GsbIntrinsicsGradArgs *intr, const float *filter3d) {
+    PointsBwdOrthoParams p;
+    static_cast<PointsBwdParams &>(p) = make_points_params(a, ws, nullptr);
+    p.pose_partials = pose ? static_cast<float *>(pose->temp) : nullptr;
+    p.num_objects = pose ? a.num_objects : 0;
+    p.intr_partials = intr ? static_cast<float *>(intr->temp) : nullptr;
+    p.filter3d = filter3d;
+    const bool cam_grad = pose != nullptr || intr != nullptr;
+    long long blocks = a.num_points > 0 ? (a.num_points + GSB_POINTS_THREADS - 1) / GSB_POINTS_THREADS : 0;
+    const long long cap = cam_grad ? (long long)GSB_POSE_PARTIAL_BLOCKS : 16LL * num_sms();
+    if (blocks > cap) blocks = cap;
+    if (blocks > 0) {
+        const bool f = filter3d != nullptr;
+        if (depth_grad) launch_ortho_kernel<true>(pose != nullptr, intr != nullptr, f, (int)blocks, stream, p);
+        else launch_ortho_kernel<false>(pose != nullptr, intr != nullptr, f, (int)blocks, stream, p);
+        GSB_CUDA_CHECK(cudaGetLastError());
+    }
+    if (pose) {
+        pose_finish_kernel<<<a.num_objects, POSE_FINISH_THREADS, 0, stream>>>(
+            p.pose_partials, (int)blocks, a.num_objects, pose->q_pointcloud_camera, a.t_pointcloud_camera,
+            pose->grad_q_pointcloud_camera, pose->grad_t_pointcloud_camera);
+        GSB_CUDA_CHECK(cudaGetLastError());
+    }
+    if (intr) {
+        intrinsics_finish_kernel<<<1, INTR_FINISH_THREADS, 0, stream>>>(p.intr_partials, (int)blocks,
+                                                                         intr->grad_camera_intrinsics);
+        GSB_CUDA_CHECK(cudaGetLastError());
+    }
     return GSB_OK;
 }
 

@@ -95,6 +95,11 @@ int launch_blend_backward(const GsbBackwardArgs &a, const Workspace &ws, cudaStr
 // gsb200_backward_equirect: the EQUIRECT per-point kernel (dense gradients as launch_backward_points, d uv / d pc and J of the
 // panorama, depth r); arguments checked by the caller
 int launch_backward_points_equirect(const GsbBackwardArgs &a, const Workspace &ws, cudaStream_t stream, bool depth_grad);
+// gsb200_backward_ortho: the ORTHO per-point kernel (dense gradients as launch_backward_points; with pose / intr also the camera
+// sums and their finishing kernels, as launch_backward_points_calib; filter3d never with pose or intr); arguments checked by the
+// caller
+int launch_backward_points_ortho(const GsbBackwardArgs &a, const Workspace &ws, cudaStream_t stream, bool depth_grad,
+                                 const GsbPoseGradArgs *pose, const GsbIntrinsicsGradArgs *intr, const float *filter3d);
 int launch_backward_points(const GsbBackwardArgs &a, const Workspace &ws, cudaStream_t stream,
                            const long long *skip_flag = nullptr, bool depth_grad = false);
 // gsb200_backward_lens: the LENS per-point kernel (dense gradients as launch_backward_points, d uv / d pc and J through the
@@ -595,6 +600,11 @@ __device__ __forceinline__ float equirect_wrap_u(float u, float tile_x0, float W
     return u + W * rintf(((tile_x0 + 0.5f * (float)GSB_TILE_WIDTH) - u) / W);
 }
 #endif
+
+// ---- orthographic (parallel-projection) views (gsb200_forward_ortho / gsb200_backward_ortho; definition in include/gsb200.h).
+// LENS_ORTHO is, like LENS_EQUIRECT, an internal model code of the per-point kernels' LENS switch, never a GsbLensArgs value.
+// (u, v) = K[:2] (x, y, 1) and J = d(u, v)/d pc = K[:2,:2] [I 0] do not depend on z: the projection is linear.
+constexpr int LENS_ORTHO = 0x4F52;
 
 // Host, double: the r^2 bound of LensParams::r2_max (definition in include/gsb200.h), inf when the map never folds back.
 // The smallest positive root of the derivative polynomial in t = r^2 (opencv) or t = theta^2 (fisheye) is bracketed

@@ -227,6 +227,9 @@ __device__ __forceinline__ bool tile_reachable(const SplatReach &r, float u, flo
 // in-view test and J come from equirect_project / equirect_jacobian (common.cuh), the depth is the ray distance r (record,
 // sort key, CNT_MAX_DEPTH_KEY), the footprint's columns from equirect_columns, and the key's tile column is taken modulo
 // W/16.  Not with ROLLING, FILTER or BLUR.
+// LENS = LENS_ORTHO (gsb200_forward_ortho): the orthographic view (definition in include/gsb200.h).  (u, v) = K[:2] (x, y, 1)
+// without a divide, J = K[:2,:2] [I 0], the in-view test and the depth z are the pinhole's, and the SH view direction is the
+// camera's forward axis, row 2 of W, for every point.  With or without FILTER; not with ROLLING or BLUR.
 template <typename KeyT, int LENS, bool ROLLING = false, bool FILTER = false, bool BLUR = false, bool DEFOCUS = false>
 __device__ __forceinline__ void preprocess_body(const PreParams p, const LensParams lens, const RsParams rs = RsParams(),
                                                 const float *filter3d = nullptr, const BlurParams blur = BlurParams(),
@@ -235,6 +238,8 @@ __device__ __forceinline__ void preprocess_body(const PreParams p, const LensPar
     static_assert(!DEFOCUS || BLUR, "the defocus runs on the motion-blur path");
     constexpr bool EQUIRECT = LENS == LENS_EQUIRECT;
     static_assert(!EQUIRECT || (!ROLLING && !FILTER && !BLUR), "the panorama is implemented without the camera extensions");
+    constexpr bool ORTHO = LENS == LENS_ORTHO;
+    static_assert(!ORTHO || (!ROLLING && !BLUR), "the orthographic view is implemented without the camera motions");
     __shared__ unsigned int s_ticket;
     __shared__ unsigned long long s_warp_sums[SCAN_BLOCK_THREADS / 32];
     __shared__ unsigned long long s_block_exclusive;
@@ -321,6 +326,9 @@ __device__ __forceinline__ void preprocess_body(const PreParams p, const LensPar
             in = equirect_project(Kc, p.W, p.near_plane, p.far_plane, pc, u, v, eq_rho, depth) &&
                  v >= (float)(-GSB_TILE_HEIGHT * GSB_BOUNDARY_TILES) &&
                  v < (float)(p.H + GSB_TILE_HEIGHT * GSB_BOUNDARY_TILES);
+        } else if (ORTHO) {  // K[:2] (x, y, 1): no divide, K's last row unread
+            u = (Kc[0] * pc[0] + Kc[1] * pc[1]) + Kc[2];
+            v = (Kc[3] * pc[0] + Kc[4] * pc[1]) + Kc[5];
         } else if (LENS == GSB_LENS_PINHOLE) {
             float uv1[3];
             matmul<3, 3, 1>(Kc, pc, uv1);
@@ -363,13 +371,17 @@ __device__ __forceinline__ void preprocess_body(const PreParams p, const LensPar
             const float fx = Kc[0], fy = Kc[4];
             J[0] = fx / pc[2]; J[1] = 0.0f; J[2] = -(fx * pc[0]) / (pc[2] * pc[2]);
             J[3] = 0.0f; J[4] = fy / pc[2]; J[5] = -(fy * pc[1]) / (pc[2] * pc[2]);
-            if (LENS != GSB_LENS_PINHOLE) {  // J = diag(fx, fy) D P, P = [1/z 0 -x/z^2; 0 1/z -y/z^2]
+            if (LENS != GSB_LENS_PINHOLE && !ORTHO) {  // J = diag(fx, fy) D P, P = [1/z 0 -x/z^2; 0 1/z -y/z^2]
                 J[0] = (fx * D[0]) / pc[2]; J[1] = (fx * D[1]) / pc[2];
                 J[2] = -(fx * (D[0] * pc[0] + D[1] * pc[1])) / (pc[2] * pc[2]);
                 J[3] = (fy * D[2]) / pc[2]; J[4] = (fy * D[3]) / pc[2];
                 J[5] = -(fy * (D[2] * pc[0] + D[3] * pc[1])) / (pc[2] * pc[2]);
             }
             if (EQUIRECT) equirect_jacobian(fx, fy, pc, eq_rho, depth, J);
+            if (ORTHO) {  // J = K[:2,:2] [I 0]
+                J[0] = Kc[0]; J[1] = Kc[1]; J[2] = 0.0f;
+                J[3] = Kc[3]; J[4] = Kc[4]; J[5] = 0.0f;
+            }
             float R[9], S[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0}, RS[9], RSS[9], RT[9], Sigma[9];
             rotation_from_quaternion(qv.x, qv.y, qv.z, qv.w, R);
             S[0] = exp_cr(f[0]); S[4] = exp_cr(f[1]); S[8] = exp_cr(f[2]);
@@ -458,8 +470,9 @@ __device__ __forceinline__ void preprocess_body(const PreParams p, const LensPar
             const float radius = sqrtf(large) * 3.0f;
             // GPCR:299-310 opacity + SH colour along (xyz - camera centre)
             const float opacity = 1.0f / (1.0f + exp_cr(-f[3]));
-            float dx = x - __ldg(&pb->centre[0]), dy = y - __ldg(&pb->centre[1]),
-                  dz = z - __ldg(&pb->centre[2]);
+            // ORTHO: along the camera's forward axis, row 2 of W, the same for every point
+            float dx = ORTHO ? T[8] : x - __ldg(&pb->centre[0]), dy = ORTHO ? T[9] : y - __ldg(&pb->centre[1]),
+                  dz = ORTHO ? T[10] : z - __ldg(&pb->centre[2]);
             float dn = sqrtf(dx * dx + dy * dy + dz * dz);
             float dinv = 1.0f / dn;
             dx = dinv * dx; dy = dinv * dy; dz = dinv * dz;
@@ -771,6 +784,13 @@ preprocess_equirect_kernel(const PreParams p) {
     preprocess_body<KeyT, LENS_EQUIRECT>(p, LensParams());
 }
 
+// FILTER = false ignores p.filter3d
+template <typename KeyT, bool FILTER>
+__global__ void __launch_bounds__(SCAN_BLOCK_THREADS, GSB_PRE_MIN_BLOCKS)
+preprocess_ortho_kernel(const PreFilterParams p) {
+    preprocess_body<KeyT, LENS_ORTHO, false, FILTER>(p, p.lens, RsParams(), p.filter3d);
+}
+
 #ifndef GSB_HOST_EMU  // tests/simt compiles the kernels above as host C++ under the SIMT emulator
 // The pose blocks of n (q, t) pairs without clearing anything (gsb200_filter3d_from_views: one per view and object).
 int launch_pose_blocks(const float *q_pc, const float *t_pc, int n, PoseBlock *poses, cudaStream_t stream) {
@@ -856,7 +876,20 @@ int launch_preprocess(const GsbForwardArgs &a, const Workspace &ws, cudaStream_t
     p.point_in_camera = ws.point_in_camera;
     p.keys = ws.keys_a;
     p.vals = ws.vals_a;
-    if (blur != nullptr || defocus != nullptr) {
+    if (lens != nullptr && lens->model == LENS_ORTHO) {  // gsb200_forward_ortho: the 3D filter or no other extension
+        PreFilterParams pf;
+        static_cast<PreParams &>(pf) = p;
+        pf.lens = *lens;
+        pf.filter3d = filter3d;
+        const dim3 grid(L.scan_blocks), block(SCAN_BLOCK_THREADS);
+        if (L.key_bytes == 4) {
+            if (filter3d != nullptr) preprocess_ortho_kernel<unsigned int, true><<<grid, block, 0, stream>>>(pf);
+            else preprocess_ortho_kernel<unsigned int, false><<<grid, block, 0, stream>>>(pf);
+        } else {
+            if (filter3d != nullptr) preprocess_ortho_kernel<unsigned long long, true><<<grid, block, 0, stream>>>(pf);
+            else preprocess_ortho_kernel<unsigned long long, false><<<grid, block, 0, stream>>>(pf);
+        }
+    } else if (blur != nullptr || defocus != nullptr) {
         PreBlurParams pb;
         static_cast<PreParams &>(pb) = p;
         pb.lens = lens != nullptr ? *lens : LensParams();

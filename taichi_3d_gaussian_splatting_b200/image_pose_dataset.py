@@ -27,6 +27,8 @@ rescaling, cropping and autoscale leave them unchanged.
 With ``"model": "equirectangular"`` and ``"coefficients": []`` the view is a 360-degree panorama: its width is resized (not
 cropped) to a multiple of 16, autoscale resizes it the same way, and fx is set so that 2 pi fx = W; its targets are resized
 with it (the depth, labels and features by nearest neighbour).
+With ``"model": "orthographic"`` and ``"coefficients": []`` the view is a parallel projection (K[:2] applied to the camera-frame
+(x, y, 1), fx and fy in pixels per scene unit): crop, resize and autoscale scale K exactly as for a pinhole.
 An optional record key ``rolling_shutter`` (an extension), ``{"linear_velocity": [3], "angular_velocity": [3],
 "readout_time": s}``, gives the view's ``CameraInfo.rolling_shutter`` (``Camera.RollingShutter.from_camera_velocity``: the
 camera's own velocities in its frame, in scene units/s and rad/s, as visual-inertial odometry reports them, and the sensor's
@@ -135,7 +137,7 @@ class ImagePoseDataset(torch.utils.data.Dataset):
 
     @staticmethod
     def _distortion(rec: dict) -> Optional[LensDistortion]:
-        """The optional record key ``"distortion": {"model": "opencv" | "fisheye" | "equirectangular", "coefficients":
+        """The optional record key ``"distortion": {"model": "opencv" | "fisheye" | "equirectangular" | "orthographic", "coefficients":
         [...]}``."""
         d = rec.get("distortion")
         if d is None:

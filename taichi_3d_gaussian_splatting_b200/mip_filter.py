@@ -95,6 +95,9 @@ def compute_filter_3d(point_cloud: torch.Tensor, point_invalid_mask: torch.Tenso
     device."""
     if len(views) < 1:
         raise ValueError("compute_filter_3d needs at least one view")
+    if any(getattr(getattr(ci, "distortion", None), "model", None) == "orthographic" for _, _, ci in views):
+        # the rule's frustum and sampling rate (f / z) are the pinhole's
+        raise ValueError("compute_filter_3d does not take orthographic views")
     if not (math.isfinite(near_plane) and near_plane >= 0 and math.isfinite(variance) and variance >= 0):
         raise ValueError(f"near_plane and variance must be finite and >= 0, got {near_plane}, {variance}")
     device = point_cloud.device

@@ -262,15 +262,15 @@ def render_views(op, make_input, view_ids: Sequence[int], streams: Optional[Sequ
     stages of frame i+1 (per-point stage, radix sort: a few hundred resident warps) run under the issue-bound blend of frame i
     instead of behind it.  Every frame owns its workspace and outputs, the operator's only host wait per frame ends after that
     frame's first kernel, so nothing else changes; the caller must synchronise the streams (or wait on the outputs' stream)
-    before reading the images.  ``ValueError`` for an equirectangular view (not implemented here; render it with ``op``
-    directly), raised before the view is rendered."""
+    before reading the images.  ``ValueError`` for an equirectangular or orthographic view (not implemented here; render it
+    with ``op`` directly), raised before the view is rendered."""
     out = {}
     with torch.no_grad():
         for n, i in enumerate(view_ids):
             inp = make_input(i)
             distortion = getattr(inp.camera_info, "distortion", None)
-            if distortion is not None and distortion.model == "equirectangular":
-                raise ValueError("parallel.render_views does not render equirectangular views")
+            if distortion is not None and distortion.model in ("equirectangular", "orthographic"):
+                raise ValueError(f"parallel.render_views does not render {distortion.model} views")
             if streams:
                 with torch.cuda.stream(streams[n % len(streams)]):
                     image, depth, count = op(inp)

@@ -120,3 +120,59 @@ def make_panorama_scene(num_points: int, height: int, width: int, sigma_med: flo
                                distortion=LensDistortion("equirectangular", ())),
         q_pointcloud_camera=torch.tensor([[0.0, math.sin(half), 0.0, math.cos(half)]], dtype=torch.float32),
         t_pointcloud_camera=torch.zeros((1, 3), dtype=torch.float32))
+
+
+# The raised blocks of make_aerial_scene: (x0, x1, y0, y1, height) as fractions of the ground's width (x0..y1) and of the
+# camera's height above the ground (height).  They do not overlap.
+AERIAL_BLOCKS = ((-0.30, -0.10, -0.25, 0.05, 0.20), (0.10, 0.35, 0.10, 0.30, 0.35), (0.05, 0.25, -0.40, -0.20, 0.12))
+
+
+def aerial_height(x: torch.Tensor, y: torch.Tensor, ground_width: float, altitude: float) -> torch.Tensor:
+    """The surface height of make_aerial_scene at scene (x, y): a block's height on its top, 0 elsewhere."""
+    h = torch.zeros_like(x)
+    for x0, x1, y0, y1, hb in AERIAL_BLOCKS:
+        inside = (x >= x0 * ground_width) & (x < x1 * ground_width) & (y >= y0 * ground_width) & (y < y1 * ground_width)
+        h = torch.where(inside, torch.full_like(x, hb * altitude), h)
+    return h
+
+
+def aerial_texture(x: torch.Tensor, y: torch.Tensor, ground_width: float) -> torch.Tensor:
+    """(..., 3) colours in [0.15, 0.85] of make_aerial_scene's ground at scene (x, y): smooth stripes of 1/8 and 1/6 of the
+    ground's width, so that a render at a few pixels per stripe period resolves them."""
+    a = 2.0 * math.pi * x / (ground_width / 8.0)
+    b = 2.0 * math.pi * y / (ground_width / 6.0)
+    return torch.stack([0.5 + 0.35 * torch.sin(a), 0.5 + 0.35 * torch.cos(b), 0.5 + 0.35 * torch.sin(a) * torch.cos(b)], -1)
+
+
+def make_aerial_scene(num_points: int, height: int, width: int, seed: int, pixel_size: float = 0.01,
+                      altitude: float = 5.0) -> SyntheticScene:
+    """A drone-survey-like scene for orthographic views: a textured ground plane z = 0 (scene up = +z) with the raised
+    blocks of ``AERIAL_BLOCKS``, made of flat, nearly opaque Gaussians at random positions on the visible surface (the blocks'
+    tops; their sides are not drawn), coloured by ``aerial_texture`` through the SH DC term alone.  The ground is 10 % wider
+    than the image's footprint at ``pixel_size`` scene units per pixel.  The camera is the nadir orthographic view of
+    ``Camera.orthographic_view`` at (0, 0, ``altitude``) with +y toward the top of the image, so pixel (u, v) sees scene
+    x = (u - W/2) pixel_size, y = (H/2 - v) pixel_size, and the height under it is ``altitude`` - depth."""
+    from .Camera import orthographic_view
+    g = torch.Generator(device="cpu").manual_seed(seed)
+    N = int(num_points)
+    gw, gh = 1.1 * width * pixel_size, 1.1 * height * pixel_size
+    u = torch.rand((N, 2), generator=g, dtype=torch.float32)
+    x, y = (u[:, 0] - 0.5) * gw, (u[:, 1] - 0.5) * gh
+    z = aerial_height(x, y, gw, altitude)
+    xyz = torch.stack([x, y, z], -1)
+    spacing = math.sqrt(gw * gh / max(N, 1))
+    q = torch.zeros((N, 4), dtype=torch.float32)
+    q[:, 3] = 1.0
+    s = torch.empty((N, 3), dtype=torch.float32)
+    s[:, 0:2] = math.log(0.7 * spacing)
+    s[:, 2] = math.log(0.1 * spacing)
+    logit = torch.full((N, 1), 4.0)
+    rgb = aerial_texture(x, y, gw)
+    sh = torch.zeros((N, 3, 16), dtype=torch.float32)
+    sh[:, :, 0] = torch.logit(rgb) / 0.28209479177387814
+    feats = torch.cat([q, s, logit, sh.reshape(N, 48)], dim=-1).contiguous()
+    q_pc, t_pc, ci = orthographic_view((0.0, 0.0, altitude), (0.0, 0.0, -1.0), (0.0, 1.0, 0.0), width, height, pixel_size)
+    return SyntheticScene(
+        point_cloud=xyz.contiguous(), point_cloud_features=feats,
+        point_invalid_mask=torch.zeros((N,), dtype=torch.int8), point_object_id=torch.zeros((N,), dtype=torch.int32),
+        camera_info=ci, q_pointcloud_camera=q_pc, t_pointcloud_camera=t_pc)

@@ -41,6 +41,10 @@ a rolling shutter and motion blur; the downsampled camera keeps (a, rho) (they a
 view-parallel exchange.  Optional defocus refinement (``TrainConfig.defocus_learning_rate``): per defocused view, its (a, rho),
 differentiated by the operator's ``differentiable_defocus`` and stepped by its own Adam; it needs a non-zero aperture (both
 gradients vanish at a = 0).  ``validation`` renders every view as its camera says: defocused views defocused.
+Orthographic views (an extension; ``CameraInfo.distortion = LensDistortion("orthographic", ())``) train and validate through
+the autograd loop, mixed with pinhole views, with pose and intrinsics refinement (a translation along a view's axis reaches its
+image only through the sort order and depth).  Not with ``fused_step``, ``mip_filter_3d``, lens, rolling-shutter motion,
+exposure-motion or defocus refinement, or the view-parallel exchange.
 Optional appearance compensation (an extension; ``TrainConfig.appearance_grid``): one bilateral grid per training view
 (``appearance.apply_bilateral_grid``), initialised to the identity, slices the image the image loss sees (after the
 background composite), with a TV prior and its own Adam that steps only the visited view's grid.  It acts on the image alone,
@@ -59,6 +63,7 @@ the view-parallel gradient exchange.
 The rasteriser is injected (default: the CUDA operator) so that tests can run the identical loop with the
 CPU oracle behind the same interface and compare PSNR trajectories.
 """
+import dataclasses
 import math
 from dataclasses import dataclass, field
 from typing import Callable, List, Optional, Tuple
@@ -88,6 +93,10 @@ def psnr(pred: torch.Tensor, target: torch.Tensor) -> float:
 
 def _is_equirect(camera_info: CameraInfo) -> bool:
     return getattr(getattr(camera_info, "distortion", None), "model", None) == "equirectangular"
+
+
+def _is_ortho(camera_info: CameraInfo) -> bool:
+    return getattr(getattr(camera_info, "distortion", None), "model", None) == "orthographic"
 
 
 def _downsampled_size(camera_info: CameraInfo, downsample_factor: int):
@@ -308,8 +317,9 @@ class GaussianPointCloudTrainer:
         self._intr = config.intrinsics_learning_rate > 0
         if self._intr and fused_step:
             raise ValueError("fused_step does not implement intrinsics refinement (intrinsics_learning_rate > 0)")
-        # a view with lens distortion (CameraInfo.distortion) trains through the autograd loop alone
-        if any(getattr(v[3], "distortion", None) is not None for v in train_views):
+        # a view with lens distortion (CameraInfo.distortion) trains through the autograd loop alone; an orthographic view
+        # refines its pose and intrinsics like a pinhole
+        if any(getattr(v[3], "distortion", None) is not None and not _is_ortho(v[3]) for v in train_views):
             for name, on in (("fused_step", fused_step), ("pose refinement (pose_learning_rate > 0)", self._pose),
                              ("intrinsics refinement (intrinsics_learning_rate > 0)", self._intr)):
                 if on:
@@ -322,6 +332,17 @@ class GaussianPointCloudTrainer:
                 if ci.camera_id not in self._intrinsics:
                     self._intrinsics[ci.camera_id] = torch.zeros(4, dtype=torch.float32, device=ci.camera_intrinsics.device,
                                                                  requires_grad=True)
+        # an orthographic view (CameraInfo.distortion, model "orthographic") trains through the autograd loop, with pose and
+        # intrinsics refinement
+        self._ortho = any(_is_ortho(v[3]) for v in train_views)
+        if self._ortho:
+            for name, on in (("fused_step", fused_step), ("mip_filter_3d", bool(config.mip_filter_3d)),
+                             ("distortion refinement (distortion_learning_rate > 0)", config.distortion_learning_rate > 0),
+                             ("motion refinement (rolling_shutter_learning_rate > 0)", config.rolling_shutter_learning_rate > 0),
+                             ("exposure-motion refinement (motion_blur_learning_rate > 0)", config.motion_blur_learning_rate > 0),
+                             ("defocus refinement (defocus_learning_rate > 0)", config.defocus_learning_rate > 0)):
+                if on:
+                    raise ValueError(f"{name} is not supported with an orthographic view")
         self._distortion = self._distortion_leaves(config, train_views)
         self._dist = config.distortion_learning_rate > 0
         # an equirectangular view (CameraInfo.distortion, model "equirectangular") trains the points alone, through the
@@ -459,6 +480,8 @@ class GaussianPointCloudTrainer:
         if self._blurred and getattr(self.rasterisation, "gradient_exchange", None) is not None:
             raise ValueError("a motion-blurred view (CameraInfo.motion_blur) is not supported with the view-parallel "
                              "gradient exchange")
+        if self._ortho and getattr(self.rasterisation, "gradient_exchange", None) is not None:
+            raise ValueError("an orthographic view is not supported with the view-parallel gradient exchange")
         if self._mip and getattr(self.rasterisation, "gradient_exchange", None) is not None:
             raise ValueError("mip_filter_3d is not implemented for the view-parallel gradient exchange")
         if self._weighted and getattr(self.rasterisation, "gradient_exchange", None) is not None:
@@ -787,10 +810,10 @@ class GaussianPointCloudTrainer:
                 appearance_optimizer.zero_grad()
             view_index = self._next_view_index(iteration)
             image_gt, q, t, camera_info, targets = self._view(view_index, downsample_factor)
-            if self._intr:  # built every iteration: the cached downsampled camera must not freeze K
-                camera_info = CameraInfo(camera_intrinsics=self._intrinsics_of(view_index, downsample_factor),
-                                         camera_height=camera_info.camera_height, camera_width=camera_info.camera_width,
-                                         camera_id=camera_info.camera_id)
+            if self._intr:  # built every iteration: the cached downsampled camera must not freeze K (the rest is the view's,
+                # e.g. an orthographic view's projection)
+                camera_info = dataclasses.replace(camera_info,
+                                                  camera_intrinsics=self._intrinsics_of(view_index, downsample_factor))
             lens_kw = self._filter_kw()
             if self._dist and camera_info.distortion is not None:  # the lens as trained, the leaf as the autograd input
                 leaf = self._distortion[camera_info.camera_id]
