@@ -455,6 +455,35 @@ int gsb200_backward_lens_grad(const GsbBackwardArgs *args, const float *grad_ras
                               const float *grad_pixel_accumulated_alpha, const GsbExtraFeatureArgs *ext,
                               const GsbLensArgs *lens, const GsbLensGradArgs *lens_grad); /* lens_grad or NULL */
 
+/* Pose and intrinsics gradients through a lens (an extension): photometric self-calibration of OpenCV and fisheye cameras.
+ * The forward is gsb200_forward_lens, unchanged.  The conventions are those of the point, pose, intrinsics and coefficient
+ * gradients: J's dependence on pc is detached, D is evaluated at the detached point, rescale, the radius, tile membership
+ * and the SH view direction are detached, the r_max validity cut is not differentiated and the 0.99 clamp is
+ * straight-through.  Per in-camera point, with gp = dL/dpc (through uv by K[:2,:2] D P, plus dL/dz of the depth term),
+ * guv = dL/duv of its accumulator row and B0, B1 the rows of G (J W) Sigma with the lens J = diag(fx, fy) D P:
+ *   pose:        dL/dW += gp xyz^T + 2 J^T G (J W) Sigma,   dL/dtw += gp
+ *                (gsb200_backward_pose's formula with the lens J and gp; summed per object, then taken to (q_pc, t_pc))
+ *   intrinsics:  dL/dK[r][c] += guv_r (xd, yd, 1)_c                    r in {0,1}, c in {0,1,2}
+ *                dL/dK[0][0] += 2 sum_c B0[c] (D P W)[0][c],   dL/dK[1][1] += 2 sum_c B1[c] (D P W)[1][c],   row 2 is 0
+ *                (with D = I: gsb200_backward_calib's formula)
+ *   coefficients: gsb200_backward_lens_grad's.
+ * With any of the three, all of them come from one pass of one per-point kernel, whose per-CTA sums go to the three temps,
+ * and the three finishing kernels of gsb200_backward_pose, gsb200_backward_calib and gsb200_backward_lens_grad add them in
+ * block order -- no float atomics. */
+/* gsb200_backward_lens_grad that also writes the pose gradients of `pose` and the intrinsics gradient of `intrinsics`.
+ * Everything else the call writes (dense gradients, hook tensors, controller accumulators) is bit-identical to
+ * gsb200_backward_lens's, whichever camera gradients are on.  NULL pose and NULL intrinsics: exactly
+ * gsb200_backward_lens_grad, with the same kernels.  Otherwise, before any CUDA call: the lens checks of
+ * gsb200_forward_lens, and those of gsb200_backward_lens_grad (lens_grad), gsb200_backward_pose (pose) and
+ * gsb200_backward_calib (intrinsics); GSB_EINVAL for a NULL or pinhole lens; GSB_EUNSUPPORTED for GSB_FLAG_COMPACT_GRADS or
+ * num_objects > GSB_POSE_MAX_OBJECTS.  An image-only loss works with either loop-A kernel; the other terms keep their
+ * requirement of GSB_FLAG_BACKWARD_TRANSPOSED. */
+int gsb200_backward_lens_calib(const GsbBackwardArgs *args, const float *grad_rasterized_depth, const float *rasterized_depth,
+                               const float *grad_pixel_accumulated_alpha, const GsbExtraFeatureArgs *ext,
+                               const GsbLensArgs *lens, const GsbLensGradArgs *lens_grad, /* or NULL */
+                               const GsbPoseGradArgs *pose,                               /* or NULL */
+                               const GsbIntrinsicsGradArgs *intrinsics);                  /* or NULL */
+
 /* Rolling shutter (an extension: the reference projects every point with one global-shutter pose).  A view carries a motion
  * m = (v, w) (float32 x 6): the apparent motion of the scene in the camera frame over one full readout, top row to bottom
  * row; v in scene units, w in radians.  The view's pose (q, t) is the pose at mid-readout.  With pc0 = W xyz + tw the camera-

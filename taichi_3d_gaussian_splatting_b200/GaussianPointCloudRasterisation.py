@@ -264,6 +264,7 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
         differentiable_rolling_shutter: bool = False,
         differentiable_motion_blur: bool = False,
         differentiable_defocus: bool = False,
+        camera_gradients_through_lens: bool = False,
     ):
         """``exact_exp``: blend kernels use ``expf`` instead of ``ex2.approx`` (parity debugging).
         ``force_key64``: sort the reference's 64-bit ``tile << 32 | depth`` keys even when the live
@@ -322,7 +323,7 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
         r_max cut not differentiated); it includes every loss term the backward takes (image, depth, alpha, features), and no
         gradient factor is applied (``gsb200_backward_lens_grad``).  An image-only loss works with either backward kernel.
         ``ValueError`` with ``config.rgb_only`` or a ``gradient_exchange``; like every lens, not with
-        ``differentiable_pose`` or ``differentiable_intrinsics``.
+        ``differentiable_pose`` or ``differentiable_intrinsics`` unless ``camera_gradients_through_lens`` is set.
         ``differentiable_rolling_shutter``: ``forward`` takes ``rolling_shutter_motion``, the values of
         ``camera_info.rolling_shutter``'s motion (v, w) as an input of the autograd graph, and ``backward`` returns their
         gradient -- to refine the camera motion of a phone, action-camera or drone view whose velocity is roughly known or
@@ -341,7 +342,16 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
         distance of a defocused view from a non-zero aperture (both gradients vanish at a = 0).  beta is detached with respect
         to the point; the gradient flows through B_d = beta M M^T and the compensation c_b (``gsb200_backward_defocus``,
         definition in ``include/gsb200.h``) and includes every loss term the backward takes (image, depth, alpha, features).
-        ``ValueError`` with ``config.rgb_only`` or a ``gradient_exchange``."""
+        ``ValueError`` with ``config.rgb_only`` or a ``gradient_exchange``.
+        ``camera_gradients_through_lens`` (opt-in): ``differentiable_pose`` and ``differentiable_intrinsics`` also
+        differentiate an OpenCV or fisheye view, alone, together and with ``differentiable_distortion`` -- photometric
+        self-calibration of the poses, K and the lens of ordinary COLMAP output.  All three camera gradients come from one
+        pass of the per-point kernel (``gsb200_backward_lens_calib``; the model is in ``include/gsb200.h``): d uv / d pc =
+        K[:2,:2] D P, J = diag(fx, fy) D P inside Sigma', and dL/dK[r] through (xd, yd, 1), with the conventions of the
+        pinhole gradients (J and D at the detached point, the r_max cut not differentiated).  Without it a lens keeps refusing
+        the two options (``ValueError``), as before.  It changes nothing for a pinhole or orthographic view.  Camera
+        gradients stay refused with a rolling shutter, motion blur, defocus, an equirectangular panorama, ``point_filter_3d``
+        and a ``gradient_exchange``; the depth, alpha and feature terms keep needing the transposed backward kernel."""
         super().__init__()
         for name, on in (("differentiable_depth", differentiable_depth), ("differentiable_alpha", differentiable_alpha)):
             if on and backward_impl == "butterfly":
@@ -381,6 +391,7 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
         if differentiable_defocus and gradient_exchange is not None:
             raise ValueError("differentiable_defocus is not supported with a gradient_exchange (view-parallel training)")
         self.differentiable_defocus = bool(differentiable_defocus)
+        self.camera_gradients_through_lens = bool(camera_gradients_through_lens)
         self.config = config
         self.backward_valid_point_hook = backward_valid_point_hook
         self._flags = (_lib.GSB_FLAG_EXACT_EXP if exact_exp else 0) | (_lib.GSB_FLAG_FORCE_KEY64 if force_key64 else 0) | \
@@ -513,11 +524,13 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                             grad_pointcloud_features if ctx.needs_input_grad[1] else None, None, None, None, None, None, None,
                             grad_extra_features if ctx.has_extra_features and ctx.needs_input_grad[8] else None, None, None,
                             grad_m if motion_grad else None)
-                if ctx.lens_input:  # eleven inputs: the extra features' and K's slots (None with a lens), then the coefficients
+                if ctx.lens_input:  # eleven inputs: the extra features' and K's slots (K possibly None), then the coefficients
                     return (grad_pointcloud if ctx.needs_input_grad[0] else None,
-                            grad_pointcloud_features if ctx.needs_input_grad[1] else None, None, None, None, None, None, None,
-                            grad_extra_features if ctx.has_extra_features and ctx.needs_input_grad[8] else None, None,
-                            grad_k if lens_grad else None)
+                            grad_pointcloud_features if ctx.needs_input_grad[1] else None, None, None,
+                            grad_q if pose and ctx.needs_input_grad[4] else None,
+                            grad_t if pose and ctx.needs_input_grad[5] else None, None, None,
+                            grad_extra_features if ctx.has_extra_features and ctx.needs_input_grad[8] else None,
+                            grad_K if intrinsics else None, grad_k if lens_grad else None)
                 if ctx.intrinsics_input:  # ten inputs: the extra features' slot (possibly None), then K
                     return (grad_pointcloud if ctx.needs_input_grad[0] else None,
                             grad_pointcloud_features if ctx.needs_input_grad[1] else None, None, None,
@@ -749,11 +762,13 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
         if distortion.model == "orthographic":
             self._check_ortho(camera_info, lens_coefficients)
             return _ORTHO
-        for name, on in (("differentiable_pose", self.differentiable_pose),
-                         ("differentiable_intrinsics", self.differentiable_intrinsics),
+        through = self.camera_gradients_through_lens
+        for name, on in (("differentiable_pose", self.differentiable_pose and not through),
+                         ("differentiable_intrinsics", self.differentiable_intrinsics and not through),
                          ("a gradient_exchange", self.gradient_exchange is not None)):
             if on:
-                raise ValueError(f"a camera with lens distortion is not supported with {name}")
+                hint = "" if name.startswith("a ") else " (camera_gradients_through_lens=True differentiates through it)"
+                raise ValueError(f"a camera with lens distortion is not supported with {name}{hint}")
         if lens_coefficients is None:
             return _lib.lens_args(distortion)
         n = len(distortion.coefficients)
@@ -915,6 +930,27 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
         return _lib.GsbDefocusArgs(aperture=values[0], inverse_focus=values[1])
 
     # ------------------------------------------------------------------ backward plumbing
+    @staticmethod
+    def _camera_grad_args(lib, ctx, q_pointcloud_camera, pose, intrinsics, device):
+        """(GsbPoseGradArgs, grad_q, grad_t, the tensors it points at) with ``pose`` and (GsbIntrinsicsGradArgs, grad_K,
+        its temp) with ``intrinsics`` (else None): the C call's arguments, kept alive by the caller."""
+        pose_args = intr_args = None
+        if pose:
+            n_obj = ctx.num_objects
+            q_pc = q_pointcloud_camera.detach().contiguous()
+            grad_q = torch.empty((n_obj, 4), dtype=torch.float32, device=device)
+            grad_t = torch.empty((n_obj, 3), dtype=torch.float32, device=device)
+            temp = torch.empty((max(int(lib.gsb200_pose_grad_temp_bytes(n_obj)), 16) // 4,), dtype=torch.float32,
+                               device=device)
+            pose_args = (_lib.GsbPoseGradArgs(q_pointcloud_camera=_ptr(q_pc), grad_q_pointcloud_camera=_ptr(grad_q),
+                                              grad_t_pointcloud_camera=_ptr(grad_t), temp=_ptr(temp)), grad_q, grad_t, temp,
+                         q_pc)
+        if intrinsics:
+            grad_K = torch.empty((3, 3), dtype=torch.float32, device=device)
+            temp = torch.empty((int(lib.gsb200_intrinsics_grad_temp_bytes()) // 4,), dtype=torch.float32, device=device)
+            intr_args = (_lib.GsbIntrinsicsGradArgs(grad_camera_intrinsics=_ptr(grad_K), temp=_ptr(temp)), grad_K, temp)
+        return pose_args, intr_args
+
     def _run_backward(self, ctx, grad_rasterized_image, grad_rasterized_depth=None, grad_pixel_accumulated_alpha=None,
                       grad_feature_map=None, pose=False, intrinsics=False, lens_grad=False, motion_grad=False,
                       blur_grad=False, defocus_grad=False):
@@ -1099,7 +1135,32 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                     "gsb200_backward_rolling_shutter")
                 if motion_grad:
                     grad_m = grad_motion.to(ctx.motion_device)
-            elif ctx.lens is not None:  # neither pose nor intrinsics gradients (refused in forward)
+            elif ctx.lens is not None and (pose or intrinsics):  # one pass for pose, K and (lens_grad) the coefficients
+                ext = None
+                if extra_features is not None and grad_feature_map is not None:
+                    grad_map = _f32(grad_feature_map)
+                    ext = _lib.GsbExtraFeatureArgs(channels=extra_features.shape[1], features=_ptr(extra_features),
+                                                   grad_rasterized=_ptr(grad_map), grad_features=_ptr(grad_extra_features))
+                pose_args, intr_args = self._camera_grad_args(lib, ctx, q_pointcloud_camera, pose, intrinsics, device)
+                lens_grad_args = None
+                if lens_grad:
+                    grad_coefficients = torch.empty((5,), dtype=torch.float32, device=device)
+                    lens_temp = torch.empty((int(lib.gsb200_lens_grad_temp_bytes()) // 4,), dtype=torch.float32, device=device)
+                    lens_grad_args = _lib.GsbLensGradArgs(grad_coefficients=_ptr(grad_coefficients), temp=_ptr(lens_temp))
+                _lib.check(lib.gsb200_backward_lens_calib(
+                    ctypes.byref(args), _ptr(grad_depth), _ptr(depth), _ptr(grad_alpha),
+                    ctypes.byref(ext) if ext is not None else None, ctypes.byref(ctx.lens),
+                    ctypes.byref(lens_grad_args) if lens_grad_args is not None else None,
+                    ctypes.byref(pose_args[0]) if pose_args is not None else None,
+                    ctypes.byref(intr_args[0]) if intr_args is not None else None), "gsb200_backward_lens_calib")
+                if pose_args is not None:
+                    grad_q, grad_t = pose_args[1], pose_args[2]
+                if intr_args is not None:
+                    grad_K = intr_args[1]
+                if lens_grad:
+                    n, k_device = ctx.lens_coefficients_like
+                    grad_k = grad_coefficients[:n].to(k_device)
+            elif ctx.lens is not None:  # neither pose nor intrinsics gradients
                 ext = None
                 if extra_features is not None and grad_feature_map is not None:
                     grad_map = _f32(grad_feature_map)
@@ -1231,7 +1292,8 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
         ``input_data.camera_info.distortion`` (an extension; ``Camera.LensDistortion``): render and differentiate through
         an OpenCV radial-tangential or fisheye lens (``gsb200_forward_lens`` / ``gsb200_backward_lens``; definition in
         ``include/gsb200.h``).  Every output and option above works with a lens, except ``differentiable_pose``,
-        ``differentiable_intrinsics`` and a ``gradient_exchange`` (``ValueError``).
+        ``differentiable_intrinsics`` (both allowed with ``camera_gradients_through_lens``, ``gsb200_backward_lens_calib``)
+        and a ``gradient_exchange`` (``ValueError``).
         ``lens_coefficients`` (with ``differentiable_distortion``; an extension): a float32 tensor of the lens model's length
         (5 for ``opencv``, 4 for ``fisheye``), on any device.  Its values are the coefficients rendered (``camera_info.
         distortion`` supplies the model), and the backward returns dL/d ``lens_coefficients`` on the tensor's device.  The
@@ -1362,14 +1424,15 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                 input_data.point_cloud, input_data.point_cloud_features, input_data.point_invalid_mask,
                 input_data.point_object_id, input_data.q_pointcloud_camera, input_data.t_pointcloud_camera, camera_info,
                 input_data.color_max_sh_band, point_extra_features, None, None, rolling_shutter_motion)
-        if lens_coefficients is not None:  # the extra features' and K's slots first (K is refused with a lens)
+        if lens_coefficients is not None:  # the extra features' and K's slots first (K: with differentiable_intrinsics)
             self._lens_args(camera_info, lens_coefficients)  # the argument checks, before any device work
             if point_extra_features is not None:
                 self._check_extra_features(point_extra_features, input_data.point_cloud)
             return self._module_function.apply(
                 input_data.point_cloud, input_data.point_cloud_features, input_data.point_invalid_mask,
                 input_data.point_object_id, input_data.q_pointcloud_camera, input_data.t_pointcloud_camera, camera_info,
-                input_data.color_max_sh_band, point_extra_features, None, lens_coefficients)
+                input_data.color_max_sh_band, point_extra_features,
+                camera_info.camera_intrinsics if self.differentiable_intrinsics else None, lens_coefficients)
         if self.differentiable_intrinsics:  # K as a tenth input, after the extra features' slot
             if point_extra_features is not None:
                 self._check_extra_features(point_extra_features, input_data.point_cloud)

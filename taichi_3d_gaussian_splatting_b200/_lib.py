@@ -234,7 +234,8 @@ EXPORTS = (
     "gsb200_backward_aux", "gsb200_supervision_temp_bytes", "gsb200_train_step_aux", "gsb200_forward_ext",
     "gsb200_backward_ext", "gsb200_feature_loss_temp_bytes", "gsb200_train_step_ext", "gsb200_backward_pose",
     "gsb200_pose_grad_temp_bytes", "gsb200_backward_calib", "gsb200_intrinsics_grad_temp_bytes", "gsb200_forward_lens",
-    "gsb200_backward_lens", "gsb200_backward_lens_grad", "gsb200_lens_grad_temp_bytes", "gsb200_forward_rolling_shutter",
+    "gsb200_backward_lens", "gsb200_backward_lens_grad", "gsb200_lens_grad_temp_bytes", "gsb200_backward_lens_calib",
+    "gsb200_forward_rolling_shutter",
     "gsb200_backward_rolling_shutter", "gsb200_rolling_shutter_grad_temp_bytes", "gsb200_bilateral_grid_temp_bytes",
     "gsb200_bilateral_grid_forward", "gsb200_bilateral_grid_backward", "gsb200_train_step_appearance",
     "gsb200_mcmc_temp_bytes", "gsb200_mcmc_regulariser", "gsb200_mcmc_noise", "gsb200_mcmc_relocate", "gsb200_train_step_mcmc",
@@ -302,6 +303,11 @@ def load() -> ctypes.CDLL:
     lib.gsb200_backward_lens_grad.restype = ctypes.c_int
     lib.gsb200_lens_grad_temp_bytes.argtypes = []
     lib.gsb200_lens_grad_temp_bytes.restype = c_i64
+    lib.gsb200_backward_lens_calib.argtypes = [ctypes.POINTER(GsbBackwardArgs), c_vp, c_vp, c_vp,
+                                               ctypes.POINTER(GsbExtraFeatureArgs), ctypes.POINTER(GsbLensArgs),
+                                               ctypes.POINTER(GsbLensGradArgs), ctypes.POINTER(GsbPoseGradArgs),
+                                               ctypes.POINTER(GsbIntrinsicsGradArgs)]
+    lib.gsb200_backward_lens_calib.restype = ctypes.c_int
     lib.gsb200_forward_rolling_shutter.argtypes = [ctypes.POINTER(GsbForwardArgs), ctypes.POINTER(GsbExtraFeatureArgs),
                                                    ctypes.POINTER(GsbLensArgs), ctypes.POINTER(GsbRollingShutterArgs)]
     lib.gsb200_forward_rolling_shutter.restype = ctypes.c_int

@@ -539,6 +539,8 @@ static int backward_impl(const GsbBackwardArgs *a, bool skip_on_overflow, const 
         return launch_backward_points_filter(*a, ws, st, skip_on_overflow ? ws.counters + CNT_OVERFLOW : nullptr,
                                              grad_depth != nullptr, lens, rs, filter3d);
     if (rs) return launch_backward_points_rs(*a, ws, st, grad_depth != nullptr, lens, *rs, rs_grad);
+    if (lens && (pose || intr))
+        return launch_backward_points_lens_calib(*a, ws, st, grad_depth != nullptr, *lens, lens_grad, pose, intr);
     if (lens && lens_grad) return launch_backward_points_lens_grad(*a, ws, st, grad_depth != nullptr, *lens, *lens_grad);
     if (lens) return launch_backward_points_lens(*a, ws, st, grad_depth != nullptr, *lens);
     if (intr) return launch_backward_points_calib(*a, ws, st, grad_depth != nullptr, pose, *intr);
@@ -558,8 +560,8 @@ int gsb200_backward_ext(const GsbBackwardArgs *a, const float *grad_rasterized_d
     return gsb200_backward_pose(a, grad_rasterized_depth, rasterized_depth, grad_pixel_accumulated_alpha, ext, nullptr);
 }
 
-// gsb200_backward_calib's checks and dispatch; `lens` (gsb200_backward_lens, checked there) comes with neither pose nor
-// intrinsics, `lens_grad` (gsb200_backward_lens_grad, checked there) only with `lens`, and `rs` / `rs_grad`
+// gsb200_backward_calib's checks and dispatch; `lens` (gsb200_backward_lens, checked there) comes with pose or intrinsics
+// only from gsb200_backward_lens_calib, `lens_grad` (gsb200_backward_lens_grad, checked there) only with `lens`, and `rs` / `rs_grad`
 // (gsb200_backward_rolling_shutter, checked there) with neither pose, intrinsics nor lens_grad
 static int backward_checked(const GsbBackwardArgs *a, const float *grad_rasterized_depth, const float *rasterized_depth,
                             const float *grad_pixel_accumulated_alpha, const GsbExtraFeatureArgs *ext, const GsbPoseGradArgs *pose,
@@ -743,37 +745,73 @@ int64_t gsb200_lens_grad_temp_bytes(void) {
     return (int64_t)GSB_LENS_GRAD_PARTIAL_BLOCKS * 5 * (int64_t)sizeof(float);
 }
 
+// The checks of gsb200_backward_lens_grad (a non-NULL lens_grad): the lens, an opencv or fisheye model, the output and temp
+// pointers, and no compact rows.  *lens is the checked lens.
+static int check_lens_grad(const char *what, const GsbBackwardArgs *a, const GsbLensArgs *lens_args,
+                           const GsbLensGradArgs *lens_grad, LensParams *lens_params, const LensParams **lens) {
+    int rc = check_lens(what, lens_args, lens_params, lens);
+    if (rc != GSB_OK) return rc;
+    if (!*lens) {
+        set_error("%s: the coefficient gradient needs an opencv or fisheye lens (got %s)", what,
+                  lens_args ? "GSB_LENS_PINHOLE" : "NULL");
+        return GSB_EINVAL;
+    }
+    if (!lens_grad->grad_coefficients || !lens_grad->temp) {
+        set_error("%s: null grad_coefficients / temp pointer", what);
+        return GSB_EINVAL;
+    }
+    if (reinterpret_cast<uintptr_t>(lens_grad->grad_coefficients) % 4 != 0) {
+        set_error("%s: grad_coefficients must be 4-byte aligned", what);
+        return GSB_EINVAL;
+    }
+    if (reinterpret_cast<uintptr_t>(lens_grad->temp) % 16 != 0) {
+        set_error("%s: the lens temp must be 16-byte aligned", what);
+        return GSB_EINVAL;
+    }
+    if (a != nullptr && (a->flags & GSB_FLAG_COMPACT_GRADS)) {
+        set_error("%s: the lens gradient is not implemented for the compact rows of the view-parallel exchange "
+                  "(GSB_FLAG_COMPACT_GRADS)", what);
+        return GSB_EUNSUPPORTED;
+    }
+    return GSB_OK;
+}
+
 int gsb200_backward_lens_grad(const GsbBackwardArgs *a, const float *grad_rasterized_depth, const float *rasterized_depth,
                               const float *grad_pixel_accumulated_alpha, const GsbExtraFeatureArgs *ext,
                               const GsbLensArgs *lens_args, const GsbLensGradArgs *lens_grad) {
     if (!lens_grad) return gsb200_backward_lens(a, grad_rasterized_depth, rasterized_depth, grad_pixel_accumulated_alpha, ext, lens_args);
     LensParams lens_params;
     const LensParams *lens;
-    int rc = check_lens("backward_lens_grad", lens_args, &lens_params, &lens);
+    int rc = check_lens_grad("backward_lens_grad", a, lens_args, lens_grad, &lens_params, &lens);
+    if (rc != GSB_OK) return rc;
+    return backward_checked(a, grad_rasterized_depth, rasterized_depth, grad_pixel_accumulated_alpha, ext, nullptr, nullptr, lens,
+                            lens_grad);
+}
+
+int gsb200_backward_lens_calib(const GsbBackwardArgs *a, const float *grad_rasterized_depth, const float *rasterized_depth,
+                               const float *grad_pixel_accumulated_alpha, const GsbExtraFeatureArgs *ext,
+                               const GsbLensArgs *lens_args, const GsbLensGradArgs *lens_grad, const GsbPoseGradArgs *pose,
+                               const GsbIntrinsicsGradArgs *intr) {
+    if (!pose && !intr)
+        return gsb200_backward_lens_grad(a, grad_rasterized_depth, rasterized_depth, grad_pixel_accumulated_alpha, ext, lens_args,
+                                         lens_grad);
+    LensParams lens_params;
+    const LensParams *lens;
+    int rc = lens_grad ? check_lens_grad("backward_lens_calib", a, lens_args, lens_grad, &lens_params, &lens)
+                       : check_lens("backward_lens_calib", lens_args, &lens_params, &lens);
     if (rc != GSB_OK) return rc;
     if (!lens) {
-        set_error("backward_lens_grad: the coefficient gradient needs an opencv or fisheye lens (got %s)",
-                  lens_args ? "GSB_LENS_PINHOLE" : "NULL");
-        return GSB_EINVAL;
-    }
-    if (!lens_grad->grad_coefficients || !lens_grad->temp) {
-        set_error("backward_lens_grad: null grad_coefficients / temp pointer");
-        return GSB_EINVAL;
-    }
-    if (reinterpret_cast<uintptr_t>(lens_grad->grad_coefficients) % 4 != 0) {
-        set_error("backward_lens_grad: grad_coefficients must be 4-byte aligned");
-        return GSB_EINVAL;
-    }
-    if (reinterpret_cast<uintptr_t>(lens_grad->temp) % 16 != 0) {
-        set_error("backward_lens_grad: the lens temp must be 16-byte aligned");
+        set_error("backward_lens_calib: the pose and intrinsics gradients through a lens need an opencv or fisheye lens (got "
+                  "%s); a pinhole camera takes gsb200_backward_calib", lens_args ? "GSB_LENS_PINHOLE" : "NULL");
         return GSB_EINVAL;
     }
     if (a != nullptr && (a->flags & GSB_FLAG_COMPACT_GRADS)) {
-        set_error("backward_lens_grad: the lens gradient is not implemented for the compact rows of the view-parallel exchange "
-                  "(GSB_FLAG_COMPACT_GRADS)");
+        set_error("backward_lens_calib: the lens gradient is not implemented for the compact rows of the view-parallel "
+                  "exchange (GSB_FLAG_COMPACT_GRADS)");
         return GSB_EUNSUPPORTED;
     }
-    return backward_checked(a, grad_rasterized_depth, rasterized_depth, grad_pixel_accumulated_alpha, ext, nullptr, nullptr, lens,
+    // the pose and intrinsics checks of gsb200_backward_calib come next, still before any CUDA call
+    return backward_checked(a, grad_rasterized_depth, rasterized_depth, grad_pixel_accumulated_alpha, ext, pose, intr, lens,
                             lens_grad);
 }
 

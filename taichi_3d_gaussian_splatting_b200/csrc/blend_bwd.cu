@@ -417,7 +417,9 @@ __device__ __forceinline__ void weighted_u_sigma(const float *U, const float *R,
 }
 // LENS = true (gsb200_backward_lens): the frame was projected through lens_distort (common.cuh), so d uv / d pc = K[:2,:2] D P
 // replaces the pinhole projection Jacobian and J = diag(fx, fy) D P replaces the pinhole J inside Sigma' (D at the point's
-// (xn, yn), detached like J).  Non-compact, without POSE / INTR.
+// (xn, yn), detached like J).  Non-compact.  With POSE (gsb200_backward_lens_calib), J is a full 2x3 matrix:
+// dL/dW[r] = gp_r xyz + 2 sum_a J[a][r] B_a.  With INTR: dL/dK[r][c] = guv_r (xd, yd, 1)_c, and fx, fy enter J through
+// diag(fx, fy): dL/dK[0][0] += 2 B0 . (D P W)[0], dL/dK[1][1] += 2 B1 . (D P W)[1].
 // LGRAD = true (gsb200_backward_lens_grad, with LENS): each in-camera point also forms its 5 coefficient values
 // (lens_coefficient_grad, common.cuh), which the warp sums (fixed butterfly order, all objects together: a frame has one lens)
 // into the per-warp row s_lgrad[warp][5]; after the loop the CTA adds its warps' rows in warp order into
@@ -470,7 +472,7 @@ __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, fl
                                                      float *mgrad_partials = nullptr, const float *filter3d = nullptr,
                                                      const BlurParams blur = BlurParams(),
                                                      const DefocusParams defocus = DefocusParams()) {
-    static_assert(!LENS || (!COMPACT && !POSE && !INTR), "the lens gradient is implemented for the dense rows alone");
+    static_assert(!LENS || !COMPACT, "the lens gradient is implemented for the dense rows alone");
     static_assert(!LGRAD || LENS, "the coefficient gradient needs the lens path");
     static_assert(!RS || (!COMPACT && !POSE && !INTR && !LGRAD), "the rolling shutter is implemented for the dense rows alone");
     static_assert(!MGRAD || RS, "the motion gradient needs the rolling-shutter path");
@@ -578,8 +580,8 @@ __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, fl
                        Kc[3] * iz, Kc[4] * iz, (-Kc[3] * pcx - Kc[4] * pcy) * iz2};
         float Jl[6];  // LENS: diag(fx, fy) D P, the J of Sigma' below
         float Mk[4] = {Kc[0], Kc[1], Kc[3], Kc[4]};  // DEFOCUS: M = K[:2,:2] (K[:2,:2] D with LENS)
+        float ox, oy, D[4];  // LENS: (xd, yd) - (xn, yn) and D = d(xd, yd)/d(xn, yn) at the point
         if (LENS) {
-            float ox, oy, D[4];  // D = d(xd, yd)/d(xn, yn) at the point
             if (lens.model == GSB_LENS_FISHEYE) lens_distort<GSB_LENS_FISHEYE>(lens.k, pcx * iz, pcy * iz, ox, oy, D);
             else lens_distort<GSB_LENS_OPENCV>(lens.k, pcx * iz, pcy * iz, ox, oy, D);
             // K[:2,:2] D P: the pinhole expression with K[:2,:2] replaced by K[:2,:2] D (exactly K[:2,:2] for D = I)
@@ -761,6 +763,10 @@ __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, fl
                     pv[c] = gp[0] * xw[c] + 2.0f * (J[0] * B0[c] + J[3] * B1[c]);
                     pv[3 + c] = gp[1] * xw[c] + 2.0f * (J[1] * B0[c] + J[4] * B1[c]);
                     pv[6 + c] = gp[2] * xw[c];
+                } else if (LENS) {  // J = diag(fx, fy) D P: all six entries
+                    pv[c] = gp[0] * xw[c] + 2.0f * (J[0] * B0[c] + J[3] * B1[c]);
+                    pv[3 + c] = gp[1] * xw[c] + 2.0f * (J[1] * B0[c] + J[4] * B1[c]);
+                    pv[6 + c] = gp[2] * xw[c] + 2.0f * (J[2] * B0[c] + J[5] * B1[c]);
                 } else {
                     pv[c] = gp[0] * xw[c] + 2.0f * (J[0] * B0[c]);
                     pv[3 + c] = gp[1] * xw[c] + 2.0f * (J[4] * B1[c]);
@@ -791,6 +797,24 @@ __device__ __forceinline__ void backward_points_body(const PointsBwdParams p, fl
                 iv[2] = a0.x;
                 iv[3] = a0.y * pcx + 2.0f * s10;
                 iv[4] = a0.y * pcy + 2.0f * s11;
+                iv[5] = a0.y;
+            } else if (LENS) {
+                // uv = K[:2] (xd, yd, 1): dL/dK[r][c] += guv_r (xd, yd, 1)_c.  Sigma' through J = diag(fx, fy) D P:
+                // dL/dfx += 2 sum_c B0[c] (D P W)[0][c], dL/dfy likewise with B1 and row 1 (D = I: the pinhole's)
+                const float xd = pcx * iz + ox, yd = pcy * iz + oy;
+                const float P0[3] = {D[0] * iz, D[1] * iz, -(D[0] * pcx + D[1] * pcy) * iz2};  // rows of D P
+                const float P1[3] = {D[2] * iz, D[3] * iz, -(D[2] * pcx + D[3] * pcy) * iz2};
+                float sx0 = 0.0f, sy1 = 0.0f;
+#pragma unroll
+                for (int c = 0; c < 3; ++c) {
+                    sx0 += B0[c] * ((P0[0] * Wm[c] + P0[1] * Wm[3 + c]) + P0[2] * Wm[6 + c]);
+                    sy1 += B1[c] * ((P1[0] * Wm[c] + P1[1] * Wm[3 + c]) + P1[2] * Wm[6 + c]);
+                }
+                iv[0] = a0.x * xd + 2.0f * sx0;
+                iv[1] = a0.x * yd;
+                iv[2] = a0.x;
+                iv[3] = a0.y * xd;
+                iv[4] = a0.y * yd + 2.0f * sy1;
                 iv[5] = a0.y;
             } else {
             const float ux = pcx * iz, uy = pcy * iz;
@@ -1244,6 +1268,26 @@ backward_points_ortho_kernel(const PointsBwdOrthoParams p) {
     backward_points_body<false, DEPTH, POSE, INTR, false, false, false, false, FILTER, false, false, false, false, false, true>(
         p, POSE ? s_pose : nullptr, p.pose_partials, p.num_objects, INTR ? s_intr : nullptr, p.intr_partials, LensParams(),
         nullptr, nullptr, RsParams(), nullptr, nullptr, p.filter3d);
+}
+
+// The parameter block of the LENS instantiations with camera gradients (pose_partials / num_objects read only with POSE,
+// intr_partials only with INTR, lens_partials only with LGRAD).
+struct PointsBwdLensCalibParams : PointsBwdCalibParams {
+    LensParams lens;
+    float *lens_partials;  // (grid, 5)
+};
+
+// Pose, intrinsics and coefficient sums through a lens in one pass over the scene rows (POSE or INTR; LGRAD optional).
+template <bool DEPTH, bool POSE, bool INTR, bool LGRAD>
+__global__ void __launch_bounds__(GSB_POINTS_THREADS, POSE && INTR ? 3 : 4)  // at one CTA per SM more, each of them spills
+backward_points_lens_calib_kernel(const PointsBwdLensCalibParams p) {
+    static_assert(POSE || INTR, "without camera gradients the lens path is backward_points_lens(_grad)_kernel");
+    __shared__ float s_pose[POSE ? (GSB_POINTS_THREADS / 32) * GSB_POSE_MAX_OBJECTS * POSE_VALUES : 1];
+    __shared__ float s_intr[INTR ? (GSB_POINTS_THREADS / 32) * INTR_VALUES : 1];
+    __shared__ float s_lgrad[LGRAD ? (GSB_POINTS_THREADS / 32) * LENS_GRAD_VALUES : 1];
+    backward_points_body<false, DEPTH, POSE, INTR, true, LGRAD>(
+        p, POSE ? s_pose : nullptr, p.pose_partials, p.num_objects, INTR ? s_intr : nullptr, p.intr_partials, p.lens,
+        LGRAD ? s_lgrad : nullptr, p.lens_partials);
 }
 
 // One CTA: adds the `blocks` partial rows in a fixed order (strided per thread, then a fixed shared-memory tree) and
@@ -1701,6 +1745,60 @@ int launch_backward_points_ortho(const GsbBackwardArgs &a, const Workspace &ws, 
     if (intr) {
         intrinsics_finish_kernel<<<1, INTR_FINISH_THREADS, 0, stream>>>(p.intr_partials, (int)blocks,
                                                                          intr->grad_camera_intrinsics);
+        GSB_CUDA_CHECK(cudaGetLastError());
+    }
+    return GSB_OK;
+}
+
+template <bool DEPTH>
+static void launch_lens_calib_kernel(bool pose, bool intr, bool lgrad, int blocks, cudaStream_t stream,
+                                     const PointsBwdLensCalibParams &p) {
+    if (pose && intr && lgrad) backward_points_lens_calib_kernel<DEPTH, true, true, true><<<blocks, GSB_POINTS_THREADS, 0, stream>>>(p);
+    else if (pose && intr) backward_points_lens_calib_kernel<DEPTH, true, true, false><<<blocks, GSB_POINTS_THREADS, 0, stream>>>(p);
+    else if (pose && lgrad) backward_points_lens_calib_kernel<DEPTH, true, false, true><<<blocks, GSB_POINTS_THREADS, 0, stream>>>(p);
+    else if (pose) backward_points_lens_calib_kernel<DEPTH, true, false, false><<<blocks, GSB_POINTS_THREADS, 0, stream>>>(p);
+    else if (lgrad) backward_points_lens_calib_kernel<DEPTH, false, true, true><<<blocks, GSB_POINTS_THREADS, 0, stream>>>(p);
+    else backward_points_lens_calib_kernel<DEPTH, false, true, false><<<blocks, GSB_POINTS_THREADS, 0, stream>>>(p);
+}
+
+// The LENS per-point kernel with pose and / or intrinsics sums (and the coefficient sums with lens_grad) on the POSE kernel's
+// grid (it depends on N alone), then the finishing kernels of launch_backward_points_calib and
+// launch_backward_points_lens_grad.  Every per-row output is written by the row's own thread, as in the LENS kernel.  The
+// caller checked the arguments (pose or intr is set).
+int launch_backward_points_lens_calib(const GsbBackwardArgs &a, const Workspace &ws, cudaStream_t stream, bool depth_grad,
+                                      const LensParams &lens, const GsbLensGradArgs *lens_grad, const GsbPoseGradArgs *pose,
+                                      const GsbIntrinsicsGradArgs *intr) {
+    static_assert(GSB_INTRINSICS_PARTIAL_BLOCKS == GSB_POSE_PARTIAL_BLOCKS &&
+                  GSB_LENS_GRAD_PARTIAL_BLOCKS == GSB_POSE_PARTIAL_BLOCKS, "the combined kernel has one grid");
+    PointsBwdLensCalibParams p;
+    static_cast<PointsBwdParams &>(p) = make_points_params(a, ws, nullptr);
+    p.pose_partials = pose ? static_cast<float *>(pose->temp) : nullptr;
+    p.num_objects = pose ? a.num_objects : 0;
+    p.intr_partials = intr ? static_cast<float *>(intr->temp) : nullptr;
+    p.lens = lens;
+    p.lens_partials = lens_grad ? static_cast<float *>(lens_grad->temp) : nullptr;
+    long long blocks = a.num_points > 0 ? (a.num_points + GSB_POINTS_THREADS - 1) / GSB_POINTS_THREADS : 0;
+    if (blocks > GSB_POSE_PARTIAL_BLOCKS) blocks = GSB_POSE_PARTIAL_BLOCKS;
+    if (blocks > 0) {
+        const bool ps = pose != nullptr, in = intr != nullptr, lg = lens_grad != nullptr;
+        if (depth_grad) launch_lens_calib_kernel<true>(ps, in, lg, (int)blocks, stream, p);
+        else launch_lens_calib_kernel<false>(ps, in, lg, (int)blocks, stream, p);
+        GSB_CUDA_CHECK(cudaGetLastError());
+    }
+    if (pose) {
+        pose_finish_kernel<<<a.num_objects, POSE_FINISH_THREADS, 0, stream>>>(
+            p.pose_partials, (int)blocks, a.num_objects, pose->q_pointcloud_camera, a.t_pointcloud_camera,
+            pose->grad_q_pointcloud_camera, pose->grad_t_pointcloud_camera);
+        GSB_CUDA_CHECK(cudaGetLastError());
+    }
+    if (intr) {
+        intrinsics_finish_kernel<<<1, INTR_FINISH_THREADS, 0, stream>>>(p.intr_partials, (int)blocks,
+                                                                         intr->grad_camera_intrinsics);
+        GSB_CUDA_CHECK(cudaGetLastError());
+    }
+    if (lens_grad) {
+        lens_grad_finish_kernel<<<1, LENS_GRAD_FINISH_THREADS, 0, stream>>>(p.lens_partials, (int)blocks,
+                                                                             lens_grad->grad_coefficients);
         GSB_CUDA_CHECK(cudaGetLastError());
     }
     return GSB_OK;

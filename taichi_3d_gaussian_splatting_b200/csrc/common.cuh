@@ -110,6 +110,11 @@ int launch_backward_points_lens(const GsbBackwardArgs &a, const Workspace &ws, c
 // lens_grad.temp), and the finishing kernel; arguments checked by the caller
 int launch_backward_points_lens_grad(const GsbBackwardArgs &a, const Workspace &ws, cudaStream_t stream, bool depth_grad,
                                      const LensParams &lens, const GsbLensGradArgs &lens_grad);
+// gsb200_backward_lens_calib with pose and / or intrinsics: the LENS per-point kernel that also sums the pose, intrinsics and
+// (with lens_grad) coefficient gradients in one pass, and their finishing kernels; arguments checked by the caller
+int launch_backward_points_lens_calib(const GsbBackwardArgs &a, const Workspace &ws, cudaStream_t stream, bool depth_grad,
+                                      const LensParams &lens, const GsbLensGradArgs *lens_grad, const GsbPoseGradArgs *pose,
+                                      const GsbIntrinsicsGradArgs *intr);
 // gsb200_backward_rolling_shutter: the RS per-point kernel (lens: NULL for a pinhole), with rs_grad also the motion sums
 // (per-CTA rows in rs_grad->temp) and the finishing kernel; arguments checked by the caller
 int launch_backward_points_rs(const GsbBackwardArgs &a, const Workspace &ws, cudaStream_t stream, bool depth_grad,

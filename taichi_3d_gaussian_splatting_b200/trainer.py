@@ -20,10 +20,14 @@ first become trainable, differentiated by the operator's ``differentiable_pose``
 Optional intrinsics refinement (an extension; ``TrainConfig.intrinsics_learning_rate``): per camera, a correction of the focal
 lengths and the principal point, differentiated by the operator's ``differentiable_intrinsics`` and stepped by its own Adam.
 Views with lens distortion (an extension; ``CameraInfo.distortion``) train through their lens in the autograd loop; the
-downsampled camera keeps the coefficients (they act on the normalised image plane).  Not with ``fused_step``, pose or
-intrinsics refinement.
+downsampled camera keeps the coefficients (they act on the normalised image plane).  Not with ``fused_step``, and not with
+pose or intrinsics refinement unless ``TrainConfig.camera_refinement_through_lens`` is set.
 Optional lens refinement (an extension; ``TrainConfig.distortion_learning_rate``): per camera with a lens, its coefficients,
 differentiated by the operator's ``differentiable_distortion`` and stepped by their own Adam.
+Optional camera refinement through the lens (an extension; ``TrainConfig.camera_refinement_through_lens``): pose and
+intrinsics refinement on distorted views, alone or together with lens refinement -- photometric self-calibration: per-view
+poses (view 0 the gauge), per-camera_id K and lens, all from one backward pass of the operator's
+``camera_gradients_through_lens`` (``refined_poses``, ``refined_intrinsics``, ``refined_distortion``).
 Views with a rolling shutter (an extension; ``CameraInfo.rolling_shutter``) train through it in the autograd loop; the
 downsampled camera keeps the motion (row time is normalised by the image height).  Not with ``fused_step``, pose, intrinsics
 or lens refinement.  Optional motion refinement (``TrainConfig.rolling_shutter_learning_rate``): per rolling-shutter view, its
@@ -223,8 +227,12 @@ class GaussianPointCloudTrainer:
         # optional lens refinement: > 0 gives every camera_id whose training views have a lens (CameraInfo.distortion) one
         # leaf tensor of its coefficients (5 for opencv, 4 for fisheye), initialised from the views' lens, kept on the host
         # and trained by its own Adam at this rate.  The views of one camera_id must share their lens.  Not with fused_step,
-        # pose or intrinsics refinement (no distorted view combines with them).
+        # and not with pose or intrinsics refinement unless camera_refinement_through_lens is set.
         distortion_learning_rate: float = 0.
+        # opt-in: pose and intrinsics refinement also on distorted training views, differentiated through the lens (the
+        # operator's camera_gradients_through_lens), alone or with distortion_learning_rate -- joint self-calibration of
+        # per-view poses and per-camera_id K and lens.  False keeps refusing the two on distorted views.
+        camera_refinement_through_lens: bool = False
         # optional motion refinement: > 0 gives every training view with a rolling shutter (CameraInfo.rolling_shutter) one
         # (6,) leaf tensor of its motion (v, w), initialised from the view's, kept on the host and trained by its own Adam at
         # this rate.  Not with fused_step, pose, intrinsics or lens refinement (no rolling-shutter view combines with them).
@@ -317,13 +325,19 @@ class GaussianPointCloudTrainer:
         self._intr = config.intrinsics_learning_rate > 0
         if self._intr and fused_step:
             raise ValueError("fused_step does not implement intrinsics refinement (intrinsics_learning_rate > 0)")
-        # a view with lens distortion (CameraInfo.distortion) trains through the autograd loop alone; an orthographic view
-        # refines its pose and intrinsics like a pinhole
+        # a view with lens distortion (CameraInfo.distortion) trains through the autograd loop alone; pose and intrinsics
+        # refinement differentiate through its lens with camera_refinement_through_lens; an orthographic view refines its
+        # pose and intrinsics like a pinhole
+        through = bool(config.camera_refinement_through_lens)
+        self._through_lens = False
         if any(getattr(v[3], "distortion", None) is not None and not _is_ortho(v[3]) for v in train_views):
-            for name, on in (("fused_step", fused_step), ("pose refinement (pose_learning_rate > 0)", self._pose),
-                             ("intrinsics refinement (intrinsics_learning_rate > 0)", self._intr)):
+            for name, on in (("fused_step", fused_step),
+                             ("pose refinement (pose_learning_rate > 0)", self._pose and not through),
+                             ("intrinsics refinement (intrinsics_learning_rate > 0)", self._intr and not through)):
                 if on:
-                    raise ValueError(f"{name} is not supported with a distorted view (CameraInfo.distortion)")
+                    hint = "" if name == "fused_step" else "; camera_refinement_through_lens=True refines it through the lens"
+                    raise ValueError(f"{name} is not supported with a distorted view (CameraInfo.distortion){hint}")
+            self._through_lens = through and (self._pose or self._intr)
         # the trainable intrinsics corrections, one per camera_id: (log fx scale, log fy scale, cx / W, cy / H)
         self._intrinsics = {}
         if self._intr:
@@ -467,6 +481,7 @@ class GaussianPointCloudTrainer:
                      **({"differentiable_pose": True} if self._pose else {}),
                      **({"differentiable_intrinsics": True} if self._intr else {}),
                      **({"differentiable_distortion": True} if self._dist else {}),
+                     **({"camera_gradients_through_lens": True} if self._through_lens else {}),
                      **({"differentiable_rolling_shutter": True} if self._rs else {}),
                      **({"differentiable_motion_blur": True} if self._mb else {}),
                      **({"differentiable_defocus": True} if self._df else {}))
