@@ -39,6 +39,9 @@ _RECORD_FLOATS = 12
 _ACCUM_FLOATS = 12
 
 
+# The projection of a pinhole, OpenCV or fisheye view: the perspective divide, with or without a GsbLensArgs
+_PERSPECTIVE = "perspective"
+
 # The lens argument of an equirectangular view: it has no GsbLensArgs and goes through gsb200_forward_equirect /
 # gsb200_backward_equirect
 _EQUIRECT = "equirectangular"
@@ -59,8 +62,47 @@ def _is_ortho(camera_info) -> bool:
     return distortion is not None and distortion.model == "orthographic"
 
 
+# The inputs of the autograd function, in order; an absent optional input is None in its slot
+(_XYZ, _FEATURES, _INVALID_MASK, _OBJECT_ID, _Q, _T, _CAMERA_INFO, _SH_BAND, _EXTRA_FEATURES, _INTRINSICS,
+ _LENS_COEFFICIENTS, _ROLLING_SHUTTER_MOTION, _FILTER_3D, _EXPOSURE_MOTION, _DEFOCUS_PARAMETERS) = range(15)
+_NUM_INPUTS = 15
+
+# The camera-parameter gradient outputs of the backward by input slot: the C argument (output, temp), the gradient's
+# shape and the library function that sizes the temp
+_CAMERA_GRADS = {
+    _INTRINSICS: (_lib.GsbIntrinsicsGradArgs, (3, 3), "gsb200_intrinsics_grad_temp_bytes"),
+    _LENS_COEFFICIENTS: (_lib.GsbLensGradArgs, (5,), "gsb200_lens_grad_temp_bytes"),
+    _ROLLING_SHUTTER_MOTION: (_lib.GsbRollingShutterGradArgs, (6,), "gsb200_rolling_shutter_grad_temp_bytes"),
+    _EXPOSURE_MOTION: (_lib.GsbMotionBlurGradArgs, (6,), "gsb200_motion_blur_grad_temp_bytes"),
+    _DEFOCUS_PARAMETERS: (_lib.GsbDefocusGradArgs, (2,), "gsb200_defocus_grad_temp_bytes"),
+}
+
+
+@dataclass
+class _Camera:
+    """The camera of one call, resolved before any device work from ``camera_info``, the optional tensors and the
+    operator's options: the projection, the C arguments of the view's extensions (None where the view has none), and
+    the length and device of each camera-parameter tensor passed (lens coefficients, motions, (a, rho)), whose gradient
+    goes back sliced to that length on that device."""
+    projection: str  # _PERSPECTIVE (pinhole, or the OpenCV / fisheye ``lens``), _EQUIRECT or _ORTHO
+    lens: Optional[_lib.GsbLensArgs]
+    rolling_shutter: Optional[_lib.GsbRollingShutterArgs]  # its row_time is set by the forward
+    motion_blur: Optional[_lib.GsbMotionBlurArgs]
+    defocus: Optional[_lib.GsbDefocusArgs]
+    filter_3d: Optional[_lib.GsbFilter3dArgs]
+    point_filter_3d: Optional[torch.Tensor]  # the array filter_3d points at, kept alive for the backward
+    gradient_like: dict  # input slot -> (length, device)
+    row_time: Optional[torch.Tensor] = None  # tau_3 of every scene row: written by the forward, read by its backward
+
+
+
 def _ptr(t: Optional[torch.Tensor]) -> Optional[int]:
     return None if t is None else t.data_ptr()
+
+
+def _ref(s: Optional[ctypes.Structure]):
+    """A C struct argument by reference (None stays NULL)."""
+    return None if s is None else ctypes.byref(s)
 
 
 def _f32(t: Optional[torch.Tensor]) -> Optional[torch.Tensor]:
@@ -361,35 +403,20 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                 raise ValueError(f"{name} needs the auxiliary outputs: config.rgb_only=True renders none")
         self.differentiable_depth = bool(differentiable_depth)
         self.differentiable_alpha = bool(differentiable_alpha)
-        if differentiable_pose and config.rgb_only:
-            raise ValueError("differentiable_pose needs the auxiliary outputs: config.rgb_only=True renders none")
-        if differentiable_pose and gradient_exchange is not None:
-            raise ValueError("differentiable_pose is not supported with a gradient_exchange (view-parallel training)")
+        for name, on in (("differentiable_pose", differentiable_pose), ("differentiable_intrinsics", differentiable_intrinsics),
+                         ("differentiable_distortion", differentiable_distortion),
+                         ("differentiable_rolling_shutter", differentiable_rolling_shutter),
+                         ("differentiable_motion_blur", differentiable_motion_blur),
+                         ("differentiable_defocus", differentiable_defocus)):
+            if on and config.rgb_only:
+                raise ValueError(f"{name} needs the auxiliary outputs: config.rgb_only=True renders none")
+            if on and gradient_exchange is not None:
+                raise ValueError(f"{name} is not supported with a gradient_exchange (view-parallel training)")
         self.differentiable_pose = bool(differentiable_pose)
-        if differentiable_intrinsics and config.rgb_only:
-            raise ValueError("differentiable_intrinsics needs the auxiliary outputs: config.rgb_only=True renders none")
-        if differentiable_intrinsics and gradient_exchange is not None:
-            raise ValueError("differentiable_intrinsics is not supported with a gradient_exchange (view-parallel training)")
         self.differentiable_intrinsics = bool(differentiable_intrinsics)
-        if differentiable_distortion and config.rgb_only:
-            raise ValueError("differentiable_distortion needs the auxiliary outputs: config.rgb_only=True renders none")
-        if differentiable_distortion and gradient_exchange is not None:
-            raise ValueError("differentiable_distortion is not supported with a gradient_exchange (view-parallel training)")
         self.differentiable_distortion = bool(differentiable_distortion)
-        if differentiable_rolling_shutter and config.rgb_only:
-            raise ValueError("differentiable_rolling_shutter needs the auxiliary outputs: config.rgb_only=True renders none")
-        if differentiable_rolling_shutter and gradient_exchange is not None:
-            raise ValueError("differentiable_rolling_shutter is not supported with a gradient_exchange (view-parallel training)")
         self.differentiable_rolling_shutter = bool(differentiable_rolling_shutter)
-        if differentiable_motion_blur and config.rgb_only:
-            raise ValueError("differentiable_motion_blur needs the auxiliary outputs: config.rgb_only=True renders none")
-        if differentiable_motion_blur and gradient_exchange is not None:
-            raise ValueError("differentiable_motion_blur is not supported with a gradient_exchange (view-parallel training)")
         self.differentiable_motion_blur = bool(differentiable_motion_blur)
-        if differentiable_defocus and config.rgb_only:
-            raise ValueError("differentiable_defocus needs the auxiliary outputs: config.rgb_only=True renders none")
-        if differentiable_defocus and gradient_exchange is not None:
-            raise ValueError("differentiable_defocus is not supported with a gradient_exchange (view-parallel training)")
         self.differentiable_defocus = bool(differentiable_defocus)
         self.camera_gradients_through_lens = bool(camera_gradients_through_lens)
         self.config = config
@@ -415,46 +442,28 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
 
             @staticmethod
             def forward(ctx, pointcloud, pointcloud_features, point_invalid_mask, point_object_id,
-                        q_pointcloud_camera, t_pointcloud_camera, camera_info, color_max_sh_band, extra_features=None,
-                        camera_intrinsics=None, lens_coefficients=None, rolling_shutter_motion=None, point_filter_3d=None,
-                        exposure_motion=None, defocus_parameters=None):
+                        q_pointcloud_camera, t_pointcloud_camera, camera_info, color_max_sh_band, extra_features,
+                        camera_intrinsics, lens_coefficients, rolling_shutter_motion, point_filter_3d, exposure_motion,
+                        defocus_parameters):
                 # camera_intrinsics (differentiable_intrinsics): camera_info.camera_intrinsics itself, passed again only so
                 # that autograd tracks it; lens_coefficients (differentiable_distortion): the coefficients rendered;
                 # rolling_shutter_motion (differentiable_rolling_shutter): the motion rendered; point_filter_3d: the 3D
                 # smoothing filter (never differentiated); exposure_motion (differentiable_motion_blur): the exposure motion
                 # rendered; defocus_parameters (differentiable_defocus): the (a, rho) rendered
-                outs, frame, saved = outer._run_forward(
-                    pointcloud, pointcloud_features, point_invalid_mask, point_object_id,
-                    q_pointcloud_camera, t_pointcloud_camera, camera_info, extra_features, lens_coefficients,
-                    rolling_shutter_motion, point_filter_3d, exposure_motion, defocus_parameters)
-                ctx.filter_3d = point_filter_3d  # read by the backward of this frame (the forward's array)
+                camera = outer._resolve_camera(camera_info, pointcloud, extra_features, lens_coefficients,
+                                               rolling_shutter_motion, point_filter_3d, exposure_motion, defocus_parameters)
+                outs, frame, K = outer._run_forward(camera, pointcloud, pointcloud_features, point_invalid_mask,
+                                                    point_object_id, q_pointcloud_camera, t_pointcloud_camera, camera_info,
+                                                    extra_features)
                 image, depth, acc_alpha, last_effective, valid_count = outs[:5]
                 ctx.save_for_backward(pointcloud, pointcloud_features, point_object_id,
-                                      t_pointcloud_camera, saved["camera_intrinsics"], acc_alpha,
-                                      last_effective, frame.ws, *((depth,) if outer.differentiable_depth else ()),
-                                      *((q_pointcloud_camera,) if outer.differentiable_pose else ()),
-                                      *((extra_features,) if extra_features is not None else ()))
+                                      q_pointcloud_camera if outer.differentiable_pose else None, t_pointcloud_camera, K,
+                                      acc_alpha, last_effective, frame.ws, depth if outer.differentiable_depth else None,
+                                      extra_features)
                 ctx.frame = frame
-                ctx.lens = saved["lens"]
-                ctx.rolling_shutter = saved["rolling_shutter"]  # (GsbRollingShutterArgs, the row times it points at) or None
-                ctx.motion_input = rolling_shutter_motion is not None
-                if ctx.motion_input:
-                    ctx.motion_device = rolling_shutter_motion.device
-                ctx.motion_blur = saved["motion_blur"]  # GsbMotionBlurArgs or None
-                ctx.blur_input = exposure_motion is not None
-                if ctx.blur_input:
-                    ctx.blur_device = exposure_motion.device
-                ctx.defocus = saved["defocus"]  # GsbDefocusArgs or None
-                ctx.defocus_input = defocus_parameters is not None
-                if ctx.defocus_input:
-                    ctx.defocus_device = defocus_parameters.device
+                ctx.camera = camera
                 ctx.num_objects = q_pointcloud_camera.shape[0]
                 ctx.color_max_sh_band = color_max_sh_band
-                ctx.has_extra_features = extra_features is not None
-                ctx.intrinsics_input = camera_intrinsics is not None
-                ctx.lens_input = lens_coefficients is not None
-                if ctx.lens_input:
-                    ctx.lens_coefficients_like = (lens_coefficients.shape[0], lens_coefficients.device)
                 if outer.differentiable_depth:
                     ctx.mark_non_differentiable(valid_count)
                 else:
@@ -467,35 +476,17 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                 return result
 
             @staticmethod
-            def backward(ctx, *grads):
-                result = _module_function._grads(ctx, *grads)
-                if ctx.defocus_input:  # fifteen inputs: the slots before (a, rho) get no gradient here
-                    result, grad_d = result
-                    return tuple(result) + (None,) * (14 - len(result)) + (grad_d,)
-                if ctx.blur_input:  # fourteen inputs: the slots before the exposure motion get no gradient here
-                    result, grad_b = result
-                    return tuple(result) + (None,) * (13 - len(result)) + (grad_b,)
-                if ctx.filter_3d is not None:  # thirteen inputs: the filter's slot ends the list and gets no gradient
-                    result = tuple(result) + (None,) * (13 - len(result))
-                return result
-
-            @staticmethod
-            def _grads(ctx, grad_rasterized_image, grad_rasterized_depth, grad_pixel_valid_point_count, *grad_extra):
+            def backward(ctx, grad_rasterized_image, grad_rasterized_depth, grad_pixel_valid_point_count, *grad_extra):
                 # grad_extra: dL/d pixel_accumulated_alpha (differentiable_alpha), then dL/d the feature map (extra features)
                 grad_pixel_accumulated_alpha = grad_extra[0] if outer.differentiable_alpha else None
-                grad_feature_map = grad_extra[-1] if ctx.has_extra_features else None
-                grad_pointcloud = grad_pointcloud_features = grad_extra_features = grad_q = grad_t = None
-                pose = outer.differentiable_pose and (ctx.needs_input_grad[4] or ctx.needs_input_grad[5])
-                intrinsics = ctx.intrinsics_input and ctx.needs_input_grad[9]
-                lens_grad = ctx.lens_input and ctx.needs_input_grad[10]
-                motion_grad = ctx.motion_input and ctx.needs_input_grad[11]
-                blur_grad = ctx.blur_input and ctx.needs_input_grad[13]
-                defocus_grad = ctx.defocus_input and ctx.needs_input_grad[14]
-                grad_K = grad_k = grad_m = grad_b = grad_d = None
-                # GPCR:1028; with extra features (or pose / intrinsics gradients) the backward also runs for them alone
+                grad_feature_map = grad_extra[-1] if len(grad_extra) > int(outer.differentiable_alpha) else None
+                needs = ctx.needs_input_grad
+                pose = outer.differentiable_pose and (needs[_Q] or needs[_T])
+                camera_grads = [slot for slot in _CAMERA_GRADS if needs[slot]]
+                result = [None] * _NUM_INPUTS
+                # GPCR:1028; with extra features or camera-parameter gradients the backward also runs for them alone
                 # (frozen scene)
-                if ctx.needs_input_grad[0] or ctx.needs_input_grad[1] or (ctx.has_extra_features and ctx.needs_input_grad[8]) \
-                        or pose or intrinsics or lens_grad or motion_grad or blur_grad or defocus_grad:
+                if needs[_XYZ] or needs[_FEATURES] or needs[_EXTRA_FEATURES] or pose or camera_grads:
                     if outer.config.rgb_only:
                         # the reference leaves accumulated alpha / last-effective offsets uninitialised in
                         # this mode (GPCR:478-484), so its backward is undefined; refuse instead
@@ -505,51 +496,12 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                         frame = ctx.frame
                         grad_rasterized_image = torch.zeros((frame.height, frame.width, 3), dtype=torch.float32,
                                                             device=frame.ws.device)
-                    grad_pointcloud, grad_pointcloud_features, grad_extra_features, grad_q, grad_t, grad_K, grad_k, grad_m, \
-                        grad_b, grad_d = outer._run_backward(ctx, grad_rasterized_image, grad_rasterized_depth,
-                                                             grad_pixel_accumulated_alpha, grad_feature_map, pose, intrinsics,
-                                                             lens_grad, motion_grad, blur_grad, defocus_grad)
-                if ctx.defocus_input:  # (a, rho)'s gradient goes back beside the leading slots (see backward)
-                    return ((grad_pointcloud if ctx.needs_input_grad[0] else None,
-                             grad_pointcloud_features if ctx.needs_input_grad[1] else None, None, None, None, None, None, None,
-                             grad_extra_features if ctx.has_extra_features and ctx.needs_input_grad[8] else None),
-                            grad_d if defocus_grad else None)
-                if ctx.blur_input:  # the exposure motion's gradient goes back beside the leading slots (see backward)
-                    return ((grad_pointcloud if ctx.needs_input_grad[0] else None,
-                             grad_pointcloud_features if ctx.needs_input_grad[1] else None, None, None, None, None, None, None,
-                             grad_extra_features if ctx.has_extra_features and ctx.needs_input_grad[8] else None),
-                            grad_b if blur_grad else None)
-                if ctx.motion_input:  # twelve inputs: the extra features', K's and the coefficients' slots (None), then m
-                    return (grad_pointcloud if ctx.needs_input_grad[0] else None,
-                            grad_pointcloud_features if ctx.needs_input_grad[1] else None, None, None, None, None, None, None,
-                            grad_extra_features if ctx.has_extra_features and ctx.needs_input_grad[8] else None, None, None,
-                            grad_m if motion_grad else None)
-                if ctx.lens_input:  # eleven inputs: the extra features' and K's slots (K possibly None), then the coefficients
-                    return (grad_pointcloud if ctx.needs_input_grad[0] else None,
-                            grad_pointcloud_features if ctx.needs_input_grad[1] else None, None, None,
-                            grad_q if pose and ctx.needs_input_grad[4] else None,
-                            grad_t if pose and ctx.needs_input_grad[5] else None, None, None,
-                            grad_extra_features if ctx.has_extra_features and ctx.needs_input_grad[8] else None,
-                            grad_K if intrinsics else None, grad_k if lens_grad else None)
-                if ctx.intrinsics_input:  # ten inputs: the extra features' slot (possibly None), then K
-                    return (grad_pointcloud if ctx.needs_input_grad[0] else None,
-                            grad_pointcloud_features if ctx.needs_input_grad[1] else None, None, None,
-                            grad_q if pose and ctx.needs_input_grad[4] else None,
-                            grad_t if pose and ctx.needs_input_grad[5] else None, None, None,
-                            grad_extra_features if ctx.has_extra_features and ctx.needs_input_grad[8] else None,
-                            grad_K if intrinsics else None)
-                if pose:
-                    grad_q = grad_q if ctx.needs_input_grad[4] else None
-                    grad_t = grad_t if ctx.needs_input_grad[5] else None
-                    return ((grad_pointcloud if ctx.needs_input_grad[0] else None,
-                             grad_pointcloud_features if ctx.needs_input_grad[1] else None, None, None, grad_q, grad_t, None,
-                             None) + ((grad_extra_features if ctx.needs_input_grad[8] else None,) if ctx.has_extra_features
-                                      else ()))
-                if ctx.has_extra_features:  # frozen geometry: None for the scene tensors that do not need a gradient
-                    return (grad_pointcloud if ctx.needs_input_grad[0] else None,
-                            grad_pointcloud_features if ctx.needs_input_grad[1] else None, None, None, None, None, None, None,
-                            grad_extra_features if ctx.needs_input_grad[8] else None)
-                return grad_pointcloud, grad_pointcloud_features, None, None, None, None, None, None
+                    grads = outer._run_backward(ctx, grad_rasterized_image, grad_rasterized_depth,
+                                                grad_pixel_accumulated_alpha, grad_feature_map, pose, camera_grads)
+                    for slot, grad in grads.items():
+                        if needs[slot]:
+                            result[slot] = grad
+                return tuple(result)
 
         self._module_function = _module_function
 
@@ -613,15 +565,51 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
         if not point_filter_3d.is_contiguous():
             raise ValueError("point_filter_3d must be contiguous")
 
-    def _run_forward(self, pointcloud, pointcloud_features, point_invalid_mask, point_object_id,
-                     q_pointcloud_camera, t_pointcloud_camera, camera_info, extra_features=None, lens_coefficients=None,
-                     rolling_shutter_motion=None, point_filter_3d=None, exposure_motion=None, defocus_parameters=None):
+    def _resolve_camera(self, camera_info, pointcloud, extra_features=None, lens_coefficients=None,
+                        rolling_shutter_motion=None, point_filter_3d=None, exposure_motion=None,
+                        defocus_parameters=None) -> _Camera:
+        """The camera of a call (``_Camera``), after every argument check that needs no device: each refusal of what the
+        view does not combine with is raised here, before any CUDA call."""
+        if _is_equirect(camera_info):
+            self._check_equirect(camera_info, lens_coefficients, rolling_shutter_motion, point_filter_3d, exposure_motion,
+                                 defocus_parameters)
+        if _is_ortho(camera_info):
+            self._check_ortho(camera_info, lens_coefficients, rolling_shutter_motion, exposure_motion, defocus_parameters)
+        assert camera_info.camera_width % TILE_WIDTH == 0
+        assert camera_info.camera_height % TILE_HEIGHT == 0
+        # Which refusal wins where several apply: defocus, motion blur, the filter and each camera-parameter tensor are
+        # checked before the feature channels, a lens or rolling shutter that comes with camera_info alone after them.
+        defocus = self._defocus_args(camera_info, defocus_parameters, rolling_shutter_motion, point_filter_3d, exposure_motion)
+        blur = self._motion_blur_args(camera_info, exposure_motion, rolling_shutter_motion, point_filter_3d)
+        if point_filter_3d is not None:
+            for name, value in (("lens_coefficients", lens_coefficients), ("rolling_shutter_motion", rolling_shutter_motion)):
+                if value is not None:
+                    raise ValueError(f"point_filter_3d is not supported with {name} (no camera-parameter gradient with the "
+                                     "filter)")
+            self._check_filter_3d(point_filter_3d, pointcloud)
+        if rolling_shutter_motion is not None:
+            rs = self._rolling_shutter_args(camera_info, rolling_shutter_motion)
+        if lens_coefficients is not None:
+            lens = self._lens_args(camera_info, lens_coefficients)
+        if extra_features is not None:
+            self._check_extra_features(extra_features, pointcloud)
+        if lens_coefficients is None:
+            lens = self._lens_args(camera_info)
+        if rolling_shutter_motion is None:
+            rs = self._rolling_shutter_args(camera_info)
+        projection = lens if lens is _EQUIRECT or lens is _ORTHO else _PERSPECTIVE
+        gradient_like = {slot: (t.shape[0], t.device) for slot, t in (
+            (_LENS_COEFFICIENTS, lens_coefficients), (_ROLLING_SHUTTER_MOTION, rolling_shutter_motion),
+            (_EXPOSURE_MOTION, exposure_motion), (_DEFOCUS_PARAMETERS, defocus_parameters)) if t is not None}
+        return _Camera(projection=projection, lens=lens if projection is _PERSPECTIVE else None, rolling_shutter=rs,
+                       motion_blur=blur, defocus=defocus,
+                       filter_3d=None if point_filter_3d is None else _lib.GsbFilter3dArgs(filter3d=_ptr(point_filter_3d)),
+                       point_filter_3d=point_filter_3d, gradient_like=gradient_like)
+
+    def _run_forward(self, camera: _Camera, pointcloud, pointcloud_features, point_invalid_mask, point_object_id,
+                     q_pointcloud_camera, t_pointcloud_camera, camera_info, extra_features=None):
         cfg = self.config
         lib = _lib.load()
-        lens = self._lens_args(camera_info, lens_coefficients)
-        rs = self._rolling_shutter_args(camera_info, rolling_shutter_motion)
-        blur = self._motion_blur_args(camera_info, exposure_motion, rolling_shutter_motion, point_filter_3d)
-        defocus = self._defocus_args(camera_info, defocus_parameters, rolling_shutter_motion, point_filter_3d, exposure_motion)
         _require(pointcloud, "point_cloud", torch.float32, (3,))
         _require(pointcloud_features, "point_cloud_features", torch.float32, (56,))
         _require(point_invalid_mask, "point_invalid_mask", torch.int8)
@@ -662,10 +650,18 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                 C = extra_features.shape[1]
                 feature_map = torch.empty((H, W, C), dtype=torch.float32, device=device)
                 ext = _lib.GsbExtraFeatureArgs(channels=C, features=_ptr(extra_features), rasterized=_ptr(feature_map))
-            row_time = None
-            if rs is not None:  # tau_3 of every scene row, read back by the backward of this frame
-                row_time = torch.empty((max(N, 1),), dtype=torch.float32, device=device)
-                rs.row_time = _ptr(row_time)
+            if camera.rolling_shutter is not None:  # read back by the backward of this frame
+                camera.row_time = torch.empty((max(N, 1),), dtype=torch.float32, device=device)
+                camera.rolling_shutter.row_time = _ptr(camera.row_time)
+            if camera.projection is _EQUIRECT:
+                entry, camera_args = "gsb200_forward_equirect", (ext,)
+            elif camera.projection is _ORTHO:
+                entry, camera_args = "gsb200_forward_ortho", (ext, camera.filter_3d)
+            elif camera.motion_blur is not None or camera.defocus is not None:
+                entry, camera_args = "gsb200_forward_defocus", (ext, camera.lens, camera.rolling_shutter, camera.motion_blur,
+                                                                camera.defocus)
+            else:
+                entry, camera_args = "gsb200_forward_filter3d", (ext, camera.lens, camera.rolling_shutter, camera.filter_3d)
             readback = _PinnedCounters.acquire(device)
             pinned, event = readback
             retry_flag = 0
@@ -689,41 +685,7 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                         host_counters=pinned.data_ptr(), host_counters_event=event.cuda_event)
                     # The whole frame is enqueued by this one call; the library copies {M, K, overflow} to pinned
                     # host memory right after the per-point stage and records `event` behind that copy.
-                    if lens is _EQUIRECT:
-                        _lib.check(lib.gsb200_forward_equirect(ctypes.byref(args), ctypes.byref(ext) if ext is not None else None),
-                                   "gsb200_forward_equirect")
-                    elif lens is _ORTHO:
-                        _lib.check(lib.gsb200_forward_ortho(
-                            ctypes.byref(args), ctypes.byref(ext) if ext is not None else None,
-                            ctypes.byref(_lib.GsbFilter3dArgs(filter3d=_ptr(point_filter_3d)))
-                            if point_filter_3d is not None else None), "gsb200_forward_ortho")
-                    elif defocus is not None:
-                        _lib.check(lib.gsb200_forward_defocus(
-                            ctypes.byref(args), ctypes.byref(ext) if ext is not None else None,
-                            ctypes.byref(lens) if lens is not None else None, ctypes.byref(rs) if rs is not None else None,
-                            ctypes.byref(blur) if blur is not None else None, ctypes.byref(defocus)), "gsb200_forward_defocus")
-                    elif blur is not None:
-                        _lib.check(lib.gsb200_forward_motion_blur(
-                            ctypes.byref(args), ctypes.byref(ext) if ext is not None else None,
-                            ctypes.byref(lens) if lens is not None else None, ctypes.byref(rs) if rs is not None else None,
-                            ctypes.byref(blur)), "gsb200_forward_motion_blur")
-                    elif point_filter_3d is not None:
-                        _lib.check(lib.gsb200_forward_filter3d(
-                            ctypes.byref(args), ctypes.byref(ext) if ext is not None else None,
-                            ctypes.byref(lens) if lens is not None else None, ctypes.byref(rs) if rs is not None else None,
-                            ctypes.byref(_lib.GsbFilter3dArgs(filter3d=_ptr(point_filter_3d)))), "gsb200_forward_filter3d")
-                    elif rs is not None:
-                        _lib.check(lib.gsb200_forward_rolling_shutter(
-                            ctypes.byref(args), ctypes.byref(ext) if ext is not None else None,
-                            ctypes.byref(lens) if lens is not None else None, ctypes.byref(rs)),
-                            "gsb200_forward_rolling_shutter")
-                    elif lens is not None:
-                        _lib.check(lib.gsb200_forward_lens(ctypes.byref(args), ctypes.byref(ext) if ext is not None else None,
-                                                           ctypes.byref(lens)), "gsb200_forward_lens")
-                    elif ext is None:
-                        _lib.check(lib.gsb200_forward(ctypes.byref(args)), "gsb200_forward")
-                    else:  # the re-run after an overflow renders the feature map as well
-                        _lib.check(lib.gsb200_forward_ext(ctypes.byref(args), ctypes.byref(ext)), "gsb200_forward_ext")
+                    _lib.check(getattr(lib, entry)(ctypes.byref(args), *map(_ref, camera_args)), entry)
                     frame = Frame(ws, layout, N, key_capacity, H, W, self._flags)
                     # ONE host wait per frame (the reference syncs twice, GPCR:864 and GPCR:916-931), and it ends
                     # when the first kernel is done: sort + blend are still in flight when we return.
@@ -740,9 +702,7 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                 _PinnedCounters.release(device, readback)
         self.last_frame = frame
         outs = (image, depth, acc_alpha, last_effective, valid_count) + ((feature_map,) if feature_map is not None else ())
-        return outs, frame, {"camera_intrinsics": K, "lens": lens,
-                             "rolling_shutter": (rs, row_time) if rs is not None else None, "motion_blur": blur,
-                             "defocus": defocus}
+        return outs, frame, K
 
     def _lens_args(self, camera_info, lens_coefficients=None) -> Optional[_lib.GsbLensArgs]:
         """The C lens argument of ``camera_info.distortion`` (None: the pinhole kernels), after the checks of the options
@@ -930,45 +890,20 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
         return _lib.GsbDefocusArgs(aperture=values[0], inverse_focus=values[1])
 
     # ------------------------------------------------------------------ backward plumbing
-    @staticmethod
-    def _camera_grad_args(lib, ctx, q_pointcloud_camera, pose, intrinsics, device):
-        """(GsbPoseGradArgs, grad_q, grad_t, the tensors it points at) with ``pose`` and (GsbIntrinsicsGradArgs, grad_K,
-        its temp) with ``intrinsics`` (else None): the C call's arguments, kept alive by the caller."""
-        pose_args = intr_args = None
-        if pose:
-            n_obj = ctx.num_objects
-            q_pc = q_pointcloud_camera.detach().contiguous()
-            grad_q = torch.empty((n_obj, 4), dtype=torch.float32, device=device)
-            grad_t = torch.empty((n_obj, 3), dtype=torch.float32, device=device)
-            temp = torch.empty((max(int(lib.gsb200_pose_grad_temp_bytes(n_obj)), 16) // 4,), dtype=torch.float32,
-                               device=device)
-            pose_args = (_lib.GsbPoseGradArgs(q_pointcloud_camera=_ptr(q_pc), grad_q_pointcloud_camera=_ptr(grad_q),
-                                              grad_t_pointcloud_camera=_ptr(grad_t), temp=_ptr(temp)), grad_q, grad_t, temp,
-                         q_pc)
-        if intrinsics:
-            grad_K = torch.empty((3, 3), dtype=torch.float32, device=device)
-            temp = torch.empty((int(lib.gsb200_intrinsics_grad_temp_bytes()) // 4,), dtype=torch.float32, device=device)
-            intr_args = (_lib.GsbIntrinsicsGradArgs(grad_camera_intrinsics=_ptr(grad_K), temp=_ptr(temp)), grad_K, temp)
-        return pose_args, intr_args
-
     def _run_backward(self, ctx, grad_rasterized_image, grad_rasterized_depth=None, grad_pixel_accumulated_alpha=None,
-                      grad_feature_map=None, pose=False, intrinsics=False, lens_grad=False, motion_grad=False,
-                      blur_grad=False, defocus_grad=False):
-        """Returns dL/dxyz, dL/dfeatures, for a call with extra features dL/d of them ((N, C); zeros when the feature map
-        was not used), with ``pose`` dL/dq_pointcloud_camera (K, 4) and dL/dt_pointcloud_camera (K, 3) (else None), with
-        ``intrinsics`` dL/dcamera_intrinsics (3, 3) (else None), with ``lens_grad`` dL/dlens_coefficients on the
-        coefficient tensor's device (else None), with ``motion_grad`` dL/drolling_shutter_motion on the motion tensor's
-        device (else None), with ``blur_grad`` dL/dexposure_motion on that tensor's device (else None), and with
-        ``defocus_grad`` dL/ddefocus_parameters on that tensor's device (else None)."""
+                      grad_feature_map=None, pose=False, camera_grads=()):
+        """The gradients by input slot: dL/dxyz, dL/dfeatures, for a call with extra features dL/d of them ((N, C); zeros
+        when the feature map was not used), with ``pose`` dL/dq_pointcloud_camera (K, 4) and dL/dt_pointcloud_camera
+        (K, 3), and for each slot of ``camera_grads`` (``_CAMERA_GRADS``) that tensor's gradient: K's (3, 3), the others
+        sliced to the tensor's length on its device."""
         cfg = self.config
         lib = _lib.load()
-        saved = ctx.saved_tensors
-        (pointcloud, pointcloud_features, point_object_id, t_pointcloud_camera, K, acc_alpha,
-         last_effective, ws) = saved[:8]
+        (pointcloud, pointcloud_features, point_object_id, q_pointcloud_camera, t_pointcloud_camera, K, acc_alpha,
+         last_effective, ws, depth, extra_features) = ctx.saved_tensors
         # differentiable_depth: the depth gradient (None when the loss does not use depth) and the forward's depth map
-        depth = saved[8] if self.differentiable_depth and grad_rasterized_depth is not None else None
-        q_pointcloud_camera = saved[8 + int(self.differentiable_depth)] if self.differentiable_pose else None
-        extra_features = saved[-1] if ctx.has_extra_features else None
+        if grad_rasterized_depth is None:
+            depth = None
+        camera: _Camera = ctx.camera
         frame: Frame = ctx.frame
         device = pointcloud.device
         N = pointcloud.shape[0]
@@ -1020,211 +955,60 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
             grad_depth = _f32(grad_rasterized_depth) if depth is not None else None
             # differentiable_alpha: None when the loss does not use the accumulated alpha
             grad_alpha = _f32(grad_pixel_accumulated_alpha) if self.differentiable_alpha else None
-            grad_extra_features = None
+            grads = {_XYZ: grad_pointcloud, _FEATURES: grad_pointcloud_features}
+            ext = None
             if extra_features is not None:  # dL/df: written by the call, or zero when the feature map was not used
                 C = extra_features.shape[1]
-                grad_extra_features = torch.zeros((N, C), dtype=torch.float32, device=device) if grad_feature_map is None \
-                    else torch.empty((N, C), dtype=torch.float32, device=device)
-            grad_q = grad_t = grad_K = grad_k = grad_m = grad_b = grad_d = None
-            if ctx.lens is _EQUIRECT:  # no camera-parameter gradient or other extension (refused in forward)
-                ext = None
-                if extra_features is not None and grad_feature_map is not None:
-                    grad_map = _f32(grad_feature_map)
-                    ext = _lib.GsbExtraFeatureArgs(channels=extra_features.shape[1], features=_ptr(extra_features),
-                                                   grad_rasterized=_ptr(grad_map), grad_features=_ptr(grad_extra_features))
-                _lib.check(lib.gsb200_backward_equirect(ctypes.byref(args), _ptr(grad_depth), _ptr(depth), _ptr(grad_alpha),
-                                                        ctypes.byref(ext) if ext is not None else None),
-                           "gsb200_backward_equirect")
-            elif ctx.lens is _ORTHO:  # the 3D filter, pose and intrinsics gradients (the filter never with the latter two)
-                pose_args = intr_args = None
-                if pose:
-                    n_obj = ctx.num_objects
-                    q_pc = q_pointcloud_camera.detach().contiguous()
-                    grad_q = torch.empty((n_obj, 4), dtype=torch.float32, device=device)
-                    grad_t = torch.empty((n_obj, 3), dtype=torch.float32, device=device)
-                    pose_temp = torch.empty((max(int(lib.gsb200_pose_grad_temp_bytes(n_obj)), 16) // 4,),
-                                            dtype=torch.float32, device=device)
-                    pose_args = _lib.GsbPoseGradArgs(q_pointcloud_camera=_ptr(q_pc), grad_q_pointcloud_camera=_ptr(grad_q),
-                                                     grad_t_pointcloud_camera=_ptr(grad_t), temp=_ptr(pose_temp))
-                if intrinsics:
-                    grad_K = torch.empty((3, 3), dtype=torch.float32, device=device)
-                    intr_temp = torch.empty((int(lib.gsb200_intrinsics_grad_temp_bytes()) // 4,), dtype=torch.float32,
-                                            device=device)
-                    intr_args = _lib.GsbIntrinsicsGradArgs(grad_camera_intrinsics=_ptr(grad_K), temp=_ptr(intr_temp))
-                ext = None
-                if extra_features is not None and grad_feature_map is not None:
-                    grad_map = _f32(grad_feature_map)
-                    ext = _lib.GsbExtraFeatureArgs(channels=extra_features.shape[1], features=_ptr(extra_features),
-                                                   grad_rasterized=_ptr(grad_map), grad_features=_ptr(grad_extra_features))
-                _lib.check(lib.gsb200_backward_ortho(
-                    ctypes.byref(args), _ptr(grad_depth), _ptr(depth), _ptr(grad_alpha),
-                    ctypes.byref(ext) if ext is not None else None,
-                    ctypes.byref(_lib.GsbFilter3dArgs(filter3d=_ptr(ctx.filter_3d))) if ctx.filter_3d is not None else None,
-                    ctypes.byref(pose_args) if pose_args is not None else None,
-                    ctypes.byref(intr_args) if intr_args is not None else None), "gsb200_backward_ortho")
-            elif ctx.defocus is not None:  # no other camera-parameter gradient (refused in forward)
-                ext = None
-                if extra_features is not None and grad_feature_map is not None:
-                    grad_map = _f32(grad_feature_map)
-                    ext = _lib.GsbExtraFeatureArgs(channels=extra_features.shape[1], features=_ptr(extra_features),
-                                                   grad_rasterized=_ptr(grad_map), grad_features=_ptr(grad_extra_features))
-                rs = ctx.rolling_shutter[0] if ctx.rolling_shutter is not None else None
-                defocus_grad_args = None
-                if defocus_grad:
-                    grad_defocus = torch.empty((2,), dtype=torch.float32, device=device)
-                    defocus_temp = torch.empty((int(lib.gsb200_defocus_grad_temp_bytes()) // 4,), dtype=torch.float32,
-                                               device=device)
-                    defocus_grad_args = _lib.GsbDefocusGradArgs(grad=_ptr(grad_defocus), temp=_ptr(defocus_temp))
-                _lib.check(lib.gsb200_backward_defocus(
-                    ctypes.byref(args), _ptr(grad_depth), _ptr(depth), _ptr(grad_alpha),
-                    ctypes.byref(ext) if ext is not None else None, ctypes.byref(ctx.lens) if ctx.lens is not None else None,
-                    ctypes.byref(rs) if rs is not None else None,
-                    ctypes.byref(ctx.motion_blur) if ctx.motion_blur is not None else None, ctypes.byref(ctx.defocus),
-                    ctypes.byref(defocus_grad_args) if defocus_grad_args is not None else None), "gsb200_backward_defocus")
-                if defocus_grad:
-                    grad_d = grad_defocus.to(ctx.defocus_device)
-            elif ctx.motion_blur is not None:  # no other camera-parameter gradient (refused in forward)
-                ext = None
-                if extra_features is not None and grad_feature_map is not None:
-                    grad_map = _f32(grad_feature_map)
-                    ext = _lib.GsbExtraFeatureArgs(channels=extra_features.shape[1], features=_ptr(extra_features),
-                                                   grad_rasterized=_ptr(grad_map), grad_features=_ptr(grad_extra_features))
-                rs = ctx.rolling_shutter[0] if ctx.rolling_shutter is not None else None
-                blur_grad_args = None
-                if blur_grad:
-                    grad_blur = torch.empty((6,), dtype=torch.float32, device=device)
-                    blur_temp = torch.empty((int(lib.gsb200_motion_blur_grad_temp_bytes()) // 4,), dtype=torch.float32,
-                                            device=device)
-                    blur_grad_args = _lib.GsbMotionBlurGradArgs(grad_motion=_ptr(grad_blur), temp=_ptr(blur_temp))
-                _lib.check(lib.gsb200_backward_motion_blur(
-                    ctypes.byref(args), _ptr(grad_depth), _ptr(depth), _ptr(grad_alpha),
-                    ctypes.byref(ext) if ext is not None else None, ctypes.byref(ctx.lens) if ctx.lens is not None else None,
-                    ctypes.byref(rs) if rs is not None else None, ctypes.byref(ctx.motion_blur),
-                    ctypes.byref(blur_grad_args) if blur_grad_args is not None else None), "gsb200_backward_motion_blur")
-                if blur_grad:
-                    grad_b = grad_blur.to(ctx.blur_device)
-            elif ctx.filter_3d is not None:  # no camera-parameter gradient (refused in forward)
-                ext = None
-                if extra_features is not None and grad_feature_map is not None:
-                    grad_map = _f32(grad_feature_map)
-                    ext = _lib.GsbExtraFeatureArgs(channels=extra_features.shape[1], features=_ptr(extra_features),
-                                                   grad_rasterized=_ptr(grad_map), grad_features=_ptr(grad_extra_features))
-                rs = ctx.rolling_shutter[0] if ctx.rolling_shutter is not None else None
-                _lib.check(lib.gsb200_backward_filter3d(
-                    ctypes.byref(args), _ptr(grad_depth), _ptr(depth), _ptr(grad_alpha),
-                    ctypes.byref(ext) if ext is not None else None, ctypes.byref(ctx.lens) if ctx.lens is not None else None,
-                    ctypes.byref(rs) if rs is not None else None,
-                    ctypes.byref(_lib.GsbFilter3dArgs(filter3d=_ptr(ctx.filter_3d)))), "gsb200_backward_filter3d")
-            elif ctx.rolling_shutter is not None:  # neither pose, intrinsics nor lens gradients (refused in forward)
-                rs, _row_time = ctx.rolling_shutter
-                ext = None
-                if extra_features is not None and grad_feature_map is not None:
-                    grad_map = _f32(grad_feature_map)
-                    ext = _lib.GsbExtraFeatureArgs(channels=extra_features.shape[1], features=_ptr(extra_features),
-                                                   grad_rasterized=_ptr(grad_map), grad_features=_ptr(grad_extra_features))
-                rs_grad = None
-                if motion_grad:
-                    grad_motion = torch.empty((6,), dtype=torch.float32, device=device)
-                    rs_temp = torch.empty((int(lib.gsb200_rolling_shutter_grad_temp_bytes()) // 4,), dtype=torch.float32,
-                                          device=device)
-                    rs_grad = _lib.GsbRollingShutterGradArgs(grad_motion=_ptr(grad_motion), temp=_ptr(rs_temp))
-                _lib.check(lib.gsb200_backward_rolling_shutter(
-                    ctypes.byref(args), _ptr(grad_depth), _ptr(depth), _ptr(grad_alpha),
-                    ctypes.byref(ext) if ext is not None else None, ctypes.byref(ctx.lens) if ctx.lens is not None else None,
-                    ctypes.byref(rs), ctypes.byref(rs_grad) if rs_grad is not None else None),
-                    "gsb200_backward_rolling_shutter")
-                if motion_grad:
-                    grad_m = grad_motion.to(ctx.motion_device)
-            elif ctx.lens is not None and (pose or intrinsics):  # one pass for pose, K and (lens_grad) the coefficients
-                ext = None
-                if extra_features is not None and grad_feature_map is not None:
-                    grad_map = _f32(grad_feature_map)
-                    ext = _lib.GsbExtraFeatureArgs(channels=extra_features.shape[1], features=_ptr(extra_features),
-                                                   grad_rasterized=_ptr(grad_map), grad_features=_ptr(grad_extra_features))
-                pose_args, intr_args = self._camera_grad_args(lib, ctx, q_pointcloud_camera, pose, intrinsics, device)
-                lens_grad_args = None
-                if lens_grad:
-                    grad_coefficients = torch.empty((5,), dtype=torch.float32, device=device)
-                    lens_temp = torch.empty((int(lib.gsb200_lens_grad_temp_bytes()) // 4,), dtype=torch.float32, device=device)
-                    lens_grad_args = _lib.GsbLensGradArgs(grad_coefficients=_ptr(grad_coefficients), temp=_ptr(lens_temp))
-                _lib.check(lib.gsb200_backward_lens_calib(
-                    ctypes.byref(args), _ptr(grad_depth), _ptr(depth), _ptr(grad_alpha),
-                    ctypes.byref(ext) if ext is not None else None, ctypes.byref(ctx.lens),
-                    ctypes.byref(lens_grad_args) if lens_grad_args is not None else None,
-                    ctypes.byref(pose_args[0]) if pose_args is not None else None,
-                    ctypes.byref(intr_args[0]) if intr_args is not None else None), "gsb200_backward_lens_calib")
-                if pose_args is not None:
-                    grad_q, grad_t = pose_args[1], pose_args[2]
-                if intr_args is not None:
-                    grad_K = intr_args[1]
-                if lens_grad:
-                    n, k_device = ctx.lens_coefficients_like
-                    grad_k = grad_coefficients[:n].to(k_device)
-            elif ctx.lens is not None:  # neither pose nor intrinsics gradients
-                ext = None
-                if extra_features is not None and grad_feature_map is not None:
-                    grad_map = _f32(grad_feature_map)
-                    ext = _lib.GsbExtraFeatureArgs(channels=extra_features.shape[1], features=_ptr(extra_features),
-                                                   grad_rasterized=_ptr(grad_map), grad_features=_ptr(grad_extra_features))
-                if lens_grad:
-                    grad_coefficients = torch.empty((5,), dtype=torch.float32, device=device)
-                    lens_temp = torch.empty((int(lib.gsb200_lens_grad_temp_bytes()) // 4,), dtype=torch.float32, device=device)
-                    lens_grad_args = _lib.GsbLensGradArgs(grad_coefficients=_ptr(grad_coefficients), temp=_ptr(lens_temp))
-                    _lib.check(lib.gsb200_backward_lens_grad(
-                        ctypes.byref(args), _ptr(grad_depth), _ptr(depth), _ptr(grad_alpha),
-                        ctypes.byref(ext) if ext is not None else None, ctypes.byref(ctx.lens), ctypes.byref(lens_grad_args)),
-                        "gsb200_backward_lens_grad")
-                    n, k_device = ctx.lens_coefficients_like
-                    grad_k = grad_coefficients[:n].to(k_device)
+                if grad_feature_map is None:
+                    grads[_EXTRA_FEATURES] = torch.zeros((N, C), dtype=torch.float32, device=device)
                 else:
-                    _lib.check(lib.gsb200_backward_lens(ctypes.byref(args), _ptr(grad_depth), _ptr(depth), _ptr(grad_alpha),
-                                                        ctypes.byref(ext) if ext is not None else None, ctypes.byref(ctx.lens)),
-                               "gsb200_backward_lens")
-            elif pose or intrinsics:
-                pose_args = intr_args = None
-                if pose:
-                    n_obj = ctx.num_objects
-                    q_pc = q_pointcloud_camera.detach().contiguous()
-                    grad_q = torch.empty((n_obj, 4), dtype=torch.float32, device=device)
-                    grad_t = torch.empty((n_obj, 3), dtype=torch.float32, device=device)
-                    pose_temp = torch.empty((max(int(lib.gsb200_pose_grad_temp_bytes(n_obj)), 16) // 4,),
-                                            dtype=torch.float32, device=device)
-                    pose_args = _lib.GsbPoseGradArgs(q_pointcloud_camera=_ptr(q_pc), grad_q_pointcloud_camera=_ptr(grad_q),
-                                                     grad_t_pointcloud_camera=_ptr(grad_t), temp=_ptr(pose_temp))
-                if intrinsics:
-                    grad_K = torch.empty((3, 3), dtype=torch.float32, device=device)
-                    intr_temp = torch.empty((int(lib.gsb200_intrinsics_grad_temp_bytes()) // 4,), dtype=torch.float32,
-                                            device=device)
-                    intr_args = _lib.GsbIntrinsicsGradArgs(grad_camera_intrinsics=_ptr(grad_K), temp=_ptr(intr_temp))
-                ext = None
-                if extra_features is not None and grad_feature_map is not None:
+                    grads[_EXTRA_FEATURES] = torch.empty((N, C), dtype=torch.float32, device=device)
                     grad_map = _f32(grad_feature_map)
-                    ext = _lib.GsbExtraFeatureArgs(channels=extra_features.shape[1], features=_ptr(extra_features),
-                                                   grad_rasterized=_ptr(grad_map), grad_features=_ptr(grad_extra_features))
-                if intrinsics:
-                    _lib.check(lib.gsb200_backward_calib(
-                        ctypes.byref(args), _ptr(grad_depth), _ptr(depth), _ptr(grad_alpha),
-                        ctypes.byref(ext) if ext is not None else None,
-                        ctypes.byref(pose_args) if pose_args is not None else None, ctypes.byref(intr_args)),
-                        "gsb200_backward_calib")
-                else:
-                    _lib.check(lib.gsb200_backward_pose(ctypes.byref(args), _ptr(grad_depth), _ptr(depth), _ptr(grad_alpha),
-                                                        ctypes.byref(ext) if ext is not None else None,
-                                                        ctypes.byref(pose_args)), "gsb200_backward_pose")
-            elif extra_features is not None and grad_feature_map is not None:
-                grad_map = _f32(grad_feature_map)
-                ext = _lib.GsbExtraFeatureArgs(channels=extra_features.shape[1], features=_ptr(extra_features),
-                                               grad_rasterized=_ptr(grad_map), grad_features=_ptr(grad_extra_features))
-                _lib.check(lib.gsb200_backward_ext(ctypes.byref(args), _ptr(grad_depth), _ptr(depth), _ptr(grad_alpha),
-                                                   ctypes.byref(ext)), "gsb200_backward_ext")
-            elif grad_alpha is not None:
-                _lib.check(lib.gsb200_backward_aux(ctypes.byref(args), _ptr(grad_depth), _ptr(depth), _ptr(grad_alpha)),
-                           "gsb200_backward_aux")
-            elif depth is not None:
-                _lib.check(lib.gsb200_backward_with_depth(ctypes.byref(args), _ptr(grad_depth), _ptr(depth)),
-                           "gsb200_backward_with_depth")
+                    ext = _lib.GsbExtraFeatureArgs(channels=C, features=_ptr(extra_features), grad_rasterized=_ptr(grad_map),
+                                                   grad_features=_ptr(grads[_EXTRA_FEATURES]))
+            temps = []  # the camera-gradient temps, alive until the call returns
+            pose_args = None
+            if pose:
+                n_obj = ctx.num_objects
+                q_pc = q_pointcloud_camera.detach().contiguous()
+                grads[_Q] = torch.empty((n_obj, 4), dtype=torch.float32, device=device)
+                grads[_T] = torch.empty((n_obj, 3), dtype=torch.float32, device=device)
+                temps.append(torch.empty((max(int(lib.gsb200_pose_grad_temp_bytes(n_obj)), 16) // 4,), dtype=torch.float32,
+                                         device=device))
+                pose_args = _lib.GsbPoseGradArgs(q_pointcloud_camera=_ptr(q_pc), grad_q_pointcloud_camera=_ptr(grads[_Q]),
+                                                 grad_t_pointcloud_camera=_ptr(grads[_T]), temp=_ptr(temps[-1]))
+            grad_args = dict.fromkeys(_CAMERA_GRADS)
+            for slot in camera_grads:
+                struct, shape, temp_bytes = _CAMERA_GRADS[slot]
+                grads[slot] = torch.empty(shape, dtype=torch.float32, device=device)
+                temps.append(torch.empty((int(getattr(lib, temp_bytes)()) // 4,), dtype=torch.float32, device=device))
+                grad_args[slot] = struct(_ptr(grads[slot]), _ptr(temps[-1]))
+            # backward_impl's precedence (csrc/api.cu): every refused combination was refused by _resolve_camera
+            if camera.projection is _EQUIRECT:
+                entry, camera_args = "gsb200_backward_equirect", ()
+            elif camera.projection is _ORTHO:
+                entry, camera_args = "gsb200_backward_ortho", (camera.filter_3d, pose_args, grad_args[_INTRINSICS])
+            elif camera.defocus is not None:
+                entry, camera_args = "gsb200_backward_defocus", (camera.lens, camera.rolling_shutter, camera.motion_blur,
+                                                                 camera.defocus, grad_args[_DEFOCUS_PARAMETERS])
+            elif camera.motion_blur is not None:
+                entry, camera_args = "gsb200_backward_motion_blur", (camera.lens, camera.rolling_shutter, camera.motion_blur,
+                                                                     grad_args[_EXPOSURE_MOTION])
+            elif camera.filter_3d is not None:
+                entry, camera_args = "gsb200_backward_filter3d", (camera.lens, camera.rolling_shutter, camera.filter_3d)
+            elif camera.rolling_shutter is not None:
+                entry, camera_args = "gsb200_backward_rolling_shutter", (camera.lens, camera.rolling_shutter,
+                                                                         grad_args[_ROLLING_SHUTTER_MOTION])
+            elif camera.lens is not None:
+                entry, camera_args = "gsb200_backward_lens_calib", (camera.lens, grad_args[_LENS_COEFFICIENTS], pose_args,
+                                                                    grad_args[_INTRINSICS])
             else:
-                _lib.check(lib.gsb200_backward(ctypes.byref(args)), "gsb200_backward")
+                entry, camera_args = "gsb200_backward_calib", (pose_args, grad_args[_INTRINSICS])
+            _lib.check(getattr(lib, entry)(ctypes.byref(args), _ptr(grad_depth), _ptr(depth), _ptr(grad_alpha), _ref(ext),
+                                           *map(_ref, camera_args)), entry)
+            for slot, (length, like_device) in camera.gradient_like.items():
+                if slot in grads:
+                    grads[slot] = grads[slot][:length].to(like_device)
             own_view_grad_xyz = None
             if compact:
                 exchange.rows_written(grad_sum, blocks)
@@ -1261,10 +1045,9 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
                     num_overlap_tiles=frame.num_overlap_tiles,
                     num_affected_pixels=acc[:, 10].round().to(torch.int32),
                     point_uv_in_camera=frame.point_uv.contiguous(),
-                    point_depth=frame.records[:, 7] if ctx.lens is _EQUIRECT else frame.point_in_camera[:, 2],
+                    point_depth=frame.records[:, 7] if camera.projection is _EQUIRECT else frame.point_in_camera[:, 2],
                 ))
-        return grad_pointcloud, grad_pointcloud_features, grad_extra_features, grad_q, grad_t, grad_K, grad_k, grad_m, grad_b, \
-            grad_d
+        return grads
 
     def backward_flags(self, frame_flags: int) -> int:
         """Flags of the backward call for a frame rendered with ``frame_flags`` (adds the experimental kernel selection)."""
@@ -1350,112 +1133,12 @@ class GaussianPointCloudRasterisation(torch.nn.Module):
         ``differentiable_defocus``, a ``gradient_exchange``, a rolling shutter, motion blur or defocus on the camera, or their
         tensors."""
         camera_info = input_data.camera_info
-        if _is_equirect(camera_info):  # the argument checks, before any device work
-            self._check_equirect(camera_info, lens_coefficients, rolling_shutter_motion, point_filter_3d, exposure_motion,
-                                 defocus_parameters)
-        if _is_ortho(camera_info):
-            self._check_ortho(camera_info, lens_coefficients, rolling_shutter_motion, exposure_motion, defocus_parameters)
-        assert camera_info.camera_width % TILE_WIDTH == 0
-        assert camera_info.camera_height % TILE_HEIGHT == 0
-        if getattr(camera_info, "defocus", None) is not None or defocus_parameters is not None:
-            # the argument checks, before any device work; K, the coefficients, both motions and the filter are refused,
-            # so their slots are None
-            self._defocus_args(camera_info, defocus_parameters, rolling_shutter_motion, point_filter_3d, exposure_motion)
-            self._motion_blur_args(camera_info)
-            self._lens_args(camera_info, lens_coefficients)
-            self._rolling_shutter_args(camera_info)
-            if lens_coefficients is not None:
-                raise ValueError("a defocused camera is not supported with lens_coefficients")
-            if point_extra_features is not None:
-                self._check_extra_features(point_extra_features, input_data.point_cloud)
-            tail = (None,) * 5 + (defocus_parameters,) if defocus_parameters is not None else ()
-            if point_extra_features is not None or tail:
-                return self._module_function.apply(
-                    input_data.point_cloud, input_data.point_cloud_features, input_data.point_invalid_mask,
-                    input_data.point_object_id, input_data.q_pointcloud_camera, input_data.t_pointcloud_camera, camera_info,
-                    input_data.color_max_sh_band, point_extra_features, *tail)
-            return self._module_function.apply(
-                input_data.point_cloud, input_data.point_cloud_features, input_data.point_invalid_mask,
-                input_data.point_object_id, input_data.q_pointcloud_camera, input_data.t_pointcloud_camera, camera_info,
-                input_data.color_max_sh_band)
-        if getattr(camera_info, "motion_blur", None) is not None or exposure_motion is not None:
-            # the argument checks, before any device work; K, the coefficients, the row-time motion and the filter are
-            # refused, so their slots are None
-            self._motion_blur_args(camera_info, exposure_motion, rolling_shutter_motion, point_filter_3d)
-            self._lens_args(camera_info, lens_coefficients)
-            self._rolling_shutter_args(camera_info)
-            if lens_coefficients is not None:
-                raise ValueError("a motion-blurred camera is not supported with lens_coefficients")
-            if point_extra_features is not None:
-                self._check_extra_features(point_extra_features, input_data.point_cloud)
-            if exposure_motion is not None:
-                return self._module_function.apply(
-                    input_data.point_cloud, input_data.point_cloud_features, input_data.point_invalid_mask,
-                    input_data.point_object_id, input_data.q_pointcloud_camera, input_data.t_pointcloud_camera, camera_info,
-                    input_data.color_max_sh_band, point_extra_features, None, None, None, None, exposure_motion)
-            if point_extra_features is not None:
-                return self._module_function.apply(
-                    input_data.point_cloud, input_data.point_cloud_features, input_data.point_invalid_mask,
-                    input_data.point_object_id, input_data.q_pointcloud_camera, input_data.t_pointcloud_camera, camera_info,
-                    input_data.color_max_sh_band, point_extra_features)
-            return self._module_function.apply(
-                input_data.point_cloud, input_data.point_cloud_features, input_data.point_invalid_mask,
-                input_data.point_object_id, input_data.q_pointcloud_camera, input_data.t_pointcloud_camera, camera_info,
-                input_data.color_max_sh_band)
-        if point_filter_3d is not None:  # lens coefficients, K and the motion are refused with it: their slots are None
-            for name, value in (("lens_coefficients", lens_coefficients), ("rolling_shutter_motion", rolling_shutter_motion)):
-                if value is not None:
-                    raise ValueError(f"point_filter_3d is not supported with {name} (no camera-parameter gradient with the "
-                                     "filter)")
-            self._check_filter_3d(point_filter_3d, input_data.point_cloud)
-            if point_extra_features is not None:
-                self._check_extra_features(point_extra_features, input_data.point_cloud)
-            self._lens_args(camera_info)  # the lens and rolling-shutter checks, before any device work
-            self._rolling_shutter_args(camera_info)
-            return self._module_function.apply(
-                input_data.point_cloud, input_data.point_cloud_features, input_data.point_invalid_mask,
-                input_data.point_object_id, input_data.q_pointcloud_camera, input_data.t_pointcloud_camera, camera_info,
-                input_data.color_max_sh_band, point_extra_features, None, None, None, point_filter_3d)
-        if rolling_shutter_motion is not None:  # the extra features', K's and the coefficients' slots first (all refused)
-            self._rolling_shutter_args(camera_info, rolling_shutter_motion)  # the argument checks, before any device work
-            if point_extra_features is not None:
-                self._check_extra_features(point_extra_features, input_data.point_cloud)
-            return self._module_function.apply(
-                input_data.point_cloud, input_data.point_cloud_features, input_data.point_invalid_mask,
-                input_data.point_object_id, input_data.q_pointcloud_camera, input_data.t_pointcloud_camera, camera_info,
-                input_data.color_max_sh_band, point_extra_features, None, None, rolling_shutter_motion)
-        if lens_coefficients is not None:  # the extra features' and K's slots first (K: with differentiable_intrinsics)
-            self._lens_args(camera_info, lens_coefficients)  # the argument checks, before any device work
-            if point_extra_features is not None:
-                self._check_extra_features(point_extra_features, input_data.point_cloud)
-            return self._module_function.apply(
-                input_data.point_cloud, input_data.point_cloud_features, input_data.point_invalid_mask,
-                input_data.point_object_id, input_data.q_pointcloud_camera, input_data.t_pointcloud_camera, camera_info,
-                input_data.color_max_sh_band, point_extra_features,
-                camera_info.camera_intrinsics if self.differentiable_intrinsics else None, lens_coefficients)
-        if self.differentiable_intrinsics:  # K as a tenth input, after the extra features' slot
-            if point_extra_features is not None:
-                self._check_extra_features(point_extra_features, input_data.point_cloud)
-            return self._module_function.apply(
-                input_data.point_cloud, input_data.point_cloud_features, input_data.point_invalid_mask,
-                input_data.point_object_id, input_data.q_pointcloud_camera, input_data.t_pointcloud_camera, camera_info,
-                input_data.color_max_sh_band, point_extra_features, camera_info.camera_intrinsics)
-        if point_extra_features is not None:
-            self._check_extra_features(point_extra_features, input_data.point_cloud)
-            return self._module_function.apply(
-                input_data.point_cloud, input_data.point_cloud_features, input_data.point_invalid_mask,
-                input_data.point_object_id, input_data.q_pointcloud_camera, input_data.t_pointcloud_camera, camera_info,
-                input_data.color_max_sh_band, point_extra_features)
         return self._module_function.apply(
-            input_data.point_cloud,
-            input_data.point_cloud_features,
-            input_data.point_invalid_mask,
-            input_data.point_object_id,
-            input_data.q_pointcloud_camera,
-            input_data.t_pointcloud_camera,
-            camera_info,
-            input_data.color_max_sh_band,
-        )
+            input_data.point_cloud, input_data.point_cloud_features, input_data.point_invalid_mask,
+            input_data.point_object_id, input_data.q_pointcloud_camera, input_data.t_pointcloud_camera, camera_info,
+            input_data.color_max_sh_band, point_extra_features,
+            camera_info.camera_intrinsics if self.differentiable_intrinsics else None, lens_coefficients,
+            rolling_shutter_motion, point_filter_3d, exposure_motion, defocus_parameters)
 
 
 @dataclass
